@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""bench.py — NeRF-SH SH16 training throughput (BASELINE.json metric) on N B200s of one node.
+"""bench.py — NeRF-SH SH16 training throughput (BASELINE.json metric) on N H100s of one node.
 
     python bench.py --gpus 1 --steps 20 --warmup 5
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port P bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference --gpus 1 --steps 3 --warmup 1     # CPU oracle arm
+    python bench.py --gpus 1 --steps 20 --warmup 5 --dump-outputs DIR  # + the last timed step's results as .npy
 
 Workload (config.workload): BASELINE.json configs[1] — nerf_sh/config/blender (SH16, 64 coarse + 128
 fine samples = 256 MLP evaluations per ray, white background, sparsity loss on 10,000 points), synthetic
@@ -18,7 +19,8 @@ sparsity points per step (the reference draws those per device, nerf_sh/train.py
            memory and the step's loss statistics read back to the host inside the timed region.
 `roofline`: dominant kernel class (and, under `kernels`, all three), algorithmic GEMM FLOPs (SURVEY.md §8d:
            1,007,104 fwd / 942,592 dgrad / 1,007,104 wgrad FLOP per MLP-sample, SH16) / CUDA-event kernel time,
-           vs the measured sustained bf16 tensor peak in MEASURED_PEAKS.json; `step_frac` = the whole step.
+           vs the sustained bf16 tensor peak in MEASURED_PEAKS.json when present, else the H100 SXM data-sheet
+           dense fp16 figure (989 TFLOP/s, not measured); `step_frac` = the whole step.
 `strong`, `tt_sh25`, `c4_extraction`, `c5_octree_opt`, `render_eval`: the other BASELINE configurations, timed after the main
            region on the same ranks (bench_extras.py); skipped with --no-extras.
 """
@@ -53,7 +55,7 @@ def measured_peaks():
     if os.path.exists(path):
         p = json.load(open(path))
         return dict(tflops=float(p.get("bf16_tflops_sustained", p.get("bf16_tflops"))), src="measured (sustained bf16)")
-    return dict(tflops=1400.0, src="fallback (B200_PROFILING.md sustained)")
+    return dict(tflops=989.0, src="H100 SXM data sheet, dense fp16 (not measured)")
 
 
 class ClockSampler(threading.Thread):
@@ -193,14 +195,18 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=30)
     ap.add_argument("--warmup", type=int, default=5)
-    ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--impl", default="cuda", choices=["cuda", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the strong-scaling / SH25 / extraction / octree extras")
     ap.add_argument("--workload", default="blender", choices=["blender", "tt"],
                     help="blender = BASELINE configs[1] (SH16, near/far 2/6; the default and the quoted metric); "
                          "tt = configs[2] (SH25, near/far 0/4, sparsity radius 5 / length 0.2)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (updated parameters, "
+                         "gradient, loss sums) as DIR/<name>.npy; the inputs are seeded, so runs with the same "
+                         "arguments can be compared output for output")
     args = ap.parse_args()
-    args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
+    args.warmup = max(args.warmup, 3) if args.impl == "cuda" else args.warmup
 
     if args.impl == "reference":
         run_reference(args)
@@ -234,7 +240,7 @@ def main():
     state = T.TrainState(model)
 
     # ---- synthetic ray pool: (2K + 2W) batches, different data per rank, host pinned + device copy
-    nb = max(2 * (K + W), 800)        # >= 800 batches x 4096 rays x 48 B = 157 MB > the 126 MB L2
+    nb = max(2 * (K + W), 800)        # >= 800 batches x 4096 rays x 48 B = 157 MB > the 50 MB L2
     o, d, vd, px = random_rays_np(nb * RAYS, 20200823 + 7919 * rank)
     host = torch.from_numpy(np.concatenate([o, d, vd, px], axis=1)).contiguous().pin_memory()   # [nb*RAYS, 12]
     pool = host.to(dev)                                                                          # HBM resident
@@ -313,9 +319,15 @@ def main():
     launches0 = _lib.lib.pob_launch_count()
     ms_total = timed(step_resident, W)
     launches = int(_lib.lib.pob_launch_count() - launches0)
-    # ---- per-step distribution over a longer run (the contract region above is K steps long; the driver's K = 20
-    # is 80 ms): every step bracketed by its own pair of events, no host sync inside the loop
-    ND = 100
+    if args.dump_outputs and rank == 0:
+        # what the last timed step left for its caller: Adam-updated parameters of both MLPs (reference flat order),
+        # the gradient it applied, and the loss sums of stats_raw (pob_loss_and_grad); float32, ~10 MB in all
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in (("params", model.params), ("grads", state.grads), ("loss_stats", state.stats_raw)):
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), t.detach().float().cpu().numpy())
+    # ---- per-step distribution: every one of K more steps bracketed by its own pair of events, no host sync
+    # inside the loop
+    ND = K
     evs = [torch.cuda.Event(enable_timing=True) for _ in range(ND + 1)]
     barrier()
     evs[0].record()
@@ -355,19 +367,9 @@ def main():
     dom = max(alg, key=lambda k: per_step_ms[k])
     peaks = measured_peaks()
     achieved = alg[dom] / (per_step_ms[dom] * 1e-3) / 1e12
-    # dram__bytes_read.sum + dram__bytes_write.sum per kernel class and step, from the committed `ncu --set full`
-    # capture of this round (profiles/r2_dram_traffic.json; scaled there to the 4096-ray step)
-    traffic_all = {}
-    for name in ("r2_dram_traffic.json", "r1_dram_traffic.json"):
-        tpath = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(tpath):
-            traffic_all = json.load(open(tpath))
-            break
-    traffic = traffic_all.get(dom)
     kernels = {k: {"ms_per_step": per_step_ms[k], "algorithmic_flops_per_step": alg[k],
                    "achieved": alg[k] / (per_step_ms[k] * 1e-3) / 1e12,
-                   "frac": alg[k] / (per_step_ms[k] * 1e-3) / 1e12 / peaks["tflops"],
-                   "traffic": traffic_all.get(k)} for k in alg}
+                   "frac": alg[k] / (per_step_ms[k] * 1e-3) / 1e12 / peaks["tflops"]} for k in alg}
 
     # ---- the other BASELINE configurations (bounded; never allowed to break the contract line) ----
     extras = {}
@@ -391,7 +393,7 @@ def main():
         line = {
             "metric": METRIC, "value": value, "unit": "rays/s", "n_gpus": world, "steps": K, "warmup": W,
             "ms_per_step": ms_total / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "dtype": "f16 operands / f32 accumulate (tcgen05 kind::f16), f32 params+Adam",
+            "dtype": "f16 operands / f32 accumulate (wgmma), f32 params+Adam",
             "data": "synthetic",
             "config": {"workload": ("configs[2]: NeRF-SH SH25 training, nerf_sh/config/tt hyper-parameters, synthetic random "
                                     "poses, batch 4096 rays per GPU") if tt else
@@ -400,8 +402,7 @@ def main():
                        "rays_per_gpu_per_step": RAYS, "global_batch": RAYS * world,
                        "samples_per_ray": "64 coarse (MLP_0) + 192 fine (MLP_1) = 256 MLP evaluations",
                        "sparsity_points_per_gpu": NSP, "parallelism": f"dp{world}",
-                       "l2_policy": f"inputs larger than L2: {pool_mb:.0f} MB ray pool, a fresh batch every step; "
-                                    "per-step activation traffic ~17 GB"},
+                       "l2_policy": f"inputs larger than L2: {pool_mb:.0f} MB ray pool, a fresh batch every step"},
             "e2e": {"value": e2e, "unit": "rays/s", "ms_per_step": ms_e2e / K,
                     "h2d_bytes_per_step": RAYS * 12 * 4, "d2h_bytes_per_step": 8 * 4},
             "gpu_launches": launches,
@@ -409,7 +410,7 @@ def main():
             "step_ms_distribution": step_dist,
             "step_tflops_algorithmic": FLOP_PER_STEP * f_scale / (ms_total / K * 1e-3) / 1e12,
             "roofline": {"bound": "tensor", "kernel": dom, "achieved": achieved, "peak": peaks["tflops"],
-                         "unit": "TFLOP/s", "frac": achieved / peaks["tflops"], "traffic": traffic,
+                         "unit": "TFLOP/s", "frac": achieved / peaks["tflops"],
                          "peak_source": peaks["src"],
                          "algorithmic_flops_per_step": alg[dom], "share_of_step": per_step_ms[dom] / sum(per_step_ms.values()),
                          "step_frac": FLOP_PER_STEP * f_scale / (ms_total / K * 1e-3) / 1e12 / peaks["tflops"],

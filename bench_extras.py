@@ -196,7 +196,7 @@ def c4_extraction(dev, peak_tflops, depth=8, samples_per_cell=256, keep_fraction
         # Tree build and step 2 are host-driven (torch bookkeeping, caching-allocator traffic): with 8 processes that
         # hold a peer-mapped NCCL communicator they took 58 s + 71 s on the 8-GPU box (4 GPUs: 10 s + 0.73 s; 1 GPU:
         # 0.09 s + 2.6 s) — a host / driver effect, not a kernel one (DESIGN.md section 7).  The bench line stays bounded.
-        res["tree_build_and_step2"] = "skipped at more than 4 ranks (measured once: profiles/r2_bench_n8.json)"
+        res["tree_build_and_step2"] = "skipped at more than 4 ranks"
         res["total_ms"] = res["sigma_sweep_ms"] + res["slab_allgather_ms"] + res["grid_weights_100_cameras_ms"]
         return res
     # a random-init field has no surfaces: keep the `keep_fraction` heaviest voxels (a synthetic scene keeps ~2.7 %)

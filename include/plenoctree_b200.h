@@ -1,4 +1,4 @@
-/* plenoctree_b200.h — C ABI of the B200-native NeRF-SH hot path.
+/* plenoctree_b200.h — C ABI of the H100-native (sm_90a) NeRF-SH hot path.
  *
  * The reference (sxyu/plenoctree) has no FFI layer of its own: its boundary for this path is a
  * set of Python call signatures (SURVEY.md §8b).  Each entry point below is what a binding for
@@ -11,7 +11,7 @@
  *   - all functions return 0 on success, non-zero on error; pob_last_error() returns a
  *     thread-local message for the last failure (never NULL);
  *   - nothing here falls back to the CPU: without a CUDA device every compute call fails.
- *   - precision: POB_PREC_FP16 = fp16 operands / fp32 accumulate on tcgen05 (the numerics class
+ *   - precision: POB_PREC_FP16 = fp16 operands / fp32 accumulate on wgmma (the numerics class
  *     of the reference's TF32-default XLA GPU path); POB_PREC_FP16X3 = error-compensated 3-pass
  *     split (fp32-class accuracy, 1/3 of the tensor throughput).
  */
@@ -190,22 +190,6 @@ int pob_adam_update(int sh_deg, int num_mlps, float* params_dev, const float* gr
                     float* v_dev, float lr, float step, const float* lr_step_dev, float grad_mult,
                     float weight_decay_coef, void* packed_coarse_dev, void* packed_fine_dev, void* stream);
 
-/* Profiling aid: pob_eval_points_raw (sigma only, FP16) that also records clock64() stamps of CTA 0 into
- * trace_dev[3][256] (role 0 = MMA issuer, 1/2 = first epilogue warp of tile X/Y); scripts/trace_summary.py.
- * save_*_dev (all or none; sized like the training workspace: 512 KB, 16 KB and 4 KB per 128 samples) turn
- * on the training-mode stores so their cost shows in the trace. */
-int pob_debug_trace_fwd(const void* packed_dev, int sh_deg, const float* points_dev, int64_t m,
-                        float* raw_sigma_dev, unsigned long long* trace_dev, int debug_flags, void* save_h_dev,
-                        void* save_e_dev, void* save_mask_dev, void* stream);
-
-/* Profiling aid: one mlp_bwd launch (dgrad chain, FP16) on caller-provided inputs — per-sample gradients g_dev
- * [m,4], view directions [m,3], relu masks (4 KB per 128 samples and layer), dZ / dO destinations sized like the
- * training workspace — recording clock64() stamps of CTA 0 into trace_dev[2][256] (role 0 = MMA issuer, 1 = first
- * epilogue warp of tile X); scripts/trace_summary.py.  debug_flags: timing experiments (results invalid). */
-int pob_debug_trace_bwd(const void* packed_dev, int sh_deg, int64_t m, const float* g_dev, const float* viewdirs_dev,
-                        const void* mask_dev, void* save_dz_dev, void* save_do_dev, unsigned long long* trace_dev,
-                        int debug_flags, void* stream);
-
 /* ---------------------------------------------------------------------------------------------
  * PlenOctree side (SURVEY.md §8 rows a13-middle and a15).  These entry points stand where the
  * reference calls the third-party `svox` extension (absent from the reference tree; the oracle
@@ -296,24 +280,6 @@ int pob_octree_query(const pob_octree* tree, const float* points_dev, int64_t n,
 int pob_grid_weight_render(const float* sigma_grid_dev, int reso, const pob_camera* cams_dev, int n_cams,
                            int max_width, int max_height, const float offset[3], const float invradius[3],
                            const pob_octree_opts* opts, float* max_weight_dev, uint8_t* hit_dev, void* stream);
-
-/* ---------------------------------------------------------------------------------------------
- * Test bench for the tcgen05 descriptor conventions (tests/test_umma_probe.py).
- * Runs `nops` tcgen05.mma (kind::f16, M=128) on two shared-memory images and returns the
- * [128 x out_cols] fp32 accumulator.
- * ------------------------------------------------------------------------------------------- */
-int pob_umma_probe(const void* a_img_dev, uint32_t a_bytes, const void* b_img_dev,
-                   uint32_t b_bytes, uint32_t b_off, const uint64_t* adesc_dev,
-                   const uint64_t* bdesc_dev, const uint32_t* dcol_dev, const uint32_t* accum_dev,
-                   int nops, uint32_t idesc, int out_cols, float* out_dev, void* stream);
-
-/* CTA-pair variant (tcgen05 cta_group::2, cluster of two CTAs, M = 256 in idesc): CTA r stages
- * a_img + r*a_bytes and b_img + r*b_bytes (its 128 A rows and its half of the B rows) at the same
- * shared-memory offsets; returns the [256 x out_cols] accumulator (rows 128r.. from CTA r). */
-int pob_umma_probe_pair(const void* a_img_dev, uint32_t a_bytes, const void* b_img_dev,
-                        uint32_t b_bytes, uint32_t b_off, const uint64_t* adesc_dev,
-                        const uint64_t* bdesc_dev, const uint32_t* dcol_dev, const uint32_t* accum_dev,
-                        int nops, uint32_t idesc, int out_cols, float* out_dev, void* stream);
 
 #ifdef __cplusplus
 }

@@ -1,7 +1,7 @@
 """ctypes binding of libplenoctree_b200.so (the C ABI in include/plenoctree_b200.h).
 
 There is no fallback: if the shared library is missing the import raises, and every compute entry
-point fails when no sm_100 device is present.
+point fails when no sm_90 device is present.
 """
 import ctypes
 import os
@@ -13,7 +13,7 @@ PREC_FP16 = 1
 PREC_FP16X3 = 3
 
 _c = ctypes
-_vp, _i, _i64, _u32, _fp = _c.c_void_p, _c.c_int, _c.c_int64, _c.c_uint32, _c.c_void_p
+_vp, _i, _i64, _fp = _c.c_void_p, _c.c_int, _c.c_int64, _c.c_void_p
 
 # name -> (restype, argtypes); must list every symbol the header declares
 SIGNATURES = {
@@ -27,8 +27,6 @@ SIGNATURES = {
     "pob_packed_bytes": (_i64, [_i]),
     "pob_pack_weights": (_i, [_fp, _i, _vp, _vp]),
     "pob_eval_points_raw": (_i, [_vp, _i, _fp, _i64, _fp, _fp, _i, _vp]),
-    "pob_debug_trace_fwd": (_i, [_vp, _i, _fp, _i64, _fp, _vp, _i, _vp, _vp, _vp, _vp]),
-    "pob_debug_trace_bwd": (_i, [_vp, _i, _i64, _fp, _fp, _vp, _vp, _vp, _vp, _i, _vp]),
     "pob_eval_points": (_i, [_vp, _i, _fp, _fp, _i64, _fp, _i, _vp]),
     "pob_eval_cells_mean": (_i, [_vp, _i, _fp, _i64, _i, _fp, _i, _vp]),
     "pob_eval_grid": (_i, [_vp, _i, _i, _i, _i, _i, _i, _c.POINTER(_c.c_float), _c.POINTER(_c.c_float),
@@ -53,8 +51,6 @@ SIGNATURES = {
     "pob_octree_query": (_i, [_vp, _fp, _i64, _vp, _vp]),
     "pob_grid_weight_render": (_i, [_fp, _i, _vp, _i, _i, _i, _c.POINTER(_c.c_float), _c.POINTER(_c.c_float),
                                     _vp, _fp, _vp, _vp]),
-    "pob_umma_probe": (_i, [_vp, _u32, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _i, _u32, _i, _fp, _vp]),
-    "pob_umma_probe_pair": (_i, [_vp, _u32, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _i, _u32, _i, _fp, _vp]),
 }
 
 

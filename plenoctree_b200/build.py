@@ -1,4 +1,4 @@
-"""In-tree build of libplenoctree_b200.so (explicit nvcc, sm_100a only).
+"""In-tree build of libplenoctree_b200.so (explicit nvcc, sm_90a only).
 
 `python -m plenoctree_b200.build` compiles every .cu under csrc/ that is newer than its object
 and links the shared library next to this file.  nvcc cross-compiles without a GPU.
@@ -15,7 +15,7 @@ LIB = os.path.join(HERE, "libplenoctree_b200.so")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",

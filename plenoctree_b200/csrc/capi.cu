@@ -71,9 +71,10 @@ int sm_count() {
   int dev = 0, n = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return -1;
   if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return -1;
-  int major = 0;
+  int major = 0, minor = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-  if (major != 10) return -2;  // sm_100a only
+  cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
+  if (major != 9 || minor != 0) return -2;  // sm_90a only (wgmma)
   g_sm_count = n;
   return n;
 }
@@ -110,7 +111,7 @@ int check_common(const char* where, const void* packed, int sh_deg, int precisio
   if (precision != POB_PREC_FP16 && precision != POB_PREC_FP16X3)
     return fail(where, "precision must be POB_PREC_FP16 or POB_PREC_FP16X3");
   int n = sm_count();
-  if (n == -2) return fail(where, "device is not compute capability 10.x (sm_100a build)");
+  if (n == -2) return fail(where, "device is not compute capability 9.0 (sm_90a build)");
   if (n <= 0) return fail(where, "no CUDA device");
   return 0;
 }
@@ -135,7 +136,7 @@ pob::FwdParams pob_base_params(const void* packed, int sh_deg) { return base_par
 
 extern "C" {
 
-int pob_abi_version(void) { return 4; }   // 4: pob_loss_and_grad(mlp0_done_event), pob_adam_update(lr_step_dev); 3: CTA-pair kernels
+int pob_abi_version(void) { return 5; }   // 5: sm_90a, no debug-trace / descriptor-probe entry points; 4: pob_loss_and_grad(mlp0_done_event), pob_adam_update(lr_step_dev)
 
 long long pob_launch_count(void) { return g_launches.load(); }
 
@@ -200,53 +201,6 @@ int pob_eval_points_raw(const void* packed_dev, int sh_deg, const float* points_
   POB_CUDA("pob_eval_points_raw",
            pob::launch_mlp_fwd(p, precision, precision == POB_PREC_FP16X3, sm_count(),
                                (cudaStream_t)stream));
-  return 0;
-}
-
-int pob_debug_trace_fwd(const void* packed_dev, int sh_deg, const float* points_dev, int64_t m,
-                        float* raw_sigma_dev, unsigned long long* trace_dev, int debug_flags, void* save_h_dev,
-                        void* save_e_dev, void* save_mask_dev, void* stream) {
-  if (int e = check_common("pob_debug_trace_fwd", packed_dev, sh_deg, POB_PREC_FP16)) return e;
-  if (!points_dev || !raw_sigma_dev || !trace_dev || m <= 0) return fail("pob_debug_trace_fwd", "bad arguments");
-  pob::FwdParams p = base_params(packed_dev, sh_deg);
-  p.src_mode = pob::SRC_POINTS;
-  p.M = m;
-  p.points = points_dev;
-  p.out_mode = pob::OUT_SIGMA;
-  p.out_sigma = raw_sigma_dev;
-  p.trace = trace_dev;
-  p.debug_flags = debug_flags;
-  p.save_h = static_cast<uint8_t*>(save_h_dev);
-  p.save_e = static_cast<uint8_t*>(save_e_dev);
-  p.save_mask = static_cast<uint32_t*>(save_mask_dev);
-  POB_CUDA("pob_debug_trace_fwd", pob::launch_mlp_fwd(p, 1, false, sm_count(), (cudaStream_t)stream));
-  return 0;
-}
-
-int pob_debug_trace_bwd(const void* packed_dev, int sh_deg, int64_t m, const float* g_dev, const float* viewdirs_dev,
-                        const void* mask_dev, void* save_dz_dev, void* save_do_dev, unsigned long long* trace_dev,
-                        int debug_flags, void* stream) {
-  if (int e = check_common("pob_debug_trace_bwd", packed_dev, sh_deg, POB_PREC_FP16)) return e;
-  if (!g_dev || !viewdirs_dev || !mask_dev || !save_dz_dev || !save_do_dev || m <= 0)
-    return fail("pob_debug_trace_bwd", "bad arguments");
-  pob::FwdParams base = base_params(packed_dev, sh_deg);
-  pob::BwdParams b;
-  memset(&b, 0, sizeof(b));
-  b.M = m;
-  b.G = reinterpret_cast<const float4*>(g_dev);
-  b.viewdirs = viewdirs_dev;
-  b.n_per_ray = 0;
-  b.M_rays = m;
-  b.w = base.w;
-  b.sh_deg = sh_deg;
-  b.K = base.K;
-  b.NH = base.NH;
-  b.mask = static_cast<const uint32_t*>(mask_dev);
-  b.save_dz = static_cast<uint8_t*>(save_dz_dev);
-  b.save_do = static_cast<uint8_t*>(save_do_dev);
-  b.trace = trace_dev;
-  b.debug_flags = debug_flags;
-  POB_CUDA("pob_debug_trace_bwd", pob::launch_mlp_bwd(b, sm_count(), (cudaStream_t)stream));
   return 0;
 }
 
@@ -381,7 +335,7 @@ int pob_draw_uniforms(uint64_t seed, float step, const float* step_dev, float* t
   if (n_t < 0 || n_u < 0 || n_sp < 0) return fail("pob_draw_uniforms", "negative size");
   if ((n_t && !t_rand_dev) || (n_u && !u_dev) || (n_sp && !sp_points_dev))
     return fail("pob_draw_uniforms", "NULL pointer");
-  if (sm_count() <= 0) return fail("pob_draw_uniforms", "no sm_100 CUDA device (there is no CPU fallback)");
+  if (sm_count() <= 0) return fail("pob_draw_uniforms", "no sm_90 CUDA device (there is no CPU fallback)");
   pob_count_launch();
   POB_CUDA("pob_draw_uniforms", pob::launch_draw_uniforms(seed, step, step_dev, t_rand_dev, n_t, u_dev, n_u,
                                                           sp_points_dev, n_sp, sp_radius, (cudaStream_t)stream));
@@ -426,36 +380,5 @@ int pob_sample_pdf(const float* z_coarse_dev, const float* weights_dev, const fl
   return 0;
 }
 
-int pob_umma_probe(const void* a_img_dev, uint32_t a_bytes, const void* b_img_dev,
-                   uint32_t b_bytes, uint32_t b_off, const uint64_t* adesc_dev,
-                   const uint64_t* bdesc_dev, const uint32_t* dcol_dev, const uint32_t* accum_dev,
-                   int nops, uint32_t idesc, int out_cols, float* out_dev, void* stream) {
-  if (sm_count() <= 0) return fail("pob_umma_probe", "no sm_100 CUDA device");
-  if (a_bytes % 16 || b_bytes % 16 || b_off % 1024 || b_off < a_bytes ||
-      (size_t)b_off + b_bytes > 200 * 1024)
-    return fail("pob_umma_probe", "bad image sizes/offsets");
-  if (out_cols <= 0 || out_cols > 512) return fail("pob_umma_probe", "out_cols out of range");
-  POB_CUDA("pob_umma_probe",
-           pob::launch_umma_probe(a_img_dev, a_bytes, b_img_dev, b_bytes, b_off, adesc_dev,
-                                  bdesc_dev, dcol_dev, accum_dev, nops, idesc, out_cols, out_dev,
-                                  (cudaStream_t)stream));
-  return 0;
-}
-
-int pob_umma_probe_pair(const void* a_img_dev, uint32_t a_bytes, const void* b_img_dev,
-                        uint32_t b_bytes, uint32_t b_off, const uint64_t* adesc_dev,
-                        const uint64_t* bdesc_dev, const uint32_t* dcol_dev, const uint32_t* accum_dev,
-                        int nops, uint32_t idesc, int out_cols, float* out_dev, void* stream) {
-  if (sm_count() <= 0) return fail("pob_umma_probe_pair", "no sm_100 CUDA device");
-  if (a_bytes % 16 || b_bytes % 16 || b_off % 1024 || b_off < a_bytes ||
-      (size_t)b_off + b_bytes > 200 * 1024)
-    return fail("pob_umma_probe_pair", "bad image sizes/offsets");
-  if (out_cols <= 0 || out_cols > 512) return fail("pob_umma_probe_pair", "out_cols out of range");
-  POB_CUDA("pob_umma_probe_pair",
-           pob::launch_umma_probe_pair(a_img_dev, a_bytes, b_img_dev, b_bytes, b_off, adesc_dev,
-                                       bdesc_dev, dcol_dev, accum_dev, nops, idesc, out_cols, out_dev,
-                                       (cudaStream_t)stream));
-  return 0;
-}
 
 }  // extern "C"

@@ -51,10 +51,6 @@ struct FwdParams {
   uint8_t* save_h;             // [ntile][8][64 KB] activation tile images h_0..h_7
   uint8_t* save_e;             // [ntile][16 KB]   posenc tile images
   uint32_t* save_mask;         // [8][ntile*128][8] relu masks (bit i of word c = col 32c+i)
-  // ---- optional cycle trace of CTA 0 (debug/profiling; null = off): [3 roles][256] clock64 stamps
-  unsigned long long* trace;
-  int debug_flags;             // timing experiments only (results invalid; pob_debug_trace_fwd): 8 no weight loads,
-                               // 16 h stores to one L2-resident tile per CTA, 32 drop in-epilogue stores, 64 drop deferred stores
 };
 
 // padded heads width for K spherical-harmonic coefficients per channel
@@ -68,24 +64,12 @@ inline size_t bwd_image_bytes(int NH) { return size_t((NH + 31) / 32 + 7 * 8) * 
 //            3 = error-compensated 3-pass split (hi*hi + lo*hi + hi*lo)
 cudaError_t launch_mlp_fwd(const FwdParams& p, int nsplit, bool precise_sin, int num_sms,
                            cudaStream_t stream);
-// single-pass forward / dgrad kernels run as CTA pairs (cta_group::2) unless POB_PAIR=0
-bool pair_mode_enabled();
 
 // flat fp32 parameters of one MLP in reference order (Dense_0..Dense_9: kernel [in,out] then
 // bias) -> packed images.  `nparams` = param_count(K).
 cudaError_t launch_pack_weights(const float* flat, int K, uint8_t* w_hi, uint8_t* w_lo,
                                 uint8_t* wt_hi, float* bias, cudaStream_t stream);
 
-cudaError_t launch_umma_probe(const void* a_img, uint32_t a_bytes, const void* b_img,
-                              uint32_t b_bytes, uint32_t b_off, const uint64_t* adesc,
-                              const uint64_t* bdesc, const uint32_t* dcol, const uint32_t* accum,
-                              int nops, uint32_t idesc, int out_cols, float* out,
-                              cudaStream_t stream);
-cudaError_t launch_umma_probe_pair(const void* a_img, uint32_t a_bytes, const void* b_img,
-                              uint32_t b_bytes, uint32_t b_off, const uint64_t* adesc,
-                              const uint64_t* bdesc, const uint32_t* dcol, const uint32_t* accum,
-                              int nops, uint32_t idesc, int out_cols, float* out,
-                              cudaStream_t stream);
 
 
 // ---- render.cu ------------------------------------------------------------------------------
@@ -120,8 +104,6 @@ struct BwdParams {
   const uint32_t* mask;     // [8][Mpad][8] from mlp_fwd
   uint8_t* save_dz;         // [ntile][8][64 KB]
   uint8_t* save_do;         // [ntile][32 KB]
-  unsigned long long* trace;   // optional cycle trace of CTA 0 (null = off): [2 roles][256] clock64 stamps
-  int debug_flags;          // timing experiments only (results invalid): 1 no tile copy-out, 2 no mask loads
 };
 cudaError_t launch_mlp_bwd(const BwdParams& p, int num_sms, cudaStream_t stream);
 

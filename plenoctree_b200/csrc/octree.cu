@@ -10,7 +10,7 @@
 // products, exp, sigmoid, compositing sums) may contract to FMA and uses the fast exp / reciprocal — the march is
 // instruction-issue bound (ncu: sm__throughput 73-79 %, DRAM 5 %), so instruction count is what matters.
 //
-// Thread mapping (B200-first, not svox's thread-per-ray): a *group* of G lanes owns one ray (G = 4 by default,
+// Thread mapping (GPU-first, not svox's thread-per-ray): a *group* of G lanes owns one ray (G = 4 by default,
 // see group_width(); 8 / 16 / 32 selectable for profiling).  All lanes of a group walk the tree together
 // (same-address loads broadcast), lane l owns basis functions l, l+G, ...: the 3K coefficient gather of a
 // contributing leaf is three coalesced segments per group instead of 3K strided scalar loads per thread, the dot
@@ -705,7 +705,7 @@ int tree_dev(const char* where, const pob_octree* t, TreeDev& T) {
     T.off[a] = t->offset[a];
     T.inv[a] = t->invradius[a];
   }
-  if (pob_sm_count_cached() <= 0) return pob_fail(where, "no sm_100 CUDA device (there is no CPU fallback)");
+  if (pob_sm_count_cached() <= 0) return pob_fail(where, "no sm_90 CUDA device (there is no CPU fallback)");
   return 0;
 }
 
@@ -860,7 +860,7 @@ int pob_octree_sgd_step(float* data_dev, float* grad_dev, int64_t n, float lr, v
   if (!data_dev || !grad_dev) return pob_fail(W, "NULL pointer");
   if (n < 0) return pob_fail(W, "negative size");
   const int sms = pob_sm_count_cached();
-  if (sms <= 0) return pob_fail(W, "no sm_100 CUDA device (there is no CPU fallback)");
+  if (sms <= 0) return pob_fail(W, "no sm_90 CUDA device (there is no CPU fallback)");
   if ((reinterpret_cast<uintptr_t>(data_dev) | reinterpret_cast<uintptr_t>(grad_dev)) & 15)
     return pob_fail(W, "data / grad must be 16-byte aligned");
   if (n == 0) return 0;
@@ -875,7 +875,7 @@ int pob_octree_adam_step(float* data_dev, float* grad_dev, float* m_dev, float* 
   const char* W = "pob_octree_adam_step";
   if (!data_dev || !grad_dev || !m_dev || !v_dev) return pob_fail(W, "NULL pointer");
   if (n < 0) return pob_fail(W, "negative size");
-  if (pob_sm_count_cached() <= 0) return pob_fail(W, "no sm_100 CUDA device (there is no CPU fallback)");
+  if (pob_sm_count_cached() <= 0) return pob_fail(W, "no sm_90 CUDA device (there is no CPU fallback)");
   if (n == 0) return 0;
   pob_count_launch();
   POB_CUDA(W, pob::launch_adam(data_dev, grad_dev, m_dev, v_dev, n, lr, step, nullptr, 0.9f, 0.999f, eps, 1.0f,
@@ -908,7 +908,7 @@ int pob_grid_weight_render(const float* sigma_grid_dev, int reso, const pob_came
   if (reso < 1 || reso > 2048) return pob_fail(W, "reso must be in [1, 2048]");
   if (n_cams < 0 || n_cams > 65535) return pob_fail(W, "n_cams must be in [0, 65535] per call");
   if (max_width < 1 || max_height < 1) return pob_fail(W, "bad image size");
-  if (pob_sm_count_cached() <= 0) return pob_fail(W, "no sm_100 CUDA device (there is no CPU fallback)");
+  if (pob_sm_count_cached() <= 0) return pob_fail(W, "no sm_90 CUDA device (there is no CPU fallback)");
   if (n_cams == 0) return 0;
   dim3 grid(unsigned(((max_width + 15) / 16) * ((max_height + 15) / 16)), unsigned(n_cams));
   pob_count_launch();

@@ -7,17 +7,17 @@
 namespace pob {
 
 // Work split of the wgrad launch.  The kernel is bound by the tile bytes each role streams
-// (128 KB per tile for the 256x256 layers, ~80-96 KB for Dense_0 / the skip rows / the heads).
+// (96 KB per tile and row half for the 256x256 layers, ~40-64 KB for Dense_0 / the skip rows / the heads).  Every
+// role gets an even number of CTAs: CTA index i of a role computes result rows [128 (i & 1), +128) over the tiles
+// i / 2, i / 2 + count / 2, ...
 int wgrad_assign_roles(WgradParams& p, int n_in, int role_start[WG_NUM_ROLES],
                        int role_count[WG_NUM_ROLES]) {
   int n = n_in < WG_MAX_CTAS ? n_in : WG_MAX_CTAS;
-  if (n < WG_NUM_ROLES) n = WG_NUM_ROLES;  // one CTA per role at the very least (they time-share SMs)
-  int small = (n * 8) / 100;               // per small role
-  if (small < 1) small = 1;
-  int big = (n - 3 * small) / 7;
-  if (big < 1) big = 1;
-  small = (n - 7 * big) / 3;
-  if (small < 1) small = 1;
+  if (n < 2 * WG_NUM_ROLES) n = 2 * WG_NUM_ROLES;  // one CTA per role and row half at the very least
+  auto even = [](int x) { return x < 2 ? 2 : x & ~1; };
+  int small = even((n * 8) / 100);         // per small role
+  const int big = even((n - 3 * small) / 7);
+  small = even((n - 7 * big) / 3);
   int cta = 0;
   for (int r = 0; r < WG_NUM_ROLES; ++r) {
     const int c = r < 7 ? big : small;
@@ -32,7 +32,7 @@ int wgrad_assign_roles(WgradParams& p, int n_in, int role_start[WG_NUM_ROLES],
   for (int i = cta; i < WG_MAX_CTAS; ++i) {   // spare CTAs idle (role -1)
     p.cta_role[i] = -1;
     p.cta_index[i] = 0;
-    p.cta_count[i] = 1;
+    p.cta_count[i] = 2;
   }
   return cta;
 }
@@ -89,15 +89,19 @@ __device__ __forceinline__ void locate(const ReduceArgs& a, int layer, int i, in
   }
 }
 
+// sum over the role's CTAs that computed the element: those of its result row half (the heads bias, a column
+// sum of dO, comes from row half 0)
 __device__ __forceinline__ float sum_partials(const ReduceArgs& a, int role, int off) {
+  const int pitch = role < 7 ? 256 : (role < 9 ? 64 : a.NH);
+  const int row = off < 65536 ? off / pitch : (role == 9 ? 0 : off - 65536);
   float s = 0.f;
   const float* p = a.partials + size_t(a.role_start[role]) * WG_PARTIAL_FLOATS + off;
-  for (int c = 0; c < a.role_count[role]; ++c) s += p[size_t(c) * WG_PARTIAL_FLOATS];
+  for (int c = row >> 7; c < a.role_count[role]; c += 2) s += p[size_t(c) * WG_PARTIAL_FLOATS];
   return s;
 }
 
 // grid (in tiles of 32, out tiles of 32, 10 layers + 1 bias slice), block (32, 8).  The trunk partials are
-// [out][in] (TMEM lane = out feature) and the flat gradient is flax's kernel [in][out]: every 32x32 tile is read
+// [out][in] (accumulator row = out feature) and the flat gradient is flax's kernel [in][out]: every 32x32 tile is read
 // along `in` (coalesced in the partials), summed over the role's CTAs, transposed through shared memory and written
 // along `out` (coalesced in the gradient).  (A one-thread-per-gradient-element version read with a 1 KB stride:
 // 64 us per step instead of ~15.)

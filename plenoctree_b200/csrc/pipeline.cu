@@ -39,7 +39,7 @@ struct Workspace {
 
 size_t up(size_t x) { return (x + 1023) / 1024 * 1024; }
 
-// tiles are scheduled four at a time (one CTA pair x two tiles): every per-tile array is padded to that unit
+// every per-tile array is padded to a multiple of four 128-row tiles (common.cuh: padded_rows)
 long long tiles_for(long long M) { return padded_rows(M) / TILE_M; }
 
 // deterministic carve of the caller-provided workspace

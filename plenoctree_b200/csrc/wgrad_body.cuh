@@ -2,21 +2,21 @@
 // wgrad_body.cuh — device body of mlp_wgrad.cu: weight-gradient contraction over samples (the wgrad half of jax.value_and_grad,
 // nerf_sh/train.py:116):   dW_l[out, in] = sum_s dZ_l[s, out] * h_{l-1}[s, in],  db_l = sum_s dZ_l[s, :]
 //
-// A 256x256 fp32 accumulator is exactly one SM's tensor memory (2 x 128 lanes x 256 columns), so
-// every persistent CTA owns ONE layer ("role") for the whole launch and streams the [sample x
-// feature] tile images that mlp_fwd (h_l, posenc) and mlp_bwd (dZ_l, dO) left in global memory.
-// Both MMA operands are read MN-major straight from those images (K = samples): no transposes.
-// dZ / dO / posenc tiles are K-major SW128 images (read MN-major with the same swizzle), the h_l tiles
-// are "T" images (no swizzle, 128 B core matrices; tests/test_umma_probe.py pins both conventions).
-// CTAs of the same role split the tiles round-robin and each writes an fp32 partial; reduce_grads
+// Every persistent CTA owns one layer ("role") and one half of its 256 result rows for the whole launch: a 128 x 256
+// fp32 accumulator is half of an SM's register file (two warpgroups, one m64n256 accumulator each), so the two row
+// halves of a role are separate CTAs.  A CTA streams the [sample x feature] tile images that mlp_fwd (h_l, posenc)
+// and mlp_bwd (dZ_l, dO) left in global memory; both wgmma operands are read MN-major straight from those images
+// (K = samples): no transposes.  dZ / dO / posenc tiles are K-major SW128 images (read MN-major with the same
+// swizzle), the h_l tiles are "T" images (no swizzle, 128 B core matrices; layouts.py: t_tile_offset).
+// CTAs of the same role and row half split the tiles round-robin and each writes an fp32 partial; reduce_grads
 // (optim.cu) sums the partials into the flat gradient (deterministic, no atomics).
 //
 // Roles: 0..6 = Dense_1,2,3,4,5(h4 rows),6,7   A = dZ_l (256 out)  B = h_{l-1} (256 in)
 //        7    = Dense_0                         A = dZ_0            B = posenc   (64)
 //        8    = Dense_5 (posenc rows)           A = dZ_5            B = posenc   (64)
 //        9    = heads (Dense_8 | Dense_9)       A = h_7 (256 in)    B = dO       (NH)  [transposed result]
-// Bias gradients are column sums of the A (or, for the heads, B) tile, computed by four otherwise
-// idle warps from the staged shared-memory tiles.
+// Bias gradients are column sums of the A (or, for the heads, B) tile, summed by the consumer warps from the staged
+// shared-memory tiles while their MMAs run.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -24,17 +24,18 @@ namespace pob {
 
 namespace {
 
-constexpr int WG_THREADS = 192;       // warps 0-3: bias sums + final drain, warp 4: loads, warp 5: MMA
-constexpr int WG_STAGES = 3;
+constexpr int WG_THREADS = 288;       // warps 0-7: two consumer warpgroups, warp 8: loads
+constexpr int WG_STAGES = 4;
 constexpr int WG_SUB = 64;            // samples per stage
-constexpr uint32_t WG_HALF = 4 * WG_SUB * 128;     // one operand sub-image: 4 chunks x 64 rows x 128 B
-constexpr uint32_t WG_STAGE_BYTES = 2 * WG_HALF;   // 64 KB
+constexpr uint32_t WG_PIECE = WG_SUB * 128;        // 64 samples x 128 B: one 64-feature chunk (SW128) / half a T group pair
+constexpr uint32_t WG_A_BYTES = 2 * WG_PIECE;      // the CTA's 128 A features
+constexpr uint32_t WG_B_MAX = 4 * WG_PIECE;        // up to 256 B features
+constexpr uint32_t WG_STAGE_BYTES = WG_A_BYTES + WG_B_MAX;   // 48 KB
 constexpr uint32_t WG_SMEM = WG_STAGES * WG_STAGE_BYTES;
 
 struct WgBarriers {
   uint64_t full[WG_STAGES];
   uint64_t empty[WG_STAGES];
-  uint64_t done;
 };
 
 struct RoleInfo {
@@ -68,87 +69,162 @@ __device__ __forceinline__ RoleInfo role_info(int role, int NH) {
   return r;
 }
 
+// MN-major operand descriptors.  SW128 images: LBO = next 64-feature chunk (8 KB), SBO = next 8 samples (1 KB).
+// T images: LBO = next 8 samples (128 B), SBO = next 8 features (512 B).
+constexpr uint64_t SW_DESC = make_sdesc_hi(WG_PIECE, 1024, LAYOUT_SW128);
+constexpr uint64_t T_DESC = make_sdesc_hi(128, 512, LAYOUT_NONE);
+
+// Consumer warpgroup `wg`: accumulates D[64 A features x NN] over the CTA's stages, then writes its rows of the
+// partial.  NN = MMA width (256, 64, or 80 for the heads, whose columns >= NH are never written back).
+template <int NN>
+__device__ __forceinline__ void wgrad_consume(const RoleInfo& R, uint8_t* smem, WgBarriers& bars, long long n_items,
+                                              int mh, float* out_w, float* out_b) {
+  const uint32_t warp = warp_id(), lane = lane_id();
+  const int wg = int(warp >> 2);
+  const int t = int(threadIdx.x & 127);
+  const uint32_t sbase = smem_u32(smem);
+  float acc[NN / 2];
+#pragma unroll
+  for (int i = 0; i < NN / 2; ++i) acc[i] = 0.f;
+
+  // bias column sums.  A features (this warpgroup's 64): thread -> feature pair 8*(t/32) + t%8, samples 16*((t%32)/8)..+16
+  // of every stage.  B features (heads, CTA row half 0, warpgroup 0): thread t < NH/2 -> pair t, all 64 samples.
+  const bool a_bias = R.has_bias && !R.bias_from_b;
+  const bool b_bias = R.bias_from_b && mh == 0 && wg == 0 && 2 * t < R.N;
+  const int fp = a_bias ? (t >> 5) * 8 + (t & 7) : t;
+  const int f = 2 * fp;
+  const int s_lo = a_bias ? 16 * ((t & 31) >> 3) : 0, s_n = a_bias ? 16 : 64;
+  const uint32_t bias_src = a_bias ? uint32_t(wg) * WG_PIECE : WG_A_BYTES + uint32_t(f >> 6) * WG_PIECE;
+  const uint32_t unit = uint32_t((f & 63) >> 3), wsel = uint32_t(f & 7) * 2;
+  float s0 = 0.f, s1 = 0.f;
+
+  uint32_t st = 0, phase = 0;
+  wgmma_fence();
+  for (long long i = 0; i < n_items; ++i) {
+    for (int sub = 0; sub < 2; ++sub) {
+      mbar_wait(smem_u32(&bars.full[st]), phase);
+      const uint32_t a0 = sbase + st * WG_STAGE_BYTES;
+      const uint32_t b0 = a0 + WG_A_BYTES;
+#pragma unroll
+      for (int ks = 0; ks < WG_SUB / 16; ++ks) {
+        // SW128: 16 samples = 2 KB.  T: 32-sample group = 8 KB (A half) / 16 KB (B), 16 samples inside it = 256 B.
+        const uint64_t ad = R.a_t ? sdesc(T_DESC, a0 + uint32_t(wg) * 4096u + uint32_t(ks >> 1) * 8192u + uint32_t(ks & 1) * 256u)
+                                  : sdesc(SW_DESC, a0 + uint32_t(wg) * WG_PIECE + uint32_t(ks) * 2048u);
+        const uint64_t bd = R.b_t ? sdesc(T_DESC, b0 + uint32_t(ks >> 1) * 16384u + uint32_t(ks & 1) * 256u)
+                                  : sdesc(SW_DESC, b0 + uint32_t(ks) * 2048u);
+        if constexpr (NN == 256) wgmma_m64n256<1, 1>(acc, ad, bd, 1u);
+        else if constexpr (NN == 80) wgmma_m64n80<1, 1>(acc, ad, bd, 1u);
+        else wgmma_m64n64<1, 1>(acc, ad, bd, 1u);
+      }
+      wgmma_commit();
+      if (a_bias || b_bias) {
+        const uint8_t* base = smem + st * WG_STAGE_BYTES + bias_src;
+#pragma unroll 4
+        for (int r = s_lo; r < s_lo + s_n; ++r) {
+          const float2 v = unpack_f16x2(
+              *reinterpret_cast<const uint32_t*>(base + r * 128 + ((unit ^ uint32_t(r & 7)) << 4) + wsel));
+          s0 += v.x;
+          s1 += v.y;
+        }
+      }
+      wgmma_wait<0>();
+      if (lane == 0) mbar_arrive(smem_u32(&bars.empty[st]));
+      if (++st == WG_STAGES) {
+        st = 0;
+        phase ^= 1;
+      }
+    }
+  }
+
+  // ---- partial of this CTA: rows [128 mh + 64 wg, +64) of D[A feature][B feature], row pitch R.N ----
+  const int fr = 16 * int(t >> 5) + int(lane >> 2), fc = 2 * int(lane & 3);
+#pragma unroll
+  for (int j = 0; j < NN / 8; ++j) {
+    const int n = 8 * j + fc;
+    if (n < R.N) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int m = 128 * mh + 64 * wg + fr + 8 * h;
+        *reinterpret_cast<float2*>(out_w + size_t(m) * R.N + n) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+      }
+    }
+  }
+  if (a_bias) {
+    s0 += __shfl_xor_sync(0xffffffffu, s0, 8);
+    s1 += __shfl_xor_sync(0xffffffffu, s1, 8);
+    s0 += __shfl_xor_sync(0xffffffffu, s0, 16);
+    s1 += __shfl_xor_sync(0xffffffffu, s1, 16);
+    if ((t & 31) < 8) {
+      out_b[128 * mh + 64 * wg + f] = s0;
+      out_b[128 * mh + 64 * wg + f + 1] = s1;
+    }
+  } else if (b_bias) {
+    out_b[f] = s0;
+    out_b[f + 1] = s1;
+  }
+}
+
 }  // namespace
-
-
-// One unit of work = one 128-sample tile (two 64-sample stages).
-struct WgItem {
-  const uint8_t* a_ptr;
-  const uint8_t* b_ptr;
-};
 
 // cta indexes cta_role/index/count and the partials
 __device__ __forceinline__ void wgrad_body(const WgradParams& p, uint8_t* smem, const int cta) {
   __shared__ __align__(8) WgBarriers bars;
-  __shared__ uint32_t tmem_base_s;
 
-  const uint32_t warp = warp_id(), lane = lane_id();
+  const uint32_t warp = warp_id();
   const uint32_t sbase = smem_u32(smem);
   const int role = p.cta_role[cta];
+  if (role < 0) return;   // spare CTA
   const int ridx = p.cta_index[cta];
   const int rcnt = p.cta_count[cta];
+  const int mh = ridx & 1;                       // result row half
+  const int sidx = ridx >> 1, scnt = rcnt >> 1;  // tile split among the role's CTAs of this half
   float* const out_w = p.partials + size_t(cta) * WG_PARTIAL_FLOATS;
   float* const out_b = out_w + 65536;
-  const RoleInfo R = role_info(role < 0 ? 0 : role, p.NH);
-  const uint32_t b_half_bytes = uint32_t(R.b_chunks) * WG_SUB * 128;
+  const RoleInfo R = role_info(role, p.NH);
+  const uint32_t b_bytes = R.b_t ? 4 * WG_PIECE : uint32_t(R.b_chunks) * WG_PIECE;
 
-  // work list: tiles t = ridx + i*rcnt
+  // work list: tiles t = sidx + i*scnt
   const long long total_tiles = p.seg_tiles;
-  const long long n_items = role < 0 ? 0 : ((total_tiles > ridx) ? (total_tiles - ridx + rcnt - 1) / rcnt : 0);
-
-  auto get_item = [&](long long i) -> WgItem {
-    WgItem it;
-    const long long lt = ridx + i * rcnt;
-    const WgradSegment& sg = p.seg;
-    it.a_ptr = (R.a_kind == 0 ? sg.dz : sg.h) + (size_t(lt) * NUM_TRUNK + R.a_layer) * A_TILE_BYTES;
-    if (R.b_kind == 0) it.b_ptr = sg.h + (size_t(lt) * NUM_TRUNK + R.b_layer) * A_TILE_BYTES;
-    else if (R.b_kind == 1) it.b_ptr = sg.e + size_t(lt) * E_TILE_BYTES;
-    else it.b_ptr = sg.d_o + size_t(lt) * (2 * A_CHUNK_BYTES);
-    return it;
-  };
+  const long long n_items = (total_tiles > sidx) ? (total_tiles - sidx + scnt - 1) / scnt : 0;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < WG_STAGES; ++i) {
       mbar_init(smem_u32(&bars.full[i]), 1);
-      mbar_init(smem_u32(&bars.empty[i]), 5);
+      mbar_init(smem_u32(&bars.empty[i]), 8);   // one arrival per consumer warp
     }
-    mbar_init(smem_u32(&bars.done), 1);
     fence_mbar_init();
   }
-  if (warp == 4) tmem_alloc(smem_u32(&tmem_base_s), 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_base_s;
-  bool any_mma = false;
 
-  if (warp == 4) {
+  if (warp == 8) {
     // ================================ loader ====================================
-    // whole-warp control flow, one elected lane issues (see mlp_fwd.cu)
+    // whole-warp control flow, one elected lane issues
+    const WgradSegment& sg = p.seg;
     uint32_t st = 0, phase = 0;
     for (long long i = 0; i < n_items; ++i) {
-      const WgItem it = get_item(i);
+      const long long lt = sidx + i * scnt;
+      const uint8_t* a_ptr = (R.a_kind == 0 ? sg.dz : sg.h) + (size_t(lt) * NUM_TRUNK + R.a_layer) * A_TILE_BYTES;
+      const uint8_t* b_ptr = R.b_kind == 0 ? sg.h + (size_t(lt) * NUM_TRUNK + R.b_layer) * A_TILE_BYTES
+                             : R.b_kind == 1 ? sg.e + size_t(lt) * E_TILE_BYTES
+                                             : sg.d_o + size_t(lt) * (2 * A_CHUNK_BYTES);
       for (int sub = 0; sub < 2; ++sub) {
         mbar_wait(smem_u32(&bars.empty[st]), phase ^ 1);
         if (elect_one()) {
-          mbar_arrive_expect_tx(smem_u32(&bars.full[st]), WG_HALF + b_half_bytes);
+          const uint32_t bar = smem_u32(&bars.full[st]);
+          mbar_arrive_expect_tx(bar, WG_A_BYTES + b_bytes);
           const uint32_t dst = sbase + st * WG_STAGE_BYTES;
-          // SW128 images: 64 rows of each 64-column chunk; T images: two whole 32-row groups (contiguous)
-          if (R.a_t) {
-            bulk_g2s(dst, it.a_ptr + size_t(sub) * WG_HALF, WG_HALF, smem_u32(&bars.full[st]));
-          } else {
 #pragma unroll
-            for (int c = 0; c < 4; ++c)
-              bulk_g2s(dst + c * (WG_SUB * 128), it.a_ptr + size_t(c) * A_CHUNK_BYTES + sub * (WG_SUB * 128),
-                       WG_SUB * 128, smem_u32(&bars.full[st]));
+          for (int c = 0; c < 2; ++c) {
+            if (R.a_t)   // T image: this half's 128 features = 8 KB of each 32-sample group
+              bulk_g2s(dst + c * WG_PIECE, a_ptr + size_t(2 * sub + c) * 16384 + mh * WG_PIECE, WG_PIECE, bar);
+            else         // SW128 image: 64 samples of chunks 2 mh, 2 mh + 1
+              bulk_g2s(dst + c * WG_PIECE, a_ptr + size_t(2 * mh + c) * A_CHUNK_BYTES + sub * WG_PIECE, WG_PIECE, bar);
           }
           if (R.b_t) {
-            bulk_g2s(dst + WG_HALF, it.b_ptr + size_t(sub) * WG_HALF, WG_HALF, smem_u32(&bars.full[st]));
+            bulk_g2s(dst + WG_A_BYTES, b_ptr + size_t(sub) * 4 * WG_PIECE, 4 * WG_PIECE, bar);
           } else {
             for (int c = 0; c < R.b_chunks; ++c)
-              bulk_g2s(dst + WG_HALF + c * (WG_SUB * 128),
-                       it.b_ptr + size_t(c) * A_CHUNK_BYTES + sub * (WG_SUB * 128), WG_SUB * 128,
-                       smem_u32(&bars.full[st]));
+              bulk_g2s(dst + WG_A_BYTES + c * WG_PIECE, b_ptr + size_t(c) * A_CHUNK_BYTES + sub * WG_PIECE, WG_PIECE, bar);
           }
         }
         __syncwarp();
@@ -158,110 +234,11 @@ __device__ __forceinline__ void wgrad_body(const WgradParams& p, uint8_t* smem, 
         }
       }
     }
-  } else if (warp == 5) {
-    // ================================= MMA ======================================
-    uint32_t st = 0, phase = 0;
-    const uint32_t idesc = make_idesc_f16(128, R.N, 1, 1);
-    // MN-major SW128: LBO = stride between 64-feature chunks (8 KB here), SBO = 8-sample group
-    constexpr uint64_t DESC_HI = make_sdesc_hi(1024, LAYOUT_SW128) | (uint64_t((WG_SUB * 128) >> 4) << 16);
-    // MN-major, no swizzle (T images): LBO = next 8 samples = 128 B, SBO = next 8 features = 512 B
-    constexpr uint64_t T_HI = make_sdesc_hi(512, LAYOUT_NONE) | (uint64_t(128 >> 4) << 16);
-    bool first = true;
-    for (long long i = 0; i < n_items; ++i) {
-      for (int sub = 0; sub < 2; ++sub) {
-        mbar_wait(smem_u32(&bars.full[st]), phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a0 = sbase + st * WG_STAGE_BYTES;
-          const uint64_t ad0 = (R.a_t ? T_HI : DESC_HI) | uint64_t((a0 >> 4) & 0x3FFF);
-          const uint64_t bd0 = (R.b_t ? T_HI : DESC_HI) | uint64_t(((a0 + WG_HALF) >> 4) & 0x3FFF);
-#pragma unroll
-          for (int ks = 0; ks < WG_SUB / 16; ++ks) {
-            const uint32_t acc = !(first && sub == 0 && ks == 0);
-            // SW128: 16 samples = 2048 bytes = +128 encoded; features 128..255 = +2 chunks = +1024 encoded
-            // T    : 32-sample group = 16 KB = +1024 encoded, 16 samples inside it = 256 B = +16 encoded;
-            //        features 128..255 = 16 units x 512 B = +512 encoded
-            const uint32_t sw_k = uint32_t(ks) * 128u, t_k = uint32_t(ks >> 1) * 1024u + uint32_t(ks & 1) * 16u;
-            const uint64_t ad = ad0 + (R.a_t ? t_k : sw_k), bd = bd0 + (R.b_t ? t_k : sw_k);
-            umma_f16(tmem, ad, bd, idesc, acc);
-            umma_f16(tmem + 256, ad + (R.a_t ? 512u : 1024u), bd, idesc, acc);
-          }
-          umma_commit(smem_u32(&bars.empty[st]));
-        }
-        __syncwarp();
-        if (++st == WG_STAGES) {
-          st = 0;
-          phase ^= 1;
-        }
-      }
-      first = false;
-    }
-    if (elect_one()) umma_commit(smem_u32(&bars.done));
-    __syncwarp();
-  } else if (warp < 4) {
-    // ========================= bias column sums (warps 0-3) ======================
-    const int fp = threadIdx.x;            // feature pair 0..127 -> features 2fp, 2fp+1
-    float s0 = 0.f, s1 = 0.f;
-    uint32_t st = 0, phase = 0;
-    const int nfeat = R.bias_from_b ? R.N : 256;
-    const bool active = R.has_bias && (2 * fp < nfeat);
-    const uint32_t src_off = (R.bias_from_b ? WG_HALF : 0) + uint32_t(fp >> 5) * (WG_SUB * 128);
-    const uint32_t unit = uint32_t(fp & 31) >> 2, wsel = uint32_t(fp & 3) * 4;
-    for (long long i = 0; i < n_items; ++i) {
-      any_mma = true;
-      for (int sub = 0; sub < 2; ++sub) {
-        mbar_wait(smem_u32(&bars.full[st]), phase);
-        if (active) {
-          const uint8_t* base = smem + st * WG_STAGE_BYTES + src_off;
-#pragma unroll 8
-          for (int r = 0; r < WG_SUB; ++r) {
-            const uint32_t w =
-                *reinterpret_cast<const uint32_t*>(base + r * 128 + ((unit ^ uint32_t(r & 7)) << 4) + wsel);
-            const float2 f = unpack_f16x2(w);
-            s0 += f.x;
-            s1 += f.y;
-          }
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&bars.empty[st]));
-        if (++st == WG_STAGES) {
-          st = 0;
-          phase ^= 1;
-        }
-      }
-    }
-    if (role >= 0) {
-      out_b[2 * fp] = active ? s0 : 0.f;
-      out_b[2 * fp + 1] = active ? s1 : 0.f;
-    }
-    // ============================ drain accumulators =============================
-    mbar_wait(smem_u32(&bars.done), 0);
-    tc_fence_after();
-    const int m = threadIdx.x;  // TMEM lane
-    if (role >= 0) {
-#pragma unroll 1
-      for (int half = 0; half < 2; ++half) {
-        float* dst = out_w + size_t(half * 128 + m) * R.N;
-        for (int c0 = 0; c0 < R.N; c0 += 16) {
-          uint32_t v[16];
-          if (any_mma) {
-            tmem_ld16(tmem + (uint32_t(warp * 32) << 16) + half * 256 + c0, v);
-            tmem_ld_wait();
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = 0u;
-          }
-#pragma unroll
-          for (int j = 0; j < 16; j += 4)
-            *reinterpret_cast<uint4*>(dst + c0 + j) = make_uint4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-        }
-      }
-    }
+    return;
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) tmem_dealloc(tmem, 512);
+  if (R.N == 256) wgrad_consume<256>(R, smem, bars, n_items, mh, out_w, out_b);
+  else if (R.N == 64) wgrad_consume<64>(R, smem, bars, n_items, mh, out_w, out_b);
+  else wgrad_consume<MAX_NH>(R, smem, bars, n_items, mh, out_w, out_b);
 }
 
 }  // namespace pob

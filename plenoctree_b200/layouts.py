@@ -1,15 +1,13 @@
-"""numpy mirrors of the shared-memory operand layouts and tcgen05 descriptors of csrc/common.cuh.
+"""numpy mirrors of the shared-memory operand layouts of csrc/common.cuh.
 
-Used by the tests to build operand images for the UMMA probe and to check the device pack
-kernel; kept next to the product code because the layouts are part of the kernel contract.
+Used by the tests to build operand images and to check the device pack kernel; kept next to the
+product code because the layouts are part of the kernel contract.
 """
 import numpy as np
 
 TILE_M = 128
 A_CHUNK_BYTES = 128 * 128
 WSLOT_BYTES = 256 * 64
-
-LAYOUT_NONE, LAYOUT_SW128, LAYOUT_SW64, LAYOUT_SW32 = 0, 2, 4, 6
 
 
 def a_tile_offset(row, col):
@@ -49,7 +47,7 @@ def unpack_a_tile(img, cols):
 def t_tile_offset(row, col):
     """byte offset of fp16 element (row, col) in a "T" tile image: [32-row group][8-column unit]
     [row in group][16 B].  mlp_fwd writes the saved h_l tiles in this order (one coalesced 512 B
-    store per warp instruction straight from the epilogue registers); read MN-major by the tensor
+    store per warp instruction); read MN-major by the tensor
     cores it is the canonical no-swizzle layout with 128 B core matrices (8 rows x 8 columns):
     LBO (next 8 rows) = 128 B, SBO (next 8 columns) = 512 B."""
     row = np.asarray(row)
@@ -80,15 +78,6 @@ def pack_w_slot(mat):
     r, c = np.meshgrid(np.arange(rows), np.arange(32), indexing="ij")
     img.view(np.uint16)[w_slot_offset(r, c) // 2] = mat.astype(np.float16).view(np.uint16)
     return img
-
-
-def make_idesc_f16(M, N, a_mn_major=0, b_mn_major=0):
-    return (1 << 4) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) | ((M >> 4) << 24)
-
-
-def make_sdesc(addr, lbo_bytes, sbo_bytes, layout):
-    return (((addr >> 4) & 0x3FFF) | (((lbo_bytes >> 4) & 0x3FFF) << 16)
-            | (((sbo_bytes >> 4) & 0x3FFF) << 32) | (1 << 46) | (layout << 61))
 
 
 # ---- flat parameter layout / packed image geometry (mirrors csrc/kernels.h, pack.cu) ---------

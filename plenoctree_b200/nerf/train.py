@@ -1,6 +1,6 @@
 """train_step of the reference (nerf_sh/train.py:51-121) on the CUDA library.
 
-    loss_fn + value_and_grad   -> lib.pob_loss_and_grad   (fused tcgen05 forward / dgrad / wgrad)
+    loss_fn + value_and_grad   -> lib.pob_loss_and_grad   (fused wgmma forward / dgrad / wgrad)
     lax.pmean(grad, "batch")   -> two torch.distributed all-reduces on the flat gradient (NCCL): the MLP_0 bucket
                                   on a side stream while the MLP_1 backward still runs, then [MLP_1 | stats]
     optimizer.apply_gradient   -> lib.pob_adam_update      (flax Adam + operand re-pack)

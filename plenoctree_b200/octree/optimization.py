@@ -50,10 +50,10 @@ def exchange_gradients(tree, sparse=True):
     sparse: an image's row slab only reaches the leaves its rays cross, so each rank compacts the rows of its
             buffer that received a gradient (indices + values), the ranks all-gather those lists (padded to the
             longest) and add the other ranks' rows into their own buffers.  One host read of the row counts per image.
-            Measured on 4 B200s (256^3-equivalent tree, 800x800 images; bench_extras c5_octree_opt): the four row
-            slabs of one image touch 41 k / 317 k / 369 k / 44 k of the tree's 926 k rows — 83 % of all rows between
-            them — so the padded lists (75 MB per rank) outweigh the 181 MB all-reduce: 2.89 ms per image against
-            1.77 ms dense.  A per-image gradient is dense over the visible leaves; the default stays dense.
+            With 4 ranks (256^3-equivalent tree, 800x800 images; bench_extras c5_octree_opt) the four row slabs of one
+            image touch 41 k / 317 k / 369 k / 44 k of the tree's 926 k rows — 83 % of all rows between them — so the
+            padded lists (75 MB per rank) outweigh the 181 MB all-reduce.  A per-image gradient is dense over the
+            visible leaves; the default stays dense.
     Returns a small dict describing what was exchanged."""
     import torch.distributed as dist
     rank, world = _rank_world()

@@ -87,27 +87,6 @@ def eval_grid(blob, sh_deg, reso, offset, scale, x0=0, nx=None, ny=None, nz=None
     return rgb, sig
 
 
-def umma_probe(a_img, b_img, b_off, adesc, bdesc, dcol, accum, idesc, out_cols, pair=False):
-    """Run tcgen05.mma ops on raw smem images; returns the [128, out_cols] fp32 accumulator
-    (pair=True: cta_group::2 on a CTA pair, images are [2, bytes], returns [256, out_cols])."""
-    dev = "cuda"
-    a = torch.from_numpy(np.ascontiguousarray(a_img)).to(dev)
-    b = torch.from_numpy(np.ascontiguousarray(b_img)).to(dev)
-    ad = torch.from_numpy(np.asarray(adesc, dtype=np.uint64).view(np.int64)).to(dev)
-    bd = torch.from_numpy(np.asarray(bdesc, dtype=np.uint64).view(np.int64)).to(dev)
-    dc = torch.from_numpy(np.asarray(dcol, dtype=np.uint32).view(np.int32)).to(dev)
-    ac = torch.from_numpy(np.asarray(accum, dtype=np.uint32).view(np.int32)).to(dev)
-    out = torch.zeros((256 if pair else 128, out_cols), dtype=torch.float32, device=dev)
-    if pair:
-        check(lib.pob_umma_probe_pair(ptr(a), a.numel() // 2, ptr(b), b.numel() // 2, b_off, ptr(ad), ptr(bd),
-                                      ptr(dc), ptr(ac), len(adesc), idesc, out_cols, ptr(out), stream_ptr()))
-    else:
-        check(lib.pob_umma_probe(ptr(a), a.numel(), ptr(b), b.numel(), b_off, ptr(ad), ptr(bd), ptr(dc),
-                                 ptr(ac), len(adesc), idesc, out_cols, ptr(out), stream_ptr()))
-    torch.cuda.synchronize()
-    return out.cpu().numpy()
-
-
 def grid_slab(reso, rank, world):
     """x-slab [x0, x0+nx) of the extraction grid owned by `rank` (voxel slabs, no collective)."""
     base, rem = divmod(reso, world)

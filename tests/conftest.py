@@ -10,7 +10,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu on a GPU machine)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -22,7 +22,7 @@ def pytest_collection_modifyitems(config, items):
         has_gpu = False
     if has_gpu:
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (B200); run with -m gpu on the GPU box")
+    skip = pytest.mark.skip(reason="needs a CUDA device (H100); run with -m gpu on a GPU machine")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)
