@@ -26,7 +26,6 @@ constexpr int A_TILE_BYTES  = 4 * A_CHUNK_BYTES;   // [128 x 256] fp16 = 64 KB
 constexpr int E_TILE_BYTES  = A_CHUNK_BYTES;       // [128 x 64]  fp16 = 16 KB
 constexpr int WSLOT_K       = 32;                  // K extent of one streamed weight slot
 constexpr int WSLOT_BYTES   = WIDTH * WSLOT_K * 2; // [256 x 32] fp16, SW64 = 16 KB
-constexpr int NUM_WSLOTS    = 4;                   // weight ring depth
 constexpr int MAX_NH        = 80;                  // padded heads width (1 + 3*25 -> 80)
 // Rows of every per-sample training array (tile images, relu masks), padded to a multiple of 512 rows; the
 // training forward evaluates the padded rows too (clamped to the last sample), so every saved tile is finite.

@@ -31,18 +31,27 @@ constexpr int FWD_THREADS = 384;
 constexpr int HEADS_N = 80;               // heads MMA width: MAX_NH (rows >= NH of a heads slot are never read back)
 constexpr int STAGE_PITCH = HEADS_N + 1;  // heads staging: odd pitch -> conflict-free per-row scalar access
 
-// dynamic smem map
-constexpr uint32_t SM_A0 = 0;                           // activations, fp16 (hi)
-constexpr uint32_t SM_A1 = SM_A0 + A_TILE_BYTES;        // residual (x3 only)
-constexpr uint32_t SM_E0 = SM_A1 + A_TILE_BYTES;
-constexpr uint32_t SM_E1 = SM_E0 + E_TILE_BYTES;
-constexpr uint32_t SM_W = SM_E1 + E_TILE_BYTES;
-constexpr uint32_t SM_TOTAL = SM_W + NUM_WSLOTS * WSLOT_BYTES;  // 229376
-static_assert(SM_TOTAL == 224 * 1024, "smem map");
-
+// dynamic smem map: activation tile, posenc tile, weight ring.  The x3 mode also keeps the residual (lo) tiles and
+// runs a ring of four slots (two hi/lo pairs).  The training forward (fp16, SAVE) gives those 80 KB to the ring, nine
+// slots: a slot is handed back only once both warpgroups are done with it, so the ring depth bounds how far one
+// warpgroup can run ahead while the other stores its saved tiles.  The non-saving fp16 forward measured no gain from
+// the deeper ring and keeps the x3 map (DESIGN.md §6).
+constexpr uint32_t SM_TOTAL = 224 * 1024;
+template <int NSPLIT, bool SAVE>
+struct Smem {
+  static constexpr bool DEEP = NSPLIT == 1 && SAVE;
+  static constexpr uint32_t A0 = 0;                                              // activations, fp16 (hi)
+  static constexpr uint32_t A1 = A0 + A_TILE_BYTES;                              // residual (x3 only)
+  static constexpr uint32_t E0 = DEEP ? A0 + A_TILE_BYTES : A1 + A_TILE_BYTES;
+  static constexpr uint32_t E1 = E0 + E_TILE_BYTES;                              // x3 only
+  static constexpr uint32_t W = DEEP ? E0 + E_TILE_BYTES : E1 + E_TILE_BYTES;
+  static constexpr int SLOTS = int((SM_TOTAL - W) / WSLOT_BYTES);
+  static_assert(SLOTS == (DEEP ? 9 : 4), "smem map");
+};
+template <int SLOTS>
 struct Barriers {
-  uint64_t full[NUM_WSLOTS];
-  uint64_t empty[NUM_WSLOTS];
+  uint64_t full[SLOTS];
+  uint64_t empty[SLOTS];
 };
 
 __device__ __noinline__ void load_point(const FwdParams& p, long long s, float& x, float& y,
@@ -143,7 +152,8 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
   extern __shared__ __align__(1024) uint8_t smem[];
   constexpr bool PRECISE = (NSPLIT == 3);
   constexpr int STEP = NSPLIT == 3 ? 2 : 1;   // ring slots per K-slot (hi, lo)
-  __shared__ __align__(8) Barriers bars;
+  using SM = Smem<NSPLIT, SAVE>;
+  __shared__ __align__(8) Barriers<SM::SLOTS> bars;
 
   // training launches cover the padded rows: mlp_bwd / mlp_wgrad read every tile of the padded arrays
   const long long num_tiles = SAVE ? padded_rows(p.M) / TILE_M : (p.M + TILE_M - 1) / TILE_M;
@@ -152,7 +162,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
   const int NH = p.NH;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < NUM_WSLOTS; ++i) {
+    for (int i = 0; i < SM::SLOTS; ++i) {
       mbar_init(smem_u32(&bars.full[i]), 1);
       mbar_init(smem_u32(&bars.empty[i]), 8);   // one arrival per consumer warp
     }
@@ -177,11 +187,11 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
             mbar_wait(smem_u32(&bars.empty[slot]), phase ^ 1);
             if (elect_one()) {
               mbar_arrive_expect_tx(smem_u32(&bars.full[slot]), bytes);
-              bulk_g2s(sbase + SM_W + slot * WSLOT_BYTES, (part == 0 ? p.w.w_hi : p.w.w_lo) + off, bytes,
+              bulk_g2s(sbase + SM::W + slot * WSLOT_BYTES, (part == 0 ? p.w.w_hi : p.w.w_lo) + off, bytes,
                        smem_u32(&bars.full[slot]));
             }
             __syncwarp();
-            if (++slot == NUM_WSLOTS) {
+            if (++slot == SM::SLOTS) {
               slot = 0;
               phase ^= 1;
             }
@@ -200,10 +210,10 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
   const int wq = t >> 5;                                   // warp within the warpgroup
   const int fr = 16 * wq + int(lane >> 2);                 // fragment row (and fr + 8) within the warpgroup's rows
   const int fc = 2 * int(lane & 3);                        // fragment column offset within an 8-column group
-  uint8_t* const a_hi = smem + SM_A0;
-  uint8_t* const a_lo = smem + SM_A1;
-  uint8_t* const e_hi = smem + SM_E0;
-  uint8_t* const e_lo = smem + SM_E1;
+  uint8_t* const a_hi = smem + SM::A0;
+  uint8_t* const a_lo = smem + SM::A1;
+  uint8_t* const e_hi = smem + SM::E0;
+  uint8_t* const e_lo = smem + SM::E1;
   const uint32_t rows_off = uint32_t(wg) * 64u * 128u;     // this warpgroup's 64 rows inside every 128-row chunk
   constexpr uint64_t A_DESC = make_sdesc_hi(16, 1024, LAYOUT_SW128);
   constexpr uint64_t W_DESC = make_sdesc_hi(16, 512, LAYOUT_SW64);
@@ -236,9 +246,9 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
         const bool from_e = (l == 0) || j >= 8;
         const int kk = bias_slot ? 1 : ((l == SKIP_LAYER && j >= 8) ? j - 8 : j);
         const uint32_t a_off = uint32_t(kk >> 1) * A_CHUNK_BYTES + rows_off + uint32_t(kk & 1) * 64u;
-        const uint32_t ah = sbase + (from_e ? SM_E0 : SM_A0) + a_off;
-        const uint32_t al = sbase + (from_e ? SM_E1 : SM_A1) + a_off;
-        const uint32_t bh = sbase + SM_W + slot * WSLOT_BYTES;
+        const uint32_t ah = sbase + (from_e ? SM::E0 : SM::A0) + a_off;
+        const uint32_t al = sbase + (from_e ? SM::E1 : SM::A1) + a_off;
+        const uint32_t bh = sbase + SM::W + slot * WSLOT_BYTES;
         const uint32_t bl = bh + WSLOT_BYTES;   // x3 only; the ring depth is even: hi/lo never straddle the wrap
         mbar_wait(smem_u32(&bars.full[slot]), phase);
         if (NSPLIT == 3) mbar_wait(smem_u32(&bars.full[slot + 1]), phase);
@@ -272,7 +282,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
         }
         prev = slot;
         slot += STEP;
-        if (slot == NUM_WSLOTS) {
+        if (slot == SM::SLOTS) {
           slot = 0;
           phase ^= 1;
         }
