@@ -149,6 +149,12 @@ def heads_matrix(flat, K):
     return Wh, bh
 
 
+def heads_column(K, o):
+    """packed heads column of Dense_9 output o (reference channel-major order c*K + k)."""
+    c, k = divmod(o, K)
+    return 1 + 3 * k + c
+
+
 def pack_reference(flat, sh_deg):
     """numpy model of pack.cu: returns dict of uint8 images w_hi, w_lo, wt_hi and float32 bias."""
     K = K_of(sh_deg)
@@ -217,3 +223,162 @@ def pack_reference(flat, sh_deg):
         bias[l * 256:(l + 1) * 256] = flat[b_off[l]:b_off[l] + 256]
     bias[2048:2048 + NH] = bh
     return dict(w_hi=w_hi, w_lo=w_lo, wt_hi=wt_hi, bias=bias)
+
+
+# ---- training workspace (mirrors carve() in csrc/pipeline.cu) ------------------------------------------------------
+# Every intermediate of pob_loss_and_grad stays in the caller's workspace, so that a test can check each kernel of the
+# training chain on its own, with the GPU's own inputs.  The decoders below turn those bytes into torch tensors on the
+# workspace's device (the production step's tiles are far too large for numpy).
+NUM_TRUNK = 8
+A_TILE_BYTES = 4 * A_CHUNK_BYTES          # [128 x 256] fp16
+E_TILE_BYTES = A_CHUNK_BYTES              # [128 x 64] fp16
+DO_TILE_BYTES = 2 * A_CHUNK_BYTES         # [128 x 128] fp16
+WG_MAX_CTAS = 160
+WG_PARTIAL_FLOATS = 65536 + 256
+
+
+def padded_rows(M):
+    """rows of every per-sample training array: a multiple of four 128-row tiles (common.cuh: padded_rows)."""
+    return (M + 511) // 512 * 512
+
+
+def train_workspace_views(cfg, n_rays, sparsity_on):
+    """Byte layout of the training workspace of `cfg` (a RenderConfig or anything with its fields) for a
+    pob_loss_and_grad call over `n_rays` rays; `sparsity_on` = the call carries the sparsity points (weight > 0).
+
+    Returns dict(total=bytes, partials=[offsets], levels=[...]) with one entry per level (coarse, then fine when
+    num_fine_samples > 0).  Each level holds (offset, shape) pairs for z, rgbs, weights, comp, disp, acc (float32;
+    rgbs and G as [rows, 4]), G, H [tiles, 8, 64 KB], E [tiles, 16 KB], DZ [tiles, 8, 64 KB], DO [tiles, 32 KB]
+    (uint8 tile images) and mask [8, rows, 8] (uint32 words), sized for this call, plus the call's row counts:
+    N samples per ray, M_rays, M (with the sparsity rows, which ride behind the rays of the last level), rows
+    (= padded_rows(M)) and tiles.  Buffers are carved for cfg.max_rays; the mask's per-layer stride is the call's
+    padded row count."""
+    R = int(cfg.max_rays)
+    nc, nf, nsp = int(cfg.num_coarse_samples), int(cfg.num_fine_samples), int(cfg.sparsity_npoints)
+    Ns = [nc, nc + nf if nf > 0 else 0]
+    last = 1 if nf > 0 else 0
+    off = 0
+    levels = []
+
+    def take(nbytes):
+        nonlocal off
+        o = off
+        off += (nbytes + 1023) // 1024 * 1024
+        return o
+
+    for lv in range(2):
+        Mr_cap = R * Ns[lv]
+        M_cap = Mr_cap + (nsp if lv == last else 0)
+        tiles_cap = padded_rows(M_cap) // TILE_M
+        if Mr_cap == 0:
+            continue
+        N = Ns[lv]
+        M_rays = n_rays * N
+        M = M_rays + (nsp if (lv == last and sparsity_on) else 0)
+        rows = padded_rows(M)
+        tiles = rows // TILE_M
+        v = dict(N=N, M_rays=M_rays, M=M, rows=rows, tiles=tiles)
+        v["z"] = (take(4 * Mr_cap), (n_rays, N))
+        v["rgbs"] = (take(16 * M_cap), (M, 4))
+        v["weights"] = (take(4 * Mr_cap), (n_rays, N))
+        v["comp"] = (take(12 * R), (n_rays, 3))
+        v["disp"] = (take(4 * R), (n_rays,))
+        v["acc"] = (take(4 * R), (n_rays,))
+        v["G"] = (take(16 * M_cap), (M, 4))
+        v["H"] = (take(tiles_cap * NUM_TRUNK * A_TILE_BYTES), (tiles, NUM_TRUNK, A_TILE_BYTES))
+        v["E"] = (take(tiles_cap * E_TILE_BYTES), (tiles, E_TILE_BYTES))
+        v["DZ"] = (take(tiles_cap * NUM_TRUNK * A_TILE_BYTES), (tiles, NUM_TRUNK, A_TILE_BYTES))
+        v["DO"] = (take(tiles_cap * DO_TILE_BYTES), (tiles, DO_TILE_BYTES))
+        v["mask"] = (take(NUM_TRUNK * tiles_cap * TILE_M * 8 * 4), (NUM_TRUNK, rows, 8))
+        levels.append(v)
+    partials = [take(4 * WG_MAX_CTAS * WG_PARTIAL_FLOATS) for _ in range(2)]
+    return dict(total=off, levels=levels, partials=partials)
+
+
+_VIEW_DTYPES = dict(z="float32", rgbs="float32", weights="float32", comp="float32", disp="float32", acc="float32",
+                    G="float32", H="uint8", E="uint8", DZ="uint8", DO="uint8", mask="int32")
+
+
+def workspace_view(ws, level, name):
+    """torch view of buffer `name` of one level (an entry of train_workspace_views()["levels"]) in the uint8
+    workspace tensor `ws`."""
+    import torch
+    off, shape = level[name]
+    dt = getattr(torch, _VIEW_DTYPES[name])
+    n = int(np.prod(shape)) * torch.empty((), dtype=dt).element_size()
+    return ws[off:off + n].view(dt).view(shape)
+
+
+_GATHER = {}
+
+
+def _gather_index(kind, device):
+    """int64 [128 * cols] index of fp16 element (row, col) of one tile image, row-major over (row, col)."""
+    import torch
+    key = (kind, str(device))
+    if key not in _GATHER:
+        cols = {"T": 256, "A256": 256, "A128": 128, "A64": 64}[kind]
+        r, c = np.meshgrid(np.arange(TILE_M), np.arange(cols), indexing="ij")
+        off = t_tile_offset(r, c) if kind == "T" else a_tile_offset(r, c)
+        _GATHER[key] = torch.from_numpy((off // 2).reshape(-1).astype(np.int64)).to(device)
+    return _GATHER[key]
+
+
+def _decode(tiles_u8, kind, cols):
+    import torch
+    T = tiles_u8.shape[0]
+    u16 = tiles_u8.reshape(T, -1).view(torch.int16)
+    return u16[:, _gather_index(kind, tiles_u8.device)].view(torch.float16).reshape(T * TILE_M, cols)
+
+
+def decode_h(H, layer):
+    """H [tiles, 8, 64 KB] (T layout) -> fp16 h_layer [tiles * 128, 256]."""
+    return _decode(H[:, layer].contiguous(), "T", 256)
+
+
+def decode_dz(DZ, layer):
+    """DZ [tiles, 8, 64 KB] (SW128) -> fp16 dz_layer [tiles * 128, 256]."""
+    return _decode(DZ[:, layer].contiguous(), "A256", 256)
+
+
+def decode_e(E):
+    """E [tiles, 16 KB] (SW128) -> fp16 posenc [tiles * 128, 64] (column 63 = 1)."""
+    return _decode(E, "A64", 64)
+
+
+def decode_do(DO):
+    """DO [tiles, 32 KB] (SW128) -> fp16 dO [tiles * 128, 128] (packed heads columns: sigma, then 1 + 3k + c)."""
+    return _decode(DO, "A128", 128)
+
+
+def mask_bit_of_column():
+    """bit of column j (0..31) inside its mask word: column 2k -> bit 15 - k, column 2k + 1 -> bit 31 - k."""
+    j = np.arange(32)
+    return np.where(j % 2 == 0, 15 - j // 2, 31 - j // 2)
+
+
+def decode_mask(words):
+    """mask words [..., rows, 8] (int32 or uint32) -> bool [..., rows, 256]; word c covers columns 32c..32c+31."""
+    import torch
+    w = torch.as_tensor(words)
+    w = (w.to(torch.int64) & 0xFFFFFFFF)
+    col = np.arange(256)
+    word = torch.from_numpy(col // 32).to(w.device)
+    bit = torch.from_numpy(mask_bit_of_column()[col % 32].astype(np.int64)).to(w.device)
+    return ((w[..., word] >> bit) & 1).bool()
+
+
+def encode_mask_reference(h):
+    """numpy model of mlp_fwd's mask store: h [rows, 256] -> uint32 words [rows, 8].  Per word, the sixteen fp16 pairs
+    (2k, 2k+1) are shifted in from the left, one per step: each step shifts the word left by one and adds
+    (h[2k] != 0) + ((h[2k+1] != 0) << 16)."""
+    nz = (np.asarray(h) != 0)
+    rows = nz.shape[0]
+    out = np.zeros((rows, 8), np.uint32)
+    for c in range(8):
+        m = np.zeros(rows, np.uint32)
+        for k in range(16):
+            pair = nz[:, 32 * c + 2 * k].astype(np.uint32) + (nz[:, 32 * c + 2 * k + 1].astype(np.uint32) << 16)
+            m = (m << np.uint32(1)) + pair
+        out[:, c] = m
+    return out
