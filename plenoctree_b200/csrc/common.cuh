@@ -129,6 +129,31 @@ __device__ __forceinline__ void bulk_wait_read_all() {
 __device__ __forceinline__ void bulk_wait_all() {
   asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
+// wait until every committed bulk store except the most recent group has completed (its global writes performed)
+__device__ __forceinline__ void bulk_wait_all_but_last() {
+  asm volatile("cp.async.bulk.wait_group 1;" ::: "memory");
+}
+
+// ----------------------------------------------------------------------------------
+// Cross-CTA hand-over of bulk-copied global data (mlp_bwd -> mlp_wgrad progress counters)
+// ----------------------------------------------------------------------------------
+// async-proxy global accesses <-> generic-proxy accesses of the same thread
+__device__ __forceinline__ void fence_proxy_async_global() {
+  asm volatile("fence.proxy.async.global;" ::: "memory");
+}
+__device__ __forceinline__ void red_add_release_gpu(uint32_t* p, uint32_t v) {
+  asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
+  uint32_t v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+// programmatic dependent launch: the grid launched after this one with programmatic stream serialization may start
+// once every CTA of this grid has executed this (or exited)
+__device__ __forceinline__ void griddep_launch_dependents() {
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+}
 
 // ----------------------------------------------------------------------------------
 // Named barriers (sub-CTA sync)

@@ -104,8 +104,10 @@ struct BwdParams {
   const uint32_t* mask;     // [8][Mpad][8] from mlp_fwd
   uint8_t* save_dz;         // [ntile][8][64 KB]
   uint8_t* save_do;         // [ntile][32 KB]
+  uint32_t* progress;       // [ntile], zeroed: stages of the tile whose stores have completed (wgrad_body.cuh)
 };
-cudaError_t launch_mlp_bwd(const BwdParams& p, int num_sms, cudaStream_t stream);
+// grid = min(tiles, num_ctas) persistent CTAs
+cudaError_t launch_mlp_bwd(const BwdParams& p, int num_ctas, cudaStream_t stream);
 
 // ---- mlp_wgrad.cu ---------------------------------------------------------------------------
 constexpr int WG_PARTIAL_FLOATS = 65536 + 256;
@@ -119,11 +121,13 @@ struct WgradParams {
   long long seg_tiles;
   int NH;
   float* partials;          // [num_ctas][WG_PARTIAL_FLOATS]
+  const uint32_t* progress; // [seg_tiles], advanced by the mlp_bwd launch that writes this segment's dZ / dO
   short cta_role[WG_MAX_CTAS], cta_index[WG_MAX_CTAS], cta_count[WG_MAX_CTAS];
 };
 // role -> [first CTA, count]; fills the per-CTA tables of `p`; returns number of CTAs to launch
 int wgrad_assign_roles(WgradParams& p, int num_sms, int role_start[WG_NUM_ROLES],
                        int role_count[WG_NUM_ROLES]);
+// launched with programmatic stream serialization right behind the mlp_bwd launch it consumes (wgrad_body.cuh)
 cudaError_t launch_mlp_wgrad(const WgradParams& p, int num_ctas, cudaStream_t stream);
 
 // ---- optim.cu -------------------------------------------------------------------------------

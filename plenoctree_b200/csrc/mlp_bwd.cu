@@ -13,6 +13,8 @@
 // m64n256, accumulator in registers), warp 8 = weight producer (warps 9-11 only hand their registers back).  A warpgroup writes its dZ rows into the shared
 // tile it reads as the next GEMM's A operand, and one thread hands those rows to the bulk-copy engine
 // (cp.async.bulk shared -> global), so the 64 KB per tile and GEMM leave the SM without occupying the warps.
+// mlp_wgrad runs alongside on the remaining SMs and reads each stored stage back from L2 once the per-tile progress
+// counter says it is complete (wgrad_body.cuh).
 #include "common.cuh"
 #include "kernels.h"
 
@@ -47,6 +49,8 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
   const int hs = (NH + 31) / 32;            // K slots of the heads dgrad
   const int do_chunks = (NH + 63) / 64;     // 64-wide chunks of the dO tile image
 
+  // the mlp_wgrad launch behind this one may take the SMs this grid leaves free (wgrad_body.cuh)
+  griddep_launch_dependents();
   if (threadIdx.x == 0) {
     for (int i = 0; i < BWD_WSLOTS; ++i) {
       mbar_init(smem_u32(&bars.full[i]), 1);
@@ -94,6 +98,16 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
   const bool issuer = t == 0;
   uint32_t slot = 0, phase = 0;
   float acc[128];
+  // Progress of this warpgroup's stores (wgrad_body.cuh reads it): warpgroup 0 counts in the low, warpgroup 1 in the
+  // high 16 bits of the tile's counter, one per stage (dO, dZ_7 .. dZ_0) whose bulk stores have completed.  A stage
+  // is published when the next one has been committed (wait_group 1), so the issuer does not wait on the store it
+  // just issued.
+  const uint32_t progress_inc = wg == 0 ? 1u : 0x10000u;
+  int pending = -1;                 // tile of the most recent committed, not yet published store group
+  auto publish = [&]() {            // pending's group has completed: its writes are visible to this thread
+    fence_proxy_async_global();
+    red_add_release_gpu(p.progress + pending, progress_inc);
+  };
 
   // before rewriting the warpgroup's rows: the bulk store of the previous image has read them
   auto rows_free = [&]() {
@@ -101,7 +115,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
     warpgroup_sync(wg);
   };
   // rows written: visible to the async proxy (next GEMM, bulk store); store `nchunks` 64-column chunks of them
-  auto hand_over = [&](uint8_t* dst_tile, int nchunks) {
+  auto hand_over = [&](uint8_t* dst_tile, int nchunks, int tile) {
     fence_proxy_async_smem();
     warpgroup_sync(wg);
     if (issuer) {
@@ -109,6 +123,11 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
         bulk_s2g(dst_tile + size_t(c) * A_CHUNK_BYTES + rows_off, sbase + SB_A + c * A_CHUNK_BYTES + rows_off,
                  64u * 128u);
       bulk_commit();
+      if (pending >= 0) {
+        bulk_wait_all_but_last();
+        publish();
+      }
+      pending = tile;
     }
   };
 
@@ -155,7 +174,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
           *reinterpret_cast<uint4*>(a_tile + a_tile_offset(r, 8 * u)) = make_uint4(w[0], w[1], w[2], w[3]);
         }
       }
-      hand_over(p.save_do + size_t(it) * (2 * A_CHUNK_BYTES), do_chunks);
+      hand_over(p.save_do + size_t(it) * (2 * A_CHUNK_BYTES), do_chunks, int(it));
     }
     // ---- GEMM g (heads, then Dense_7 .. Dense_1) -> dH_l -> dZ_l, l = 7 .. 0 ----
     for (int l = NUM_TRUNK - 1; l >= 0; --l) {
@@ -203,16 +222,19 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
           *reinterpret_cast<uint32_t*>(a_tile + a_tile_offset(64 * wg + fr + 8 * h, 8 * j + fc)) = w;
         }
       }
-      hand_over(p.save_dz + (size_t(it) * NUM_TRUNK + l) * A_TILE_BYTES, 4);
+      hand_over(p.save_dz + (size_t(it) * NUM_TRUNK + l) * A_TILE_BYTES, 4, int(it));
     }
   }
-  if (issuer) bulk_wait_all();
+  if (issuer) {
+    bulk_wait_all();
+    if (pending >= 0) publish();
+  }
 }
 
-cudaError_t launch_mlp_bwd(const BwdParams& p, int num_sms, cudaStream_t stream) {
+cudaError_t launch_mlp_bwd(const BwdParams& p, int num_ctas, cudaStream_t stream) {
   if (p.M <= 0) return cudaSuccess;
   const long long tiles = padded_rows(p.M) / TILE_M;
-  const int grid = int(tiles < num_sms ? tiles : num_sms);
+  const int grid = int(tiles < num_ctas ? tiles : num_ctas);
   cudaError_t e = cudaFuncSetAttribute(mlp_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SB_TOTAL);
   if (e != cudaSuccess) return e;
   mlp_bwd_kernel<<<grid, BWD_THREADS, SB_TOTAL, stream>>>(p);

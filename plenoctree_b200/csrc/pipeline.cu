@@ -34,6 +34,8 @@ struct Level {
 struct Workspace {
   Level lv[2];        // coarse, fine; in training the LAST level also carries the sparsity points behind its rays
   float* partials[2]; // wgrad partials of the two MLPs' launches
+  uint32_t* progress; // per tile of level 0, then of level 1: mlp_bwd -> mlp_wgrad progress counters (wgrad_body.cuh)
+  size_t progress_bytes;
   size_t total;
 };
 
@@ -41,6 +43,12 @@ size_t up(size_t x) { return (x + 1023) / 1024 * 1024; }
 
 // every per-tile array is padded to a multiple of four 128-row tiles (common.cuh: padded_rows)
 long long tiles_for(long long M) { return padded_rows(M) / TILE_M; }
+
+// SMs (out of an H100 SXM's 132) that run mlp_bwd during the backward; mlp_wgrad runs on the others.  Step time of
+// bench.py on an H100 80 GB HBM3 at a 400 W power limit with dgrad on 66 / 72 / 78 SMs: 10.2 / 10.4 / 13.4 ms (parent
+// without the concurrent backward: 10.7 ms).  A wgrad side that cannot keep up with dgrad misses L2 and runs a tail
+// alone; wgrad_assign_roles' even role counts make neighbouring splits differ a lot (DESIGN.md section 6).
+constexpr int DGRAD_SMS_OF_132 = 66;
 
 // deterministic carve of the caller-provided workspace
 Workspace carve(const pob_render_config& c, int training, uint8_t* base) {
@@ -78,6 +86,8 @@ Workspace carve(const pob_render_config& c, int training, uint8_t* base) {
   }
   if (training) {
     for (int i = 0; i < 2; ++i) w.partials[i] = (float*)take(sizeof(float) * WG_MAX_CTAS * WG_PARTIAL_FLOATS);
+    w.progress_bytes = sizeof(uint32_t) * size_t(w.lv[0].tiles + w.lv[1].tiles);
+    w.progress = (uint32_t*)take(w.progress_bytes);
   }
   w.total = off;
   return w;
@@ -235,6 +245,7 @@ int pob_loss_and_grad(const pob_render_config* cfg, const pob_train_hparams* hp,
   const int P = flat_layout(K).total;
   Workspace w = carve(*cfg, 1, (uint8_t*)workspace_dev);
   POB_CUDA(where, cudaMemsetAsync(stats_dev, 0, 8 * sizeof(float), st));
+  POB_CUDA(where, cudaMemsetAsync(w.progress, 0, w.progress_bytes, st));
   // The sparsity points (train.py:77-83: eval_points_raw of the fine MLP on uniform points) ride behind the ray
   // samples of the last level: same MLP, same launches, rows [n_rays * N, n_rays * N + sp_n) of its arrays.
   const long long sp_n = sparsity ? cfg->sparsity_npoints : 0;
@@ -262,6 +273,9 @@ int pob_loss_and_grad(const pob_render_config* cfg, const pob_train_hparams* hp,
   // MLP_0 (coarse level only) is finished first: its branch of the graph is independent of MLP_1's
   // (stop_gradient, model_utils.py:286), so the caller can all-reduce the MLP_0 bucket of the gradient
   // (mlp0_done_event) while the 3x larger MLP_1 backward is still running.
+  // dgrad runs on `dgrad_ctas` SMs and wgrad alongside it on the rest, reading each dZ tile from L2 shortly after it
+  // was stored (wgrad_body.cuh).
+  const int dgrad_ctas = sms * DGRAD_SMS_OF_132 / 132;
   const int NH = heads_width(K);
   for (int mlp = 0; mlp < (Nf > 0 ? 2 : 1); ++mlp) {
     Level& L = mlp == 0 ? C : F;
@@ -283,15 +297,17 @@ int pob_loss_and_grad(const pob_render_config* cfg, const pob_train_hparams* hp,
     b.mask = L.mask;
     b.save_dz = L.DZ;
     b.save_do = L.DO;
-    { pob_count_launch(); PobPhaseTimer _t(POB_PH_BWD, st); POB_CUDA(where, launch_mlp_bwd(b, sms, st)); }
+    b.progress = w.progress + (mlp == 0 ? 0 : C.tiles);
+    { pob_count_launch(); PobPhaseTimer _t(POB_PH_BWD, st); POB_CUDA(where, launch_mlp_bwd(b, dgrad_ctas, st)); }
     WgradParams g;
     memset(&g, 0, sizeof(g));
     g.seg = WgradSegment{L.H, L.DZ, L.E, L.DO};
     g.seg_tiles = tiles_for(Mm);
     g.NH = NH;
     g.partials = w.partials[mlp];
+    g.progress = b.progress;
     int rs[WG_NUM_ROLES], rc[WG_NUM_ROLES];
-    const int nctas = wgrad_assign_roles(g, sms, rs, rc);
+    const int nctas = wgrad_assign_roles(g, sms - dgrad_ctas, rs, rc);
     { pob_count_launch(); PobPhaseTimer _t(POB_PH_WGRAD, st); POB_CUDA(where, launch_mlp_wgrad(g, nctas, st)); }
     { pob_count_launch(); PobPhaseTimer _t(POB_PH_OPTIM, st); POB_CUDA(where, launch_reduce_grads(w.partials[mlp], rs, rc, K, 1.0f / hp->loss_scale,
                                         grad_flat_dev + size_t(mlp) * P, st)); }

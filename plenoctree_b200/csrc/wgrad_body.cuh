@@ -17,6 +17,26 @@
 //        9    = heads (Dense_8 | Dense_9)       A = h_7 (256 in)    B = dO       (NH)  [transposed result]
 // Bias gradients are column sums of the A (or, for the heads, B) tile, summed by the consumer warps from the staged
 // shared-memory tiles while their MMAs run.
+//
+// Concurrency with mlp_bwd.  The launch runs on the SMs that the mlp_bwd launch of the same level leaves free, right
+// behind it (programmatic stream serialization), and reads each dZ / dO tile a few microseconds after it was stored,
+// from L2.  Per tile, progress[tile] counts the stages (dO = 0, dZ_7 = 1 .. dZ_0 = 8) whose bulk stores have
+// completed: mlp_bwd's warpgroup 0 in the low and warpgroup 1 in the high 16 bits (each warpgroup stores its 64
+// rows).  Before the loads of a tile, the loader waits (ld.acquire, nanosleep back-off) until both halves exceed the
+// stage it needs, then orders its bulk loads behind that with fence.proxy.async; the writer side is wait_group
+// (completion, not .read) -> fence.proxy.async -> red.release.gpu.  h and posenc come from the earlier mlp_fwd launch.
+// The two halves are counted apart because the warpgroups may be two stages apart (the weight ring lets one run a
+// whole layer ahead), so a sum of both could reach 2 (stage + 1) with one half still missing.
+// This cannot deadlock:
+//  - this grid starts only once every mlp_bwd CTA has executed griddepcontrol.launch_dependents, so all of them are
+//    resident, and none of them ever waits on this grid;
+//  - every counter waited on belongs to a tile < seg_tiles, and mlp_bwd completes all nine stages of every such tile,
+//    padded tiles included;
+//  - if the programmatic launch is not honoured (timing events between the launches, graph capture on an older
+//    driver), this grid starts after mlp_bwd has finished and every counter is already full: the result is the same,
+//    only serial.
+// Each CTA still sums its static share of the tiles in increasing tile order: the gradient is bit-identical from run
+// to run.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -25,17 +45,18 @@ namespace pob {
 namespace {
 
 constexpr int WG_THREADS = 288;       // warps 0-7: two consumer warpgroups, warp 8: loads
-constexpr int WG_STAGES = 4;
 constexpr int WG_SUB = 64;            // samples per stage
 constexpr uint32_t WG_PIECE = WG_SUB * 128;        // 64 samples x 128 B: one 64-feature chunk (SW128) / half a T group pair
 constexpr uint32_t WG_A_BYTES = 2 * WG_PIECE;      // the CTA's 128 A features
 constexpr uint32_t WG_B_MAX = 4 * WG_PIECE;        // up to 256 B features
-constexpr uint32_t WG_STAGE_BYTES = WG_A_BYTES + WG_B_MAX;   // 48 KB
-constexpr uint32_t WG_SMEM = WG_STAGES * WG_STAGE_BYTES;
+constexpr uint32_t WG_SMEM = 4 * (WG_A_BYTES + WG_B_MAX);   // four 48 KB stages of the 256-wide roles
+// A stage holds A and the role's B features only, so the narrow roles (Dense_0, Dense_5's posenc rows, the heads:
+// 24-32 KB per stage) keep six to eight stages in flight.  Their time per stage is load latency rather than MMAs.
+constexpr int WG_MAX_STAGES = 8;
 
 struct WgBarriers {
-  uint64_t full[WG_STAGES];
-  uint64_t empty[WG_STAGES];
+  uint64_t full[WG_MAX_STAGES];
+  uint64_t empty[WG_MAX_STAGES];
 };
 
 struct RoleInfo {
@@ -77,8 +98,9 @@ constexpr uint64_t T_DESC = make_sdesc_hi(128, 512, LAYOUT_NONE);
 // Consumer warpgroup `wg`: accumulates D[64 A features x NN] over the CTA's stages, then writes its rows of the
 // partial.  NN = MMA width (256, 64, or 80 for the heads, whose columns >= NH are never written back).
 template <int NN>
-__device__ __forceinline__ void wgrad_consume(const RoleInfo& R, uint8_t* smem, WgBarriers& bars, long long n_items,
-                                              int mh, float* out_w, float* out_b) {
+__device__ __forceinline__ void wgrad_consume(const RoleInfo& R, uint8_t* smem, WgBarriers& bars, int nst,
+                                              uint32_t stage_bytes, long long n_items, int mh, float* out_w,
+                                              float* out_b) {
   const uint32_t warp = warp_id(), lane = lane_id();
   const int wg = int(warp >> 2);
   const int t = int(threadIdx.x & 127);
@@ -103,7 +125,7 @@ __device__ __forceinline__ void wgrad_consume(const RoleInfo& R, uint8_t* smem, 
   for (long long i = 0; i < n_items; ++i) {
     for (int sub = 0; sub < 2; ++sub) {
       mbar_wait(smem_u32(&bars.full[st]), phase);
-      const uint32_t a0 = sbase + st * WG_STAGE_BYTES;
+      const uint32_t a0 = sbase + st * stage_bytes;
       const uint32_t b0 = a0 + WG_A_BYTES;
 #pragma unroll
       for (int ks = 0; ks < WG_SUB / 16; ++ks) {
@@ -118,7 +140,7 @@ __device__ __forceinline__ void wgrad_consume(const RoleInfo& R, uint8_t* smem, 
       }
       wgmma_commit();
       if (a_bias || b_bias) {
-        const uint8_t* base = smem + st * WG_STAGE_BYTES + bias_src;
+        const uint8_t* base = smem + st * stage_bytes + bias_src;
 #pragma unroll 4
         for (int r = s_lo; r < s_lo + s_n; ++r) {
           const float2 v = unpack_f16x2(
@@ -129,7 +151,7 @@ __device__ __forceinline__ void wgrad_consume(const RoleInfo& R, uint8_t* smem, 
       }
       wgmma_wait<0>();
       if (lane == 0) mbar_arrive(smem_u32(&bars.empty[st]));
-      if (++st == WG_STAGES) {
+      if (++st == uint32_t(nst)) {
         st = 0;
         phase ^= 1;
       }
@@ -182,13 +204,18 @@ __device__ __forceinline__ void wgrad_body(const WgradParams& p, uint8_t* smem, 
   float* const out_b = out_w + 65536;
   const RoleInfo R = role_info(role, p.NH);
   const uint32_t b_bytes = R.b_t ? 4 * WG_PIECE : uint32_t(R.b_chunks) * WG_PIECE;
+  // room for every B feature the MMA reads: the heads MMA is 80 wide whenever NH != 64, so NH <= 64 reads a second
+  // (unused) chunk.  A multiple of 8 KB, so every stage stays 1 KB aligned.
+  const uint32_t b_room = R.N == 256 || R.N == 64 ? b_bytes : 2 * WG_PIECE;
+  const uint32_t stage_bytes = WG_A_BYTES + b_room;
+  const int nst = min(WG_MAX_STAGES, int(WG_SMEM / stage_bytes));
 
   // work list: tiles t = sidx + i*scnt
   const long long total_tiles = p.seg_tiles;
   const long long n_items = (total_tiles > sidx) ? (total_tiles - sidx + scnt - 1) / scnt : 0;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < WG_STAGES; ++i) {
+    for (int i = 0; i < nst; ++i) {
       mbar_init(smem_u32(&bars.full[i]), 1);
       mbar_init(smem_u32(&bars.empty[i]), 8);   // one arrival per consumer warp
     }
@@ -200,6 +227,8 @@ __device__ __forceinline__ void wgrad_body(const WgradParams& p, uint8_t* smem, 
     // ================================ loader ====================================
     // whole-warp control flow, one elected lane issues
     const WgradSegment& sg = p.seg;
+    // every role reads one operand mlp_bwd stores: dZ_l (stage 8 - l) or, for the heads, dO (stage 0)
+    const uint32_t want = R.a_kind == 0 ? uint32_t(NUM_TRUNK + 1 - R.a_layer) : 1u;
     uint32_t st = 0, phase = 0;
     for (long long i = 0; i < n_items; ++i) {
       const long long lt = sidx + i * scnt;
@@ -210,9 +239,17 @@ __device__ __forceinline__ void wgrad_body(const WgradParams& p, uint8_t* smem, 
       for (int sub = 0; sub < 2; ++sub) {
         mbar_wait(smem_u32(&bars.empty[st]), phase ^ 1);
         if (elect_one()) {
+          // the thread that issues the loads is the one that acquires (once the tile is complete, this is one L2 hit)
+          for (uint32_t ns = 32;;) {
+            const uint32_t v = ld_acquire_gpu(p.progress + lt);
+            if ((v & 0xFFFFu) >= want && (v >> 16) >= want) break;
+            __nanosleep(ns);
+            if (ns < 512) ns *= 2;
+          }
+          fence_proxy_async_global();
           const uint32_t bar = smem_u32(&bars.full[st]);
           mbar_arrive_expect_tx(bar, WG_A_BYTES + b_bytes);
-          const uint32_t dst = sbase + st * WG_STAGE_BYTES;
+          const uint32_t dst = sbase + st * stage_bytes;
 #pragma unroll
           for (int c = 0; c < 2; ++c) {
             if (R.a_t)   // T image: this half's 128 features = 8 KB of each 32-sample group
@@ -228,7 +265,7 @@ __device__ __forceinline__ void wgrad_body(const WgradParams& p, uint8_t* smem, 
           }
         }
         __syncwarp();
-        if (++st == WG_STAGES) {
+        if (++st == uint32_t(nst)) {
           st = 0;
           phase ^= 1;
         }
@@ -236,9 +273,9 @@ __device__ __forceinline__ void wgrad_body(const WgradParams& p, uint8_t* smem, 
     }
     return;
   }
-  if (R.N == 256) wgrad_consume<256>(R, smem, bars, n_items, mh, out_w, out_b);
-  else if (R.N == 64) wgrad_consume<64>(R, smem, bars, n_items, mh, out_w, out_b);
-  else wgrad_consume<MAX_NH>(R, smem, bars, n_items, mh, out_w, out_b);
+  if (R.N == 256) wgrad_consume<256>(R, smem, bars, nst, stage_bytes, n_items, mh, out_w, out_b);
+  else if (R.N == 64) wgrad_consume<64>(R, smem, bars, nst, stage_bytes, n_items, mh, out_w, out_b);
+  else wgrad_consume<MAX_NH>(R, smem, bars, nst, stage_bytes, n_items, mh, out_w, out_b);
 }
 
 }  // namespace pob

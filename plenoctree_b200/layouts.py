@@ -249,9 +249,9 @@ def train_workspace_views(cfg, n_rays, sparsity_on):
     Returns dict(total=bytes, partials=[offsets], levels=[...]) with one entry per level (coarse, then fine when
     num_fine_samples > 0).  Each level holds (offset, shape) pairs for z, rgbs, weights, comp, disp, acc (float32;
     rgbs and G as [rows, 4]), G, H [tiles, 8, 64 KB], E [tiles, 16 KB], DZ [tiles, 8, 64 KB], DO [tiles, 32 KB]
-    (uint8 tile images) and mask [8, rows, 8] (uint32 words), sized for this call, plus the call's row counts:
-    N samples per ray, M_rays, M (with the sparsity rows, which ride behind the rays of the last level), rows
-    (= padded_rows(M)) and tiles.  Buffers are carved for cfg.max_rays; the mask's per-layer stride is the call's
+    (uint8 tile images), mask [8, rows, 8] and progress [tiles] (uint32 words), sized for this call, plus the call's
+    row counts: N samples per ray, M_rays, M (with the sparsity rows, which ride behind the rays of the last level),
+    rows (= padded_rows(M)) and tiles.  Buffers are carved for cfg.max_rays; the mask's per-layer stride is the call's
     padded row count."""
     R = int(cfg.max_rays)
     nc, nf, nsp = int(cfg.num_coarse_samples), int(cfg.num_fine_samples), int(cfg.sparsity_npoints)
@@ -259,6 +259,7 @@ def train_workspace_views(cfg, n_rays, sparsity_on):
     last = 1 if nf > 0 else 0
     off = 0
     levels = []
+    caps = [0, 0]      # tiles carved per level
 
     def take(nbytes):
         nonlocal off
@@ -269,7 +270,7 @@ def train_workspace_views(cfg, n_rays, sparsity_on):
     for lv in range(2):
         Mr_cap = R * Ns[lv]
         M_cap = Mr_cap + (nsp if lv == last else 0)
-        tiles_cap = padded_rows(M_cap) // TILE_M
+        tiles_cap = caps[lv] = padded_rows(M_cap) // TILE_M
         if Mr_cap == 0:
             continue
         N = Ns[lv]
@@ -292,11 +293,15 @@ def train_workspace_views(cfg, n_rays, sparsity_on):
         v["mask"] = (take(NUM_TRUNK * tiles_cap * TILE_M * 8 * 4), (NUM_TRUNK, rows, 8))
         levels.append(v)
     partials = [take(4 * WG_MAX_CTAS * WG_PARTIAL_FLOATS) for _ in range(2)]
+    progress = take(4 * sum(caps))   # mlp_bwd -> mlp_wgrad progress counters, level 0's tiles then level 1's
+    for v, first in zip(levels, (0, caps[0])):
+        v["progress"] = (progress + 4 * first, (v["tiles"],))
     return dict(total=off, levels=levels, partials=partials)
 
 
 _VIEW_DTYPES = dict(z="float32", rgbs="float32", weights="float32", comp="float32", disp="float32", acc="float32",
-                    G="float32", H="uint8", E="uint8", DZ="uint8", DO="uint8", mask="int32")
+                    G="float32", H="uint8", E="uint8", DZ="uint8", DO="uint8", mask="int32",
+                    progress="int32")
 
 
 def workspace_view(ws, level, name):
