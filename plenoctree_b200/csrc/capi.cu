@@ -81,7 +81,7 @@ int sm_count() {
 
 // packed blob layout of one MLP
 struct BlobLayout {
-  size_t w_hi, w_lo, wt_hi, bias, total;
+  size_t w_hi, w_lo, wt_hi, total;
 };
 BlobLayout blob_layout(int K) {
   const int NH = pob::heads_width(K);
@@ -90,8 +90,7 @@ BlobLayout blob_layout(int K) {
   b.w_hi = 0;
   b.w_lo = up(b.w_hi + pob::fwd_image_bytes(NH));
   b.wt_hi = up(b.w_lo + pob::fwd_image_bytes(NH));
-  b.bias = up(b.wt_hi + pob::bwd_image_bytes(NH));
-  b.total = up(b.bias + (8 * 256 + pob::MAX_NH) * sizeof(float));
+  b.total = up(b.wt_hi + pob::bwd_image_bytes(NH));
   return b;
 }
 pob::MlpPacked packed_view(const void* blob, int K) {
@@ -101,7 +100,6 @@ pob::MlpPacked packed_view(const void* blob, int K) {
   w.w_hi = p + b.w_hi;
   w.w_lo = p + b.w_lo;
   w.wt_hi = p + b.wt_hi;
-  w.bias = reinterpret_cast<const float*>(p + b.bias);
   return w;
 }
 
@@ -178,8 +176,7 @@ int pob_pack_weights(const float* flat_dev, int sh_deg, void* packed_dev, void* 
   pob_count_launch();
   PobPhaseTimer _t(POB_PH_OPTIM, (cudaStream_t)stream);
   POB_CUDA("pob_pack_weights",
-           pob::launch_pack_weights(flat_dev, K, p + b.w_hi, p + b.w_lo, p + b.wt_hi,
-                                    reinterpret_cast<float*>(p + b.bias), (cudaStream_t)stream));
+           pob::launch_pack_weights(flat_dev, K, p + b.w_hi, p + b.w_lo, p + b.wt_hi, (cudaStream_t)stream));
   return 0;
 }
 
@@ -199,8 +196,7 @@ int pob_eval_points_raw(const void* packed_dev, int sh_deg, const float* points_
   pob_count_launch();
   PobPhaseTimer _t(POB_PH_FWD, (cudaStream_t)stream);
   POB_CUDA("pob_eval_points_raw",
-           pob::launch_mlp_fwd(p, precision, precision == POB_PREC_FP16X3, sm_count(),
-                               (cudaStream_t)stream));
+           pob::launch_mlp_fwd(p, precision, sm_count(), (cudaStream_t)stream));
   return 0;
 }
 
@@ -223,8 +219,7 @@ int pob_eval_points(const void* packed_dev, int sh_deg, const float* points_dev,
   pob_count_launch();
   PobPhaseTimer _t(POB_PH_FWD, (cudaStream_t)stream);
   POB_CUDA("pob_eval_points",
-           pob::launch_mlp_fwd(p, precision, precision == POB_PREC_FP16X3, sm_count(),
-                               (cudaStream_t)stream));
+           pob::launch_mlp_fwd(p, precision, sm_count(), (cudaStream_t)stream));
   return 0;
 }
 
@@ -246,7 +241,7 @@ int pob_eval_cells_mean(const void* packed_dev, int sh_deg, const float* points_
   pob_count_launch();
   PobPhaseTimer _t(POB_PH_FWD, (cudaStream_t)stream);
   POB_CUDA("pob_eval_cells_mean",
-           pob::launch_mlp_fwd(p, precision, precision == POB_PREC_FP16X3, sm_count(), (cudaStream_t)stream));
+           pob::launch_mlp_fwd(p, precision, sm_count(), (cudaStream_t)stream));
   return 0;
 }
 
@@ -279,8 +274,7 @@ int pob_eval_grid(const void* packed_dev, int sh_deg, int reso, int x0, int nx, 
   pob_count_launch();
   PobPhaseTimer _t(POB_PH_FWD, (cudaStream_t)stream);
   POB_CUDA("pob_eval_grid",
-           pob::launch_mlp_fwd(p, precision, precision == POB_PREC_FP16X3, sm_count(),
-                               (cudaStream_t)stream));
+           pob::launch_mlp_fwd(p, precision, sm_count(), (cudaStream_t)stream));
   return 0;
 }
 

@@ -43,6 +43,20 @@ __host__ __device__ constexpr int fwd_slots_of_layer(int l) {
 }
 constexpr int FWD_TRUNK_SLOTS = 2 + 9 * 4 + 10 + 9 * 2;       // 66
 constexpr int FWD_HEAD_SLOTS = 9;
+// K slots of the dgrad image: the heads' ceil(NH/32), then Dense_7 .. Dense_1 with 8 each
+__host__ __device__ constexpr int bwd_head_slots(int NH) { return (NH + 31) / 32; }
+__host__ __device__ constexpr int bwd_slots(int NH) { return bwd_head_slots(NH) + 7 * 8; }
+
+// Heads column order: packed column 0 is sigma (Dense_8), packed column 1 + 3k + c is SH coefficient k of colour
+// channel c, which is Dense_9 output c*K + k in the reference's channel-major order.
+__host__ __device__ constexpr int heads_column(int k, int c) { return 1 + 3 * k + c; }
+// Dense_9 output o (of 3K) -> packed column
+__host__ __device__ constexpr int heads_column_of_output(int o, int K) { return heads_column(o % K, o / K); }
+// packed column n >= 1 -> (k, c)
+__host__ __device__ constexpr void heads_coeff(int n, int& k, int& c) {
+  k = (n - 1) / 3;
+  c = (n - 1) % 3;
+}
 
 // ----------------------------------------------------------------------------------
 // Small helpers
@@ -94,6 +108,52 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {
   }
 }
+
+// ----------------------------------------------------------------------------------
+// Stage ring of the tensor-core kernels: one producer warp bulk-copies operands into shared-memory stages, the two
+// consumer warpgroups read every stage with wgmma.  full[s] completes once stage s's bytes have landed, empty[s]
+// once every consumer warp has released it.  The depth (<= MAX_DEPTH) is a compile-time or a run-time value.
+// ----------------------------------------------------------------------------------
+constexpr uint32_t RING_CONSUMER_WARPS = 8;   // two warpgroups; each warp releases a stage once
+
+struct RingPos {
+  uint32_t stage = 0, phase = 0;
+  __device__ __forceinline__ void advance(uint32_t depth) {
+    if (++stage == depth) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+};
+
+template <int MAX_DEPTH>
+struct Ring {
+  uint64_t full[MAX_DEPTH];
+  uint64_t empty[MAX_DEPTH];
+
+  // one thread; a __syncthreads() after it publishes the barriers
+  __device__ __forceinline__ void init(int depth) {
+    for (int i = 0; i < depth; ++i) {
+      mbar_init(smem_u32(&full[i]), 1);
+      mbar_init(smem_u32(&empty[i]), RING_CONSUMER_WARPS);
+    }
+    fence_mbar_init();
+  }
+  // producer warp: wait until the stage is free.  One elected lane then calls arm() and issues the stage's copies.
+  __device__ __forceinline__ void acquire(RingPos pos) { mbar_wait(smem_u32(&empty[pos.stage]), pos.phase ^ 1); }
+  // the stage's full barrier, expecting `bytes` of bulk copies (to be completed on it)
+  __device__ __forceinline__ uint32_t arm(RingPos pos, uint32_t bytes) {
+    const uint32_t bar = smem_u32(&full[pos.stage]);
+    mbar_arrive_expect_tx(bar, bytes);
+    return bar;
+  }
+  // consumer: wait until the stage's bytes have landed
+  __device__ __forceinline__ void wait(RingPos pos) { mbar_wait(smem_u32(&full[pos.stage]), pos.phase); }
+  // consumer warp, once its MMAs reading the stage have completed
+  __device__ __forceinline__ void release(uint32_t stage) {
+    if (lane_id() == 0) mbar_arrive(smem_u32(&empty[stage]));
+  }
+};
 
 // ----------------------------------------------------------------------------------
 // Proxy fence

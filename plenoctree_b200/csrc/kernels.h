@@ -3,14 +3,16 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "common.cuh"
+
 namespace pob {
 
 // ---- packed weights of one MLP (device pointers; produced by launch_pack_weights) ----------
+// The biases ride inside the forward slots (common.cuh); the dgrad needs none.
 struct MlpPacked {
   const uint8_t* w_hi;    // forward slot images, fp16 "hi" part  (fwd_image_bytes(NH))
   const uint8_t* w_lo;    // forward slot images, fp16 residual   (same layout)
   const uint8_t* wt_hi;   // dgrad slot images (transposed weights), fp16
-  const float* bias;      // [8*256 + MAX_NH]: trunk biases then heads bias in packed order
 };
 
 enum SrcMode : int { SRC_POINTS = 0, SRC_RAYS = 1, SRC_GRID = 2 };
@@ -55,20 +57,19 @@ struct FwdParams {
 
 // padded heads width for K spherical-harmonic coefficients per channel
 inline int heads_width(int K) { return ((1 + 3 * K) + 15) / 16 * 16; }
-// bytes of one forward weight image (hi or lo)
-inline size_t fwd_image_bytes(int NH) { return size_t(66) * 16384 + size_t(9) * NH * 64; }
-// bytes of one dgrad weight image: heads (ceil(NH/32) slots) + layers 7..1 (8 slots each)
-inline size_t bwd_image_bytes(int NH) { return size_t((NH + 31) / 32 + 7 * 8) * 16384; }
+// bytes of one forward weight image (hi or lo): the trunk slots, then the heads slots of NH rows
+inline size_t fwd_image_bytes(int NH) { return size_t(FWD_TRUNK_SLOTS) * WSLOT_BYTES + size_t(FWD_HEAD_SLOTS) * NH * 64; }
+// bytes of one dgrad weight image
+inline size_t bwd_image_bytes(int NH) { return size_t(bwd_slots(NH)) * WSLOT_BYTES; }
 
-// precision: 1 = single fp16 pass (10-bit mantissa operands, fp32 accumulate),
-//            3 = error-compensated 3-pass split (hi*hi + lo*hi + hi*lo)
-cudaError_t launch_mlp_fwd(const FwdParams& p, int nsplit, bool precise_sin, int num_sms,
-                           cudaStream_t stream);
+// precision: 1 = single fp16 pass (10-bit mantissa operands, fp32 accumulate, reduced SFU sine),
+//            3 = error-compensated 3-pass split (hi*hi + lo*hi + hi*lo, libdevice sinf)
+cudaError_t launch_mlp_fwd(const FwdParams& p, int nsplit, int num_sms, cudaStream_t stream);
 
 // flat fp32 parameters of one MLP in reference order (Dense_0..Dense_9: kernel [in,out] then
 // bias) -> packed images.  `nparams` = param_count(K).
 cudaError_t launch_pack_weights(const float* flat, int K, uint8_t* w_hi, uint8_t* w_lo,
-                                uint8_t* wt_hi, float* bias, cudaStream_t stream);
+                                uint8_t* wt_hi, cudaStream_t stream);
 
 
 
@@ -113,6 +114,38 @@ cudaError_t launch_mlp_bwd(const BwdParams& p, int num_ctas, cudaStream_t stream
 constexpr int WG_PARTIAL_FLOATS = 65536 + 256;
 constexpr int WG_MAX_CTAS = 160;
 constexpr int WG_NUM_ROLES = 10;
+
+// Roles of the wgrad CTAs.  Role r computes D[A feature][B feature] = sum over samples of A^T B, with A and B read
+// from the tile images mlp_fwd and mlp_bwd saved, and the bias gradient as column sums of A or B.  Its partial holds
+// D row-major with `width` columns, then the bias sums (at WG_PARTIAL_FLOATS - 256).
+enum WgOperand : int { WG_DZ = 0, WG_H = 1, WG_E = 2, WG_DO = 3 };   // dZ_l, h_l, posenc, dO tile images
+enum WgBias : int { WG_BIAS_NONE = 0, WG_BIAS_A = 1, WG_BIAS_B = 2 };
+constexpr int WG_WIDTH_NH = 0;   // result width of the heads role: the padded heads width NH
+struct WgradRole {
+  int dense;            // reference Dense_i (the heads role: Dense_8 and Dense_9, in packed heads columns)
+  int in0;              // first input feature of Dense_i covered (Dense_5's posenc rows start at 256)
+  int a_op, a_layer;    // A operand: result rows
+  int b_op, b_layer;    // B operand: result columns
+  int width;            // 256, 64 or WG_WIDTH_NH
+  int bias;
+};
+__host__ __device__ constexpr WgradRole wgrad_role(int r) {
+  //     Dense_i    in0   A               B              width        bias
+  return r < 7 ? WgradRole{r + 1, 0,   WG_DZ, r + 1,  WG_H, r,      256,         WG_BIAS_A}      // Dense_1..7 (h4 rows of 5)
+       : r == 7 ? WgradRole{0,    0,   WG_DZ, 0,      WG_E, 0,      64,          WG_BIAS_A}      // Dense_0
+       : r == 8 ? WgradRole{5,    256, WG_DZ, 5,      WG_E, 0,      64,          WG_BIAS_NONE}   // Dense_5 posenc rows
+       :          WgradRole{8,    0,   WG_H,  7,      WG_DO, 0,     WG_WIDTH_NH, WG_BIAS_B};     // heads
+}
+// role holding input row `in` of Dense_`dense`
+__host__ __device__ constexpr int wgrad_role_of(int dense, int in) {
+  int role = 0;
+  for (int r = 0; r < WG_NUM_ROLES; ++r)
+    if (wgrad_role(r).dense == (dense < 8 ? dense : 8) && in >= wgrad_role(r).in0) role = r;   // the last such role
+  return role;
+}
+__host__ __device__ constexpr int wgrad_role_width(const WgradRole& R, int NH) {
+  return R.width == WG_WIDTH_NH ? NH : R.width;
+}
 struct WgradSegment {
   const uint8_t *h, *dz, *e, *d_o;
 };

@@ -10,7 +10,8 @@
 // No gradient w.r.t. the inputs is needed (layer 0 and the skip slice of layer 5 stop here).
 //
 // Warp roles (384 threads): warps 0-3 and 4-7 = two consumer warpgroups, each owning 64 rows of the tile (wgmma
-// m64n256, accumulator in registers), warp 8 = weight producer (warps 9-11 only hand their registers back).  A warpgroup writes its dZ rows into the shared
+// m64n256, accumulator in registers), warp 8 = weight producer (a ring of eight 16 KB stages, one K-slot of the
+// transposed weights each; warps 9-11 only hand their registers back).  A warpgroup writes its dZ rows into the shared
 // tile it reads as the next GEMM's A operand, and one thread hands those rows to the bulk-copy engine
 // (cp.async.bulk shared -> global), so the 64 KB per tile and GEMM leave the SM without occupying the warps.
 // mlp_wgrad runs alongside on the remaining SMs and reads each stored stage back from L2 once the per-tile progress
@@ -30,55 +31,39 @@ constexpr uint32_t SB_A = 0;
 constexpr uint32_t SB_W = SB_A + A_TILE_BYTES;
 constexpr uint32_t SB_TOTAL = SB_W + BWD_WSLOTS * WSLOT_BYTES;  // 64K + 128K = 192K
 
-struct BwdBarriers {
-  uint64_t full[BWD_WSLOTS];
-  uint64_t empty[BWD_WSLOTS];
-};
-
 }  // namespace
 
 __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_constant__ BwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ __align__(8) BwdBarriers bars;
+  __shared__ __align__(8) Ring<BWD_WSLOTS> ring;
 
   const long long mrows = padded_rows(p.M);        // rows of the mask / tile arrays
   const long long num_tiles = mrows / TILE_M;      // padded tiles get zero gradients, not garbage
   const uint32_t warp = warp_id(), lane = lane_id();
   const uint32_t sbase = smem_u32(smem);
   const int NH = p.NH;
-  const int hs = (NH + 31) / 32;            // K slots of the heads dgrad
   const int do_chunks = (NH + 63) / 64;     // 64-wide chunks of the dO tile image
 
   // the mlp_wgrad launch behind this one may take the SMs this grid leaves free (wgrad_body.cuh)
   griddep_launch_dependents();
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < BWD_WSLOTS; ++i) {
-      mbar_init(smem_u32(&bars.full[i]), 1);
-      mbar_init(smem_u32(&bars.empty[i]), 8);   // one arrival per consumer warp
-    }
-    fence_mbar_init();
-  }
+  if (threadIdx.x == 0) ring.init(BWD_WSLOTS);
   __syncthreads();
 
   if (warp >= BWD_PRODUCER_WARP) {
     // whole-warp control flow, one elected lane issues
     setmaxnreg_dec<40>();
     if (warp != BWD_PRODUCER_WARP) return;
-    uint32_t slot = 0, phase = 0;
-    const int nslots = hs + 7 * 8;
+    RingPos pos;
+    const int nslots = bwd_slots(NH);
     for (long long it = blockIdx.x; it < num_tiles; it += gridDim.x) {
       for (int j = 0; j < nslots; ++j) {
-        mbar_wait(smem_u32(&bars.empty[slot]), phase ^ 1);
+        ring.acquire(pos);
         if (elect_one()) {
-          mbar_arrive_expect_tx(smem_u32(&bars.full[slot]), WSLOT_BYTES);
-          bulk_g2s(sbase + SB_W + slot * WSLOT_BYTES, p.w.wt_hi + size_t(j) * WSLOT_BYTES, WSLOT_BYTES,
-                   smem_u32(&bars.full[slot]));
+          const uint32_t bar = ring.arm(pos, WSLOT_BYTES);
+          bulk_g2s(sbase + SB_W + pos.stage * WSLOT_BYTES, p.w.wt_hi + size_t(j) * WSLOT_BYTES, WSLOT_BYTES, bar);
         }
         __syncwarp();
-        if (++slot == BWD_WSLOTS) {
-          slot = 0;
-          phase ^= 1;
-        }
+        pos.advance(BWD_WSLOTS);
       }
     }
     return;
@@ -96,7 +81,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
   constexpr uint64_t A_DESC = make_sdesc_hi(16, 1024, LAYOUT_SW128);
   constexpr uint64_t W_DESC = make_sdesc_hi(16, 512, LAYOUT_SW64);
   const bool issuer = t == 0;
-  uint32_t slot = 0, phase = 0;
+  RingPos pos;
   float acc[128];
   // Progress of this warpgroup's stores (wgrad_body.cuh reads it): warpgroup 0 counts in the low, warpgroup 1 in the
   // high 16 bits of the tile's counter, one per stage (dO, dZ_7 .. dZ_0) whose bulk stores have completed.  A stage
@@ -164,8 +149,9 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
               float v = 0.f;
               if (n == 0) v = gq.w;
               else if (n < 1 + 3 * 25) {
-                const int k = (n - 1) / 3, c = (n - 1) % 3;
-                if (k < p.K) v = gc[c] * basis[k < 25 ? k : 24];
+                int k, c;
+                heads_coeff(n, k, c);
+                if (k < p.K) v = gc[c] * basis[k];   // n < 76: k < 25
               }
               f[e] = v;
             }
@@ -178,25 +164,22 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
     }
     // ---- GEMM g (heads, then Dense_7 .. Dense_1) -> dH_l -> dZ_l, l = 7 .. 0 ----
     for (int l = NUM_TRUNK - 1; l >= 0; --l) {
-      const int ns = (l == NUM_TRUNK - 1) ? hs : 8;
+      const int ns = (l == NUM_TRUNK - 1) ? bwd_head_slots(NH) : 8;
       uint32_t prev = 0;
       wgmma_fence();
       for (int j = 0; j < ns; ++j) {
         const uint32_t a = sbase + SB_A + uint32_t(j >> 1) * A_CHUNK_BYTES + rows_off + uint32_t(j & 1) * 64u;
-        const uint32_t b = sbase + SB_W + slot * WSLOT_BYTES;
-        mbar_wait(smem_u32(&bars.full[slot]), phase);
+        const uint32_t b = sbase + SB_W + pos.stage * WSLOT_BYTES;
+        ring.wait(pos);
         wgmma_m64n256<0, 0>(acc, sdesc(A_DESC, a), sdesc(W_DESC, b), j != 0);
         wgmma_m64n256<0, 0>(acc, sdesc(A_DESC, a + 32), sdesc(W_DESC, b + 32), 1u);
         wgmma_commit();
         if (j > 0) {
           wgmma_wait<1>();
-          if (lane == 0) mbar_arrive(smem_u32(&bars.empty[prev]));
+          ring.release(prev);
         }
-        prev = slot;
-        if (++slot == BWD_WSLOTS) {
-          slot = 0;
-          phase ^= 1;
-        }
+        prev = pos.stage;
+        pos.advance(BWD_WSLOTS);
       }
       // relu masks of h_l for the fragment rows (word c: column 32c+2k <-> bit 15-k, column 32c+2k+1 <-> bit 31-k),
       // loaded while the GEMM runs
@@ -209,7 +192,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
         mw[h][4] = m1.x; mw[h][5] = m1.y; mw[h][6] = m1.z; mw[h][7] = m1.w;
       }
       wgmma_wait<0>();
-      if (lane == 0) mbar_arrive(smem_u32(&bars.empty[prev]));
+      ring.release(prev);
       rows_free();
 #pragma unroll
       for (int j = 0; j < 32; ++j) {

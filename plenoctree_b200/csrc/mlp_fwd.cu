@@ -15,10 +15,11 @@
 //
 // Warp roles (384 threads): warps 0-3 and 4-7 = two consumer warpgroups, each owning 64 rows of the tile
 // (one m64n256 accumulator = 128 registers per thread, 232 registers after setmaxnreg), warp 8 = weight producer
-// (cp.async.bulk ring of 16 KB K-slots; warps 9-11 only hand their registers back).  Both warpgroups consume every streamed weight slot; a warpgroup reads and rewrites only its
-// own rows of the activation / posenc tiles, so the two synchronise through the weight ring alone and one's
-// epilogue runs under the other's MMAs.  NSPLIT = 3 evaluates with error-compensated fp16 operands
-// (x = hi + lo; lo*hi + hi*lo + hi*hi per K step), the residual parts in a second set of tiles / slots.
+// (cp.async.bulk ring, one 16 KB K-slot per stage; warps 9-11 only hand their registers back).  Both warpgroups
+// consume every stage; a warpgroup reads and rewrites only its own rows of the activation / posenc tiles, so the two
+// synchronise through the weight ring alone and one's epilogue runs under the other's MMAs.  NSPLIT = 3 evaluates
+// with error-compensated fp16 operands (x = hi + lo; lo*hi + hi*lo + hi*hi per K step), the residual parts in a
+// second set of tiles; a stage then holds the K-slot's hi and lo parts (32 KB).
 #include "common.cuh"
 #include "kernels.h"
 
@@ -32,10 +33,10 @@ constexpr int HEADS_N = 80;               // heads MMA width: MAX_NH (rows >= NH
 constexpr int STAGE_PITCH = HEADS_N + 1;  // heads staging: odd pitch -> conflict-free per-row scalar access
 
 // dynamic smem map: activation tile, posenc tile, weight ring.  The x3 mode also keeps the residual (lo) tiles and
-// runs a ring of four slots (two hi/lo pairs).  The training forward (fp16, SAVE) gives those 80 KB to the ring, nine
-// slots: a slot is handed back only once both warpgroups are done with it, so the ring depth bounds how far one
+// runs a ring of two 32 KB stages.  The training forward (fp16, SAVE) gives those 80 KB to the ring, nine 16 KB
+// stages: a stage is handed back only once both warpgroups are done with it, so the ring depth bounds how far one
 // warpgroup can run ahead while the other stores its saved tiles.  The non-saving fp16 forward measured no gain from
-// the deeper ring and keeps the x3 map (DESIGN.md §6).
+// the deeper ring and keeps the x3 map, four stages (DESIGN.md §6).
 constexpr uint32_t SM_TOTAL = 224 * 1024;
 template <int NSPLIT, bool SAVE>
 struct Smem {
@@ -45,13 +46,13 @@ struct Smem {
   static constexpr uint32_t E0 = DEEP ? A0 + A_TILE_BYTES : A1 + A_TILE_BYTES;
   static constexpr uint32_t E1 = E0 + E_TILE_BYTES;                              // x3 only
   static constexpr uint32_t W = DEEP ? E0 + E_TILE_BYTES : E1 + E_TILE_BYTES;
-  static constexpr int SLOTS = int((SM_TOTAL - W) / WSLOT_BYTES);
-  static_assert(SLOTS == (DEEP ? 9 : 4), "smem map");
-};
-template <int SLOTS>
-struct Barriers {
-  uint64_t full[SLOTS];
-  uint64_t empty[SLOTS];
+  static constexpr uint32_t PARTS = NSPLIT == 3 ? 2 : 1;                        // per stage: hi slot (, lo slot)
+  static constexpr uint32_t STAGE_BYTES = PARTS * WSLOT_BYTES;
+  static constexpr int STAGES = int((SM_TOTAL - W) / STAGE_BYTES);
+  static_assert(STAGES == (DEEP ? 9 : NSPLIT == 3 ? 2 : 4), "smem map");
+  // Unrolling of the producer's loops (16: full).  Fully unrolled, the x3 producer adds ~2300 instructions to a kernel
+  // twice the size of the fp16 one, and the x3 sigma forward ran 7-8 % slower (H100 80 GB HBM3, 700 W).
+  static constexpr int PRODUCER_UNROLL = NSPLIT == 3 ? 1 : 16;
 };
 
 __device__ __noinline__ void load_point(const FwdParams& p, long long s, float& x, float& y,
@@ -151,9 +152,8 @@ template <int NSPLIT, int OUTM, bool SAVE>
 __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_constant__ FwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   constexpr bool PRECISE = (NSPLIT == 3);
-  constexpr int STEP = NSPLIT == 3 ? 2 : 1;   // ring slots per K-slot (hi, lo)
   using SM = Smem<NSPLIT, SAVE>;
-  __shared__ __align__(8) Barriers<SM::SLOTS> bars;
+  __shared__ __align__(8) Ring<SM::STAGES> ring;
 
   // training launches cover the padded rows: mlp_bwd / mlp_wgrad read every tile of the padded arrays
   const long long num_tiles = SAVE ? padded_rows(p.M) / TILE_M : (p.M + TILE_M - 1) / TILE_M;
@@ -161,13 +161,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
   const uint32_t sbase = smem_u32(smem);
   const int NH = p.NH;
 
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < SM::SLOTS; ++i) {
-      mbar_init(smem_u32(&bars.full[i]), 1);
-      mbar_init(smem_u32(&bars.empty[i]), 8);   // one arrival per consumer warp
-    }
-    fence_mbar_init();
-  }
+  if (threadIdx.x == 0) ring.init(SM::STAGES);
   __syncthreads();
 
   if (warp >= PRODUCER_WARP) {
@@ -175,27 +169,24 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
     // whole-warp control flow, one elected lane issues
     setmaxnreg_dec<40>();
     if (warp != PRODUCER_WARP) return;
-    uint32_t slot = 0, phase = 0;
+    RingPos pos;
     for (long long it = blockIdx.x; it < num_tiles; it += gridDim.x) {
       size_t off = 0;
+#pragma unroll (SM::PRODUCER_UNROLL)
       for (int l = 0; l <= NUM_TRUNK; ++l) {
         const int ns = (l == NUM_TRUNK) ? FWD_HEAD_SLOTS : fwd_slots_of_layer(l);
         const uint32_t bytes = (l == NUM_TRUNK) ? uint32_t(NH) * 64u : uint32_t(WSLOT_BYTES);
+#pragma unroll (SM::PRODUCER_UNROLL)
         for (int j = 0; j < ns; ++j) {
-#pragma unroll
-          for (int part = 0; part < STEP; ++part) {
-            mbar_wait(smem_u32(&bars.empty[slot]), phase ^ 1);
-            if (elect_one()) {
-              mbar_arrive_expect_tx(smem_u32(&bars.full[slot]), bytes);
-              bulk_g2s(sbase + SM::W + slot * WSLOT_BYTES, (part == 0 ? p.w.w_hi : p.w.w_lo) + off, bytes,
-                       smem_u32(&bars.full[slot]));
-            }
-            __syncwarp();
-            if (++slot == SM::SLOTS) {
-              slot = 0;
-              phase ^= 1;
-            }
+          ring.acquire(pos);
+          if (elect_one()) {
+            const uint32_t bar = ring.arm(pos, SM::PARTS * bytes);
+            const uint32_t dst = sbase + SM::W + pos.stage * SM::STAGE_BYTES;
+            bulk_g2s(dst, p.w.w_hi + off, bytes, bar);
+            if (NSPLIT == 3) bulk_g2s(dst + WSLOT_BYTES, p.w.w_lo + off, bytes, bar);
           }
+          __syncwarp();
+          pos.advance(SM::STAGES);
           off += bytes;
         }
       }
@@ -217,7 +208,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
   const uint32_t rows_off = uint32_t(wg) * 64u * 128u;     // this warpgroup's 64 rows inside every 128-row chunk
   constexpr uint64_t A_DESC = make_sdesc_hi(16, 1024, LAYOUT_SW128);
   constexpr uint64_t W_DESC = make_sdesc_hi(16, 512, LAYOUT_SW64);
-  uint32_t slot = 0, phase = 0;
+  RingPos pos;
   float acc[128];
   float hacc[HEADS_N / 2];
 
@@ -248,10 +239,9 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
         const uint32_t a_off = uint32_t(kk >> 1) * A_CHUNK_BYTES + rows_off + uint32_t(kk & 1) * 64u;
         const uint32_t ah = sbase + (from_e ? SM::E0 : SM::A0) + a_off;
         const uint32_t al = sbase + (from_e ? SM::E1 : SM::A1) + a_off;
-        const uint32_t bh = sbase + SM::W + slot * WSLOT_BYTES;
-        const uint32_t bl = bh + WSLOT_BYTES;   // x3 only; the ring depth is even: hi/lo never straddle the wrap
-        mbar_wait(smem_u32(&bars.full[slot]), phase);
-        if (NSPLIT == 3) mbar_wait(smem_u32(&bars.full[slot + 1]), phase);
+        const uint32_t bh = sbase + SM::W + pos.stage * SM::STAGE_BYTES;
+        const uint32_t bl = bh + WSLOT_BYTES;   // x3 only
+        ring.wait(pos);
 #pragma unroll
         for (int k = 0; k < 2; ++k) {
           if (k == 0 && bias_slot) continue;
@@ -273,25 +263,15 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
         }
         wgmma_commit();
         if (j > 0) {
-          // the previous K-slot's MMAs are complete: hand its ring slot(s) back to the producer
+          // the previous K-slot's MMAs are complete: hand its stage back to the producer
           wgmma_wait<1>();
-          if (lane == 0) {
-            mbar_arrive(smem_u32(&bars.empty[prev]));
-            if (NSPLIT == 3) mbar_arrive(smem_u32(&bars.empty[prev + 1]));
-          }
+          ring.release(prev);
         }
-        prev = slot;
-        slot += STEP;
-        if (slot == SM::SLOTS) {
-          slot = 0;
-          phase ^= 1;
-        }
+        prev = pos.stage;
+        pos.advance(SM::STAGES);
       }
       wgmma_wait<0>();
-      if (lane == 0) {
-        mbar_arrive(smem_u32(&bars.empty[prev]));
-        if (NSPLIT == 3) mbar_arrive(smem_u32(&bars.empty[prev + 1]));
-      }
+      ring.release(prev);
 
       if (!heads) {
         // ---- trunk epilogue: ReLU + fp16 pack straight from the accumulator fragment into the next A operand
@@ -372,7 +352,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
           float pre[3] = {0.f, 0.f, 0.f};
           for (int k = 0; k < K; ++k) {
 #pragma unroll
-            for (int c = 0; c < 3; ++c) pre[c] = fmaf(basis[k], st[1 + 3 * k + c], pre[c]);
+            for (int c = 0; c < 3; ++c) pre[c] = fmaf(basis[k], st[heads_column(k, c)], pre[c]);
           }
           float sigma_raw = st[0];
           float4 o;
@@ -387,18 +367,18 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
       } else if (OUTM == OUT_SIGMA || OUTM == OUT_RAW) {
         if (t < 64 && row0 + t < p.M) p.out_sigma[row0 + t] = stage_row(a_hi, wg, t)[0];
         if (OUTM == OUT_RAW) {
-          // reference channel-major order: out column c*K + k <- packed column 1 + 3k + c
+          // reference channel-major order
           const int C3 = 3 * K;
           for (int rr = 0; rr < 64 && row0 + rr < p.M; ++rr) {
             const float* st = stage_row(a_hi, wg, rr);
-            for (int i = t; i < C3; i += 128) p.out_rgb[(row0 + rr) * C3 + i] = st[1 + 3 * (i % K) + i / K];
+            for (int i = t; i < C3; i += 128) p.out_rgb[(row0 + rr) * C3 + i] = st[heads_column_of_output(i, K)];
           }
         }
       } else if (OUTM == OUT_CELL_MEAN) {
         // extraction step 2 (octree/extraction.py:367-394): out[cell] += cat([raw_rgb, raw_sigma]) / S.
         const int width = 3 * K + 1;
         const float inv = 1.0f / float(p.cell_S);
-        auto col_of = [&](int i) { return i == 3 * K ? 0 : 1 + 3 * (i % K) + i / K; };
+        auto col_of = [&](int i) { return i == 3 * K ? 0 : heads_column_of_output(i, K); };
         if ((p.cell_S & 31) == 0) {
           // 32 consecutive rows belong to one cell: 64 threads per 32-row half sum over rows, one atomic per column
           const int hf = t >> 6;
@@ -424,10 +404,8 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
   }
 }
 
-cudaError_t launch_mlp_fwd(const FwdParams& p, int nsplit, bool precise_sin, int num_sms,
-                           cudaStream_t stream) {
+cudaError_t launch_mlp_fwd(const FwdParams& p, int nsplit, int num_sms, cudaStream_t stream) {
   if (p.M <= 0) return cudaSuccess;
-  (void)precise_sin;   // tied to the precision mode: FP16X3 uses libdevice sinf, FP16 the reduced SFU sine
   if (nsplit != 1 && nsplit != 3) return cudaErrorInvalidValue;
   const bool save = p.save_h != nullptr;
   if (save && (nsplit != 1 || !p.save_e || !p.save_mask ||

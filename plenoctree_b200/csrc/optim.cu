@@ -20,7 +20,7 @@ int wgrad_assign_roles(WgradParams& p, int n_in, int role_start[WG_NUM_ROLES],
   small = even((n - 7 * big) / 3);
   int cta = 0;
   for (int r = 0; r < WG_NUM_ROLES; ++r) {
-    const int c = r < 7 ? big : small;
+    const int c = wgrad_role(r).width == 256 ? big : small;
     role_start[r] = cta;
     role_count[r] = c;
     for (int i = 0; i < c; ++i, ++cta) {
@@ -50,50 +50,22 @@ struct ReduceArgs {
 
 // role and offset inside a role's partial of element (layer, in i, out o) of a kernel, or (layer, out o) of a bias
 __device__ __forceinline__ void locate(const ReduceArgs& a, int layer, int i, int o, bool is_bias, int& role, int& off) {
-  if (!is_bias) {
-    if (layer == 0) {
-      role = 7;
-      off = o * 64 + i;
-    } else if (layer < 8) {
-      if (layer == 5 && i >= 256) {
-        role = 8;
-        off = o * 64 + (i - 256);
-      } else {
-        role = layer <= 4 ? layer - 1 : (layer == 5 ? 4 : layer - 1);
-        off = o * 256 + i;
-      }
-    } else {
-      role = 9;  // heads: D[in feature][packed column]
-      int n;
-      if (layer == 8) n = 0;
-      else {
-        const int c = o / a.K, k = o % a.K;
-        n = 1 + 3 * k + c;
-      }
-      off = i * a.NH + n;
-    }
-  } else {
-    if (layer < 8) {
-      role = layer == 0 ? 7 : (layer <= 4 ? layer - 1 : (layer == 5 ? 4 : layer - 1));
-      off = 65536 + o;
-    } else {
-      role = 9;
-      int n;
-      if (layer == 8) n = 0;
-      else {
-        const int c = o / a.K, k = o % a.K;
-        n = 1 + 3 * k + c;
-      }
-      off = 65536 + n;
-    }
+  role = wgrad_role_of(layer, i);
+  const WgradRole R = wgrad_role(role);
+  if (R.a_op == WG_H) {    // heads: D[in feature][packed column]
+    const int n = layer == 8 ? 0 : heads_column_of_output(o, a.K);
+    off = is_bias ? 65536 + n : i * a.NH + n;
+  } else {                 // D[out feature][in feature - in0]
+    off = is_bias ? 65536 + o : o * R.width + (i - R.in0);
   }
 }
 
-// sum over the role's CTAs that computed the element: those of its result row half (the heads bias, a column
-// sum of dO, comes from row half 0)
+// sum over the role's CTAs that computed the element: those of its result row half (a bias taken from B, the heads'
+// column sum of dO, comes from row half 0)
 __device__ __forceinline__ float sum_partials(const ReduceArgs& a, int role, int off) {
-  const int pitch = role < 7 ? 256 : (role < 9 ? 64 : a.NH);
-  const int row = off < 65536 ? off / pitch : (role == 9 ? 0 : off - 65536);
+  const WgradRole R = wgrad_role(role);
+  const int pitch = wgrad_role_width(R, a.NH);
+  const int row = off < 65536 ? off / pitch : (R.bias == WG_BIAS_B ? 0 : off - 65536);
   float s = 0.f;
   const float* p = a.partials + size_t(a.role_start[role]) * WG_PARTIAL_FLOATS + off;
   for (int c = row >> 7; c < a.role_count[role]; c += 2) s += p[size_t(c) * WG_PARTIAL_FLOATS];

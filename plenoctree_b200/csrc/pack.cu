@@ -22,7 +22,6 @@ struct PackArgs {
   FlatLayout L;
   int K, NH;
   uint8_t *w_hi, *w_lo, *wt_hi;
-  float* bias;
 };
 
 __device__ __forceinline__ void put_hilo(uint8_t* hi, uint8_t* lo, size_t off, float v) {
@@ -31,22 +30,26 @@ __device__ __forceinline__ void put_hilo(uint8_t* hi, uint8_t* lo, size_t off, f
   if (lo) *reinterpret_cast<__half*>(lo + off) = __float2half_rn(v - __half2float(h));
 }
 
-// heads: packed output column n' -> value of W[in=i -> n'] and bias
+// heads: the parameter of packed output column n, at flat offset off8 for Dense_8 (sigma) and off9 + (Dense_9 output)
+// for the SH coefficients; 0 in the padding columns
+__device__ __forceinline__ float heads_param(const PackArgs& a, int off8, int off9, int n) {
+  if (n == 0) return a.flat[off8];
+  int k, c;
+  heads_coeff(n, k, c);
+  return k < a.K ? a.flat[off9 + c * a.K + k] : 0.f;
+}
+// W[in=i -> packed column n]
 __device__ __forceinline__ float heads_weight(const PackArgs& a, int i, int n) {
-  if (n == 0) return a.flat[a.L.w_off[8] + i];  // Dense_8 kernel [256,1]
-  const int k = (n - 1) / 3, c = (n - 1) % 3;
-  if (k >= a.K) return 0.f;
-  return a.flat[a.L.w_off[9] + i * (3 * a.K) + c * a.K + k];
+  return heads_param(a, a.L.w_off[8] + i, a.L.w_off[9] + i * (3 * a.K), n);
 }
 
 __global__ void pack_weights_kernel(const __grid_constant__ PackArgs a) {
   const int NH = a.NH;
   const long long n_fwd_trunk = (long long)FWD_TRUNK_SLOTS * 256 * 32;
   const long long n_fwd_heads = (long long)FWD_HEAD_SLOTS * NH * 32;
-  const int hs = (NH + 31) / 32;
-  const long long n_bwd = (long long)(hs + 56) * 256 * 32;
-  const long long n_bias = 8 * 256 + MAX_NH;
-  const long long total = n_fwd_trunk + n_fwd_heads + n_bwd + n_bias;
+  const int hs = bwd_head_slots(NH);
+  const long long n_bwd = (long long)bwd_slots(NH) * 256 * 32;
+  const long long total = n_fwd_trunk + n_fwd_heads + n_bwd;
   for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
        t += (long long)gridDim.x * blockDim.x) {
     if (t < n_fwd_trunk) {
@@ -72,20 +75,11 @@ __global__ void pack_weights_kernel(const __grid_constant__ PackArgs a) {
       const long long u = t - n_fwd_trunk;
       const int j = int(u / (NH * 32));
       const int n = int(u / 32) % NH, kk = int(u % 32);
-      float v;
+      float v = 0.f;
       if (j < 8) v = heads_weight(a, 32 * j + kk, n);
-      else {
-        v = 0.f;
-        if (kk == 31) {
-          if (n == 0) v = a.flat[a.L.b_off[8]];
-          else {
-            const int k = (n - 1) / 3, c = (n - 1) % 3;
-            if (k < a.K) v = a.flat[a.L.b_off[9] + c * a.K + k];
-          }
-        }
-      }
+      else if (kk == 31) v = heads_param(a, a.L.b_off[8], a.L.b_off[9], n);   // bias slot
       put_hilo(a.w_hi, a.w_lo, size_t(FWD_TRUNK_SLOTS) * WSLOT_BYTES + size_t(j) * NH * 64 + w_slot_offset(n, kk), v);
-    } else if (t < n_fwd_trunk + n_fwd_heads + n_bwd) {
+    } else {
       const long long u = t - n_fwd_trunk - n_fwd_heads;
       const int slot = int(u / (256 * 32));
       const int i = int(u / 32) % 256, kk = int(u % 32);  // i = in feature (row), kk = out feature
@@ -99,20 +93,6 @@ __global__ void pack_weights_kernel(const __grid_constant__ PackArgs a) {
         v = a.flat[a.L.w_off[l] + i * 256 + ko];
       }
       put_hilo(a.wt_hi, nullptr, size_t(slot) * WSLOT_BYTES + w_slot_offset(i, kk), v);
-    } else {
-      const int b = int(t - n_fwd_trunk - n_fwd_heads - n_bwd);
-      float v = 0.f;
-      if (b < 8 * 256) {
-        v = a.flat[a.L.b_off[b / 256] + (b % 256)];
-      } else {
-        const int n = b - 8 * 256;
-        if (n == 0) v = a.flat[a.L.b_off[8]];
-        else {
-          const int k = (n - 1) / 3, c = (n - 1) % 3;
-          if (k < a.K) v = a.flat[a.L.b_off[9] + c * a.K + k];
-        }
-      }
-      a.bias[b] = v;
     }
   }
 }
@@ -120,7 +100,7 @@ __global__ void pack_weights_kernel(const __grid_constant__ PackArgs a) {
 }  // namespace
 
 cudaError_t launch_pack_weights(const float* flat, int K, uint8_t* w_hi, uint8_t* w_lo,
-                                uint8_t* wt_hi, float* bias, cudaStream_t stream) {
+                                uint8_t* wt_hi, cudaStream_t stream) {
   PackArgs a;
   a.flat = flat;
   a.L = flat_layout(K);
@@ -129,7 +109,6 @@ cudaError_t launch_pack_weights(const float* flat, int K, uint8_t* w_hi, uint8_t
   a.w_hi = w_hi;
   a.w_lo = w_lo;
   a.wt_hi = wt_hi;
-  a.bias = bias;
   pack_weights_kernel<<<592, 256, 0, stream>>>(a);
   return cudaGetLastError();
 }

@@ -18,7 +18,7 @@ using namespace pob;
 struct Level {
   // sizes
   long long M;        // samples
-  long long tiles;    // padded to an even number of 128-row tiles
+  long long tiles;    // 128-row tiles of padded_rows(M)
   // buffers
   float* z;           // [R,N]
   float4* rgbs;       // [M]
@@ -143,7 +143,7 @@ int forward_levels(const char* where, const pob_render_config& c, Workspace& w, 
       p.save_e = C.E;
       p.save_mask = C.mask;
     }
-    { pob_count_launch(1); PobPhaseTimer _t(POB_PH_FWD, st); POB_CUDA(where, launch_mlp_fwd(p, precision, precision == POB_PREC_FP16X3, sms, st)); }
+    { pob_count_launch(1); PobPhaseTimer _t(POB_PH_FWD, st); POB_CUDA(where, launch_mlp_fwd(p, precision, sms, st)); }
   }
   { pob_count_launch(1); PobPhaseTimer _t(POB_PH_RENDER, st); POB_CUDA(where, launch_composite_fwd(C.rgbs, C.z, d, R, Nc, c.white_bkgd, C.comp, C.disp, C.acc, C.weights, st)); }
   if (Nf > 0) {
@@ -164,7 +164,7 @@ int forward_levels(const char* where, const pob_render_config& c, Workspace& w, 
       p.save_e = F.E;
       p.save_mask = F.mask;
     }
-    { pob_count_launch(1); PobPhaseTimer _t(POB_PH_FWD, st); POB_CUDA(where, launch_mlp_fwd(p, precision, precision == POB_PREC_FP16X3, sms, st)); }
+    { pob_count_launch(1); PobPhaseTimer _t(POB_PH_FWD, st); POB_CUDA(where, launch_mlp_fwd(p, precision, sms, st)); }
     { pob_count_launch(1); PobPhaseTimer _t(POB_PH_RENDER, st); POB_CUDA(where, launch_composite_fwd(F.rgbs, F.z, d, R, Nc + Nf, c.white_bkgd, F.comp, F.disp, F.acc,
                                          F.weights, st)); }
   }

@@ -6,15 +6,14 @@
 // fp32 accumulator is half of an SM's register file (two warpgroups, one m64n256 accumulator each), so the two row
 // halves of a role are separate CTAs.  A CTA streams the [sample x feature] tile images that mlp_fwd (h_l, posenc)
 // and mlp_bwd (dZ_l, dO) left in global memory; both wgmma operands are read MN-major straight from those images
-// (K = samples): no transposes.  dZ / dO / posenc tiles are K-major SW128 images (read MN-major with the same
+// (K = samples): no transposes; warp 8 loads them through a ring of 64-sample stages (common.cuh: Ring) whose depth
+// depends on the role's bytes per stage.  dZ / dO / posenc tiles are K-major SW128 images (read MN-major with the same
 // swizzle), the h_l tiles are "T" images (no swizzle, 128 B core matrices; layouts.py: t_tile_offset).
 // CTAs of the same role and row half split the tiles round-robin and each writes an fp32 partial; reduce_grads
 // (optim.cu) sums the partials into the flat gradient (deterministic, no atomics).
 //
-// Roles: 0..6 = Dense_1,2,3,4,5(h4 rows),6,7   A = dZ_l (256 out)  B = h_{l-1} (256 in)
-//        7    = Dense_0                         A = dZ_0            B = posenc   (64)
-//        8    = Dense_5 (posenc rows)           A = dZ_5            B = posenc   (64)
-//        9    = heads (Dense_8 | Dense_9)       A = h_7 (256 in)    B = dO       (NH)  [transposed result]
+// Roles (kernels.h: wgrad_role): Dense_1..7 (Dense_5: its h4 rows) with A = dZ_l and B = h_{l-1}; Dense_0 and the
+// posenc rows of Dense_5 with B = posenc; the heads with A = h_7 and B = dO (a transposed result).
 // Bias gradients are column sums of the A (or, for the heads, B) tile, summed by the consumer warps from the staged
 // shared-memory tiles while their MMAs run.
 //
@@ -53,15 +52,10 @@ constexpr uint32_t WG_SMEM = 4 * (WG_A_BYTES + WG_B_MAX);   // four 48 KB stages
 // A stage holds A and the role's B features only, so the narrow roles (Dense_0, Dense_5's posenc rows, the heads:
 // 24-32 KB per stage) keep six to eight stages in flight.  Their time per stage is load latency rather than MMAs.
 constexpr int WG_MAX_STAGES = 8;
-
-struct WgBarriers {
-  uint64_t full[WG_MAX_STAGES];
-  uint64_t empty[WG_MAX_STAGES];
-};
+using WgRing = Ring<WG_MAX_STAGES>;
 
 struct RoleInfo {
-  int a_kind, a_layer;   // 0: dZ[layer], 1: H[layer]
-  int b_kind, b_layer;   // 0: H[layer], 1: E, 2: dO
+  int a_op, a_layer, b_op, b_layer;   // kernels.h: WgradRole
   int b_chunks, N;
   int bias_from_b;       // heads: bias = column sums of dO
   int has_bias;
@@ -69,24 +63,18 @@ struct RoleInfo {
 };
 
 __device__ __forceinline__ RoleInfo role_info(int role, int NH) {
+  const WgradRole W = wgrad_role(role);
   RoleInfo r;
-  r.bias_from_b = 0;
-  r.has_bias = 1;
-  r.a_t = 0;
-  r.b_t = 0;
-  if (role < 7) {
-    r.b_t = 1;
-    const int l = role < 4 ? role + 1 : (role == 4 ? 5 : role + 1);  // 1,2,3,4,5,6,7
-    r.a_kind = 0; r.a_layer = l; r.b_kind = 0; r.b_layer = l - 1; r.b_chunks = 4; r.N = 256;
-  } else if (role == 7) {
-    r.a_kind = 0; r.a_layer = 0; r.b_kind = 1; r.b_layer = 0; r.b_chunks = 1; r.N = 64;
-  } else if (role == 8) {
-    r.a_kind = 0; r.a_layer = 5; r.b_kind = 1; r.b_layer = 0; r.b_chunks = 1; r.N = 64; r.has_bias = 0;
-  } else {
-    r.a_kind = 1; r.a_layer = 7; r.b_kind = 2; r.b_layer = 0; r.b_chunks = (NH + 63) / 64; r.N = NH;
-    r.bias_from_b = 1;
-    r.a_t = 1;
-  }
+  r.a_op = W.a_op;
+  r.a_layer = W.a_layer;
+  r.b_op = W.b_op;
+  r.b_layer = W.b_layer;
+  r.N = wgrad_role_width(W, NH);
+  r.b_chunks = (r.N + 63) / 64;
+  r.bias_from_b = W.bias == WG_BIAS_B;
+  r.has_bias = W.bias != WG_BIAS_NONE;
+  r.a_t = W.a_op == WG_H;
+  r.b_t = W.b_op == WG_H;
   return r;
 }
 
@@ -98,7 +86,7 @@ constexpr uint64_t T_DESC = make_sdesc_hi(128, 512, LAYOUT_NONE);
 // Consumer warpgroup `wg`: accumulates D[64 A features x NN] over the CTA's stages, then writes its rows of the
 // partial.  NN = MMA width (256, 64, or 80 for the heads, whose columns >= NH are never written back).
 template <int NN>
-__device__ __forceinline__ void wgrad_consume(const RoleInfo& R, uint8_t* smem, WgBarriers& bars, int nst,
+__device__ __forceinline__ void wgrad_consume(const RoleInfo& R, uint8_t* smem, WgRing& ring, int nst,
                                               uint32_t stage_bytes, long long n_items, int mh, float* out_w,
                                               float* out_b) {
   const uint32_t warp = warp_id(), lane = lane_id();
@@ -120,12 +108,12 @@ __device__ __forceinline__ void wgrad_consume(const RoleInfo& R, uint8_t* smem, 
   const uint32_t unit = uint32_t((f & 63) >> 3), wsel = uint32_t(f & 7) * 2;
   float s0 = 0.f, s1 = 0.f;
 
-  uint32_t st = 0, phase = 0;
+  RingPos pos;
   wgmma_fence();
   for (long long i = 0; i < n_items; ++i) {
     for (int sub = 0; sub < 2; ++sub) {
-      mbar_wait(smem_u32(&bars.full[st]), phase);
-      const uint32_t a0 = sbase + st * stage_bytes;
+      ring.wait(pos);
+      const uint32_t a0 = sbase + pos.stage * stage_bytes;
       const uint32_t b0 = a0 + WG_A_BYTES;
 #pragma unroll
       for (int ks = 0; ks < WG_SUB / 16; ++ks) {
@@ -140,7 +128,7 @@ __device__ __forceinline__ void wgrad_consume(const RoleInfo& R, uint8_t* smem, 
       }
       wgmma_commit();
       if (a_bias || b_bias) {
-        const uint8_t* base = smem + st * stage_bytes + bias_src;
+        const uint8_t* base = smem + pos.stage * stage_bytes + bias_src;
 #pragma unroll 4
         for (int r = s_lo; r < s_lo + s_n; ++r) {
           const float2 v = unpack_f16x2(
@@ -150,11 +138,8 @@ __device__ __forceinline__ void wgrad_consume(const RoleInfo& R, uint8_t* smem, 
         }
       }
       wgmma_wait<0>();
-      if (lane == 0) mbar_arrive(smem_u32(&bars.empty[st]));
-      if (++st == uint32_t(nst)) {
-        st = 0;
-        phase ^= 1;
-      }
+      ring.release(pos.stage);
+      pos.advance(nst);
     }
   }
 
@@ -190,7 +175,7 @@ __device__ __forceinline__ void wgrad_consume(const RoleInfo& R, uint8_t* smem, 
 
 // cta indexes cta_role/index/count and the partials
 __device__ __forceinline__ void wgrad_body(const WgradParams& p, uint8_t* smem, const int cta) {
-  __shared__ __align__(8) WgBarriers bars;
+  __shared__ __align__(8) WgRing ring;
 
   const uint32_t warp = warp_id();
   const uint32_t sbase = smem_u32(smem);
@@ -214,13 +199,7 @@ __device__ __forceinline__ void wgrad_body(const WgradParams& p, uint8_t* smem, 
   const long long total_tiles = p.seg_tiles;
   const long long n_items = (total_tiles > sidx) ? (total_tiles - sidx + scnt - 1) / scnt : 0;
 
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < nst; ++i) {
-      mbar_init(smem_u32(&bars.full[i]), 1);
-      mbar_init(smem_u32(&bars.empty[i]), 8);   // one arrival per consumer warp
-    }
-    fence_mbar_init();
-  }
+  if (threadIdx.x == 0) ring.init(nst);
   __syncthreads();
 
   if (warp == 8) {
@@ -228,16 +207,16 @@ __device__ __forceinline__ void wgrad_body(const WgradParams& p, uint8_t* smem, 
     // whole-warp control flow, one elected lane issues
     const WgradSegment& sg = p.seg;
     // every role reads one operand mlp_bwd stores: dZ_l (stage 8 - l) or, for the heads, dO (stage 0)
-    const uint32_t want = R.a_kind == 0 ? uint32_t(NUM_TRUNK + 1 - R.a_layer) : 1u;
-    uint32_t st = 0, phase = 0;
+    const uint32_t want = R.a_op == WG_DZ ? uint32_t(NUM_TRUNK + 1 - R.a_layer) : 1u;
+    RingPos pos;
     for (long long i = 0; i < n_items; ++i) {
       const long long lt = sidx + i * scnt;
-      const uint8_t* a_ptr = (R.a_kind == 0 ? sg.dz : sg.h) + (size_t(lt) * NUM_TRUNK + R.a_layer) * A_TILE_BYTES;
-      const uint8_t* b_ptr = R.b_kind == 0 ? sg.h + (size_t(lt) * NUM_TRUNK + R.b_layer) * A_TILE_BYTES
-                             : R.b_kind == 1 ? sg.e + size_t(lt) * E_TILE_BYTES
-                                             : sg.d_o + size_t(lt) * (2 * A_CHUNK_BYTES);
+      const uint8_t* a_ptr = (R.a_op == WG_DZ ? sg.dz : sg.h) + (size_t(lt) * NUM_TRUNK + R.a_layer) * A_TILE_BYTES;
+      const uint8_t* b_ptr = R.b_op == WG_H ? sg.h + (size_t(lt) * NUM_TRUNK + R.b_layer) * A_TILE_BYTES
+                             : R.b_op == WG_E ? sg.e + size_t(lt) * E_TILE_BYTES
+                                              : sg.d_o + size_t(lt) * (2 * A_CHUNK_BYTES);
       for (int sub = 0; sub < 2; ++sub) {
-        mbar_wait(smem_u32(&bars.empty[st]), phase ^ 1);
+        ring.acquire(pos);
         if (elect_one()) {
           // the thread that issues the loads is the one that acquires (once the tile is complete, this is one L2 hit)
           for (uint32_t ns = 32;;) {
@@ -247,9 +226,8 @@ __device__ __forceinline__ void wgrad_body(const WgradParams& p, uint8_t* smem, 
             if (ns < 512) ns *= 2;
           }
           fence_proxy_async_global();
-          const uint32_t bar = smem_u32(&bars.full[st]);
-          mbar_arrive_expect_tx(bar, WG_A_BYTES + b_bytes);
-          const uint32_t dst = sbase + st * stage_bytes;
+          const uint32_t bar = ring.arm(pos, WG_A_BYTES + b_bytes);
+          const uint32_t dst = sbase + pos.stage * stage_bytes;
 #pragma unroll
           for (int c = 0; c < 2; ++c) {
             if (R.a_t)   // T image: this half's 128 features = 8 KB of each 32-sample group
@@ -265,17 +243,14 @@ __device__ __forceinline__ void wgrad_body(const WgradParams& p, uint8_t* smem, 
           }
         }
         __syncwarp();
-        if (++st == uint32_t(nst)) {
-          st = 0;
-          phase ^= 1;
-        }
+        pos.advance(nst);
       }
     }
     return;
   }
-  if (R.N == 256) wgrad_consume<256>(R, smem, bars, nst, stage_bytes, n_items, mh, out_w, out_b);
-  else if (R.N == 64) wgrad_consume<64>(R, smem, bars, nst, stage_bytes, n_items, mh, out_w, out_b);
-  else wgrad_consume<MAX_NH>(R, smem, bars, nst, stage_bytes, n_items, mh, out_w, out_b);
+  if (R.N == 256) wgrad_consume<256>(R, smem, ring, nst, stage_bytes, n_items, mh, out_w, out_b);
+  else if (R.N == 64) wgrad_consume<64>(R, smem, ring, nst, stage_bytes, n_items, mh, out_w, out_b);
+  else wgrad_consume<MAX_NH>(R, smem, ring, nst, stage_bytes, n_items, mh, out_w, out_b);
 }
 
 }  // namespace pob

@@ -124,10 +124,8 @@ def blob_layout(K):
     w_hi = 0
     w_lo = up(w_hi + fwd)
     wt_hi = up(w_lo + fwd)
-    bias = up(wt_hi + bwd)
-    total = up(bias + (8 * 256 + 80) * 4)
-    return dict(w_hi=w_hi, w_lo=w_lo, wt_hi=wt_hi, bias=bias, total=total, fwd_bytes=fwd,
-                bwd_bytes=bwd, NH=NH)
+    total = up(wt_hi + bwd)
+    return dict(w_hi=w_hi, w_lo=w_lo, wt_hi=wt_hi, total=total, fwd_bytes=fwd, bwd_bytes=bwd, NH=NH)
 
 
 def heads_matrix(flat, K):
@@ -156,7 +154,7 @@ def heads_column(K, o):
 
 
 def pack_reference(flat, sh_deg):
-    """numpy model of pack.cu: returns dict of uint8 images w_hi, w_lo, wt_hi and float32 bias."""
+    """numpy model of pack.cu: returns dict of uint8 images w_hi, w_lo, wt_hi."""
     K = K_of(sh_deg)
     L = blob_layout(K)
     NH = L["NH"]
@@ -218,11 +216,7 @@ def pack_reference(flat, sh_deg):
         for j in range(8):
             wt_hi[slot * 16384:(slot + 1) * 16384] = pack_w_slot(W[:, 32 * j:32 * j + 32])
             slot += 1
-    bias = np.zeros(8 * 256 + 80, np.float32)
-    for l in range(8):
-        bias[l * 256:(l + 1) * 256] = flat[b_off[l]:b_off[l] + 256]
-    bias[2048:2048 + NH] = bh
-    return dict(w_hi=w_hi, w_lo=w_lo, wt_hi=wt_hi, bias=bias)
+    return dict(w_hi=w_hi, w_lo=w_lo, wt_hi=wt_hi)
 
 
 # ---- training workspace (mirrors carve() in csrc/pipeline.cu) ------------------------------------------------------
