@@ -11,11 +11,14 @@
 //
 // Warp roles (384 threads): warps 0-3 and 4-7 = two consumer warpgroups, each owning 64 rows of the tile (wgmma
 // m64n256, accumulator in registers), warp 8 = weight producer (a ring of eight 16 KB stages, one K-slot of the
-// transposed weights each; warps 9-11 only hand their registers back).  A warpgroup writes its dZ rows into the shared
-// tile it reads as the next GEMM's A operand, and one thread hands those rows to the bulk-copy engine
-// (cp.async.bulk shared -> global), so the 64 KB per tile and GEMM leave the SM without occupying the warps.
+// transposed weights each), warps 9 and 10 = store warps of warpgroups 0 and 1 (warp 11 only hands its registers
+// back).  A warpgroup feeds dZ_l to the next GEMM as a register A fragment and copies it into its rows of the shared
+// tile behind that GEMM's MMAs; its store warp sends the rows to global memory (cp.async.bulk shared -> global), so
+// the 64 KB per tile and GEMM leave the SM without occupying the consumer warps.
 // mlp_wgrad runs alongside on the remaining SMs and reads each stored stage back from L2 once the per-tile progress
 // counter says it is complete (wgrad_body.cuh).
+#include <type_traits>
+
 #include "common.cuh"
 #include "kernels.h"
 
@@ -25,6 +28,7 @@ namespace {
 
 constexpr int BWD_THREADS = 384;
 constexpr int BWD_PRODUCER_WARP = 8;
+constexpr int BWD_STORE_WARP0 = 9;      // warps 9, 10: store warps of warpgroups 0, 1
 constexpr int BWD_WSLOTS = 8;
 
 constexpr uint32_t SB_A = 0;
@@ -36,6 +40,9 @@ constexpr uint32_t SB_TOTAL = SB_W + BWD_WSLOTS * WSLOT_BYTES;  // 64K + 128K = 
 __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_constant__ BwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   __shared__ __align__(8) Ring<BWD_WSLOTS> ring;
+  // hand-over of a warpgroup's rows of the A tile: rows_full[g] completes once its 128 threads have written a stage's
+  // rows, rows_free[g] once the store warp's bulk stores have read them
+  __shared__ __align__(8) uint64_t rows_full[2], rows_free[2];
 
   const long long mrows = padded_rows(p.M);        // rows of the mask / tile arrays
   const long long num_tiles = mrows / TILE_M;      // padded tiles get zero gradients, not garbage
@@ -46,25 +53,69 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
 
   // the mlp_wgrad launch behind this one may take the SMs this grid leaves free (wgrad_body.cuh)
   griddep_launch_dependents();
-  if (threadIdx.x == 0) ring.init(BWD_WSLOTS);
+  if (threadIdx.x == 0) {
+    ring.init(BWD_WSLOTS);
+    for (int g = 0; g < 2; ++g) {
+      mbar_init(smem_u32(&rows_full[g]), 128);
+      mbar_init(smem_u32(&rows_free[g]), 1);
+    }
+    fence_mbar_init();
+  }
   __syncthreads();
 
   if (warp >= BWD_PRODUCER_WARP) {
     // whole-warp control flow, one elected lane issues
     setmaxnreg_dec<40>();
-    if (warp != BWD_PRODUCER_WARP) return;
-    RingPos pos;
-    const int nslots = bwd_slots(NH);
-    for (long long it = blockIdx.x; it < num_tiles; it += gridDim.x) {
-      for (int j = 0; j < nslots; ++j) {
-        ring.acquire(pos);
-        if (elect_one()) {
-          const uint32_t bar = ring.arm(pos, WSLOT_BYTES);
-          bulk_g2s(sbase + SB_W + pos.stage * WSLOT_BYTES, p.w.wt_hi + size_t(j) * WSLOT_BYTES, WSLOT_BYTES, bar);
+    if (warp == BWD_PRODUCER_WARP) {
+      RingPos pos;
+      const int nslots = bwd_slots(NH);
+      for (long long it = blockIdx.x; it < num_tiles; it += gridDim.x) {
+        for (int j = 0; j < nslots; ++j) {
+          ring.acquire(pos);
+          if (elect_one()) {
+            const uint32_t bar = ring.arm(pos, WSLOT_BYTES);
+            bulk_g2s(sbase + SB_W + pos.stage * WSLOT_BYTES, p.w.wt_hi + size_t(j) * WSLOT_BYTES, WSLOT_BYTES, bar);
+          }
+          __syncwarp();
+          pos.advance(BWD_WSLOTS);
         }
-        __syncwarp();
-        pos.advance(BWD_WSLOTS);
       }
+    } else if (warp <= BWD_STORE_WARP0 + 1 && lane == 0) {
+      // ---- store warp of warpgroup g: every stage of its 64 rows (dO, dZ_7 .. dZ_0) leaves the SM as bulk stores.
+      // Progress (wgrad_body.cuh reads it): warpgroup 0 counts in the low, warpgroup 1 in the high 16 bits of the
+      // tile's counter, one per stage whose bulk stores have completed.  A stage is published once the next one has
+      // been committed (wait_group 1), so the rows go back to the warpgroup as soon as they have been read. ----
+      const int g = int(warp) - BWD_STORE_WARP0;
+      const uint32_t rows_off = uint32_t(g) * 64u * 128u;
+      const uint32_t progress_inc = g == 0 ? 1u : 0x10000u;
+      const uint32_t full = smem_u32(&rows_full[g]), free = smem_u32(&rows_free[g]);
+      uint32_t phase = 0;
+      long long pending = -1;       // tile of the most recent committed, not yet published store group
+      auto publish = [&]() {        // pending's group has completed: its writes are visible to this thread
+        fence_proxy_async_global();
+        red_add_release_gpu(p.progress + pending, progress_inc);
+      };
+      for (long long it = blockIdx.x; it < num_tiles; it += gridDim.x) {
+        for (int st = 0; st <= NUM_TRUNK; ++st) {
+          uint8_t* const dst = st == 0 ? p.save_do + size_t(it) * (2 * A_CHUNK_BYTES)
+                                       : p.save_dz + (size_t(it) * NUM_TRUNK + (NUM_TRUNK - st)) * A_TILE_BYTES;
+          const int nchunks = st == 0 ? do_chunks : 4;
+          mbar_wait(full, phase);
+          for (int c = 0; c < nchunks; ++c)
+            bulk_s2g(dst + size_t(c) * A_CHUNK_BYTES + rows_off, sbase + SB_A + c * A_CHUNK_BYTES + rows_off, 64u * 128u);
+          bulk_commit();
+          bulk_wait_read_all();
+          mbar_arrive(free);
+          if (pending >= 0) {
+            bulk_wait_all_but_last();
+            publish();
+          }
+          pending = it;
+          phase ^= 1;
+        }
+      }
+      bulk_wait_all();
+      if (pending >= 0) publish();
     }
     return;
   }
@@ -80,39 +131,57 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
   const uint32_t rows_off = uint32_t(wg) * 64u * 128u;
   constexpr uint64_t A_DESC = make_sdesc_hi(16, 1024, LAYOUT_SW128);
   constexpr uint64_t W_DESC = make_sdesc_hi(16, 512, LAYOUT_SW64);
-  const bool issuer = t == 0;
   RingPos pos;
   float acc[128];
-  // Progress of this warpgroup's stores (wgrad_body.cuh reads it): warpgroup 0 counts in the low, warpgroup 1 in the
-  // high 16 bits of the tile's counter, one per stage (dO, dZ_7 .. dZ_0) whose bulk stores have completed.  A stage
-  // is published when the next one has been committed (wait_group 1), so the issuer does not wait on the store it
-  // just issued.
-  const uint32_t progress_inc = wg == 0 ? 1u : 0x10000u;
-  int pending = -1;                 // tile of the most recent committed, not yet published store group
-  auto publish = [&]() {            // pending's group has completed: its writes are visible to this thread
-    fence_proxy_async_global();
-    red_add_release_gpu(p.progress + pending, progress_inc);
-  };
+  uint32_t afr[64];        // dZ_l as the register A operand of the GEMM for dH_{l-1}
+  uint32_t mw[2][8];       // relu mask words of h_l for the fragment rows fr, fr + 8
 
-  // before rewriting the warpgroup's rows: the bulk store of the previous image has read them
-  auto rows_free = [&]() {
-    if (issuer) bulk_wait_read_all();
-    warpgroup_sync(wg);
+  // the warpgroup's rows of the A tile: wait until the store warp has read the previous stage, and hand a written
+  // stage to it (each thread's writes made visible to the async proxy, then one arrival per thread)
+  // (the __syncwarp reconverges the warp after the spin: without it ptxas serializes every wgmma of the kernel, C7520)
+  uint32_t rows_phase = 0;
+  auto rows_acquire = [&]() {
+    mbar_wait(smem_u32(&rows_free[wg]), rows_phase ^ 1);
+    __syncwarp();
   };
-  // rows written: visible to the async proxy (next GEMM, bulk store); store `nchunks` 64-column chunks of them
-  auto hand_over = [&](uint8_t* dst_tile, int nchunks, int tile) {
+  auto rows_hand_over = [&]() {
     fence_proxy_async_smem();
-    warpgroup_sync(wg);
-    if (issuer) {
-      for (int c = 0; c < nchunks; ++c)
-        bulk_s2g(dst_tile + size_t(c) * A_CHUNK_BYTES + rows_off, sbase + SB_A + c * A_CHUNK_BYTES + rows_off,
-                 64u * 128u);
-      bulk_commit();
-      if (pending >= 0) {
-        bulk_wait_all_but_last();
-        publish();
+    mbar_arrive(smem_u32(&rows_full[wg]));
+    rows_phase ^= 1;
+  };
+  // columns 32c..32c+31 of dZ (afr[8c + i]: k16 step i/4, register i%4) -> the warpgroup's rows of the A tile
+  // (a_tile_offset: rows fr and fr + 8 share the swizzle row & 7 = lane / 4)
+  uint8_t* const share_base = a_tile + uint32_t(64 * wg + fr) * 128u + uint32_t(fc) * 2u;
+  const uint32_t swz = (lane >> 2) << 4;
+  auto write_share = [&](int c) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const uint32_t unit = uint32_t(4 * c + 2 * (i >> 2) + ((i >> 1) & 1)) & 7u;   // 16-byte unit of the column
+      const uint32_t off = uint32_t(c >> 1) * A_CHUNK_BYTES + uint32_t(i & 1) * 1024u + ((unit << 4) ^ swz);
+      *reinterpret_cast<uint32_t*>(share_base + off) = afr[8 * c + i];
+    }
+  };
+  auto load_masks = [&](int l, long long it) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint4* mp = reinterpret_cast<const uint4*>(p.mask + (size_t(l) * mrows + it * TILE_M + 64 * wg + fr + 8 * h) * 8);
+      const uint4 m0 = __ldg(mp), m1 = __ldg(mp + 1);
+      mw[h][0] = m0.x; mw[h][1] = m0.y; mw[h][2] = m0.z; mw[h][3] = m0.w;
+      mw[h][4] = m1.x; mw[h][5] = m1.y; mw[h][6] = m1.z; mw[h][7] = m1.w;
+    }
+  };
+  // dZ = dH * relu'(h): fp16 pack of the accumulator, masked (word c: column 32c+2k <-> bit 15-k, column 32c+2k+1 <->
+  // bit 31-k).  afr[2j + h] holds 8-column group j of row fr + 8h.
+  auto make_dz = [&]() {
+    acc_to_afrag<false>(acc, afr);
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      const int k = (j & 3) * 4 + (fc >> 1);      // pair index inside the 32-column mask word j / 4
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t m = mw[h][j >> 2];
+        afr[2 * j + h] &= ((m >> (15 - k)) & 1u ? 0x0000FFFFu : 0u) | ((m >> (31 - k)) & 1u ? 0xFFFF0000u : 0u);
       }
-      pending = tile;
     }
   };
 
@@ -134,11 +203,13 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
         if (p.sh_deg >= 0) sh_basis(p.sh_deg, __ldg(vd), __ldg(vd + 1), __ldg(vd + 2), basis);
       }
       const float gc[3] = {gq.x, gq.y, gq.z};
-      rows_free();
-      if (hf < do_chunks) {
+      // dO columns 64hf .. 64hf + 63 of row r; the half is a template argument so that the SH basis is indexed with
+      // constants and stays in registers
+      auto build_do = [&](auto half) {
+        constexpr int HF = decltype(half)::value;
 #pragma unroll
         for (int uu = 0; uu < 8; ++uu) {            // 16-byte units of 8 columns
-          const int u = 8 * hf + uu;
+          const int u = 8 * HF + uu;
           uint32_t w[4];
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
@@ -159,12 +230,16 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
           }
           *reinterpret_cast<uint4*>(a_tile + a_tile_offset(r, 8 * u)) = make_uint4(w[0], w[1], w[2], w[3]);
         }
-      }
-      hand_over(p.save_do + size_t(it) * (2 * A_CHUNK_BYTES), do_chunks, int(it));
+      };
+      rows_acquire();
+      if (hf == 0) build_do(std::integral_constant<int, 0>());
+      else if (do_chunks > 1) build_do(std::integral_constant<int, 1>());
+      rows_hand_over();
+      warpgroup_sync(wg);   // every row of dO written before the heads GEMM reads it
     }
-    // ---- GEMM g (heads, then Dense_7 .. Dense_1) -> dH_l -> dZ_l, l = 7 .. 0 ----
-    for (int l = NUM_TRUNK - 1; l >= 0; --l) {
-      const int ns = (l == NUM_TRUNK - 1) ? bwd_head_slots(NH) : 8;
+    // ---- heads GEMM: dH_7 = dO . W_heads, A = the dO rows in shared memory ----
+    {
+      const int ns = bwd_head_slots(NH);
       uint32_t prev = 0;
       wgmma_fence();
       for (int j = 0; j < ns; ++j) {
@@ -174,6 +249,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
         wgmma_m64n256<0, 0>(acc, sdesc(A_DESC, a), sdesc(W_DESC, b), j != 0);
         wgmma_m64n256<0, 0>(acc, sdesc(A_DESC, a + 32), sdesc(W_DESC, b + 32), 1u);
         wgmma_commit();
+        if (j == 0) load_masks(NUM_TRUNK - 1, it);   // loaded while the GEMM runs
         if (j > 0) {
           wgmma_wait<1>();
           ring.release(prev);
@@ -181,36 +257,43 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
         prev = pos.stage;
         pos.advance(BWD_WSLOTS);
       }
-      // relu masks of h_l for the fragment rows (word c: column 32c+2k <-> bit 15-k, column 32c+2k+1 <-> bit 31-k),
-      // loaded while the GEMM runs
-      uint32_t mw[2][8];
+      wgmma_wait<0>();
+      ring.release(prev);
+      make_dz();
+    }
+    // ---- GEMM for dH_l (Dense_{l+1}^T, l = 6 .. 0), A = dZ_{l+1} from registers.  dZ_{l+1} goes to the A tile one
+    // K-slot behind the MMAs that read it and is handed to the store warp at the end of the GEMM. ----
+    for (int l = NUM_TRUNK - 2; l >= 0; --l) {
+      uint32_t prev = 0;
+      wgmma_fence();
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const uint4* mp = reinterpret_cast<const uint4*>(p.mask + (size_t(l) * mrows + it * TILE_M + 64 * wg + fr + 8 * h) * 8);
-        const uint4 m0 = __ldg(mp), m1 = __ldg(mp + 1);
-        mw[h][0] = m0.x; mw[h][1] = m0.y; mw[h][2] = m0.z; mw[h][3] = m0.w;
-        mw[h][4] = m1.x; mw[h][5] = m1.y; mw[h][6] = m1.z; mw[h][7] = m1.w;
+      for (int j = 0; j < 8; ++j) {
+        const uint32_t b = sbase + SB_W + pos.stage * WSLOT_BYTES;
+        ring.wait(pos);
+        wgmma_m64n256_rs(acc, afr[8 * j], afr[8 * j + 1], afr[8 * j + 2], afr[8 * j + 3], sdesc(W_DESC, b), j != 0);
+        wgmma_m64n256_rs(acc, afr[8 * j + 4], afr[8 * j + 5], afr[8 * j + 6], afr[8 * j + 7], sdesc(W_DESC, b + 32), 1u);
+        wgmma_commit();
+        if (j == 0) load_masks(l, it);
+        if (j > 0) {
+          wgmma_wait<1>();
+          ring.release(prev);
+          if (j == 1) rows_acquire();
+          write_share(j - 1);
+        }
+        prev = pos.stage;
+        pos.advance(BWD_WSLOTS);
       }
       wgmma_wait<0>();
       ring.release(prev);
-      rows_free();
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int k = (j & 3) * 4 + (fc >> 1);      // pair index inside the 32-column mask word j / 4
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const uint32_t m = mw[h][j >> 2];
-          const uint32_t keep = ((m >> (15 - k)) & 1u ? 0x0000FFFFu : 0u) | ((m >> (31 - k)) & 1u ? 0xFFFF0000u : 0u);
-          const uint32_t w = pack_f16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]) & keep;
-          *reinterpret_cast<uint32_t*>(a_tile + a_tile_offset(64 * wg + fr + 8 * h, 8 * j + fc)) = w;
-        }
-      }
-      hand_over(p.save_dz + (size_t(it) * NUM_TRUNK + l) * A_TILE_BYTES, 4, int(it));
+      write_share(7);
+      rows_hand_over();
+      make_dz();
     }
-  }
-  if (issuer) {
-    bulk_wait_all();
-    if (pending >= 0) publish();
+    // ---- dZ_0 ----
+    rows_acquire();
+#pragma unroll
+    for (int c = 0; c < 8; ++c) write_share(c);
+    rows_hand_over();
   }
 }
 

@@ -7,8 +7,9 @@
 //   reference path                                      this kernel
 //   -------------------------------------------------   ------------------------------------
 //   model_utils.posenc      (model_utils.py:145-173)    consumer warps -> E tile (smem, fp16)
-//   model_utils.MLP         (model_utils.py:30-94)      wgmma, fp32 accumulators in registers,
-//                                                       ReLU epilogue registers -> smem (next A operand)
+//   model_utils.MLP         (model_utils.py:30-94)      wgmma, fp32 accumulators in registers; fp16: ReLU +
+//                                                       pack into the next layer's register A operand
+//                                                       (x3: ReLU epilogue registers -> smem A tiles)
 //   sh.eval_sh + sigmoid/relu (sh.py:54-109,            heads epilogue (registers -> smem staging)
 //                              models.py:269-281)
 //   NerfModel.eval_points_raw (models.py:143-181)       OUT_RAW / OUT_SIGMA
@@ -17,7 +18,8 @@
 // (one m64n256 accumulator = 128 registers per thread, 232 registers after setmaxnreg), warp 8 = weight producer
 // (cp.async.bulk ring, one 16 KB K-slot per stage; warps 9-11 only hand their registers back).  Both warpgroups
 // consume every stage; a warpgroup reads and rewrites only its own rows of the activation / posenc tiles, so the two
-// synchronise through the weight ring alone and one's epilogue runs under the other's MMAs.  NSPLIT = 3 evaluates
+// synchronise through the weight ring alone.  fp16 chains the layers through registers (the activation tile only
+// stages the heads); the training saves of h_l run one K-slot behind layer l+1's MMAs.  NSPLIT = 3 evaluates
 // with error-compensated fp16 operands (x = hi + lo; lo*hi + hi*lo + hi*hi per K step), the residual parts in a
 // second set of tiles; a stage then holds the K-slot's hi and lo parts (32 KB).
 #include "common.cuh"
@@ -208,11 +210,182 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
   const uint32_t rows_off = uint32_t(wg) * 64u * 128u;     // this warpgroup's 64 rows inside every 128-row chunk
   constexpr uint64_t A_DESC = make_sdesc_hi(16, 1024, LAYOUT_SW128);
   constexpr uint64_t W_DESC = make_sdesc_hi(16, 512, LAYOUT_SW64);
+  static_assert(!SAVE || NSPLIT == 1, "the training forward is fp16");
   RingPos pos;
   float acc[128];
   float hacc[HEADS_N / 2];
+  uint32_t afr[64];        // fp16: the previous layer's ReLU output as the register A operand (acc_to_afrag)
+  long long it = blockIdx.x;
 
-  for (long long it = blockIdx.x; it < num_tiles; it += gridDim.x) {
+  // shared-memory A operand of k16 group pair kk (columns 32kk..32kk+31) of the posenc tile
+  auto e_operand = [&](int kk) {
+    return sbase + SM::E0 + uint32_t(kk >> 1) * A_CHUNK_BYTES + rows_off + uint32_t(kk & 1) * 64u;
+  };
+
+  // Training save of K-slot c's share of h_lh (columns 32c..32c+31) from the A registers that carried it, once the
+  // slot's MMAs have completed: the "T" image (layouts.py: t_tile_offset), in which each warp store of one 8-column
+  // group is one contiguous 128 B core matrix, and mask word c.  Word c covers columns 32c..32c+31: column 32c+2k is
+  // bit 15-k, column 32c+2k+1 is bit 31-k, derived from the fp16 values (h > 0 <=> fp16(h) != 0 up to fp16
+  // underflow).  The four lanes of a quad hold one row's 16 pairs; lane q keeps words 4(q&1)..+3 of row fr + 8(q>>1).
+  auto save_slot = [&](int lh, int c, uint32_t (&maskw)[4]) {
+    uint8_t* const h_glob = p.save_h + (size_t(it) * NUM_TRUNK + lh) * A_TILE_BYTES +
+                            uint32_t(2 * wg + (wq >> 1)) * 16384u + uint32_t(16 * (wq & 1) + int(lane >> 2)) * 16u +
+                            uint32_t(fc) * 2u;
+    uint32_t m[2] = {0u, 0u};
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {            // afr[8c + i]: k16 step i/4 of the slot, register i%4
+      const uint32_t w = afr[8 * c + i];
+      const int h = i & 1;                    // row fr + 8h
+      const int hi8 = (i >> 1) & 1;           // second 8 columns of the k16 step
+      *reinterpret_cast<uint32_t*>(h_glob + uint32_t(4 * c + 2 * (i >> 2) + hi8) * 512u + uint32_t(h) * 128u) = w;
+      const int k = 8 * (i >> 2) + 4 * hi8 + int(lane & 3);   // column pair within the mask word
+      m[h] |= __vminu2(w, 0x00010001u) << (15 - k);           // non-negative fp16 pair -> 0/1 per half
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      m[h] |= __shfl_xor_sync(0xffffffffu, m[h], 1);
+      m[h] |= __shfl_xor_sync(0xffffffffu, m[h], 2);
+    }
+    const uint32_t q = lane & 3;
+    if ((q & 1) == uint32_t(c >> 2)) maskw[c & 3] = (q >> 1) ? m[1] : m[0];
+  };
+
+  // fp16 layer l >= 1 (l = NUM_TRUNK: the heads, into hacc): K-slots 0..7 take h_{l-1} from afr, the bias slot and
+  // layer 5's skip slots the posenc tile.  The first MMA is issued as soon as h_{l-1} is packed; the training save of
+  // h_{l-1} then runs one K-slot behind the MMAs.
+  auto chain_layer = [&](auto& d, const int l) {
+    constexpr bool HEADS = sizeof(d) == sizeof(hacc);
+    const int ns = HEADS ? FWD_HEAD_SLOTS : fwd_slots_of_layer(l);
+    uint32_t maskw[4];
+    uint32_t prev = 0;
+    wgmma_fence();
+#pragma unroll
+    for (int j = 0; j < 10; ++j) {
+      if (j == ns) break;
+      const uint32_t b = sbase + SM::W + pos.stage * SM::STAGE_BYTES;
+      ring.wait(pos);
+      if (j < 8) {
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          const uint32_t* a = afr + 8 * j + 4 * k;
+          const uint64_t bd = sdesc(W_DESC, b + 32u * k);
+          const uint32_t sd = (j != 0 || k != 0) ? 1u : 0u;
+          if constexpr (HEADS) wgmma_m64n80_rs(d, a[0], a[1], a[2], a[3], bd, sd);
+          else wgmma_m64n256_rs(d, a[0], a[1], a[2], a[3], bd, sd);
+        }
+      } else {
+        // the bias slot only multiplies the k16 group [48,64) of the posenc tile (column 63 = 1) with its row k = 31
+        const bool bias_slot = fwd_has_bias_slot(l);
+        const uint32_t a = e_operand(bias_slot ? 1 : j - 8);
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          if (k == 0 && bias_slot) continue;
+          const uint32_t ko = uint32_t(k) * 32u;
+          if constexpr (HEADS) wgmma_m64n80<0, 0>(d, sdesc(A_DESC, a + ko), sdesc(W_DESC, b + ko), 1u);
+          else wgmma_m64n256<0, 0>(d, sdesc(A_DESC, a + ko), sdesc(W_DESC, b + ko), 1u);
+        }
+      }
+      wgmma_commit();
+      if (j > 0) {
+        // the previous K-slot's MMAs are complete: hand its stage back to the producer, save its share of h_{l-1}
+        wgmma_wait<1>();
+        ring.release(prev);
+        if (SAVE && j <= 8) save_slot(l - 1, j - 1, maskw);
+      }
+      prev = pos.stage;
+      pos.advance(SM::STAGES);
+    }
+    wgmma_wait<0>();
+    ring.release(prev);
+    if (SAVE) {
+      const uint32_t q = lane & 3;
+      const long long s = it * TILE_M + 64 * wg + fr + 8 * int(q >> 1);
+      *reinterpret_cast<uint4*>(p.save_mask + (size_t(l - 1) * padded_rows(p.M) + s) * 8 + 4 * (q & 1)) =
+          make_uint4(maskw[0], maskw[1], maskw[2], maskw[3]);
+    }
+  };
+
+  // heads: accumulator fragment -> per-row fp32 staging (column n = packed heads column) inside the warpgroup's own
+  // rows of the activation tile, then one thread per row.  The staging rows are rewritten only after the next tile's
+  // posenc barrier.
+  auto heads_epilogue = [&]() {
+#pragma unroll
+    for (int j = 0; j < HEADS_N / 8; ++j) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float* st = stage_row(a_hi, wg, fr + 8 * h);
+        st[8 * j + fc] = hacc[4 * j + 2 * h];
+        st[8 * j + fc + 1] = hacc[4 * j + 2 * h + 1];
+      }
+    }
+    warpgroup_sync(wg);
+    const int K = p.K;
+    const long long row0 = it * TILE_M + 64 * wg;   // first sample of the warpgroup's rows
+    if (OUTM == OUT_RGBS) {
+      if (t < 64 && row0 + t < p.M) {
+        const long long s = row0 + t;
+        const float* st = stage_row(a_hi, wg, t);
+        float basis[25];
+        const long long vi = (p.src_mode == SRC_RAYS) ? (s < p.M_rays ? s / p.n_per_ray : 0) : s;   // free points: any direction
+        const float* vd = p.viewdirs + 3 * vi;
+        if (p.sh_deg >= 0) sh_basis(p.sh_deg, __ldg(vd), __ldg(vd + 1), __ldg(vd + 2), basis);
+        else basis[0] = 1.f;
+        float pre[3] = {0.f, 0.f, 0.f};
+        for (int k = 0; k < K; ++k) {
+#pragma unroll
+          for (int c = 0; c < 3; ++c) pre[c] = fmaf(basis[k], st[heads_column(k, c)], pre[c]);
+        }
+        float sigma_raw = st[0];
+        float4 o;
+        o.x = 1.f / (1.f + expf(-pre[0]));
+        o.y = 1.f / (1.f + expf(-pre[1]));
+        o.z = 1.f / (1.f + expf(-pre[2]));
+        if (p.sigma_noise != nullptr && (p.src_mode != SRC_RAYS || s < p.M_rays))
+          sigma_raw += __ldg(p.sigma_noise + s);  // add_gaussian_noise
+        o.w = fmaxf(sigma_raw, 0.f);
+        p.out_rgbs[s] = o;
+      }
+    } else if (OUTM == OUT_SIGMA || OUTM == OUT_RAW) {
+      if (t < 64 && row0 + t < p.M) p.out_sigma[row0 + t] = stage_row(a_hi, wg, t)[0];
+      if (OUTM == OUT_RAW) {
+        // reference channel-major order
+        const int C3 = 3 * K;
+        for (int rr = 0; rr < 64 && row0 + rr < p.M; ++rr) {
+          const float* st = stage_row(a_hi, wg, rr);
+          for (int i = t; i < C3; i += 128) p.out_rgb[(row0 + rr) * C3 + i] = st[heads_column_of_output(i, K)];
+        }
+      }
+    } else if (OUTM == OUT_CELL_MEAN) {
+      // extraction step 2 (octree/extraction.py:367-394): out[cell] += cat([raw_rgb, raw_sigma]) / S.
+      const int width = 3 * K + 1;
+      const float inv = 1.0f / float(p.cell_S);
+      auto col_of = [&](int i) { return i == 3 * K ? 0 : heads_column_of_output(i, K); };
+      if ((p.cell_S & 31) == 0) {
+        // 32 consecutive rows belong to one cell: 64 threads per 32-row half sum over rows, one atomic per column
+        const int hf = t >> 6;
+        const long long r0 = row0 + 32 * hf;
+        if (r0 < p.M) {
+          float* dst = p.out_cell + (r0 / p.cell_S) * width;
+          for (int i = t & 63; i < width; i += 64) {
+            const int n = col_of(i);
+            float a = 0.f;
+            for (int rr = 0; rr < 32; ++rr) a += stage_row(a_hi, wg, 32 * hf + rr)[n];
+            atomicAdd(dst + i, a * inv);
+          }
+        }
+      } else {
+        for (int rr = 0; rr < 64 && row0 + rr < p.M; ++rr) {
+          float* dst = p.out_cell + ((row0 + rr) / p.cell_S) * width;
+          for (int i = t; i < width; i += 128) atomicAdd(dst + i, stage_row(a_hi, wg, rr)[col_of(i)] * inv);
+        }
+      }
+    }
+    // reconverge before the next tile's MMAs: after the cell-mean loops ptxas otherwise serializes every wgmma of the
+    // kernel (C7520).  The x3 forwards keep their instruction stream.
+    if (NSPLIT == 1) __syncwarp();
+  };
+
+  for (; it < num_tiles; it += gridDim.x) {
     // ---- positional encoding of the warpgroup's 64 rows (two threads per row, four 16-byte units each) ----
     {
       const int r = 64 * wg + (t & 63);
@@ -224,46 +397,19 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
       fence_proxy_async_smem();
       warpgroup_sync(wg);
     }
-    for (int l = 0; l <= NUM_TRUNK; ++l) {
-      const bool heads = l == NUM_TRUNK;
-      const int ns = heads ? FWD_HEAD_SLOTS : fwd_slots_of_layer(l);
+    if constexpr (NSPLIT == 1) {
+      // ---- fp16: layer 0 from the posenc tile, then every layer's activations stay in registers ----
       uint32_t prev = 0;
       wgmma_fence();
-      for (int j = 0; j < ns; ++j) {
-        // A operand of K-slot j: the previous layer's activations, or the posenc tile for layer 0, the skip slots
-        // of layer 5, and the bias slot (j == 8) of every other layer, which only multiplies the k16 group
-        // [48,64) of the posenc tile (column 63 = 1) with its row k = 31.
-        const bool bias_slot = (heads || fwd_has_bias_slot(l)) && j == 8;
-        const bool from_e = (l == 0) || j >= 8;
-        const int kk = bias_slot ? 1 : ((l == SKIP_LAYER && j >= 8) ? j - 8 : j);
-        const uint32_t a_off = uint32_t(kk >> 1) * A_CHUNK_BYTES + rows_off + uint32_t(kk & 1) * 64u;
-        const uint32_t ah = sbase + (from_e ? SM::E0 : SM::A0) + a_off;
-        const uint32_t al = sbase + (from_e ? SM::E1 : SM::A1) + a_off;
-        const uint32_t bh = sbase + SM::W + pos.stage * SM::STAGE_BYTES;
-        const uint32_t bl = bh + WSLOT_BYTES;   // x3 only
-        ring.wait(pos);
 #pragma unroll
-        for (int k = 0; k < 2; ++k) {
-          if (k == 0 && bias_slot) continue;
-          const uint32_t sd = (j != 0 || k != 0) ? 1u : 0u;
-          const uint32_t ko = uint32_t(k) * 32u;   // k16 step: +32 bytes inside the swizzled rows
-          if (heads) {
-            if (NSPLIT == 3) {
-              wgmma_m64n80<0, 0>(hacc, sdesc(A_DESC, al + ko), sdesc(W_DESC, bh + ko), sd);
-              wgmma_m64n80<0, 0>(hacc, sdesc(A_DESC, ah + ko), sdesc(W_DESC, bl + ko), 1u);
-            }
-            wgmma_m64n80<0, 0>(hacc, sdesc(A_DESC, ah + ko), sdesc(W_DESC, bh + ko), NSPLIT == 3 ? 1u : sd);
-          } else {
-            if (NSPLIT == 3) {
-              wgmma_m64n256<0, 0>(acc, sdesc(A_DESC, al + ko), sdesc(W_DESC, bh + ko), sd);
-              wgmma_m64n256<0, 0>(acc, sdesc(A_DESC, ah + ko), sdesc(W_DESC, bl + ko), 1u);
-            }
-            wgmma_m64n256<0, 0>(acc, sdesc(A_DESC, ah + ko), sdesc(W_DESC, bh + ko), NSPLIT == 3 ? 1u : sd);
-          }
-        }
+      for (int j = 0; j < 2; ++j) {
+        const uint32_t a = e_operand(j);
+        const uint32_t b = sbase + SM::W + pos.stage * SM::STAGE_BYTES;
+        ring.wait(pos);
+        wgmma_m64n256<0, 0>(acc, sdesc(A_DESC, a), sdesc(W_DESC, b), j != 0);
+        wgmma_m64n256<0, 0>(acc, sdesc(A_DESC, a + 32), sdesc(W_DESC, b + 32), 1u);
         wgmma_commit();
         if (j > 0) {
-          // the previous K-slot's MMAs are complete: hand its stage back to the producer
           wgmma_wait<1>();
           ring.release(prev);
         }
@@ -272,134 +418,83 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
       }
       wgmma_wait<0>();
       ring.release(prev);
+      // ReLU + fp16 pack of the accumulator (the bias was accumulated by the tensor cores) into the next A operand
+      acc_to_afrag<true>(acc, afr);
+      for (int l = 1; l < NUM_TRUNK; ++l) {
+        chain_layer(acc, l);
+        acc_to_afrag<true>(acc, afr);
+      }
+      chain_layer(hacc, NUM_TRUNK);
+      heads_epilogue();
+    } else {
+      // ---- x3: every operand from shared memory; the epilogue rewrites the warpgroup's rows of the A tiles ----
+      for (int l = 0; l <= NUM_TRUNK; ++l) {
+        const bool heads = l == NUM_TRUNK;
+        const int ns = heads ? FWD_HEAD_SLOTS : fwd_slots_of_layer(l);
+        uint32_t prev = 0;
+        wgmma_fence();
+        for (int j = 0; j < ns; ++j) {
+          // A operand of K-slot j: the previous layer's activations, or the posenc tile for layer 0, the skip slots
+          // of layer 5, and the bias slot (j == 8) of every other layer, which only multiplies the k16 group
+          // [48,64) of the posenc tile (column 63 = 1) with its row k = 31.
+          const bool bias_slot = (heads || fwd_has_bias_slot(l)) && j == 8;
+          const bool from_e = (l == 0) || j >= 8;
+          const int kk = bias_slot ? 1 : ((l == SKIP_LAYER && j >= 8) ? j - 8 : j);
+          const uint32_t a_off = uint32_t(kk >> 1) * A_CHUNK_BYTES + rows_off + uint32_t(kk & 1) * 64u;
+          const uint32_t ah = sbase + (from_e ? SM::E0 : SM::A0) + a_off;
+          const uint32_t al = sbase + (from_e ? SM::E1 : SM::A1) + a_off;
+          const uint32_t bh = sbase + SM::W + pos.stage * SM::STAGE_BYTES;
+          const uint32_t bl = bh + WSLOT_BYTES;
+          ring.wait(pos);
+#pragma unroll
+          for (int k = 0; k < 2; ++k) {
+            if (k == 0 && bias_slot) continue;
+            const uint32_t sd = (j != 0 || k != 0) ? 1u : 0u;
+            const uint32_t ko = uint32_t(k) * 32u;   // k16 step: +32 bytes inside the swizzled rows
+            if (heads) {
+              wgmma_m64n80<0, 0>(hacc, sdesc(A_DESC, al + ko), sdesc(W_DESC, bh + ko), sd);
+              wgmma_m64n80<0, 0>(hacc, sdesc(A_DESC, ah + ko), sdesc(W_DESC, bl + ko), 1u);
+              wgmma_m64n80<0, 0>(hacc, sdesc(A_DESC, ah + ko), sdesc(W_DESC, bh + ko), 1u);
+            } else {
+              wgmma_m64n256<0, 0>(acc, sdesc(A_DESC, al + ko), sdesc(W_DESC, bh + ko), sd);
+              wgmma_m64n256<0, 0>(acc, sdesc(A_DESC, ah + ko), sdesc(W_DESC, bl + ko), 1u);
+              wgmma_m64n256<0, 0>(acc, sdesc(A_DESC, ah + ko), sdesc(W_DESC, bh + ko), 1u);
+            }
+          }
+          wgmma_commit();
+          if (j > 0) {
+            // the previous K-slot's MMAs are complete: hand its stage back to the producer
+            wgmma_wait<1>();
+            ring.release(prev);
+          }
+          prev = pos.stage;
+          pos.advance(SM::STAGES);
+        }
+        wgmma_wait<0>();
+        ring.release(prev);
 
-      if (!heads) {
-        // ---- trunk epilogue: ReLU + fp16 pack straight from the accumulator fragment into the next A operand
-        // (the bias was accumulated by the tensor cores).  Only this warpgroup's MMAs read these rows. ----
+        if (!heads) {
+          // ---- trunk epilogue: ReLU + hi/lo fp16 split straight from the accumulator fragment into the next A
+          // operands (the bias was accumulated by the tensor cores).  Only this warpgroup's MMAs read these rows. ----
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
+          for (int j = 0; j < 32; ++j) {
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int row = 64 * wg + fr + 8 * h;
-            const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-            const uint32_t off = a_tile_offset(row, 8 * j + fc);
-            const uint32_t w = pack_f16x2_relu(v0, v1);
-            *reinterpret_cast<uint32_t*>(a_hi + off) = w;
-            if (NSPLIT == 3) {
+            for (int h = 0; h < 2; ++h) {
+              const int row = 64 * wg + fr + 8 * h;
+              const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+              const uint32_t off = a_tile_offset(row, 8 * j + fc);
+              const uint32_t w = pack_f16x2_relu(v0, v1);
+              *reinterpret_cast<uint32_t*>(a_hi + off) = w;
               const float2 hv = unpack_f16x2(w);
               *reinterpret_cast<uint32_t*>(a_lo + off) = pack_f16x2(fmaxf(v0, 0.f) - hv.x, fmaxf(v1, 0.f) - hv.y);
             }
           }
+          fence_proxy_async_smem();
+          warpgroup_sync(wg);
+          continue;
         }
-        fence_proxy_async_smem();
-        warpgroup_sync(wg);
-        if (SAVE) {
-          // Training saves: every thread reads half of one row of the finished tile back from shared memory (the
-          // next layer's MMAs only read it too), stores it to global memory in the "T" layout (layouts.py:
-          // t_tile_offset; 512 contiguous bytes per warp store) that mlp_wgrad contracts MN-major without swizzle,
-          // and derives the ReLU mask from the fp16 values (h > 0 <=> fp16(h) != 0 up to fp16 underflow).  Mask
-          // word c covers columns 32c..32c+31: column 32c+2k is bit 15-k, column 32c+2k+1 is bit 31-k.
-          const int row = 64 * wg + (t & 63);
-          const int c0 = 4 * (t >> 6);
-          uint8_t* const h_glob = p.save_h + (size_t(it) * NUM_TRUNK + l) * A_TILE_BYTES;
-          uint32_t maskw[4];
-#pragma unroll
-          for (int cc = 0; cc < 4; ++cc) {
-            const int c = c0 + cc;
-            uint32_t mbits = 0;
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-              const uint4 q = *reinterpret_cast<const uint4*>(a_hi + a_tile_offset(row, 32 * c + 8 * u));
-              *reinterpret_cast<uint4*>(h_glob + uint32_t(row >> 5) * 16384u + uint32_t(c * 4 + u) * 512u +
-                                        uint32_t(row & 31) * 16u) = q;
-              const uint32_t qw[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-              for (int i = 0; i < 4; ++i)   // non-negative fp16 pair -> 0/1 per half, shifted in
-                mbits = (mbits << 1) + __vminu2(qw[i], 0x00010001u);
-            }
-            maskw[cc] = mbits;
-          }
-          const long long s = it * TILE_M + row;
-          *reinterpret_cast<uint4*>(p.save_mask + (size_t(l) * padded_rows(p.M) + s) * 8 + c0) =
-              make_uint4(maskw[0], maskw[1], maskw[2], maskw[3]);
-        }
-        continue;
+        heads_epilogue();
       }
-
-      // -------------------------------- heads ------------------------------------------
-      // accumulator fragment -> per-row fp32 staging (column n = packed heads column), then one thread per row
-#pragma unroll
-      for (int j = 0; j < HEADS_N / 8; ++j) {
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          float* st = stage_row(a_hi, wg, fr + 8 * h);
-          st[8 * j + fc] = hacc[4 * j + 2 * h];
-          st[8 * j + fc + 1] = hacc[4 * j + 2 * h + 1];
-        }
-      }
-      warpgroup_sync(wg);
-      const int K = p.K;
-      const long long row0 = it * TILE_M + 64 * wg;   // first sample of the warpgroup's rows
-      if (OUTM == OUT_RGBS) {
-        if (t < 64 && row0 + t < p.M) {
-          const long long s = row0 + t;
-          const float* st = stage_row(a_hi, wg, t);
-          float basis[25];
-          const long long vi = (p.src_mode == SRC_RAYS) ? (s < p.M_rays ? s / p.n_per_ray : 0) : s;   // free points: any direction
-          const float* vd = p.viewdirs + 3 * vi;
-          if (p.sh_deg >= 0) sh_basis(p.sh_deg, __ldg(vd), __ldg(vd + 1), __ldg(vd + 2), basis);
-          else basis[0] = 1.f;
-          float pre[3] = {0.f, 0.f, 0.f};
-          for (int k = 0; k < K; ++k) {
-#pragma unroll
-            for (int c = 0; c < 3; ++c) pre[c] = fmaf(basis[k], st[heads_column(k, c)], pre[c]);
-          }
-          float sigma_raw = st[0];
-          float4 o;
-          o.x = 1.f / (1.f + expf(-pre[0]));
-          o.y = 1.f / (1.f + expf(-pre[1]));
-          o.z = 1.f / (1.f + expf(-pre[2]));
-          if (p.sigma_noise != nullptr && (p.src_mode != SRC_RAYS || s < p.M_rays))
-            sigma_raw += __ldg(p.sigma_noise + s);  // add_gaussian_noise
-          o.w = fmaxf(sigma_raw, 0.f);
-          p.out_rgbs[s] = o;
-        }
-      } else if (OUTM == OUT_SIGMA || OUTM == OUT_RAW) {
-        if (t < 64 && row0 + t < p.M) p.out_sigma[row0 + t] = stage_row(a_hi, wg, t)[0];
-        if (OUTM == OUT_RAW) {
-          // reference channel-major order
-          const int C3 = 3 * K;
-          for (int rr = 0; rr < 64 && row0 + rr < p.M; ++rr) {
-            const float* st = stage_row(a_hi, wg, rr);
-            for (int i = t; i < C3; i += 128) p.out_rgb[(row0 + rr) * C3 + i] = st[heads_column_of_output(i, K)];
-          }
-        }
-      } else if (OUTM == OUT_CELL_MEAN) {
-        // extraction step 2 (octree/extraction.py:367-394): out[cell] += cat([raw_rgb, raw_sigma]) / S.
-        const int width = 3 * K + 1;
-        const float inv = 1.0f / float(p.cell_S);
-        auto col_of = [&](int i) { return i == 3 * K ? 0 : heads_column_of_output(i, K); };
-        if ((p.cell_S & 31) == 0) {
-          // 32 consecutive rows belong to one cell: 64 threads per 32-row half sum over rows, one atomic per column
-          const int hf = t >> 6;
-          const long long r0 = row0 + 32 * hf;
-          if (r0 < p.M) {
-            float* dst = p.out_cell + (r0 / p.cell_S) * width;
-            for (int i = t & 63; i < width; i += 64) {
-              const int n = col_of(i);
-              float a = 0.f;
-              for (int rr = 0; rr < 32; ++rr) a += stage_row(a_hi, wg, 32 * hf + rr)[n];
-              atomicAdd(dst + i, a * inv);
-            }
-          }
-        } else {
-          for (int rr = 0; rr < 64 && row0 + rr < p.M; ++rr) {
-            float* dst = p.out_cell + ((row0 + rr) / p.cell_S) * width;
-            for (int i = t; i < width; i += 128) atomicAdd(dst + i, stage_row(a_hi, wg, rr)[col_of(i)] * inv);
-          }
-        }
-      }
-      // the staging rows are rewritten only by the next tile's layer-0 epilogue, after the posenc barrier
     }
   }
 }

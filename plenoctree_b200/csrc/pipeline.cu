@@ -45,9 +45,10 @@ size_t up(size_t x) { return (x + 1023) / 1024 * 1024; }
 long long tiles_for(long long M) { return padded_rows(M) / TILE_M; }
 
 // SMs (out of an H100 SXM's 132) that run mlp_bwd during the backward; mlp_wgrad runs on the others.  Step time of
-// bench.py on an H100 80 GB HBM3 at a 400 W power limit with dgrad on 66 / 72 / 78 SMs: 10.2 / 10.4 / 13.4 ms (parent
-// without the concurrent backward: 10.7 ms).  A wgrad side that cannot keep up with dgrad misses L2 and runs a tail
-// alone; wgrad_assign_roles' even role counts make neighbouring splits differ a lot (DESIGN.md section 6).
+// bench.py on an H100 80 GB HBM3 at a 400 W power limit with dgrad on 54 / 58 / 60 / 62 / 64 / 66 / 70 SMs (register-A
+// dgrad, two runs each): 10.2 / 10.4 / 14.0 / 14.2 / 14.3 / 9.75-9.94 / 10.4-10.45 ms.  A wgrad side that cannot keep
+// up with dgrad misses L2 and runs a tail alone; wgrad_assign_roles' even role counts make neighbouring splits differ a
+// lot (DESIGN.md section 6).
 constexpr int DGRAD_SMS_OF_132 = 66;
 
 // deterministic carve of the caller-provided workspace
