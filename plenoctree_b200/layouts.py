@@ -236,7 +236,7 @@ def padded_rows(M):
     return (M + 511) // 512 * 512
 
 
-def train_workspace_views(cfg, n_rays, sparsity_on):
+def train_workspace_views(cfg, n_rays, sparsity_on, training=True):
     """Byte layout of the training workspace of `cfg` (a RenderConfig or anything with its fields) for a
     pob_loss_and_grad call over `n_rays` rays; `sparsity_on` = the call carries the sparsity points (weight > 0).
 
@@ -246,7 +246,10 @@ def train_workspace_views(cfg, n_rays, sparsity_on):
     (uint8 tile images), mask [8, rows, 8] and progress [tiles] (uint32 words), sized for this call, plus the call's
     row counts: N samples per ray, M_rays, M (with the sparsity rows, which ride behind the rays of the last level),
     rows (= padded_rows(M)) and tiles.  Buffers are carved for cfg.max_rays; the mask's per-layer stride is the call's
-    padded row count."""
+    padded row count.
+
+    training=False: the render workspace of pob_render_rays (pob_workspace_bytes(cfg, 0)).  Each level then holds
+    only z, rgbs, weights, comp, disp and acc, no sparsity rows, and partials is empty."""
     R = int(cfg.max_rays)
     nc, nf, nsp = int(cfg.num_coarse_samples), int(cfg.num_fine_samples), int(cfg.sparsity_npoints)
     Ns = [nc, nc + nf if nf > 0 else 0]
@@ -263,13 +266,13 @@ def train_workspace_views(cfg, n_rays, sparsity_on):
 
     for lv in range(2):
         Mr_cap = R * Ns[lv]
-        M_cap = Mr_cap + (nsp if lv == last else 0)
+        M_cap = Mr_cap + (nsp if (training and lv == last) else 0)
         tiles_cap = caps[lv] = padded_rows(M_cap) // TILE_M
         if Mr_cap == 0:
             continue
         N = Ns[lv]
         M_rays = n_rays * N
-        M = M_rays + (nsp if (lv == last and sparsity_on) else 0)
+        M = M_rays + (nsp if (training and lv == last and sparsity_on) else 0)
         rows = padded_rows(M)
         tiles = rows // TILE_M
         v = dict(N=N, M_rays=M_rays, M=M, rows=rows, tiles=tiles)
@@ -279,6 +282,9 @@ def train_workspace_views(cfg, n_rays, sparsity_on):
         v["comp"] = (take(12 * R), (n_rays, 3))
         v["disp"] = (take(4 * R), (n_rays,))
         v["acc"] = (take(4 * R), (n_rays,))
+        if not training:
+            levels.append(v)
+            continue
         v["G"] = (take(16 * M_cap), (M, 4))
         v["H"] = (take(tiles_cap * NUM_TRUNK * A_TILE_BYTES), (tiles, NUM_TRUNK, A_TILE_BYTES))
         v["E"] = (take(tiles_cap * E_TILE_BYTES), (tiles, E_TILE_BYTES))
@@ -286,6 +292,8 @@ def train_workspace_views(cfg, n_rays, sparsity_on):
         v["DO"] = (take(tiles_cap * DO_TILE_BYTES), (tiles, DO_TILE_BYTES))
         v["mask"] = (take(NUM_TRUNK * tiles_cap * TILE_M * 8 * 4), (NUM_TRUNK, rows, 8))
         levels.append(v)
+    if not training:
+        return dict(total=off, levels=levels, partials=[])
     partials = [take(4 * WG_MAX_CTAS * WG_PARTIAL_FLOATS) for _ in range(2)]
     progress = take(4 * sum(caps))   # mlp_bwd -> mlp_wgrad progress counters, level 0's tiles then level 1's
     for v, first in zip(levels, (0, caps[0])):

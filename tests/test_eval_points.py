@@ -89,25 +89,30 @@ def test_eval_points_raw_vs_reference_golden(golden_dir, name, sh_deg):
 def test_ragged_sizes_and_sigma_only(m):
     from oracle import nerf_sh_oracle as O
     from plenoctree_b200 import ops
+    from plenoctree_b200._lib import check, lib, ptr, stream_ptr
     sh_deg = 3
     flat = O.init_flat_params(sh_deg, 11, bias_scale=0.05)
     blob = _blob(flat, sh_deg)
     rs = np.random.RandomState(m)
     pts_np = rs.uniform(-1.5, 1.5, size=(m, 3)).astype(np.float32)
     pts = torch.from_numpy(pts_np).cuda()
-    guard = torch.full((m + 64, 48), 7.0, device="cuda")  # detect out-of-bounds row writes
     for prec, tol in ((ops.PREC_FP16X3, TOL_X3), (ops.PREC_FP16, TOL_FP16_ANY)):
         rgb, sig = ops.eval_points_raw(blob, sh_deg, pts, precision=prec)
         _, sig_only = ops.eval_points_raw(blob, sh_deg, pts, want_rgb=False, precision=prec)
+        # the same call into outputs with 64 guard rows behind them: detects out-of-bounds row writes
+        guard = torch.full((m + 64, 48), 7.0, device="cuda")
+        sguard = torch.full((m + 64,), 7.0, device="cuda")
+        check(lib.pob_eval_points_raw(ptr(blob), sh_deg, ptr(pts), m, ptr(guard), ptr(sguard), prec, stream_ptr()))
         torch.cuda.synchronize()
         assert torch.equal(sig, sig_only)
+        assert torch.equal(guard[:m], rgb) and torch.equal(sguard[:m], sig[:, 0])
+        assert bool((guard[m:] == 7.0).all()) and bool((sguard[m:] == 7.0).all())
         idx = np.unique(np.concatenate([np.arange(min(m, 300)), np.arange(max(0, m - 300), m)]))
         with torch.no_grad():
             rgb_o, sig_o = O.eval_points_raw(O.unflatten(flat, sh_deg), torch.from_numpy(pts_np[idx]))
         assert _relmax(rgb.cpu().numpy()[idx], rgb_o.numpy()) < tol
         assert _relmax(sig.cpu().numpy()[idx], sig_o.numpy()) < tol
         assert torch.isfinite(rgb).all() and torch.isfinite(sig).all()
-    assert float(guard.min()) == 7.0
 
 
 def test_empty_input_is_a_noop():

@@ -83,6 +83,37 @@ def test_workspace_mirror_matches_library():
     assert n > 1000
 
 
+def test_render_workspace_mirror_matches_library():
+    """train_workspace_views(training=False) reproduces carve() for pob_render_rays: same total as
+    pob_workspace_bytes(cfg, 0) (the sparsity point count must not change it), six buffers per level, no overlap."""
+    from plenoctree_b200._lib import RenderConfig, lib
+    from plenoctree_b200.nerf.models import ctypes_ref
+    n = 0
+    for sh in range(-1, 5):
+        for nc, nf in ((3, 0), (64, 0), (3, 5), (64, 128), (64, 192), (256, 0), (100, 156)):
+            for nsp in (0, 300):
+                for R in (1, 40, 4096):
+                    cfg = RenderConfig(sh, nc, nf, 1, R, nsp)
+                    want = int(lib.pob_workspace_bytes(ctypes_ref(cfg), 0))
+                    for n_rays in sorted({1, (R + 1) // 2, R}):
+                        v = L.train_workspace_views(cfg, n_rays, True, training=False)
+                        assert v["total"] == want, (sh, nc, nf, nsp, R)
+                        assert len(v["levels"]) == (2 if nf else 1) and v["partials"] == []
+                        ext = []
+                        for lv in v["levels"]:
+                            assert sorted(k for k in lv if isinstance(lv[k], tuple)) == \
+                                ["acc", "comp", "disp", "rgbs", "weights", "z"]
+                            assert lv["M"] == lv["M_rays"] == n_rays * lv["N"]
+                            for name in ("z", "rgbs", "weights", "comp", "disp", "acc"):
+                                off, shape = lv[name]
+                                ext.append((off, off + int(np.prod(shape)) * 4))
+                        ext.sort()
+                        for (a0, a1), (b0, _) in zip(ext, ext[1:] + [(want, 0)]):
+                            assert a0 % 1024 == 0 and a1 <= b0
+                        n += 1
+    assert n > 200
+
+
 def test_mask_codec_roundtrip():
     """decode_mask inverts mlp_fwd's bit-shifting store (column 32c+2k -> bit 15-k, 32c+2k+1 -> bit 31-k)."""
     rs = np.random.RandomState(0)
@@ -137,13 +168,15 @@ def _params(sh_deg, seed):
 class Case:
     # sparsity_weight: 100x the training default, so that the sparsity rows (which ride in the last tiles of the last
     # level) carry gradients of the same order as the ray samples and a lost sparsity tile is visible in every tensor
-    def __init__(self, sh, R, nc, nf, nsp, noise=False, seed=17, sparsity_weight=0.1):
+    # sp_radius: the sparsity points are drawn in [-sp_radius, sp_radius]^3 (train.py's sparsity_radius)
+    def __init__(self, sh, R, nc, nf, nsp, noise=False, seed=17, sparsity_weight=0.1, sp_radius=1.5):
         self.sh, self.R, self.nc, self.nf, self.nsp, self.noise = sh, R, nc, nf, nsp, noise
-        self.seed, self.sparsity_weight = seed, sparsity_weight
+        self.seed, self.sparsity_weight, self.sp_radius = seed, sparsity_weight, sp_radius
 
     @property
     def name(self):
-        return (f"sh{self.sh}_R{self.R}_{self.nc}+{self.nf}_nsp{self.nsp}" + ("_noise" if self.noise else ""))
+        return (f"sh{self.sh}_R{self.R}_{self.nc}+{self.nf}_nsp{self.nsp}" + ("_noise" if self.noise else "")
+                + (f"_r{self.sp_radius:g}" if self.sp_radius != 1.5 else ""))
 
     def inputs(self, n):
         from plenoctree_b200.nerf.rays import random_rays_np
@@ -151,7 +184,8 @@ class Case:
         rs = np.random.RandomState(self.seed + 1)
         t_rand = rs.uniform(0, 1, size=(n, self.nc)).astype(np.float32)
         u = rs.uniform(0, 1, size=(n, self.nf)).astype(np.float32) if self.nf else None
-        sp = rs.uniform(-1.5, 1.5, size=(self.nsp, 3)).astype(np.float32) if self.nsp else None
+        r = self.sp_radius
+        sp = rs.uniform(-r, r, size=(self.nsp, 3)).astype(np.float32) if self.nsp else None
         noise = None
         if self.noise:
             noise = (rs.normal(size=(n, self.nc)).astype(np.float32) * 0.5,
