@@ -192,7 +192,8 @@ class N3Tree:
         depth = self.leaf_depths(leaves).astype(f32)
         corn_unit = self._corners_exact(leaves)
         corn = ((corn_unit - self.offset) / self.invradius).astype(f32)
-        length = (np.exp2(-depth - f32(1.0))[:, None] / self.invradius).astype(f32)
+        length = (np.power(np.float64(self.N), -depth.astype(np.float64) - 1.0).astype(f32)[:, None]
+                  / self.invradius).astype(f32)   # N^-(depth+1); exact for N = 2
         return (corn[:, None, :] + uniforms.astype(f32) * length[:, None, :]).astype(f32)
 
     def _corners_exact(self, leaves):
@@ -310,10 +311,11 @@ def _leaf_color_pre(tree, basis, node, ijk, basis_dim, rgba):
 
 
 def volume_render(tree, origins, dirs, vdirs, step_size=1e-3, background_brightness=1.0, sigma_thresh=0.0,
-                  stop_thresh=0.0, return_steps=False):
+                  stop_thresh=0.0, return_steps=False, _record=None):
     """rt_kernel.cu `trace_ray` (forward of svox.VolumeRenderer; octree/optimization.py:178,202,
     octree/nerf/utils.py:472).  fast=True in svox sets sigma_thresh = stop_thresh = 1e-2.
-    -> rgb [R,3] (and the number of leaf visits / contributing visits per ray)."""
+    -> rgb [R,3] (and the number of leaf visits / contributing visits per ray).
+    `_record` (a dict, see march_visits) receives every visit of the march as it happens."""
     rgba = tree.data_format is None or str(tree.data_format).upper().startswith("RGBA")
     K = 1 if rgba else (tree.data_dim - 1) // 3
     R = np.asarray(origins).shape[0]
@@ -337,6 +339,8 @@ def volume_render(tree, origins, dirs, vdirs, step_size=1e-3, background_brightn
         delta_t = (t_sub + f32(step_size)).astype(f32)
         sigma = tree.data[node, ijk[:, 0], ijk[:, 1], ijk[:, 2], tree.data_dim - 1]
         visits[a] += 1
+        if _record is not None:
+            _record["steps"].append((a, tree.pack_index(node, ijk), delta_t))
         h = sigma > f32(sigma_thresh)
         if h.any():
             ah = a[h]
@@ -356,9 +360,33 @@ def volume_render(tree, origins, dirs, vdirs, step_size=1e-3, background_brightn
         active = active & ~done_full & (t < tmax)
     bg = ~miss & ~done_full
     out[bg] = (out[bg] + light[bg][:, None] * f32(background_brightness)).astype(f32)
+    if _record is not None:
+        _record.update(delta_scale=delta_scale, miss=miss, stopped=done_full)
     if return_steps:
         return out, visits, hits
     return out
+
+
+def march_visits(tree, origins, dirs, vdirs, step_size=1e-3, background_brightness=1.0, sigma_thresh=0.0,
+                 stop_thresh=0.0):
+    """The leaf visits of `volume_render`'s float32 march (the same march, recorded as it runs), ray by ray in march
+    order: dict of
+        ray [V] int64, leaf [V] int64 (packed leaf index), delta_t [V] float32   one entry per visit
+        delta_scale [R] float32, miss [R] bool (the ray misses the box), stopped [R] bool (early termination)
+        rgb [R,3], visits [R], hits [R]                                          volume_render's return values
+    A ray's march depends on the tree data only through early termination (stop_thresh > 0)."""
+    rec = {"steps": []}
+    rgb, visits, hits = volume_render(tree, origins, dirs, vdirs, step_size, background_brightness, sigma_thresh,
+                                      stop_thresh, return_steps=True, _record=rec)
+    steps = rec.pop("steps")
+    if steps:
+        ray, leaf, dt = (np.concatenate([s[i] for s in steps]) for i in range(3))
+    else:
+        ray, leaf, dt = np.zeros(0, np.int64), np.zeros(0, np.int64), np.zeros(0, f32)
+    order = np.argsort(ray, kind="stable")           # iterations were appended in march order
+    rec.update(ray=ray[order].astype(np.int64), leaf=leaf[order].astype(np.int64), delta_t=dt[order].astype(f32),
+               rgb=rgb, visits=visits, hits=hits)
+    return rec
 
 
 def volume_render_backward(tree, origins, dirs, vdirs, grad_out, step_size=1e-3, background_brightness=1.0):

@@ -319,27 +319,23 @@ def test_optimization_loop_matches_executed_reference(golden_dir):
     assert np.abs(best_data - z["data_best"]).max() < 2e-5 * np.abs(z["data_best"]).max()
 
 
-@pytest.mark.gpu
-def test_query_and_tree_build_bit_exact():
+def assert_device_tree_build_matches(otree, refines, radius, center, rs, query_box=2.0):
+    """A device N3Tree refined by the same sequence of `tree[points].refine()` calls as the oracle tree `otree`
+    (refines: float32 [n,3] world-point arrays, one call each) has the oracle's topology bit for bit; query_packed is
+    bit-exact on points of [-query_box, query_box]^3 around the box centre, leaves / depths are identical and sample
+    agrees."""
     import torch
     from plenoctree_b200.octree import N3Tree
-    rs = np.random.RandomState(1)
-    L = 4
-    reso = 2 ** (L + 1)
-    mask = rs.rand(reso, reso, reso) < 0.08
-    otree, grid = OO.build_tree_from_grid(mask, L, [1.5, 1.2, 1.0], [0.1, 0.0, -0.2], 49, "SH16", refine_chunk=700)
-    tree = N3Tree(N=2, data_dim=49, depth_limit=L, init_reserve=16, geom_resize_fact=1.0, radius=[1.5, 1.2, 1.0],
-                  center=[0.1, 0.0, -0.2], data_format="SH16")
-    g = torch.from_numpy(grid).cuda()
-    for _ in range(L - 1):
-        tree[g].refine()
-    for j in range(0, g.shape[0], 700):
-        tree[g[j:j + 700]].refine()
+    L = otree.depth_limit
+    tree = N3Tree(N=otree.N, data_dim=otree.data_dim, depth_limit=L, init_reserve=16, geom_resize_fact=1.0,
+                  radius=radius, center=center, data_format=otree.data_format)
+    for pts in refines:
+        tree[torch.from_numpy(pts).cuda()].refine()
     n = otree.n_internal
-    assert tree.n_internal == n and tree.max_depth == L
+    assert tree.n_internal == n and tree.max_depth == otree.max_depth == L
     assert (tree.child[:n].cpu().numpy() == otree.child[:n]).all()
     assert (tree.parent_depth[:n].cpu().numpy() == otree.parent_depth[:n]).all()
-    pts = rs.uniform(-2, 2, size=(5000, 3)).astype(np.float32)
+    pts = (np.asarray(center, dtype=np.float32) + rs.uniform(-query_box, query_box, size=(5000, 3))).astype(np.float32)
     node, ijk, _, _ = otree.query(pts)
     want = otree.pack_index(node, ijk)
     got = tree.query_packed(torch.from_numpy(pts).cuda()).cpu().numpy()
@@ -353,6 +349,18 @@ def test_query_and_tree_build_bit_exact():
     got = tree[torch.from_numpy(sel).cuda()].sample(5, torch.from_numpy(u).cuda()).cpu().numpy()
     want = otree.sample(lv[sel], 5, u)
     np.testing.assert_allclose(got, want, rtol=0, atol=1e-6)
+    return tree
+
+
+@pytest.mark.gpu
+def test_query_and_tree_build_bit_exact():
+    rs = np.random.RandomState(1)
+    L = 4
+    reso = 2 ** (L + 1)
+    mask = rs.rand(reso, reso, reso) < 0.08
+    otree, grid = OO.build_tree_from_grid(mask, L, [1.5, 1.2, 1.0], [0.1, 0.0, -0.2], 49, "SH16", refine_chunk=700)
+    refines = [grid] * (L - 1) + [grid[j:j + 700] for j in range(0, grid.shape[0], 700)]
+    assert_device_tree_build_matches(otree, refines, [1.5, 1.2, 1.0], [0.1, 0.0, -0.2], rs)
 
 
 @pytest.mark.gpu
