@@ -113,38 +113,42 @@ cudaError_t launch_mlp_bwd(const BwdParams& p, int num_ctas, cudaStream_t stream
 // ---- mlp_wgrad.cu ---------------------------------------------------------------------------
 constexpr int WG_PARTIAL_FLOATS = 65536 + 256;
 constexpr int WG_MAX_CTAS = 160;
-constexpr int WG_NUM_ROLES = 10;
+constexpr int WG_NUM_ROLES = 9;
 
 // Roles of the wgrad CTAs.  Role r computes D[A feature][B feature] = sum over samples of A^T B, with A and B read
-// from the tile images mlp_fwd and mlp_bwd saved, and the bias gradient as column sums of A or B.  Its partial holds
-// D row-major with `width` columns, then the bias sums (at WG_PARTIAL_FLOATS - 256).
+// from the tile images mlp_fwd and mlp_bwd saved, and the bias gradient as column sums of A or B.  B is always 256
+// features wide (h_l or dZ_0), so every MMA is an m64n256.
+//  - Dense_1..7 ("halved" roles): A = dZ_l, B = h_{l-1}.  A CTA owns one 128-row half of D, so the role's CTAs come
+//    in pairs.  Its partial holds D's rows [128 half, +128) at row pitch 256.  Dense_5 also contracts its A with the
+//    posenc tile (the skip rows, inputs 256..318) into a second, 64-wide accumulator; those 128 x 64 go to the rows
+//    of the partial its half leaves unused: floats [32768 (1 - half), +8192) at row pitch 64.
+//  - Dense_0 and the heads ("transposed" roles): A = posenc or dO (64 or NH features), B = dZ_0 or h_7, so D is the
+//    transposed weight gradient.  Every CTA computes all of D; warpgroup w writes partial rows [64 w, +64) at pitch
+//    256.  With A <= 64 features (wgrad_split_k) both warpgroups compute the same 64 rows over alternate halves of
+//    each stage's samples, and row r of D is the sum of partial rows r and 64 + r; with NH = 80 warpgroup w computes
+//    A features [64 w, +64).
+// The bias sums follow at WG_PARTIAL_FLOATS - 256, indexed by output feature (the split-K halves already added).
 enum WgOperand : int { WG_DZ = 0, WG_H = 1, WG_E = 2, WG_DO = 3 };   // dZ_l, h_l, posenc, dO tile images
-enum WgBias : int { WG_BIAS_NONE = 0, WG_BIAS_A = 1, WG_BIAS_B = 2 };
-constexpr int WG_WIDTH_NH = 0;   // result width of the heads role: the padded heads width NH
+enum WgBias : int { WG_BIAS_A = 1, WG_BIAS_B = 2 };
 struct WgradRole {
   int dense;            // reference Dense_i (the heads role: Dense_8 and Dense_9, in packed heads columns)
-  int in0;              // first input feature of Dense_i covered (Dense_5's posenc rows start at 256)
   int a_op, a_layer;    // A operand: result rows
   int b_op, b_layer;    // B operand: result columns
-  int width;            // 256, 64 or WG_WIDTH_NH
+  int halves;           // 2: the CTAs own 128-row halves of D; 1: transposed, every CTA computes all rows
+  int skip;             // Dense_5: A is also contracted with the posenc tile
   int bias;
 };
 __host__ __device__ constexpr WgradRole wgrad_role(int r) {
-  //     Dense_i    in0   A               B              width        bias
-  return r < 7 ? WgradRole{r + 1, 0,   WG_DZ, r + 1,  WG_H, r,      256,         WG_BIAS_A}      // Dense_1..7 (h4 rows of 5)
-       : r == 7 ? WgradRole{0,    0,   WG_DZ, 0,      WG_E, 0,      64,          WG_BIAS_A}      // Dense_0
-       : r == 8 ? WgradRole{5,    256, WG_DZ, 5,      WG_E, 0,      64,          WG_BIAS_NONE}   // Dense_5 posenc rows
-       :          WgradRole{8,    0,   WG_H,  7,      WG_DO, 0,     WG_WIDTH_NH, WG_BIAS_B};     // heads
+  //     Dense_i    A               B              halves  skip                bias
+  return r < 7 ? WgradRole{r + 1, WG_DZ, r + 1,  WG_H, r,       2, r + 1 == SKIP_LAYER, WG_BIAS_A}   // Dense_1..7
+       : r == 7 ? WgradRole{0,    WG_E, 0,       WG_DZ, 0,      1, 0,                   WG_BIAS_B}   // Dense_0^T
+       :          WgradRole{8,    WG_DO, 0,      WG_H, 7,       1, 0,                   WG_BIAS_A};  // heads^T
 }
-// role holding input row `in` of Dense_`dense`
-__host__ __device__ constexpr int wgrad_role_of(int dense, int in) {
-  int role = 0;
-  for (int r = 0; r < WG_NUM_ROLES; ++r)
-    if (wgrad_role(r).dense == (dense < 8 ? dense : 8) && in >= wgrad_role(r).in0) role = r;   // the last such role
-  return role;
-}
-__host__ __device__ constexpr int wgrad_role_width(const WgradRole& R, int NH) {
-  return R.width == WG_WIDTH_NH ? NH : R.width;
+// role holding Dense_`dense`'s gradient (8 and 9: the heads)
+__host__ __device__ constexpr int wgrad_role_of(int dense) { return dense == 0 ? 7 : dense < 8 ? dense - 1 : 8; }
+// transposed role whose A (posenc, or dO with NH <= 64) fits one m64: its warpgroups split each stage's samples
+__host__ __device__ constexpr bool wgrad_split_k(const WgradRole& R, int NH) {
+  return R.halves == 1 && (R.a_op == WG_E || NH <= 64);
 }
 struct WgradSegment {
   const uint8_t *h, *dz, *e, *d_o;

@@ -6,21 +6,39 @@
 
 namespace pob {
 
-// Work split of the wgrad launch.  The kernel is bound by the tile bytes each role streams
-// (96 KB per tile and row half for the 256x256 layers, ~40-64 KB for Dense_0 / the skip rows / the heads).  Every
-// role gets an even number of CTAs: CTA index i of a role computes result rows [128 (i & 1), +128) over the tiles
-// i / 2, i / 2 + count / 2, ...
+// Work split of the wgrad launch.  The units are the two row halves of each of Dense_1..7 and the transposed
+// Dense_0 and heads roles (kernels.h: WgradRole).  A unit's cost is the bytes it streams per 128-sample tile: 96 KB
+// for a row half (32 KB of dZ_l, 64 KB of h_{l-1}), 112 KB for Dense_5's (+ the posenc tile), 80 KB for Dense_0 and
+// the SH16 heads (16 KB of posenc / dO, 64 KB of dZ_0 / h_7), 96 KB for the SH25 heads.  CTAs go one at a time to
+// the unit with the most cost per CTA (the halves of a role in pairs), so that the units finish together.  CTA
+// index i of a halved role computes result rows [128 (i & 1), +128) over the tiles i / 2, i / 2 + count / 2, ...;
+// CTA i of a transposed role the tiles i, i + count, ...
 int wgrad_assign_roles(WgradParams& p, int n_in, int role_start[WG_NUM_ROLES],
                        int role_count[WG_NUM_ROLES]) {
   int n = n_in < WG_MAX_CTAS ? n_in : WG_MAX_CTAS;
-  if (n < 2 * WG_NUM_ROLES) n = 2 * WG_NUM_ROLES;  // one CTA per role and row half at the very least
-  auto even = [](int x) { return x < 2 ? 2 : x & ~1; };
-  int small = even((n * 8) / 100);         // per small role
-  const int big = even((n - 3 * small) / 7);
-  small = even((n - 7 * big) / 3);
+  int units = 0;
+  for (int r = 0; r < WG_NUM_ROLES; ++r) units += wgrad_role(r).halves;
+  if (n < units) n = units;   // one CTA per unit at the very least
+  int cost[WG_NUM_ROLES], per_unit[WG_NUM_ROLES];
+  for (int r = 0; r < WG_NUM_ROLES; ++r) {
+    const WgradRole R = wgrad_role(r);
+    const int a_kb = R.halves == 2 ? 32 : (wgrad_split_k(R, p.NH) ? 16 : 32);
+    cost[r] = a_kb + 64 + (R.skip ? 16 : 0);
+    per_unit[r] = 1;
+  }
+  for (int left = n - units;;) {
+    int best = -1;
+    for (int r = 0; r < WG_NUM_ROLES; ++r) {   // cost[r] / per_unit[r] largest; ties: the first
+      if (wgrad_role(r).halves > left) continue;
+      if (best < 0 || cost[r] * per_unit[best] > cost[best] * per_unit[r]) best = r;
+    }
+    if (best < 0) break;
+    ++per_unit[best];
+    left -= wgrad_role(best).halves;
+  }
   int cta = 0;
   for (int r = 0; r < WG_NUM_ROLES; ++r) {
-    const int c = wgrad_role(r).width == 256 ? big : small;
+    const int c = per_unit[r] * wgrad_role(r).halves;
     role_start[r] = cta;
     role_count[r] = c;
     for (int i = 0; i < c; ++i, ++cta) {
@@ -48,60 +66,68 @@ struct ReduceArgs {
   float* grad;
 };
 
-// role and offset inside a role's partial of element (layer, in i, out o) of a kernel, or (layer, out o) of a bias
-__device__ __forceinline__ void locate(const ReduceArgs& a, int layer, int i, int o, bool is_bias, int& role, int& off) {
-  role = wgrad_role_of(layer, i);
-  const WgradRole R = wgrad_role(role);
-  if (R.a_op == WG_H) {    // heads: D[in feature][packed column]
-    const int n = layer == 8 ? 0 : heads_column_of_output(o, a.K);
-    off = is_bias ? 65536 + n : i * a.NH + n;
-  } else {                 // D[out feature][in feature - in0]
-    off = is_bias ? 65536 + o : o * R.width + (i - R.in0);
+// Where element (layer, in i, out o) of a kernel, or (layer, out o) of a bias, lies in its role's partials
+// (kernels.h: WgradRole): offset `off`, plus `off2` >= 0 for the second warpgroup's rows of a split-K role; `row_half`
+// = the result row half of a halved role (its CTAs with index & 1 == half), -1 for a transposed role (all its CTAs).
+struct Loc {
+  int role, off, off2, row_half;
+};
+__device__ __forceinline__ Loc locate(const ReduceArgs& a, int layer, int i, int o, bool is_bias) {
+  Loc l;
+  l.role = wgrad_role_of(layer);
+  const WgradRole R = wgrad_role(l.role);
+  l.off2 = -1;
+  if (R.halves == 2) {     // D[out feature][in feature]
+    l.row_half = o >> 7;
+    l.off = is_bias ? 65536 + o
+          : i < WIDTH ? o * WIDTH + i
+                      : (l.row_half ? 0 : 32768) + (o & 127) * 64 + (i - WIDTH);   // Dense_5's skip rows
+  } else {                 // transposed: D[A feature][B feature], A = posenc (Dense_0) or packed heads column
+    l.row_half = -1;
+    const int r = layer == 0 ? i : layer == 8 ? 0 : heads_column_of_output(o, a.K);
+    const int col = layer == 0 ? o : i;
+    l.off = is_bias ? 65536 + (layer == 0 ? o : r) : r * WIDTH + col;
+    if (!is_bias && wgrad_split_k(R, a.NH)) l.off2 = l.off + 64 * WIDTH;
   }
+  return l;
 }
 
-// sum over the role's CTAs that computed the element: those of its result row half (a bias taken from B, the heads'
-// column sum of dO, comes from row half 0)
-__device__ __forceinline__ float sum_partials(const ReduceArgs& a, int role, int off) {
-  const WgradRole R = wgrad_role(role);
-  const int pitch = wgrad_role_width(R, a.NH);
-  const int row = off < 65536 ? off / pitch : (R.bias == WG_BIAS_B ? 0 : off - 65536);
+// sum over the role's CTAs that computed the element, in CTA order
+__device__ __forceinline__ float sum_partials(const ReduceArgs& a, const Loc& l) {
   float s = 0.f;
-  const float* p = a.partials + size_t(a.role_start[role]) * WG_PARTIAL_FLOATS + off;
-  for (int c = row >> 7; c < a.role_count[role]; c += 2) s += p[size_t(c) * WG_PARTIAL_FLOATS];
+  const float* p = a.partials + size_t(a.role_start[l.role]) * WG_PARTIAL_FLOATS;
+  const int step = l.row_half < 0 ? 1 : 2;
+  for (int c = l.row_half < 0 ? 0 : l.row_half; c < a.role_count[l.role]; c += step) {
+    s += p[size_t(c) * WG_PARTIAL_FLOATS + l.off];
+    if (l.off2 >= 0) s += p[size_t(c) * WG_PARTIAL_FLOATS + l.off2];
+  }
   return s;
 }
 
-// grid (in tiles of 32, out tiles of 32, 10 layers + 1 bias slice), block (32, 8).  The trunk partials are
-// [out][in] (accumulator row = out feature) and the flat gradient is flax's kernel [in][out]: every 32x32 tile is read
-// along `in` (coalesced in the partials), summed over the role's CTAs, transposed through shared memory and written
-// along `out` (coalesced in the gradient).  (A one-thread-per-gradient-element version read with a 1 KB stride:
-// 64 us per step instead of ~15.)
+// grid (in tiles of 32, out tiles of 32, 10 layers + 1 bias slice), block (32, 8).  The partials of Dense_1..9 are
+// [out][in] (accumulator row = out feature or packed heads column) and the flat gradient is flax's kernel [in][out]:
+// every 32x32 tile is read along `in` (coalesced in the partials), summed over the role's CTAs, transposed through
+// shared memory and written along `out` (coalesced in the gradient).  Dense_0's partials are [in][out].  (A
+// one-thread-per-gradient-element version read with a 1 KB stride: 64 us per step instead of ~15.)
 __global__ void reduce_grads_kernel(const __grid_constant__ ReduceArgs a) {
   __shared__ float tile[32][33];
   const int layer = blockIdx.z;
   if (layer == 10) {                      // biases: block x = layer, one thread per output
     const int l = blockIdx.x, o = threadIdx.y * 32 + threadIdx.x;
     if (blockIdx.y != 0 || l >= 10 || o >= a.L.out_dim[l]) return;
-    int role, off;
-    locate(a, l, 0, o, true, role, off);
-    a.grad[a.L.b_off[l] + o] = sum_partials(a, role, off) * a.inv_scale;
+    a.grad[a.L.b_off[l] + o] = sum_partials(a, locate(a, l, 0, o, true)) * a.inv_scale;
     return;
   }
   const int in_dim = a.L.in_dim[layer], out_dim = a.L.out_dim[layer];
   const int i0 = blockIdx.x * 32, o0 = blockIdx.y * 32;
   if (i0 >= in_dim || o0 >= out_dim) return;
-  const bool heads = layer >= 8;          // heads partials are [in][out]: read along `out` instead
+  const bool in_major = layer == 0;      // Dense_0's partials are [in][out]: read along `out` instead
   for (int k = threadIdx.y; k < 32; k += 8) {
-    const int i = heads ? i0 + k : i0 + threadIdx.x;
-    const int o = heads ? o0 + threadIdx.x : o0 + k;
+    const int i = in_major ? i0 + k : i0 + threadIdx.x;
+    const int o = in_major ? o0 + threadIdx.x : o0 + k;
     float v = 0.f;
-    if (i < in_dim && o < out_dim) {
-      int role, off;
-      locate(a, layer, i, o, false, role, off);
-      v = sum_partials(a, role, off);
-    }
-    if (heads) tile[k][threadIdx.x] = v;   // tile[i - i0][o - o0]
+    if (i < in_dim && o < out_dim) v = sum_partials(a, locate(a, layer, i, o, false));
+    if (in_major) tile[k][threadIdx.x] = v;   // tile[i - i0][o - o0]
     else tile[threadIdx.x][k] = v;
   }
   __syncthreads();

@@ -44,12 +44,14 @@ size_t up(size_t x) { return (x + 1023) / 1024 * 1024; }
 // every per-tile array is padded to a multiple of four 128-row tiles (common.cuh: padded_rows)
 long long tiles_for(long long M) { return padded_rows(M) / TILE_M; }
 
-// SMs (out of an H100 SXM's 132) that run mlp_bwd during the backward; mlp_wgrad runs on the others.  Step time of
-// bench.py on an H100 80 GB HBM3 at a 400 W power limit with dgrad on 54 / 58 / 60 / 62 / 64 / 66 / 70 SMs (register-A
-// dgrad, two runs each): 10.2 / 10.4 / 14.0 / 14.2 / 14.3 / 9.75-9.94 / 10.4-10.45 ms.  A wgrad side that cannot keep
-// up with dgrad misses L2 and runs a tail alone; wgrad_assign_roles' even role counts make neighbouring splits differ a
-// lot (DESIGN.md section 6).
-constexpr int DGRAD_SMS_OF_132 = 66;
+// SMs (out of an H100 SXM's 132) that run mlp_bwd during the backward; mlp_wgrad runs on the others.  SH16 training
+// step (bench.py's workload, 20 eager steps) on an H100 80 GB HBM3 at a 700 W power limit (1980 MHz maximum SM clock),
+// with dgrad on 56 / 58 / 60 / 62 / 64 / 66 / 68 / 70 / 72 / 74 / 76 / 78 SMs (four runs each for 56-66, two for the
+// rest): 6.48-7.86 / 6.57-6.81 / 6.58-6.69 / 6.77-6.79 / 6.89-6.94 / 6.99-7.91 / 7.87-8.57 / 7.70-7.91 / 7.91-8.02 /
+// 7.88-7.93 / 7.86-7.93 / 8.03-8.20 ms.  From 66 down to 60 the weight gradient gets more CTAs and its tail behind
+// the data gradient shrinks; from 68 up its transposed roles get three CTAs, it falls behind, its dZ reads miss L2
+// and it runs a tail alone; below 58 the data gradient becomes the long pole (DESIGN.md section 6).
+constexpr int DGRAD_SMS_OF_132 = 60;
 
 // deterministic carve of the caller-provided workspace
 Workspace carve(const pob_render_config& c, int training, uint8_t* base) {

@@ -3,7 +3,9 @@
     python scripts/profile_step.py --out DIR [--steps 10] [--warmup 5]
 
 Prints, per step, the summed duration of the saving and non-saving mlp_fwd, mlp_bwd and mlp_wgrad kernels, and each
-level's backward span (first mlp_bwd start to last mlp_wgrad end of the level).  bench.py's kernel_ms_per_step puts
+level's backward span (first mlp_bwd start to last mlp_wgrad end of the level) and its data-gradient idle time (how far
+the last mlp_wgrad end falls behind the mlp_bwd end: the SMs that ran mlp_bwd wait that long for the weight gradient;
+negative when the weight gradient finishes first).  bench.py's kernel_ms_per_step puts
 events between mlp_bwd and mlp_wgrad, which serialises them; the trace here shows them running together.  Writes
 summary.json (with the card name and power limit) and the Chrome trace under the output directory.
 """
@@ -75,7 +77,7 @@ def main():
     kern = sorted((e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA),
                   key=lambda e: e.time_range.start)
     per = {}
-    spans = []          # backward spans in launch order: two levels per step
+    spans = []          # [mlp_bwd start, mlp_bwd end, last mlp_wgrad end] in launch order: two levels per step
     cur = None
     for e in kern:
         c = kernel_class(e.name)
@@ -83,17 +85,22 @@ def main():
             continue
         per[c] = per.get(c, 0.0) + (e.time_range.end - e.time_range.start) / 1e3
         if c == "mlp_bwd":
-            cur = [e.time_range.start, e.time_range.end]
+            cur = [e.time_range.start, e.time_range.end, e.time_range.end]
             spans.append(cur)
         elif c == "mlp_wgrad" and cur is not None:
-            cur[1] = max(cur[1], e.time_range.end)
+            cur[2] = max(cur[2], e.time_range.end)
     K = args.steps
     per_step = {k: v / K for k, v in sorted(per.items())}
-    levels = {}
-    for i, (s, t) in enumerate(spans):
+    levels, idle = {}, {}
+    for i, (s, b, t) in enumerate(spans):
         levels.setdefault(f"level {i % 2} backward span", []).append((t - s) / 1e3)
+        idle.setdefault(f"level {i % 2} dgrad idle", []).append((t - b) / 1e3)
+
+    def stats(d):
+        return {k: {"min": min(v), "median": float(np.median(v)), "max": max(v)} for k, v in d.items()}
+
     res = {"card": card(), "steps": K, "kernel_ms_per_step": per_step,
-           "backward_span_ms": {k: {"min": min(v), "median": float(np.median(v)), "max": max(v)} for k, v in levels.items()}}
+           "backward_span_ms": stats(levels), "dgrad_idle_ms": stats(idle)}
     print(json.dumps(res, indent=1))
     with open(os.path.join(args.out, "summary.json"), "w") as f:
         json.dump(res, f, indent=1)
