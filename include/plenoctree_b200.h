@@ -181,6 +181,26 @@ int pob_loss_and_grad(const pob_render_config* cfg, const pob_train_hparams* hp,
                       const float* sp_points_dev, float* grad_flat_dev, float* stats_dev, void* workspace_dev,
                       void* mlp0_done_event, void* stream);
 
+/* bytes of device scratch pob_loss_and_grad_prec needs at `precision`; for POB_PREC_FP16 the same as
+ * pob_workspace_bytes(cfg, 1).  -1 on a bad config or precision. */
+int64_t pob_train_workspace_bytes(const pob_render_config* cfg, int precision);
+
+/* pob_loss_and_grad at `precision`.  POB_PREC_FP16 is pob_loss_and_grad (params_dev may be NULL).
+ * POB_PREC_FP16X3 runs the forward, the data gradient and the weight gradient with error-compensated operands
+ * (x = hi + lo, both fp16; every product lo*hi + hi*lo + hi*hi, fp32 accumulation): the render forward of
+ * POB_PREC_FP16X3, saving its activations, and a gradient within a few 2^-24 of fp64 per stage.  It needs params_dev
+ * (the flat fp32 parameters of all MLPs, [num_mlps * pob_param_count], consistent with the packed blobs as
+ * pob_adam_update leaves them) and a workspace of pob_train_workspace_bytes(cfg, POB_PREC_FP16X3) bytes.  The call
+ * refuses a workspace whose device allocation (cuMemGetAddressRange) ends before that size; it cannot see the bounds
+ * of a block that a caching allocator (torch.empty) cuts out of a larger allocation, so such callers must size the
+ * block themselves. */
+int pob_loss_and_grad_prec(const pob_render_config* cfg, const pob_train_hparams* hp, const void* packed_coarse_dev,
+                           const void* packed_fine_dev, const float* origins_dev, const float* directions_dev,
+                           const float* viewdirs_dev, const float* pixels_dev, int n_rays, const float* z_base_dev,
+                           const float* t_rand_dev, const float* u_dev, int u_per_ray, const float* z_fine_dev,
+                           const float* sp_points_dev, float* grad_flat_dev, float* stats_dev, void* workspace_dev,
+                           void* mlp0_done_event, const float* params_dev, int precision, void* stream);
+
 /* flax.optim.Adam (beta1 .9, beta2 .999, eps 1e-8; nerf_sh/nerf/models.py:44) on the flat buffers of
  * num_mlps MLPs, g = grad*grad_mult + weight_decay_coef*param, then re-packs the operand blobs.
  * `step` = number of updates already applied (flax optimizer.state.step).  lr_step_dev (device float[2] = {lr,

@@ -41,6 +41,9 @@ SIGNATURES = {
     "pob_render_rays": (_i, [_vp, _vp, _vp, _fp, _fp, _fp, _i, _fp, _fp, _fp, _i, _fp, _fp, _fp, _vp, _i, _vp]),
     "pob_loss_and_grad": (_i, [_vp, _vp, _vp, _vp, _fp, _fp, _fp, _fp, _i, _fp, _fp, _fp, _i, _fp, _fp, _fp, _fp,
                                _vp, _vp, _vp]),
+    "pob_train_workspace_bytes": (_i64, [_vp, _i]),
+    "pob_loss_and_grad_prec": (_i, [_vp, _vp, _vp, _vp, _fp, _fp, _fp, _fp, _i, _fp, _fp, _fp, _i, _fp, _fp, _fp,
+                                    _fp, _vp, _vp, _fp, _i, _vp]),
     "pob_adam_update": (_i, [_i, _i, _fp, _fp, _fp, _fp, _c.c_float, _c.c_float, _fp, _c.c_float, _c.c_float,
                              _vp, _vp, _vp]),
     "pob_octree_render": (_i, [_vp, _vp, _fp, _fp, _fp, _i64, _vp, _i, _i, _fp, _vp, _vp]),

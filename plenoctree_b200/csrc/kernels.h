@@ -49,10 +49,13 @@ struct FwdParams {
   float4* out_rgbs;            // OUT_RGBS: [M] (sigmoid(rgb), relu(sigma))
   float* out_cell;             // OUT_CELL_MEAN: [M / cell_S, 3K+1] += mean over the cell's samples of
   int cell_S;                  //   cat([raw_rgb, raw_sigma]) (octree/extraction.py:391-393); zeroed by caller
-  // ---- training saves (fast mode only; null = off) ----
+  // ---- training saves (null = off; x3 also needs save_h_lo / save_e_lo) ----
   uint8_t* save_h;             // [ntile][8][64 KB] activation tile images h_0..h_7
   uint8_t* save_e;             // [ntile][16 KB]   posenc tile images
   uint32_t* save_mask;         // [8][ntile*128][8] relu masks (bit i of word c = col 32c+i)
+  // ---- x3 training saves (NSPLIT = 3): the residual (lo) images beside save_h / save_e ----
+  uint8_t* save_h_lo;          // [ntile][8][64 KB]
+  uint8_t* save_e_lo;          // [ntile][16 KB]
 };
 
 // padded heads width for K spherical-harmonic coefficients per channel
@@ -70,6 +73,8 @@ cudaError_t launch_mlp_fwd(const FwdParams& p, int nsplit, int num_sms, cudaStre
 // bias) -> packed images.  `nparams` = param_count(K).
 cudaError_t launch_pack_weights(const float* flat, int K, uint8_t* w_hi, uint8_t* w_lo,
                                 uint8_t* wt_hi, cudaStream_t stream);
+// the residual (lo) of the dgrad images only, in the layout of wt_hi (bwd_image_bytes(NH)): the x3 data gradient
+cudaError_t launch_pack_wt_lo(const float* flat, int K, uint8_t* wt_lo, cudaStream_t stream);
 
 
 
@@ -106,9 +111,13 @@ struct BwdParams {
   uint8_t* save_dz;         // [ntile][8][64 KB]
   uint8_t* save_do;         // [ntile][32 KB]
   uint32_t* progress;       // [ntile], zeroed: stages of the tile whose stores have completed (wgrad_body.cuh)
+  // ---- x3 (nsplit = 3): residual images of the operands and of the saved tiles ----
+  const uint8_t* wt_lo;     // residual of w.wt_hi (launch_pack_wt_lo)
+  uint8_t* save_dz_lo;      // [ntile][8][64 KB]
+  uint8_t* save_do_lo;      // [ntile][32 KB]
 };
-// grid = min(tiles, num_ctas) persistent CTAs
-cudaError_t launch_mlp_bwd(const BwdParams& p, int num_ctas, cudaStream_t stream);
+// grid = min(tiles, num_ctas) persistent CTAs.  nsplit 3: dZ_l = hi + lo, every product lo*hi + hi*lo + hi*hi
+cudaError_t launch_mlp_bwd(const BwdParams& p, int nsplit, int num_ctas, cudaStream_t stream);
 
 // ---- mlp_wgrad.cu ---------------------------------------------------------------------------
 constexpr int WG_PARTIAL_FLOATS = 65536 + 256;
@@ -168,10 +177,22 @@ int wgrad_assign_roles(WgradParams& p, int num_sms, int role_start[WG_NUM_ROLES]
 cudaError_t launch_mlp_wgrad(const WgradParams& p, int num_ctas, cudaStream_t stream);
 
 // ---- optim.cu -------------------------------------------------------------------------------
-// partials of one wgrad launch -> flat gradient of one MLP (reference layout), times inv_scale
-cudaError_t launch_reduce_grads(const float* partials, const int role_start[WG_NUM_ROLES],
-                                const int role_count[WG_NUM_ROLES], int K, float inv_scale,
-                                float* grad_flat, cudaStream_t stream);
+// one mlp_wgrad launch: its partials and its role -> CTA table (wgrad_assign_roles)
+struct WgradPass {
+  const float* partials;
+  int role_start[WG_NUM_ROLES], role_count[WG_NUM_ROLES];
+};
+// The x3 weight gradient is three launches of mlp_wgrad over the hi / lo tile images (by linearity):
+//   pass 0: h hi, dz hi, e hi, d_o hi   -> A_hi B_hi for every role
+//   pass 1: h hi, dz lo, e hi, d_o lo   -> A_lo B_hi (Dense_1..7, heads), E_hi dZ0_lo (Dense_0), dZ5_lo E_hi (skip)
+//   pass 2: h lo, dz hi, e lo, d_o hi   -> A_hi B_lo (Dense_1..7, heads), E_lo dZ0_hi (Dense_0), dZ5_hi E_lo (skip)
+// The bias sums (columns of dZ_l / dO, Dense_0: of dZ_0) of pass 2 repeat pass 0's: only passes 0 and 1 count them.
+constexpr int X3_WGRAD_PASSES = 3;
+constexpr int X3_BIAS_PASSES = 2;
+// partials of `npass` wgrad launches -> flat gradient of one MLP (reference layout), times inv_scale.  Every element
+// sums its passes in order; the biases only the first min(npass, X3_BIAS_PASSES).
+cudaError_t launch_reduce_grads(const WgradPass* passes, int npass, int K, float inv_scale, float* grad_flat,
+                                cudaStream_t stream);
 // flax.optim.Adam.apply_gradient on a flat buffer; grad is multiplied by grad_mult first
 // lr_step_dev (optional, device [2] = {lr, step}) overrides the host lr / step: a captured graph replays with new values
 cudaError_t launch_adam(float* param, const float* grad, float* m, float* v, long long n, float lr,

@@ -297,13 +297,272 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
   }
 }
 
-cudaError_t launch_mlp_bwd(const BwdParams& p, int num_ctas, cudaStream_t stream) {
+// ================================== x3 data gradient ===============================================================
+// The same chain with error-compensated operands: dO and every dZ_l are formed in fp32 (masked), split into
+// x = hi + lo (fp16 each) and stored as two tile images; every K step issues lo*hi + hi*lo + hi*hi against a ring
+// stage holding the K-slot of wt_hi and of wt_lo.  An m64n256 accumulator and two 64-register A fragments do not fit
+// 232 registers, so A is read from shared memory (as in the x3 forward):
+//   A_hi 64 KB | A_lo 64 KB | three 32 KB weight stages = 224 KB.
+// The warpgroup writes dZ_l (hi and lo) into its rows of the A tiles once its MMAs of the previous GEMM have
+// completed (wgmma.wait) and its store warp has read the previous stage (rows_free); the next GEMM then reads the
+// rows while the store warp bulk-stores both images.  A stage's progress count is published once both of its images
+// have been stored.
+namespace {
+constexpr int X3_STAGES = 3;
+constexpr uint32_t X3_STAGE_BYTES = 2 * WSLOT_BYTES;      // wt_hi slot | wt_lo slot
+constexpr uint32_t X3_A_HI = 0;
+constexpr uint32_t X3_A_LO = X3_A_HI + A_TILE_BYTES;
+constexpr uint32_t X3_W = X3_A_LO + A_TILE_BYTES;
+constexpr uint32_t X3_TOTAL = X3_W + X3_STAGES * X3_STAGE_BYTES;   // 224 KB
+}  // namespace
+
+__global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_x3_kernel(const __grid_constant__ BwdParams p) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  __shared__ __align__(8) Ring<X3_STAGES> ring;
+  __shared__ __align__(8) uint64_t rows_full[2], rows_free[2];
+
+  const long long mrows = padded_rows(p.M);
+  const long long num_tiles = mrows / TILE_M;
+  const uint32_t warp = warp_id(), lane = lane_id();
+  const uint32_t sbase = smem_u32(smem);
+  const int NH = p.NH;
+  const int do_chunks = (NH + 63) / 64;
+
+  griddep_launch_dependents();
+  if (threadIdx.x == 0) {
+    ring.init(X3_STAGES);
+    for (int g = 0; g < 2; ++g) {
+      mbar_init(smem_u32(&rows_full[g]), 128);
+      mbar_init(smem_u32(&rows_free[g]), 1);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (warp >= BWD_PRODUCER_WARP) {
+    setmaxnreg_dec<40>();
+    if (warp == BWD_PRODUCER_WARP) {
+      RingPos pos;
+      const int nslots = bwd_slots(NH);
+      for (long long it = blockIdx.x; it < num_tiles; it += gridDim.x) {
+        for (int j = 0; j < nslots; ++j) {
+          ring.acquire(pos);
+          if (elect_one()) {
+            const uint32_t bar = ring.arm(pos, X3_STAGE_BYTES);
+            const uint32_t dst = sbase + X3_W + pos.stage * X3_STAGE_BYTES;
+            bulk_g2s(dst, p.w.wt_hi + size_t(j) * WSLOT_BYTES, WSLOT_BYTES, bar);
+            bulk_g2s(dst + WSLOT_BYTES, p.wt_lo + size_t(j) * WSLOT_BYTES, WSLOT_BYTES, bar);
+          }
+          __syncwarp();
+          pos.advance(X3_STAGES);
+        }
+      }
+    } else if (warp <= BWD_STORE_WARP0 + 1 && lane == 0) {
+      // store warp of warpgroup g: as in mlp_bwd_kernel, with the hi and lo images of a stage in one bulk group
+      const int g = int(warp) - BWD_STORE_WARP0;
+      const uint32_t rows_off = uint32_t(g) * 64u * 128u;
+      const uint32_t progress_inc = g == 0 ? 1u : 0x10000u;
+      const uint32_t full = smem_u32(&rows_full[g]), free = smem_u32(&rows_free[g]);
+      uint32_t phase = 0;
+      long long pending = -1;
+      auto publish = [&]() {
+        fence_proxy_async_global();
+        red_add_release_gpu(p.progress + pending, progress_inc);
+      };
+      for (long long it = blockIdx.x; it < num_tiles; it += gridDim.x) {
+        for (int st = 0; st <= NUM_TRUNK; ++st) {
+          const size_t o = st == 0 ? size_t(it) * (2 * A_CHUNK_BYTES)
+                                   : (size_t(it) * NUM_TRUNK + (NUM_TRUNK - st)) * A_TILE_BYTES;
+          uint8_t* const dst_hi = (st == 0 ? p.save_do : p.save_dz) + o;
+          uint8_t* const dst_lo = (st == 0 ? p.save_do_lo : p.save_dz_lo) + o;
+          const int nchunks = st == 0 ? do_chunks : 4;
+          mbar_wait(full, phase);
+          for (int c = 0; c < nchunks; ++c) {
+            const uint32_t so = c * A_CHUNK_BYTES + rows_off;
+            bulk_s2g(dst_hi + so, sbase + X3_A_HI + so, 64u * 128u);
+            bulk_s2g(dst_lo + so, sbase + X3_A_LO + so, 64u * 128u);
+          }
+          bulk_commit();
+          bulk_wait_read_all();
+          mbar_arrive(free);
+          if (pending >= 0) {
+            bulk_wait_all_but_last();
+            publish();
+          }
+          pending = it;
+          phase ^= 1;
+        }
+      }
+      bulk_wait_all();
+      if (pending >= 0) publish();
+    }
+    return;
+  }
+
+  // ================================ consumer warpgroups =================================
+  setmaxnreg_inc<232>();
+  const int wg = int(warp >> 2);
+  const int t = int(threadIdx.x & 127);
+  const int wq = t >> 5;
+  const int fr = 16 * wq + int(lane >> 2);
+  const int fc = 2 * int(lane & 3);
+  uint8_t* const a_hi = smem + X3_A_HI;
+  uint8_t* const a_lo = smem + X3_A_LO;
+  const uint32_t rows_off = uint32_t(wg) * 64u * 128u;
+  constexpr uint64_t A_DESC = make_sdesc_hi(16, 1024, LAYOUT_SW128);
+  constexpr uint64_t W_DESC = make_sdesc_hi(16, 512, LAYOUT_SW64);
+  RingPos pos;
+  float acc[128];
+  uint32_t mw[2][8];
+
+  uint32_t rows_phase = 0;
+  auto rows_acquire = [&]() {
+    mbar_wait(smem_u32(&rows_free[wg]), rows_phase ^ 1);
+    __syncwarp();
+  };
+  auto rows_hand_over = [&]() {
+    fence_proxy_async_smem();
+    mbar_arrive(smem_u32(&rows_full[wg]));
+    rows_phase ^= 1;
+  };
+  auto load_masks = [&](int l, long long it) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint4* mp = reinterpret_cast<const uint4*>(p.mask + (size_t(l) * mrows + it * TILE_M + 64 * wg + fr + 8 * h) * 8);
+      const uint4 m0 = __ldg(mp), m1 = __ldg(mp + 1);
+      mw[h][0] = m0.x; mw[h][1] = m0.y; mw[h][2] = m0.z; mw[h][3] = m0.w;
+      mw[h][4] = m1.x; mw[h][5] = m1.y; mw[h][6] = m1.z; mw[h][7] = m1.w;
+    }
+  };
+  // GEMM over `ns` K-slots, A = the warpgroup's rows of the hi / lo tiles (K-slot j: chunk j/2, half j%2)
+  auto gemm = [&](int ns, int mask_layer, long long it) {
+    uint32_t prev = 0;
+    wgmma_fence();
+    for (int j = 0; j < ns; ++j) {
+      const uint32_t a_off = uint32_t(j >> 1) * A_CHUNK_BYTES + rows_off + uint32_t(j & 1) * 64u;
+      const uint32_t ah = sbase + X3_A_HI + a_off, al = sbase + X3_A_LO + a_off;
+      const uint32_t bh = sbase + X3_W + pos.stage * X3_STAGE_BYTES, bl = bh + WSLOT_BYTES;
+      ring.wait(pos);
+      // per K-slot: without it ptxas injects the warpgroup.arrive after the ring spin itself and serializes every
+      // wgmma of the kernel (C7520)
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        const uint32_t ko = uint32_t(k) * 32u;
+        wgmma_m64n256<0, 0>(acc, sdesc(A_DESC, al + ko), sdesc(W_DESC, bh + ko), (j != 0 || k != 0) ? 1u : 0u);
+        wgmma_m64n256<0, 0>(acc, sdesc(A_DESC, ah + ko), sdesc(W_DESC, bl + ko), 1u);
+        wgmma_m64n256<0, 0>(acc, sdesc(A_DESC, ah + ko), sdesc(W_DESC, bh + ko), 1u);
+      }
+      wgmma_commit();
+      if (j == 0) load_masks(mask_layer, it);   // loaded while the GEMM runs
+      if (j > 0) {
+        wgmma_wait<1>();
+        ring.release(prev);
+      }
+      prev = pos.stage;
+      pos.advance(X3_STAGES);
+    }
+    wgmma_wait<0>();
+    ring.release(prev);
+  };
+  // dZ = dH * relu'(h) in fp32 (mask word c: column 32c+2k <-> bit 15-k, 32c+2k+1 <-> bit 31-k), split into hi + lo
+  // and written to the warpgroup's rows of the A tiles, then handed to the store warp
+  auto store_dz = [&]() {
+    rows_acquire();
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      const int k = (j & 3) * 4 + (fc >> 1);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t m = mw[h][j >> 2];
+        const float v0 = (m >> (15 - k)) & 1u ? acc[4 * j + 2 * h] : 0.f;
+        const float v1 = (m >> (31 - k)) & 1u ? acc[4 * j + 2 * h + 1] : 0.f;
+        const uint32_t w = pack_f16x2(v0, v1);
+        const float2 hv = unpack_f16x2(w);
+        const uint32_t off = a_tile_offset(64 * wg + fr + 8 * h, 8 * j + fc);
+        *reinterpret_cast<uint32_t*>(a_hi + off) = w;
+        *reinterpret_cast<uint32_t*>(a_lo + off) = pack_f16x2(v0 - hv.x, v1 - hv.y);
+      }
+    }
+    rows_hand_over();
+    warpgroup_sync(wg);   // every row written before the next GEMM reads them
+  };
+
+  for (long long it = blockIdx.x; it < num_tiles; it += gridDim.x) {
+    // ---- dO rows (two threads per row, 64 columns each), fp32 -> hi + lo ----
+    {
+      const int r = 64 * wg + (t & 63);
+      const int hf = t >> 6;
+      const long long s = it * TILE_M + r;
+      float4 gq = make_float4(0.f, 0.f, 0.f, 0.f);
+      float basis[25];
+#pragma unroll
+      for (int k = 0; k < 25; ++k) basis[k] = 0.f;
+      basis[0] = 1.f;
+      if (s < p.M) {
+        gq = p.G[s];
+        const long long vi = p.n_per_ray > 0 ? (s < p.M_rays ? s / p.n_per_ray : 0) : s;
+        const float* vd = p.viewdirs + 3 * vi;
+        if (p.sh_deg >= 0) sh_basis(p.sh_deg, __ldg(vd), __ldg(vd + 1), __ldg(vd + 2), basis);
+      }
+      const float gc[3] = {gq.x, gq.y, gq.z};
+      auto build_do = [&](auto half) {
+        constexpr int HF = decltype(half)::value;
+#pragma unroll
+        for (int uu = 0; uu < 8; ++uu) {
+          const int u = 8 * HF + uu;
+          uint32_t w[4], wl[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            float f[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int n = u * 8 + 2 * i + e;
+              float v = 0.f;
+              if (n == 0) v = gq.w;
+              else if (n < 1 + 3 * 25) {
+                int k, c;
+                heads_coeff(n, k, c);
+                if (k < p.K) v = gc[c] * basis[k];
+              }
+              f[e] = v;
+            }
+            w[i] = pack_f16x2(f[0], f[1]);
+            const float2 hv = unpack_f16x2(w[i]);
+            // unfused: lo is the residual of the rounded product f, not of the exact one
+            wl[i] = pack_f16x2(__fsub_rn(f[0], hv.x), __fsub_rn(f[1], hv.y));
+          }
+          const uint32_t off = a_tile_offset(r, 8 * u);
+          *reinterpret_cast<uint4*>(a_hi + off) = make_uint4(w[0], w[1], w[2], w[3]);
+          *reinterpret_cast<uint4*>(a_lo + off) = make_uint4(wl[0], wl[1], wl[2], wl[3]);
+        }
+      };
+      rows_acquire();
+      if (hf == 0) build_do(std::integral_constant<int, 0>());
+      else if (do_chunks > 1) build_do(std::integral_constant<int, 1>());
+      rows_hand_over();
+      warpgroup_sync(wg);
+    }
+    // ---- dH_7 = dO . W_heads; then dZ_l, and dH_{l-1} = dZ_l . W_l (l = 7 .. 1), dZ_0 ----
+    gemm(bwd_head_slots(NH), NUM_TRUNK - 1, it);
+    for (int l = NUM_TRUNK - 1; l >= 0; --l) {
+      store_dz();
+      if (l > 0) gemm(8, l - 1, it);
+    }
+  }
+}
+
+cudaError_t launch_mlp_bwd(const BwdParams& p, int nsplit, int num_ctas, cudaStream_t stream) {
   if (p.M <= 0) return cudaSuccess;
+  if (nsplit != 1 && nsplit != 3) return cudaErrorInvalidValue;
+  if (nsplit == 3 && (!p.wt_lo || !p.save_dz_lo || !p.save_do_lo)) return cudaErrorInvalidValue;
   const long long tiles = padded_rows(p.M) / TILE_M;
   const int grid = int(tiles < num_ctas ? tiles : num_ctas);
-  cudaError_t e = cudaFuncSetAttribute(mlp_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SB_TOTAL);
+  auto kernel = nsplit == 1 ? mlp_bwd_kernel : mlp_bwd_x3_kernel;
+  const uint32_t smem = nsplit == 1 ? SB_TOTAL : X3_TOTAL;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  mlp_bwd_kernel<<<grid, BWD_THREADS, SB_TOTAL, stream>>>(p);
+  kernel<<<grid, BWD_THREADS, smem, stream>>>(p);
   return cudaGetLastError();
 }
 

@@ -21,7 +21,8 @@
 // synchronise through the weight ring alone.  fp16 chains the layers through registers (the activation tile only
 // stages the heads); the training saves of h_l run one K-slot behind layer l+1's MMAs.  NSPLIT = 3 evaluates
 // with error-compensated fp16 operands (x = hi + lo; lo*hi + hi*lo + hi*hi per K step), the residual parts in a
-// second set of tiles; a stage then holds the K-slot's hi and lo parts (32 KB).
+// second set of tiles; a stage then holds the K-slot's hi and lo parts (32 KB).  The x3 training forward (SAVE)
+// stores h_l's hi and lo from the trunk epilogue and the posenc tile's lo behind the posenc barrier.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -210,7 +211,6 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
   const uint32_t rows_off = uint32_t(wg) * 64u * 128u;     // this warpgroup's 64 rows inside every 128-row chunk
   constexpr uint64_t A_DESC = make_sdesc_hi(16, 1024, LAYOUT_SW128);
   constexpr uint64_t W_DESC = make_sdesc_hi(16, 512, LAYOUT_SW64);
-  static_assert(!SAVE || NSPLIT == 1, "the training forward is fp16");
   RingPos pos;
   float acc[128];
   float hacc[HEADS_N / 2];
@@ -396,6 +396,15 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
                                   SAVE ? p.save_e + size_t(it) * E_TILE_BYTES : nullptr);
       fence_proxy_async_smem();
       warpgroup_sync(wg);
+      if constexpr (SAVE && NSPLIT == 3) {
+        // x3 training save of the posenc residual: the warpgroup's 64 rows of the lo tile (8 KB), as written above
+        uint8_t* const dst = p.save_e_lo + size_t(it) * E_TILE_BYTES + rows_off;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const uint32_t o = (uint32_t(i) * 128u + uint32_t(t)) * 16u;
+          *reinterpret_cast<uint4*>(dst + o) = *reinterpret_cast<const uint4*>(e_lo + rows_off + o);
+        }
+      }
     }
     if constexpr (NSPLIT == 1) {
       // ---- fp16: layer 0 from the posenc tile, then every layer's activations stay in registers ----
@@ -475,7 +484,17 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
 
         if (!heads) {
           // ---- trunk epilogue: ReLU + hi/lo fp16 split straight from the accumulator fragment into the next A
-          // operands (the bias was accumulated by the tensor cores).  Only this warpgroup's MMAs read these rows. ----
+          // operands (the bias was accumulated by the tensor cores).  Only this warpgroup's MMAs read these rows.
+          // Training (SAVE): the same hi and lo values go to the "T" images of h_l (layouts.py: t_tile_offset; one
+          // warp store = one contiguous 128 B core-matrix row group, as in the fp16 save_slot), and the mask words
+          // of h_l take their bits from the sign of the fp32 pre-activation: relu(v) < 2^-25 rounds to hi = lo = 0
+          // but still has a gradient.  Word c, column 32c+2k <-> bit 15-k, 32c+2k+1 <-> bit 31-k; lane q of a quad
+          // keeps words 4(q&1)..+3 of row fr + 8(q>>1). ----
+          size_t t_off = 0;
+          uint32_t mrow[2] = {0u, 0u}, maskw[4] = {0u, 0u, 0u, 0u};
+          if constexpr (SAVE)
+            t_off = (size_t(it) * NUM_TRUNK + l) * A_TILE_BYTES + uint32_t(2 * wg + (wq >> 1)) * 16384u +
+                    uint32_t(16 * (wq & 1) + int(lane >> 2)) * 16u + uint32_t(fc) * 2u;
 #pragma unroll
           for (int j = 0; j < 32; ++j) {
 #pragma unroll
@@ -486,8 +505,33 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
               const uint32_t w = pack_f16x2_relu(v0, v1);
               *reinterpret_cast<uint32_t*>(a_hi + off) = w;
               const float2 hv = unpack_f16x2(w);
-              *reinterpret_cast<uint32_t*>(a_lo + off) = pack_f16x2(fmaxf(v0, 0.f) - hv.x, fmaxf(v1, 0.f) - hv.y);
+              const uint32_t wl = pack_f16x2(fmaxf(v0, 0.f) - hv.x, fmaxf(v1, 0.f) - hv.y);
+              *reinterpret_cast<uint32_t*>(a_lo + off) = wl;
+              if constexpr (SAVE) {
+                const size_t go = t_off + uint32_t(j) * 512u + uint32_t(h) * 128u;
+                *reinterpret_cast<uint32_t*>(p.save_h + go) = w;
+                *reinterpret_cast<uint32_t*>(p.save_h_lo + go) = wl;
+                const int k = 4 * (j & 3) + (fc >> 1);   // column pair within the mask word
+                mrow[h] |= (v0 > 0.f ? 1u << (15 - k) : 0u) | (v1 > 0.f ? 1u << (31 - k) : 0u);
+              }
             }
+            if (SAVE && (j & 3) == 3) {
+              const int c = j >> 2;
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                mrow[h] |= __shfl_xor_sync(0xffffffffu, mrow[h], 1);
+                mrow[h] |= __shfl_xor_sync(0xffffffffu, mrow[h], 2);
+              }
+              const uint32_t q = lane & 3;
+              if ((q & 1) == uint32_t(c >> 2)) maskw[c & 3] = (q >> 1) ? mrow[1] : mrow[0];
+              mrow[0] = mrow[1] = 0u;
+            }
+          }
+          if constexpr (SAVE) {
+            const uint32_t q = lane & 3;
+            const long long s = it * TILE_M + 64 * wg + fr + 8 * int(q >> 1);
+            *reinterpret_cast<uint4*>(p.save_mask + (size_t(l) * padded_rows(p.M) + s) * 8 + 4 * (q & 1)) =
+                make_uint4(maskw[0], maskw[1], maskw[2], maskw[3]);
           }
           fence_proxy_async_smem();
           warpgroup_sync(wg);
@@ -503,9 +547,10 @@ cudaError_t launch_mlp_fwd(const FwdParams& p, int nsplit, int num_sms, cudaStre
   if (p.M <= 0) return cudaSuccess;
   if (nsplit != 1 && nsplit != 3) return cudaErrorInvalidValue;
   const bool save = p.save_h != nullptr;
-  if (save && (nsplit != 1 || !p.save_e || !p.save_mask ||
-               (p.out_mode != OUT_RGBS && p.out_mode != OUT_SIGMA)))
+  if (save && (!p.save_e || !p.save_mask || (p.out_mode != OUT_RGBS && p.out_mode != OUT_SIGMA)))
     return cudaErrorInvalidValue;
+  // the x3 training forward: the rgbs epilogue of the render path, plus the residual images
+  if (save && nsplit == 3 && (!p.save_h_lo || !p.save_e_lo || p.out_mode != OUT_RGBS)) return cudaErrorInvalidValue;
   const long long tiles = save ? padded_rows(p.M) / TILE_M : (p.M + TILE_M - 1) / TILE_M;
   const int grid = int(tiles < num_sms ? tiles : num_sms);
   auto launch = [&](auto kernel) -> cudaError_t {
@@ -522,7 +567,7 @@ cudaError_t launch_mlp_fwd(const FwdParams& p, int nsplit, int num_sms, cudaStre
       if (save) return launch(mlp_fwd_kernel<1, OUT_SIGMA, true>);
       return nsplit == 1 ? launch(mlp_fwd_kernel<1, OUT_SIGMA, false>) : launch(mlp_fwd_kernel<3, OUT_SIGMA, false>);
     case OUT_RGBS:
-      if (save) return launch(mlp_fwd_kernel<1, OUT_RGBS, true>);
+      if (save) return nsplit == 1 ? launch(mlp_fwd_kernel<1, OUT_RGBS, true>) : launch(mlp_fwd_kernel<3, OUT_RGBS, true>);
       return nsplit == 1 ? launch(mlp_fwd_kernel<1, OUT_RGBS, false>) : launch(mlp_fwd_kernel<3, OUT_RGBS, false>);
     case OUT_CELL_MEAN:
       return nsplit == 1 ? launch(mlp_fwd_kernel<1, OUT_CELL_MEAN, false>)

@@ -1,6 +1,8 @@
 // optim.cu — gradient finalisation and the optimiser step.
 //   reduce_grads : per-CTA wgrad partials -> flat fp32 gradient in reference parameter order
 //   adam         : flax.optim.Adam.apply_gradient (nerf_sh/train.py:119, models.py:44)
+#include <cstring>
+
 #include "common.cuh"
 #include "kernels.h"
 
@@ -58,8 +60,8 @@ int wgrad_assign_roles(WgradParams& p, int n_in, int role_start[WG_NUM_ROLES],
 namespace {
 
 struct ReduceArgs {
-  const float* partials;
-  int role_start[WG_NUM_ROLES], role_count[WG_NUM_ROLES];
+  WgradPass pass[X3_WGRAD_PASSES];
+  int npass;
   FlatLayout L;
   int K, NH;
   float inv_scale;
@@ -92,14 +94,17 @@ __device__ __forceinline__ Loc locate(const ReduceArgs& a, int layer, int i, int
   return l;
 }
 
-// sum over the role's CTAs that computed the element, in CTA order
-__device__ __forceinline__ float sum_partials(const ReduceArgs& a, const Loc& l) {
+// sum over the passes and, in each, over the role's CTAs that computed the element, in CTA order
+__device__ __forceinline__ float sum_partials(const ReduceArgs& a, const Loc& l, int npass) {
   float s = 0.f;
-  const float* p = a.partials + size_t(a.role_start[l.role]) * WG_PARTIAL_FLOATS;
   const int step = l.row_half < 0 ? 1 : 2;
-  for (int c = l.row_half < 0 ? 0 : l.row_half; c < a.role_count[l.role]; c += step) {
-    s += p[size_t(c) * WG_PARTIAL_FLOATS + l.off];
-    if (l.off2 >= 0) s += p[size_t(c) * WG_PARTIAL_FLOATS + l.off2];
+  for (int q = 0; q < npass; ++q) {
+    const WgradPass& g = a.pass[q];
+    const float* p = g.partials + size_t(g.role_start[l.role]) * WG_PARTIAL_FLOATS;
+    for (int c = l.row_half < 0 ? 0 : l.row_half; c < g.role_count[l.role]; c += step) {
+      s += p[size_t(c) * WG_PARTIAL_FLOATS + l.off];
+      if (l.off2 >= 0) s += p[size_t(c) * WG_PARTIAL_FLOATS + l.off2];
+    }
   }
   return s;
 }
@@ -115,7 +120,8 @@ __global__ void reduce_grads_kernel(const __grid_constant__ ReduceArgs a) {
   if (layer == 10) {                      // biases: block x = layer, one thread per output
     const int l = blockIdx.x, o = threadIdx.y * 32 + threadIdx.x;
     if (blockIdx.y != 0 || l >= 10 || o >= a.L.out_dim[l]) return;
-    a.grad[a.L.b_off[l] + o] = sum_partials(a, locate(a, l, 0, o, true)) * a.inv_scale;
+    a.grad[a.L.b_off[l] + o] =
+        sum_partials(a, locate(a, l, 0, o, true), min(a.npass, X3_BIAS_PASSES)) * a.inv_scale;
     return;
   }
   const int in_dim = a.L.in_dim[layer], out_dim = a.L.out_dim[layer];
@@ -126,7 +132,7 @@ __global__ void reduce_grads_kernel(const __grid_constant__ ReduceArgs a) {
     const int i = in_major ? i0 + k : i0 + threadIdx.x;
     const int o = in_major ? o0 + threadIdx.x : o0 + k;
     float v = 0.f;
-    if (i < in_dim && o < out_dim) v = sum_partials(a, locate(a, layer, i, o, false));
+    if (i < in_dim && o < out_dim) v = sum_partials(a, locate(a, layer, i, o, false), a.npass);
     if (in_major) tile[k][threadIdx.x] = v;   // tile[i - i0][o - o0]
     else tile[threadIdx.x][k] = v;
   }
@@ -165,15 +171,13 @@ __global__ void adam_kernel(float* __restrict__ param, const float* __restrict__
 
 }  // namespace
 
-cudaError_t launch_reduce_grads(const float* partials, const int role_start[WG_NUM_ROLES],
-                                const int role_count[WG_NUM_ROLES], int K, float inv_scale,
-                                float* grad_flat, cudaStream_t stream) {
+cudaError_t launch_reduce_grads(const WgradPass* passes, int npass, int K, float inv_scale, float* grad_flat,
+                                cudaStream_t stream) {
+  if (npass < 1 || npass > X3_WGRAD_PASSES) return cudaErrorInvalidValue;
   ReduceArgs a;
-  a.partials = partials;
-  for (int r = 0; r < WG_NUM_ROLES; ++r) {
-    a.role_start[r] = role_start[r];
-    a.role_count[r] = role_count[r];
-  }
+  memset(&a, 0, sizeof(a));
+  for (int q = 0; q < npass; ++q) a.pass[q] = passes[q];
+  a.npass = npass;
   a.L = flat_layout(K);
   a.K = K;
   a.NH = heads_width(K);

@@ -9,7 +9,8 @@
 //   in the order mlp_fwd consumes them.  Heads rows are re-ordered to [sigma, (k, c) ...] so the
 //   epilogue can index the SH basis with compile-time constants.
 // Backward images (wt_hi): the transposed weights, slots [rows = in feature][32 out features],
-//   in the order mlp_bwd consumes them (heads, then Dense_7 .. Dense_1).
+//   in the order mlp_bwd consumes them (heads, then Dense_7 .. Dense_1).  Their fp16 residual (wt_lo, same layout)
+//   is not part of the blob: the x3 training step writes it into its workspace (launch_pack_wt_lo).
 #include "common.cuh"
 #include "kernels.h"
 
@@ -21,12 +22,14 @@ struct PackArgs {
   const float* flat;
   FlatLayout L;
   int K, NH;
-  uint8_t *w_hi, *w_lo, *wt_hi;
+  uint8_t *w_hi, *w_lo, *wt_hi, *wt_lo;
+  int dgrad_only;   // write the dgrad slots only (the forward images are left alone)
 };
 
+// fp16 hi part and residual of v; either destination may be null
 __device__ __forceinline__ void put_hilo(uint8_t* hi, uint8_t* lo, size_t off, float v) {
   __half h = __float2half_rn(v);
-  *reinterpret_cast<__half*>(hi + off) = h;
+  if (hi) *reinterpret_cast<__half*>(hi + off) = h;
   if (lo) *reinterpret_cast<__half*>(lo + off) = __float2half_rn(v - __half2float(h));
 }
 
@@ -50,7 +53,8 @@ __global__ void pack_weights_kernel(const __grid_constant__ PackArgs a) {
   const int hs = bwd_head_slots(NH);
   const long long n_bwd = (long long)bwd_slots(NH) * 256 * 32;
   const long long total = n_fwd_trunk + n_fwd_heads + n_bwd;
-  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
+  const long long first = a.dgrad_only ? n_fwd_trunk + n_fwd_heads : 0;
+  for (long long t = first + blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
        t += (long long)gridDim.x * blockDim.x) {
     if (t < n_fwd_trunk) {
       const int slot = int(t / (256 * 32));
@@ -92,15 +96,13 @@ __global__ void pack_weights_kernel(const __grid_constant__ PackArgs a) {
         const int ko = 32 * ((slot - hs) % 8) + kk;
         v = a.flat[a.L.w_off[l] + i * 256 + ko];
       }
-      put_hilo(a.wt_hi, nullptr, size_t(slot) * WSLOT_BYTES + w_slot_offset(i, kk), v);
+      put_hilo(a.wt_hi, a.wt_lo, size_t(slot) * WSLOT_BYTES + w_slot_offset(i, kk), v);
     }
   }
 }
 
-}  // namespace
-
-cudaError_t launch_pack_weights(const float* flat, int K, uint8_t* w_hi, uint8_t* w_lo,
-                                uint8_t* wt_hi, cudaStream_t stream) {
+cudaError_t launch_pack(const float* flat, int K, uint8_t* w_hi, uint8_t* w_lo, uint8_t* wt_hi, uint8_t* wt_lo,
+                        int dgrad_only, cudaStream_t stream) {
   PackArgs a;
   a.flat = flat;
   a.L = flat_layout(K);
@@ -109,8 +111,21 @@ cudaError_t launch_pack_weights(const float* flat, int K, uint8_t* w_hi, uint8_t
   a.w_hi = w_hi;
   a.w_lo = w_lo;
   a.wt_hi = wt_hi;
+  a.wt_lo = wt_lo;
+  a.dgrad_only = dgrad_only;
   pack_weights_kernel<<<592, 256, 0, stream>>>(a);
   return cudaGetLastError();
+}
+
+}  // namespace
+
+cudaError_t launch_pack_weights(const float* flat, int K, uint8_t* w_hi, uint8_t* w_lo,
+                                uint8_t* wt_hi, cudaStream_t stream) {
+  return launch_pack(flat, K, w_hi, w_lo, wt_hi, nullptr, 0, stream);
+}
+
+cudaError_t launch_pack_wt_lo(const float* flat, int K, uint8_t* wt_lo, cudaStream_t stream) {
+  return launch_pack(flat, K, nullptr, nullptr, nullptr, wt_lo, 1, stream);
 }
 
 }  // namespace pob

@@ -3,6 +3,8 @@
 //   pob_loss_and_grad  = value_and_grad(loss_fn)       (nerf_sh/train.py:66-116)
 //   pob_adam_update    = optimizer.apply_gradient      (nerf_sh/train.py:119) + operand re-pack
 // Everything is enqueued on the caller's stream; nothing synchronises with the host.
+#include <cuda.h>
+
 #include <cstring>
 #include <string>
 
@@ -29,6 +31,7 @@ struct Level {
   float4* G;          // [M]
   uint8_t *H, *E, *DZ, *DO;
   uint32_t* mask;
+  uint8_t *H_lo, *E_lo, *DZ_lo, *DO_lo;   // x3 training: residual images of H, E, DZ, DO
 };
 
 struct Workspace {
@@ -36,6 +39,9 @@ struct Workspace {
   float* partials[2]; // wgrad partials of the two MLPs' launches
   uint32_t* progress; // per tile of level 0, then of level 1: mlp_bwd -> mlp_wgrad progress counters (wgrad_body.cuh)
   size_t progress_bytes;
+  // x3 training only, behind everything the fp16 step uses (so that its layout is the fp16 one plus this tail)
+  float* partials_x3[2][2];   // [mlp][wgrad pass 1, 2]
+  uint8_t* wt_lo[2];          // [mlp] residual of the dgrad weight images, written from params_dev by every call
   size_t total;
 };
 
@@ -53,8 +59,8 @@ long long tiles_for(long long M) { return padded_rows(M) / TILE_M; }
 // and it runs a tail alone; below 58 the data gradient becomes the long pole (DESIGN.md section 6).
 constexpr int DGRAD_SMS_OF_132 = 60;
 
-// deterministic carve of the caller-provided workspace
-Workspace carve(const pob_render_config& c, int training, uint8_t* base) {
+// deterministic carve of the caller-provided workspace (x3: the training workspace of the fp16x3 step)
+Workspace carve(const pob_render_config& c, int training, uint8_t* base, bool x3 = false) {
   Workspace w;
   memset(&w, 0, sizeof(w));
   size_t off = 0;
@@ -91,6 +97,20 @@ Workspace carve(const pob_render_config& c, int training, uint8_t* base) {
     for (int i = 0; i < 2; ++i) w.partials[i] = (float*)take(sizeof(float) * WG_MAX_CTAS * WG_PARTIAL_FLOATS);
     w.progress_bytes = sizeof(uint32_t) * size_t(w.lv[0].tiles + w.lv[1].tiles);
     w.progress = (uint32_t*)take(w.progress_bytes);
+  }
+  if (training && x3) {
+    for (int l = 0; l < 2; ++l) {
+      Level& L = w.lv[l];
+      if (R * Ns[l] == 0) continue;
+      L.H_lo = take(size_t(L.tiles) * NUM_TRUNK * A_TILE_BYTES);
+      L.E_lo = take(size_t(L.tiles) * E_TILE_BYTES);
+      L.DZ_lo = take(size_t(L.tiles) * NUM_TRUNK * A_TILE_BYTES);
+      L.DO_lo = take(size_t(L.tiles) * 2 * A_CHUNK_BYTES);
+    }
+    for (int i = 0; i < 2; ++i)
+      for (int q = 0; q < 2; ++q) w.partials_x3[i][q] = (float*)take(sizeof(float) * WG_MAX_CTAS * WG_PARTIAL_FLOATS);
+    const int K = c.sh_deg < 0 ? 1 : (c.sh_deg + 1) * (c.sh_deg + 1);
+    for (int i = 0; i < 2; ++i) w.wt_lo[i] = take(bwd_image_bytes(heads_width(K)));
   }
   w.total = off;
   return w;
@@ -145,6 +165,8 @@ int forward_levels(const char* where, const pob_render_config& c, Workspace& w, 
       p.save_h = C.H;
       p.save_e = C.E;
       p.save_mask = C.mask;
+      p.save_h_lo = C.H_lo;   // x3 only (null otherwise)
+      p.save_e_lo = C.E_lo;
     }
     { pob_count_launch(1); PobPhaseTimer _t(POB_PH_FWD, st); POB_CUDA(where, launch_mlp_fwd(p, precision, sms, st)); }
   }
@@ -166,6 +188,8 @@ int forward_levels(const char* where, const pob_render_config& c, Workspace& w, 
       p.save_h = F.H;
       p.save_e = F.E;
       p.save_mask = F.mask;
+      p.save_h_lo = F.H_lo;   // x3 only (null otherwise)
+      p.save_e_lo = F.E_lo;
     }
     { pob_count_launch(1); PobPhaseTimer _t(POB_PH_FWD, st); POB_CUDA(where, launch_mlp_fwd(p, precision, sms, st)); }
     { pob_count_launch(1); PobPhaseTimer _t(POB_PH_RENDER, st); POB_CUDA(where, launch_composite_fwd(F.rgbs, F.z, d, R, Nc + Nf, c.white_bkgd, F.comp, F.disp, F.acc,
@@ -184,6 +208,30 @@ __global__ void pack_outputs_kernel(const float* comp, const float* disp, const 
   out[5 * r + 4] = acc[r];
 }
 
+// The device allocation that holds `ws` must extend to ws + bytes: a workspace sized for the fp16 step (the x3
+// tail missing) is refused instead of written past.  The query is the driver's cuMemGetAddressRange, which neither
+// synchronises nor enqueues work, so the check is also made under stream capture.  It sees allocations, not the
+// blocks a caching allocator cuts out of them: a too-small block inside a larger allocation passes.
+int check_workspace_extent(const char* where, const void* ws, size_t bytes) {
+  using RangeFn = CUresult (*)(CUdeviceptr*, size_t*, CUdeviceptr);
+  static RangeFn range = [] {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPointByVersion("cuMemGetAddressRange", &fn, 12000, cudaEnableDefault, &q) != cudaSuccess ||
+        q != cudaDriverEntryPointSuccess)
+      fn = nullptr;
+    return reinterpret_cast<RangeFn>(fn);
+  }();
+  if (!range) return pob_fail(where, "cannot query the workspace allocation (cuMemGetAddressRange)");
+  CUdeviceptr base = 0;
+  size_t size = 0;
+  if (range(&base, &size, (CUdeviceptr)ws) != CUDA_SUCCESS)
+    return pob_fail(where, "workspace is not a device allocation");
+  if ((CUdeviceptr)ws + bytes > base + size)
+    return pob_fail(where, "workspace too small for this precision (pob_train_workspace_bytes)");
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -191,6 +239,15 @@ extern "C" {
 int64_t pob_workspace_bytes(const pob_render_config* cfg, int training) {
   if (check_cfg("pob_workspace_bytes", cfg)) return -1;
   return (int64_t)carve(*cfg, training, nullptr).total;
+}
+
+int64_t pob_train_workspace_bytes(const pob_render_config* cfg, int precision) {
+  if (check_cfg("pob_train_workspace_bytes", cfg)) return -1;
+  if (precision != POB_PREC_FP16 && precision != POB_PREC_FP16X3) {
+    pob_fail("pob_train_workspace_bytes", "precision must be POB_PREC_FP16 or POB_PREC_FP16X3");
+    return -1;
+  }
+  return (int64_t)carve(*cfg, 1, nullptr, precision == POB_PREC_FP16X3).total;
 }
 
 int pob_render_rays(const pob_render_config* cfg, const void* packed_coarse_dev, const void* packed_fine_dev,
@@ -222,20 +279,22 @@ int pob_render_rays(const pob_render_config* cfg, const void* packed_coarse_dev,
   return 0;
 }
 
-int pob_loss_and_grad(const pob_render_config* cfg, const pob_train_hparams* hp, const void* packed_coarse_dev,
-                      const void* packed_fine_dev, const float* origins_dev, const float* directions_dev,
-                      const float* viewdirs_dev, const float* pixels_dev, int n_rays, const float* z_base_dev,
-                      const float* t_rand_dev, const float* u_dev, int u_per_ray, const float* z_fine_dev,
-                      const float* sp_points_dev, float* grad_flat_dev, float* stats_dev, void* workspace_dev,
-                      void* mlp0_done_event, void* stream) {
+int pob_loss_and_grad_prec(const pob_render_config* cfg, const pob_train_hparams* hp, const void* packed_coarse_dev,
+                           const void* packed_fine_dev, const float* origins_dev, const float* directions_dev,
+                           const float* viewdirs_dev, const float* pixels_dev, int n_rays, const float* z_base_dev,
+                           const float* t_rand_dev, const float* u_dev, int u_per_ray, const float* z_fine_dev,
+                           const float* sp_points_dev, float* grad_flat_dev, float* stats_dev, void* workspace_dev,
+                           void* mlp0_done_event, const float* params_dev, int precision, void* stream) {
   const char* where = "pob_loss_and_grad";
   if (int e = check_cfg(where, cfg)) return e;
   if (!hp) return pob_fail(where, "hparams is NULL");
-  if (int e = pob_check_common(where, packed_coarse_dev, cfg->sh_deg, POB_PREC_FP16)) return e;
+  if (int e = pob_check_common(where, packed_coarse_dev, cfg->sh_deg, precision)) return e;
+  const bool x3 = precision == POB_PREC_FP16X3;
   if (n_rays <= 0 || n_rays > cfg->max_rays) return pob_fail(where, "n_rays out of range");
   if (!origins_dev || !directions_dev || !viewdirs_dev || !pixels_dev || !z_base_dev || !workspace_dev ||
       !grad_flat_dev || !stats_dev)
     return pob_fail(where, "NULL pointer");
+  if (x3 && !params_dev) return pob_fail(where, "POB_PREC_FP16X3 needs params_dev (the flat fp32 parameters)");
   const int Nc = cfg->num_coarse_samples, Nf = cfg->num_fine_samples;
   if (Nf > 0 && (!packed_fine_dev || (!u_dev && !z_fine_dev)))
     return pob_fail(where, "fine level needs packed_fine and u (or z_fine)");
@@ -246,15 +305,22 @@ int pob_loss_and_grad(const pob_render_config* cfg, const pob_train_hparams* hp,
   const int sms = pob_sm_count_cached();
   const int K = cfg->sh_deg < 0 ? 1 : (cfg->sh_deg + 1) * (cfg->sh_deg + 1);
   const int P = flat_layout(K).total;
-  Workspace w = carve(*cfg, 1, (uint8_t*)workspace_dev);
+  Workspace w = carve(*cfg, 1, (uint8_t*)workspace_dev, x3);
+  if (x3)
+    if (int e = check_workspace_extent(where, workspace_dev, w.total)) return e;
   POB_CUDA(where, cudaMemsetAsync(stats_dev, 0, 8 * sizeof(float), st));
   POB_CUDA(where, cudaMemsetAsync(w.progress, 0, w.progress_bytes, st));
+  if (x3) {
+    // residual of the transposed weights (the packed blob holds only their hi part)
+    for (int mlp = 0; mlp < (Nf > 0 ? 2 : 1); ++mlp)
+      { pob_count_launch(1); PobPhaseTimer _t(POB_PH_OPTIM, st); POB_CUDA(where, launch_pack_wt_lo(params_dev + size_t(mlp) * P, K, w.wt_lo[mlp], st)); }
+  }
   // The sparsity points (train.py:77-83: eval_points_raw of the fine MLP on uniform points) ride behind the ray
   // samples of the last level: same MLP, same launches, rows [n_rays * N, n_rays * N + sp_n) of its arrays.
   const long long sp_n = sparsity ? cfg->sparsity_npoints : 0;
   if (int e = forward_levels(where, *cfg, w, packed_coarse_dev, packed_fine_dev, origins_dev, directions_dev,
                              viewdirs_dev, n_rays, z_base_dev, t_rand_dev, u_dev, u_per_ray, z_fine_dev,
-                             POB_PREC_FP16, true, st, sp_points_dev, sp_n))
+                             precision, true, st, sp_points_dev, sp_n))
     return e;
   const float gscale = hp->loss_scale * 2.0f / (3.0f * float(n_rays));
   Level& C = w.lv[0];
@@ -277,7 +343,9 @@ int pob_loss_and_grad(const pob_render_config* cfg, const pob_train_hparams* hp,
   // (stop_gradient, model_utils.py:286), so the caller can all-reduce the MLP_0 bucket of the gradient
   // (mlp0_done_event) while the 3x larger MLP_1 backward is still running.
   // dgrad runs on `dgrad_ctas` SMs and wgrad alongside it on the rest, reading each dZ tile from L2 shortly after it
-  // was stored (wgrad_body.cuh).
+  // was stored (wgrad_body.cuh).  x3: the data gradient runs on all SMs, then the three wgrad passes (kernels.h:
+  // X3_WGRAD_PASSES) one after the other, each on all SMs.  SH16 step (bench.py's workload) on an H100 80 GB HBM3 at a
+  // 400 W power limit: 29.1-29.6 ms against 31.8-32.1 ms with the fp16 split (pass 0 beside the data gradient).
   const int dgrad_ctas = sms * DGRAD_SMS_OF_132 / 132;
   const int NH = heads_width(K);
   for (int mlp = 0; mlp < (Nf > 0 ? 2 : 1); ++mlp) {
@@ -301,22 +369,46 @@ int pob_loss_and_grad(const pob_render_config* cfg, const pob_train_hparams* hp,
     b.save_dz = L.DZ;
     b.save_do = L.DO;
     b.progress = w.progress + (mlp == 0 ? 0 : C.tiles);
-    { pob_count_launch(); PobPhaseTimer _t(POB_PH_BWD, st); POB_CUDA(where, launch_mlp_bwd(b, dgrad_ctas, st)); }
-    WgradParams g;
-    memset(&g, 0, sizeof(g));
-    g.seg = WgradSegment{L.H, L.DZ, L.E, L.DO};
-    g.seg_tiles = tiles_for(Mm);
-    g.NH = NH;
-    g.partials = w.partials[mlp];
-    g.progress = b.progress;
-    int rs[WG_NUM_ROLES], rc[WG_NUM_ROLES];
-    const int nctas = wgrad_assign_roles(g, sms - dgrad_ctas, rs, rc);
-    { pob_count_launch(); PobPhaseTimer _t(POB_PH_WGRAD, st); POB_CUDA(where, launch_mlp_wgrad(g, nctas, st)); }
-    { pob_count_launch(); PobPhaseTimer _t(POB_PH_OPTIM, st); POB_CUDA(where, launch_reduce_grads(w.partials[mlp], rs, rc, K, 1.0f / hp->loss_scale,
+    b.wt_lo = w.wt_lo[mlp];
+    b.save_dz_lo = L.DZ_lo;
+    b.save_do_lo = L.DO_lo;
+    { pob_count_launch(); PobPhaseTimer _t(POB_PH_BWD, st); POB_CUDA(where, launch_mlp_bwd(b, precision, x3 ? sms : dgrad_ctas, st)); }
+    const WgradSegment segs[X3_WGRAD_PASSES] = {{L.H, L.DZ, L.E, L.DO},
+                                                {L.H, L.DZ_lo, L.E, L.DO_lo},
+                                                {L.H_lo, L.DZ, L.E_lo, L.DO}};
+    float* const partials[X3_WGRAD_PASSES] = {w.partials[mlp], w.partials_x3[mlp][0], w.partials_x3[mlp][1]};
+    const int npass = x3 ? X3_WGRAD_PASSES : 1;
+    WgradPass passes[X3_WGRAD_PASSES];
+    for (int q = 0; q < npass; ++q) {
+      WgradParams g;
+      memset(&g, 0, sizeof(g));
+      g.seg = segs[q];
+      g.seg_tiles = tiles_for(Mm);
+      g.NH = NH;
+      g.partials = partials[q];
+      g.progress = b.progress;
+      passes[q].partials = partials[q];
+      const int nctas = wgrad_assign_roles(g, (q == 0 && !x3) ? sms - dgrad_ctas : sms, passes[q].role_start,
+                                           passes[q].role_count);
+      { pob_count_launch(); PobPhaseTimer _t(POB_PH_WGRAD, st); POB_CUDA(where, launch_mlp_wgrad(g, nctas, st)); }
+    }
+    { pob_count_launch(); PobPhaseTimer _t(POB_PH_OPTIM, st); POB_CUDA(where, launch_reduce_grads(passes, npass, K, 1.0f / hp->loss_scale,
                                         grad_flat_dev + size_t(mlp) * P, st)); }
     if (mlp == 0 && Nf > 0 && mlp0_done_event) POB_CUDA(where, cudaEventRecord((cudaEvent_t)mlp0_done_event, st));
   }
   return 0;
+}
+
+int pob_loss_and_grad(const pob_render_config* cfg, const pob_train_hparams* hp, const void* packed_coarse_dev,
+                      const void* packed_fine_dev, const float* origins_dev, const float* directions_dev,
+                      const float* viewdirs_dev, const float* pixels_dev, int n_rays, const float* z_base_dev,
+                      const float* t_rand_dev, const float* u_dev, int u_per_ray, const float* z_fine_dev,
+                      const float* sp_points_dev, float* grad_flat_dev, float* stats_dev, void* workspace_dev,
+                      void* mlp0_done_event, void* stream) {
+  return pob_loss_and_grad_prec(cfg, hp, packed_coarse_dev, packed_fine_dev, origins_dev, directions_dev, viewdirs_dev,
+                                pixels_dev, n_rays, z_base_dev, t_rand_dev, u_dev, u_per_ray, z_fine_dev, sp_points_dev,
+                                grad_flat_dev, stats_dev, workspace_dev, mlp0_done_event, nullptr, POB_PREC_FP16,
+                                stream);
 }
 
 int pob_adam_update(int sh_deg, int num_mlps, float* params_dev, const float* grads_dev, float* m_dev,

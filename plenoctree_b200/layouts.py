@@ -236,7 +236,12 @@ def padded_rows(M):
     return (M + 511) // 512 * 512
 
 
-def train_workspace_views(cfg, n_rays, sparsity_on, training=True):
+def bwd_image_bytes(K):
+    """bytes of one dgrad weight image (kernels.h: bwd_image_bytes)."""
+    return blob_layout(K)["bwd_bytes"]
+
+
+def train_workspace_views(cfg, n_rays, sparsity_on, training=True, precision=1):
     """Byte layout of the training workspace of `cfg` (a RenderConfig or anything with its fields) for a
     pob_loss_and_grad call over `n_rays` rays; `sparsity_on` = the call carries the sparsity points (weight > 0).
 
@@ -249,7 +254,12 @@ def train_workspace_views(cfg, n_rays, sparsity_on, training=True):
     padded row count.
 
     training=False: the render workspace of pob_render_rays (pob_workspace_bytes(cfg, 0)).  Each level then holds
-    only z, rgbs, weights, comp, disp and acc, no sparsity rows, and partials is empty."""
+    only z, rgbs, weights, comp, disp and acc, no sparsity rows, and partials is empty.
+
+    precision=3 (POB_PREC_FP16X3): the workspace of pob_loss_and_grad_prec at fp16x3
+    (pob_train_workspace_bytes(cfg, 3)): the fp16 views, plus per level the residual images H_lo, E_lo, DZ_lo, DO_lo
+    (shaped like H, E, DZ, DO), partials_x3 = [[mlp 0 pass 1, pass 2], [mlp 1 ...]] and wt_lo = [mlp 0, mlp 1]
+    (offset, bytes) of the residual dgrad weight images."""
     R = int(cfg.max_rays)
     nc, nf, nsp = int(cfg.num_coarse_samples), int(cfg.num_fine_samples), int(cfg.sparsity_npoints)
     Ns = [nc, nc + nf if nf > 0 else 0]
@@ -298,12 +308,21 @@ def train_workspace_views(cfg, n_rays, sparsity_on, training=True):
     progress = take(4 * sum(caps))   # mlp_bwd -> mlp_wgrad progress counters, level 0's tiles then level 1's
     for v, first in zip(levels, (0, caps[0])):
         v["progress"] = (progress + 4 * first, (v["tiles"],))
-    return dict(total=off, levels=levels, partials=partials)
+    if precision != 3:
+        return dict(total=off, levels=levels, partials=partials)
+    for v, cap in zip(levels, caps):
+        for name, per_tile in (("H", NUM_TRUNK * A_TILE_BYTES), ("E", E_TILE_BYTES), ("DZ", NUM_TRUNK * A_TILE_BYTES),
+                               ("DO", DO_TILE_BYTES)):
+            v[name + "_lo"] = (take(cap * per_tile), v[name][1])
+    partials_x3 = [[take(4 * WG_MAX_CTAS * WG_PARTIAL_FLOATS) for _ in range(2)] for _ in range(2)]
+    nb = bwd_image_bytes(K_of(int(cfg.sh_deg)))
+    wt_lo = [(take(nb), nb) for _ in range(2)]
+    return dict(total=off, levels=levels, partials=partials, partials_x3=partials_x3, wt_lo=wt_lo)
 
 
 _VIEW_DTYPES = dict(z="float32", rgbs="float32", weights="float32", comp="float32", disp="float32", acc="float32",
                     G="float32", H="uint8", E="uint8", DZ="uint8", DO="uint8", mask="int32",
-                    progress="int32")
+                    progress="int32", H_lo="uint8", E_lo="uint8", DZ_lo="uint8", DO_lo="uint8")
 
 
 def workspace_view(ws, level, name):

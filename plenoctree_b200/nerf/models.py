@@ -106,10 +106,14 @@ class NerfModel:
             check(lib.pob_pack_weights(ptr(self.params[i * self.P:(i + 1) * self.P]), self.sh_deg,
                                        ptr(self.blobs[i]), stream_ptr()))
 
-    def workspace(self, training):
-        key = bool(training)
+    def workspace(self, training, precision=PREC_FP16):
+        """device scratch of the render call (training False) or of the training step at `precision`"""
+        key = bool(training) if precision == PREC_FP16 else (bool(training), precision)
         if key not in self._ws:
-            nbytes = int(lib.pob_workspace_bytes(ctypes_ref(self.cfg), int(key)))
+            if training and precision != PREC_FP16:
+                nbytes = int(lib.pob_train_workspace_bytes(ctypes_ref(self.cfg), int(precision)))
+            else:
+                nbytes = int(lib.pob_workspace_bytes(ctypes_ref(self.cfg), int(bool(training))))
             if nbytes < 0:
                 raise _lib.PobError(lib.pob_last_error().decode())
             self._ws[key] = torch.empty(nbytes, dtype=torch.uint8, device=self.device)

@@ -16,7 +16,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from .._lib import TrainHParams, check, lib, ptr, stream_ptr
+from .._lib import PREC_FP16, PREC_FP16X3, TrainHParams, check, lib, ptr, stream_ptr
 from .models import _cuda_f32, ctypes_ref
 
 # nerf_sh/nerf/utils.py:43-50
@@ -62,16 +62,27 @@ class TrainState:
         return self.gbuf[self.model.params.numel():]
 
 
-def default_loss_scale(n_rays):
+# x3 training: extra factor of the loss scale.  The residual lo of a stored dZ entry falls into fp16's subnormal range
+# below |dZ| = 2^-3 (hi + lo then only holds ~2^-25 absolute), so the x3 step scales the chain up further.  2^8 keeps
+# the largest |dZ| of the production step 10x below 65504; 2^10 measured the same end-to-end gradient error with 2.4x
+# (DESIGN.md section 3).
+X3_LOSS_SCALE_FACTOR = 2.0 ** 8
+
+
+def default_loss_scale(n_rays, precision=PREC_FP16):
     """power-of-two scale that keeps the fp16 gradient chain in range: dL/dC = scale*2(C-px)/(3R)."""
-    return float(2 ** int(round(math.log2(128.0 * max(1, n_rays)))))
+    s = float(2 ** int(round(math.log2(128.0 * max(1, n_rays)))))
+    return s * X3_LOSS_SCALE_FACTOR if precision == PREC_FP16X3 else s
 
 
 def loss_and_grad(model, state, batch, sparsity_weight=1e-3, sparsity_length=0.05, sparsity_radius=1.5,
                   randomized=True, t_rand=None, u=None, sp_points=None, loss_scale=None, z_fine=None,
-                  sigma_noise=None, mlp0_event=None, lr_step_on_device=False):
+                  sigma_noise=None, mlp0_event=None, lr_step_on_device=False, precision=PREC_FP16):
     """value_and_grad(loss_fn) for this rank's shard; fills state.grads / state.stats_raw (device).
-    mlp0_event (torch.cuda.Event): recorded on the current stream once the MLP_0 half of the gradient is final."""
+    mlp0_event (torch.cuda.Event): recorded on the current stream once the MLP_0 half of the gradient is final.
+    precision: PREC_FP16 (default) or PREC_FP16X3, the error-compensated forward / data / weight gradient."""
+    if precision not in (PREC_FP16, PREC_FP16X3):
+        raise ValueError("precision must be PREC_FP16 or PREC_FP16X3")
     rays = batch["rays"]
     o = _cuda_f32(rays.origins, "rays.origins", 3)
     d = _cuda_f32(rays.directions, "rays.directions", 3)
@@ -92,15 +103,18 @@ def loss_and_grad(model, state, batch, sparsity_weight=1e-3, sparsity_length=0.0
             raise ValueError("sp_points must have sparsity_npoints rows")
     z_fine = None if z_fine is None else _cuda_f32(z_fine, "z_fine")   # keep alive until the launch
     noise = model._set_sigma_noise(n, randomized, sigma_noise)          # noqa: F841  (same)
-    ws = model.workspace(True)
+    ws = model.workspace(True, precision)
     hp = TrainHParams(float(sparsity_weight if use_sp else 0.0), float(sparsity_length),
-                      float(loss_scale or default_loss_scale(n)))
-    check(lib.pob_loss_and_grad(ctypes_ref(model.cfg), ctypes_ref(hp), ptr(model.blobs[0]),
-                                ptr(model.blobs[1]) if model.num_mlps == 2 else None, ptr(o), ptr(d), ptr(v),
-                                ptr(px), n, ptr(model.z_base), ptr(t_rand), ptr(u), upr,
-                                ptr(z_fine), ptr(sp_points) if use_sp else None, ptr(state.grads),
-                                ptr(state.stats_raw), ptr(ws),
-                                mlp0_event.cuda_event if mlp0_event is not None else None, stream_ptr()))
+                      float(loss_scale or default_loss_scale(n, precision)))
+    args = (ctypes_ref(model.cfg), ctypes_ref(hp), ptr(model.blobs[0]),
+            ptr(model.blobs[1]) if model.num_mlps == 2 else None, ptr(o), ptr(d), ptr(v),
+            ptr(px), n, ptr(model.z_base), ptr(t_rand), ptr(u), upr,
+            ptr(z_fine), ptr(sp_points) if use_sp else None, ptr(state.grads),
+            ptr(state.stats_raw), ptr(ws), mlp0_event.cuda_event if mlp0_event is not None else None)
+    if precision == PREC_FP16:
+        check(lib.pob_loss_and_grad(*args, stream_ptr()))
+    else:
+        check(lib.pob_loss_and_grad_prec(*args, ptr(model.params), int(precision), stream_ptr()))
     return n
 
 
@@ -177,7 +191,7 @@ def shard_batch(batch_size, rank, world):
 
 def train_step(model, state, batch, lr, sparsity_weight=1e-3, sparsity_length=0.05, sparsity_radius=1.5,
                weight_decay_mult=0.0, randomized=True, t_rand=None, u=None, sp_points=None, loss_scale=None,
-               sync_stats=False, lr_step_on_device=False, collective=True):
+               sync_stats=False, lr_step_on_device=False, collective=True, precision=PREC_FP16):
     """One optimisation step (nerf_sh/train.py:51-121).  Returns Stats when sync_stats (forces a
     device->host read of the six scalars, like the reference's periodic logging), else None."""
     world = _world() if collective else 1     # collective=False: single-rank semantics inside a multi-rank job
@@ -187,7 +201,8 @@ def train_step(model, state, batch, lr, sparsity_weight=1e-3, sparsity_length=0.
         # recorded inside pob_loss_and_grad), hidden under the MLP_1 backward; [MLP_1 | stats] follows on this stream
         side, ev_mlp0, ev_b0 = _bucket_plumbing(state)
         n = loss_and_grad(model, state, batch, sparsity_weight, sparsity_length, sparsity_radius, randomized, t_rand,
-                          u, sp_points, loss_scale, mlp0_event=ev_mlp0, lr_step_on_device=lr_step_on_device)
+                          u, sp_points, loss_scale, mlp0_event=ev_mlp0, lr_step_on_device=lr_step_on_device,
+                          precision=precision)
         side.wait_event(ev_mlp0)
         with torch.cuda.stream(side):
             dist.all_reduce(state.gbuf[:P], op=dist.ReduceOp.SUM)
@@ -196,7 +211,7 @@ def train_step(model, state, batch, lr, sparsity_weight=1e-3, sparsity_length=0.
         torch.cuda.current_stream().wait_event(ev_b0)
     else:
         n = loss_and_grad(model, state, batch, sparsity_weight, sparsity_length, sparsity_radius, randomized, t_rand,
-                          u, sp_points, loss_scale, lr_step_on_device=lr_step_on_device)
+                          u, sp_points, loss_scale, lr_step_on_device=lr_step_on_device, precision=precision)
         if world > 1:
             allreduce_gradients(state.gbuf)   # pmean(grad) and pmean(stats) in one bucket
     # weight_l2 = sum(theta^2)/numel  ->  d/dtheta = 2*theta/numel  (train.py:101-108,114)
@@ -229,7 +244,7 @@ class GraphedTrainStep:
     HYPER_SLOTS = 16
 
     def __init__(self, model, state, n_rays, sparsity_weight=1e-3, sparsity_length=0.05, sparsity_radius=1.5,
-                 weight_decay_mult=0.0, warmup=3, collective=True):
+                 weight_decay_mult=0.0, warmup=3, collective=True, precision=PREC_FP16):
         self.model, self.state, self.n = model, state, int(n_rays)
         dev = model.device
         self.buf = torch.zeros((self.n, 12), dtype=torch.float32, device=dev)       # [o | d | v | px]
@@ -240,7 +255,7 @@ class GraphedTrainStep:
         self._slot = 0
         self.kw = dict(sparsity_weight=sparsity_weight, sparsity_length=sparsity_length,
                        sparsity_radius=sparsity_radius, weight_decay_mult=weight_decay_mult, lr_step_on_device=True,
-                       collective=collective)
+                       collective=collective, precision=precision)
         b = self._batch()
         # warm-up on a side stream (allocations, NCCL communicator, lazy module loads), then capture
         s = torch.cuda.Stream(device=dev)

@@ -10,12 +10,18 @@ import time
 import numpy as np
 import torch
 import torch.distributed as dist
-from absl import app
+from absl import app, flags
 
+from .._lib import PREC_FP16, PREC_FP16X3
 from ..nerf import checkpoints, datasets, flags as F, models, train as T, utils
 
 FLAGS = F.FLAGS
 F.define_flags()
+# not a reference flag: fp16x3 trains with error-compensated operands (fp32-class gradients, DESIGN.md section 3)
+if "train_precision" not in FLAGS:
+    flags.DEFINE_enum("train_precision", "fp16", ["fp16", "fp16x3"],
+                      "tensor-core operands of the training step: fp16, or the hi + lo split fp16x3.")
+_TRAIN_PRECISION = {"fp16": PREC_FP16, "fp16x3": PREC_FP16X3}
 
 
 from .._dist import dist_init as _dist_init  # noqa: E402
@@ -67,7 +73,7 @@ def main(unused_argv):
         stats = T.train_step(model, state, batch, lr, sparsity_weight=FLAGS.sparsity_weight,
                              sparsity_length=FLAGS.sparsity_length, sparsity_radius=FLAGS.sparsity_radius,
                              weight_decay_mult=FLAGS.weight_decay_mult, randomized=FLAGS.randomized,
-                             sync_stats=want_stats)
+                             sync_stats=want_stats, precision=_TRAIN_PRECISION[FLAGS.train_precision])
         if step % FLAGS.gc_every == 0:
             gc.collect()
         if rank == 0 and stats is not None:
