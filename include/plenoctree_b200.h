@@ -283,6 +283,13 @@ int pob_octree_train_persp(const pob_octree* tree, const pob_octree_opts* opts, 
  * data -= lr * grad; grad = 0, touching only entries whose gradient is non-zero. */
 int pob_octree_sgd_step(float* data_dev, float* grad_dev, int64_t n, float lr, void* stream);
 
+/* torch.optim.SGD(lr, momentum, dampening 0, nesterov).step() fused with zero_grad (octree/optimization.py:180-181,
+ * 205-208), every element: buf = momentum * buf + grad (two roundings, as torch); d = nesterov ? grad + momentum * buf
+ * : buf; data -= lr * d; grad = 0.  buf_dev is the caller's momentum buffer (same length as data), zero before the
+ * first step.  Entries with grad = buf = 0 are not written.  momentum must be finite and >= 0. */
+int pob_octree_sgd_momentum_step(float* data_dev, float* grad_dev, float* buf_dev, int64_t n, float lr, float momentum,
+                                 int nesterov, void* stream);
+
 /* torch.optim.Adam(lr, eps) (betas 0.9 / 0.999, no weight decay; octree/optimization.py:190-193, the `--nosgd` branch)
  * fused with zero_grad: m, v are the caller's moment buffers (same shape as data), `step` = updates already applied. */
 int pob_octree_adam_step(float* data_dev, float* grad_dev, float* m_dev, float* v_dev, int64_t n, float lr, float step,

@@ -134,7 +134,7 @@ pob::FwdParams pob_base_params(const void* packed, int sh_deg) { return base_par
 
 extern "C" {
 
-int pob_abi_version(void) { return 6; }   // 6: pob_train_workspace_bytes, pob_loss_and_grad_prec (fp16x3 training); 5: sm_90a, no debug-trace / descriptor-probe entry points; 4: pob_loss_and_grad(mlp0_done_event), pob_adam_update(lr_step_dev)
+int pob_abi_version(void) { return 7; }   // 7: pob_octree_sgd_momentum_step; 6: pob_train_workspace_bytes, pob_loss_and_grad_prec (fp16x3 training); 5: sm_90a, no debug-trace / descriptor-probe entry points; 4: pob_loss_and_grad(mlp0_done_event), pob_adam_update(lr_step_dev)
 
 long long pob_launch_count(void) { return g_launches.load(); }
 

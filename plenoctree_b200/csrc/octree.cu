@@ -608,6 +608,66 @@ __global__ void octree_sgd_kernel(float* __restrict__ data, float* __restrict__ 
   }
 }
 
+// One element of torch.optim.SGD(lr, momentum=mu, dampening=0, nesterov): b <- mu*b + g with two roundings, as torch's
+// buf.mul_(mu).add_(g) (a zero buffer gives fl(fl(mu*0) + g) = g, torch's first-step clone(g)); the direction
+// d = nesterov ? g + mu*b : b (one FMA, torch's grad.add(buf, alpha=mu)); data <- data - lr*d (one FMA).
+__device__ __forceinline__ void sgd_momentum_elem(float& data, float g, float& b, float lr, float mu, bool nesterov) {
+  b = __fadd_rn(__fmul_rn(mu, b), g);
+  const float d = nesterov ? __fmaf_rn(mu, b, g) : b;
+  data = __fmaf_rn(-lr, d, data);
+}
+
+// The SGD-with-momentum step fused with zero_grad (octree/optimization.py:180-181,205-208).  Elements with g = 0 and
+// b = 0 are only read (g, b) and keep their bits; elements with g = 0 and b != 0 still move.  Up to 28 B per element
+// (read g, b, data; write data, b, g) against the plain step's 16 B.
+__global__ void octree_sgd_momentum_kernel(float* __restrict__ data, float* __restrict__ grad, float* __restrict__ buf,
+                                           long long n, float lr, float mu, bool nesterov) {
+  const long long n4 = n / 4;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  float4* d4 = reinterpret_cast<float4*>(data);
+  float4* g4 = reinterpret_cast<float4*>(grad);
+  float4* b4 = reinterpret_cast<float4*>(buf);
+  // four independent 16-byte loads of g and of b in flight per thread, as in octree_sgd_kernel
+  for (long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x; i0 < n4; i0 += 4 * stride) {
+    float4 g[4], b[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const long long i = i0 + u * stride;
+      g[u] = i < n4 ? __ldcs(g4 + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+      b[u] = i < n4 ? __ldcs(b4 + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const long long i = i0 + u * stride;
+      const bool gx = g[u].x != 0.f, gy = g[u].y != 0.f, gz = g[u].z != 0.f, gw = g[u].w != 0.f;
+      const bool mx = gx || b[u].x != 0.f, my = gy || b[u].y != 0.f, mz = gz || b[u].z != 0.f,
+                 mw = gw || b[u].w != 0.f;
+      if (mx || my || mz || mw) {
+        float4 d = d4[i];
+        float4 bb = b[u];
+        if (mx) sgd_momentum_elem(d.x, g[u].x, bb.x, lr, mu, nesterov);
+        if (my) sgd_momentum_elem(d.y, g[u].y, bb.y, lr, mu, nesterov);
+        if (mz) sgd_momentum_elem(d.z, g[u].z, bb.z, lr, mu, nesterov);
+        if (mw) sgd_momentum_elem(d.w, g[u].w, bb.w, lr, mu, nesterov);
+        d4[i] = d;
+        b4[i] = bb;
+        if (gx || gy || gz || gw) g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+    }
+  }
+  for (long long i = n4 * 4 + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const float g = grad[i];
+    float b = buf[i];
+    if (g != 0.f || b != 0.f) {
+      float d = data[i];
+      sgd_momentum_elem(d, g, b, lr, mu, nesterov);
+      data[i] = d;
+      buf[i] = b;
+      if (g != 0.f) grad[i] = 0.f;
+    }
+  }
+}
+
 // N3Tree.__getitem__(points) (svox query_vertical): world points -> packed leaf index node*N^3 + (i*N+j)*N+k
 __global__ void octree_query_kernel(TreeDev T, const float* __restrict__ pts, long long n, long long* __restrict__ out) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -866,6 +926,25 @@ int pob_octree_sgd_step(float* data_dev, float* grad_dev, int64_t n, float lr, v
   if (n == 0) return 0;
   pob_count_launch();
   octree_sgd_kernel<<<sms * 16, 256, 0, (cudaStream_t)stream>>>(data_dev, grad_dev, n, lr);
+  POB_CUDA(W, cudaGetLastError());
+  return 0;
+}
+
+int pob_octree_sgd_momentum_step(float* data_dev, float* grad_dev, float* buf_dev, int64_t n, float lr, float momentum,
+                                 int nesterov, void* stream) {
+  const char* W = "pob_octree_sgd_momentum_step";
+  if (!data_dev || !grad_dev || !buf_dev) return pob_fail(W, "NULL pointer");
+  if (n < 0) return pob_fail(W, "negative size");
+  if (!(momentum >= 0.f) || !isfinite(momentum)) return pob_fail(W, "momentum must be finite and >= 0");
+  const int sms = pob_sm_count_cached();
+  if (sms <= 0) return pob_fail(W, "no sm_90 CUDA device (there is no CPU fallback)");
+  if ((reinterpret_cast<uintptr_t>(data_dev) | reinterpret_cast<uintptr_t>(grad_dev) |
+       reinterpret_cast<uintptr_t>(buf_dev)) & 15)
+    return pob_fail(W, "data / grad / buf must be 16-byte aligned");
+  if (n == 0) return 0;
+  pob_count_launch();
+  octree_sgd_momentum_kernel<<<sms * 16, 256, 0, (cudaStream_t)stream>>>(data_dev, grad_dev, buf_dev, n, lr, momentum,
+                                                                         nesterov != 0);
   POB_CUDA(W, cudaGetLastError());
   return 0;
 }

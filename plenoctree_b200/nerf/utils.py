@@ -108,3 +108,20 @@ def save_img(img, pth):
     from PIL import Image
     arr = img.detach().cpu().numpy() if hasattr(img, "detach") else np.asarray(img)
     Image.fromarray((np.clip(arr, 0.0, 1.0) * 255.0).astype(np.uint8)).save(pth, "PNG")
+
+
+def write_video(path, frames, fps):
+    """frames [n,h,w,3] float in [0,1] -> mp4 (OpenCV's mp4v writer stands in for imageio.mimwrite, which this image
+    does not carry); returns False when no encoder is available."""
+    try:
+        import cv2
+    except ImportError:
+        return False
+    h, w = frames.shape[1:3]
+    vw = cv2.VideoWriter(path, cv2.VideoWriter_fourcc(*"mp4v"), float(fps), (w, h))
+    if not vw.isOpened():
+        return False
+    for f in frames:
+        vw.write(np.ascontiguousarray((np.clip(f, 0.0, 1.0) * 255).astype(np.uint8)[..., ::-1]))     # RGB -> BGR
+    vw.release()
+    return True

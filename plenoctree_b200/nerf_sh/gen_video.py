@@ -13,6 +13,7 @@ from .. import _dist
 from ..nerf import checkpoints, flags as F, models, utils
 from ..nerf.models import Rays
 from ..nerf.rays import generate_rays, pose_spherical
+from ..nerf.utils import write_video
 
 FLAGS = F.FLAGS
 F.define_flags()
@@ -36,22 +37,6 @@ def orbit_poses(num_views, elevation, radius, up_axis):
     """[num_views,4,4] cameras on a circle around the up axis (gen_video.py:113-119; up_axis is 1-based)."""
     angles = np.linspace(-180, 180, num_views + 1)[:-1]
     return np.stack([pose_spherical(a, elevation, radius, up_axis - 1) for a in angles], 0)
-
-
-def write_video(path, frames, fps):
-    """frames [n,h,w,3] float in [0,1] -> mp4; returns False when no encoder is available."""
-    try:
-        import cv2
-    except ImportError:
-        return False
-    h, w = frames.shape[1:3]
-    vw = cv2.VideoWriter(path, cv2.VideoWriter_fourcc(*"mp4v"), float(fps), (w, h))
-    if not vw.isOpened():
-        return False
-    for f in frames:
-        vw.write(np.ascontiguousarray((np.clip(f, 0.0, 1.0) * 255).astype(np.uint8)[..., ::-1]))     # RGB -> BGR
-    vw.release()
-    return True
 
 
 def main(unused_argv):

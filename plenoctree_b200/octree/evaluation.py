@@ -6,7 +6,7 @@ import os
 import numpy as np
 import torch
 
-from ..nerf.utils import compute_psnr, compute_ssim, save_img
+from ..nerf.utils import compute_psnr, compute_ssim, save_img, write_video
 from .n3tree import N3Tree
 from .renderer import VolumeRenderer
 
@@ -36,11 +36,22 @@ def eval_octree(t, dataset, args, want_frames=False, lpips_fn=None, metrics=None
     return (avg_psnr / n, avg_ssim / n, frames) if want_frames else (avg_psnr / n, avg_ssim / n)
 
 
-def main(unused_argv):
-    from ..nerf import datasets, flags as F
+def _define_cli_flags():
+    from ..nerf import flags as F
     F.define_flags(octree=True)
     F.define({"input": ("string", "./tree.npz", "Input octree npz"),
+              "write_vid": ("string", None, "If specified, writes rendered video to given path (*.mp4)"),
               "write_images": ("string", None, "If specified, writes rendered images to this directory")})
+    return F
+
+
+def _cli_main(argv):
+    main(argv)          # absl exits with main's return value; the command line exits 0 on success
+
+
+def main(unused_argv):
+    from ..nerf import datasets
+    F = _define_cli_flags()
     FLAGS = F.FLAGS
     F.update_flags(FLAGS)
     dev = torch.device("cuda")
@@ -50,6 +61,11 @@ def main(unused_argv):
     extra = {}
     psnr, ssim, frames = eval_octree(t, dataset, FLAGS, want_frames=True, lpips_fn=load_lpips(dev), metrics=extra)
     print("Average PSNR", psnr, "SSIM", ssim, "LPIPS", extra["lpips"])
+    if FLAGS.write_vid and frames:
+        # evaluation.py:88-90: imageio.mimwrite at its default 10 fps
+        print("Writing to", FLAGS.write_vid)
+        if not write_video(FLAGS.write_vid, np.stack(frames).astype(np.float32) / 255.0, 10):
+            print("* No mp4 encoder available: frames only")
     if FLAGS.write_images:
         os.makedirs(FLAGS.write_images, exist_ok=True)
         for i, fr in enumerate(frames):
@@ -59,4 +75,5 @@ def main(unused_argv):
 
 if __name__ == "__main__":
     from absl import app
-    app.run(main)
+    _define_cli_flags()       # before app.run parses the command line
+    app.run(_cli_main)

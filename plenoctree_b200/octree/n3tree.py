@@ -210,12 +210,31 @@ class N3Tree:
             self.grad = torch.zeros_like(self.data)
         return self.grad
 
+    @staticmethod
+    def check_sgd_options(momentum, nesterov):
+        """torch.optim.SGD's checks on (momentum, nesterov), with its messages; -> momentum as a float."""
+        momentum = float(momentum)
+        if momentum < 0.0:
+            raise ValueError(f"Invalid momentum value: {momentum}")
+        if nesterov and momentum <= 0.0:
+            raise ValueError("Nesterov momentum requires a momentum and zero dampening")
+        return momentum
+
     @torch.no_grad()
-    def sgd_step(self, lr):
-        """torch.optim.SGD(lr, momentum=0).step() + zero_grad (octree/optimization.py:187-189,205-208)."""
+    def sgd_step(self, lr, momentum=0.0, nesterov=False):
+        """torch.optim.SGD(lr, momentum, nesterov=nesterov).step() + zero_grad (octree/optimization.py:180-181,
+        205-208).  With momentum the buffer (`_sgd_buf`, zero on first use, like torch's clone of the first gradient)
+        lives with this tree across images and epochs; clone() and shrink_to_fit() drop it."""
+        momentum = self.check_sgd_options(momentum, nesterov)
         g = self.grad_buffer()
         n = self.n_internal * self.N ** 3 * self.data_dim
-        check(lib.pob_octree_sgd_step(ptr(self.data), ptr(g), n, float(lr), stream_ptr()))
+        if momentum == 0.0:
+            check(lib.pob_octree_sgd_step(ptr(self.data), ptr(g), n, float(lr), stream_ptr()))
+            return
+        if getattr(self, "_sgd_buf", None) is None or self._sgd_buf.shape != self.data.shape:
+            self._sgd_buf = torch.zeros_like(self.data)
+        check(lib.pob_octree_sgd_momentum_step(ptr(self.data), ptr(g), ptr(self._sgd_buf), n, float(lr), momentum,
+                                               int(bool(nesterov)), stream_ptr()))
 
     @torch.no_grad()
     def adam_step(self, lr, eps=1e-8):
@@ -236,6 +255,7 @@ class N3Tree:
         self.parent_depth = self.parent_depth[:n].clone()
         self.grad = None
         self._leaves = None
+        self._sgd_buf = None
 
     def clone(self, device=None):
         t = N3Tree.__new__(N3Tree)
@@ -247,6 +267,7 @@ class N3Tree:
         t.grad = None
         t._leaves = None
         t._adam = None
+        t._sgd_buf = None
         return t
 
     def state(self):

@@ -3,7 +3,9 @@
     reference                                             here
     run_test_step          optimization.py:191-209        run_test_step
     epoch loop             optimization.py:213-243        optimize  (SGD path: one fused launch per image +
-                                                          pob_octree_sgd_step; no autograd graph)
+                                                          pob_octree_sgd_step, or pob_octree_sgd_momentum_step
+                                                          with --sgd_momentum / --sgd_nesterov; no autograd graph)
+    --render_interval      optimization.py:163-164,202-205  run_test_step(vis_dir, i, render_interval)
     svox.N3Tree.load/save  optimization.py:168,245-248    plenoctree_b200.octree.N3Tree
 
 Multi-GPU (SURVEY §8e, C5): every image's pixel rows are split over the ranks, each rank scatters into its own
@@ -11,6 +13,7 @@ dense gradient buffer, and the touched rows are exchanged (exchange_gradients: c
 before the replicated SGD update.  Both optimiser branches of the reference are fused with zero_grad: SGD (`--sgd`, all shipped configs) and Adam (`--nosgd`).
 """
 import math
+import os
 import types
 
 import numpy as np
@@ -88,18 +91,37 @@ def exchange_gradients(tree, sparse=True):
             "bytes_per_rank": kmax * (D * 4 + 8)}
 
 
-def run_test_step(r, test_c2w, test_gt, H, W, focal):
-    """optimization.py:191-209: mean PSNR of full-quality renders (fast=False) over the validation images."""
+def render_dir(input_path):
+    """optimization.py:163: where --render_interval writes its validation images."""
+    return os.path.splitext(input_path)[0] + "_render"
+
+
+def render_vis_name(vis_dir, i, j):
+    """optimization.py:205: validation view j at validation i (0 = before training, epoch + 1 after it)."""
+    return f"{vis_dir}/{i:04}_{j:04}.png"
+
+
+def render_vis_image(im_gt, im):
+    """optimization.py:203-204: [ground truth | clamped render] side by side, scaled by 255 and truncated to uint8."""
+    return (torch.cat((im_gt.to(im.device), im), dim=1) * 255).cpu().numpy().astype(np.uint8)
+
+
+def run_test_step(r, test_c2w, test_gt, H, W, focal, vis_dir=None, i=0, render_interval=0):
+    """optimization.py:191-209: mean PSNR of full-quality renders (fast=False) over the validation images.  With
+    vis_dir and render_interval K > 0, every K-th view is also written as a [gt | render] PNG."""
+    from PIL import Image
     tpsnr = 0.0
     with torch.no_grad():
-        for c2w, im_gt in zip(test_c2w, test_gt):
+        for j, (c2w, im_gt) in enumerate(zip(test_c2w, test_gt)):
             im = r.render_persp(c2w, height=H, width=W, fx=focal, fast=False).clamp_(0.0, 1.0)
             mse = ((im - im_gt.to(im.device)) ** 2).mean()
             tpsnr += -10.0 * math.log10(float(mse))
+            if vis_dir is not None and render_interval > 0 and j % render_interval == 0:
+                Image.fromarray(render_vis_image(im_gt, im)).save(render_vis_name(vis_dir, i, j), "PNG")
     return tpsnr / max(len(test_c2w), 1)
 
 
-def train_epoch(tree, r, train_c2w, train_gt, H, W, focal, lr, adam_eps=None):
+def train_epoch(tree, r, train_c2w, train_gt, H, W, focal, lr, adam_eps=None, momentum=0.0, nesterov=False):
     """one pass over the training images (optimization.py:216-229); returns the mean train PSNR."""
     import torch.distributed as dist
     rank, world = _rank_world()
@@ -110,7 +132,7 @@ def train_epoch(tree, r, train_c2w, train_gt, H, W, focal, lr, adam_eps=None):
         if world > 1:
             exchange_gradients(tree, sparse=False)   # dense wins: one image touches most visible leaves (see below)
         if adam_eps is None:
-            tree.sgd_step(lr)
+            tree.sgd_step(lr, momentum, nesterov)     # after the exchange: every rank's momentum buffer stays equal
         else:
             tree.adam_step(lr, adam_eps)
     if world > 1:
@@ -122,21 +144,27 @@ def train_epoch(tree, r, train_c2w, train_gt, H, W, focal, lr, adam_eps=None):
 def optimize(args, tree, train_c2w, train_gt, test_c2w, test_gt, focal, log=print):
     """optimization.py:134-248 without dataset/flag plumbing.  train_gt/test_gt: [n,H,W,3] float tensors."""
     adam_eps = None if args.sgd else 1e-8      # optimization.py:190-193 (1e-4 only for fp16 trees)
-    if args.sgd and (args.sgd_momentum != 0.0 or args.sgd_nesterov):
-        raise NotImplementedError("SGD momentum is not built (reference configs use momentum 0)")
+    momentum, nesterov = float(args.sgd_momentum), bool(args.sgd_nesterov)
+    if args.sgd:
+        N3Tree.check_sgd_options(momentum, nesterov)     # torch.optim.SGD raises when it is built, before any render
     H, W = int(train_gt[0].shape[0]), int(train_gt[0].shape[1])
     rank, _ = _rank_world()
     if rank != 0:                       # every rank renders / trains the same replicated tree; rank 0 talks and saves
         log = lambda *a, **k: None      # noqa: E731
+    K = int(getattr(args, "render_interval", 0) or 0)
+    vis_dir = None
+    if K > 0 and rank == 0:
+        vis_dir = render_dir(args.input)
+        os.makedirs(vis_dir, exist_ok=True)
     r = VolumeRenderer(tree, step_size=args.renderer_step_size)
-    best_validation_psnr = run_test_step(r, test_c2w, test_gt, H, W, focal)
+    best_validation_psnr = run_test_step(r, test_c2w, test_gt, H, W, focal, vis_dir, 0, K)
     log(f"** initial val psnr {best_validation_psnr}")
     best_t = None
     for i in range(args.num_epochs):
-        tpsnr = train_epoch(tree, r, train_c2w, train_gt, H, W, focal, args.lr, adam_eps)
+        tpsnr = train_epoch(tree, r, train_c2w, train_gt, H, W, focal, args.lr, adam_eps, momentum, nesterov)
         log(f"** train_psnr {tpsnr}")
         if i % args.val_interval == args.val_interval - 1 or i == args.num_epochs - 1:
-            validation_psnr = run_test_step(r, test_c2w, test_gt, H, W, focal)
+            validation_psnr = run_test_step(r, test_c2w, test_gt, H, W, focal, vis_dir, i + 1, K)
             log(f"** val psnr {validation_psnr} best {best_validation_psnr}")
             if validation_psnr > best_validation_psnr:
                 best_validation_psnr = validation_psnr
@@ -170,6 +198,10 @@ def _define_cli_flags():
         "continue_on_decrease": ("bool", False, "If set, continues training even if validation PSNR decreases"),
     })
     return F
+
+
+def _cli_main(argv):
+    main(argv)          # absl exits with main's return value; the command line exits 0 on success
 
 
 def main(unused_argv):
@@ -206,4 +238,4 @@ def main(unused_argv):
 if __name__ == "__main__":
     from absl import app
     _define_cli_flags()
-    app.run(main)
+    app.run(_cli_main)
