@@ -504,6 +504,46 @@ def grid_weight_render(sigma_grid, origins, dirs, offset, invradius, step_size=1
     return gw
 
 
+def grid_march_visits(reso, origins, dirs, offset, invradius, step_size=1e-3):
+    """The voxel visits of `grid_weight_render`'s float32 march (same setup, clamp to 1 - 1e-6, floor and
+    _dda_unit), ray by ray in march order, as if no ray stopped early: dict of
+        ray [V] int64, voxel [V] int64 (flat x-major index), delta_t [V] float32   one entry per visit
+        delta_scale [R] float32, miss [R] bool (the ray misses the box)
+    The positions depend on the ray geometry alone.  sigma selects the hits (sigma > sigma_thresh) and ends a ray
+    early through stop_thresh (with stop_thresh = 0 only once its light is exactly 0), so one list serves any grid."""
+    R = np.asarray(origins).shape[0]
+    o, d, delta_scale, invdir, tmin, tmax = _setup(np.asarray(offset, dtype=f32), np.asarray(invradius, dtype=f32),
+                                                   origins, dirs)
+    miss = (tmax < 0) | (tmin > tmax)
+    t = tmin.copy()
+    active = ~miss & (t < tmax)
+    steps = []
+    while active.any():
+        a = np.nonzero(active)[0]
+        pos = (o[a] + t[a][:, None] * d[a]).astype(f32)
+        pos = np.maximum(f32(0.0), np.minimum(f32(1.0) - f32(1e-6), pos)).astype(f32)
+        pos = (pos * f32(reso)).astype(f32)
+        u = np.floor(pos).astype(np.int64)
+        rel = (pos - u.astype(f32)).astype(f32)
+        smin, smax = _dda_unit(rel, invdir[a])
+        delta_t = (((smax - smin) / f32(reso)).astype(f32) + f32(step_size)).astype(f32)
+        steps.append((a, (u[:, 0] * reso + u[:, 1]) * reso + u[:, 2], delta_t))
+        t[a] = (t[a] + delta_t).astype(f32)
+        active[a] = t[a] < tmax[a]
+    # every active ray takes one step per iteration and a ray that leaves never returns, so iteration k holds
+    # visit k of each of its rays: scatter straight into ray-major order
+    count = np.zeros(R, dtype=np.int64)
+    for a, _, _ in steps:
+        count[a] += 1
+    first = np.cumsum(count) - count
+    V = int(count.sum())
+    ray, vox, dt = np.empty(V, np.int64), np.empty(V, np.int64), np.empty(V, f32)
+    for k, (a, v, dtk) in enumerate(steps):
+        at = first[a] + k
+        ray[at], vox[at], dt[at] = a, v, dtk
+    return dict(ray=ray, voxel=vox, delta_t=dt, delta_scale=delta_scale, miss=miss)
+
+
 def build_tree_from_grid(mask, init_grid_depth, radius, center, data_dim, data_format, refine_chunk=2000000):
     """octree/extraction.py:330-353 restated literally: the voxel centres of the masked init grid
     (reso = 2^(init_grid_depth+1), x-major like torch.meshgrid(...).reshape(3,-1).T) refine the tree
