@@ -359,6 +359,46 @@ __host__ __device__ __forceinline__ constexpr uint32_t a_tile_offset(int row, in
   return uint32_t(col >> 6) * A_CHUNK_BYTES + uint32_t(row) * 128u +
          ((uint32_t((col >> 3) & 7) ^ uint32_t(row & 7)) << 4) + uint32_t(col & 7) * 2u;
 }
+// Saved activation tile ("T image", layouts.py: t_tile_offset): [32-row group][8-column group][row & 31][16 B], so
+// a warp's store of one 8-column group of an accumulator fragment is one contiguous 512 B.  t_frag_base: byte offset,
+// in the [tiles][NUM_TRUNK] T images, of the first fragment element of thread `lane` of warp `wq` of warpgroup `wg`
+// (row 64wg + 16wq + lane/4, column 2(lane%4)) in layer `layer`'s tile `it`; t_frag_offset: that element's
+// offset in 8-column group g, row + 8h.
+__device__ __forceinline__ size_t t_frag_base(long long it, int layer, int wg, int wq, uint32_t lane) {
+  return (size_t(it) * NUM_TRUNK + layer) * A_TILE_BYTES + uint32_t(2 * wg + (wq >> 1)) * 16384u +
+         uint32_t(16 * (wq & 1) + int(lane >> 2)) * 16u + uint32_t(2 * int(lane & 3)) * 2u;
+}
+__host__ __device__ __forceinline__ constexpr uint32_t t_frag_offset(int g, int h) {
+  return uint32_t(g) * 512u + uint32_t(h) * 128u;
+}
+// ReLU masks (layouts.py: decode_mask): [layer][row][8] words, 1 bit per activation.  Word c covers columns
+// 32c..32c+31; column 32c + 2k + e (pair k = 0..15, e = 0, 1) is bit mask_bit(k, e).
+__host__ __device__ constexpr int mask_bit(int k, int e) { return 15 - k + 16 * e; }
+// bits of pair k from its two flags held as the halves of one word (bit 0: column 2k, bit 16: column 2k + 1)
+__device__ __forceinline__ uint32_t mask_pair_bits(uint32_t flags, int k) {
+  static_assert(mask_bit(0, 1) == mask_bit(0, 0) + 16, "a pair's bits are 16 apart");
+  return flags << mask_bit(k, 0);
+}
+// Mask words of an accumulator fragment: the four lanes of a quad hold 4 pairs each of word c of rows fr and fr + 8
+// (m[0], m[1]).  OR them over the quad; lane q keeps words 4(q&1)..+3 of row fr + 8(q>>1), word c in maskw[c & 3].
+__device__ __forceinline__ void mask_quad_reduce(uint32_t (&m)[2], int c, uint32_t (&maskw)[4]) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    m[h] |= __shfl_xor_sync(0xffffffffu, m[h], 1);
+    m[h] |= __shfl_xor_sync(0xffffffffu, m[h], 2);
+  }
+  const uint32_t q = lane_id() & 3;
+  if ((q & 1) == uint32_t(c >> 2)) maskw[c & 3] = (q >> 1) ? m[1] : m[0];
+}
+// lane q's four words (mask_quad_reduce) -> layer `layer` of a [layers][rows][8] mask array; row: the quad's fragment
+// row fr
+__device__ __forceinline__ void store_mask_words(uint32_t* mask, long long rows, int layer, long long row,
+                                                 const uint32_t (&maskw)[4]) {
+  const uint32_t q = lane_id() & 3;
+  const long long s = row + 8 * int(q >> 1);
+  *reinterpret_cast<uint4*>(mask + (size_t(layer) * rows + s) * 8 + 4 * (q & 1)) =
+      make_uint4(maskw[0], maskw[1], maskw[2], maskw[3]);
+}
 // Weight slot ("W image"): [rows][64 B] = 32 fp16 (K) per output row, 16-byte units
 // XOR-swizzled with ((row >> 1) & 3)  (= cute Swizzle<2,4,3>, K-major SW64 atom).
 __host__ __device__ __forceinline__ constexpr uint32_t w_slot_offset(int row, int k) {

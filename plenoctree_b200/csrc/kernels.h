@@ -52,7 +52,7 @@ struct FwdParams {
   // ---- training saves (null = off; x3 also needs save_h_lo / save_e_lo) ----
   uint8_t* save_h;             // [ntile][8][64 KB] activation tile images h_0..h_7
   uint8_t* save_e;             // [ntile][16 KB]   posenc tile images
-  uint32_t* save_mask;         // [8][ntile*128][8] relu masks (bit i of word c = col 32c+i)
+  uint32_t* save_mask;         // [8][ntile*128][8] relu masks (common.cuh: mask_bit)
   // ---- x3 training saves (NSPLIT = 3): the residual (lo) images beside save_h / save_e ----
   uint8_t* save_h_lo;          // [ntile][8][64 KB]
   uint8_t* save_e_lo;          // [ntile][16 KB]

@@ -223,31 +223,21 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
   };
 
   // Training save of K-slot c's share of h_lh (columns 32c..32c+31) from the A registers that carried it, once the
-  // slot's MMAs have completed: the "T" image (layouts.py: t_tile_offset), in which each warp store of one 8-column
-  // group is one contiguous 128 B core matrix, and mask word c.  Word c covers columns 32c..32c+31: column 32c+2k is
-  // bit 15-k, column 32c+2k+1 is bit 31-k, derived from the fp16 values (h > 0 <=> fp16(h) != 0 up to fp16
-  // underflow).  The four lanes of a quad hold one row's 16 pairs; lane q keeps words 4(q&1)..+3 of row fr + 8(q>>1).
+  // slot's MMAs have completed: the "T" image and mask word c, whose bits come from the fp16 values (h > 0 <=>
+  // fp16(h) != 0 up to fp16 underflow).
   auto save_slot = [&](int lh, int c, uint32_t (&maskw)[4]) {
-    uint8_t* const h_glob = p.save_h + (size_t(it) * NUM_TRUNK + lh) * A_TILE_BYTES +
-                            uint32_t(2 * wg + (wq >> 1)) * 16384u + uint32_t(16 * (wq & 1) + int(lane >> 2)) * 16u +
-                            uint32_t(fc) * 2u;
+    uint8_t* const h_glob = p.save_h + t_frag_base(it, lh, wg, wq, lane);
     uint32_t m[2] = {0u, 0u};
 #pragma unroll
     for (int i = 0; i < 8; ++i) {            // afr[8c + i]: k16 step i/4 of the slot, register i%4
       const uint32_t w = afr[8 * c + i];
       const int h = i & 1;                    // row fr + 8h
       const int hi8 = (i >> 1) & 1;           // second 8 columns of the k16 step
-      *reinterpret_cast<uint32_t*>(h_glob + uint32_t(4 * c + 2 * (i >> 2) + hi8) * 512u + uint32_t(h) * 128u) = w;
+      *reinterpret_cast<uint32_t*>(h_glob + t_frag_offset(4 * c + 2 * (i >> 2) + hi8, h)) = w;
       const int k = 8 * (i >> 2) + 4 * hi8 + int(lane & 3);   // column pair within the mask word
-      m[h] |= __vminu2(w, 0x00010001u) << (15 - k);           // non-negative fp16 pair -> 0/1 per half
+      m[h] |= mask_pair_bits(__vminu2(w, 0x00010001u), k);    // non-negative fp16 pair -> 0/1 per half
     }
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      m[h] |= __shfl_xor_sync(0xffffffffu, m[h], 1);
-      m[h] |= __shfl_xor_sync(0xffffffffu, m[h], 2);
-    }
-    const uint32_t q = lane & 3;
-    if ((q & 1) == uint32_t(c >> 2)) maskw[c & 3] = (q >> 1) ? m[1] : m[0];
+    mask_quad_reduce(m, c, maskw);
   };
 
   // fp16 layer l >= 1 (l = NUM_TRUNK: the heads, into hacc): K-slots 0..7 take h_{l-1} from afr, the bias slot and
@@ -297,12 +287,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
     }
     wgmma_wait<0>();
     ring.release(prev);
-    if (SAVE) {
-      const uint32_t q = lane & 3;
-      const long long s = it * TILE_M + 64 * wg + fr + 8 * int(q >> 1);
-      *reinterpret_cast<uint4*>(p.save_mask + (size_t(l - 1) * padded_rows(p.M) + s) * 8 + 4 * (q & 1)) =
-          make_uint4(maskw[0], maskw[1], maskw[2], maskw[3]);
-    }
+    if (SAVE) store_mask_words(p.save_mask, padded_rows(p.M), l - 1, it * TILE_M + 64 * wg + fr, maskw);
   };
 
   // heads: accumulator fragment -> per-row fp32 staging (column n = packed heads column) inside the warpgroup's own
@@ -485,16 +470,12 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
         if (!heads) {
           // ---- trunk epilogue: ReLU + hi/lo fp16 split straight from the accumulator fragment into the next A
           // operands (the bias was accumulated by the tensor cores).  Only this warpgroup's MMAs read these rows.
-          // Training (SAVE): the same hi and lo values go to the "T" images of h_l (layouts.py: t_tile_offset; one
-          // warp store = one contiguous 128 B core-matrix row group, as in the fp16 save_slot), and the mask words
-          // of h_l take their bits from the sign of the fp32 pre-activation: relu(v) < 2^-25 rounds to hi = lo = 0
-          // but still has a gradient.  Word c, column 32c+2k <-> bit 15-k, 32c+2k+1 <-> bit 31-k; lane q of a quad
-          // keeps words 4(q&1)..+3 of row fr + 8(q>>1). ----
+          // Training (SAVE): the same hi and lo values go to the "T" images of h_l, and the mask words of h_l take
+          // their bits from the sign of the fp32 pre-activation: relu(v) < 2^-25 rounds to hi = lo = 0 but still has
+          // a gradient. ----
           size_t t_off = 0;
           uint32_t mrow[2] = {0u, 0u}, maskw[4] = {0u, 0u, 0u, 0u};
-          if constexpr (SAVE)
-            t_off = (size_t(it) * NUM_TRUNK + l) * A_TILE_BYTES + uint32_t(2 * wg + (wq >> 1)) * 16384u +
-                    uint32_t(16 * (wq & 1) + int(lane >> 2)) * 16u + uint32_t(fc) * 2u;
+          if constexpr (SAVE) t_off = t_frag_base(it, l, wg, wq, lane);
 #pragma unroll
           for (int j = 0; j < 32; ++j) {
 #pragma unroll
@@ -508,31 +489,19 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
               const uint32_t wl = pack_f16x2(fmaxf(v0, 0.f) - hv.x, fmaxf(v1, 0.f) - hv.y);
               *reinterpret_cast<uint32_t*>(a_lo + off) = wl;
               if constexpr (SAVE) {
-                const size_t go = t_off + uint32_t(j) * 512u + uint32_t(h) * 128u;
+                const size_t go = t_off + t_frag_offset(j, h);
                 *reinterpret_cast<uint32_t*>(p.save_h + go) = w;
                 *reinterpret_cast<uint32_t*>(p.save_h_lo + go) = wl;
                 const int k = 4 * (j & 3) + (fc >> 1);   // column pair within the mask word
-                mrow[h] |= (v0 > 0.f ? 1u << (15 - k) : 0u) | (v1 > 0.f ? 1u << (31 - k) : 0u);
+                mrow[h] |= (v0 > 0.f ? 1u << mask_bit(k, 0) : 0u) | (v1 > 0.f ? 1u << mask_bit(k, 1) : 0u);
               }
             }
             if (SAVE && (j & 3) == 3) {
-              const int c = j >> 2;
-#pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                mrow[h] |= __shfl_xor_sync(0xffffffffu, mrow[h], 1);
-                mrow[h] |= __shfl_xor_sync(0xffffffffu, mrow[h], 2);
-              }
-              const uint32_t q = lane & 3;
-              if ((q & 1) == uint32_t(c >> 2)) maskw[c & 3] = (q >> 1) ? mrow[1] : mrow[0];
+              mask_quad_reduce(mrow, j >> 2, maskw);
               mrow[0] = mrow[1] = 0u;
             }
           }
-          if constexpr (SAVE) {
-            const uint32_t q = lane & 3;
-            const long long s = it * TILE_M + 64 * wg + fr + 8 * int(q >> 1);
-            *reinterpret_cast<uint4*>(p.save_mask + (size_t(l) * padded_rows(p.M) + s) * 8 + 4 * (q & 1)) =
-                make_uint4(maskw[0], maskw[1], maskw[2], maskw[3]);
-          }
+          if constexpr (SAVE) store_mask_words(p.save_mask, padded_rows(p.M), l, it * TILE_M + 64 * wg + fr, maskw);
           fence_proxy_async_smem();
           warpgroup_sync(wg);
           continue;
