@@ -28,6 +28,12 @@ extern "C" {
 #define POB_PREC_FP16 1
 #define POB_PREC_FP16X3 3
 
+/* flag sigma_activation (nerf_sh/nerf/utils.py:153, models.py:280-281): the density activation of the ray samples
+ * and of pob_eval_points_act.  Raw sigma (eval_points_raw, the extraction grids and cell means) never takes one, and
+ * the sparsity term of the training step keeps relu on raw sigma whatever the flag (nerf_sh/train.py:77-83). */
+#define POB_SIGMA_RELU 0
+#define POB_SIGMA_SOFTPLUS 1 /* log(1 + exp(x)), evaluated in fp32 as max(x, 0) + log1p(exp(-|x|)) */
+
 /* ---------------------------------------------------------------------------------------------
  * Library / device
  * ------------------------------------------------------------------------------------------- */
@@ -65,10 +71,15 @@ int pob_eval_points_raw(const void* packed_dev, int sh_deg, const float* points_
                         float* raw_rgb_dev, float* raw_sigma_dev, int precision, void* stream);
 
 /* NerfModel.eval_points(points, viewdirs) -> (rgb[M,3], sigma[M,1])  (models.py:183-214):
- * eval_sh at the per-point view direction, sigmoid / relu.  out_rgbs_dev: [M,4] = (r,g,b,sigma). */
+ * eval_sh at the per-point view direction, sigmoid / relu.  out_rgbs_dev: [M,4] = (r,g,b,sigma).
+ * pob_eval_points is pob_eval_points_act with POB_SIGMA_RELU. */
 int pob_eval_points(const void* packed_dev, int sh_deg, const float* points_dev,
                     const float* viewdirs_dev, int64_t m, float* out_rgbs_dev, int precision,
                     void* stream);
+/* the same with the density activation sigma_activation (POB_SIGMA_*) in place of relu */
+int pob_eval_points_act(const void* packed_dev, int sh_deg, const float* points_dev,
+                        const float* viewdirs_dev, int64_t m, float* out_rgbs_dev, int sigma_activation,
+                        int precision, void* stream);
 
 /* Dense-grid sweep of octree.extraction (auto_scale / step1: octree/extraction.py:244-320).
  * Evaluates raw sigma (and optionally raw SH coefficients) at the voxel centres
@@ -141,6 +152,9 @@ typedef struct pob_render_config {
    * coarse [n_rays, Nc] and fine [n_rays, Nc+Nf] level; NULL = off (randomized False or noise_std None). */
   const float* sigma_noise_coarse_dev;
   const float* sigma_noise_fine_dev;
+  /* flag sigma_activation: POB_SIGMA_* applied to the (noised) raw sigma of the ray samples; 0 = relu.  The
+   * sparsity points of the training step keep relu (nerf_sh/train.py:82). */
+  int sigma_activation;
 } pob_render_config;
 
 /* bytes of device scratch the render (training=0) / training (training=1) calls need */

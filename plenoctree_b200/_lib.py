@@ -12,6 +12,9 @@ LIB_PATH = os.environ.get("POB_LIB_PATH") or os.path.join(_HERE, "libplenoctree_
 PREC_FP16 = 1
 PREC_FP16X3 = 3
 
+SIGMA_RELU = 0        # POB_SIGMA_*: density activation of the ray samples and of eval_points
+SIGMA_SOFTPLUS = 1
+
 _c = ctypes
 _vp, _i, _i64, _fp = _c.c_void_p, _c.c_int, _c.c_int64, _c.c_void_p
 
@@ -28,6 +31,7 @@ SIGNATURES = {
     "pob_pack_weights": (_i, [_fp, _i, _vp, _vp]),
     "pob_eval_points_raw": (_i, [_vp, _i, _fp, _i64, _fp, _fp, _i, _vp]),
     "pob_eval_points": (_i, [_vp, _i, _fp, _fp, _i64, _fp, _i, _vp]),
+    "pob_eval_points_act": (_i, [_vp, _i, _fp, _fp, _i64, _fp, _i, _i, _vp]),
     "pob_eval_cells_mean": (_i, [_vp, _i, _fp, _i64, _i, _fp, _i, _vp]),
     "pob_eval_grid": (_i, [_vp, _i, _i, _i, _i, _i, _i, _c.POINTER(_c.c_float), _c.POINTER(_c.c_float),
                            _fp, _fp, _i, _vp]),
@@ -61,7 +65,7 @@ SIGNATURES = {
 class RenderConfig(_c.Structure):
     _fields_ = [("sh_deg", _i), ("num_coarse_samples", _i), ("num_fine_samples", _i), ("white_bkgd", _i),
                 ("max_rays", _i), ("sparsity_npoints", _i), ("sigma_noise_coarse_dev", _vp),
-                ("sigma_noise_fine_dev", _vp)]
+                ("sigma_noise_fine_dev", _vp), ("sigma_activation", _i)]
 
 
 class TrainHParams(_c.Structure):

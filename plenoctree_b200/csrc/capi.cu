@@ -131,10 +131,15 @@ int pob_check_common(const char* where, const void* packed, int sh_deg, int prec
   return check_common(where, packed, sh_deg, precision);
 }
 pob::FwdParams pob_base_params(const void* packed, int sh_deg) { return base_params(packed, sh_deg); }
+int pob_check_sigma_activation(const char* where, int sigma_activation) {
+  if (sigma_activation != POB_SIGMA_RELU && sigma_activation != POB_SIGMA_SOFTPLUS)
+    return fail(where, "sigma_activation must be POB_SIGMA_RELU or POB_SIGMA_SOFTPLUS");
+  return 0;
+}
 
 extern "C" {
 
-int pob_abi_version(void) { return 7; }   // 7: pob_octree_sgd_momentum_step; 6: pob_train_workspace_bytes, pob_loss_and_grad_prec (fp16x3 training); 5: sm_90a, no debug-trace / descriptor-probe entry points; 4: pob_loss_and_grad(mlp0_done_event), pob_adam_update(lr_step_dev)
+int pob_abi_version(void) { return 8; }   // 8: pob_render_config.sigma_activation, pob_eval_points_act; 7:pob_octree_sgd_momentum_step; 6: pob_train_workspace_bytes, pob_loss_and_grad_prec (fp16x3 training); 5: sm_90a, no debug-trace / descriptor-probe entry points; 4: pob_loss_and_grad(mlp0_done_event), pob_adam_update(lr_step_dev)
 
 long long pob_launch_count(void) { return g_launches.load(); }
 
@@ -200,15 +205,17 @@ int pob_eval_points_raw(const void* packed_dev, int sh_deg, const float* points_
   return 0;
 }
 
-int pob_eval_points(const void* packed_dev, int sh_deg, const float* points_dev,
-                    const float* viewdirs_dev, int64_t m, float* out_rgbs_dev, int precision,
-                    void* stream) {
-  if (int e = check_common("pob_eval_points", packed_dev, sh_deg, precision)) return e;
-  if (m < 0) return fail("pob_eval_points", "negative point count");
+int pob_eval_points_act(const void* packed_dev, int sh_deg, const float* points_dev,
+                        const float* viewdirs_dev, int64_t m, float* out_rgbs_dev, int sigma_activation,
+                        int precision, void* stream) {
+  const char* where = "pob_eval_points";
+  if (int e = check_common(where, packed_dev, sh_deg, precision)) return e;
+  if (int e = pob_check_sigma_activation(where, sigma_activation)) return e;
+  if (m < 0) return fail(where, "negative point count");
   if (m == 0) return 0;
-  if (!points_dev || !out_rgbs_dev) return fail("pob_eval_points", "NULL pointer");
+  if (!points_dev || !out_rgbs_dev) return fail(where, "NULL pointer");
   if (sh_deg >= 0 && !viewdirs_dev)
-    return fail("pob_eval_points", "viewdirs required when sh_deg >= 0 (models.py:199)");
+    return fail(where, "viewdirs required when sh_deg >= 0 (models.py:199)");
   pob::FwdParams p = base_params(packed_dev, sh_deg);
   p.src_mode = pob::SRC_POINTS;
   p.M = m;
@@ -216,11 +223,18 @@ int pob_eval_points(const void* packed_dev, int sh_deg, const float* points_dev,
   p.viewdirs = viewdirs_dev ? viewdirs_dev : points_dev;
   p.out_mode = pob::OUT_RGBS;
   p.out_rgbs = reinterpret_cast<float4*>(out_rgbs_dev);
+  p.sigma_act = sigma_activation;
   pob_count_launch();
   PobPhaseTimer _t(POB_PH_FWD, (cudaStream_t)stream);
-  POB_CUDA("pob_eval_points",
-           pob::launch_mlp_fwd(p, precision, sm_count(), (cudaStream_t)stream));
+  POB_CUDA(where, pob::launch_mlp_fwd(p, precision, sm_count(), (cudaStream_t)stream));
   return 0;
+}
+
+int pob_eval_points(const void* packed_dev, int sh_deg, const float* points_dev,
+                    const float* viewdirs_dev, int64_t m, float* out_rgbs_dev, int precision,
+                    void* stream) {
+  return pob_eval_points_act(packed_dev, sh_deg, points_dev, viewdirs_dev, m, out_rgbs_dev, POB_SIGMA_RELU, precision,
+                             stream);
 }
 
 int pob_eval_cells_mean(const void* packed_dev, int sh_deg, const float* points_dev, int64_t n_cells,
@@ -358,7 +372,7 @@ int pob_composite_bwd(const float* rgbs_dev, const float* z_dev, const float* di
   pob_count_launch();
   POB_CUDA("pob_composite_bwd",
            pob::launch_composite_bwd(reinterpret_cast<const float4*>(rgbs_dev), z_dev, dirs_dev, comp_rgb_dev,
-                                     pixels_dev, n_rays, n_samples, white_bkgd, gscale,
+                                     pixels_dev, n_rays, n_samples, white_bkgd, gscale, pob::SIGMA_RELU,
                                      reinterpret_cast<float4*>(g_out_dev), sq_err_sum_dev, (cudaStream_t)stream));
   return 0;
 }

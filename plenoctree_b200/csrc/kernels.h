@@ -17,6 +17,15 @@ struct MlpPacked {
 
 enum SrcMode : int { SRC_POINTS = 0, SRC_RAYS = 1, SRC_GRID = 2 };
 enum OutMode : int { OUT_RAW = 0, OUT_SIGMA = 1, OUT_RGBS = 2, OUT_CELL_MEAN = 3 };
+// density activation of OUT_RGBS (the values of POB_SIGMA_* in the C ABI)
+enum SigmaAct : int { SIGMA_RELU = 0, SIGMA_SOFTPLUS = 1 };
+
+// softplus in fp32, stable for every x: max(x, 0) + log1p(exp(-|x|)).  expf (2 ulp) and log1pf (1 ulp) and the
+// final add keep it within 4 * 2^-24 * softplus(x) of the exact value of the fp32 argument, down to where expf's
+// output turns denormal (x < -87); DESIGN.md section 3 gives the measured figure.
+__device__ __forceinline__ float softplus_f32(float x) { return fmaxf(x, 0.f) + log1pf(expf(-fabsf(x))); }
+// its derivative from its own output: d softplus / dx = sigmoid(x) = 1 - exp(-softplus(x)) = -expm1(-sigma)
+__device__ __forceinline__ float softplus_grad_of_output(float sigma) { return -expm1f(-sigma); }
 
 struct FwdParams {
   // ---- sample source ----
@@ -33,6 +42,7 @@ struct FwdParams {
   const float* extra_points;   // [M - M_rays, 3]
   const float* viewdirs;       // OUT_RGBS: [R,3] (SRC_RAYS) or [M,3] (SRC_POINTS)
   const float* sigma_noise;    // OUT_RGBS, optional [M]: added to raw sigma before relu (model_utils.py:317-332)
+  int sigma_act;               // OUT_RGBS: SIGMA_RELU / SIGMA_SOFTPLUS of the ray (or SRC_POINTS) rows; free rows: relu
   // SRC_GRID: voxel centres ((i + 0.5)/reso - offset)/scale, x-major flattening (ix,iy,iz)
   int g_reso;                  // arange length the reference normalises by
   int g_x0, g_nx, g_ny, g_nz;  // slab: ix in [g_x0, g_x0+g_nx), iy in [0,g_ny), iz in [0,g_nz)
@@ -46,7 +56,7 @@ struct FwdParams {
   int out_mode;
   float* out_rgb;              // OUT_RAW: [M, 3K] (reference channel-major order c*K+k)
   float* out_sigma;            // OUT_RAW / OUT_SIGMA: [M]
-  float4* out_rgbs;            // OUT_RGBS: [M] (sigmoid(rgb), relu(sigma))
+  float4* out_rgbs;            // OUT_RGBS: [M] (sigmoid(rgb), relu(sigma) or softplus(sigma))
   float* out_cell;             // OUT_CELL_MEAN: [M / cell_S, 3K+1] += mean over the cell's samples of
   int cell_S;                  //   cat([raw_rgb, raw_sigma]) (octree/extraction.py:391-393); zeroed by caller
   // ---- training saves (null = off; x3 also needs save_h_lo / save_e_lo) ----
@@ -84,9 +94,10 @@ cudaError_t launch_sample_coarse(const float* z_base, const float* t_rand, int R
 cudaError_t launch_composite_fwd(const float4* rgbs, const float* z, const float* dirs, int R, int N,
                                  int white_bkgd, float* out_rgb, float* out_disp, float* out_acc,
                                  float* out_weights, cudaStream_t st);
+// sigma_act: the activation rgbs.w went through (SigmaAct); G.w takes its derivative, formed from rgbs.w
 cudaError_t launch_composite_bwd(const float4* rgbs, const float* z, const float* dirs,
                                  const float* comp_rgb, const float* pixels, int R, int N, int white_bkgd,
-                                 float gscale, float4* G, float* sq_err_sum, cudaStream_t st);
+                                 float gscale, int sigma_act, float4* G, float* sq_err_sum, cudaStream_t st);
 cudaError_t launch_sample_pdf(const float* z_c, const float* weights, const float* u, int u_per_ray, int R,
                               int Nc, int Nf, float* z_out, cudaStream_t st);
 // t_rand [n_t], u [n_u] ~ U[0,1), sp [n_sp] ~ U[-radius, radius): Philox4x32-10 keyed by seed, counter (index, stream, step);

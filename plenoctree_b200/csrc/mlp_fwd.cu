@@ -10,8 +10,8 @@
 //   model_utils.MLP         (model_utils.py:30-94)      wgmma, fp32 accumulators in registers; fp16: ReLU +
 //                                                       pack into the next layer's register A operand
 //                                                       (x3: ReLU epilogue registers -> smem A tiles)
-//   sh.eval_sh + sigmoid/relu (sh.py:54-109,            heads epilogue (registers -> smem staging)
-//                              models.py:269-281)
+//   sh.eval_sh + sigmoid/relu (sh.py:54-109,            heads epilogue (registers -> smem staging); the density
+//     or softplus              models.py:269-281)       activation is p.sigma_act
 //   NerfModel.eval_points_raw (models.py:143-181)       OUT_RAW / OUT_SIGMA
 //
 // Warp roles (384 threads): warps 0-3 and 4-7 = two consumer warpgroups, each owning 64 rows of the tile
@@ -325,9 +325,11 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
         o.x = 1.f / (1.f + expf(-pre[0]));
         o.y = 1.f / (1.f + expf(-pre[1]));
         o.z = 1.f / (1.f + expf(-pre[2]));
-        if (p.sigma_noise != nullptr && (p.src_mode != SRC_RAYS || s < p.M_rays))
-          sigma_raw += __ldg(p.sigma_noise + s);  // add_gaussian_noise
-        o.w = fmaxf(sigma_raw, 0.f);
+        // ray samples (and SRC_POINTS rows) take the noise and the model's density activation; the free sparsity
+        // points behind them keep relu of raw sigma, the value sparsity_grad_kernel reads (train.py:82)
+        const bool sample_row = p.src_mode != SRC_RAYS || s < p.M_rays;
+        if (p.sigma_noise != nullptr && sample_row) sigma_raw += __ldg(p.sigma_noise + s);  // add_gaussian_noise
+        o.w = (p.sigma_act == SIGMA_SOFTPLUS && sample_row) ? softplus_f32(sigma_raw) : fmaxf(sigma_raw, 0.f);
         p.out_rgbs[s] = o;
       }
     } else if (OUTM == OUT_SIGMA || OUTM == OUT_RAW) {
@@ -515,6 +517,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
 cudaError_t launch_mlp_fwd(const FwdParams& p, int nsplit, int num_sms, cudaStream_t stream) {
   if (p.M <= 0) return cudaSuccess;
   if (nsplit != 1 && nsplit != 3) return cudaErrorInvalidValue;
+  if (p.sigma_act != SIGMA_RELU && p.sigma_act != SIGMA_SOFTPLUS) return cudaErrorInvalidValue;
   const bool save = p.save_h != nullptr;
   if (save && (!p.save_e || !p.save_mask || (p.out_mode != OUT_RGBS && p.out_mode != OUT_SIGMA)))
     return cudaErrorInvalidValue;

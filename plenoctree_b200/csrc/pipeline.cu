@@ -125,7 +125,7 @@ int check_cfg(const char* where, const pob_render_config* c) {
     return pob_fail(where, "num_coarse_samples + num_fine_samples must be <= 256");
   if (c->max_rays <= 0) return pob_fail(where, "max_rays must be positive");
   if (c->sparsity_npoints < 0) return pob_fail(where, "sparsity_npoints must be >= 0");
-  return 0;
+  return pob_check_sigma_activation(where, c->sigma_activation);
 }
 
 FwdParams ray_fwd_params(const void* packed, int sh_deg, const float* o, const float* d, const float* v,
@@ -157,6 +157,7 @@ int forward_levels(const char* where, const pob_render_config& c, Workspace& w, 
   {
     FwdParams p = ray_fwd_params(pk_c, c.sh_deg, o, d, v, C.z, R, Nc, C.rgbs);
     p.sigma_noise = c.sigma_noise_coarse_dev;
+    p.sigma_act = c.sigma_activation;
     if (Nf == 0 && sp_n > 0) {     // single-level model: the sparsity points ride on this launch
       p.M += sp_n;
       p.extra_points = sp_points;
@@ -180,6 +181,7 @@ int forward_levels(const char* where, const pob_render_config& c, Workspace& w, 
       { pob_count_launch(1); PobPhaseTimer _t(POB_PH_RENDER, st); POB_CUDA(where, launch_sample_pdf(C.z, C.weights, u, u_per_ray, R, Nc, Nf, F.z, st)); }
     FwdParams p = ray_fwd_params(pk_f, c.sh_deg, o, d, v, F.z, R, Nc + Nf, F.rgbs);
     p.sigma_noise = c.sigma_noise_fine_dev;
+    p.sigma_act = c.sigma_activation;
     if (sp_n > 0) {                // the sparsity points ride behind the fine level's ray samples (same MLP)
       p.M += sp_n;
       p.extra_points = sp_points;
@@ -329,10 +331,10 @@ int pob_loss_and_grad_prec(const pob_render_config* cfg, const pob_train_hparams
   const long long Mr_last = (long long)n_rays * (Nf > 0 ? Nc + Nf : Nc);
   // ---- upstream gradients ----
   { pob_count_launch(1); PobPhaseTimer _t(POB_PH_RENDER, st); POB_CUDA(where, launch_composite_bwd(C.rgbs, C.z, directions_dev, C.comp, pixels_dev, n_rays, Nc,
-                                       cfg->white_bkgd, gscale, C.G, stats_dev + (Nf > 0 ? 1 : 0), st)); }
+                                       cfg->white_bkgd, gscale, cfg->sigma_activation, C.G, stats_dev + (Nf > 0 ? 1 : 0), st)); }
   if (Nf > 0)
     { pob_count_launch(1); PobPhaseTimer _t(POB_PH_RENDER, st); POB_CUDA(where, launch_composite_bwd(F.rgbs, F.z, directions_dev, F.comp, pixels_dev, n_rays, Nc + Nf,
-                                         cfg->white_bkgd, gscale, F.G, stats_dev + 0, st)); }
+                                         cfg->white_bkgd, gscale, cfg->sigma_activation, F.G, stats_dev + 0, st)); }
   if (sparsity) {
     const float coef = hp->loss_scale * hp->sparsity_weight * hp->sparsity_length / float(sp_n);
     { pob_count_launch(1); PobPhaseTimer _t(POB_PH_RENDER, st); POB_CUDA(where, launch_sparsity_grad(LAST.rgbs + Mr_last, int(sp_n), hp->sparsity_length, coef,

@@ -176,7 +176,7 @@ composite_fwd_kernel(const CompositeArgs a) {
 // ---------------------------------------------------------------------------------------------
 // Backward of compositing + MSE.  Emits, per sample, the gradient w.r.t. the PRE-activation head
 // outputs after SH evaluation: (d pre_r, d pre_g, d pre_b, d sigma_raw), already multiplied by
-// sigmoid' and relu' — mlp_bwd only has to expand it with the SH basis.
+// sigmoid' and relu' (or softplus') — mlp_bwd only has to expand it with the SH basis.
 //   dL/dC = gscale * (C - px);   gscale = loss_scale * 2 / (3 * R_global_per_rank)
 // ---------------------------------------------------------------------------------------------
 struct CompositeBwdArgs {
@@ -187,6 +187,7 @@ struct CompositeBwdArgs {
   const float* pixels;     // [R,3]
   int R, N, white_bkgd;
   float gscale;
+  int sigma_act;           // SigmaAct of rgbs.w: the sigma factor of G.w is relu' = [sigma > 0] or softplus'
   float4* G;               // [R,N]
   float* sq_err_sum;       // += sum_{rays,ch} (C - px)^2   (loss numerator)
 };
@@ -231,7 +232,8 @@ composite_bwd_kernel(const CompositeBwdArgs a) {
       g.x = w[i] * dcx * r.c[i].x * (1.0f - r.c[i].x);
       g.y = w[i] * dcy * r.c[i].y * (1.0f - r.c[i].y);
       g.z = w[i] * dcz * r.c[i].z * (1.0f - r.c[i].z);
-      g.w = r.c[i].w > 0.f ? dsigma : 0.f;
+      // the activation's derivative at the (noised) raw sigma, from its output: softplus' = -expm1(-sigma)
+      g.w = a.sigma_act == SIGMA_SOFTPLUS ? dsigma * softplus_grad_of_output(r.c[i].w) : (r.c[i].w > 0.f ? dsigma : 0.f);
       a.G[ray * a.N + idx] = g;
     }
     suffix += gi[i] * w[i];
@@ -450,9 +452,10 @@ cudaError_t launch_composite_fwd(const float4* rgbs, const float* z, const float
 
 cudaError_t launch_composite_bwd(const float4* rgbs, const float* z, const float* dirs,
                                  const float* comp_rgb, const float* pixels, int R, int N, int white_bkgd,
-                                 float gscale, float4* G, float* sq_err_sum, cudaStream_t st) {
+                                 float gscale, int sigma_act, float4* G, float* sq_err_sum, cudaStream_t st) {
   if (R == 0) return cudaSuccess;
-  CompositeBwdArgs a{rgbs, z, dirs, comp_rgb, pixels, R, N, white_bkgd, gscale, G, sq_err_sum};
+  if (sigma_act != SIGMA_RELU && sigma_act != SIGMA_SOFTPLUS) return cudaErrorInvalidValue;
+  CompositeBwdArgs a{rgbs, z, dirs, comp_rgb, pixels, R, N, white_bkgd, gscale, sigma_act, G, sq_err_sum};
   const unsigned grid = (R + RAYS_PER_BLOCK - 1) / RAYS_PER_BLOCK;
   return dispatch_seg(N, [&](auto s) {
     composite_bwd_kernel<decltype(s)::value><<<grid, RAYS_PER_BLOCK * 32, 0, st>>>(a);

@@ -127,6 +127,18 @@ def check_flags(args, require_data=True, world=1):
         raise ValueError("Batch size must be divisible by the number of devices.")
 
 
+SIGMA_ACTIVATIONS = {"relu": 0, "softplus": 1}   # _lib.SIGMA_RELU / SIGMA_SOFTPLUS
+
+
+def sigma_activation_code(name):
+    """flag sigma_activation -> POB_SIGMA_* code.  The nerf_sh side names flax's nn.relu / nn.softplus, the octree
+    side torch's nn.ReLU / nn.Softplus (octree/nerf/utils.py:136), so the name is matched case-insensitively."""
+    code = SIGMA_ACTIVATIONS.get(str(name).lower())
+    if code is None:
+        raise NotImplementedError(f"sigma_activation {name!r}: relu or softplus expected")
+    return code
+
+
 def check_scope(args):
     """features of the reference this path does not cover: fail loudly instead of training something else."""
     if args.use_viewdirs:
@@ -137,9 +149,9 @@ def check_scope(args):
         raise NotImplementedError(f"dataset {args.dataset!r}: blender, llff or nsvf expected")
     if (args.net_depth, args.net_width, args.skip_layer, args.min_deg_point, args.max_deg_point) != (8, 256, 4, 0, 10):
         raise NotImplementedError("the fused kernel is built for the 8x256 trunk, skip 4, posenc degrees 0..10")
-    if tuple(str(a).lower() for a in (args.net_activation, args.rgb_activation, args.sigma_activation)) != (
-            "relu", "sigmoid", "relu"):
-        raise NotImplementedError("activations other than relu / sigmoid / relu")   # models.py:280-281 raise the same
+    if (str(args.net_activation).lower(), str(args.rgb_activation).lower()) != ("relu", "sigmoid"):
+        raise NotImplementedError("activations other than relu (trunk) / sigmoid (rgb)")
+    sigma_activation_code(args.sigma_activation)
     if args.legacy_posenc_order:
         raise NotImplementedError("legacy_posenc_order is outside the scope of this path")
     if (args.render_path or args.spherify) and args.dataset != "llff":

@@ -52,9 +52,14 @@ class NerfModel:
 
     def __init__(self, sh_deg=3, num_coarse_samples=64, num_fine_samples=128, near=2.0, far=6.0,
                  white_bkgd=True, lindisp=False, max_rays=4096, sparsity_npoints=0, device="cuda",
-                 precision=PREC_FP16, noise_std=None):
+                 precision=PREC_FP16, noise_std=None, sigma_activation="relu"):
+        from .flags import sigma_activation_code
         if not (-1 <= sh_deg <= 4):
             raise ValueError("sh_deg must be in [-1, 4]")
+        # flag sigma_activation (nerf_sh/nerf/models.py:280-281): relu or softplus of the ray samples' raw sigma and
+        # of eval_points; raw sigma (eval_points_raw, extraction) and the sparsity term never take it
+        self.sigma_activation = str(sigma_activation)
+        self.sigma_act_code = sigma_activation_code(sigma_activation)
         self.sh_deg = sh_deg
         self.num_coarse_samples = int(num_coarse_samples)
         self.num_fine_samples = int(num_fine_samples)
@@ -73,6 +78,7 @@ class NerfModel:
         self.blobs = [torch.zeros(nb, dtype=torch.uint8, device=self.device) for _ in range(self.num_mlps)]
         self.cfg = RenderConfig(sh_deg, self.num_coarse_samples, self.num_fine_samples, int(self.white_bkgd),
                                 self.max_rays, self.sparsity_npoints)
+        self.cfg.sigma_activation = self.sigma_act_code
         self._ws = {}
         # un-jittered depth table, computed with the reference expression (model_utils.py:125-129)
         t_vals = torch.linspace(0.0, 1.0, self.num_coarse_samples, dtype=torch.float32)
@@ -200,7 +206,7 @@ class NerfModel:
             raise AssertionError("viewdirs required when sh_deg >= 0")
         vd = None if viewdirs is None else _cuda_f32(viewdirs, "viewdirs", 3)
         return ops.eval_points(self._blob(coarse), self.sh_deg, _cuda_f32(points, "points", 3), vd,
-                               precision or self.precision)
+                               precision or self.precision, sigma_activation=self.sigma_act_code)
 
 
 def ctypes_ref(struct):
@@ -217,7 +223,8 @@ def get_model_state(args, device="cuda", seed=20200823, restore=True):
                       num_fine_samples=args.num_fine_samples, near=args.near, far=args.far,
                       white_bkgd=args.white_bkgd, lindisp=getattr(args, "lindisp", False),
                       max_rays=getattr(args, "batch_size", 4096),
-                      sparsity_npoints=getattr(args, "sparsity_npoints", 0), device=device)
+                      sparsity_npoints=getattr(args, "sparsity_npoints", 0), device=device,
+                      sigma_activation=getattr(args, "sigma_activation", "relu"))
     model.init_params(seed)
     state = TrainState(model)
     if restore and getattr(args, "train_dir", None):

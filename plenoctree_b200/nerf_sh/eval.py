@@ -21,7 +21,8 @@ def main(unused_argv):
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
     torch.cuda.set_device(dev)
     dataset = datasets.get_dataset("test", FLAGS, device=dev)
-    margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, num_coarse_samples=FLAGS.num_coarse_samples,
+    margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, sigma_activation=FLAGS.sigma_activation,
+                               num_coarse_samples=FLAGS.num_coarse_samples,
                                num_fine_samples=FLAGS.num_fine_samples, near=FLAGS.near, far=FLAGS.far,
                                white_bkgd=FLAGS.white_bkgd, lindisp=FLAGS.lindisp, batch_size=min(FLAGS.chunk, 8192),
                                sparsity_npoints=0, train_dir=None))

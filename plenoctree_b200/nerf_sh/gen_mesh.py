@@ -66,7 +66,8 @@ def main(unused_argv):
     F.check_scope(FLAGS)
     reso, c1, c2 = _triple(FLAGS.reso, int), _triple(FLAGS.c1, float), _triple(FLAGS.c2, float)
     rank, world, dev = _dist.dist_init()
-    margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, num_coarse_samples=FLAGS.num_coarse_samples,
+    margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, sigma_activation=FLAGS.sigma_activation,
+                               num_coarse_samples=FLAGS.num_coarse_samples,
                                num_fine_samples=FLAGS.num_fine_samples, near=FLAGS.near, far=FLAGS.far,
                                white_bkgd=FLAGS.white_bkgd, lindisp=FLAGS.lindisp, batch_size=1024,
                                sparsity_npoints=0, train_dir=None))

@@ -52,7 +52,8 @@ def main(unused_argv):
     if FLAGS.intrin is not None:
         K = np.loadtxt(FLAGS.intrin)
         focal = (K[0, 0] + K[1, 1]) * 0.5
-    margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, num_coarse_samples=FLAGS.num_coarse_samples,
+    margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, sigma_activation=FLAGS.sigma_activation,
+                               num_coarse_samples=FLAGS.num_coarse_samples,
                                num_fine_samples=FLAGS.num_fine_samples, near=FLAGS.near, far=FLAGS.far,
                                white_bkgd=FLAGS.white_bkgd, lindisp=FLAGS.lindisp, batch_size=min(FLAGS.chunk, 8192),
                                sparsity_npoints=0, train_dir=None))

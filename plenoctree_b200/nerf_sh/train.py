@@ -44,7 +44,8 @@ def main(unused_argv):
     test_dataset = datasets.get_dataset("test", FLAGS, device=dev)
     h0print("* Load model")
     per_rank = FLAGS.batch_size // world
-    margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, num_coarse_samples=FLAGS.num_coarse_samples,
+    margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, sigma_activation=FLAGS.sigma_activation,
+                               num_coarse_samples=FLAGS.num_coarse_samples,
                                num_fine_samples=FLAGS.num_fine_samples, near=FLAGS.near, far=FLAGS.far,
                                white_bkgd=FLAGS.white_bkgd, lindisp=FLAGS.lindisp,
                                batch_size=per_rank,   # workspace capacity; test renders chunk by it

@@ -288,7 +288,8 @@ def load_nerf(FLAGS, device):
     """models.get_model_state(FLAGS, restore=True) of the octree side (octree/nerf/models.py:38-49): torch *.ckpt, or
     a flax-format checkpoint_<step> with --is_jaxnerf_ckpt."""
     from ..nerf import checkpoints, models
-    margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, num_coarse_samples=FLAGS.num_coarse_samples,
+    margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, sigma_activation=FLAGS.sigma_activation,
+                               num_coarse_samples=FLAGS.num_coarse_samples,
                                num_fine_samples=FLAGS.num_fine_samples, near=FLAGS.near, far=FLAGS.far,
                                white_bkgd=FLAGS.white_bkgd, lindisp=FLAGS.lindisp, batch_size=min(FLAGS.chunk, 8192),
                                sparsity_npoints=0, train_dir=None))

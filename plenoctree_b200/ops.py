@@ -4,7 +4,8 @@ import ctypes
 import numpy as np
 import torch
 
-from ._lib import PREC_FP16, PREC_FP16X3, check, lib, ptr, stream_ptr  # noqa: F401  (precision modes re-exported)
+from ._lib import (PREC_FP16, PREC_FP16X3, SIGMA_RELU, SIGMA_SOFTPLUS, check, lib, ptr,  # noqa: F401  (modes re-exported)
+                   stream_ptr)
 from .layouts import K_of
 
 
@@ -45,15 +46,16 @@ def eval_points_raw(blob, sh_deg, points, want_rgb=True, precision=PREC_FP16):
     return rgb, sig
 
 
-def eval_points(blob, sh_deg, points, viewdirs, precision=PREC_FP16):
-    """NerfModel.eval_points (models.py:183-214): -> (rgb [M,3], sigma [M,1]) after sigmoid / relu."""
+def eval_points(blob, sh_deg, points, viewdirs, precision=PREC_FP16, sigma_activation=SIGMA_RELU):
+    """NerfModel.eval_points (models.py:183-214): -> (rgb [M,3], sigma [M,1]) after sigmoid / the density activation
+    (SIGMA_RELU or SIGMA_SOFTPLUS)."""
     _f32c(points, "points")
     if viewdirs is not None:
         _f32c(viewdirs, "viewdirs")
     m = points.shape[0]
     out = torch.empty((m, 4), dtype=torch.float32, device=points.device)
-    check(lib.pob_eval_points(ptr(blob), sh_deg, ptr(points), ptr(viewdirs), m, ptr(out), precision,
-                              stream_ptr()))
+    check(lib.pob_eval_points_act(ptr(blob), sh_deg, ptr(points), ptr(viewdirs), m, ptr(out), int(sigma_activation),
+                                  precision, stream_ptr()))
     return out[:, :3], out[:, 3:4]
 
 
