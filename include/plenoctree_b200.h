@@ -284,6 +284,29 @@ int pob_octree_render_backward(const pob_octree* tree, const pob_octree_opts* op
                                const float* dirs_dev, const float* vdirs_dev, int64_t n_rays, const pob_camera* cam,
                                int row0, int nrows, const float* grad_out_dev, float* grad_data_dev, void* stream);
 
+/* pob_octree_render that also returns depth and opacity, the (rgb, disp, acc) of the NeRF-SH renderer minus the
+ * disparity (acc / depth, formed by the caller).  out_rgb_dev and counters_dev are bit-identical to
+ * pob_octree_render's.  Over the contributing visits i (sigma_i > sigma_thresh), visit i starting at t_i with step
+ * dt_i and weight w_i = T_i (1 - exp(-dt_i * delta_scale * sigma_i)):
+ *   out_acc_dev   [n] = sum_i w_i                      (the background is not included)
+ *   out_depth_dev [n] = sum_i w_i (t_i + dt_i / 2) * delta_scale
+ * a distance along the ray's direction vector (explicit rays: the parameter z of origin + z * dir), times
+ * 1 / |(x, y, -1)| for a perspective pixel (camera-axis depth).  Early termination rescales both by 1 / (1 - T) like
+ * the colour, so a stopped ray has acc = 1; a ray that misses the box has depth = acc = 0. */
+int pob_octree_render_depth(const pob_octree* tree, const pob_octree_opts* opts, const float* origins_dev,
+                            const float* dirs_dev, const float* vdirs_dev, int64_t n_rays, const pob_camera* cam,
+                            int row0, int nrows, float* out_rgb_dev, float* out_depth_dev, float* out_acc_dev,
+                            unsigned long long* counters_dev, void* stream);
+
+/* reverse mode of pob_octree_render_depth: grad_data_dev (ACCUMULATED into) += d(<grad_rgb, rgb> + <grad_depth,
+ * depth> + <grad_acc, acc>) / d data.  grad_rgb_dev [n,3], grad_depth_dev [n], grad_acc_dev [n]; any of the three
+ * may be NULL (zero).  Depth and acc reach sigma only.  Thresholds are ignored like in pob_octree_render_backward. */
+int pob_octree_render_depth_backward(const pob_octree* tree, const pob_octree_opts* opts, const float* origins_dev,
+                                     const float* dirs_dev, const float* vdirs_dev, int64_t n_rays,
+                                     const pob_camera* cam, int row0, int nrows, const float* grad_rgb_dev,
+                                     const float* grad_depth_dev, const float* grad_acc_dev, float* grad_data_dev,
+                                     void* stream);
+
 /* One training image of octree.optimization (octree/optimization.py:201-207) in one launch:
  *   im = render_persp(c2w); mse = mean((clamp(im,0,1) - gt)^2); mse.backward()
  * over the pixel rows [row0,row0+nrows): grad_data += grad_scale * d sum((clamp(im)-gt)^2) / d data,

@@ -52,6 +52,8 @@ SIGNATURES = {
                              _vp, _vp, _vp]),
     "pob_octree_render": (_i, [_vp, _vp, _fp, _fp, _fp, _i64, _vp, _i, _i, _fp, _vp, _vp]),
     "pob_octree_render_backward": (_i, [_vp, _vp, _fp, _fp, _fp, _i64, _vp, _i, _i, _fp, _fp, _vp]),
+    "pob_octree_render_depth": (_i, [_vp, _vp, _fp, _fp, _fp, _i64, _vp, _i, _i, _fp, _fp, _fp, _vp, _vp]),
+    "pob_octree_render_depth_backward": (_i, [_vp, _vp, _fp, _fp, _fp, _i64, _vp, _i, _i, _fp, _fp, _fp, _fp, _vp]),
     "pob_octree_train_persp": (_i, [_vp, _vp, _vp, _i, _i, _fp, _c.c_float, _fp, _vp, _fp, _vp]),
     "pob_octree_sgd_step": (_i, [_fp, _fp, _i64, _c.c_float, _vp]),
     "pob_octree_sgd_momentum_step": (_i, [_fp, _fp, _fp, _i64, _c.c_float, _c.c_float, _i, _vp]),

@@ -18,6 +18,7 @@
 // per CTA so that neighbouring rays share L1 lines.
 #include <cstdint>
 #include <cstdlib>
+#include <type_traits>
 
 #include "../../include/plenoctree_b200.h"
 #include "capi_util.h"
@@ -77,8 +78,9 @@ __device__ __forceinline__ void dda_unit(const float* cen, const float* invd, fl
   }
 }
 
-// persp pixel -> world ray (svox render_image_kernel: no +0.5 pixel centre; README.md:184)
-__device__ __forceinline__ void cam_ray(const Cam& c, int ix, int iy, float* o, float* d) {
+// persp pixel -> world ray (svox render_image_kernel: no +0.5 pixel centre; README.md:184); returns |(x, y, -1)|,
+// whose reciprocal turns a distance along the unit ray into camera-axis depth
+__device__ __forceinline__ float cam_ray(const Cam& c, int ix, int iy, float* o, float* d) {
   float x = __fsub_rn(float(ix), __fmul_rn(0.5f, c.width)) / c.fx;
   float y = -__fsub_rn(float(iy), __fmul_rn(0.5f, c.height)) / c.fy;
   float z = -1.0f;
@@ -92,6 +94,7 @@ __device__ __forceinline__ void cam_ray(const Cam& c, int ix, int iy, float* o, 
                      __fmul_rn(c.c2w[4 * a + 2], z));
     o[a] = c.c2w[4 * a + 3];
   }
+  return nrm;
 }
 
 // transform_coord + _get_delta_scale + unit-cube intersection (svox trace_ray prologue)
@@ -278,9 +281,19 @@ struct Marcher {
 // ---- forward march of one ray by one lane group -------------------------------------------------------
 // Software-pipelined: the loads of the current leaf (sigma and this lane's three coefficients, issued
 // unconditionally) are in flight while the next leaf is located; the march itself never depends on the data.
-template <int G, int KPL>
+//
+// DEPTH = true also accumulates, over the contributing visits i (sigma_i > sigma_thresh; visit i starts at t_i, has
+// step delta_t_i and weight w_i = T_i (1 - exp(-delta_t_i * delta_scale * sigma_i))):
+//   dz[0] = depth = sum_i w_i z_i,  z_i = (t_i + delta_t_i / 2) * delta_scale   (midpoint of the visit's
+//           constant-density segment, as a parameter along the caller's direction vector)
+//   dz[1] = acc   = sum_i w_i                                                   (the background not included)
+// Early termination rescales both by 1 / (1 - light) like the colour, so a stopped ray has acc = 1.  A ray that
+// misses the box has depth = acc = 0.  The colour, the march and the counters are those of DEPTH = false.
+template <int G, int KPL, bool DEPTH = false>
 __device__ __forceinline__ void trace_forward(const TreeDev& T, const Opts& O, const Ray& r, const float* basis_l, int l,
-                                              unsigned mask, float* out, unsigned& visits, unsigned& hits) {
+                                              unsigned mask, float* out, unsigned& visits, unsigned& hits,
+                                              float* dz = nullptr) {
+  if constexpr (DEPTH) dz[0] = dz[1] = 0.f;
   if (!r.hit) {
     out[0] = out[1] = out[2] = O.bg;
     return;
@@ -334,12 +347,20 @@ __device__ __forceinline__ void trace_forward(const TreeDev& T, const Opts& O, c
       out[0] += weight * sigmoidf(p0);
       out[1] += weight * sigmoidf(p1);
       out[2] += weight * sigmoidf(p2);
+      if constexpr (DEPTH) {
+        dz[0] += weight * ((t + 0.5f * delta_t) * r.delta_scale);
+        dz[1] += weight;
+      }
       light *= att;
       if (light <= O.stop_thresh) {
         const float scale = 1.0f / (1.0f - light);
         out[0] *= scale;
         out[1] *= scale;
         out[2] *= scale;
+        if constexpr (DEPTH) {
+          dz[0] *= scale;
+          dz[1] *= scale;
+        }
         return;
       }
     }
@@ -356,10 +377,13 @@ __device__ __forceinline__ void trace_forward(const TreeDev& T, const Opts& O, c
 // ---- backward march: colour and density gradients in one pass ---------------------------------------
 // accum enters as sum_j w_j (c_j . g) + T_end * bg * sum(g) = g . out (svox computes it with an extra march:
 // trace_ray_backward pass 1); every contributing leaf then peels its own term off.
-template <int G, int KPL>
+// DEPTH = true adds the upstream gradients gz = d loss / d depth and ga = d loss / d acc of trace_forward<DEPTH>: each
+// visit's `total` gains z_i gz + ga (the value it composites into g . out + gz depth + ga acc, which the caller passes
+// as accum) and only the sigma gradient changes, since depth and acc do not depend on the colour coefficients.
+template <int G, int KPL, bool DEPTH = false>
 __device__ __forceinline__ void trace_backward(const TreeDev& T, const Opts& O, const Ray& r, const float* basis_l, int l,
                                                unsigned mask, const float* g, float accum,
-                                               float* __restrict__ grad) {
+                                               float* __restrict__ grad, float gz = 0.f, float ga = 0.f) {
   if (!r.hit) return;
   float light = 1.0f;
   float t = r.tmin;
@@ -415,7 +439,9 @@ __device__ __forceinline__ void trace_backward(const TreeDev& T, const Opts& O, 
           atomicAdd(gv + 2 * K + k, basis_l[j] * t2);
         }
       }
-      const float total = s0 * g[0] + s1 * g[1] + s2 * g[2];
+      float total = s0 * g[0] + s1 * g[1] + s2 * g[2];
+      // (rounded separately: with gz = ga = 0 the colour's total keeps its bits)
+      if constexpr (DEPTH) total = __fadd_rn(total, __fmaf_rn((t + 0.5f * delta_t) * r.delta_scale, gz, ga));
       light *= att;
       accum -= weight * total;
       if (l == 0) atomicAdd(gv + D - 1, delta_t * r.delta_scale * (total * light - accum));
@@ -428,8 +454,11 @@ __device__ __forceinline__ void trace_backward(const TreeDev& T, const Opts& O, 
 }
 
 // ---- ray fetch: lane group -> ray index (pixel tiles for the perspective camera) --------------------------
+// zscale (optional) receives the factor from a distance along the ray's direction vector to the reported depth:
+// 1 for explicit rays, the camera-axis factor 1 / |(x, y, -1)| for a perspective pixel.
 template <int G>
-__device__ __forceinline__ bool fetch_ray(const RaySrc& S, const TreeDev& T, Ray& r, long long& out_index) {
+__device__ __forceinline__ bool fetch_ray(const RaySrc& S, const TreeDev& T, Ray& r, long long& out_index,
+                                          float* zscale = nullptr) {
   constexpr int RPB = 256 / G;  // rays per CTA
   const int grp = threadIdx.x / G;
   float o[3], d[3];
@@ -444,6 +473,7 @@ __device__ __forceinline__ bool fetch_ray(const RaySrc& S, const TreeDev& T, Ray
     float v[3] = {__ldg(S.v + 3 * i), __ldg(S.v + 3 * i + 1), __ldg(S.v + 3 * i + 2)};
     setup_ray(T.off, T.inv, o, d, v, r);
     out_index = i;
+    if (zscale) *zscale = 1.0f;
     return true;
   }
   constexpr int TW = RPB >= 64 ? 8 : 4, TH = RPB / TW;
@@ -453,9 +483,10 @@ __device__ __forceinline__ bool fetch_ray(const RaySrc& S, const TreeDev& T, Ray
   const int ix = tx * TW + grp % TW;
   const int iyl = ty * TH + grp / TW;  // row inside the slab
   if (ix >= W || iyl >= S.nrows) return false;
-  cam_ray(S.cam, ix, S.row0 + iyl, o, d);
+  const float nrm = cam_ray(S.cam, ix, S.row0 + iyl, o, d);
   setup_ray(T.off, T.inv, o, d, d, r);
   out_index = (long long)iyl * W + ix;
+  if (zscale) *zscale = 1.0f / nrm;
   return true;
 }
 
@@ -480,47 +511,73 @@ __device__ __forceinline__ void lane_basis(const TreeDev& T, const Ray& r, int l
   }
 }
 
-template <int G, int KPL>
+// DEPTH = true also stores depth [n] (times fetch_ray's zscale) and acc [n] (trace_forward<DEPTH>)
+template <int G, int KPL, bool DEPTH = false>
 __global__ void __launch_bounds__(256) octree_render_kernel(TreeDev T, Opts O, RaySrc S, float* __restrict__ out_rgb,
-                                                            unsigned long long* __restrict__ counters) {
+                                                            unsigned long long* __restrict__ counters,
+                                                            float* __restrict__ out_depth, float* __restrict__ out_acc) {
   Ray r;
   long long oi;
-  if (!fetch_ray<G>(S, T, r, oi)) return;
+  float zscale;
+  if (!fetch_ray<G>(S, T, r, oi, DEPTH ? &zscale : nullptr)) return;
   const int l = threadIdx.x % G;
   const unsigned mask = group_mask<G>();
   float bl[KPL];
   lane_basis<G, KPL>(T, r, l, bl);
-  float out[3];
+  float out[3], dz[2];
   unsigned visits = 0, hits = 0;
-  trace_forward<G, KPL>(T, O, r, bl, l, mask, out, visits, hits);
+  trace_forward<G, KPL, DEPTH>(T, O, r, bl, l, mask, out, visits, hits, dz);
   if (l < 3) out_rgb[3 * oi + l] = l == 0 ? out[0] : l == 1 ? out[1] : out[2];
+  if constexpr (DEPTH) {
+    if (l == 0) {
+      out_depth[oi] = dz[0] * zscale;
+      out_acc[oi] = dz[1];
+    }
+  }
   if (counters != nullptr && l == 0) {
     atomicAdd(counters + 0, (unsigned long long)visits);
     atomicAdd(counters + 1, (unsigned long long)hits);
   }
 }
 
-// VolumeRenderer backward for an upstream gradient d loss / d rgb  (svox trace_ray_backward)
-template <int G, int KPL>
+// VolumeRenderer backward for an upstream gradient d loss / d rgb  (svox trace_ray_backward).  DEPTH = true adds
+// d loss / d depth and d loss / d acc of octree_render_kernel<DEPTH>; each of the three gradient arrays may be null
+// (zero).
+template <int G, int KPL, bool DEPTH = false>
 __global__ void __launch_bounds__(256) octree_backward_kernel(TreeDev T, Opts O, RaySrc S,
                                                               const float* __restrict__ grad_out,
-                                                              float* __restrict__ grad_data) {
+                                                              float* __restrict__ grad_data,
+                                                              const float* __restrict__ grad_depth,
+                                                              const float* __restrict__ grad_acc) {
   Ray r;
   long long oi;
-  if (!fetch_ray<G>(S, T, r, oi)) return;
+  float zscale;
+  if (!fetch_ray<G>(S, T, r, oi, DEPTH ? &zscale : nullptr)) return;
   const int l = threadIdx.x % G;
   const unsigned mask = group_mask<G>();
   float bl[KPL];
   lane_basis<G, KPL>(T, r, l, bl);
-  float out[3];
+  float out[3], dz[2];
   unsigned visits = 0, hits = 0;
   Opts Of = O;
   Of.sigma_thresh = 0.f;
   Of.stop_thresh = 0.f;
-  trace_forward<G, KPL>(T, Of, r, bl, l, mask, out, visits, hits);
-  float g[3] = {__ldg(grad_out + 3 * oi), __ldg(grad_out + 3 * oi + 1), __ldg(grad_out + 3 * oi + 2)};
-  const float accum = g[0] * out[0] + g[1] * out[1] + g[2] * out[2];
-  trace_backward<G, KPL>(T, Of, r, bl, l, mask, g, accum, grad_data);
+  trace_forward<G, KPL, DEPTH>(T, Of, r, bl, l, mask, out, visits, hits, dz);
+  if constexpr (!DEPTH) {
+    float g[3] = {__ldg(grad_out + 3 * oi), __ldg(grad_out + 3 * oi + 1), __ldg(grad_out + 3 * oi + 2)};
+    const float accum = g[0] * out[0] + g[1] * out[1] + g[2] * out[2];
+    trace_backward<G, KPL>(T, Of, r, bl, l, mask, g, accum, grad_data);
+  } else {
+    float g[3] = {0.f, 0.f, 0.f};
+    if (grad_out != nullptr)
+      for (int c = 0; c < 3; ++c) g[c] = __ldg(grad_out + 3 * oi + c);
+    // the reported depth is zscale * sum_i w_i z_i: its gradient reaches the march's z_i through zscale
+    const float gz = grad_depth != nullptr ? __ldg(grad_depth + oi) * zscale : 0.f;
+    const float ga = grad_acc != nullptr ? __ldg(grad_acc + oi) : 0.f;
+    float accum = g[0] * out[0] + g[1] * out[1] + g[2] * out[2];
+    accum = __fadd_rn(accum, __fmaf_rn(gz, dz[0], ga * dz[1]));
+    trace_backward<G, KPL, true>(T, Of, r, bl, l, mask, g, accum, grad_data, gz, ga);
+  }
 }
 
 // One training pass over a camera slab (octree/optimization.py:201-207 minus the optimiser):
@@ -799,18 +856,25 @@ int group_width(int K) {
   return 4;
 }
 
-#define POB_OCTREE_DISPATCH(KERNEL, G, K, ...)                                   \
-  do {                                                                           \
-    if ((G) == 32) KERNEL<32, 1><<<blocks, 256, 0, st>>>(__VA_ARGS__);           \
-    else if ((G) == 16) KERNEL<16, 1><<<blocks, 256, 0, st>>>(__VA_ARGS__);      \
-    else if ((G) == 4 && (K) <= 4) KERNEL<4, 1><<<blocks, 256, 0, st>>>(__VA_ARGS__);   \
-    else if ((G) == 4 && (K) <= 12) KERNEL<4, 3><<<blocks, 256, 0, st>>>(__VA_ARGS__);  \
-    else if ((G) == 4 && (K) <= 16) KERNEL<4, 4><<<blocks, 256, 0, st>>>(__VA_ARGS__);  \
-    else if ((G) == 4) KERNEL<4, 7><<<blocks, 256, 0, st>>>(__VA_ARGS__);               \
-    else if ((K) <= 8) KERNEL<8, 1><<<blocks, 256, 0, st>>>(__VA_ARGS__);        \
-    else if ((K) <= 16) KERNEL<8, 2><<<blocks, 256, 0, st>>>(__VA_ARGS__);       \
-    else KERNEL<8, 4><<<blocks, 256, 0, st>>>(__VA_ARGS__);                      \
-  } while (0)
+// (G, K) -> the <G, KPL> instantiation: f(integral_constant G, integral_constant KPL) launches it
+template <class F>
+void octree_dispatch(int G, int K, F&& f) {
+  using std::integral_constant;
+  if (G == 32) f(integral_constant<int, 32>(), integral_constant<int, 1>());
+  else if (G == 16) f(integral_constant<int, 16>(), integral_constant<int, 1>());
+  else if (G == 4 && K <= 4) f(integral_constant<int, 4>(), integral_constant<int, 1>());
+  else if (G == 4 && K <= 12) f(integral_constant<int, 4>(), integral_constant<int, 3>());
+  else if (G == 4 && K <= 16) f(integral_constant<int, 4>(), integral_constant<int, 4>());
+  else if (G == 4) f(integral_constant<int, 4>(), integral_constant<int, 7>());
+  else if (K <= 8) f(integral_constant<int, 8>(), integral_constant<int, 1>());
+  else if (K <= 16) f(integral_constant<int, 8>(), integral_constant<int, 2>());
+  else f(integral_constant<int, 8>(), integral_constant<int, 4>());
+}
+
+#define POB_OCTREE_DISPATCH(KERNEL, G, K, ...)                                                               \
+  octree_dispatch((G), (K), [&](auto g_, auto kpl_) {                                                        \
+    KERNEL<decltype(g_)::value, decltype(kpl_)::value><<<blocks, 256, 0, st>>>(__VA_ARGS__);                 \
+  })
 
 int ray_src(const char* where, const float* o, const float* d, const float* v, long long n, const pob_camera* cam,
             int row0, int nrows, RaySrc& S, unsigned& blocks, int G) {
@@ -864,7 +928,32 @@ int pob_octree_render(const pob_octree* tree, const pob_octree_opts* opts, const
   if (blocks == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   pob_count_launch();
-  POB_OCTREE_DISPATCH(octree_render_kernel, G, T.K, T, O, S, out_rgb_dev, counters_dev);
+  POB_OCTREE_DISPATCH(octree_render_kernel, G, T.K, T, O, S, out_rgb_dev, counters_dev, nullptr, nullptr);
+  POB_CUDA(W, cudaGetLastError());
+  return 0;
+}
+
+int pob_octree_render_depth(const pob_octree* tree, const pob_octree_opts* opts, const float* origins_dev,
+                            const float* dirs_dev, const float* vdirs_dev, int64_t n_rays, const pob_camera* cam,
+                            int row0, int nrows, float* out_rgb_dev, float* out_depth_dev, float* out_acc_dev,
+                            unsigned long long* counters_dev, void* stream) {
+  const char* W = "pob_octree_render_depth";
+  TreeDev T;
+  Opts O;
+  RaySrc S;
+  unsigned blocks = 0;
+  if (int rc = tree_dev(W, tree, T)) return rc;
+  if (int rc = opts_dev(W, opts, O)) return rc;
+  const int G = group_width(T.K);
+  if (int rc = ray_src(W, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0, nrows, S, blocks, G)) return rc;
+  if (!out_rgb_dev || !out_depth_dev || !out_acc_dev) return pob_fail(W, "output pointer is NULL");
+  if (blocks == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  pob_count_launch();
+  octree_dispatch(G, T.K, [&](auto g_, auto kpl_) {
+    octree_render_kernel<decltype(g_)::value, decltype(kpl_)::value, true><<<blocks, 256, 0, st>>>(
+        T, O, S, out_rgb_dev, counters_dev, out_depth_dev, out_acc_dev);
+  });
   POB_CUDA(W, cudaGetLastError());
   return 0;
 }
@@ -885,7 +974,33 @@ int pob_octree_render_backward(const pob_octree* tree, const pob_octree_opts* op
   if (blocks == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   pob_count_launch();
-  POB_OCTREE_DISPATCH(octree_backward_kernel, G, T.K, T, O, S, grad_out_dev, grad_data_dev);
+  POB_OCTREE_DISPATCH(octree_backward_kernel, G, T.K, T, O, S, grad_out_dev, grad_data_dev, nullptr, nullptr);
+  POB_CUDA(W, cudaGetLastError());
+  return 0;
+}
+
+int pob_octree_render_depth_backward(const pob_octree* tree, const pob_octree_opts* opts, const float* origins_dev,
+                                     const float* dirs_dev, const float* vdirs_dev, int64_t n_rays,
+                                     const pob_camera* cam, int row0, int nrows, const float* grad_rgb_dev,
+                                     const float* grad_depth_dev, const float* grad_acc_dev, float* grad_data_dev,
+                                     void* stream) {
+  const char* W = "pob_octree_render_depth_backward";
+  TreeDev T;
+  Opts O;
+  RaySrc S;
+  unsigned blocks = 0;
+  if (int rc = tree_dev(W, tree, T)) return rc;
+  if (int rc = opts_dev(W, opts, O)) return rc;
+  const int G = group_width(T.K);
+  if (int rc = ray_src(W, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0, nrows, S, blocks, G)) return rc;
+  if (!grad_data_dev) return pob_fail(W, "gradient pointer is NULL");
+  if (blocks == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  pob_count_launch();
+  octree_dispatch(G, T.K, [&](auto g_, auto kpl_) {
+    octree_backward_kernel<decltype(g_)::value, decltype(kpl_)::value, true><<<blocks, 256, 0, st>>>(
+        T, O, S, grad_rgb_dev, grad_data_dev, grad_depth_dev, grad_acc_dev);
+  });
   POB_CUDA(W, cudaGetLastError());
   return 0;
 }

@@ -1,6 +1,7 @@
 """`python -m plenoctree_b200.octree.evaluation` and `eval_octree` (octree/evaluation.py:75-123,
 octree/nerf/utils.py:448-498): render every test view of a PlenOctree, PSNR / SSIM against the ground truth
-LPIPS is added when its downloaded weights can be found (nerf/lpips.py), else reported as nan."""
+LPIPS is added when its downloaded weights can be found (nerf/lpips.py), else reported as nan.  `--write_disp DIR`
+writes each view's disparity map as `disp_{i:04d}.png`, as nerf_sh.eval does for the NeRF."""
 import os
 
 import numpy as np
@@ -8,12 +9,13 @@ import torch
 
 from ..nerf.utils import compute_psnr, compute_ssim, save_img, write_video
 from .n3tree import N3Tree
-from .renderer import VolumeRenderer
+from .renderer import VolumeRenderer, disparity
 
 
-def eval_octree(t, dataset, args, want_frames=False, lpips_fn=None, metrics=None):
+def eval_octree(t, dataset, args, want_frames=False, lpips_fn=None, metrics=None, disp_fn=None):
     """utils.eval_octree (octree/nerf/utils.py:448-498): -> (avg_psnr, avg_ssim[, frames]).  With `lpips_fn`
-    (nerf/lpips.py::load_lpips) the mean LPIPS(gt, render) is left in `metrics["lpips"]`."""
+    (nerf/lpips.py::load_lpips) the mean LPIPS(gt, render) is left in `metrics["lpips"]`.  With `disp_fn`, each view's
+    disparity [H,W,1] (renderer.disparity of the same render's depth and acc) is passed to disp_fn(idx, disp)."""
     w, h, focal = dataset.w, dataset.h, dataset.focal
     r = VolumeRenderer(t, step_size=args.renderer_step_size)
     avg_psnr = avg_ssim = avg_lpips = 0.0
@@ -22,7 +24,13 @@ def eval_octree(t, dataset, args, want_frames=False, lpips_fn=None, metrics=None
         for idx in range(dataset.size):
             c2w = dataset.camtoworlds[idx]
             im_gt = torch.from_numpy(dataset.images[idx]).float().to(t.device)
-            im = r.render_persp(c2w, width=w, height=h, fx=focal, fast=not args.no_early_stop).clamp_(0.0, 1.0)
+            if disp_fn is None:
+                im = r.render_persp(c2w, width=w, height=h, fx=focal, fast=not args.no_early_stop)
+            else:
+                im, depth, acc = r.render_persp(c2w, width=w, height=h, fx=focal, fast=not args.no_early_stop,
+                                                return_depth=True)
+                disp_fn(idx, disparity(depth, acc))
+            im = im.clamp_(0.0, 1.0)
             mse = float(((im - im_gt) ** 2).mean())
             avg_psnr += float(compute_psnr(mse))
             avg_ssim += float(compute_ssim(im, im_gt, max_val=1.0, padding="same"))   # octree/nerf/utils.py twin
@@ -41,7 +49,8 @@ def _define_cli_flags():
     F.define_flags(octree=True)
     F.define({"input": ("string", "./tree.npz", "Input octree npz"),
               "write_vid": ("string", None, "If specified, writes rendered video to given path (*.mp4)"),
-              "write_images": ("string", None, "If specified, writes rendered images to this directory")})
+              "write_images": ("string", None, "If specified, writes rendered images to this directory"),
+              "write_disp": ("string", None, "If specified, writes disparity maps (disp_XXXX.png) to this directory")})
     return F
 
 
@@ -59,7 +68,14 @@ def main(unused_argv):
     t = N3Tree.load(FLAGS.input, map_location=dev)
     from ..nerf.lpips import load_lpips
     extra = {}
-    psnr, ssim, frames = eval_octree(t, dataset, FLAGS, want_frames=True, lpips_fn=load_lpips(dev), metrics=extra)
+    disp_fn = None
+    if FLAGS.write_disp:
+        os.makedirs(FLAGS.write_disp, exist_ok=True)
+
+        def disp_fn(i, disp):    # nerf_sh.eval: save_img(pred_disp[..., 0]), i.e. disparity clipped to [0, 1]
+            save_img(disp[..., 0], os.path.join(FLAGS.write_disp, f"disp_{i:04d}.png"))
+    psnr, ssim, frames = eval_octree(t, dataset, FLAGS, want_frames=True, lpips_fn=load_lpips(dev), metrics=extra,
+                                     disp_fn=disp_fn)
     print("Average PSNR", psnr, "SSIM", ssim, "LPIPS", extra["lpips"])
     if FLAGS.write_vid and frames:
         # evaluation.py:88-90: imageio.mimwrite at its default 10 fps

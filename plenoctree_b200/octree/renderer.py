@@ -6,6 +6,9 @@
     r.render_persp(c2w, height=H, width=W, fx=focal, fast=False)     render_persp (autograd-aware: the image
       octree/optimization.py:178,202, octree/nerf/utils.py:471        carries a grad_fn that fills tree.data.grad)
     r.forward(rays)  (svox.Rays(origins, dirs, viewdirs))            forward / __call__
+    (no svox counterpart)                                            forward / render_persp(..., return_depth=True)
+                                                                     -> (rgb, depth, acc) like nerf/utils.py's
+                                                                     render_image; disparity(depth, acc) -> disp
     mse.backward(); optimizer.step()  optimization.py:205-208        train_persp + N3Tree.sgd_step: one launch for
                                                                      render + clamp-MSE gradient + scatter
 
@@ -80,6 +83,42 @@ class _RenderFn(torch.autograd.Function):
         return g, None, None, None, None, None, None
 
 
+class _RenderDepthFn(torch.autograd.Function):
+    """autograd edge of (rgb, depth, acc): d loss / d tree.data through pob_octree_render_depth_backward (an output
+    whose gradient autograd leaves undefined is passed as NULL, i.e. zero)."""
+
+    @staticmethod
+    def forward(ctx, data, renderer, rays, cam, row0, nrows, opts):
+        ctx.set_materialize_grads(False)
+        ctx.renderer, ctx.rays, ctx.cam, ctx.row0, ctx.nrows = renderer, rays, cam, row0, nrows
+        return renderer._render_raw(rays, cam, row0, nrows, opts, return_depth=True)
+
+    @staticmethod
+    def backward(ctx, g_rgb, g_depth, g_acc):
+        r = ctx.renderer
+        tree = r.tree
+        g = torch.zeros_like(tree.data)
+        t = tree.c_struct()
+        o = r._opts(False)
+        flat = lambda x, c: None if x is None else x.reshape(-1, c).contiguous().float()   # noqa: E731
+        gr, gd, ga = flat(g_rgb, 3), flat(g_depth, 1), flat(g_acc, 1)
+        if ctx.cam is None:
+            ro, rd, rv = ctx.rays
+            src = (ptr(ro), ptr(rd), ptr(rv), ro.shape[0], None, 0, 0)
+        else:
+            src = (None, None, None, 0, ctypes.byref(ctx.cam), ctx.row0, ctx.nrows)
+        check(lib.pob_octree_render_depth_backward(ctypes.byref(t), ctypes.byref(o), *src, ptr(gr), ptr(gd), ptr(ga),
+                                                   ptr(g), stream_ptr()))
+        return g, None, None, None, None, None, None
+
+
+def disparity(depth, acc):
+    """disp = acc / depth where 0 < acc / depth < 1e10 and acc > 1e-10, else 1e10: the rule of the NeRF-SH compositing
+    kernel (render.cu, model_utils.volumetric_rendering), so a ray that misses the box gets 1e10."""
+    disp = acc / depth
+    return torch.where((disp > 0) & (disp < 1e10) & (acc > 1e-10), disp, torch.full_like(disp, 1e10))
+
+
 class VolumeRenderer:
     def __init__(self, tree, step_size=1e-3, background_brightness=1.0, ndc=None):
         if ndc is not None:
@@ -96,21 +135,28 @@ class VolumeRenderer:
         o.stop_thresh = 1e-2 if fast else 0.0
         return o
 
-    def _render_raw(self, rays, cam, row0, nrows, opts, counters=None):
+    def _render_raw(self, rays, cam, row0, nrows, opts, counters=None, return_depth=False):
+        """-> rgb [n,3] (explicit rays) / [nrows,W,3] (camera slab); with return_depth (rgb, depth, acc), the last two
+        of the same shape with 1 channel"""
         tree = self.tree
         t = tree.c_struct()
         if cam is None:
             ro, rd, rv = rays
-            n = ro.shape[0]
-            out = torch.empty((n, 3), dtype=torch.float32, device=tree.device)
-            check(lib.pob_octree_render(ctypes.byref(t), ctypes.byref(opts), ptr(ro), ptr(rd), ptr(rv), n, None, 0, 0,
-                                        ptr(out), ptr(counters), stream_ptr()))
+            shape = (ro.shape[0],)
+            src = (ptr(ro), ptr(rd), ptr(rv), ro.shape[0], None, 0, 0)
+        else:
+            shape = (nrows, int(cam.width))
+            src = (None, None, None, 0, ctypes.byref(cam), row0, nrows)
+        out = torch.empty(shape + (3,), dtype=torch.float32, device=tree.device)
+        if not return_depth:
+            check(lib.pob_octree_render(ctypes.byref(t), ctypes.byref(opts), *src, ptr(out), ptr(counters),
+                                        stream_ptr()))
             return out
-        W = int(cam.width)
-        out = torch.empty((nrows, W, 3), dtype=torch.float32, device=tree.device)
-        check(lib.pob_octree_render(ctypes.byref(t), ctypes.byref(opts), None, None, None, 0, ctypes.byref(cam), row0,
-                                    nrows, ptr(out), ptr(counters), stream_ptr()))
-        return out
+        depth = torch.empty(shape + (1,), dtype=torch.float32, device=tree.device)
+        acc = torch.empty(shape + (1,), dtype=torch.float32, device=tree.device)
+        check(lib.pob_octree_render_depth(ctypes.byref(t), ctypes.byref(opts), *src, ptr(out), ptr(depth), ptr(acc),
+                                          ptr(counters), stream_ptr()))
+        return out, depth, acc
 
     @staticmethod
     def _f32(t, dev):
@@ -118,29 +164,32 @@ class VolumeRenderer:
             t = torch.from_numpy(t)
         return t.to(device=dev, dtype=torch.float32).reshape(-1, 3).contiguous()
 
-    def forward(self, rays, fast=False, counters=None):
-        """VolumeRenderer.forward(rays: Rays(origins, dirs, viewdirs)) -> rgb [n,3]."""
-        dev = self.tree.device
-        r3 = (self._f32(rays.origins, dev), self._f32(rays.dirs, dev), self._f32(rays.viewdirs, dev))
-        opts = self._opts(fast)
+    def _render(self, rays, cam, row0, nrows, opts, counters, return_depth):
         data = self.tree.data
         if torch.is_grad_enabled() and data.requires_grad:
-            return _RenderFn.apply(data, self, r3, None, 0, 0, opts)
-        return self._render_raw(r3, None, 0, 0, opts, counters)
+            fn = _RenderDepthFn if return_depth else _RenderFn
+            return fn.apply(data, self, rays, cam, row0, nrows, opts)
+        return self._render_raw(rays, cam, row0, nrows, opts, counters, return_depth)
+
+    def forward(self, rays, fast=False, counters=None, return_depth=False):
+        """VolumeRenderer.forward(rays: Rays(origins, dirs, viewdirs)) -> rgb [n,3].  return_depth=True -> (rgb [n,3],
+        depth [n,1], acc [n,1]): acc = sum of the compositing weights (background excluded), depth = their sum over
+        the segment midpoints z, as the parameter of origin + z * dirs (csrc/octree.cu, trace_forward)."""
+        dev = self.tree.device
+        r3 = (self._f32(rays.origins, dev), self._f32(rays.dirs, dev), self._f32(rays.viewdirs, dev))
+        return self._render(r3, None, 0, 0, self._opts(fast), counters, return_depth)
 
     __call__ = forward
 
     def render_persp(self, c2w, width=256, height=256, fx=1111.111, fy=None, fast=False, cuda=True, rows=None,
-                     counters=None):
+                     counters=None, return_depth=False):
         """render_persp(c2w, width, height, fx) -> [H,W,3] (octree/optimization.py:178,202).  rows=(row0,nrows)
-        renders one pixel-row slab (rank sharding of evaluation renders)."""
+        renders one pixel-row slab (rank sharding of evaluation renders).  return_depth=True -> (rgb [H,W,3],
+        depth [H,W,1], acc [H,W,1]), depth along the camera axis (the distance along the pixel's unit ray times
+        1 / |(x, y, -1)|), the quantity disparity() turns into nerf_sh.eval's disparity maps."""
         cam = make_camera(c2w, width, height, fx, fy)
         row0, nrows = (0, int(height)) if rows is None else rows
-        opts = self._opts(fast)
-        data = self.tree.data
-        if torch.is_grad_enabled() and data.requires_grad:
-            return _RenderFn.apply(data, self, None, cam, row0, nrows, opts)
-        return self._render_raw(None, cam, row0, nrows, opts, counters)
+        return self._render(None, cam, row0, nrows, self._opts(fast), counters, return_depth)
 
     def train_persp(self, c2w, gt, width, height, fx, fy=None, rows=None, want_image=False, sq_err=None):
         """One training image of octree.optimization (octree/optimization.py:201-207) in ONE kernel: render the slab,
