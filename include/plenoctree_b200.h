@@ -34,6 +34,21 @@ extern "C" {
 #define POB_SIGMA_RELU 0
 #define POB_SIGMA_SOFTPLUS 1 /* log(1 + exp(x)), evaluated in fp32 as max(x, 0) + log1p(exp(-|x|)) */
 
+/* flags min_deg_point, max_deg_point, legacy_posenc_order (nerf_sh/nerf/utils.py:119-124,155-159): the point encoder
+ * posenc(x, min_deg, max_deg, legacy_order) (nerf_sh/nerf/model_utils.py:145-173) of a model.  Its width
+ * W = 3 + 6 (max_deg - min_deg) sets the parameter shapes Dense_0 [W, 256] and Dense_5 [256 + W, 256], so the flat
+ * layout, the packed blob's contents and every evaluation depend on it.  Accepted: 0 <= min_deg <= max_deg <= 10
+ * (W <= 63), legacy_order 0 or 1.  Feature order, c = 0..2, j = min_deg..max_deg-1:
+ *   legacy_order 0: [x, sin(2^j x_c) at 3 + 3(j - min_deg) + c, sin(2^j x_c + pi/2) at 3 + 3L + 3(j - min_deg) + c]
+ *   legacy_order 1: [x, sin(2^j x_c) at 3 + 6(j - min_deg) + c, sin(2^j x_c + pi/2) at 3 + 6(j - min_deg) + 3 + c]
+ * with L = max_deg - min_deg.  Every entry point taking a `const pob_posenc*` reads NULL as the reference default
+ * {0, 10, 0}, W = 63; the entry points without one use that default. */
+typedef struct pob_posenc {
+  int min_deg;
+  int max_deg;
+  int legacy_order;
+} pob_posenc;
+
 /* ---------------------------------------------------------------------------------------------
  * Library / device
  * ------------------------------------------------------------------------------------------- */
@@ -61,6 +76,10 @@ int64_t pob_param_count(int sh_deg);
 int64_t pob_packed_bytes(int sh_deg);
 /* flat fp32 parameters -> packed blob (fp16 hi/lo forward images, transposed images, biases) */
 int pob_pack_weights(const float* flat_dev, int sh_deg, void* packed_dev, void* stream);
+/* the same for a model with point encoder `posenc` (NULL = default): pob_param_count_pe parameters; the blob keeps
+ * pob_packed_bytes(sh_deg) bytes and its format */
+int64_t pob_param_count_pe(int sh_deg, const pob_posenc* posenc);
+int pob_pack_weights_pe(const float* flat_dev, int sh_deg, const pob_posenc* posenc, void* packed_dev, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * NerfModel.eval_points_raw(points, viewdirs=None, coarse=False) -> (raw_rgb[M,3K], raw_sigma[M,1])
@@ -101,6 +120,23 @@ int pob_eval_cells_mean(const void* packed_dev, int sh_deg, const float* points_
 int pob_eval_points_raw_host(const void* packed_dev, int sh_deg, const float* points_host,
                              int64_t m, float* raw_rgb_host, float* raw_sigma_host,
                              int precision);
+
+/* The point, grid and cell evaluators of a model with point encoder `posenc` (NULL = default; the blob packed with
+ * the same descriptor).  Each is the entry point above without `_pe`, which is its NULL case; pob_eval_points_pe
+ * takes the density activation like pob_eval_points_act. */
+int pob_eval_points_raw_pe(const void* packed_dev, int sh_deg, const pob_posenc* posenc, const float* points_dev,
+                           int64_t m, float* raw_rgb_dev, float* raw_sigma_dev, int precision, void* stream);
+int pob_eval_points_pe(const void* packed_dev, int sh_deg, const pob_posenc* posenc, const float* points_dev,
+                       const float* viewdirs_dev, int64_t m, float* out_rgbs_dev, int sigma_activation, int precision,
+                       void* stream);
+int pob_eval_grid_pe(const void* packed_dev, int sh_deg, const pob_posenc* posenc, int reso, int x0, int nx, int ny,
+                     int nz, const float offset[3], const float scale[3], float* raw_rgb_dev, float* raw_sigma_dev,
+                     int precision, void* stream);
+int pob_eval_cells_mean_pe(const void* packed_dev, int sh_deg, const pob_posenc* posenc, const float* points_dev,
+                           int64_t n_cells, int samples_per_cell, float* out_dev, int precision, void* stream);
+int pob_eval_points_raw_host_pe(const void* packed_dev, int sh_deg, const pob_posenc* posenc,
+                                const float* points_host, int64_t m, float* raw_rgb_host, float* raw_sigma_host,
+                                int precision);
 
 /* ---------------------------------------------------------------------------------------------
  * Per-ray stages (exposed individually for parity tests; pob_render_rays chains them).
@@ -155,6 +191,9 @@ typedef struct pob_render_config {
   /* flag sigma_activation: POB_SIGMA_* applied to the (noised) raw sigma of the ray samples; 0 = relu.  The
    * sparsity points of the training step keep relu (nerf_sh/train.py:82). */
   int sigma_activation;
+  /* flags min_deg_point / max_deg_point / legacy_posenc_order of both MLPs (pob_posenc); NULL = default.  The
+   * training step's grad_flat and params_dev follow its flat layout (pob_param_count_pe). */
+  const pob_posenc* posenc;
 } pob_render_config;
 
 /* bytes of device scratch the render (training=0) / training (training=1) calls need */
@@ -223,6 +262,11 @@ int pob_loss_and_grad_prec(const pob_render_config* cfg, const pob_train_hparams
 int pob_adam_update(int sh_deg, int num_mlps, float* params_dev, const float* grads_dev, float* m_dev,
                     float* v_dev, float lr, float step, const float* lr_step_dev, float grad_mult,
                     float weight_decay_coef, void* packed_coarse_dev, void* packed_fine_dev, void* stream);
+/* pob_adam_update of a model with point encoder `posenc` (NULL = default): num_mlps * pob_param_count_pe elements,
+ * re-packed with the same descriptor */
+int pob_adam_update_pe(int sh_deg, const pob_posenc* posenc, int num_mlps, float* params_dev, const float* grads_dev,
+                       float* m_dev, float* v_dev, float lr, float step, const float* lr_step_dev, float grad_mult,
+                       float weight_decay_coef, void* packed_coarse_dev, void* packed_fine_dev, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * PlenOctree side (SURVEY.md §8 rows a13-middle and a15).  These entry points stand where the

@@ -29,6 +29,8 @@ SIGNATURES = {
     "pob_param_count": (_i64, [_i]),
     "pob_packed_bytes": (_i64, [_i]),
     "pob_pack_weights": (_i, [_fp, _i, _vp, _vp]),
+    "pob_param_count_pe": (_i64, [_i, _vp]),
+    "pob_pack_weights_pe": (_i, [_fp, _i, _vp, _vp, _vp]),
     "pob_eval_points_raw": (_i, [_vp, _i, _fp, _i64, _fp, _fp, _i, _vp]),
     "pob_eval_points": (_i, [_vp, _i, _fp, _fp, _i64, _fp, _i, _vp]),
     "pob_eval_points_act": (_i, [_vp, _i, _fp, _fp, _i64, _fp, _i, _i, _vp]),
@@ -36,6 +38,12 @@ SIGNATURES = {
     "pob_eval_grid": (_i, [_vp, _i, _i, _i, _i, _i, _i, _c.POINTER(_c.c_float), _c.POINTER(_c.c_float),
                            _fp, _fp, _i, _vp]),
     "pob_eval_points_raw_host": (_i, [_vp, _i, _fp, _i64, _fp, _fp, _i]),
+    "pob_eval_points_raw_pe": (_i, [_vp, _i, _vp, _fp, _i64, _fp, _fp, _i, _vp]),
+    "pob_eval_points_pe": (_i, [_vp, _i, _vp, _fp, _fp, _i64, _fp, _i, _i, _vp]),
+    "pob_eval_grid_pe": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _c.POINTER(_c.c_float), _c.POINTER(_c.c_float),
+                              _fp, _fp, _i, _vp]),
+    "pob_eval_cells_mean_pe": (_i, [_vp, _i, _vp, _fp, _i64, _i, _fp, _i, _vp]),
+    "pob_eval_points_raw_host_pe": (_i, [_vp, _i, _vp, _fp, _i64, _fp, _fp, _i]),
     "pob_sample_coarse": (_i, [_fp, _fp, _i, _i, _fp, _vp]),
     "pob_draw_uniforms": (_i, [_c.c_uint64, _c.c_float, _fp, _fp, _i64, _fp, _i64, _fp, _i64, _c.c_float, _vp]),
     "pob_composite": (_i, [_fp, _fp, _fp, _i, _i, _i, _fp, _fp, _fp, _fp, _vp]),
@@ -50,6 +58,8 @@ SIGNATURES = {
                                     _fp, _vp, _vp, _fp, _i, _vp]),
     "pob_adam_update": (_i, [_i, _i, _fp, _fp, _fp, _fp, _c.c_float, _c.c_float, _fp, _c.c_float, _c.c_float,
                              _vp, _vp, _vp]),
+    "pob_adam_update_pe": (_i, [_i, _vp, _i, _fp, _fp, _fp, _fp, _c.c_float, _c.c_float, _fp, _c.c_float,
+                                _c.c_float, _vp, _vp, _vp]),
     "pob_octree_render": (_i, [_vp, _vp, _fp, _fp, _fp, _i64, _vp, _i, _i, _fp, _vp, _vp]),
     "pob_octree_render_backward": (_i, [_vp, _vp, _fp, _fp, _fp, _i64, _vp, _i, _i, _fp, _fp, _vp]),
     "pob_octree_render_depth": (_i, [_vp, _vp, _fp, _fp, _fp, _i64, _vp, _i, _i, _fp, _fp, _fp, _vp, _vp]),
@@ -64,10 +74,32 @@ SIGNATURES = {
 }
 
 
+class Posenc(_c.Structure):
+    """pob_posenc: the point encoder posenc(x, min_deg, max_deg, legacy_order); a NULL pointer is (0, 10, 0)."""
+    _fields_ = [("min_deg", _i), ("max_deg", _i), ("legacy_order", _i)]
+
+
+POSENC_DEFAULT = (0, 10, False)   # flags min_deg_point, max_deg_point, legacy_posenc_order of the reference
+
+
+def posenc_struct(posenc):
+    """(min_deg, max_deg, legacy) -> Posenc, or None (NULL) for the default, so that a default model calls the
+    library exactly as before the descriptor existed."""
+    if posenc is None or tuple(posenc) == POSENC_DEFAULT:
+        return None
+    mn, mx, legacy = posenc
+    return Posenc(int(mn), int(mx), int(bool(legacy)))
+
+
+def posenc_ref(struct):
+    """pointer argument of a Posenc (None -> NULL)."""
+    return None if struct is None else _c.addressof(struct)
+
+
 class RenderConfig(_c.Structure):
     _fields_ = [("sh_deg", _i), ("num_coarse_samples", _i), ("num_fine_samples", _i), ("white_bkgd", _i),
                 ("max_rays", _i), ("sparsity_npoints", _i), ("sigma_noise_coarse_dev", _vp),
-                ("sigma_noise_fine_dev", _vp), ("sigma_activation", _i)]
+                ("sigma_noise_fine_dev", _vp), ("sigma_activation", _i), ("posenc", _vp)]
 
 
 class TrainHParams(_c.Structure):

@@ -114,9 +114,10 @@ int check_common(const char* where, const void* packed, int sh_deg, int precisio
   return 0;
 }
 
-pob::FwdParams base_params(const void* packed, int sh_deg) {
+pob::FwdParams base_params(const void* packed, int sh_deg, pob::PosencDesc pe) {
   pob::FwdParams p;
   memset(&p, 0, sizeof(p));
+  p.pe = pe;
   p.sh_deg = sh_deg;
   p.K = K_of(sh_deg);
   p.NH = pob::heads_width(p.K);
@@ -130,7 +131,19 @@ int pob_sm_count_cached() { return sm_count(); }
 int pob_check_common(const char* where, const void* packed, int sh_deg, int precision) {
   return check_common(where, packed, sh_deg, precision);
 }
-pob::FwdParams pob_base_params(const void* packed, int sh_deg) { return base_params(packed, sh_deg); }
+pob::FwdParams pob_base_params(const void* packed, int sh_deg, pob::PosencDesc pe) {
+  return base_params(packed, sh_deg, pe);
+}
+int pob_check_posenc(const char* where, const pob_posenc* posenc, pob::PosencDesc& out) {
+  out = pob::POSENC_DEFAULT;
+  if (!posenc) return 0;
+  const pob::PosencDesc pe = {posenc->min_deg, posenc->max_deg, posenc->legacy_order};
+  if (!pob::posenc_valid(pe))
+    return fail(where, "posenc needs 0 <= min_deg <= max_deg <= 10 (width 3 + 6 (max_deg - min_deg) <= 63, the "
+                       "64-column posenc tile with its constant-one bias column) and legacy_order 0 or 1");
+  out = pe;
+  return 0;
+}
 int pob_check_sigma_activation(const char* where, int sigma_activation) {
   if (sigma_activation != POB_SIGMA_RELU && sigma_activation != POB_SIGMA_SOFTPLUS)
     return fail(where, "sigma_activation must be POB_SIGMA_RELU or POB_SIGMA_SOFTPLUS");
@@ -139,6 +152,8 @@ int pob_check_sigma_activation(const char* where, int sigma_activation) {
 
 extern "C" {
 
+// pob_posenc (pob_render_config.posenc, the *_pe entry points) left the version at 8, which callers pin; a caller
+// detects the descriptor by the presence of pob_param_count_pe
 int pob_abi_version(void) { return 8; }   // 8: pob_render_config.sigma_activation, pob_eval_points_act; 7:pob_octree_sgd_momentum_step; 6: pob_train_workspace_bytes, pob_loss_and_grad_prec (fp16x3 training); 5: sm_90a, no debug-trace / descriptor-probe entry points; 4: pob_loss_and_grad(mlp0_done_event), pob_adam_update(lr_step_dev)
 
 long long pob_launch_count(void) { return g_launches.load(); }
@@ -163,17 +178,21 @@ int pob_timing_read(double* ms_out, long long* launches_out) {
 const char* pob_last_error(void) { return g_err.c_str(); }
 int pob_sm_count(void) { return sm_count(); }
 
-int64_t pob_param_count(int sh_deg) {
-  if (!valid_deg(sh_deg)) return -1;
-  return pob::flat_layout(K_of(sh_deg)).total;
+int64_t pob_param_count_pe(int sh_deg, const pob_posenc* posenc) {
+  pob::PosencDesc pe;
+  if (!valid_deg(sh_deg) || pob_check_posenc("pob_param_count", posenc, pe)) return -1;
+  return pob::flat_layout(K_of(sh_deg), pob::posenc_width(pe)).total;
 }
+int64_t pob_param_count(int sh_deg) { return pob_param_count_pe(sh_deg, nullptr); }
 int64_t pob_packed_bytes(int sh_deg) {
   if (!valid_deg(sh_deg)) return -1;
   return (int64_t)blob_layout(K_of(sh_deg)).total;
 }
 
-int pob_pack_weights(const float* flat_dev, int sh_deg, void* packed_dev, void* stream) {
+int pob_pack_weights_pe(const float* flat_dev, int sh_deg, const pob_posenc* posenc, void* packed_dev, void* stream) {
   if (!valid_deg(sh_deg)) return fail("pob_pack_weights", "sh_deg must be in [-1, 4]");
+  pob::PosencDesc pe;
+  if (int e = pob_check_posenc("pob_pack_weights", posenc, pe)) return e;
   if (!flat_dev || !packed_dev) return fail("pob_pack_weights", "NULL pointer");
   const int K = K_of(sh_deg);
   const BlobLayout b = blob_layout(K);
@@ -181,17 +200,23 @@ int pob_pack_weights(const float* flat_dev, int sh_deg, void* packed_dev, void* 
   pob_count_launch();
   PobPhaseTimer _t(POB_PH_OPTIM, (cudaStream_t)stream);
   POB_CUDA("pob_pack_weights",
-           pob::launch_pack_weights(flat_dev, K, p + b.w_hi, p + b.w_lo, p + b.wt_hi, (cudaStream_t)stream));
+           pob::launch_pack_weights(flat_dev, K, pob::posenc_width(pe), p + b.w_hi, p + b.w_lo, p + b.wt_hi,
+                                    (cudaStream_t)stream));
   return 0;
 }
+int pob_pack_weights(const float* flat_dev, int sh_deg, void* packed_dev, void* stream) {
+  return pob_pack_weights_pe(flat_dev, sh_deg, nullptr, packed_dev, stream);
+}
 
-int pob_eval_points_raw(const void* packed_dev, int sh_deg, const float* points_dev, int64_t m,
-                        float* raw_rgb_dev, float* raw_sigma_dev, int precision, void* stream) {
+int pob_eval_points_raw_pe(const void* packed_dev, int sh_deg, const pob_posenc* posenc, const float* points_dev,
+                           int64_t m, float* raw_rgb_dev, float* raw_sigma_dev, int precision, void* stream) {
   if (int e = check_common("pob_eval_points_raw", packed_dev, sh_deg, precision)) return e;
+  pob::PosencDesc pe;
+  if (int e = pob_check_posenc("pob_eval_points_raw", posenc, pe)) return e;
   if (m < 0) return fail("pob_eval_points_raw", "negative point count");
   if (m == 0) return 0;
   if (!points_dev || !raw_sigma_dev) return fail("pob_eval_points_raw", "NULL pointer");
-  pob::FwdParams p = base_params(packed_dev, sh_deg);
+  pob::FwdParams p = base_params(packed_dev, sh_deg, pe);
   p.src_mode = pob::SRC_POINTS;
   p.M = m;
   p.points = points_dev;
@@ -204,19 +229,26 @@ int pob_eval_points_raw(const void* packed_dev, int sh_deg, const float* points_
            pob::launch_mlp_fwd(p, precision, sm_count(), (cudaStream_t)stream));
   return 0;
 }
+int pob_eval_points_raw(const void* packed_dev, int sh_deg, const float* points_dev, int64_t m,
+                        float* raw_rgb_dev, float* raw_sigma_dev, int precision, void* stream) {
+  return pob_eval_points_raw_pe(packed_dev, sh_deg, nullptr, points_dev, m, raw_rgb_dev, raw_sigma_dev, precision,
+                                stream);
+}
 
-int pob_eval_points_act(const void* packed_dev, int sh_deg, const float* points_dev,
-                        const float* viewdirs_dev, int64_t m, float* out_rgbs_dev, int sigma_activation,
-                        int precision, void* stream) {
+int pob_eval_points_pe(const void* packed_dev, int sh_deg, const pob_posenc* posenc, const float* points_dev,
+                       const float* viewdirs_dev, int64_t m, float* out_rgbs_dev, int sigma_activation, int precision,
+                       void* stream) {
   const char* where = "pob_eval_points";
   if (int e = check_common(where, packed_dev, sh_deg, precision)) return e;
+  pob::PosencDesc pe;
+  if (int e = pob_check_posenc(where, posenc, pe)) return e;
   if (int e = pob_check_sigma_activation(where, sigma_activation)) return e;
   if (m < 0) return fail(where, "negative point count");
   if (m == 0) return 0;
   if (!points_dev || !out_rgbs_dev) return fail(where, "NULL pointer");
   if (sh_deg >= 0 && !viewdirs_dev)
     return fail(where, "viewdirs required when sh_deg >= 0 (models.py:199)");
-  pob::FwdParams p = base_params(packed_dev, sh_deg);
+  pob::FwdParams p = base_params(packed_dev, sh_deg, pe);
   p.src_mode = pob::SRC_POINTS;
   p.M = m;
   p.points = points_dev;
@@ -230,6 +262,13 @@ int pob_eval_points_act(const void* packed_dev, int sh_deg, const float* points_
   return 0;
 }
 
+int pob_eval_points_act(const void* packed_dev, int sh_deg, const float* points_dev,
+                        const float* viewdirs_dev, int64_t m, float* out_rgbs_dev, int sigma_activation,
+                        int precision, void* stream) {
+  return pob_eval_points_pe(packed_dev, sh_deg, nullptr, points_dev, viewdirs_dev, m, out_rgbs_dev, sigma_activation,
+                            precision, stream);
+}
+
 int pob_eval_points(const void* packed_dev, int sh_deg, const float* points_dev,
                     const float* viewdirs_dev, int64_t m, float* out_rgbs_dev, int precision,
                     void* stream) {
@@ -237,13 +276,15 @@ int pob_eval_points(const void* packed_dev, int sh_deg, const float* points_dev,
                              stream);
 }
 
-int pob_eval_cells_mean(const void* packed_dev, int sh_deg, const float* points_dev, int64_t n_cells,
-                        int samples_per_cell, float* out_dev, int precision, void* stream) {
+int pob_eval_cells_mean_pe(const void* packed_dev, int sh_deg, const pob_posenc* posenc, const float* points_dev,
+                           int64_t n_cells, int samples_per_cell, float* out_dev, int precision, void* stream) {
   if (int e = check_common("pob_eval_cells_mean", packed_dev, sh_deg, precision)) return e;
+  pob::PosencDesc pe;
+  if (int e = pob_check_posenc("pob_eval_cells_mean", posenc, pe)) return e;
   if (n_cells < 0 || samples_per_cell <= 0) return fail("pob_eval_cells_mean", "bad sizes");
   if (n_cells == 0) return 0;
   if (!points_dev || !out_dev) return fail("pob_eval_cells_mean", "NULL pointer");
-  pob::FwdParams p = base_params(packed_dev, sh_deg);
+  pob::FwdParams p = base_params(packed_dev, sh_deg, pe);
   p.src_mode = pob::SRC_POINTS;
   p.M = n_cells * (int64_t)samples_per_cell;
   p.points = points_dev;
@@ -258,11 +299,18 @@ int pob_eval_cells_mean(const void* packed_dev, int sh_deg, const float* points_
            pob::launch_mlp_fwd(p, precision, sm_count(), (cudaStream_t)stream));
   return 0;
 }
+int pob_eval_cells_mean(const void* packed_dev, int sh_deg, const float* points_dev, int64_t n_cells,
+                        int samples_per_cell, float* out_dev, int precision, void* stream) {
+  return pob_eval_cells_mean_pe(packed_dev, sh_deg, nullptr, points_dev, n_cells, samples_per_cell, out_dev,
+                                precision, stream);
+}
 
-int pob_eval_grid(const void* packed_dev, int sh_deg, int reso, int x0, int nx, int ny, int nz,
-                  const float offset[3], const float scale[3], float* raw_rgb_dev,
-                  float* raw_sigma_dev, int precision, void* stream) {
+int pob_eval_grid_pe(const void* packed_dev, int sh_deg, const pob_posenc* posenc, int reso, int x0, int nx, int ny,
+                     int nz, const float offset[3], const float scale[3], float* raw_rgb_dev, float* raw_sigma_dev,
+                     int precision, void* stream) {
   if (int e = check_common("pob_eval_grid", packed_dev, sh_deg, precision)) return e;
+  pob::PosencDesc pe;
+  if (int e = pob_check_posenc("pob_eval_grid", posenc, pe)) return e;
   if (reso <= 0 || (reso & (reso - 1)))
     return fail("pob_eval_grid", "reso must be a power of two (extraction.py:246,290)");
   if (x0 < 0 || nx < 0 || ny < 0 || nz < 0 || x0 + nx > reso || ny > reso || nz > reso)
@@ -270,7 +318,7 @@ int pob_eval_grid(const void* packed_dev, int sh_deg, int reso, int x0, int nx, 
   if (!offset || !scale || !raw_sigma_dev) return fail("pob_eval_grid", "NULL pointer");
   const long long m = (long long)nx * ny * nz;
   if (m == 0) return 0;
-  pob::FwdParams p = base_params(packed_dev, sh_deg);
+  pob::FwdParams p = base_params(packed_dev, sh_deg, pe);
   p.src_mode = pob::SRC_GRID;
   p.M = m;
   p.g_reso = reso;
@@ -291,11 +339,19 @@ int pob_eval_grid(const void* packed_dev, int sh_deg, int reso, int x0, int nx, 
            pob::launch_mlp_fwd(p, precision, sm_count(), (cudaStream_t)stream));
   return 0;
 }
+int pob_eval_grid(const void* packed_dev, int sh_deg, int reso, int x0, int nx, int ny, int nz,
+                  const float offset[3], const float scale[3], float* raw_rgb_dev,
+                  float* raw_sigma_dev, int precision, void* stream) {
+  return pob_eval_grid_pe(packed_dev, sh_deg, nullptr, reso, x0, nx, ny, nz, offset, scale, raw_rgb_dev,
+                          raw_sigma_dev, precision, stream);
+}
 
-int pob_eval_points_raw_host(const void* packed_dev, int sh_deg, const float* points_host,
-                             int64_t m, float* raw_rgb_host, float* raw_sigma_host,
-                             int precision) {
+int pob_eval_points_raw_host_pe(const void* packed_dev, int sh_deg, const pob_posenc* posenc,
+                                const float* points_host, int64_t m, float* raw_rgb_host, float* raw_sigma_host,
+                                int precision) {
   if (int e = check_common("pob_eval_points_raw_host", packed_dev, sh_deg, precision)) return e;
+  pob::PosencDesc pe;
+  if (int e = pob_check_posenc("pob_eval_points_raw_host", posenc, pe)) return e;
   if (m <= 0) return m == 0 ? 0 : fail("pob_eval_points_raw_host", "negative point count");
   if (!points_host || !raw_sigma_host) return fail("pob_eval_points_raw_host", "NULL pointer");
   const int K = K_of(sh_deg);
@@ -314,7 +370,7 @@ int pob_eval_points_raw_host(const void* packed_dev, int sh_deg, const float* po
       rc = fail("pob_eval_points_raw_host", "H2D copy failed");
       break;
     }
-    rc = pob_eval_points_raw(packed_dev, sh_deg, d_pts, m, d_rgb, d_sig, precision, st);
+    rc = pob_eval_points_raw_pe(packed_dev, sh_deg, posenc, d_pts, m, d_rgb, d_sig, precision, st);
     if (rc) break;
     if (raw_rgb_host)
       cudaMemcpyAsync(raw_rgb_host, d_rgb, sizeof(float) * 3 * K * m, cudaMemcpyDeviceToHost, st);
@@ -326,6 +382,12 @@ int pob_eval_points_raw_host(const void* packed_dev, int sh_deg, const float* po
   cudaFree(d_rgb);
   cudaFree(d_sig);
   return rc;
+}
+int pob_eval_points_raw_host(const void* packed_dev, int sh_deg, const float* points_host,
+                             int64_t m, float* raw_rgb_host, float* raw_sigma_host,
+                             int precision) {
+  return pob_eval_points_raw_host_pe(packed_dev, sh_deg, nullptr, points_host, m, raw_rgb_host, raw_sigma_host,
+                                     precision);
 }
 
 int pob_sample_coarse(const float* z_base_dev, const float* t_rand_dev, int n_rays, int n_samples,

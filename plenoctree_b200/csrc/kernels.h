@@ -27,6 +27,21 @@ __device__ __forceinline__ float softplus_f32(float x) { return fmaxf(x, 0.f) + 
 // its derivative from its own output: d softplus / dx = sigmoid(x) = 1 - exp(-softplus(x)) = -expm1(-sigma)
 __device__ __forceinline__ float softplus_grad_of_output(float sigma) { return -expm1f(-sigma); }
 
+// The point encoder posenc(x, min_deg, max_deg, legacy) (model_utils.py:145-173; flags min_deg_point, max_deg_point,
+// legacy_posenc_order).  Its W = 3 + 6 (max_deg - min_deg) features fill posenc tile columns [0, W); columns [W, 63)
+// are 0 and column 63 is the constant 1 that carries the biases.  0 <= min_deg <= max_deg <= POSENC_MAX_DEG keeps
+// W <= 63 and the top scale 2^(max_deg - 1) inside posenc_sin's range (common.cuh).
+constexpr int POSENC_MAX_DEG = 10;
+struct PosencDesc {
+  int min_deg, max_deg, legacy;
+};
+constexpr PosencDesc POSENC_DEFAULT = {0, 10, 0};   // the reference default: W = 63 = ENC_DIM
+__host__ __device__ constexpr int posenc_width(PosencDesc pe) { return 3 + 6 * (pe.max_deg - pe.min_deg); }
+inline bool posenc_valid(PosencDesc pe) {
+  return pe.min_deg >= 0 && pe.min_deg <= pe.max_deg && pe.max_deg <= POSENC_MAX_DEG &&
+         (pe.legacy == 0 || pe.legacy == 1);
+}
+
 struct FwdParams {
   // ---- sample source ----
   int src_mode;
@@ -49,6 +64,7 @@ struct FwdParams {
   float g_offset[3], g_scale[3];
   // ---- model ----
   MlpPacked w;
+  PosencDesc pe;               // point encoder of the model (the packed Dense_0 / Dense_5 rows follow it)
   int sh_deg;                  // -1: 3 raw rgb channels, K = 1
   int K;                       // (sh_deg+1)^2
   int NH;                      // padded heads width, multiple of 16, <= 80
@@ -80,11 +96,12 @@ inline size_t bwd_image_bytes(int NH) { return size_t(bwd_slots(NH)) * WSLOT_BYT
 cudaError_t launch_mlp_fwd(const FwdParams& p, int nsplit, int num_sms, cudaStream_t stream);
 
 // flat fp32 parameters of one MLP in reference order (Dense_0..Dense_9: kernel [in,out] then
-// bias) -> packed images.  `nparams` = param_count(K).
-cudaError_t launch_pack_weights(const float* flat, int K, uint8_t* w_hi, uint8_t* w_lo,
+// bias; flat_layout(K, W), W = posenc_width) -> packed images.  The images do not depend on W: rows [W, 63) of the
+// posenc slots are 0.
+cudaError_t launch_pack_weights(const float* flat, int K, int W, uint8_t* w_hi, uint8_t* w_lo,
                                 uint8_t* wt_hi, cudaStream_t stream);
 // the residual (lo) of the dgrad images only, in the layout of wt_hi (bwd_image_bytes(NH)): the x3 data gradient
-cudaError_t launch_pack_wt_lo(const float* flat, int K, uint8_t* wt_lo, cudaStream_t stream);
+cudaError_t launch_pack_wt_lo(const float* flat, int K, int W, uint8_t* wt_lo, cudaStream_t stream);
 
 
 
@@ -200,9 +217,10 @@ struct WgradPass {
 // The bias sums (columns of dZ_l / dO, Dense_0: of dZ_0) of pass 2 repeat pass 0's: only passes 0 and 1 count them.
 constexpr int X3_WGRAD_PASSES = 3;
 constexpr int X3_BIAS_PASSES = 2;
-// partials of `npass` wgrad launches -> flat gradient of one MLP (reference layout), times inv_scale.  Every element
-// sums its passes in order; the biases only the first min(npass, X3_BIAS_PASSES).
-cudaError_t launch_reduce_grads(const WgradPass* passes, int npass, int K, float inv_scale, float* grad_flat,
+// partials of `npass` wgrad launches -> flat gradient of one MLP (reference layout flat_layout(K, W)), times
+// inv_scale.  Every element sums its passes in order; the biases only the first min(npass, X3_BIAS_PASSES).  The
+// rows of posenc columns [W, 64) are not part of the layout: they are dropped.
+cudaError_t launch_reduce_grads(const WgradPass* passes, int npass, int K, int W, float inv_scale, float* grad_flat,
                                 cudaStream_t stream);
 // flax.optim.Adam.apply_gradient on a flat buffer; grad is multiplied by grad_mult first
 // lr_step_dev (optional, device [2] = {lr, step}) overrides the host lr / step: a captured graph replays with new values
@@ -211,15 +229,16 @@ cudaError_t launch_adam(float* param, const float* grad, float* m, float* v, lon
                         float weight_decay_coef, cudaStream_t stream);
 
 // ---- flat parameter layout of one MLP (reference order) -------------------------------------
-// Dense_i kernel is [in,out] row-major (flax), followed by its bias [out].
+// Dense_i kernel is [in,out] row-major (flax), followed by its bias [out].  W = posenc width: Dense_0 is [W, 256],
+// Dense_5 [256 + W, 256] with rows [h4 | posenc].
 struct FlatLayout {
   int w_off[10], b_off[10], in_dim[10], out_dim[10], total;
 };
-inline FlatLayout flat_layout(int K) {
+inline FlatLayout flat_layout(int K, int W) {
   FlatLayout L;
   int off = 0;
   for (int i = 0; i < 10; ++i) {
-    int in = (i == 0) ? 63 : (i == 5 ? 319 : 256);
+    int in = (i == 0) ? W : (i == SKIP_LAYER ? WIDTH + W : WIDTH);
     int out = (i < 8) ? 256 : (i == 8 ? 1 : 3 * K);
     L.in_dim[i] = in;
     L.out_dim[i] = out;

@@ -97,27 +97,40 @@ __device__ __noinline__ void load_point(const FwdParams& p, long long s, float& 
   }
 }
 
-// Positional encoding of one sample into the E tile(s).  Feature order (model_utils.py:162-173):
-// [x(3), sin(2^j x_c) j-major (30), sin(2^j x_c + pi/2) (30)], column 63 = 1 (bias carrier).
-// unit_lo/unit_hi: which 16-byte units (8 features each) this thread stores.
-template <int NSPLIT, bool PRECISE>
-__device__ __noinline__ void posenc_row(uint8_t* e_hi, uint8_t* e_lo, int row, float x, float y,
-                                           float z, int unit_lo, int unit_hi, uint8_t* e_glob = nullptr) {
+// Positional encoding of one sample into the E tile(s), posenc(x, min_deg, max_deg, legacy) with L = max_deg - min_deg
+// (model_utils.py:145-173).  Feature k = 3 + i of the W = 3 + 6L is, for i < 6L and c = i % 3:
+//   standard order: [x(3), sin(2^j x_c) j-major (3L), sin(2^j x_c + pi/2) (3L)]
+//   legacy order:   [x(3), per degree j: sin(2^j x_c) (3), sin(2^j x_c + pi/2) (3)]
+// (the default (0, 10, standard) is [x, 30 sines, 30 cosines]).  Columns [W, 63) are 0 and column 63 = 1 (bias
+// carrier).  xb = x_c * 2^j is the exact fp32 product, the cosine the sine of the fp32 sum xb + pi/2, as the
+// reference's jnp expression.  unit_lo/unit_hi: which 16-byte units (8 features each) this thread stores.
+// GENERIC = false is the default encoder (0, 10, standard) with every index, scale and order a compile-time constant:
+// the fixed encoder's code.  The runtime decode of GENERIC = true sits on the forward's critical path (the MMAs wait
+// for the tile): compiled into the default's function it cost the default fp16 training step 2.4 %, and beside it
+// 0.5 % (H100 80 GB HBM3, 700 W), so the fp16 forwards call a separate instantiation for the default (posenc_row).
+// 2^j is built from its exponent bits there, exact for 0 <= j <= 30.
+template <int NSPLIT, bool PRECISE, bool GENERIC>
+__device__ __noinline__ void posenc_row_of(uint8_t* e_hi, uint8_t* e_lo, int row, float x, float y,
+                                           float z, int unit_lo, int unit_hi, PosencDesc pe, uint8_t* e_glob) {
   float f[64];
   f[0] = x;
   f[1] = y;
   f[2] = z;
   const float xyz[3] = {x, y, z};
   const float half_pi = 1.5707963267948966f;
+  const int min_deg = GENERIC ? pe.min_deg : 0;
+  const bool legacy = GENERIC ? pe.legacy != 0 : false;
+  const int L3 = GENERIC ? 3 * (pe.max_deg - pe.min_deg) : 30;   // sines (and cosines) per sample
 #pragma unroll
-  for (int j = 0; j < 10; ++j) {
-    const float sc = float(1 << j);
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      float xb = __fmul_rn(xyz[c], sc);
-      f[3 + 3 * j + c] = posenc_sin<PRECISE>(xb);
-      f[33 + 3 * j + c] = posenc_sin<PRECISE>(__fadd_rn(xb, half_pi));
-    }
+  for (int i = 0; i < ENC_DIM - 3; ++i) {
+    const int c = i % 3;                          // the same in both orders: every block is a multiple of 3 wide
+    const bool cosine = legacy ? (i % 6) >= 3 : i >= L3;
+    const bool on = i < 2 * L3;
+    const int j = on ? min_deg + (legacy ? i / 6 : (cosine ? i - L3 : i) / 3) : 0;
+    const float sc = GENERIC ? __int_as_float((127 + j) << 23) : float(1 << j);
+    const float xb = __fmul_rn(xyz[c], sc);
+    const float v = posenc_sin<PRECISE>(cosine ? __fadd_rn(xb, half_pi) : xb);
+    f[3 + i] = on ? v : 0.f;
   }
   f[63] = 1.f;   // constant-one column: carries the biases through the tensor cores (common.cuh)
 #pragma unroll
@@ -138,6 +151,16 @@ __device__ __noinline__ void posenc_row(uint8_t* e_hi, uint8_t* e_lo, int row, f
     if (NSPLIT == 3) *reinterpret_cast<uint4*>(e_lo + off) = make_uint4(wl[0], wl[1], wl[2], wl[3]);
     if (e_glob) *reinterpret_cast<uint4*>(e_glob + off) = make_uint4(w[0], w[1], w[2], w[3]);
   }
+}
+
+template <int NSPLIT, bool PRECISE>
+__device__ __forceinline__ void posenc_row(uint8_t* e_hi, uint8_t* e_lo, int row, float x, float y, float z,
+                                           int unit_lo, int unit_hi, PosencDesc pe, uint8_t* e_glob) {
+  // x3 runs the generic code for every encoder: a default instantiation beside libdevice sinf raised its spills
+  if (NSPLIT == 1 && pe.min_deg == POSENC_DEFAULT.min_deg && pe.max_deg == POSENC_DEFAULT.max_deg && pe.legacy == 0)
+    posenc_row_of<NSPLIT, PRECISE, false>(e_hi, e_lo, row, x, y, z, unit_lo, unit_hi, pe, e_glob);
+  else
+    posenc_row_of<NSPLIT, PRECISE, true>(e_hi, e_lo, row, x, y, z, unit_lo, unit_hi, pe, e_glob);
 }
 
 
@@ -379,7 +402,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
       const int u0 = 4 * (t >> 6);
       float x, y, z;
       load_point(p, it * TILE_M + r, x, y, z);
-      posenc_row<NSPLIT, PRECISE>(e_hi, e_lo, r, x, y, z, u0, u0 + 4,
+      posenc_row<NSPLIT, PRECISE>(e_hi, e_lo, r, x, y, z, u0, u0 + 4, p.pe,
                                   SAVE ? p.save_e + size_t(it) * E_TILE_BYTES : nullptr);
       fence_proxy_async_smem();
       warpgroup_sync(wg);
@@ -518,6 +541,7 @@ cudaError_t launch_mlp_fwd(const FwdParams& p, int nsplit, int num_sms, cudaStre
   if (p.M <= 0) return cudaSuccess;
   if (nsplit != 1 && nsplit != 3) return cudaErrorInvalidValue;
   if (p.sigma_act != SIGMA_RELU && p.sigma_act != SIGMA_SOFTPLUS) return cudaErrorInvalidValue;
+  if (!posenc_valid(p.pe)) return cudaErrorInvalidValue;
   const bool save = p.save_h != nullptr;
   if (save && (!p.save_e || !p.save_mask || (p.out_mode != OUT_RGBS && p.out_mode != OUT_SIGMA)))
     return cudaErrorInvalidValue;

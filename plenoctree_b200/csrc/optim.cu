@@ -171,14 +171,14 @@ __global__ void adam_kernel(float* __restrict__ param, const float* __restrict__
 
 }  // namespace
 
-cudaError_t launch_reduce_grads(const WgradPass* passes, int npass, int K, float inv_scale, float* grad_flat,
+cudaError_t launch_reduce_grads(const WgradPass* passes, int npass, int K, int W, float inv_scale, float* grad_flat,
                                 cudaStream_t stream) {
   if (npass < 1 || npass > X3_WGRAD_PASSES) return cudaErrorInvalidValue;
   ReduceArgs a;
   memset(&a, 0, sizeof(a));
   for (int q = 0; q < npass; ++q) a.pass[q] = passes[q];
   a.npass = npass;
-  a.L = flat_layout(K);
+  a.L = flat_layout(K, W);   // Dense_0 / Dense_5 rows i < W (+ 256) only: the zero posenc columns are dropped
   a.K = K;
   a.NH = heads_width(K);
   a.inv_scale = inv_scale;

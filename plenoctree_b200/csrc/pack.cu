@@ -2,8 +2,9 @@
 //
 // Flat layout of one MLP (matches the flax pytree MLP_i/Dense_0..Dense_9, kernels [in,out];
 // octree/nerf/models.py:75-102 documents the Dense index <-> layer mapping):
-//   Dense_0 63x256, Dense_1..4 256x256, Dense_5 319x256 ([h4 | posenc] rows), Dense_6..7,
-//   Dense_8 256x1 (sigma), Dense_9 256x3K (rgb / SH coefficients, channel-major c*K+k).
+//   Dense_0 Wx256, Dense_1..4 256x256, Dense_5 (256+W)x256 ([h4 | posenc] rows), Dense_6..7,
+//   Dense_8 256x1 (sigma), Dense_9 256x3K (rgb / SH coefficients, channel-major c*K+k);
+//   W = 3 + 6 (max_deg - min_deg) is the posenc width (63 by default).
 //
 // Forward images  (w_hi / w_lo): sequence of K-major SW64 slots [rows = out feature][32 k],
 //   in the order mlp_fwd consumes them.  Heads rows are re-ordered to [sigma, (k, c) ...] so the
@@ -21,7 +22,7 @@ namespace {
 struct PackArgs {
   const float* flat;
   FlatLayout L;
-  int K, NH;
+  int K, NH, W;
   uint8_t *w_hi, *w_lo, *wt_hi, *wt_lo;
   int dgrad_only;   // write the dgrad slots only (the forward images are left alone)
 };
@@ -67,12 +68,15 @@ __global__ void pack_weights_kernel(const __grid_constant__ PackArgs a) {
       }
       const int kin = 32 * j + kk;  // input feature index in the layer's [in] axis
       float v = 0.f;
-      if (fwd_has_bias_slot(l) && j == 8) {
-        if (kk == 31) v = a.flat[a.L.b_off[l] + n];            // bias slot: k = 31 <-> posenc column 63 (= 1)
-      } else if (kin < a.L.in_dim[l]) {
-        v = a.flat[a.L.w_off[l] + kin * 256 + n];
-      } else if (kin == a.L.in_dim[l] && !fwd_has_bias_slot(l)) {
-        v = a.flat[a.L.b_off[l] + n];                          // layers 0 / 5: the padding row k = 63 of posenc
+      if (fwd_has_bias_slot(l)) {
+        if (j < 8) v = a.flat[a.L.w_off[l] + kin * 256 + n];
+        else if (kk == 31) v = a.flat[a.L.b_off[l] + n];       // bias slot: k = 31 <-> posenc column 63 (= 1)
+      } else {
+        // layers 0 / 5: posenc column pc = kin (minus h4's 256 rows in layer 5) holds Dense row (256 +) pc for
+        // pc < W, 0 for pc in [W, 63), and the bias at pc = 63 (the constant-one column)
+        const int pc = l == SKIP_LAYER ? kin - WIDTH : kin;
+        if (pc < a.W) v = a.flat[a.L.w_off[l] + kin * 256 + n];
+        else if (pc == ENC_PAD - 1) v = a.flat[a.L.b_off[l] + n];
       }
       put_hilo(a.w_hi, a.w_lo, size_t(slot) * WSLOT_BYTES + w_slot_offset(n, kk), v);
     } else if (t < n_fwd_trunk + n_fwd_heads) {
@@ -101,12 +105,13 @@ __global__ void pack_weights_kernel(const __grid_constant__ PackArgs a) {
   }
 }
 
-cudaError_t launch_pack(const float* flat, int K, uint8_t* w_hi, uint8_t* w_lo, uint8_t* wt_hi, uint8_t* wt_lo,
-                        int dgrad_only, cudaStream_t stream) {
+cudaError_t launch_pack(const float* flat, int K, int W, uint8_t* w_hi, uint8_t* w_lo, uint8_t* wt_hi,
+                        uint8_t* wt_lo, int dgrad_only, cudaStream_t stream) {
   PackArgs a;
   a.flat = flat;
-  a.L = flat_layout(K);
+  a.L = flat_layout(K, W);
   a.K = K;
+  a.W = W;
   a.NH = heads_width(K);
   a.w_hi = w_hi;
   a.w_lo = w_lo;
@@ -119,13 +124,13 @@ cudaError_t launch_pack(const float* flat, int K, uint8_t* w_hi, uint8_t* w_lo, 
 
 }  // namespace
 
-cudaError_t launch_pack_weights(const float* flat, int K, uint8_t* w_hi, uint8_t* w_lo,
+cudaError_t launch_pack_weights(const float* flat, int K, int W, uint8_t* w_hi, uint8_t* w_lo,
                                 uint8_t* wt_hi, cudaStream_t stream) {
-  return launch_pack(flat, K, w_hi, w_lo, wt_hi, nullptr, 0, stream);
+  return launch_pack(flat, K, W, w_hi, w_lo, wt_hi, nullptr, 0, stream);
 }
 
-cudaError_t launch_pack_wt_lo(const float* flat, int K, uint8_t* wt_lo, cudaStream_t stream) {
-  return launch_pack(flat, K, nullptr, nullptr, nullptr, wt_lo, 1, stream);
+cudaError_t launch_pack_wt_lo(const float* flat, int K, int W, uint8_t* wt_lo, cudaStream_t stream) {
+  return launch_pack(flat, K, W, nullptr, nullptr, nullptr, wt_lo, 1, stream);
 }
 
 }  // namespace pob

@@ -125,12 +125,21 @@ int check_cfg(const char* where, const pob_render_config* c) {
     return pob_fail(where, "num_coarse_samples + num_fine_samples must be <= 256");
   if (c->max_rays <= 0) return pob_fail(where, "max_rays must be positive");
   if (c->sparsity_npoints < 0) return pob_fail(where, "sparsity_npoints must be >= 0");
+  PosencDesc pe;
+  if (int e = pob_check_posenc(where, c->posenc, pe)) return e;
   return pob_check_sigma_activation(where, c->sigma_activation);
 }
 
-FwdParams ray_fwd_params(const void* packed, int sh_deg, const float* o, const float* d, const float* v,
-                         const float* z, int R, int N, float4* out) {
-  FwdParams p = pob_base_params(packed, sh_deg);
+// the point encoder of a config that check_cfg accepted
+PosencDesc cfg_posenc(const pob_render_config& c) {
+  PosencDesc pe;
+  pob_check_posenc("", c.posenc, pe);
+  return pe;
+}
+
+FwdParams ray_fwd_params(const void* packed, int sh_deg, PosencDesc pe, const float* o, const float* d,
+                         const float* v, const float* z, int R, int N, float4* out) {
+  FwdParams p = pob_base_params(packed, sh_deg, pe);
   p.src_mode = SRC_RAYS;
   p.M = (long long)R * N;
   p.M_rays = p.M;
@@ -152,10 +161,11 @@ int forward_levels(const char* where, const pob_render_config& c, Workspace& w, 
                    const float* sp_points = nullptr, long long sp_n = 0) {
   const int sms = pob_sm_count_cached();
   const int Nc = c.num_coarse_samples, Nf = c.num_fine_samples;
+  const PosencDesc pe = cfg_posenc(c);
   Level& C = w.lv[0];
   { pob_count_launch(1); PobPhaseTimer _t(POB_PH_RENDER, st); POB_CUDA(where, launch_sample_coarse(z_base, t_rand, R, Nc, C.z, st)); }
   {
-    FwdParams p = ray_fwd_params(pk_c, c.sh_deg, o, d, v, C.z, R, Nc, C.rgbs);
+    FwdParams p = ray_fwd_params(pk_c, c.sh_deg, pe, o, d, v, C.z, R, Nc, C.rgbs);
     p.sigma_noise = c.sigma_noise_coarse_dev;
     p.sigma_act = c.sigma_activation;
     if (Nf == 0 && sp_n > 0) {     // single-level model: the sparsity points ride on this launch
@@ -179,7 +189,7 @@ int forward_levels(const char* where, const pob_render_config& c, Workspace& w, 
                                       cudaMemcpyDeviceToDevice, st));
     else
       { pob_count_launch(1); PobPhaseTimer _t(POB_PH_RENDER, st); POB_CUDA(where, launch_sample_pdf(C.z, C.weights, u, u_per_ray, R, Nc, Nf, F.z, st)); }
-    FwdParams p = ray_fwd_params(pk_f, c.sh_deg, o, d, v, F.z, R, Nc + Nf, F.rgbs);
+    FwdParams p = ray_fwd_params(pk_f, c.sh_deg, pe, o, d, v, F.z, R, Nc + Nf, F.rgbs);
     p.sigma_noise = c.sigma_noise_fine_dev;
     p.sigma_act = c.sigma_activation;
     if (sp_n > 0) {                // the sparsity points ride behind the fine level's ray samples (same MLP)
@@ -306,7 +316,9 @@ int pob_loss_and_grad_prec(const pob_render_config* cfg, const pob_train_hparams
   cudaStream_t st = (cudaStream_t)stream;
   const int sms = pob_sm_count_cached();
   const int K = cfg->sh_deg < 0 ? 1 : (cfg->sh_deg + 1) * (cfg->sh_deg + 1);
-  const int P = flat_layout(K).total;
+  const PosencDesc pe = cfg_posenc(*cfg);
+  const int W = posenc_width(pe);
+  const int P = flat_layout(K, W).total;
   Workspace w = carve(*cfg, 1, (uint8_t*)workspace_dev, x3);
   if (x3)
     if (int e = check_workspace_extent(where, workspace_dev, w.total)) return e;
@@ -315,7 +327,7 @@ int pob_loss_and_grad_prec(const pob_render_config* cfg, const pob_train_hparams
   if (x3) {
     // residual of the transposed weights (the packed blob holds only their hi part)
     for (int mlp = 0; mlp < (Nf > 0 ? 2 : 1); ++mlp)
-      { pob_count_launch(1); PobPhaseTimer _t(POB_PH_OPTIM, st); POB_CUDA(where, launch_pack_wt_lo(params_dev + size_t(mlp) * P, K, w.wt_lo[mlp], st)); }
+      { pob_count_launch(1); PobPhaseTimer _t(POB_PH_OPTIM, st); POB_CUDA(where, launch_pack_wt_lo(params_dev + size_t(mlp) * P, K, W, w.wt_lo[mlp], st)); }
   }
   // The sparsity points (train.py:77-83: eval_points_raw of the fine MLP on uniform points) ride behind the ray
   // samples of the last level: same MLP, same launches, rows [n_rays * N, n_rays * N + sp_n) of its arrays.
@@ -362,7 +374,7 @@ int pob_loss_and_grad_prec(const pob_render_config* cfg, const pob_train_hparams
     b.G = L.G;
     b.viewdirs = viewdirs_dev;
     b.n_per_ray = mlp == 0 ? Nc : Nc + Nf;
-    FwdParams base = pob_base_params(pk, cfg->sh_deg);
+    FwdParams base = pob_base_params(pk, cfg->sh_deg, pe);
     b.w = base.w;
     b.sh_deg = cfg->sh_deg;
     b.K = base.K;
@@ -394,7 +406,7 @@ int pob_loss_and_grad_prec(const pob_render_config* cfg, const pob_train_hparams
                                            passes[q].role_count);
       { pob_count_launch(); PobPhaseTimer _t(POB_PH_WGRAD, st); POB_CUDA(where, launch_mlp_wgrad(g, nctas, st)); }
     }
-    { pob_count_launch(); PobPhaseTimer _t(POB_PH_OPTIM, st); POB_CUDA(where, launch_reduce_grads(passes, npass, K, 1.0f / hp->loss_scale,
+    { pob_count_launch(); PobPhaseTimer _t(POB_PH_OPTIM, st); POB_CUDA(where, launch_reduce_grads(passes, npass, K, W, 1.0f / hp->loss_scale,
                                         grad_flat_dev + size_t(mlp) * P, st)); }
     if (mlp == 0 && Nf > 0 && mlp0_done_event) POB_CUDA(where, cudaEventRecord((cudaEvent_t)mlp0_done_event, st));
   }
@@ -413,23 +425,32 @@ int pob_loss_and_grad(const pob_render_config* cfg, const pob_train_hparams* hp,
                                 stream);
 }
 
-int pob_adam_update(int sh_deg, int num_mlps, float* params_dev, const float* grads_dev, float* m_dev,
-                    float* v_dev, float lr, float step, const float* lr_step_dev, float grad_mult,
-                    float weight_decay_coef, void* packed_coarse_dev, void* packed_fine_dev, void* stream) {
+int pob_adam_update_pe(int sh_deg, const pob_posenc* posenc, int num_mlps, float* params_dev, const float* grads_dev,
+                       float* m_dev, float* v_dev, float lr, float step, const float* lr_step_dev, float grad_mult,
+                       float weight_decay_coef, void* packed_coarse_dev, void* packed_fine_dev, void* stream) {
   const char* where = "pob_adam_update";
   if (sh_deg < -1 || sh_deg > 4) return pob_fail(where, "sh_deg must be in [-1, 4]");
+  PosencDesc pe;
+  if (int e = pob_check_posenc(where, posenc, pe)) return e;
   if (num_mlps < 1 || num_mlps > 2) return pob_fail(where, "num_mlps must be 1 or 2");
   if (!params_dev || !grads_dev || !m_dev || !v_dev || !packed_coarse_dev || (num_mlps == 2 && !packed_fine_dev))
     return pob_fail(where, "NULL pointer");
   cudaStream_t st = (cudaStream_t)stream;
   const int K = sh_deg < 0 ? 1 : (sh_deg + 1) * (sh_deg + 1);
-  const long long P = flat_layout(K).total;
+  const long long P = flat_layout(K, posenc_width(pe)).total;
   { pob_count_launch(1); PobPhaseTimer _t(POB_PH_OPTIM, st); POB_CUDA(where, launch_adam(params_dev, grads_dev, m_dev, v_dev, P * num_mlps, lr, step, lr_step_dev, 0.9f, 0.999f, 1e-8f,
                               grad_mult, weight_decay_coef, st)); }
-  if (int e = pob_pack_weights(params_dev, sh_deg, packed_coarse_dev, stream)) return e;
+  if (int e = pob_pack_weights_pe(params_dev, sh_deg, posenc, packed_coarse_dev, stream)) return e;
   if (num_mlps == 2)
-    if (int e = pob_pack_weights(params_dev + P, sh_deg, packed_fine_dev, stream)) return e;
+    if (int e = pob_pack_weights_pe(params_dev + P, sh_deg, posenc, packed_fine_dev, stream)) return e;
   return 0;
+}
+
+int pob_adam_update(int sh_deg, int num_mlps, float* params_dev, const float* grads_dev, float* m_dev,
+                    float* v_dev, float lr, float step, const float* lr_step_dev, float grad_mult,
+                    float weight_decay_coef, void* packed_coarse_dev, void* packed_fine_dev, void* stream) {
+  return pob_adam_update_pe(sh_deg, nullptr, num_mlps, params_dev, grads_dev, m_dev, v_dev, lr, step, lr_step_dev,
+                            grad_mult, weight_decay_coef, packed_coarse_dev, packed_fine_dev, stream);
 }
 
 }  // extern "C"

@@ -97,18 +97,37 @@ def fwd_slots_of_layer(l):
     return 2 if l == 0 else (10 if l == 5 else 9)
 
 
-def layer_dims(K):
+ENC_DIM = 63      # posenc width of the default encoder (0, 10); columns [W, 63) of the posenc tile are 0, 63 is 1
+POSENC_MAX_DEG = 10
+
+
+def posenc_width(posenc=None):
+    """W = 3 + 6 (max_deg - min_deg) of the point encoder (min_deg, max_deg, legacy); None = (0, 10) -> 63."""
+    if posenc is None:
+        return ENC_DIM
+    return 3 + 6 * (int(posenc[1]) - int(posenc[0]))
+
+
+def posenc_valid(posenc):
+    """the encoders the kernels take: 0 <= min_deg <= max_deg <= 10 (mirrors kernels.h posenc_valid)."""
+    mn, mx = int(posenc[0]), int(posenc[1])
+    return 0 <= mn <= mx <= POSENC_MAX_DEG
+
+
+def layer_dims(K, W=ENC_DIM):
+    """(in, out) of Dense_0..Dense_9 for K SH coefficients and posenc width W: Dense_0 [W, 256], Dense_5 [256 + W, 256]
+    (rows [h4 | posenc])."""
     dims = []
     for i in range(10):
-        cin = 63 if i == 0 else (319 if i == 5 else 256)
+        cin = W if i == 0 else (256 + W if i == 5 else 256)
         cout = 256 if i < 8 else (1 if i == 8 else 3 * K)
         dims.append((cin, cout))
     return dims
 
 
-def flat_offsets(K):
+def flat_offsets(K, W=ENC_DIM):
     w_off, b_off, off = [], [], 0
-    for cin, cout in layer_dims(K):
+    for cin, cout in layer_dims(K, W):
         w_off.append(off)
         off += cin * cout
         b_off.append(off)
@@ -128,9 +147,9 @@ def blob_layout(K):
     return dict(w_hi=w_hi, w_lo=w_lo, wt_hi=wt_hi, total=total, fwd_bytes=fwd, bwd_bytes=bwd, NH=NH)
 
 
-def heads_matrix(flat, K):
+def heads_matrix(flat, K, W=ENC_DIM):
     """packed heads weight [256 in, NH] and bias [NH] in kernel column order [sigma, (k,c)...]."""
-    w_off, b_off, _ = flat_offsets(K)
+    w_off, b_off, _ = flat_offsets(K, W)
     NH = heads_width(K)
     W8 = flat[w_off[8]:w_off[8] + 256].reshape(256, 1)
     W9 = flat[w_off[9]:w_off[9] + 256 * 3 * K].reshape(256, 3 * K)
@@ -153,15 +172,17 @@ def heads_column(K, o):
     return 1 + 3 * k + c
 
 
-def pack_reference(flat, sh_deg):
-    """numpy model of pack.cu: returns dict of uint8 images w_hi, w_lo, wt_hi."""
+def pack_reference(flat, sh_deg, posenc=None):
+    """numpy model of pack.cu: returns dict of uint8 images w_hi, w_lo, wt_hi.  posenc = (min_deg, max_deg, legacy)
+    of the model (None: the default); the images keep their size, with rows [W, 63) of the posenc slots zero."""
     K = K_of(sh_deg)
+    W = posenc_width(posenc)
     L = blob_layout(K)
     NH = L["NH"]
-    w_off, b_off, total = flat_offsets(K)
+    w_off, b_off, total = flat_offsets(K, W)
     flat = np.asarray(flat, np.float32)
     assert flat.size == total
-    dims = layer_dims(K)
+    dims = layer_dims(K, W)
     w_hi = np.zeros(L["fwd_bytes"], np.uint8)
     w_lo = np.zeros(L["fwd_bytes"], np.uint8)
     wt_hi = np.zeros(L["bwd_bytes"], np.uint8)
@@ -174,23 +195,26 @@ def pack_reference(flat, sh_deg):
     slot = 0
     for l in range(8):
         cin = dims[l][0]
-        W = flat[w_off[l]:w_off[l] + cin * 256].reshape(cin, 256)  # [in, out]
+        Wl = flat[w_off[l]:w_off[l] + cin * 256].reshape(cin, 256)  # [in, out]
+        if not fwd_has_bias_slot(l):
+            # layers 0 / 5: the K rows follow the posenc tile's 64 columns, the bias on its constant column 63
+            h = cin - W                            # h4 rows before the posenc rows (layer 5)
+            full = np.zeros((h + 64, 256), np.float32)
+            full[:cin] = Wl
+            full[h + 63] = flat[b_off[l]:b_off[l] + 256]
+            Wl = full
         bias_l = flat[b_off[l]:b_off[l] + 256]
         for j in range(fwd_slots_of_layer(l)):
             blk = np.zeros((256, 32), np.float32)  # [out row, k]
             if fwd_has_bias_slot(l) and j == 8:
                 blk[:, 31] = bias_l                # bias slot: multiplied by posenc column 63 (= 1)
             else:
-                k0 = 32 * j
-                kn = max(0, min(32, cin - k0))
-                blk[:, :kn] = W[k0:k0 + kn, :].T
-                if not fwd_has_bias_slot(l) and k0 <= cin < k0 + 32:
-                    blk[:, cin - k0] = bias_l      # layers 0 / 5: padding row k = 63 of the posenc operand
+                blk[:, :] = Wl[32 * j:32 * j + 32, :].T
             hi, lo = hilo(blk)
             w_hi[slot * 16384:(slot + 1) * 16384] = pack_w_slot(hi)
             w_lo[slot * 16384:(slot + 1) * 16384] = pack_w_slot(lo)
             slot += 1
-    Wh, bh = heads_matrix(flat, K)
+    Wh, bh = heads_matrix(flat, K, W)
     base = 66 * 16384
     for j in range(9):
         if j < 8:
@@ -212,9 +236,9 @@ def pack_reference(flat, sh_deg):
         slot += 1
     for l in range(7, 0, -1):
         cin = dims[l][0]
-        W = flat[w_off[l]:w_off[l] + cin * 256].reshape(cin, 256)[:256]  # [in(256), out]
+        Wl = flat[w_off[l]:w_off[l] + cin * 256].reshape(cin, 256)[:256]  # [in(256), out]
         for j in range(8):
-            wt_hi[slot * 16384:(slot + 1) * 16384] = pack_w_slot(W[:, 32 * j:32 * j + 32])
+            wt_hi[slot * 16384:(slot + 1) * 16384] = pack_w_slot(Wl[:, 32 * j:32 * j + 32])
             slot += 1
     return dict(w_hi=w_hi, w_lo=w_lo, wt_hi=wt_hi)
 
@@ -368,7 +392,7 @@ def decode_dz(DZ, layer):
 
 
 def decode_e(E):
-    """E [tiles, 16 KB] (SW128) -> fp16 posenc [tiles * 128, 64] (column 63 = 1)."""
+    """E [tiles, 16 KB] (SW128) -> fp16 posenc [tiles * 128, 64] (columns [W, 63) = 0, column 63 = 1)."""
     return _decode(E, "A64", 64)
 
 

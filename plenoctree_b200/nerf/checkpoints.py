@@ -22,28 +22,39 @@ import re
 import msgpack
 import numpy as np
 
-from ..layouts import K_of, layer_dims
+from ..layouts import K_of, layer_dims, posenc_width
 
 _EXT_NDARRAY, _EXT_NATIVE_COMPLEX, _EXT_NPSCALAR = 1, 2, 3
 
 
 # ---- flat <-> nested parameter dicts -------------------------------------------------------------------------
-def param_count(sh_deg):
-    return sum(i * o + o for i, o in layer_dims(K_of(sh_deg)))
+# `posenc` = (min_deg_point, max_deg_point, legacy_posenc_order) of the model, None = the default (0, 10, False): its
+# width W = 3 + 6 (max - min) sets the shapes Dense_0 [W, 256] and Dense_5 [256 + W, 256].
+def _dims(sh_deg, posenc):
+    return layer_dims(K_of(sh_deg), posenc_width(posenc))
 
 
-def flat_to_flax_params(flat, sh_deg):
+def _posenc_of(model):
+    """the model's encoder; objects without one (duck-typed models) have the default"""
+    return getattr(model, "posenc", None)
+
+
+def param_count(sh_deg, posenc=None):
+    return sum(i * o + o for i, o in _dims(sh_deg, posenc))
+
+
+def flat_to_flax_params(flat, sh_deg, posenc=None):
     """flat [num_mlps * P] -> {"MLP_0": {"Dense_i": {"kernel": [in,out], "bias": [out]}}, "MLP_1": ...}
     (the pytree under ["optimizer"]["target"]["params"], nerf_sh/nerf/model_utils.py:60-93)."""
     flat = np.asarray(flat, dtype=np.float32).reshape(-1)
-    P = param_count(sh_deg)
+    P = param_count(sh_deg, posenc)
     if flat.size % P != 0 or flat.size // P not in (1, 2):
         raise ValueError(f"expected {P} or {2 * P} parameters, got {flat.size}")
     out = {}
     for m in range(flat.size // P):
         off = m * P
         mlp = {}
-        for i, (cin, cout) in enumerate(layer_dims(K_of(sh_deg))):
+        for i, (cin, cout) in enumerate(_dims(sh_deg, posenc)):
             k = flat[off:off + cin * cout].reshape(cin, cout).copy()
             off += cin * cout
             b = flat[off:off + cout].copy()
@@ -53,17 +64,19 @@ def flat_to_flax_params(flat, sh_deg):
     return out
 
 
-def flax_params_to_flat(params, sh_deg):
+def flax_params_to_flat(params, sh_deg, posenc=None):
     parts = []
     m = 0
     while f"MLP_{m}" in params:
         mlp = params[f"MLP_{m}"]
-        for i, (cin, cout) in enumerate(layer_dims(K_of(sh_deg))):
+        for i, (cin, cout) in enumerate(_dims(sh_deg, posenc)):
             d = mlp[f"Dense_{i}"]
             k = np.asarray(d["kernel"], dtype=np.float32)
             b = np.asarray(d["bias"], dtype=np.float32)
             if k.shape != (cin, cout) or b.shape != (cout,):
-                raise ValueError(f"MLP_{m}/Dense_{i}: expected kernel {(cin, cout)}, got {k.shape} (wrong sh_deg?)")
+                hint = ("wrong min_deg_point / max_deg_point? Dense_0 has 3 + 6 (max_deg_point - min_deg_point) rows"
+                        if i in (0, 5) and k.shape[1:] == (cout,) else "wrong sh_deg?")
+                raise ValueError(f"MLP_{m}/Dense_{i}: expected kernel {(cin, cout)}, got {k.shape} ({hint})")
             parts += [k.reshape(-1), b]
         m += 1
     if m == 0:
@@ -74,18 +87,18 @@ def flax_params_to_flat(params, sh_deg):
 _TORCH_NAMES = [f"input_layers.{i}" for i in range(8)] + ["sigma_layer", "rgb_layer"]
 
 
-def flat_to_torch_state_dict(flat, sh_deg):
+def flat_to_torch_state_dict(flat, sh_deg, posenc=None):
     """-> {"MLP_0.input_layers.0.weight": [out,in], ...} as numpy arrays: the state_dict of the reference's torch
     twin (octree/nerf/models.py:116-209, octree/nerf/model_utils.py:36-95), nn.Linear weight = kernel.T."""
     out = {}
-    for mname, mlp in flat_to_flax_params(flat, sh_deg).items():
+    for mname, mlp in flat_to_flax_params(flat, sh_deg, posenc).items():
         for i, tname in enumerate(_TORCH_NAMES):
             out[f"{mname}.{tname}.weight"] = np.ascontiguousarray(mlp[f"Dense_{i}"]["kernel"].T)
             out[f"{mname}.{tname}.bias"] = mlp[f"Dense_{i}"]["bias"]
     return out
 
 
-def torch_state_dict_to_flat(sd, sh_deg):
+def torch_state_dict_to_flat(sd, sh_deg, posenc=None):
     params = {}
     m = 0
     while f"MLP_{m}.input_layers.0.weight" in sd:
@@ -95,7 +108,7 @@ def torch_state_dict_to_flat(sd, sh_deg):
             mlp[f"Dense_{i}"] = {"kernel": w.T, "bias": np.asarray(sd[f"MLP_{m}.{tname}.bias"], dtype=np.float32)}
         params[f"MLP_{m}"] = mlp
         m += 1
-    return flax_params_to_flat(params, sh_deg)
+    return flax_params_to_flat(params, sh_deg, posenc)
 
 
 # ---- flax.serialization msgpack encoding -------------------------------------------------------------------------
@@ -141,13 +154,13 @@ def msgpack_restore(data):
 
 
 # ---- TrainState <-> flax state dict ---------------------------------------------------------------------------
-def train_state_dict(params_flat, m_flat, v_flat, step, sh_deg):
+def train_state_dict(params_flat, m_flat, v_flat, step, sh_deg, posenc=None):
     """to_state_dict(utils.TrainState(optimizer=flax.optim.Adam(...).create(variables))):
     {"optimizer": {"target": {"params": ...}, "state": {"step": int32, "param_states": {"params": <same tree with
     {"grad_ema", "grad_sq_ema"} leaves>}}}}  (nerf_sh/nerf/models.py:44-48, flax.optim.Adam._AdamParamState)."""
-    tgt = flat_to_flax_params(params_flat, sh_deg)
-    gm = flat_to_flax_params(m_flat, sh_deg)
-    gv = flat_to_flax_params(v_flat, sh_deg)
+    tgt = flat_to_flax_params(params_flat, sh_deg, posenc)
+    gm = flat_to_flax_params(m_flat, sh_deg, posenc)
+    gv = flat_to_flax_params(v_flat, sh_deg, posenc)
     ps = {}
     for mname in tgt:
         ps[mname] = {}
@@ -158,10 +171,10 @@ def train_state_dict(params_flat, m_flat, v_flat, step, sh_deg):
                           "state": {"step": np.int32(step), "param_states": {"params": ps}}}}
 
 
-def state_dict_to_flat(sd, sh_deg):
+def state_dict_to_flat(sd, sh_deg, posenc=None):
     """-> (params, m, v, step); m / v are None when the file holds no optimiser state."""
     opt = sd["optimizer"]
-    params = flax_params_to_flat(opt["target"]["params"], sh_deg)
+    params = flax_params_to_flat(opt["target"]["params"], sh_deg, posenc)
     m = v = None
     step = 0
     if "state" in opt and opt["state"] is not None:
@@ -170,7 +183,7 @@ def state_dict_to_flat(sd, sh_deg):
         if ps:
             gm = {mn: {dn: {w: ps[mn][dn][w]["grad_ema"] for w in ("kernel", "bias")} for dn in ps[mn]} for mn in ps}
             gv = {mn: {dn: {w: ps[mn][dn][w]["grad_sq_ema"] for w in ("kernel", "bias")} for dn in ps[mn]} for mn in ps}
-            m, v = flax_params_to_flat(gm, sh_deg), flax_params_to_flat(gv, sh_deg)
+            m, v = flax_params_to_flat(gm, sh_deg, posenc), flax_params_to_flat(gv, sh_deg, posenc)
     return params, m, v, step
 
 
@@ -190,7 +203,7 @@ def save_checkpoint(train_dir, model, state, step=None, keep=100, prefix="checkp
     step = int(state.step if step is None else step)
     os.makedirs(train_dir, exist_ok=True)
     sd = train_state_dict(model.params.detach().cpu().numpy(), state.m.detach().cpu().numpy(),
-                          state.v.detach().cpu().numpy(), state.step, model.sh_deg)
+                          state.v.detach().cpu().numpy(), state.step, model.sh_deg, _posenc_of(model))
     path = os.path.join(train_dir, f"{prefix}{step}")
     tmp = path + ".tmp"
     with open(tmp, "wb") as f:
@@ -224,7 +237,7 @@ def restore_checkpoint(train_dir, model, state=None):
     sd = restore_flax_state_dict(train_dir)
     if sd is None:
         return None
-    params, m, v, step = state_dict_to_flat(sd, model.sh_deg)
+    params, m, v, step = state_dict_to_flat(sd, model.sh_deg, _posenc_of(model))
     model.set_params(params)
     if state is not None:
         import torch
@@ -239,7 +252,8 @@ def save_torch_ckpt(path, model):
     """torch `*.ckpt` = {"model": state_dict} of the reference's torch twin (octree/nerf/models.py:52-63)."""
     import torch
     sd = {k: torch.from_numpy(np.ascontiguousarray(v))
-          for k, v in flat_to_torch_state_dict(model.params.detach().cpu().numpy(), model.sh_deg).items()}
+          for k, v in flat_to_torch_state_dict(model.params.detach().cpu().numpy(), model.sh_deg,
+                                                     _posenc_of(model)).items()}
     torch.save({"model": sd}, path)
 
 
@@ -251,7 +265,7 @@ def restore_model_state(train_dir, model):
         return None
     ckpt = torch.load(paths[-1], map_location="cpu")
     sd = {k: v.numpy() for k, v in ckpt["model"].items()}
-    model.set_params(torch_state_dict_to_flat(sd, model.sh_deg))
+    model.set_params(torch_state_dict_to_flat(sd, model.sh_deg, _posenc_of(model)))
     return paths[-1]
 
 
@@ -260,5 +274,5 @@ def restore_model_state_from_jaxnerf(train_dir, model):
     sd = restore_flax_state_dict(train_dir)
     if sd is None:
         return None
-    model.set_params(flax_params_to_flat(sd["optimizer"]["target"]["params"], model.sh_deg))
+    model.set_params(flax_params_to_flat(sd["optimizer"]["target"]["params"], model.sh_deg, _posenc_of(model)))
     return True

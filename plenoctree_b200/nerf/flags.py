@@ -139,6 +139,21 @@ def sigma_activation_code(name):
     return code
 
 
+POSENC_MAX_DEG = 10
+
+
+def check_posenc(min_deg_point, max_deg_point):
+    """flags min_deg_point / max_deg_point (either legacy_posenc_order) that the kernels take: 0 <= min <= max <= 10.
+    The W = 3 + 6 (max - min) features must fit the 64-column posenc tile beside its constant-one bias column
+    (W <= 63), and the top scale 2^(max - 1) must stay inside the posenc sine's accurate range."""
+    mn, mx = int(min_deg_point), int(max_deg_point)
+    if not 0 <= mn <= mx <= POSENC_MAX_DEG:
+        raise NotImplementedError(
+            f"posenc degrees min_deg_point={mn}, max_deg_point={mx}: 0 <= min_deg_point <= max_deg_point <= 10 "
+            f"expected (the width 3 + 6 (max - min) = {3 + 6 * (mx - mn)} must fit the 64-column posenc tile with its "
+            "bias column, and scales above 2^9 leave the posenc sine's range)")
+
+
 def check_scope(args):
     """features of the reference this path does not cover: fail loudly instead of training something else."""
     if args.use_viewdirs:
@@ -147,12 +162,11 @@ def check_scope(args):
         raise NotImplementedError("spherical gaussians (sg_dim) are outside the NeRF-SH path")
     if args.dataset not in ("blender", "llff", "nsvf"):
         raise NotImplementedError(f"dataset {args.dataset!r}: blender, llff or nsvf expected")
-    if (args.net_depth, args.net_width, args.skip_layer, args.min_deg_point, args.max_deg_point) != (8, 256, 4, 0, 10):
-        raise NotImplementedError("the fused kernel is built for the 8x256 trunk, skip 4, posenc degrees 0..10")
+    if (args.net_depth, args.net_width, args.skip_layer) != (8, 256, 4):
+        raise NotImplementedError("the fused kernel is built for the 8x256 trunk with the skip after layer 4")
+    check_posenc(args.min_deg_point, args.max_deg_point)
     if (str(args.net_activation).lower(), str(args.rgb_activation).lower()) != ("relu", "sigmoid"):
         raise NotImplementedError("activations other than relu (trunk) / sigmoid (rgb)")
     sigma_activation_code(args.sigma_activation)
-    if args.legacy_posenc_order:
-        raise NotImplementedError("legacy_posenc_order is outside the scope of this path")
     if (args.render_path or args.spherify) and args.dataset != "llff":
         raise ValueError("render_path / spherify apply to the llff dataset only")        # datasets.py:194-195,496-497

@@ -16,8 +16,8 @@ import numpy as np
 import torch
 
 from .. import _lib
-from .._lib import PREC_FP16, RenderConfig, check, lib, ptr, stream_ptr
-from ..layouts import K_of
+from .._lib import PREC_FP16, RenderConfig, check, lib, posenc_ref, posenc_struct, ptr, stream_ptr
+from ..layouts import K_of, posenc_width, posenc_valid
 
 from .rays import Rays  # noqa: F401  (nerf_sh/nerf/utils.py:53)
 
@@ -33,11 +33,12 @@ def _cuda_f32(t, name, shape_last=None):
     return t
 
 
-def glorot_uniform_flat(sh_deg, generator=None):
-    """Dense kernel_init=glorot_uniform, zero bias (nerf_sh/nerf/model_utils.py:63-65)."""
+def glorot_uniform_flat(sh_deg, generator=None, posenc=None):
+    """Dense kernel_init=glorot_uniform, zero bias (nerf_sh/nerf/model_utils.py:63-65); the fan-in of Dense_0 and
+    Dense_5 follows the posenc width of `posenc` (min_deg, max_deg, legacy; None = the default)."""
     from ..layouts import layer_dims
     parts = []
-    for cin, cout in layer_dims(K_of(sh_deg)):
+    for cin, cout in layer_dims(K_of(sh_deg), posenc_width(posenc)):
         a = math.sqrt(6.0 / (cin + cout))
         parts.append((torch.rand(cin * cout, generator=generator) * 2 - 1) * a)
         parts.append(torch.zeros(cout))
@@ -52,10 +53,17 @@ class NerfModel:
 
     def __init__(self, sh_deg=3, num_coarse_samples=64, num_fine_samples=128, near=2.0, far=6.0,
                  white_bkgd=True, lindisp=False, max_rays=4096, sparsity_npoints=0, device="cuda",
-                 precision=PREC_FP16, noise_std=None, sigma_activation="relu"):
+                 precision=PREC_FP16, noise_std=None, sigma_activation="relu", min_deg_point=0, max_deg_point=10,
+                 legacy_posenc_order=False):
         from .flags import sigma_activation_code
         if not (-1 <= sh_deg <= 4):
             raise ValueError("sh_deg must be in [-1, 4]")
+        # flags min_deg_point / max_deg_point / legacy_posenc_order (nerf_sh/nerf/models.py:121-126): the point
+        # encoder of both MLPs, which also sets the shapes of Dense_0 [W, 256] and Dense_5 [256 + W, 256]
+        self.posenc = (int(min_deg_point), int(max_deg_point), bool(legacy_posenc_order))
+        if not posenc_valid(self.posenc):
+            raise ValueError("posenc degrees must satisfy 0 <= min_deg_point <= max_deg_point <= 10")
+        self._posenc_struct = posenc_struct(self.posenc)   # None (NULL) for the default encoder
         # flag sigma_activation (nerf_sh/nerf/models.py:280-281): relu or softplus of the ray samples' raw sigma and
         # of eval_points; raw sigma (eval_points_raw, extraction) and the sparsity term never take it
         self.sigma_activation = str(sigma_activation)
@@ -72,13 +80,14 @@ class NerfModel:
         self.noise_std = noise_std   # flag noise_std (nerf_sh/nerf/utils.py:137-142); None = no density noise
         self.device = torch.device(device)
         self.num_mlps = 2 if self.num_fine_samples > 0 else 1
-        self.P = int(lib.pob_param_count(sh_deg))
+        self.P = int(lib.pob_param_count_pe(sh_deg, posenc_ref(self._posenc_struct)))
         self.params = torch.zeros(self.num_mlps * self.P, dtype=torch.float32, device=self.device)
         nb = int(lib.pob_packed_bytes(sh_deg))
         self.blobs = [torch.zeros(nb, dtype=torch.uint8, device=self.device) for _ in range(self.num_mlps)]
         self.cfg = RenderConfig(sh_deg, self.num_coarse_samples, self.num_fine_samples, int(self.white_bkgd),
                                 self.max_rays, self.sparsity_npoints)
         self.cfg.sigma_activation = self.sigma_act_code
+        self.cfg.posenc = posenc_ref(self._posenc_struct)
         self._ws = {}
         # un-jittered depth table, computed with the reference expression (model_utils.py:125-129)
         t_vals = torch.linspace(0.0, 1.0, self.num_coarse_samples, dtype=torch.float32)
@@ -97,7 +106,7 @@ class NerfModel:
     # ---- parameters --------------------------------------------------------------------------
     def init_params(self, seed=20200823):
         g = torch.Generator().manual_seed(seed)
-        flat = torch.cat([glorot_uniform_flat(self.sh_deg, g) for _ in range(self.num_mlps)])
+        flat = torch.cat([glorot_uniform_flat(self.sh_deg, g, self.posenc) for _ in range(self.num_mlps)])
         self.set_params(flat)
 
     def set_params(self, flat):
@@ -109,8 +118,8 @@ class NerfModel:
 
     def repack(self):
         for i in range(self.num_mlps):
-            check(lib.pob_pack_weights(ptr(self.params[i * self.P:(i + 1) * self.P]), self.sh_deg,
-                                       ptr(self.blobs[i]), stream_ptr()))
+            check(lib.pob_pack_weights_pe(ptr(self.params[i * self.P:(i + 1) * self.P]), self.sh_deg,
+                                          posenc_ref(self._posenc_struct), ptr(self.blobs[i]), stream_ptr()))
 
     def workspace(self, training, precision=PREC_FP16):
         """device scratch of the render call (training False) or of the training step at `precision`"""
@@ -198,7 +207,7 @@ class NerfModel:
     def eval_points_raw(self, points, viewdirs=None, coarse=False, want_rgb=True, precision=None):
         from .. import ops
         return ops.eval_points_raw(self._blob(coarse), self.sh_deg, _cuda_f32(points, "points", 3), want_rgb,
-                                   precision or self.precision)
+                                   precision or self.precision, posenc=self.posenc)
 
     def eval_points(self, points, viewdirs=None, coarse=False, precision=None):
         from .. import ops
@@ -206,7 +215,8 @@ class NerfModel:
             raise AssertionError("viewdirs required when sh_deg >= 0")
         vd = None if viewdirs is None else _cuda_f32(viewdirs, "viewdirs", 3)
         return ops.eval_points(self._blob(coarse), self.sh_deg, _cuda_f32(points, "points", 3), vd,
-                               precision or self.precision, sigma_activation=self.sigma_act_code)
+                               precision or self.precision, sigma_activation=self.sigma_act_code,
+                               posenc=self.posenc)
 
 
 def ctypes_ref(struct):
@@ -224,7 +234,9 @@ def get_model_state(args, device="cuda", seed=20200823, restore=True):
                       white_bkgd=args.white_bkgd, lindisp=getattr(args, "lindisp", False),
                       max_rays=getattr(args, "batch_size", 4096),
                       sparsity_npoints=getattr(args, "sparsity_npoints", 0), device=device,
-                      sigma_activation=getattr(args, "sigma_activation", "relu"))
+                      sigma_activation=getattr(args, "sigma_activation", "relu"),
+                      min_deg_point=getattr(args, "min_deg_point", 0), max_deg_point=getattr(args, "max_deg_point", 10),
+                      legacy_posenc_order=getattr(args, "legacy_posenc_order", False))
     model.init_params(seed)
     state = TrainState(model)
     if restore and getattr(args, "train_dir", None):

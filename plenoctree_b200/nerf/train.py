@@ -3,7 +3,7 @@
     loss_fn + value_and_grad   -> lib.pob_loss_and_grad   (fused wgmma forward / dgrad / wgrad)
     lax.pmean(grad, "batch")   -> two torch.distributed all-reduces on the flat gradient (NCCL): the MLP_0 bucket
                                   on a side stream while the MLP_1 backward still runs, then [MLP_1 | stats]
-    optimizer.apply_gradient   -> lib.pob_adam_update      (flax Adam + operand re-pack)
+    optimizer.apply_gradient   -> lib.pob_adam_update_pe   (flax Adam + operand re-pack)
 GraphedTrainStep captures the whole step (jitter draws, kernels, collectives, Adam) in one CUDA graph.
 
 Data parallel layout = one process per GPU; `batch` holds this rank's shard of the global batch
@@ -216,11 +216,11 @@ def train_step(model, state, batch, lr, sparsity_weight=1e-3, sparsity_length=0.
             allreduce_gradients(state.gbuf)   # pmean(grad) and pmean(stats) in one bucket
     # weight_l2 = sum(theta^2)/numel  ->  d/dtheta = 2*theta/numel  (train.py:101-108,114)
     wd = 2.0 * weight_decay_mult / model.params.numel() if weight_decay_mult else 0.0
-    check(lib.pob_adam_update(model.sh_deg, model.num_mlps, ptr(model.params), ptr(state.grads), ptr(state.m),
-                              ptr(state.v), float(lr), float(state.step),
-                              ptr(state.lr_step) if lr_step_on_device else None, 1.0 / world, wd,
-                              ptr(model.blobs[0]), ptr(model.blobs[1]) if model.num_mlps == 2 else None,
-                              stream_ptr()))
+    check(lib.pob_adam_update_pe(model.sh_deg, model.cfg.posenc, model.num_mlps, ptr(model.params), ptr(state.grads),
+                                 ptr(state.m), ptr(state.v), float(lr), float(state.step),
+                                 ptr(state.lr_step) if lr_step_on_device else None, 1.0 / world, wd,
+                                 ptr(model.blobs[0]), ptr(model.blobs[1]) if model.num_mlps == 2 else None,
+                                 stream_ptr()))
     state.step += 1
     if sync_stats:
         raw = state.stats_raw / world

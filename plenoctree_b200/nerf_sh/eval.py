@@ -22,6 +22,8 @@ def main(unused_argv):
     torch.cuda.set_device(dev)
     dataset = datasets.get_dataset("test", FLAGS, device=dev)
     margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, sigma_activation=FLAGS.sigma_activation,
+                               min_deg_point=FLAGS.min_deg_point, max_deg_point=FLAGS.max_deg_point,
+                               legacy_posenc_order=FLAGS.legacy_posenc_order,
                                num_coarse_samples=FLAGS.num_coarse_samples,
                                num_fine_samples=FLAGS.num_fine_samples, near=FLAGS.near, far=FLAGS.far,
                                white_bkgd=FLAGS.white_bkgd, lindisp=FLAGS.lindisp, batch_size=min(FLAGS.chunk, 8192),

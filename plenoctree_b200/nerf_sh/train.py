@@ -45,6 +45,8 @@ def main(unused_argv):
     h0print("* Load model")
     per_rank = FLAGS.batch_size // world
     margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, sigma_activation=FLAGS.sigma_activation,
+                               min_deg_point=FLAGS.min_deg_point, max_deg_point=FLAGS.max_deg_point,
+                               legacy_posenc_order=FLAGS.legacy_posenc_order,
                                num_coarse_samples=FLAGS.num_coarse_samples,
                                num_fine_samples=FLAGS.num_fine_samples, near=FLAGS.near, far=FLAGS.far,
                                white_bkgd=FLAGS.white_bkgd, lindisp=FLAGS.lindisp,
