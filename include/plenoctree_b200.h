@@ -254,6 +254,21 @@ int pob_loss_and_grad_prec(const pob_render_config* cfg, const pob_train_hparams
                            const float* sp_points_dev, float* grad_flat_dev, float* stats_dev, void* workspace_dev,
                            void* mlp0_done_event, const float* params_dev, int precision, void* stream);
 
+/* flags of pob_loss_and_grad_flags.
+ * POB_TRAIN_DISCARD_SAVED_GRADS: the caller will not read the data-gradient tiles (dZ, dO) the call leaves in the
+ *   workspace, so the weight gradient drops each of them from L2 once it has loaded it, and they are never written
+ *   back to HBM.  After such a call those workspace regions hold undefined bytes; every other region, grad_flat and
+ *   stats are as without the flag.  POB_PREC_FP16X3 accepts the flag and ignores it: its weight-gradient passes run
+ *   after the data gradient and read every dZ tile twice. */
+#define POB_TRAIN_DISCARD_SAVED_GRADS 1
+/* pob_loss_and_grad_prec with `flags` (POB_TRAIN_*; 0 is pob_loss_and_grad_prec).  Unknown bits are refused. */
+int pob_loss_and_grad_flags(const pob_render_config* cfg, const pob_train_hparams* hp, const void* packed_coarse_dev,
+                            const void* packed_fine_dev, const float* origins_dev, const float* directions_dev,
+                            const float* viewdirs_dev, const float* pixels_dev, int n_rays, const float* z_base_dev,
+                            const float* t_rand_dev, const float* u_dev, int u_per_ray, const float* z_fine_dev,
+                            const float* sp_points_dev, float* grad_flat_dev, float* stats_dev, void* workspace_dev,
+                            void* mlp0_done_event, const float* params_dev, int precision, int flags, void* stream);
+
 /* flax.optim.Adam (beta1 .9, beta2 .999, eps 1e-8; nerf_sh/nerf/models.py:44) on the flat buffers of
  * num_mlps MLPs, g = grad*grad_mult + weight_decay_coef*param, then re-packs the operand blobs.
  * `step` = number of updates already applied (flax optimizer.state.step).  lr_step_dev (device float[2] = {lr,

@@ -12,6 +12,8 @@ LIB_PATH = os.environ.get("POB_LIB_PATH") or os.path.join(_HERE, "libplenoctree_
 PREC_FP16 = 1
 PREC_FP16X3 = 3
 
+TRAIN_DISCARD_SAVED_GRADS = 1   # POB_TRAIN_*: flags of pob_loss_and_grad_flags
+
 SIGMA_RELU = 0        # POB_SIGMA_*: density activation of the ray samples and of eval_points
 SIGMA_SOFTPLUS = 1
 
@@ -56,6 +58,8 @@ SIGNATURES = {
     "pob_train_workspace_bytes": (_i64, [_vp, _i]),
     "pob_loss_and_grad_prec": (_i, [_vp, _vp, _vp, _vp, _fp, _fp, _fp, _fp, _i, _fp, _fp, _fp, _i, _fp, _fp, _fp,
                                     _fp, _vp, _vp, _fp, _i, _vp]),
+    "pob_loss_and_grad_flags": (_i, [_vp, _vp, _vp, _vp, _fp, _fp, _fp, _fp, _i, _fp, _fp, _fp, _i, _fp, _fp, _fp,
+                                     _fp, _vp, _vp, _fp, _i, _i, _vp]),
     "pob_adam_update": (_i, [_i, _i, _fp, _fp, _fp, _fp, _c.c_float, _c.c_float, _fp, _c.c_float, _c.c_float,
                              _vp, _vp, _vp]),
     "pob_adam_update_pe": (_i, [_i, _vp, _i, _fp, _fp, _fp, _fp, _c.c_float, _c.c_float, _fp, _c.c_float,

@@ -179,6 +179,35 @@ __device__ __forceinline__ void bulk_s2g(void* dst, uint32_t src_smem, uint32_t 
                "r"(src_smem), "r"(bytes)
                : "memory");
 }
+// L2 cache policies (createpolicy: the whole access gets the priority) and the .L2::cache_hint forms of the bulk copies
+__device__ __forceinline__ uint64_t l2_policy_evict_last() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ void bulk_g2s_hint(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar,
+                                              uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::
+          "r"(dst_smem),
+      "l"(src), "r"(bytes), "r"(bar), "l"(policy)
+      : "memory");
+}
+__device__ __forceinline__ void bulk_s2g_hint(void* dst, uint32_t src_smem, uint32_t bytes, uint64_t policy) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;" ::"l"(dst),
+               "r"(src_smem), "r"(bytes), "l"(policy)
+               : "memory");
+}
+// Drop the 128-byte line at p (128-byte aligned) from L2 without writing it back: a weak write of an undefined value.
+// SASS: CCTL.E.RML2.
+__device__ __forceinline__ void discard_l2_line(const void* p) {
+  asm volatile("discard.global.L2 [%0], 128;" ::"l"(p) : "memory");
+}
 __device__ __forceinline__ void bulk_commit() {
   asm volatile("cp.async.bulk.commit_group;" ::: "memory");
 }

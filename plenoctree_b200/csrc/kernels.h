@@ -181,6 +181,26 @@ __host__ __device__ constexpr WgradRole wgrad_role(int r) {
        : r == 7 ? WgradRole{0,    WG_E, 0,       WG_DZ, 0,      1, 0,                   WG_BIAS_B}   // Dense_0^T
        :          WgradRole{8,    WG_DO, 0,      WG_H, 7,       1, 0,                   WG_BIAS_A};  // heads^T
 }
+// Every tile image mlp_bwd stores (dZ_0..dZ_7, dO) is an operand of exactly one role: the two row halves of a halved
+// role load disjoint chunks of its dZ, a transposed role loads all of it, and the CTAs of a role (half) split the
+// tiles.  So each stored byte is loaded by exactly one CTA, which may then discard it from L2 (WgradParams::discard).
+// A role that read a dZ or dO a second time would read discarded lines: it must not build.
+__host__ __device__ constexpr int wgrad_readers(int op, int layer) {
+  int n = 0;
+  for (int r = 0; r < WG_NUM_ROLES; ++r) {
+    const WgradRole W = wgrad_role(r);
+    n += (W.a_op == op && W.a_layer == layer) + (W.b_op == op && W.b_layer == layer);
+  }
+  return n;
+}
+__host__ __device__ constexpr bool wgrad_reads_saved_grads_once() {
+  for (int l = 0; l < NUM_TRUNK; ++l)
+    if (wgrad_readers(WG_DZ, l) != 1) return false;
+  for (int r = 0; r < WG_NUM_ROLES; ++r)   // a transposed role loads only its first A chunks: all of dO, none of dZ
+    if (wgrad_role(r).halves == 1 && wgrad_role(r).a_op == WG_DZ) return false;
+  return wgrad_readers(WG_DO, 0) == 1;
+}
+static_assert(wgrad_reads_saved_grads_once(), "every dZ_l and dO tile must be loaded by exactly one wgrad role");
 // role holding Dense_`dense`'s gradient (8 and 9: the heads)
 __host__ __device__ constexpr int wgrad_role_of(int dense) { return dense == 0 ? 7 : dense < 8 ? dense - 1 : 8; }
 // transposed role whose A (posenc, or dO with NH <= 64) fits one m64: its warpgroups split each stage's samples
@@ -196,6 +216,7 @@ struct WgradParams {
   int NH;
   float* partials;          // [num_ctas][WG_PARTIAL_FLOATS]
   const uint32_t* progress; // [seg_tiles], advanced by the mlp_bwd launch that writes this segment's dZ / dO
+  int discard;              // 1: drop every dZ / dO line from L2 once loaded (no write-back; the images become undefined)
   short cta_role[WG_MAX_CTAS], cta_index[WG_MAX_CTAS], cta_count[WG_MAX_CTAS];
 };
 // role -> [first CTA, count]; fills the per-CTA tables of `p`; returns number of CTAs to launch

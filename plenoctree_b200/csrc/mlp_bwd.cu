@@ -112,6 +112,9 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
       const uint32_t full = smem_u32(&rows_full[g]), free = smem_u32(&rows_free[g]);
       uint32_t phase = 0;
       long long pending = -1;       // tile of the most recent committed, not yet published store group
+      // fp16: mlp_wgrad reads each stage from L2 shortly after it was stored, while ~4.5 GB of forward-saved h tiles
+      // stream through L2 around it; evict_last keeps the stored lines resident until then (DESIGN.md section 6).
+      const uint64_t keep_l2 = l2_policy_evict_last();
       auto publish = [&]() {        // pending's group has completed: its writes are visible to this thread
         fence_proxy_async_global();
         red_add_release_gpu(p.progress + pending, progress_inc);
@@ -126,8 +129,12 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
           mbar_wait(full, phase);
           for (int c = 0; c < nchunks; ++c) {
             const uint32_t so = c * A_CHUNK_BYTES + rows_off;
-            bulk_s2g(dst_hi + size_t(c) * A_CHUNK_BYTES + rows_off, sbase + SM::A_HI + so, 64u * 128u);
-            if constexpr (NSPLIT == 3) bulk_s2g(dst_lo + size_t(c) * A_CHUNK_BYTES + rows_off, sbase + SM::A_LO + so, 64u * 128u);
+            if constexpr (NSPLIT == 1) {
+              bulk_s2g_hint(dst_hi + size_t(c) * A_CHUNK_BYTES + rows_off, sbase + SM::A_HI + so, 64u * 128u, keep_l2);
+            } else {
+              bulk_s2g(dst_hi + size_t(c) * A_CHUNK_BYTES + rows_off, sbase + SM::A_HI + so, 64u * 128u);
+              bulk_s2g(dst_lo + size_t(c) * A_CHUNK_BYTES + rows_off, sbase + SM::A_LO + so, 64u * 128u);
+            }
           }
           bulk_commit();
           bulk_wait_read_all();

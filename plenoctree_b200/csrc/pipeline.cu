@@ -51,13 +51,16 @@ size_t up(size_t x) { return (x + 1023) / 1024 * 1024; }
 long long tiles_for(long long M) { return padded_rows(M) / TILE_M; }
 
 // SMs (out of an H100 SXM's 132) that run mlp_bwd during the backward; mlp_wgrad runs on the others.  SH16 training
-// step (bench.py's workload, 20 eager steps) on an H100 80 GB HBM3 at a 700 W power limit (1980 MHz maximum SM clock),
-// with dgrad on 56 / 58 / 60 / 62 / 64 / 66 / 68 / 70 / 72 / 74 / 76 / 78 SMs (four runs each for 56-66, two for the
-// rest): 6.48-7.86 / 6.57-6.81 / 6.58-6.69 / 6.77-6.79 / 6.89-6.94 / 6.99-7.91 / 7.87-8.57 / 7.70-7.91 / 7.91-8.02 /
-// 7.88-7.93 / 7.86-7.93 / 8.03-8.20 ms.  From 66 down to 60 the weight gradient gets more CTAs and its tail behind
-// the data gradient shrinks; from 68 up its transposed roles get three CTAs, it falls behind, its dZ reads miss L2
-// and it runs a tail alone; below 58 the data gradient becomes the long pole (DESIGN.md section 6).
-constexpr int DGRAD_SMS_OF_132 = 60;
+// step (bench.py --steps 30 --warmup 5) on an H100 80 GB HBM3 at a 700 W power limit (1980 MHz maximum SM clock), with
+// train_step discarding dZ / dO from L2 (wgrad_body.cuh), dgrad on 52 / 54 / 56 / 58 / 60 SMs, two sessions of two or
+// three runs each: 6.57 / 6.39-6.51 / 6.41-6.54 / 6.45-6.54 / 6.55-6.60 ms.  Without the write-backs the data gradient
+// on 60 SMs ended 0.2 ms before the weight gradient (fine level), so SMs move to the weight gradient until, at 52, the
+// data gradient becomes the long pole.  The split sets how many CTAs sum each layer's partial gradient (optim.cu:
+// wgrad_assign_roles), so changing it changes the gradient's fp32 summation order (DESIGN.md section 6).
+// SH25 (heads width 80: a third heads K-slot in the data gradient, a 128-feature dO for the weight gradient) keeps 60:
+// its tt step (bench_extras tt_sh25) took 7.13 ms at 56 against 6.84 ms for the kernels before the discard at 60.
+constexpr int DGRAD_SMS_OF_132 = 56;
+constexpr int DGRAD_SMS_OF_132_NH80 = 60;
 
 // deterministic carve of the caller-provided workspace (x3: the training workspace of the fp16x3 step)
 Workspace carve(const pob_render_config& c, int training, uint8_t* base, bool x3 = false) {
@@ -291,13 +294,14 @@ int pob_render_rays(const pob_render_config* cfg, const void* packed_coarse_dev,
   return 0;
 }
 
-int pob_loss_and_grad_prec(const pob_render_config* cfg, const pob_train_hparams* hp, const void* packed_coarse_dev,
-                           const void* packed_fine_dev, const float* origins_dev, const float* directions_dev,
-                           const float* viewdirs_dev, const float* pixels_dev, int n_rays, const float* z_base_dev,
-                           const float* t_rand_dev, const float* u_dev, int u_per_ray, const float* z_fine_dev,
-                           const float* sp_points_dev, float* grad_flat_dev, float* stats_dev, void* workspace_dev,
-                           void* mlp0_done_event, const float* params_dev, int precision, void* stream) {
+int pob_loss_and_grad_flags(const pob_render_config* cfg, const pob_train_hparams* hp, const void* packed_coarse_dev,
+                            const void* packed_fine_dev, const float* origins_dev, const float* directions_dev,
+                            const float* viewdirs_dev, const float* pixels_dev, int n_rays, const float* z_base_dev,
+                            const float* t_rand_dev, const float* u_dev, int u_per_ray, const float* z_fine_dev,
+                            const float* sp_points_dev, float* grad_flat_dev, float* stats_dev, void* workspace_dev,
+                            void* mlp0_done_event, const float* params_dev, int precision, int flags, void* stream) {
   const char* where = "pob_loss_and_grad";
+  if (flags & ~POB_TRAIN_DISCARD_SAVED_GRADS) return pob_fail(where, "unknown bits in flags");
   if (int e = check_cfg(where, cfg)) return e;
   if (!hp) return pob_fail(where, "hparams is NULL");
   if (int e = pob_check_common(where, packed_coarse_dev, cfg->sh_deg, precision)) return e;
@@ -360,8 +364,8 @@ int pob_loss_and_grad_prec(const pob_render_config* cfg, const pob_train_hparams
   // was stored (wgrad_body.cuh).  x3: the data gradient runs on all SMs, then the three wgrad passes (kernels.h:
   // X3_WGRAD_PASSES) one after the other, each on all SMs.  SH16 step (bench.py's workload) on an H100 80 GB HBM3 at a
   // 400 W power limit: 29.1-29.6 ms against 31.8-32.1 ms with the fp16 split (pass 0 beside the data gradient).
-  const int dgrad_ctas = sms * DGRAD_SMS_OF_132 / 132;
   const int NH = heads_width(K);
+  const int dgrad_ctas = sms * (NH <= 64 ? DGRAD_SMS_OF_132 : DGRAD_SMS_OF_132_NH80) / 132;
   for (int mlp = 0; mlp < (Nf > 0 ? 2 : 1); ++mlp) {
     Level& L = mlp == 0 ? C : F;
     const long long Mr = (long long)n_rays * (mlp == 0 ? Nc : Nc + Nf);
@@ -401,6 +405,8 @@ int pob_loss_and_grad_prec(const pob_render_config* cfg, const pob_train_hparams
       g.NH = NH;
       g.partials = partials[q];
       g.progress = b.progress;
+      // fp16x3: the passes run after the data gradient and read dZ twice, so the tiles stay
+      g.discard = !x3 && (flags & POB_TRAIN_DISCARD_SAVED_GRADS);
       passes[q].partials = partials[q];
       const int nctas = wgrad_assign_roles(g, (q == 0 && !x3) ? sms - dgrad_ctas : sms, passes[q].role_start,
                                            passes[q].role_count);
@@ -411,6 +417,18 @@ int pob_loss_and_grad_prec(const pob_render_config* cfg, const pob_train_hparams
     if (mlp == 0 && Nf > 0 && mlp0_done_event) POB_CUDA(where, cudaEventRecord((cudaEvent_t)mlp0_done_event, st));
   }
   return 0;
+}
+
+int pob_loss_and_grad_prec(const pob_render_config* cfg, const pob_train_hparams* hp, const void* packed_coarse_dev,
+                           const void* packed_fine_dev, const float* origins_dev, const float* directions_dev,
+                           const float* viewdirs_dev, const float* pixels_dev, int n_rays, const float* z_base_dev,
+                           const float* t_rand_dev, const float* u_dev, int u_per_ray, const float* z_fine_dev,
+                           const float* sp_points_dev, float* grad_flat_dev, float* stats_dev, void* workspace_dev,
+                           void* mlp0_done_event, const float* params_dev, int precision, void* stream) {
+  return pob_loss_and_grad_flags(cfg, hp, packed_coarse_dev, packed_fine_dev, origins_dev, directions_dev,
+                                 viewdirs_dev, pixels_dev, n_rays, z_base_dev, t_rand_dev, u_dev, u_per_ray, z_fine_dev,
+                                 sp_points_dev, grad_flat_dev, stats_dev, workspace_dev, mlp0_done_event, params_dev,
+                                 precision, 0, stream);
 }
 
 int pob_loss_and_grad(const pob_render_config* cfg, const pob_train_hparams* hp, const void* packed_coarse_dev,

@@ -241,6 +241,29 @@ __device__ __forceinline__ void wgrad_body(const WgradParams& p, uint8_t* smem, 
     const int dz_layer = R.a_op == WG_DZ ? R.a_layer : R.b_op == WG_DZ ? R.b_layer : -1;
     const uint32_t want = dz_layer >= 0 ? uint32_t(NUM_TRUNK + 1 - dz_layer) : 1u;
     const int a_chunk0 = R.halves == 2 ? 2 * mh : 0;
+    // p.discard: once a stage has been consumed, its dZ / dO pieces are dropped from L2.  mlp_bwd stored them a few
+    // microseconds earlier and they are still dirty there; nothing reads them again in this launch (kernels.h:
+    // wgrad_reads_saved_grads_once), so writing them back to HBM on eviction would be wasted bandwidth.  Ordering:
+    // the bulk read of load k is complete -> full barrier of its stage -> every consumer warp's MMAs on the stage
+    // have completed and it released the stage -> this warp acquires the stage again (for load k + nst, or after
+    // the last load) -> the 32 lanes discard load k's lines, two per lane per 8 KB piece.
+    const uint8_t* const saved0 = R.a_op == WG_DZ ? sg.dz + size_t(R.a_layer) * A_TILE_BYTES + size_t(a_chunk0) * A_CHUNK_BYTES
+                                  : R.a_op == WG_DO ? sg.d_o
+                                                    : sg.dz + size_t(R.b_layer) * A_TILE_BYTES;   // B = dZ_0
+    const size_t saved_tile = R.a_op == WG_DO ? 2 * A_CHUNK_BYTES : size_t(NUM_TRUNK) * A_TILE_BYTES;
+    const int saved_pieces = R.a_op == WG_E ? 4 : R.a_chunks;
+    const uint32_t lane = lane_id();
+    auto discard_load = [&](long long k) {   // load k = stage `k & 1` of the CTA's item k / 2
+      const uint8_t* const s = saved0 + size_t(sidx + (k >> 1) * scnt) * saved_tile + size_t(k & 1) * WG_PIECE;
+      for (int c = 0; c < saved_pieces; ++c) {
+        discard_l2_line(s + size_t(c) * A_CHUNK_BYTES + lane * 128u);
+        discard_l2_line(s + size_t(c) * A_CHUNK_BYTES + (lane + 32u) * 128u);
+      }
+    };
+    // h tiles come from HBM and are read at most twice (both row halves of a layer), close together: evict_first
+    // keeps them from pushing out the dZ / dO lines that mlp_bwd stores for this launch (DESIGN.md section 6)
+    const uint64_t stream_l2 = l2_policy_evict_first();
+    long long k = 0;   // stage loads issued
     RingPos pos;
     for (long long i = 0; i < n_items; ++i) {
       const long long lt = sidx + i * scnt;
@@ -266,7 +289,7 @@ __device__ __forceinline__ void wgrad_body(const WgradParams& p, uint8_t* smem, 
           for (int c = 0; c < R.a_chunks; ++c)
             bulk_g2s(dst + c * WG_PIECE, a_ptr + size_t(a_chunk0 + c) * A_CHUNK_BYTES + sub * WG_PIECE, WG_PIECE, bar);
           if (R.b_t) {   // T image: two 32-sample groups of all 256 features
-            bulk_g2s(dst + a_bytes, b_ptr + size_t(sub) * WG_B_BYTES, WG_B_BYTES, bar);
+            bulk_g2s_hint(dst + a_bytes, b_ptr + size_t(sub) * WG_B_BYTES, WG_B_BYTES, bar, stream_l2);
           } else {
 #pragma unroll
             for (int c = 0; c < 4; ++c)
@@ -275,9 +298,18 @@ __device__ __forceinline__ void wgrad_body(const WgradParams& p, uint8_t* smem, 
           if (R.skip) bulk_g2s(dst + a_bytes + WG_B_BYTES, e_ptr + sub * WG_PIECE, WG_PIECE, bar);
         }
         __syncwarp();
+        if (p.discard && k >= nst) discard_load(k - nst);   // the stage's previous load
+        ++k;
         pos.advance(nst);
       }
     }
+    // the last nst loads (positions of never-filled stages, j < 0, are free at once)
+    if (p.discard)
+      for (long long j = k - nst; j < k; ++j) {
+        ring.acquire(pos);
+        if (j >= 0) discard_load(j);
+        pos.advance(nst);
+      }
     return;
   }
   setmaxnreg_inc<232>();

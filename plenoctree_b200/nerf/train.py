@@ -1,6 +1,6 @@
 """train_step of the reference (nerf_sh/train.py:51-121) on the CUDA library.
 
-    loss_fn + value_and_grad   -> lib.pob_loss_and_grad   (fused wgmma forward / dgrad / wgrad)
+    loss_fn + value_and_grad   -> lib.pob_loss_and_grad_flags   (fused wgmma forward / dgrad / wgrad)
     lax.pmean(grad, "batch")   -> two torch.distributed all-reduces on the flat gradient (NCCL): the MLP_0 bucket
                                   on a side stream while the MLP_1 backward still runs, then [MLP_1 | stats]
     optimizer.apply_gradient   -> lib.pob_adam_update_pe   (flax Adam + operand re-pack)
@@ -16,7 +16,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from .._lib import PREC_FP16, PREC_FP16X3, TrainHParams, check, lib, ptr, stream_ptr
+from .._lib import PREC_FP16, PREC_FP16X3, TRAIN_DISCARD_SAVED_GRADS, TrainHParams, check, lib, ptr, stream_ptr
 from .models import _cuda_f32, ctypes_ref
 
 # nerf_sh/nerf/utils.py:43-50
@@ -77,10 +77,14 @@ def default_loss_scale(n_rays, precision=PREC_FP16):
 
 def loss_and_grad(model, state, batch, sparsity_weight=1e-3, sparsity_length=0.05, sparsity_radius=1.5,
                   randomized=True, t_rand=None, u=None, sp_points=None, loss_scale=None, z_fine=None,
-                  sigma_noise=None, mlp0_event=None, lr_step_on_device=False, precision=PREC_FP16):
+                  sigma_noise=None, mlp0_event=None, lr_step_on_device=False, precision=PREC_FP16,
+                  keep_saved_tiles=True):
     """value_and_grad(loss_fn) for this rank's shard; fills state.grads / state.stats_raw (device).
     mlp0_event (torch.cuda.Event): recorded on the current stream once the MLP_0 half of the gradient is final.
-    precision: PREC_FP16 (default) or PREC_FP16X3, the error-compensated forward / data / weight gradient."""
+    precision: PREC_FP16 (default) or PREC_FP16X3, the error-compensated forward / data / weight gradient.
+    keep_saved_tiles: False when the caller will not read the data-gradient tiles (dZ, dO) of the workspace
+    (layouts.train_workspace_views): the weight gradient then drops them from L2 instead of letting them be written
+    back to HBM, and those regions are left undefined (POB_TRAIN_DISCARD_SAVED_GRADS)."""
     if precision not in (PREC_FP16, PREC_FP16X3):
         raise ValueError("precision must be PREC_FP16 or PREC_FP16X3")
     rays = batch["rays"]
@@ -111,10 +115,8 @@ def loss_and_grad(model, state, batch, sparsity_weight=1e-3, sparsity_length=0.0
             ptr(px), n, ptr(model.z_base), ptr(t_rand), ptr(u), upr,
             ptr(z_fine), ptr(sp_points) if use_sp else None, ptr(state.grads),
             ptr(state.stats_raw), ptr(ws), mlp0_event.cuda_event if mlp0_event is not None else None)
-    if precision == PREC_FP16:
-        check(lib.pob_loss_and_grad(*args, stream_ptr()))
-    else:
-        check(lib.pob_loss_and_grad_prec(*args, ptr(model.params), int(precision), stream_ptr()))
+    flags = 0 if keep_saved_tiles else TRAIN_DISCARD_SAVED_GRADS
+    check(lib.pob_loss_and_grad_flags(*args, ptr(model.params), int(precision), flags, stream_ptr()))
     return n
 
 
@@ -202,7 +204,7 @@ def train_step(model, state, batch, lr, sparsity_weight=1e-3, sparsity_length=0.
         side, ev_mlp0, ev_b0 = _bucket_plumbing(state)
         n = loss_and_grad(model, state, batch, sparsity_weight, sparsity_length, sparsity_radius, randomized, t_rand,
                           u, sp_points, loss_scale, mlp0_event=ev_mlp0, lr_step_on_device=lr_step_on_device,
-                          precision=precision)
+                          precision=precision, keep_saved_tiles=False)
         side.wait_event(ev_mlp0)
         with torch.cuda.stream(side):
             dist.all_reduce(state.gbuf[:P], op=dist.ReduceOp.SUM)
@@ -211,7 +213,8 @@ def train_step(model, state, batch, lr, sparsity_weight=1e-3, sparsity_length=0.
         torch.cuda.current_stream().wait_event(ev_b0)
     else:
         n = loss_and_grad(model, state, batch, sparsity_weight, sparsity_length, sparsity_radius, randomized, t_rand,
-                          u, sp_points, loss_scale, lr_step_on_device=lr_step_on_device, precision=precision)
+                          u, sp_points, loss_scale, lr_step_on_device=lr_step_on_device, precision=precision,
+                          keep_saved_tiles=False)
         if world > 1:
             allreduce_gradients(state.gbuf)   # pmean(grad) and pmean(stats) in one bucket
     # weight_l2 = sum(theta^2)/numel  ->  d/dtheta = 2*theta/numel  (train.py:101-108,114)

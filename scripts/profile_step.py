@@ -8,6 +8,12 @@ the last mlp_wgrad end falls behind the mlp_bwd end: the SMs that ran mlp_bwd wa
 negative when the weight gradient finishes first).  bench.py's kernel_ms_per_step puts
 events between mlp_bwd and mlp_wgrad, which serialises them; the trace here shows them running together.  Writes
 summary.json (with the card name and power limit) and the Chrome trace under the output directory.
+
+Beside the times it prints the HBM byte model of the step (hbm_bytes: the tile images each kernel class writes and
+reads, from the workspace layout in layouts.py), the achieved GB/s of each kernel class and backward span, and the
+least time each kernel could take from its HBM bytes (at --hbm-gbps, e.g. the copy rate scripts/hbm_probe.py measures
+in the same session; default: the data-sheet 3350 GB/s) and from its algorithmic FLOPs (at --tflops, default the
+data-sheet 989 dense fp16 TFLOP/s): the larger of the two names the bound the kernel is closer to.
 """
 import argparse
 import json
@@ -21,6 +27,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import bench  # noqa: E402  (workload constants)
+from plenoctree_b200 import layouts as L  # noqa: E402
 from plenoctree_b200.nerf import train as T  # noqa: E402
 from plenoctree_b200.nerf.models import NerfModel, Rays  # noqa: E402
 from plenoctree_b200.nerf.utils import random_rays_np  # noqa: E402
@@ -43,11 +50,36 @@ def kernel_class(name):
     return None
 
 
+def hbm_bytes(cfg, n_rays, discard=True):
+    """HBM bytes per training step by kernel class and per level's backward, from the workspace layout.
+    Saving forward: writes h_0..h_7, the posenc tile and the ReLU masks.  Data gradient: reads the masks and writes
+    dZ_0..dZ_7 and dO, unless the weight gradient discards them from L2 (train_step does: nerf/train.py), in which
+    case they never reach HBM.  Weight gradient: reads h_0..h_7 and posenc (once: both row halves of a layer read
+    the same h tile, the second from L2) and dZ / dO from L2 right after they were stored.  Weights, rays and the
+    per-sample arrays (< 1 % of the bytes) are left out.  The write-back of a dirty line happens when L2 evicts it,
+    so the data gradient's write bytes land somewhere in its level's backward span, not necessarily in its kernel."""
+    K = L.K_of(int(cfg.sh_deg))
+    do_bytes = (L.heads_width(K) + 63) // 64 * L.A_CHUNK_BYTES
+    per, levels = {"mlp_fwd (saving)": 0, "mlp_bwd": 0, "mlp_wgrad": 0}, []
+    for v in L.train_workspace_views(cfg, n_rays, True)["levels"]:
+        t = v["tiles"]
+        h_e = t * (L.NUM_TRUNK * L.A_TILE_BYTES + L.E_TILE_BYTES)
+        mask = L.NUM_TRUNK * v["rows"] * 8 * 4
+        dz_do = 0 if discard else t * (L.NUM_TRUNK * L.A_TILE_BYTES + do_bytes)
+        per["mlp_fwd (saving)"] += h_e + mask
+        per["mlp_bwd"] += mask + dz_do
+        per["mlp_wgrad"] += h_e
+        levels.append(mask + dz_do + h_e)
+    return per, levels
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--out", required=True, help="directory for summary.json and the Chrome trace")
+    ap.add_argument("--hbm-gbps", type=float, default=3350.0, help="HBM bandwidth ceiling for the bound")
+    ap.add_argument("--tflops", type=float, default=989.0, help="tensor-core ceiling for the bound")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "profile_step.py needs a GPU"
     dev = torch.device("cuda", 0)
@@ -99,8 +131,21 @@ def main():
     def stats(d):
         return {k: {"min": min(v), "median": float(np.median(v)), "max": max(v)} for k, v in d.items()}
 
+    nbytes, span_bytes = hbm_bytes(model.cfg, bench.RAYS)
+    flops = {"mlp_fwd (saving)": bench.F_FWD, "mlp_bwd": bench.F_DGRAD, "mlp_wgrad": bench.F_WGRAD}
+    rows = sum(v["M"] for v in L.train_workspace_views(model.cfg, bench.RAYS, True)["levels"])
+    hbm = {}
+    for k, b in nbytes.items():
+        ms = per_step.get(k)
+        t_bytes, t_flops = b / (args.hbm_gbps * 1e6), rows * flops[k] / (args.tflops * 1e9)   # ms
+        hbm[k] = {"bytes": b, "gbps": b / (ms * 1e6) if ms else None, "min_ms_bytes": t_bytes,
+                  "min_ms_flops": t_flops, "closer_to": "HBM bytes" if t_bytes > t_flops else "tensor FLOPs"}
+    for i, b in enumerate(span_bytes):
+        med = float(np.median(levels[f"level {i} backward span"]))
+        hbm[f"level {i} backward span"] = {"bytes": b, "gbps": b / (med * 1e6)}
     res = {"card": card(), "steps": K, "kernel_ms_per_step": per_step,
-           "backward_span_ms": stats(levels), "dgrad_idle_ms": stats(idle)}
+           "backward_span_ms": stats(levels), "dgrad_idle_ms": stats(idle),
+           "hbm": hbm, "hbm_gbps_ceiling": args.hbm_gbps, "tflops_ceiling": args.tflops}
     print(json.dumps(res, indent=1))
     with open(os.path.join(args.out, "summary.json"), "w") as f:
         json.dump(res, f, indent=1)
