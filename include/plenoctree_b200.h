@@ -41,12 +41,21 @@ extern "C" {
  * (W <= 63), legacy_order 0 or 1.  Feature order, c = 0..2, j = min_deg..max_deg-1:
  *   legacy_order 0: [x, sin(2^j x_c) at 3 + 3(j - min_deg) + c, sin(2^j x_c + pi/2) at 3 + 3L + 3(j - min_deg) + c]
  *   legacy_order 1: [x, sin(2^j x_c) at 3 + 6(j - min_deg) + c, sin(2^j x_c + pi/2) at 3 + 6(j - min_deg) + 3 + c]
- * with L = max_deg - min_deg.  Every entry point taking a `const pob_posenc*` reads NULL as the reference default
- * {0, 10, 0}, W = 63; the entry points without one use that default. */
+ * with L = max_deg - min_deg.
+ * The descriptor describes the network beyond sh_deg: it also carries the trunk activation net_activation (POB_NET_*,
+ * flag net_activation, nerf_sh/nerf/model_utils.py:69), applied after each of Dense_0..Dense_7.  It changes neither
+ * the parameter layout nor the packed blob.  Every entry point taking a `const pob_posenc*` reads NULL as the
+ * reference default {0, 10, 0, POB_NET_RELU}, W = 63; the entry points without one use that default, and a
+ * zero-filled descriptor is that default too.  Other net_activation values are refused. */
+#define POB_NET_RELU 0
+#define POB_NET_ELU 1      /* z if z > 0 else expm1(z) */
+#define POB_NET_SOFTPLUS 2 /* max(z, 0) + log1p(exp(-|z|)) */
+#define POB_NET_TANH 3     /* tanh(z) */
 typedef struct pob_posenc {
   int min_deg;
   int max_deg;
   int legacy_order;
+  int net_activation;
 } pob_posenc;
 
 /* ---------------------------------------------------------------------------------------------

@@ -17,6 +17,11 @@ TRAIN_DISCARD_SAVED_GRADS = 1   # POB_TRAIN_*: flags of pob_loss_and_grad_flags
 SIGMA_RELU = 0        # POB_SIGMA_*: density activation of the ray samples and of eval_points
 SIGMA_SOFTPLUS = 1
 
+NET_RELU = 0          # POB_NET_*: trunk activation (pob_posenc.net_activation)
+NET_ELU = 1
+NET_SOFTPLUS = 2
+NET_TANH = 3
+
 _c = ctypes
 _vp, _i, _i64, _fp = _c.c_void_p, _c.c_int, _c.c_int64, _c.c_void_p
 
@@ -79,20 +84,27 @@ SIGNATURES = {
 
 
 class Posenc(_c.Structure):
-    """pob_posenc: the point encoder posenc(x, min_deg, max_deg, legacy_order); a NULL pointer is (0, 10, 0)."""
+    """The point-encoder fields of pob_posenc: posenc(x, min_deg, max_deg, legacy_order); a NULL pointer is
+    (0, 10, 0).  The library also reads the trailing net_activation (NetDesc); ctypes keeps a structure of up to
+    16 bytes in a zero-filled inline buffer, so a bare Posenc reads as a relu trunk."""
     _fields_ = [("min_deg", _i), ("max_deg", _i), ("legacy_order", _i)]
+
+
+class NetDesc(Posenc):
+    """the whole pob_posenc: Posenc's fields, then net_activation (NET_*; 0 = relu)."""
+    _fields_ = [("net_activation", _i)]
 
 
 POSENC_DEFAULT = (0, 10, False)   # flags min_deg_point, max_deg_point, legacy_posenc_order of the reference
 
 
-def posenc_struct(posenc):
-    """(min_deg, max_deg, legacy) -> Posenc, or None (NULL) for the default, so that a default model calls the
-    library exactly as before the descriptor existed."""
-    if posenc is None or tuple(posenc) == POSENC_DEFAULT:
+def posenc_struct(posenc, net_activation=NET_RELU):
+    """(min_deg, max_deg, legacy) and a NET_* code -> NetDesc, or None (NULL) for the default encoder with a relu
+    trunk, so that a default model calls the library exactly as before the descriptor existed."""
+    if (posenc is None or tuple(posenc) == POSENC_DEFAULT) and int(net_activation) == NET_RELU:
         return None
-    mn, mx, legacy = posenc
-    return Posenc(int(mn), int(mx), int(bool(legacy)))
+    mn, mx, legacy = POSENC_DEFAULT if posenc is None else posenc
+    return NetDesc(int(mn), int(mx), int(bool(legacy)), int(net_activation))
 
 
 def posenc_ref(struct):

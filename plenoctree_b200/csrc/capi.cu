@@ -114,10 +114,11 @@ int check_common(const char* where, const void* packed, int sh_deg, int precisio
   return 0;
 }
 
-pob::FwdParams base_params(const void* packed, int sh_deg, pob::PosencDesc pe) {
+pob::FwdParams base_params(const void* packed, int sh_deg, pob::NetDesc net) {
   pob::FwdParams p;
   memset(&p, 0, sizeof(p));
-  p.pe = pe;
+  p.pe = net.pe;
+  p.net_act = net.net_act;
   p.sh_deg = sh_deg;
   p.K = K_of(sh_deg);
   p.NH = pob::heads_width(p.K);
@@ -131,17 +132,18 @@ int pob_sm_count_cached() { return sm_count(); }
 int pob_check_common(const char* where, const void* packed, int sh_deg, int precision) {
   return check_common(where, packed, sh_deg, precision);
 }
-pob::FwdParams pob_base_params(const void* packed, int sh_deg, pob::PosencDesc pe) {
-  return base_params(packed, sh_deg, pe);
+pob::FwdParams pob_base_params(const void* packed, int sh_deg, pob::NetDesc net) {
+  return base_params(packed, sh_deg, net);
 }
-int pob_check_posenc(const char* where, const pob_posenc* posenc, pob::PosencDesc& out) {
-  out = pob::POSENC_DEFAULT;
+int pob_check_posenc(const char* where, const pob_posenc* posenc, pob::NetDesc& out) {
+  out = {pob::POSENC_DEFAULT, pob::NET_RELU};
   if (!posenc) return 0;
-  const pob::PosencDesc pe = {posenc->min_deg, posenc->max_deg, posenc->legacy_order};
-  if (!pob::posenc_valid(pe))
+  const pob::NetDesc net = {{posenc->min_deg, posenc->max_deg, posenc->legacy_order}, posenc->net_activation};
+  if (!pob::posenc_valid(net.pe) || !pob::net_act_valid(net.net_act))
     return fail(where, "posenc needs 0 <= min_deg <= max_deg <= 10 (width 3 + 6 (max_deg - min_deg) <= 63, the "
-                       "64-column posenc tile with its constant-one bias column) and legacy_order 0 or 1");
-  out = pe;
+                       "64-column posenc tile with its constant-one bias column), legacy_order 0 or 1 and "
+                       "net_activation one of POB_NET_RELU, POB_NET_ELU, POB_NET_SOFTPLUS, POB_NET_TANH");
+  out = net;
   return 0;
 }
 int pob_check_sigma_activation(const char* where, int sigma_activation) {
@@ -179,9 +181,9 @@ const char* pob_last_error(void) { return g_err.c_str(); }
 int pob_sm_count(void) { return sm_count(); }
 
 int64_t pob_param_count_pe(int sh_deg, const pob_posenc* posenc) {
-  pob::PosencDesc pe;
-  if (!valid_deg(sh_deg) || pob_check_posenc("pob_param_count", posenc, pe)) return -1;
-  return pob::flat_layout(K_of(sh_deg), pob::posenc_width(pe)).total;
+  pob::NetDesc net;
+  if (!valid_deg(sh_deg) || pob_check_posenc("pob_param_count", posenc, net)) return -1;
+  return pob::flat_layout(K_of(sh_deg), pob::posenc_width(net.pe)).total;
 }
 int64_t pob_param_count(int sh_deg) { return pob_param_count_pe(sh_deg, nullptr); }
 int64_t pob_packed_bytes(int sh_deg) {
@@ -191,8 +193,8 @@ int64_t pob_packed_bytes(int sh_deg) {
 
 int pob_pack_weights_pe(const float* flat_dev, int sh_deg, const pob_posenc* posenc, void* packed_dev, void* stream) {
   if (!valid_deg(sh_deg)) return fail("pob_pack_weights", "sh_deg must be in [-1, 4]");
-  pob::PosencDesc pe;
-  if (int e = pob_check_posenc("pob_pack_weights", posenc, pe)) return e;
+  pob::NetDesc net;
+  if (int e = pob_check_posenc("pob_pack_weights", posenc, net)) return e;
   if (!flat_dev || !packed_dev) return fail("pob_pack_weights", "NULL pointer");
   const int K = K_of(sh_deg);
   const BlobLayout b = blob_layout(K);
@@ -200,7 +202,7 @@ int pob_pack_weights_pe(const float* flat_dev, int sh_deg, const pob_posenc* pos
   pob_count_launch();
   PobPhaseTimer _t(POB_PH_OPTIM, (cudaStream_t)stream);
   POB_CUDA("pob_pack_weights",
-           pob::launch_pack_weights(flat_dev, K, pob::posenc_width(pe), p + b.w_hi, p + b.w_lo, p + b.wt_hi,
+           pob::launch_pack_weights(flat_dev, K, pob::posenc_width(net.pe), p + b.w_hi, p + b.w_lo, p + b.wt_hi,
                                     (cudaStream_t)stream));
   return 0;
 }
@@ -211,12 +213,12 @@ int pob_pack_weights(const float* flat_dev, int sh_deg, void* packed_dev, void* 
 int pob_eval_points_raw_pe(const void* packed_dev, int sh_deg, const pob_posenc* posenc, const float* points_dev,
                            int64_t m, float* raw_rgb_dev, float* raw_sigma_dev, int precision, void* stream) {
   if (int e = check_common("pob_eval_points_raw", packed_dev, sh_deg, precision)) return e;
-  pob::PosencDesc pe;
-  if (int e = pob_check_posenc("pob_eval_points_raw", posenc, pe)) return e;
+  pob::NetDesc net;
+  if (int e = pob_check_posenc("pob_eval_points_raw", posenc, net)) return e;
   if (m < 0) return fail("pob_eval_points_raw", "negative point count");
   if (m == 0) return 0;
   if (!points_dev || !raw_sigma_dev) return fail("pob_eval_points_raw", "NULL pointer");
-  pob::FwdParams p = base_params(packed_dev, sh_deg, pe);
+  pob::FwdParams p = base_params(packed_dev, sh_deg, net);
   p.src_mode = pob::SRC_POINTS;
   p.M = m;
   p.points = points_dev;
@@ -240,15 +242,15 @@ int pob_eval_points_pe(const void* packed_dev, int sh_deg, const pob_posenc* pos
                        void* stream) {
   const char* where = "pob_eval_points";
   if (int e = check_common(where, packed_dev, sh_deg, precision)) return e;
-  pob::PosencDesc pe;
-  if (int e = pob_check_posenc(where, posenc, pe)) return e;
+  pob::NetDesc net;
+  if (int e = pob_check_posenc(where, posenc, net)) return e;
   if (int e = pob_check_sigma_activation(where, sigma_activation)) return e;
   if (m < 0) return fail(where, "negative point count");
   if (m == 0) return 0;
   if (!points_dev || !out_rgbs_dev) return fail(where, "NULL pointer");
   if (sh_deg >= 0 && !viewdirs_dev)
     return fail(where, "viewdirs required when sh_deg >= 0 (models.py:199)");
-  pob::FwdParams p = base_params(packed_dev, sh_deg, pe);
+  pob::FwdParams p = base_params(packed_dev, sh_deg, net);
   p.src_mode = pob::SRC_POINTS;
   p.M = m;
   p.points = points_dev;
@@ -279,12 +281,12 @@ int pob_eval_points(const void* packed_dev, int sh_deg, const float* points_dev,
 int pob_eval_cells_mean_pe(const void* packed_dev, int sh_deg, const pob_posenc* posenc, const float* points_dev,
                            int64_t n_cells, int samples_per_cell, float* out_dev, int precision, void* stream) {
   if (int e = check_common("pob_eval_cells_mean", packed_dev, sh_deg, precision)) return e;
-  pob::PosencDesc pe;
-  if (int e = pob_check_posenc("pob_eval_cells_mean", posenc, pe)) return e;
+  pob::NetDesc net;
+  if (int e = pob_check_posenc("pob_eval_cells_mean", posenc, net)) return e;
   if (n_cells < 0 || samples_per_cell <= 0) return fail("pob_eval_cells_mean", "bad sizes");
   if (n_cells == 0) return 0;
   if (!points_dev || !out_dev) return fail("pob_eval_cells_mean", "NULL pointer");
-  pob::FwdParams p = base_params(packed_dev, sh_deg, pe);
+  pob::FwdParams p = base_params(packed_dev, sh_deg, net);
   p.src_mode = pob::SRC_POINTS;
   p.M = n_cells * (int64_t)samples_per_cell;
   p.points = points_dev;
@@ -309,8 +311,8 @@ int pob_eval_grid_pe(const void* packed_dev, int sh_deg, const pob_posenc* posen
                      int nz, const float offset[3], const float scale[3], float* raw_rgb_dev, float* raw_sigma_dev,
                      int precision, void* stream) {
   if (int e = check_common("pob_eval_grid", packed_dev, sh_deg, precision)) return e;
-  pob::PosencDesc pe;
-  if (int e = pob_check_posenc("pob_eval_grid", posenc, pe)) return e;
+  pob::NetDesc net;
+  if (int e = pob_check_posenc("pob_eval_grid", posenc, net)) return e;
   if (reso <= 0 || (reso & (reso - 1)))
     return fail("pob_eval_grid", "reso must be a power of two (extraction.py:246,290)");
   if (x0 < 0 || nx < 0 || ny < 0 || nz < 0 || x0 + nx > reso || ny > reso || nz > reso)
@@ -318,7 +320,7 @@ int pob_eval_grid_pe(const void* packed_dev, int sh_deg, const pob_posenc* posen
   if (!offset || !scale || !raw_sigma_dev) return fail("pob_eval_grid", "NULL pointer");
   const long long m = (long long)nx * ny * nz;
   if (m == 0) return 0;
-  pob::FwdParams p = base_params(packed_dev, sh_deg, pe);
+  pob::FwdParams p = base_params(packed_dev, sh_deg, net);
   p.src_mode = pob::SRC_GRID;
   p.M = m;
   p.g_reso = reso;
@@ -350,8 +352,8 @@ int pob_eval_points_raw_host_pe(const void* packed_dev, int sh_deg, const pob_po
                                 const float* points_host, int64_t m, float* raw_rgb_host, float* raw_sigma_host,
                                 int precision) {
   if (int e = check_common("pob_eval_points_raw_host", packed_dev, sh_deg, precision)) return e;
-  pob::PosencDesc pe;
-  if (int e = pob_check_posenc("pob_eval_points_raw_host", posenc, pe)) return e;
+  pob::NetDesc net;
+  if (int e = pob_check_posenc("pob_eval_points_raw_host", posenc, net)) return e;
   if (m <= 0) return m == 0 ? 0 : fail("pob_eval_points_raw_host", "negative point count");
   if (!points_host || !raw_sigma_host) return fail("pob_eval_points_raw_host", "NULL pointer");
   const int K = K_of(sh_deg);

@@ -10,11 +10,11 @@ int pob_sm_count_cached();
 int pob_check_common(const char* where, const void* packed, int sh_deg, int precision);
 // POB_SIGMA_RELU or POB_SIGMA_SOFTPLUS, else pob_fail
 int pob_check_sigma_activation(const char* where, int sigma_activation);
-// NULL -> the reference default; else the descriptor if 0 <= min_deg <= max_deg <= 10 and legacy_order is 0 / 1,
-// otherwise pob_fail
+// NULL -> the reference default (relu trunk); else the descriptor if 0 <= min_deg <= max_deg <= 10, legacy_order is
+// 0 / 1 and net_activation a POB_NET_* code, otherwise pob_fail
 struct pob_posenc;
-int pob_check_posenc(const char* where, const pob_posenc* posenc, pob::PosencDesc& out);
-pob::FwdParams pob_base_params(const void* packed, int sh_deg, pob::PosencDesc pe);
+int pob_check_posenc(const char* where, const pob_posenc* posenc, pob::NetDesc& out);
+pob::FwdParams pob_base_params(const void* packed, int sh_deg, pob::NetDesc net);
 
 #define POB_CUDA(where, call)                               \
   do {                                                      \

@@ -203,6 +203,10 @@ __device__ __forceinline__ void bulk_s2g_hint(void* dst, uint32_t src_smem, uint
                "r"(src_smem), "r"(bytes), "l"(policy)
                : "memory");
 }
+// Fetch the line holding p into L2 (no register is written; the later load of the line hits L2).  SASS: CCTL.E.PF2.
+__device__ __forceinline__ void prefetch_l2(const void* p) {
+  asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
+}
 // Drop the 128-byte line at p (128-byte aligned) from L2 without writing it back: a weak write of an undefined value.
 // SASS: CCTL.E.RML2.
 __device__ __forceinline__ void discard_l2_line(const void* p) {

@@ -27,6 +27,29 @@ __device__ __forceinline__ float softplus_f32(float x) { return fmaxf(x, 0.f) + 
 // its derivative from its own output: d softplus / dx = sigmoid(x) = 1 - exp(-softplus(x)) = -expm1(-sigma)
 __device__ __forceinline__ float softplus_grad_of_output(float sigma) { return -expm1f(-sigma); }
 
+// Trunk activation (flag net_activation, model_utils.py:69; the values of POB_NET_* in the C ABI), applied after
+// every Dense_0..Dense_7.  Each one is 1-Lipschitz and its derivative is a function of its output h, so the data
+// gradient forms dZ_l = dH_l * f'(h_l) from the h_l tiles the saving forward stores for the weight gradient; only relu
+// needs the mask words.  fp32 forms: expm1f (1 ulp), softplus_f32 (above), tanhf (2 ulp): each within
+// 4 * 2^-24 * |f(z)| of f at the fp32 argument z.
+enum NetAct : int { NET_RELU = 0, NET_ELU = 1, NET_SOFTPLUS = 2, NET_TANH = 3 };
+constexpr int NET_ACT_COUNT = 4;
+template <int ACT>
+__device__ __forceinline__ float net_act_f32(float z) {
+  if constexpr (ACT == NET_ELU) return z > 0.f ? z : expm1f(z);
+  else if constexpr (ACT == NET_SOFTPLUS) return softplus_f32(z);
+  else if constexpr (ACT == NET_TANH) return tanhf(z);
+  else return fmaxf(z, 0.f);
+}
+// f'(z) as a function of h = f(z): elu 1 | h + 1 (= exp(z) for z <= 0), softplus -expm1(-h), tanh (1 - h)(1 + h)
+template <int ACT>
+__device__ __forceinline__ float net_act_grad_of_output(float h) {
+  if constexpr (ACT == NET_ELU) return h > 0.f ? 1.f : h + 1.f;
+  else if constexpr (ACT == NET_SOFTPLUS) return softplus_grad_of_output(h);
+  else if constexpr (ACT == NET_TANH) return (1.f - h) * (1.f + h);
+  else return h > 0.f ? 1.f : 0.f;
+}
+
 // The point encoder posenc(x, min_deg, max_deg, legacy) (model_utils.py:145-173; flags min_deg_point, max_deg_point,
 // legacy_posenc_order).  Its W = 3 + 6 (max_deg - min_deg) features fill posenc tile columns [0, W); columns [W, 63)
 // are 0 and column 63 is the constant 1 that carries the biases.  0 <= min_deg <= max_deg <= POSENC_MAX_DEG keeps
@@ -41,6 +64,12 @@ inline bool posenc_valid(PosencDesc pe) {
   return pe.min_deg >= 0 && pe.min_deg <= pe.max_deg && pe.max_deg <= POSENC_MAX_DEG &&
          (pe.legacy == 0 || pe.legacy == 1);
 }
+// The network beyond sh_deg (the C ABI's pob_posenc): the point encoder and the trunk activation.
+struct NetDesc {
+  PosencDesc pe;
+  int net_act;   // NetAct
+};
+inline bool net_act_valid(int a) { return a >= 0 && a < NET_ACT_COUNT; }
 
 struct FwdParams {
   // ---- sample source ----
@@ -78,10 +107,12 @@ struct FwdParams {
   // ---- training saves (null = off; x3 also needs save_h_lo / save_e_lo) ----
   uint8_t* save_h;             // [ntile][8][64 KB] activation tile images h_0..h_7
   uint8_t* save_e;             // [ntile][16 KB]   posenc tile images
-  uint32_t* save_mask;         // [8][ntile*128][8] relu masks (common.cuh: mask_bit)
+  uint32_t* save_mask;         // [8][ntile*128][8] relu masks (common.cuh: mask_bit); left unwritten by other pe.net_act
   // ---- x3 training saves (NSPLIT = 3): the residual (lo) images beside save_h / save_e ----
   uint8_t* save_h_lo;          // [ntile][8][64 KB]
   uint8_t* save_e_lo;          // [ntile][16 KB]
+  // ---- model, continued ----
+  int net_act;                 // NetAct of Dense_0..Dense_7
 };
 
 // padded heads width for K spherical-harmonic coefficients per channel
@@ -135,7 +166,7 @@ struct BwdParams {
   long long M_rays;         // rows [M_rays, M) are free points (sigma gradient only): no view direction
   MlpPacked w;
   int sh_deg, K, NH;
-  const uint32_t* mask;     // [8][Mpad][8] from mlp_fwd
+  const uint32_t* mask;     // [8][Mpad][8] from mlp_fwd (net_act relu)
   uint8_t* save_dz;         // [ntile][8][64 KB]
   uint8_t* save_do;         // [ntile][32 KB]
   uint32_t* progress;       // [ntile], zeroed: stages of the tile whose stores have completed (wgrad_body.cuh)
@@ -143,6 +174,10 @@ struct BwdParams {
   const uint8_t* wt_lo;     // residual of w.wt_hi (launch_pack_wt_lo)
   uint8_t* save_dz_lo;      // [ntile][8][64 KB]
   uint8_t* save_do_lo;      // [ntile][32 KB]
+  // ---- trunk activation: NET_RELU reads `mask`, the others form f'(h) from `h` (x3: h + h_lo) ----
+  int net_act;              // NetAct
+  const uint8_t* h;         // [ntile][8][64 KB] h_0..h_7 tile images from mlp_fwd (save_h)
+  const uint8_t* h_lo;      // x3: their residual images (save_h_lo)
 };
 // grid = min(tiles, num_ctas) persistent CTAs.  nsplit 3: dZ_l = hi + lo, every product lo*hi + hi*lo + hi*hi
 cudaError_t launch_mlp_bwd(const BwdParams& p, int nsplit, int num_ctas, cudaStream_t stream);

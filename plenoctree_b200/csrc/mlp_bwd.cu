@@ -2,9 +2,10 @@
 // nerf_sh/train.py:116), fused per 128-sample tile like mlp_fwd:
 //
 //   G' (per-sample d pre_rgb[3], d sigma_raw from render.cu)  --SH basis-->  dO [128 x NH]
-//   dH_7 = dO . W_heads ;  dZ_l = dH_l * relu'(h_l) ;  dH_{l-1} = dZ_l . W_l   (l = 7..1)
+//   dH_7 = dO . W_heads ;  dZ_l = dH_l * f'(h_l) ;  dH_{l-1} = dZ_l . W_l   (l = 7..1)
 //
-// ReLU masks come from the forward pass (1 bit per activation), the transposed weights from the
+// f = the trunk activation.  ReLU masks come from the forward pass (1 bit per activation); the other activations form
+// f'(h_l) from the forward's saved h_l tiles (kernels.h: net_act_grad_of_output).  The transposed weights come from the
 // packed `wt_hi` images.  Every dZ_l tile (and dO) is stored to global memory in the same
 // swizzled tile-image format as the forward activations; mlp_wgrad contracts them over samples.
 // No gradient w.r.t. the inputs is needed (layer 0 and the skip slice of layer 5 stop here).
@@ -53,7 +54,11 @@ struct BwdSmem {
 
 }  // namespace
 
-template <int NSPLIT>
+// ACT (= p.net_act): relu masks dH_l with the forward's mask words; the other trunk activations multiply it by
+// f'(h_l) in fp32, formed from the saved h_l tile images (x3: hi + lo).  A thread reads the h_l elements of its own
+// accumulator fragment, the addressing the forward stored them with (t_frag_base); their lines are fetched into L2
+// while the GEMM for dH_l runs, as the mask words are loaded for relu.
+template <int NSPLIT, int ACT>
 __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_constant__ BwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   using SM = BwdSmem<NSPLIT>;
@@ -195,25 +200,63 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
       *reinterpret_cast<uint32_t*>(share_base + off) = afr[8 * c + i];
     }
   };
+  // h_l of this thread's fragment (ACT != relu): element (row fr + 8h, columns 8j + fc, +1) at h_src + t_frag_offset(j, h)
+  size_t h_src = 0;
   auto load_masks = [&](int l, long long it) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const uint4* mp = reinterpret_cast<const uint4*>(p.mask + (size_t(l) * mrows + it * TILE_M + 64 * wg + fr + 8 * h) * 8);
-      const uint4 m0 = __ldg(mp), m1 = __ldg(mp + 1);
-      mw[h][0] = m0.x; mw[h][1] = m0.y; mw[h][2] = m0.z; mw[h][3] = m0.w;
-      mw[h][4] = m1.x; mw[h][5] = m1.y; mw[h][6] = m1.z; mw[h][7] = m1.w;
-    }
-  };
-  // fp16: dZ = dH * relu'(h), fp16 pack of the accumulator, masked.  afr[2j + h] holds 8-column group j of row fr + 8h.
-  auto make_dz = [&]() {
-    acc_to_afrag<false>(acc, afr);
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      const int k = (j & 3) * 4 + (fc >> 1);      // pair index inside the 32-column mask word j / 4
+    if constexpr (ACT == NET_RELU) {
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const uint32_t m = mw[h][j >> 2];
-        afr[2 * j + h] &= ((m >> mask_bit(k, 0)) & 1u ? 0x0000FFFFu : 0u) | ((m >> mask_bit(k, 1)) & 1u ? 0xFFFF0000u : 0u);
+        const uint4* mp = reinterpret_cast<const uint4*>(p.mask + (size_t(l) * mrows + it * TILE_M + 64 * wg + fr + 8 * h) * 8);
+        const uint4 m0 = __ldg(mp), m1 = __ldg(mp + 1);
+        mw[h][0] = m0.x; mw[h][1] = m0.y; mw[h][2] = m0.z; mw[h][3] = m0.w;
+        mw[h][4] = m1.x; mw[h][5] = m1.y; mw[h][6] = m1.z; mw[h][7] = m1.w;
+      }
+    } else {
+      h_src = t_frag_base(it, l, wg, wq, lane);
+      // the warp's share of the tile image: 256 contiguous bytes of each 8-column group (512-byte pitch), one group
+      // per lane
+      const size_t warp_lines = (size_t(it) * NUM_TRUNK + l) * A_TILE_BYTES + uint32_t(2 * wg + (wq >> 1)) * 16384u +
+                                uint32_t(wq & 1) * 256u + lane * 512u;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        prefetch_l2(p.h + warp_lines + 128 * i);
+        if constexpr (NSPLIT == 3) prefetch_l2(p.h_lo + warp_lines + 128 * i);
+      }
+    }
+  };
+  // f'(h) of the fragment pair (row fr + 8h, columns 8j + fc, +1)
+  auto act_grad = [&](int j, int h) {
+    const uint32_t o = t_frag_offset(j, h);
+    float2 hv = unpack_f16x2(__ldg(reinterpret_cast<const uint32_t*>(p.h + h_src + o)));
+    if constexpr (NSPLIT == 3) {
+      const float2 lv = unpack_f16x2(__ldg(reinterpret_cast<const uint32_t*>(p.h_lo + h_src + o)));
+      hv.x += lv.x;
+      hv.y += lv.y;
+    }
+    return make_float2(net_act_grad_of_output<ACT>(hv.x), net_act_grad_of_output<ACT>(hv.y));
+  };
+  // fp16: dZ = dH * f'(h), fp16 pack of the accumulator (relu: masked).  afr[2j + h] holds 8-column group j of row
+  // fr + 8h.
+  auto make_dz = [&]() {
+    if constexpr (ACT == NET_RELU) {
+      acc_to_afrag<false>(acc, afr);
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        const int k = (j & 3) * 4 + (fc >> 1);      // pair index inside the 32-column mask word j / 4
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint32_t m = mw[h][j >> 2];
+          afr[2 * j + h] &= ((m >> mask_bit(k, 0)) & 1u ? 0x0000FFFFu : 0u) | ((m >> mask_bit(k, 1)) & 1u ? 0xFFFF0000u : 0u);
+        }
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float2 g = act_grad(j, h);
+          afr[2 * j + h] = pack_f16x2(acc[4 * j + 2 * h] * g.x, acc[4 * j + 2 * h + 1] * g.y);
+        }
       }
     }
   };
@@ -248,8 +291,8 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
     wgmma_wait<0>();
     ring.release(prev);
   };
-  // x3: dZ = dH * relu'(h) in fp32, split into hi + lo and written to the warpgroup's rows of the A tiles, then
-  // handed to the store warp
+  // x3: dZ = dH * f'(h) in fp32 (relu: masked), split into hi + lo and written to the warpgroup's rows of the A tiles,
+  // then handed to the store warp
   auto store_dz = [&]() {
     rows_acquire();
 #pragma unroll
@@ -257,9 +300,16 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) mlp_bwd_kernel(const __grid_co
       const int k = (j & 3) * 4 + (fc >> 1);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const uint32_t m = mw[h][j >> 2];
-        const float v0 = (m >> mask_bit(k, 0)) & 1u ? acc[4 * j + 2 * h] : 0.f;
-        const float v1 = (m >> mask_bit(k, 1)) & 1u ? acc[4 * j + 2 * h + 1] : 0.f;
+        float v0, v1;
+        if constexpr (ACT == NET_RELU) {
+          const uint32_t m = mw[h][j >> 2];
+          v0 = (m >> mask_bit(k, 0)) & 1u ? acc[4 * j + 2 * h] : 0.f;
+          v1 = (m >> mask_bit(k, 1)) & 1u ? acc[4 * j + 2 * h + 1] : 0.f;
+        } else {
+          const float2 g = act_grad(j, h);
+          v0 = acc[4 * j + 2 * h] * g.x;
+          v1 = acc[4 * j + 2 * h + 1] * g.y;
+        }
         const uint32_t w = pack_f16x2(v0, v1);
         const float2 hv = unpack_f16x2(w);
         const uint32_t off = a_tile_offset(64 * wg + fr + 8 * h, 8 * j + fc);
@@ -404,14 +454,25 @@ cudaError_t launch_mlp_bwd(const BwdParams& p, int nsplit, int num_ctas, cudaStr
   if (p.M <= 0) return cudaSuccess;
   if (nsplit != 1 && nsplit != 3) return cudaErrorInvalidValue;
   if (nsplit == 3 && (!p.wt_lo || !p.save_dz_lo || !p.save_do_lo)) return cudaErrorInvalidValue;
+  if (p.net_act != NET_RELU && (!p.h || (nsplit == 3 && !p.h_lo))) return cudaErrorInvalidValue;
   const long long tiles = padded_rows(p.M) / TILE_M;
   const int grid = int(tiles < num_ctas ? tiles : num_ctas);
-  auto kernel = nsplit == 1 ? mlp_bwd_kernel<1> : mlp_bwd_kernel<3>;
-  const uint32_t smem = nsplit == 1 ? BwdSmem<1>::TOTAL : BwdSmem<3>::TOTAL;
-  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
-  kernel<<<grid, BWD_THREADS, smem, stream>>>(p);
-  return cudaGetLastError();
+  auto launch = [&](auto act) -> cudaError_t {
+    constexpr int A = decltype(act)::value;
+    auto kernel = nsplit == 1 ? mlp_bwd_kernel<1, A> : mlp_bwd_kernel<3, A>;
+    const uint32_t smem = nsplit == 1 ? BwdSmem<1>::TOTAL : BwdSmem<3>::TOTAL;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    kernel<<<grid, BWD_THREADS, smem, stream>>>(p);
+    return cudaGetLastError();
+  };
+  switch (p.net_act) {
+    case NET_RELU: return launch(std::integral_constant<int, NET_RELU>());
+    case NET_ELU: return launch(std::integral_constant<int, NET_ELU>());
+    case NET_SOFTPLUS: return launch(std::integral_constant<int, NET_SOFTPLUS>());
+    case NET_TANH: return launch(std::integral_constant<int, NET_TANH>());
+    default: return cudaErrorInvalidValue;
+  }
 }
 
 }  // namespace pob

@@ -7,9 +7,9 @@
 //   reference path                                      this kernel
 //   -------------------------------------------------   ------------------------------------
 //   model_utils.posenc      (model_utils.py:145-173)    consumer warps -> E tile (smem, fp16)
-//   model_utils.MLP         (model_utils.py:30-94)      wgmma, fp32 accumulators in registers; fp16: ReLU +
-//                                                       pack into the next layer's register A operand
-//                                                       (x3: ReLU epilogue registers -> smem A tiles)
+//   model_utils.MLP         (model_utils.py:30-94)      wgmma, fp32 accumulators in registers; fp16: activation
+//                                                       (relu / elu / softplus / tanh, ACT) + pack into the next
+//                                                       layer's register A operand (x3: epilogue -> smem A tiles)
 //   sh.eval_sh + sigmoid/relu (sh.py:54-109,            heads epilogue (registers -> smem staging); the density
 //     or softplus              models.py:269-281)       activation is p.sigma_act
 //   NerfModel.eval_points_raw (models.py:143-181)       OUT_RAW / OUT_SIGMA
@@ -23,6 +23,8 @@
 // with error-compensated fp16 operands (x = hi + lo; lo*hi + hi*lo + hi*hi per K step), the residual parts in a
 // second set of tiles; a stage then holds the K-slot's hi and lo parts (32 KB).  The x3 training forward (SAVE)
 // stores h_l's hi and lo from the trunk epilogue and the posenc tile's lo behind the posenc barrier.
+#include <type_traits>
+
 #include "common.cuh"
 #include "kernels.h"
 
@@ -164,6 +166,18 @@ __device__ __forceinline__ void posenc_row(uint8_t* e_hi, uint8_t* e_lo, int row
 }
 
 
+// fp16 trunk epilogue: activation of the accumulator in fp32, then the fp16 pack into the next A operand.  Relu is
+// the fused cvt.rn.relu of acc_to_afrag.
+template <int ACT>
+__device__ __forceinline__ void act_to_afrag(const float (&acc)[128], uint32_t (&a)[64]) {
+  if constexpr (ACT == NET_RELU) {
+    acc_to_afrag<true>(acc, a);
+  } else {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) a[i] = pack_f16x2(net_act_f32<ACT>(acc[2 * i]), net_act_f32<ACT>(acc[2 * i + 1]));
+  }
+}
+
 // heads staging row r (0..63) of warpgroup wg: inside the warpgroup's own (dead after the heads MMAs) rows of the
 // activation tile, 16 rows per 8 KB piece
 __device__ __forceinline__ float* stage_row(uint8_t* a_tile, int wg, int r) {
@@ -173,9 +187,12 @@ __device__ __forceinline__ float* stage_row(uint8_t* a_tile, int wg, int r) {
 
 }  // namespace
 
-// OUTM (= p.out_mode) is a template parameter so that each instantiation carries only its own heads epilogue.
-template <int NSPLIT, int OUTM, bool SAVE>
+// OUTM (= p.out_mode) is a template parameter so that each instantiation carries only its own heads epilogue, ACT
+// (= p.net_act) so that each carries only its trunk activation; the relu instantiations are the relu-only kernel's
+// code.  Only relu writes mask words (SAVE): the data gradient of the others reads h_l itself.
+template <int NSPLIT, int OUTM, bool SAVE, int ACT>
 __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_constant__ FwdParams p) {
+  constexpr bool MASKS = SAVE && ACT == NET_RELU;
   extern __shared__ __align__(1024) uint8_t smem[];
   constexpr bool PRECISE = (NSPLIT == 3);
   using SM = Smem<NSPLIT, SAVE>;
@@ -257,10 +274,12 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
       const int h = i & 1;                    // row fr + 8h
       const int hi8 = (i >> 1) & 1;           // second 8 columns of the k16 step
       *reinterpret_cast<uint32_t*>(h_glob + t_frag_offset(4 * c + 2 * (i >> 2) + hi8, h)) = w;
-      const int k = 8 * (i >> 2) + 4 * hi8 + int(lane & 3);   // column pair within the mask word
-      m[h] |= mask_pair_bits(__vminu2(w, 0x00010001u), k);    // non-negative fp16 pair -> 0/1 per half
+      if constexpr (MASKS) {
+        const int k = 8 * (i >> 2) + 4 * hi8 + int(lane & 3);   // column pair within the mask word
+        m[h] |= mask_pair_bits(__vminu2(w, 0x00010001u), k);    // non-negative fp16 pair -> 0/1 per half
+      }
     }
-    mask_quad_reduce(m, c, maskw);
+    if constexpr (MASKS) mask_quad_reduce(m, c, maskw);
   };
 
   // fp16 layer l >= 1 (l = NUM_TRUNK: the heads, into hacc): K-slots 0..7 take h_{l-1} from afr, the bias slot and
@@ -310,7 +329,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
     }
     wgmma_wait<0>();
     ring.release(prev);
-    if (SAVE) store_mask_words(p.save_mask, padded_rows(p.M), l - 1, it * TILE_M + 64 * wg + fr, maskw);
+    if (MASKS) store_mask_words(p.save_mask, padded_rows(p.M), l - 1, it * TILE_M + 64 * wg + fr, maskw);
   };
 
   // heads: accumulator fragment -> per-row fp32 staging (column n = packed heads column) inside the warpgroup's own
@@ -437,11 +456,12 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
       }
       wgmma_wait<0>();
       ring.release(prev);
-      // ReLU + fp16 pack of the accumulator (the bias was accumulated by the tensor cores) into the next A operand
-      acc_to_afrag<true>(acc, afr);
+      // activation + fp16 pack of the accumulator (the bias was accumulated by the tensor cores) into the next A
+      // operand
+      act_to_afrag<ACT>(acc, afr);
       for (int l = 1; l < NUM_TRUNK; ++l) {
         chain_layer(acc, l);
-        acc_to_afrag<true>(acc, afr);
+        act_to_afrag<ACT>(acc, afr);
       }
       chain_layer(hacc, NUM_TRUNK);
       heads_epilogue();
@@ -493,11 +513,11 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
         ring.release(prev);
 
         if (!heads) {
-          // ---- trunk epilogue: ReLU + hi/lo fp16 split straight from the accumulator fragment into the next A
+          // ---- trunk epilogue: activation + hi/lo fp16 split straight from the accumulator fragment into the next A
           // operands (the bias was accumulated by the tensor cores).  Only this warpgroup's MMAs read these rows.
-          // Training (SAVE): the same hi and lo values go to the "T" images of h_l, and the mask words of h_l take
-          // their bits from the sign of the fp32 pre-activation: relu(v) < 2^-25 rounds to hi = lo = 0 but still has
-          // a gradient. ----
+          // Training (SAVE): the same hi and lo values go to the "T" images of h_l, and (relu) the mask words of h_l
+          // take their bits from the sign of the fp32 pre-activation: relu(v) < 2^-25 rounds to hi = lo = 0 but still
+          // has a gradient.  The other activations are applied in fp32 before the split. ----
           size_t t_off = 0;
           uint32_t mrow[2] = {0u, 0u}, maskw[4] = {0u, 0u, 0u, 0u};
           if constexpr (SAVE) t_off = t_frag_base(it, l, wg, wq, lane);
@@ -508,25 +528,28 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
               const int row = 64 * wg + fr + 8 * h;
               const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
               const uint32_t off = a_tile_offset(row, 8 * j + fc);
-              const uint32_t w = pack_f16x2_relu(v0, v1);
+              const float f0 = net_act_f32<ACT>(v0), f1 = net_act_f32<ACT>(v1);
+              const uint32_t w = ACT == NET_RELU ? pack_f16x2_relu(v0, v1) : pack_f16x2(f0, f1);
               *reinterpret_cast<uint32_t*>(a_hi + off) = w;
               const float2 hv = unpack_f16x2(w);
-              const uint32_t wl = pack_f16x2(fmaxf(v0, 0.f) - hv.x, fmaxf(v1, 0.f) - hv.y);
+              const uint32_t wl = pack_f16x2(f0 - hv.x, f1 - hv.y);
               *reinterpret_cast<uint32_t*>(a_lo + off) = wl;
               if constexpr (SAVE) {
                 const size_t go = t_off + t_frag_offset(j, h);
                 *reinterpret_cast<uint32_t*>(p.save_h + go) = w;
                 *reinterpret_cast<uint32_t*>(p.save_h_lo + go) = wl;
+              }
+              if constexpr (MASKS) {
                 const int k = 4 * (j & 3) + (fc >> 1);   // column pair within the mask word
                 mrow[h] |= (v0 > 0.f ? 1u << mask_bit(k, 0) : 0u) | (v1 > 0.f ? 1u << mask_bit(k, 1) : 0u);
               }
             }
-            if (SAVE && (j & 3) == 3) {
+            if (MASKS && (j & 3) == 3) {
               mask_quad_reduce(mrow, j >> 2, maskw);
               mrow[0] = mrow[1] = 0u;
             }
           }
-          if constexpr (SAVE) store_mask_words(p.save_mask, padded_rows(p.M), l, it * TILE_M + 64 * wg + fr, maskw);
+          if constexpr (MASKS) store_mask_words(p.save_mask, padded_rows(p.M), l, it * TILE_M + 64 * wg + fr, maskw);
           fence_proxy_async_smem();
           warpgroup_sync(wg);
           continue;
@@ -556,20 +579,32 @@ cudaError_t launch_mlp_fwd(const FwdParams& p, int nsplit, int num_sms, cudaStre
     kernel<<<grid, FWD_THREADS, SM_TOTAL, stream>>>(p);
     return cudaGetLastError();
   };
-  switch (p.out_mode) {
-    case OUT_RAW:
-      return nsplit == 1 ? launch(mlp_fwd_kernel<1, OUT_RAW, false>) : launch(mlp_fwd_kernel<3, OUT_RAW, false>);
-    case OUT_SIGMA:
-      if (save) return launch(mlp_fwd_kernel<1, OUT_SIGMA, true>);
-      return nsplit == 1 ? launch(mlp_fwd_kernel<1, OUT_SIGMA, false>) : launch(mlp_fwd_kernel<3, OUT_SIGMA, false>);
-    case OUT_RGBS:
-      if (save) return nsplit == 1 ? launch(mlp_fwd_kernel<1, OUT_RGBS, true>) : launch(mlp_fwd_kernel<3, OUT_RGBS, true>);
-      return nsplit == 1 ? launch(mlp_fwd_kernel<1, OUT_RGBS, false>) : launch(mlp_fwd_kernel<3, OUT_RGBS, false>);
-    case OUT_CELL_MEAN:
-      return nsplit == 1 ? launch(mlp_fwd_kernel<1, OUT_CELL_MEAN, false>)
-                         : launch(mlp_fwd_kernel<3, OUT_CELL_MEAN, false>);
-    default:
-      return cudaErrorInvalidValue;
+  auto dispatch = [&](auto act) -> cudaError_t {
+    constexpr int A = decltype(act)::value;
+    switch (p.out_mode) {
+      case OUT_RAW:
+        return nsplit == 1 ? launch(mlp_fwd_kernel<1, OUT_RAW, false, A>) : launch(mlp_fwd_kernel<3, OUT_RAW, false, A>);
+      case OUT_SIGMA:
+        if (save) return launch(mlp_fwd_kernel<1, OUT_SIGMA, true, A>);
+        return nsplit == 1 ? launch(mlp_fwd_kernel<1, OUT_SIGMA, false, A>)
+                           : launch(mlp_fwd_kernel<3, OUT_SIGMA, false, A>);
+      case OUT_RGBS:
+        if (save)
+          return nsplit == 1 ? launch(mlp_fwd_kernel<1, OUT_RGBS, true, A>) : launch(mlp_fwd_kernel<3, OUT_RGBS, true, A>);
+        return nsplit == 1 ? launch(mlp_fwd_kernel<1, OUT_RGBS, false, A>) : launch(mlp_fwd_kernel<3, OUT_RGBS, false, A>);
+      case OUT_CELL_MEAN:
+        return nsplit == 1 ? launch(mlp_fwd_kernel<1, OUT_CELL_MEAN, false, A>)
+                           : launch(mlp_fwd_kernel<3, OUT_CELL_MEAN, false, A>);
+      default:
+        return cudaErrorInvalidValue;
+    }
+  };
+  switch (p.net_act) {
+    case NET_RELU: return dispatch(std::integral_constant<int, NET_RELU>());
+    case NET_ELU: return dispatch(std::integral_constant<int, NET_ELU>());
+    case NET_SOFTPLUS: return dispatch(std::integral_constant<int, NET_SOFTPLUS>());
+    case NET_TANH: return dispatch(std::integral_constant<int, NET_TANH>());
+    default: return cudaErrorInvalidValue;
   }
 }
 

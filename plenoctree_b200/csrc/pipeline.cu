@@ -128,21 +128,21 @@ int check_cfg(const char* where, const pob_render_config* c) {
     return pob_fail(where, "num_coarse_samples + num_fine_samples must be <= 256");
   if (c->max_rays <= 0) return pob_fail(where, "max_rays must be positive");
   if (c->sparsity_npoints < 0) return pob_fail(where, "sparsity_npoints must be >= 0");
-  PosencDesc pe;
-  if (int e = pob_check_posenc(where, c->posenc, pe)) return e;
+  NetDesc net;
+  if (int e = pob_check_posenc(where, c->posenc, net)) return e;
   return pob_check_sigma_activation(where, c->sigma_activation);
 }
 
-// the point encoder of a config that check_cfg accepted
-PosencDesc cfg_posenc(const pob_render_config& c) {
-  PosencDesc pe;
-  pob_check_posenc("", c.posenc, pe);
-  return pe;
+// the point encoder and trunk activation of a config that check_cfg accepted
+NetDesc cfg_net(const pob_render_config& c) {
+  NetDesc net;
+  pob_check_posenc("", c.posenc, net);
+  return net;
 }
 
-FwdParams ray_fwd_params(const void* packed, int sh_deg, PosencDesc pe, const float* o, const float* d,
+FwdParams ray_fwd_params(const void* packed, int sh_deg, NetDesc net, const float* o, const float* d,
                          const float* v, const float* z, int R, int N, float4* out) {
-  FwdParams p = pob_base_params(packed, sh_deg, pe);
+  FwdParams p = pob_base_params(packed, sh_deg, net);
   p.src_mode = SRC_RAYS;
   p.M = (long long)R * N;
   p.M_rays = p.M;
@@ -164,11 +164,11 @@ int forward_levels(const char* where, const pob_render_config& c, Workspace& w, 
                    const float* sp_points = nullptr, long long sp_n = 0) {
   const int sms = pob_sm_count_cached();
   const int Nc = c.num_coarse_samples, Nf = c.num_fine_samples;
-  const PosencDesc pe = cfg_posenc(c);
+  const NetDesc net = cfg_net(c);
   Level& C = w.lv[0];
   { pob_count_launch(1); PobPhaseTimer _t(POB_PH_RENDER, st); POB_CUDA(where, launch_sample_coarse(z_base, t_rand, R, Nc, C.z, st)); }
   {
-    FwdParams p = ray_fwd_params(pk_c, c.sh_deg, pe, o, d, v, C.z, R, Nc, C.rgbs);
+    FwdParams p = ray_fwd_params(pk_c, c.sh_deg, net, o, d, v, C.z, R, Nc, C.rgbs);
     p.sigma_noise = c.sigma_noise_coarse_dev;
     p.sigma_act = c.sigma_activation;
     if (Nf == 0 && sp_n > 0) {     // single-level model: the sparsity points ride on this launch
@@ -192,7 +192,7 @@ int forward_levels(const char* where, const pob_render_config& c, Workspace& w, 
                                       cudaMemcpyDeviceToDevice, st));
     else
       { pob_count_launch(1); PobPhaseTimer _t(POB_PH_RENDER, st); POB_CUDA(where, launch_sample_pdf(C.z, C.weights, u, u_per_ray, R, Nc, Nf, F.z, st)); }
-    FwdParams p = ray_fwd_params(pk_f, c.sh_deg, pe, o, d, v, F.z, R, Nc + Nf, F.rgbs);
+    FwdParams p = ray_fwd_params(pk_f, c.sh_deg, net, o, d, v, F.z, R, Nc + Nf, F.rgbs);
     p.sigma_noise = c.sigma_noise_fine_dev;
     p.sigma_act = c.sigma_activation;
     if (sp_n > 0) {                // the sparsity points ride behind the fine level's ray samples (same MLP)
@@ -320,8 +320,8 @@ int pob_loss_and_grad_flags(const pob_render_config* cfg, const pob_train_hparam
   cudaStream_t st = (cudaStream_t)stream;
   const int sms = pob_sm_count_cached();
   const int K = cfg->sh_deg < 0 ? 1 : (cfg->sh_deg + 1) * (cfg->sh_deg + 1);
-  const PosencDesc pe = cfg_posenc(*cfg);
-  const int W = posenc_width(pe);
+  const NetDesc net = cfg_net(*cfg);
+  const int W = posenc_width(net.pe);
   const int P = flat_layout(K, W).total;
   Workspace w = carve(*cfg, 1, (uint8_t*)workspace_dev, x3);
   if (x3)
@@ -378,12 +378,15 @@ int pob_loss_and_grad_flags(const pob_render_config* cfg, const pob_train_hparam
     b.G = L.G;
     b.viewdirs = viewdirs_dev;
     b.n_per_ray = mlp == 0 ? Nc : Nc + Nf;
-    FwdParams base = pob_base_params(pk, cfg->sh_deg, pe);
+    FwdParams base = pob_base_params(pk, cfg->sh_deg, net);
     b.w = base.w;
     b.sh_deg = cfg->sh_deg;
     b.K = base.K;
     b.NH = base.NH;
+    b.net_act = net.net_act;
     b.mask = L.mask;
+    b.h = L.H;
+    b.h_lo = L.H_lo;
     b.save_dz = L.DZ;
     b.save_do = L.DO;
     b.progress = w.progress + (mlp == 0 ? 0 : C.tiles);
@@ -448,14 +451,14 @@ int pob_adam_update_pe(int sh_deg, const pob_posenc* posenc, int num_mlps, float
                        float weight_decay_coef, void* packed_coarse_dev, void* packed_fine_dev, void* stream) {
   const char* where = "pob_adam_update";
   if (sh_deg < -1 || sh_deg > 4) return pob_fail(where, "sh_deg must be in [-1, 4]");
-  PosencDesc pe;
-  if (int e = pob_check_posenc(where, posenc, pe)) return e;
+  NetDesc net;
+  if (int e = pob_check_posenc(where, posenc, net)) return e;
   if (num_mlps < 1 || num_mlps > 2) return pob_fail(where, "num_mlps must be 1 or 2");
   if (!params_dev || !grads_dev || !m_dev || !v_dev || !packed_coarse_dev || (num_mlps == 2 && !packed_fine_dev))
     return pob_fail(where, "NULL pointer");
   cudaStream_t st = (cudaStream_t)stream;
   const int K = sh_deg < 0 ? 1 : (sh_deg + 1) * (sh_deg + 1);
-  const long long P = flat_layout(K, posenc_width(pe)).total;
+  const long long P = flat_layout(K, posenc_width(net.pe)).total;
   { pob_count_launch(1); PobPhaseTimer _t(POB_PH_OPTIM, st); POB_CUDA(where, launch_adam(params_dev, grads_dev, m_dev, v_dev, P * num_mlps, lr, step, lr_step_dev, 0.9f, 0.999f, 1e-8f,
                               grad_mult, weight_decay_coef, st)); }
   if (int e = pob_pack_weights_pe(params_dev, sh_deg, posenc, packed_coarse_dev, stream)) return e;

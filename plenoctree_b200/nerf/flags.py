@@ -3,7 +3,7 @@ the same names and defaults, and `update_flags` (utils.py:233-244): a YAML file 
 reference's own config files (nerf_sh/config/blender.yaml, tt.yaml) drive this package unchanged.
 
 Flags that select features outside the scope of this path are accepted (so existing command lines keep parsing) and
-rejected by `check_scope` when set to an unsupported value."""
+rejected by `check_model_scope` (every CLI's check) when set to an unsupported value."""
 import os
 
 import yaml
@@ -139,6 +139,27 @@ def sigma_activation_code(name):
     return code
 
 
+# flag net_activation: the trunk activations the kernels build (_lib.NET_*), by their flax (nn.elu) and torch
+# (nn.ELU) names.  Each is 1-Lipschitz with a derivative that is a function of its output, so the training step forms
+# it from the saved activations.  gelu / swish / silu need the pre-activation, which the step does not save.
+NET_ACTIVATIONS = {"relu": 0, "elu": 1, "softplus": 2, "tanh": 3}
+_NET_NEEDS_PREACTIVATION = ("gelu", "swish", "silu")
+
+
+def net_activation_code(name):
+    """flag net_activation -> POB_NET_* code, matched case-insensitively like sigma_activation_code (the octree
+    side's default is torch's "ReLU")."""
+    key = str(name).lower()
+    code = NET_ACTIVATIONS.get(key)
+    if code is not None:
+        return code
+    if key in _NET_NEEDS_PREACTIVATION:
+        raise NotImplementedError(
+            f"net_activation {name!r}: its derivative needs the pre-activation, which the training step does not "
+            "save (the data gradient forms f'(h) from the saved activations h); relu, elu, softplus or tanh expected")
+    raise NotImplementedError(f"net_activation {name!r} is not built: relu, elu, softplus or tanh expected")
+
+
 POSENC_MAX_DEG = 10
 
 
@@ -155,7 +176,8 @@ def check_posenc(min_deg_point, max_deg_point):
 
 
 def check_scope(args):
-    """features of the reference this path does not cover: fail loudly instead of training something else."""
+    """features of the reference the relu-trunk path does not cover: fail loudly instead of training something else.
+    A model with another trunk activation is checked by check_model_scope, which every CLI calls."""
     if args.use_viewdirs:
         raise NotImplementedError("use_viewdirs (vanilla NeRF colour head) is outside the NeRF-SH path")
     if args.sg_dim > 0:
@@ -170,3 +192,21 @@ def check_scope(args):
     sigma_activation_code(args.sigma_activation)
     if (args.render_path or args.spherify) and args.dataset != "llff":
         raise ValueError("render_path / spherify apply to the llff dataset only")        # datasets.py:194-195,496-497
+
+
+class _Trunk:
+    """`args` with its net_activation replaced (absl FlagValues cannot be copied field by field)"""
+
+    def __init__(self, args, net_activation):
+        self._args, self.net_activation = args, net_activation
+
+    def __getattr__(self, name):
+        return getattr(self._args, name)
+
+
+def check_model_scope(args):
+    """check_scope for a model with any trunk activation the kernels build: net_activation relu, elu, softplus or
+    tanh in any case (net_activation_code, which refuses the others and says why), every other flag as check_scope
+    has it."""
+    net_activation_code(args.net_activation)
+    check_scope(_Trunk(args, "relu"))

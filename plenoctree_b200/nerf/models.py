@@ -54,8 +54,8 @@ class NerfModel:
     def __init__(self, sh_deg=3, num_coarse_samples=64, num_fine_samples=128, near=2.0, far=6.0,
                  white_bkgd=True, lindisp=False, max_rays=4096, sparsity_npoints=0, device="cuda",
                  precision=PREC_FP16, noise_std=None, sigma_activation="relu", min_deg_point=0, max_deg_point=10,
-                 legacy_posenc_order=False):
-        from .flags import sigma_activation_code
+                 legacy_posenc_order=False, net_activation="relu"):
+        from .flags import net_activation_code, sigma_activation_code
         if not (-1 <= sh_deg <= 4):
             raise ValueError("sh_deg must be in [-1, 4]")
         # flags min_deg_point / max_deg_point / legacy_posenc_order (nerf_sh/nerf/models.py:121-126): the point
@@ -63,7 +63,11 @@ class NerfModel:
         self.posenc = (int(min_deg_point), int(max_deg_point), bool(legacy_posenc_order))
         if not posenc_valid(self.posenc):
             raise ValueError("posenc degrees must satisfy 0 <= min_deg_point <= max_deg_point <= 10")
-        self._posenc_struct = posenc_struct(self.posenc)   # None (NULL) for the default encoder
+        # flag net_activation (nerf_sh/nerf/models.py:362, model_utils.py:69): the activation after every trunk layer;
+        # it rides in the same descriptor, so the parameters and the packed blob do not depend on it
+        self.net_activation = str(net_activation)
+        self.net_act_code = net_activation_code(net_activation)
+        self._posenc_struct = posenc_struct(self.posenc, self.net_act_code)   # None (NULL): default encoder, relu
         # flag sigma_activation (nerf_sh/nerf/models.py:280-281): relu or softplus of the ray samples' raw sigma and
         # of eval_points; raw sigma (eval_points_raw, extraction) and the sparsity term never take it
         self.sigma_activation = str(sigma_activation)
@@ -207,7 +211,7 @@ class NerfModel:
     def eval_points_raw(self, points, viewdirs=None, coarse=False, want_rgb=True, precision=None):
         from .. import ops
         return ops.eval_points_raw(self._blob(coarse), self.sh_deg, _cuda_f32(points, "points", 3), want_rgb,
-                                   precision or self.precision, posenc=self.posenc)
+                                   precision or self.precision, posenc=self.posenc, net_activation=self.net_act_code)
 
     def eval_points(self, points, viewdirs=None, coarse=False, precision=None):
         from .. import ops
@@ -216,7 +220,7 @@ class NerfModel:
         vd = None if viewdirs is None else _cuda_f32(viewdirs, "viewdirs", 3)
         return ops.eval_points(self._blob(coarse), self.sh_deg, _cuda_f32(points, "points", 3), vd,
                                precision or self.precision, sigma_activation=self.sigma_act_code,
-                               posenc=self.posenc)
+                               posenc=self.posenc, net_activation=self.net_act_code)
 
 
 def ctypes_ref(struct):
@@ -236,7 +240,8 @@ def get_model_state(args, device="cuda", seed=20200823, restore=True):
                       sparsity_npoints=getattr(args, "sparsity_npoints", 0), device=device,
                       sigma_activation=getattr(args, "sigma_activation", "relu"),
                       min_deg_point=getattr(args, "min_deg_point", 0), max_deg_point=getattr(args, "max_deg_point", 10),
-                      legacy_posenc_order=getattr(args, "legacy_posenc_order", False))
+                      legacy_posenc_order=getattr(args, "legacy_posenc_order", False),
+                      net_activation=getattr(args, "net_activation", "relu"))
     model.init_params(seed)
     state = TrainState(model)
     if restore and getattr(args, "train_dir", None):

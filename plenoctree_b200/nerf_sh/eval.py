@@ -17,11 +17,12 @@ F.define_flags()
 def main(unused_argv):
     F.update_flags(FLAGS)
     F.check_flags(FLAGS)
-    F.check_scope(FLAGS)
+    F.check_model_scope(FLAGS)
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
     torch.cuda.set_device(dev)
     dataset = datasets.get_dataset("test", FLAGS, device=dev)
     margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, sigma_activation=FLAGS.sigma_activation,
+                               net_activation=FLAGS.net_activation,
                                min_deg_point=FLAGS.min_deg_point, max_deg_point=FLAGS.max_deg_point,
                                legacy_posenc_order=FLAGS.legacy_posenc_order,
                                num_coarse_samples=FLAGS.num_coarse_samples,

@@ -42,7 +42,7 @@ def orbit_poses(num_views, elevation, radius, up_axis):
 def main(unused_argv):
     F.update_flags(FLAGS)
     F.check_flags(FLAGS, require_data=False)
-    F.check_scope(FLAGS)
+    F.check_model_scope(FLAGS)
     rank, world, dev = _dist.dist_init()
     render_poses = orbit_poses(FLAGS.num_views, FLAGS.elevation, float(FLAGS.radius), FLAGS.up_axis)
     if FLAGS.write_poses and rank == 0:
@@ -53,6 +53,7 @@ def main(unused_argv):
         K = np.loadtxt(FLAGS.intrin)
         focal = (K[0, 0] + K[1, 1]) * 0.5
     margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, sigma_activation=FLAGS.sigma_activation,
+                               net_activation=FLAGS.net_activation,
                                min_deg_point=FLAGS.min_deg_point, max_deg_point=FLAGS.max_deg_point,
                                legacy_posenc_order=FLAGS.legacy_posenc_order,
                                num_coarse_samples=FLAGS.num_coarse_samples,

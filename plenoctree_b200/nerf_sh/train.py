@@ -31,7 +31,7 @@ def main(unused_argv):
     rank, world, dev = _dist_init()
     F.update_flags(FLAGS)
     F.check_flags(FLAGS, world=world)
-    F.check_scope(FLAGS)
+    F.check_model_scope(FLAGS)
     torch.manual_seed(20200823 + rank)
     os.makedirs(FLAGS.train_dir, exist_ok=True)
     render_dir = os.path.join(FLAGS.train_dir, "render")
@@ -45,6 +45,7 @@ def main(unused_argv):
     h0print("* Load model")
     per_rank = FLAGS.batch_size // world
     margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, sigma_activation=FLAGS.sigma_activation,
+                               net_activation=FLAGS.net_activation,
                                min_deg_point=FLAGS.min_deg_point, max_deg_point=FLAGS.max_deg_point,
                                legacy_posenc_order=FLAGS.legacy_posenc_order,
                                num_coarse_samples=FLAGS.num_coarse_samples,

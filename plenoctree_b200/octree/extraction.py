@@ -54,7 +54,8 @@ def _grid_sigmas(nerf, reso, offset, scale):
     rank, world = _rank_world()
     x0, nx = ops.grid_slab(reso, rank, world)
     _, sig = ops.eval_grid(nerf._blob(False), nerf.sh_deg, reso, offset, scale, x0=x0, nx=nx, want_rgb=False,
-                           precision=nerf.precision, device=nerf.device, posenc=nerf.posenc)
+                           precision=nerf.precision, device=nerf.device, posenc=nerf.posenc,
+                           net_activation=nerf.net_act_code)
     if world == 1:
         return sig
     slabs = [ops.grid_slab(reso, r, world) for r in range(world)]
@@ -194,7 +195,8 @@ def step2(args, tree, nerf, cells_per_launch=None):
         points = tree[chunk_inds].sample(S, uniforms=u)
         if not rgba_tree:
             out[i:i + cells_per_launch] = ops.eval_cells_mean(nerf._blob(False), nerf.sh_deg, points.contiguous(), S,
-                                                              precision=nerf.precision, posenc=nerf.posenc)
+                                                              precision=nerf.precision, posenc=nerf.posenc,
+                                                              net_activation=nerf.net_act_code)
         else:
             # RGBA trees (extraction.py:378-390): sigma = mean, rgb = alpha-weighted mean with alpha of a 2/reso step
             rgb, sigma = nerf.eval_points_raw(points.reshape(-1, 3).contiguous())
@@ -289,6 +291,7 @@ def load_nerf(FLAGS, device):
     a flax-format checkpoint_<step> with --is_jaxnerf_ckpt."""
     from ..nerf import checkpoints, models
     margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, sigma_activation=FLAGS.sigma_activation,
+                               net_activation=FLAGS.net_activation,
                                min_deg_point=FLAGS.min_deg_point, max_deg_point=FLAGS.max_deg_point,
                                legacy_posenc_order=FLAGS.legacy_posenc_order,
                                num_coarse_samples=FLAGS.num_coarse_samples,
@@ -308,7 +311,7 @@ def main(unused_argv):
     F = _define_cli_flags()
     FLAGS = F.FLAGS
     F.update_flags(FLAGS)
-    F.check_scope(FLAGS)
+    F.check_model_scope(FLAGS)
     torch.manual_seed(20200823)
     from .._dist import dist_finish, dist_init
     rank, _, dev = dist_init()       # under torchrun: NCCL group, this rank's GPU (x-slabs / leaf blocks / cameras)
