@@ -148,7 +148,9 @@ int pob_eval_points_raw_host_pe(const void* packed_dev, int sh_deg, const pob_po
                                 int precision);
 
 /* ---------------------------------------------------------------------------------------------
- * Per-ray stages (exposed individually for parity tests; pob_render_rays chains them).
+ * Per-ray stages (exposed individually for parity tests; pob_render_rays chains them).  They take up to
+ * 1024 samples per ray: n_samples <= 1024, n_coarse >= 3 and n_coarse + n_fine <= 1024, the bound
+ * pob_render_config's num_coarse_samples / num_fine_samples are checked against.
  * ------------------------------------------------------------------------------------------- */
 /* model_utils.sample_along_rays (nerf_sh/nerf/model_utils.py:104-142).  z_base[n_samples] is the
  * un-jittered table near*(1-t)+far*t (or the lindisp form) built by the host with the reference

@@ -418,7 +418,8 @@ int pob_composite(const float* rgbs_dev, const float* z_dev, const float* dirs_d
                   int white_bkgd, float* out_rgb_dev, float* out_disp_dev, float* out_acc_dev,
                   float* out_weights_dev, void* stream) {
   if (!rgbs_dev || !z_dev || !dirs_dev || !out_rgb_dev) return fail("pob_composite", "NULL pointer");
-  if (n_rays < 0 || n_samples < 1 || n_samples > 256) return fail("pob_composite", "n_samples must be in [1,256]");
+  if (n_rays < 0 || n_samples < 1 || n_samples > pob::MAX_RAY_SAMPLES)
+    return fail("pob_composite", "n_samples must be in [1,1024]");
   pob_count_launch();
   POB_CUDA("pob_composite",
            pob::launch_composite_fwd(reinterpret_cast<const float4*>(rgbs_dev), z_dev, dirs_dev, n_rays, n_samples,
@@ -432,7 +433,8 @@ int pob_composite_bwd(const float* rgbs_dev, const float* z_dev, const float* di
                       float* g_out_dev, float* sq_err_sum_dev, void* stream) {
   if (!rgbs_dev || !z_dev || !dirs_dev || !comp_rgb_dev || !pixels_dev || !g_out_dev)
     return fail("pob_composite_bwd", "NULL pointer");
-  if (n_rays < 0 || n_samples < 1 || n_samples > 256) return fail("pob_composite_bwd", "n_samples must be in [1,256]");
+  if (n_rays < 0 || n_samples < 1 || n_samples > pob::MAX_RAY_SAMPLES)
+    return fail("pob_composite_bwd", "n_samples must be in [1,1024]");
   pob_count_launch();
   POB_CUDA("pob_composite_bwd",
            pob::launch_composite_bwd(reinterpret_cast<const float4*>(rgbs_dev), z_dev, dirs_dev, comp_rgb_dev,
@@ -444,8 +446,8 @@ int pob_composite_bwd(const float* rgbs_dev, const float* z_dev, const float* di
 int pob_sample_pdf(const float* z_coarse_dev, const float* weights_dev, const float* u_dev, int u_per_ray,
                    int n_rays, int n_coarse, int n_fine, float* z_out_dev, void* stream) {
   if (!z_coarse_dev || !weights_dev || !u_dev || !z_out_dev) return fail("pob_sample_pdf", "NULL pointer");
-  if (n_coarse < 3 || n_fine < 1 || n_coarse + n_fine > 256)
-    return fail("pob_sample_pdf", "need n_coarse >= 3 and n_coarse + n_fine <= 256");
+  if (n_coarse < 3 || n_fine < 1 || n_coarse + n_fine > pob::MAX_RAY_SAMPLES)
+    return fail("pob_sample_pdf", "need n_coarse >= 3 and n_coarse + n_fine <= 1024");
   pob_count_launch();
   POB_CUDA("pob_sample_pdf", pob::launch_sample_pdf(z_coarse_dev, weights_dev, u_dev, u_per_ray, n_rays, n_coarse,
                                                     n_fine, z_out_dev, (cudaStream_t)stream));

@@ -20,6 +20,9 @@ enum OutMode : int { OUT_RAW = 0, OUT_SIGMA = 1, OUT_RGBS = 2, OUT_CELL_MEAN = 3
 // density activation of OUT_RGBS (the values of POB_SIGMA_* in the C ABI)
 enum SigmaAct : int { SIGMA_RELU = 0, SIGMA_SOFTPLUS = 1 };
 
+// samples per ray the per-ray stages (render.cu) take: 3 <= Nc and Nc + Nf <= MAX_RAY_SAMPLES
+constexpr int MAX_RAY_SAMPLES = 1024;
+
 // softplus in fp32, stable for every x: max(x, 0) + log1p(exp(-|x|)).  expf (2 ulp) and log1pf (1 ulp) and the
 // final add keep it within 4 * 2^-24 * softplus(x) of the exact value of the fp32 argument, down to where expf's
 // output turns denormal (x < -87); DESIGN.md section 3 gives the measured figure.

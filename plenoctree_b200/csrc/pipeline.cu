@@ -122,10 +122,10 @@ Workspace carve(const pob_render_config& c, int training, uint8_t* base, bool x3
 int check_cfg(const char* where, const pob_render_config* c) {
   if (!c) return pob_fail(where, "config is NULL");
   if (c->sh_deg < -1 || c->sh_deg > 4) return pob_fail(where, "sh_deg must be in [-1, 4]");
-  if (c->num_coarse_samples < 3 || c->num_coarse_samples > 256)
-    return pob_fail(where, "num_coarse_samples must be in [3, 256]");
-  if (c->num_fine_samples < 0 || c->num_coarse_samples + c->num_fine_samples > 256)
-    return pob_fail(where, "num_coarse_samples + num_fine_samples must be <= 256");
+  if (c->num_coarse_samples < 3 || c->num_coarse_samples > MAX_RAY_SAMPLES)
+    return pob_fail(where, "num_coarse_samples must be in [3, 1024]");
+  if (c->num_fine_samples < 0 || c->num_coarse_samples + c->num_fine_samples > MAX_RAY_SAMPLES)
+    return pob_fail(where, "num_coarse_samples + num_fine_samples must be <= 1024");
   if (c->max_rays <= 0) return pob_fail(where, "max_rays must be positive");
   if (c->sparsity_npoints < 0) return pob_fail(where, "sparsity_npoints must be >= 0");
   NetDesc net;

@@ -1,6 +1,9 @@
 // render.cu — per-ray stages of NerfModel.__call__ that are not GEMMs: stratified sampling,
 // volumetric alpha-compositing (forward and backward), inverse-CDF hierarchical resampling with the
-// union sort, MSE loss gradient.  One warp per ray, all fp32, warp-shuffle scans / reductions.
+// union sort, MSE loss gradient.  All fp32.  A ray is a group of W warps at up to MAX_SEG samples per lane: W = 1
+// (four rays per 128-thread block, warp-shuffle scans / reductions) for N <= 256, and W = 4 (one ray per block) for
+// 256 < N <= MAX_RAY_SAMPLES, where each scan and reduction adds one cross-warp step through shared memory.  The
+// W = 1 instantiations compile to the kernels as they were before W existed.
 //
 //   sample_along_rays       nerf_sh/nerf/model_utils.py:104-142
 //   volumetric_rendering    nerf_sh/nerf/model_utils.py:176-222
@@ -15,8 +18,22 @@ namespace pob {
 namespace {
 
 constexpr int RAYS_PER_BLOCK = 4;
-constexpr int MAX_SEG = 8;  // samples per lane  (N <= 256)
+constexpr int MAX_SEG = 8;  // samples per lane
+constexpr int WIDE = 4;     // warps per ray for N > 32 * MAX_SEG
+static_assert(32 * MAX_SEG * WIDE == MAX_RAY_SAMPLES && WIDE == RAYS_PER_BLOCK, "a wide ray fills one block");
 constexpr unsigned FULL = 0xffffffffu;
+
+// the ray of this thread and its index among the ray's 32 * W threads
+template <int W>
+__device__ __forceinline__ long long ray_of_thread() {
+  return blockIdx.x * (long long)(RAYS_PER_BLOCK / W) + (threadIdx.x >> 5) / W;
+}
+template <int W>
+__device__ __forceinline__ int ray_thread() { return threadIdx.x & (32 * W - 1); }
+template <int W>
+__device__ __forceinline__ void ray_sync() {
+  if constexpr (W == 1) __syncwarp(); else __syncthreads();
+}
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -57,6 +74,43 @@ __device__ __forceinline__ float warp_excl_suffix_sum(float v, int lane) {
   return lane == 31 ? 0.f : ex;
 }
 
+// Cross-warp steps of a W-warp ray (W > 1: one ray per block, warp wid of W).  Each warp's total is the combination
+// of its last (prefix) or first (suffix) lane's exclusive scan with that lane's own value.  Every helper owns its
+// shared array, so a kernel calls each of them at most once.
+// exclusive product over the warps in front of mine, in warp order
+template <int W>
+__device__ __forceinline__ float warps_front_prod(float warp_total, int lane, int wid) {
+  __shared__ float s_tot[W];
+  if (lane == 0) s_tot[wid] = warp_total;
+  __syncthreads();
+  float p = 1.f;
+  for (int k = 0; k < wid; ++k) p *= s_tot[k];
+  return p;
+}
+// exclusive sum over the warps in front of mine (front = true, in warp order) or behind it (from the last warp back)
+template <int W>
+__device__ __forceinline__ float warps_excl_sum(float warp_total, int lane, int wid, bool front) {
+  __shared__ float s_tot[W];
+  if (lane == 0) s_tot[wid] = warp_total;
+  __syncthreads();
+  float s = 0.f;
+  if (front)
+    for (int k = 0; k < wid; ++k) s += s_tot[k];
+  else
+    for (int k = W - 1; k > wid; --k) s += s_tot[k];
+  return s;
+}
+// sum over all W warps, in warp order, in every thread
+template <int W>
+__device__ __forceinline__ float warps_sum(float warp_total, int lane, int wid) {
+  __shared__ float s_tot[W];
+  if (lane == 0) s_tot[wid] = warp_total;
+  __syncthreads();
+  float s = s_tot[0];
+  for (int k = 1; k < W; ++k) s += s_tot[k];
+  return s;
+}
+
 // ---------------------------------------------------------------------------------------------
 // Stratified sampling.  z_base[N] = near*(1-t)+far*t (or the lindisp form) is tabulated by the host
 // with the reference's own expression so that no linspace rounding ambiguity enters.
@@ -87,16 +141,17 @@ struct RaySeg {
   float T0;            // transmittance in front of my first sample
 };
 
-template <int S>
+template <int S, int W>
 __device__ __forceinline__ void load_ray(const float4* __restrict__ rgbs, const float* __restrict__ z,
                                          const float* __restrict__ dirs, long long ray, int N, int lane,
                                          RaySeg& r) {
+  const int seg = ray_thread<W>();
   const float dx = dirs[3 * ray], dy = dirs[3 * ray + 1], dz = dirs[3 * ray + 2];
   const float dnorm = sqrtf(dx * dx + dy * dy + dz * dz);
   float prod = 1.f;
 #pragma unroll
   for (int i = 0; i < S; ++i) {
-    const int idx = lane * S + i;
+    const int idx = seg * S + i;
     if (idx < N) {
       r.c[i] = rgbs[ray * N + idx];
       r.z[i] = z[ray * N + idx];
@@ -118,6 +173,7 @@ __device__ __forceinline__ void load_ray(const float4* __restrict__ rgbs, const 
     }
   }
   r.T0 = warp_excl_prod(prod, lane);
+  if constexpr (W > 1) r.T0 *= warps_front_prod<W>(__shfl_sync(FULL, r.T0 * prod, 31), lane, threadIdx.x >> 5);
 }
 
 struct CompositeArgs {
@@ -128,18 +184,18 @@ struct CompositeArgs {
   float *out_rgb, *out_disp, *out_acc, *out_weights;
 };
 
-template <int S>
+template <int S, int W>
 __global__ void __launch_bounds__(RAYS_PER_BLOCK * 32)
 composite_fwd_kernel(const CompositeArgs a) {
-  const int lane = threadIdx.x & 31;
-  const long long ray = blockIdx.x * (long long)RAYS_PER_BLOCK + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31, seg = ray_thread<W>();
+  const long long ray = ray_of_thread<W>();
   if (ray >= a.R) return;
   RaySeg r;
-  load_ray<S>(a.rgbs, a.z, a.dirs, ray, a.N, lane, r);
+  load_ray<S, W>(a.rgbs, a.z, a.dirs, ray, a.N, lane, r);
   float T = r.T0, cr = 0.f, cg = 0.f, cb = 0.f, depth = 0.f, acc = 0.f;
 #pragma unroll
   for (int i = 0; i < S; ++i) {
-    const int idx = lane * S + i;
+    const int idx = seg * S + i;
     const float w = r.alpha[i] * T;
     if (idx < a.N) {
       cr += w * r.c[i].x;
@@ -156,7 +212,27 @@ composite_fwd_kernel(const CompositeArgs a) {
   cb = warp_sum(cb);
   depth = warp_sum(depth);
   acc = warp_sum(acc);
-  if (lane == 0) {
+  if constexpr (W > 1) {   // the five sums over the W warps, in warp order
+    __shared__ float s_part[5][W];
+    const int wid = threadIdx.x >> 5;
+    if (lane == 0) {
+      s_part[0][wid] = cr;
+      s_part[1][wid] = cg;
+      s_part[2][wid] = cb;
+      s_part[3][wid] = depth;
+      s_part[4][wid] = acc;
+    }
+    __syncthreads();
+    cr = s_part[0][0], cg = s_part[1][0], cb = s_part[2][0], depth = s_part[3][0], acc = s_part[4][0];
+    for (int k = 1; k < W; ++k) {
+      cr += s_part[0][k];
+      cg += s_part[1][k];
+      cb += s_part[2][k];
+      depth += s_part[3][k];
+      acc += s_part[4][k];
+    }
+  }
+  if (seg == 0) {
     const float inv_eps = 1e10f;
     float disp = acc / depth;
     disp = (disp > 0.f && disp < inv_eps && acc > 1e-10f) ? disp : inv_eps;
@@ -192,14 +268,14 @@ struct CompositeBwdArgs {
   float* sq_err_sum;       // += sum_{rays,ch} (C - px)^2   (loss numerator)
 };
 
-template <int S>
+template <int S, int W>
 __global__ void __launch_bounds__(RAYS_PER_BLOCK * 32)
 composite_bwd_kernel(const CompositeBwdArgs a) {
-  const int lane = threadIdx.x & 31;
-  const long long ray = blockIdx.x * (long long)RAYS_PER_BLOCK + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31, seg = ray_thread<W>();
+  const long long ray = ray_of_thread<W>();
   if (ray >= a.R) return;
   RaySeg r;
-  load_ray<S>(a.rgbs, a.z, a.dirs, ray, a.N, lane, r);
+  load_ray<S, W>(a.rgbs, a.z, a.dirs, ray, a.N, lane, r);
   const float ex = a.comp_rgb[3 * ray] - a.pixels[3 * ray];
   const float ey = a.comp_rgb[3 * ray + 1] - a.pixels[3 * ray + 1];
   const float ez = a.comp_rgb[3 * ray + 2] - a.pixels[3 * ray + 2];
@@ -218,9 +294,11 @@ composite_bwd_kernel(const CompositeBwdArgs a) {
     T *= r.om[i];
   }
   float suffix = warp_excl_suffix_sum(local, lane);  // sum over lanes > me
+  if constexpr (W > 1)                                // + sum over the warps behind mine
+    suffix += warps_excl_sum<W>(__shfl_sync(FULL, suffix + local, 0), lane, threadIdx.x >> 5, false);
 #pragma unroll
   for (int i = S - 1; i >= 0; --i) {
-    const int idx = lane * S + i;
+    const int idx = seg * S + i;
     if (idx < a.N) {
       // dL/dalpha_i = g_i T_i - (sum_{k>i} g_k w_k) / (1 - alpha_i + eps)
       const float dalpha = gi[i] * Tpre[i] - suffix / r.om[i];
@@ -238,7 +316,7 @@ composite_bwd_kernel(const CompositeBwdArgs a) {
     }
     suffix += gi[i] * w[i];
   }
-  if (lane == 0 && a.sq_err_sum) atomicAdd(a.sq_err_sum, ex * ex + ey * ey + ez * ez);
+  if (seg == 0 && a.sq_err_sum) atomicAdd(a.sq_err_sum, ex * ex + ey * ey + ez * ez);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -254,33 +332,40 @@ struct PdfArgs {
   float* z_out;           // [R, Nc+Nf]
 };
 
+// W = 1: one warp per ray, a 256-key union sort.  W = WIDE: one block per ray, bins / cdf / union buffer of 1024
+// floats each, a block scan for the cdf and a 1024-key sort under __syncthreads.
+template <int W>
 __global__ void __launch_bounds__(RAYS_PER_BLOCK * 32) sample_pdf_kernel(const PdfArgs a) {
-  __shared__ float s_bins[RAYS_PER_BLOCK][256];
-  __shared__ float s_cdf[RAYS_PER_BLOCK][256];
-  __shared__ float s_sort[RAYS_PER_BLOCK][256];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const long long ray = blockIdx.x * (long long)RAYS_PER_BLOCK + wid;
+  constexpr int RB = RAYS_PER_BLOCK / W;   // rays per block
+  constexpr int NK = 256 * W;              // sort keys per ray (a power of two >= Nc + Nf)
+  constexpr int NT = 32 * W;               // threads per ray
+  __shared__ float s_bins[RB][NK];
+  __shared__ float s_cdf[RB][NK];
+  __shared__ float s_sort[RB][NK];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, seg = ray_thread<W>();
+  const long long ray = ray_of_thread<W>();
   if (ray >= a.R) return;
   const int Nc = a.Nc, Nf = a.Nf;
   const int nb = Nc - 1;   // bins (mid points): 63
   const int nw = Nc - 2;   // interior weights:   62
-  float* bins = s_bins[wid];
-  float* cdf = s_cdf[wid];
-  float* sb = s_sort[wid];
+  float* bins = s_bins[wid / W];
+  float* cdf = s_cdf[wid / W];
+  float* sb = s_sort[wid / W];
   const float* zc = a.z_c + ray * Nc;
   const float* wt = a.weights + ray * Nc;
-  for (int i = lane; i < nb; i += 32) bins[i] = __fmul_rn(0.5f, __fadd_rn(zc[i + 1], zc[i]));
+  for (int i = seg; i < nb; i += NT) bins[i] = __fmul_rn(0.5f, __fadd_rn(zc[i + 1], zc[i]));
   // weights[..., 1:-1], padded so that the sum is at least eps
-  const int S = (nw + 31) / 32;
+  const int S = (nw + NT - 1) / NT;
   float wl[MAX_SEG];
   float lsum = 0.f;
 #pragma unroll
   for (int i = 0; i < MAX_SEG; ++i) {
-    const int idx = lane * S + i;
+    const int idx = seg * S + i;
     wl[i] = (i < S && idx < nw) ? wt[idx + 1] : 0.f;
     lsum += wl[i];
   }
   float wsum = warp_sum(lsum);
+  if constexpr (W > 1) wsum = warps_sum<W>(wsum, lane, wid);
   const float padding = fmaxf(0.f, 1e-5f - wsum);
   const float padw = padding / float(nw);
   wsum += padding;
@@ -288,7 +373,7 @@ __global__ void __launch_bounds__(RAYS_PER_BLOCK * 32) sample_pdf_kernel(const P
   float run = 0.f;
 #pragma unroll
   for (int i = 0; i < MAX_SEG; ++i) {
-    const int idx = lane * S + i;
+    const int idx = seg * S + i;
     if (i < S && idx < nw) {
       wl[i] = (wl[i] + padw) / wsum;
       run += wl[i];
@@ -297,22 +382,23 @@ __global__ void __launch_bounds__(RAYS_PER_BLOCK * 32) sample_pdf_kernel(const P
     }
   }
   float pre = warp_excl_sum(run, lane);
+  if constexpr (W > 1) pre += warps_excl_sum<W>(__shfl_sync(FULL, pre + run, 31), lane, wid, true);
 #pragma unroll
   for (int i = 0; i < MAX_SEG; ++i) {
-    const int idx = lane * S + i;
+    const int idx = seg * S + i;
     if (i < S && idx < nw) {
       pre += wl[i];
       if (idx < nw - 1) cdf[idx + 1] = fminf(1.f, pre);
     }
   }
-  if (lane == 0) {
+  if (seg == 0) {
     cdf[0] = 0.f;
     cdf[nb - 1] = 1.f;
   }
-  __syncwarp();
+  ray_sync<W>();
   // union buffer: coarse depths first
-  for (int i = lane; i < Nc; i += 32) sb[i] = zc[i];
-  for (int j = lane; j < Nf; j += 32) {
+  for (int i = seg; i < Nc; i += NT) sb[i] = zc[i];
+  for (int j = seg; j < Nf; j += NT) {
     const float u = a.u_per_ray ? a.u[ray * Nf + j] : a.u[j];
     // count of cdf entries <= u (cdf is non-decreasing): upper bound
     int lo = 0, hi = nb;
@@ -329,15 +415,15 @@ __global__ void __launch_bounds__(RAYS_PER_BLOCK * 32) sample_pdf_kernel(const P
     const float b0 = bins[i0], b1 = bins[i1];
     sb[Nc + j] = __fadd_rn(b0, __fmul_rn(t, __fsub_rn(b1, b0)));
   }
-  for (int i = Nc + Nf + lane; i < 256; i += 32) sb[i] = __int_as_float(0x7f800000);
-  __syncwarp();
-  // bitonic sort of 256 keys, 4 compare-exchanges per lane per pass
-  for (int k = 2; k <= 256; k <<= 1) {
+  for (int i = Nc + Nf + seg; i < NK; i += NT) sb[i] = __int_as_float(0x7f800000);
+  ray_sync<W>();
+  // bitonic sort of NK keys, 4 compare-exchanges per thread per pass
+  for (int k = 2; k <= NK; k <<= 1) {
     for (int j = k >> 1; j > 0; j >>= 1) {
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
-        const int t = lane + 32 * q;                // 0..127: index of the compare-exchange
-        const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1));
+        const int c = seg + NT * q;                // 0..NK/2-1: index of the compare-exchange
+        const int i = ((c & ~(j - 1)) << 1) | (c & (j - 1));
         const int p = i | j;
         const bool up = (i & k) == 0;
         const float x = sb[i], y = sb[p];
@@ -346,11 +432,11 @@ __global__ void __launch_bounds__(RAYS_PER_BLOCK * 32) sample_pdf_kernel(const P
           sb[p] = x;
         }
       }
-      __syncwarp();
+      ray_sync<W>();
     }
   }
   float* zo = a.z_out + ray * (long long)(Nc + Nf);
-  for (int i = lane; i < Nc + Nf; i += 32) zo[i] = sb[i];
+  for (int i = seg; i < Nc + Nf; i += NT) zo[i] = sb[i];
 }
 
 // sparsity-loss gradient (nerf_sh/train.py:77-83): G.w = coef * exp(-len * relu(s)) * [s > 0]; the forward
@@ -412,18 +498,30 @@ __global__ void draw_uniforms_kernel(unsigned long long seed, float step_host, c
   }
 }
 
+// warps per ray for N samples
+int ray_warps(int N) { return N <= 32 * MAX_SEG ? 1 : WIDE; }
+
+// f(S, W): W = ray_warps(N), S = ceil(N / (32 W)) samples per lane (3..8 when W = WIDE)
 template <typename F>
 cudaError_t dispatch_seg(int N, F&& f) {
-  const int S = (N + 31) / 32;
-  switch (S) {
-    case 1: return f(std::integral_constant<int, 1>());
-    case 2: return f(std::integral_constant<int, 2>());
-    case 3: return f(std::integral_constant<int, 3>());
-    case 4: return f(std::integral_constant<int, 4>());
-    case 5: return f(std::integral_constant<int, 5>());
-    case 6: return f(std::integral_constant<int, 6>());
-    case 7: return f(std::integral_constant<int, 7>());
-    case 8: return f(std::integral_constant<int, 8>());
+  if (N < 1 || N > MAX_RAY_SAMPLES) return cudaErrorInvalidValue;
+  using W1 = std::integral_constant<int, 1>;
+  using W4 = std::integral_constant<int, WIDE>;
+  switch (ray_warps(N) == 1 ? (N + 31) / 32 : (N + 32 * WIDE - 1) / (32 * WIDE) + MAX_SEG) {
+    case 1: return f(std::integral_constant<int, 1>(), W1());
+    case 2: return f(std::integral_constant<int, 2>(), W1());
+    case 3: return f(std::integral_constant<int, 3>(), W1());
+    case 4: return f(std::integral_constant<int, 4>(), W1());
+    case 5: return f(std::integral_constant<int, 5>(), W1());
+    case 6: return f(std::integral_constant<int, 6>(), W1());
+    case 7: return f(std::integral_constant<int, 7>(), W1());
+    case 8: return f(std::integral_constant<int, 8>(), W1());
+    case MAX_SEG + 3: return f(std::integral_constant<int, 3>(), W4());
+    case MAX_SEG + 4: return f(std::integral_constant<int, 4>(), W4());
+    case MAX_SEG + 5: return f(std::integral_constant<int, 5>(), W4());
+    case MAX_SEG + 6: return f(std::integral_constant<int, 6>(), W4());
+    case MAX_SEG + 7: return f(std::integral_constant<int, 7>(), W4());
+    case MAX_SEG + 8: return f(std::integral_constant<int, 8>(), W4());
     default: return cudaErrorInvalidValue;
   }
 }
@@ -443,9 +541,10 @@ cudaError_t launch_composite_fwd(const float4* rgbs, const float* z, const float
                                  float* out_weights, cudaStream_t st) {
   if (R == 0) return cudaSuccess;
   CompositeArgs a{rgbs, z, dirs, R, N, white_bkgd, out_rgb, out_disp, out_acc, out_weights};
-  const unsigned grid = (R + RAYS_PER_BLOCK - 1) / RAYS_PER_BLOCK;
-  return dispatch_seg(N, [&](auto s) {
-    composite_fwd_kernel<decltype(s)::value><<<grid, RAYS_PER_BLOCK * 32, 0, st>>>(a);
+  const int rb = RAYS_PER_BLOCK / ray_warps(N);
+  const unsigned grid = (R + rb - 1) / rb;
+  return dispatch_seg(N, [&](auto s, auto w) {
+    composite_fwd_kernel<decltype(s)::value, decltype(w)::value><<<grid, RAYS_PER_BLOCK * 32, 0, st>>>(a);
     return cudaGetLastError();
   });
 }
@@ -456,9 +555,10 @@ cudaError_t launch_composite_bwd(const float4* rgbs, const float* z, const float
   if (R == 0) return cudaSuccess;
   if (sigma_act != SIGMA_RELU && sigma_act != SIGMA_SOFTPLUS) return cudaErrorInvalidValue;
   CompositeBwdArgs a{rgbs, z, dirs, comp_rgb, pixels, R, N, white_bkgd, gscale, sigma_act, G, sq_err_sum};
-  const unsigned grid = (R + RAYS_PER_BLOCK - 1) / RAYS_PER_BLOCK;
-  return dispatch_seg(N, [&](auto s) {
-    composite_bwd_kernel<decltype(s)::value><<<grid, RAYS_PER_BLOCK * 32, 0, st>>>(a);
+  const int rb = RAYS_PER_BLOCK / ray_warps(N);
+  const unsigned grid = (R + rb - 1) / rb;
+  return dispatch_seg(N, [&](auto s, auto w) {
+    composite_bwd_kernel<decltype(s)::value, decltype(w)::value><<<grid, RAYS_PER_BLOCK * 32, 0, st>>>(a);
     return cudaGetLastError();
   });
 }
@@ -466,10 +566,12 @@ cudaError_t launch_composite_bwd(const float4* rgbs, const float* z, const float
 cudaError_t launch_sample_pdf(const float* z_c, const float* weights, const float* u, int u_per_ray, int R,
                               int Nc, int Nf, float* z_out, cudaStream_t st) {
   if (R == 0) return cudaSuccess;
-  if (Nc < 3 || Nc + Nf > 256 || Nc - 2 > 32 * MAX_SEG) return cudaErrorInvalidValue;
+  if (Nc < 3 || Nf < 0 || Nc + Nf > MAX_RAY_SAMPLES) return cudaErrorInvalidValue;
   PdfArgs a{z_c, weights, u, u_per_ray, R, Nc, Nf, z_out};
-  const unsigned grid = (R + RAYS_PER_BLOCK - 1) / RAYS_PER_BLOCK;
-  sample_pdf_kernel<<<grid, RAYS_PER_BLOCK * 32, 0, st>>>(a);
+  if (ray_warps(Nc + Nf) == 1)
+    sample_pdf_kernel<1><<<(R + RAYS_PER_BLOCK - 1) / RAYS_PER_BLOCK, RAYS_PER_BLOCK * 32, 0, st>>>(a);
+  else
+    sample_pdf_kernel<WIDE><<<R, RAYS_PER_BLOCK * 32, 0, st>>>(a);
   return cudaGetLastError();
 }
 

@@ -175,6 +175,24 @@ def check_posenc(min_deg_point, max_deg_point):
             "bias column, and scales above 2^9 leave the posenc sine's range)")
 
 
+MAX_RAY_SAMPLES = 1024
+
+
+def check_samples(num_coarse_samples, num_fine_samples):
+    """flags num_coarse_samples / num_fine_samples that the per-ray kernels take: 3 <= Nc and Nc + Nf <= 1024.  A ray
+    is one warp up to 256 samples and four warps (one 128-thread block, 8 samples per lane) up to 1024; resampling
+    needs at least one interior coarse weight."""
+    nc, nf = int(num_coarse_samples), int(num_fine_samples)
+    bound = f"3 <= num_coarse_samples and num_coarse_samples + num_fine_samples <= {MAX_RAY_SAMPLES}"
+    if nc < 3 or nf < 0:
+        raise ValueError(f"num_coarse_samples={nc}, num_fine_samples={nf}: {bound} and num_fine_samples >= 0 expected "
+                         "(resampling draws from the coarse weights between the first and the last sample)")
+    if nc + nf > MAX_RAY_SAMPLES:
+        raise NotImplementedError(
+            f"num_coarse_samples={nc}, num_fine_samples={nf}: {bound} expected (the per-ray kernels hold at most "
+            f"{MAX_RAY_SAMPLES} samples of a ray, 8 per thread of one 128-thread block)")
+
+
 def check_scope(args):
     """features of the reference the relu-trunk path does not cover: fail loudly instead of training something else.
     A model with another trunk activation is checked by check_model_scope, which every CLI calls."""
@@ -187,6 +205,7 @@ def check_scope(args):
     if (args.net_depth, args.net_width, args.skip_layer) != (8, 256, 4):
         raise NotImplementedError("the fused kernel is built for the 8x256 trunk with the skip after layer 4")
     check_posenc(args.min_deg_point, args.max_deg_point)
+    check_samples(getattr(args, "num_coarse_samples", 64), getattr(args, "num_fine_samples", 128))
     if (str(args.net_activation).lower(), str(args.rgb_activation).lower()) != ("relu", "sigmoid"):
         raise NotImplementedError("activations other than relu (trunk) / sigmoid (rgb)")
     sigma_activation_code(args.sigma_activation)

@@ -55,9 +55,10 @@ class NerfModel:
                  white_bkgd=True, lindisp=False, max_rays=4096, sparsity_npoints=0, device="cuda",
                  precision=PREC_FP16, noise_std=None, sigma_activation="relu", min_deg_point=0, max_deg_point=10,
                  legacy_posenc_order=False, net_activation="relu"):
-        from .flags import net_activation_code, sigma_activation_code
+        from .flags import check_samples, net_activation_code, sigma_activation_code
         if not (-1 <= sh_deg <= 4):
             raise ValueError("sh_deg must be in [-1, 4]")
+        check_samples(num_coarse_samples, num_fine_samples)
         # flags min_deg_point / max_deg_point / legacy_posenc_order (nerf_sh/nerf/models.py:121-126): the point
         # encoder of both MLPs, which also sets the shapes of Dense_0 [W, 256] and Dense_5 [256 + W, 256]
         self.posenc = (int(min_deg_point), int(max_deg_point), bool(legacy_posenc_order))
