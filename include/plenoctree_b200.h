@@ -377,6 +377,43 @@ int pob_octree_render_depth_backward(const pob_octree* tree, const pob_octree_op
                                      const float* grad_depth_dev, const float* grad_acc_dev, float* grad_data_dev,
                                      void* stream);
 
+/* A compressed PlenOctree, as octree.compression writes it for the web viewer: no `data`; per leaf an fp32 sigma
+ * and, for each basis function k, the RGB triple of its coefficients either kept in fp16 (k < retain) or as an index
+ * into a 2^bits-entry fp16 palette of that basis function (k >= retain).  With L = n_nodes * N^3 leaves (< 2^32):
+ *   sigma_dev    [L] fp32                                 (quantised file key `sigma`)
+ *   map_dev      [basis_dim - retain, L] uint16, < 2^bits (`quant_map`; the caller checks the range)
+ *   palette_dev  [basis_dim - retain, 2^bits, 3] fp16     (`quant_colors`, as raw fp16 bits)
+ *   retained_dev [retain, L, 3] fp16                      (`data_retained`; may be NULL when retain = 0)
+ * child, N, format, offset and invradius as in pob_octree; 1 <= bits <= 16, 0 <= retain <= basis_dim.  The tree is
+ * read-only: there is no backward or training pass for it. */
+typedef struct pob_octree_quant {
+  const int32_t* child_dev;
+  int64_t n_nodes;
+  int N;
+  int basis_dim;
+  int format;     /* POB_OCTREE_* */
+  int retain;
+  int bits;
+  const float* sigma_dev;
+  const uint16_t* map_dev;
+  const uint16_t* palette_dev;
+  const uint16_t* retained_dev;
+  float offset[3];
+  float invradius[3];
+} pob_octree_quant;
+
+/* pob_octree_render / pob_octree_render_depth on a compressed tree: the same march, ray sources, outputs and counters.
+ * On the fp32 tree whose coefficients are the fp16 values the compressed tree decodes to (and the same sigma, child
+ * and geometry), the outputs are bit-identical to the fp32 entry points'. */
+int pob_octree_render_quant(const pob_octree_quant* tree, const pob_octree_opts* opts, const float* origins_dev,
+                            const float* dirs_dev, const float* vdirs_dev, int64_t n_rays, const pob_camera* cam,
+                            int row0, int nrows, float* out_rgb_dev, unsigned long long* counters_dev, void* stream);
+int pob_octree_render_depth_quant(const pob_octree_quant* tree, const pob_octree_opts* opts, const float* origins_dev,
+                                  const float* dirs_dev, const float* vdirs_dev, int64_t n_rays,
+                                  const pob_camera* cam, int row0, int nrows, float* out_rgb_dev,
+                                  float* out_depth_dev, float* out_acc_dev, unsigned long long* counters_dev,
+                                  void* stream);
+
 /* One training image of octree.optimization (octree/optimization.py:201-207) in one launch:
  *   im = render_persp(c2w); mse = mean((clamp(im,0,1) - gt)^2); mse.backward()
  * over the pixel rows [row0,row0+nrows): grad_data += grad_scale * d sum((clamp(im)-gt)^2) / d data,

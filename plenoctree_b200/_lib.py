@@ -73,6 +73,8 @@ SIGNATURES = {
     "pob_octree_render_backward": (_i, [_vp, _vp, _fp, _fp, _fp, _i64, _vp, _i, _i, _fp, _fp, _vp]),
     "pob_octree_render_depth": (_i, [_vp, _vp, _fp, _fp, _fp, _i64, _vp, _i, _i, _fp, _fp, _fp, _vp, _vp]),
     "pob_octree_render_depth_backward": (_i, [_vp, _vp, _fp, _fp, _fp, _i64, _vp, _i, _i, _fp, _fp, _fp, _fp, _vp]),
+    "pob_octree_render_quant": (_i, [_vp, _vp, _fp, _fp, _fp, _i64, _vp, _i, _i, _fp, _vp, _vp]),
+    "pob_octree_render_depth_quant": (_i, [_vp, _vp, _fp, _fp, _fp, _i64, _vp, _i, _i, _fp, _fp, _fp, _vp, _vp]),
     "pob_octree_train_persp": (_i, [_vp, _vp, _vp, _i, _i, _fp, _c.c_float, _fp, _vp, _fp, _vp]),
     "pob_octree_sgd_step": (_i, [_fp, _fp, _i64, _c.c_float, _vp]),
     "pob_octree_sgd_momentum_step": (_i, [_fp, _fp, _fp, _i64, _c.c_float, _c.c_float, _i, _vp]),
@@ -125,6 +127,13 @@ class TrainHParams(_c.Structure):
 class Octree(_c.Structure):
     _fields_ = [("data_dev", _vp), ("child_dev", _vp), ("n_nodes", _i64), ("N", _i), ("data_dim", _i),
                 ("basis_dim", _i), ("format", _i), ("offset", _c.c_float * 3), ("invradius", _c.c_float * 3)]
+
+
+class OctreeQuant(_c.Structure):
+    """pob_octree_quant: a compressed (palette-indexed) tree; palette / retained are fp16 bit patterns."""
+    _fields_ = [("child_dev", _vp), ("n_nodes", _i64), ("N", _i), ("basis_dim", _i), ("format", _i),
+                ("retain", _i), ("bits", _i), ("sigma_dev", _vp), ("map_dev", _vp), ("palette_dev", _vp),
+                ("retained_dev", _vp), ("offset", _c.c_float * 3), ("invradius", _c.c_float * 3)]
 
 
 class OctreeOpts(_c.Structure):

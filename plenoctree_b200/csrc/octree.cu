@@ -41,6 +41,18 @@ struct TreeDev {
   float off[3], inv[3];
 };
 
+// A compressed (palette-indexed) tree, the format octree.compression writes: the walk uses TreeDev's child /
+// N / K / rgba / off / inv (data and D are unused); a leaf's colour coefficient of basis function k is read from
+// `retained` for k < retain, else through map[k - retain][leaf] into palette[k - retain].
+struct QuantTreeDev : TreeDev {
+  const float* sigma;        // [leaves]
+  const uint16_t* map;       // [K - retain][leaves]
+  const __half* palette;     // [K - retain][ncolors][3]
+  const __half* retained;    // [retain][leaves][3]
+  int retain, ncolors;
+  unsigned long long leaves; // n_nodes * N^3: the plane stride of map / retained (Kq * leaves may pass 2^32)
+};
+
 struct Opts {
   float step, bg, sigma_thresh, stop_thresh;
 };
@@ -278,42 +290,17 @@ struct Marcher {
   }
 };
 
-// ---- forward march of one ray by one lane group -------------------------------------------------------
-// Software-pipelined: the loads of the current leaf (sigma and this lane's three coefficients, issued
-// unconditionally) are in flight while the next leaf is located; the march itself never depends on the data.
-//
-// DEPTH = true also accumulates, over the contributing visits i (sigma_i > sigma_thresh; visit i starts at t_i, has
-// step delta_t_i and weight w_i = T_i (1 - exp(-delta_t_i * delta_scale * sigma_i))):
-//   dz[0] = depth = sum_i w_i z_i,  z_i = (t_i + delta_t_i / 2) * delta_scale   (midpoint of the visit's
-//           constant-density segment, as a parameter along the caller's direction vector)
-//   dz[1] = acc   = sum_i w_i                                                   (the background not included)
-// Early termination rescales both by 1 / (1 - light) like the colour, so a stopped ray has acc = 1.  A ray that
-// misses the box has depth = acc = 0.  The colour, the march and the counters are those of DEPTH = false.
-template <int G, int KPL, bool DEPTH = false>
-__device__ __forceinline__ void trace_forward(const TreeDev& T, const Opts& O, const Ray& r, const float* basis_l, int l,
-                                              unsigned mask, float* out, unsigned& visits, unsigned& hits,
-                                              float* dz = nullptr) {
-  if constexpr (DEPTH) dz[0] = dz[1] = 0.f;
-  if (!r.hit) {
-    out[0] = out[1] = out[2] = O.bg;
-    return;
-  }
-  out[0] = out[1] = out[2] = 0.f;
-  float light = 1.0f;
-  float t = r.tmin;
-  const int K = T.K, D = T.D;
-  if (!(t < r.tmax)) {
-    out[0] = out[1] = out[2] = O.bg;  // light = 1
-    return;
-  }
-  Marcher<G> m;
-  m.init();
-  float delta_t;
-  unsigned idx = m.locate(T, r, O.step, t, l, mask, delta_t);
-  for (int it = 0; it < MAX_MARCH_STEPS; ++it) {
+// ---- leaf fetch: the forward march's policy for where a leaf's sigma and coefficients live ---------------------
+// issue() runs before the next leaf is located, finish() after it.  fp32 trees load everything in issue(); compressed
+// trees load sigma, the retained coefficients and the palette indices in issue() and the palette entries in finish()
+// (a dependent gather, so it waits for the indices while locate() runs).  Both produce fp32 coefficients that the
+// shading arithmetic consumes unchanged: lane l owns basis functions l, l+G, ...
+template <int G, int KPL>
+struct DenseFetch {
+  __device__ __forceinline__ float issue(const TreeDev& T, unsigned idx, int l, float* c0, float* c1, float* c2) {
+    const int K = T.K, D = T.D;
     const float* __restrict__ val = T.data + size_t(idx) * unsigned(D);
     const float sigma = __ldg(val + D - 1);
-    float c0[KPL], c1[KPL], c2[KPL];  // lane l owns basis functions l, l+G, ...
 #pragma unroll
     for (int j = 0; j < KPL; ++j) {
       const int k = l + j * G;
@@ -324,11 +311,101 @@ __device__ __forceinline__ void trace_forward(const TreeDev& T, const Opts& O, c
         c2[j] = __ldg(val + 2 * K + k);
       }
     }
+    return sigma;
+  }
+  __device__ __forceinline__ void finish(const TreeDev&, int, bool, float*, float*, float*) {}
+};
+
+template <int G, int KPL>
+struct QuantFetch {
+  unsigned m[KPL];   // palette index of basis function l + j*G (palette-coded functions only)
+
+  __device__ __forceinline__ float issue(const QuantTreeDev& T, unsigned idx, int l, float* c0, float* c1, float* c2) {
+    const float sigma = __ldg(T.sigma + idx);
+#pragma unroll
+    for (int j = 0; j < KPL; ++j) {
+      const int k = l + j * G;
+      c0[j] = c1[j] = c2[j] = 0.f;
+      m[j] = 0;
+      if (k < T.retain) {
+        const __half* p = T.retained + (unsigned long long)k * T.leaves * 3 + size_t(idx) * 3;
+        c0[j] = __half2float(__ldg(p));
+        c1[j] = __half2float(__ldg(p + 1));
+        c2[j] = __half2float(__ldg(p + 2));
+      } else if (k < T.K) {
+        m[j] = __ldg(T.map + (unsigned long long)(k - T.retain) * T.leaves + idx);
+      }
+    }
+    return sigma;
+  }
+  // `use`: the leaf contributes (sigma > sigma_thresh); the palette is only read for leaves that are shaded
+  __device__ __forceinline__ void finish(const QuantTreeDev& T, int l, bool use, float* c0, float* c1, float* c2) {
+    if (!use) return;
+#pragma unroll
+    for (int j = 0; j < KPL; ++j) {
+      const int k = l + j * G;
+      if (k >= T.retain && k < T.K) {
+        const __half* p = T.palette + ((size_t)(k - T.retain) * unsigned(T.ncolors) + m[j]) * 3;
+        c0[j] = __half2float(__ldg(p));
+        c1[j] = __half2float(__ldg(p + 1));
+        c2[j] = __half2float(__ldg(p + 2));
+      }
+    }
+  }
+};
+
+template <class Tree, int G, int KPL>
+struct LeafFetch {
+  using type = DenseFetch<G, KPL>;
+};
+template <int G, int KPL>
+struct LeafFetch<QuantTreeDev, G, KPL> {
+  using type = QuantFetch<G, KPL>;
+};
+
+// ---- forward march of one ray by one lane group -------------------------------------------------------
+// Software-pipelined: the loads of the current leaf (sigma and this lane's three coefficients, issued
+// unconditionally; for a compressed tree the palette indices, then the palette entries once the next leaf is
+// located) are in flight while the next leaf is located; the march itself never depends on the data.
+//
+// DEPTH = true also accumulates, over the contributing visits i (sigma_i > sigma_thresh; visit i starts at t_i, has
+// step delta_t_i and weight w_i = T_i (1 - exp(-delta_t_i * delta_scale * sigma_i))):
+//   dz[0] = depth = sum_i w_i z_i,  z_i = (t_i + delta_t_i / 2) * delta_scale   (midpoint of the visit's
+//           constant-density segment, as a parameter along the caller's direction vector)
+//   dz[1] = acc   = sum_i w_i                                                   (the background not included)
+// Early termination rescales both by 1 / (1 - light) like the colour, so a stopped ray has acc = 1.  A ray that
+// misses the box has depth = acc = 0.  The colour, the march and the counters are those of DEPTH = false.
+// Tree = QuantTreeDev marches a compressed tree: only the leaf fetch differs (LeafFetch).
+template <int G, int KPL, bool DEPTH = false, class Tree = TreeDev>
+__device__ __forceinline__ void trace_forward(const Tree& T, const Opts& O, const Ray& r, const float* basis_l, int l,
+                                              unsigned mask, float* out, unsigned& visits, unsigned& hits,
+                                              float* dz = nullptr) {
+  if constexpr (DEPTH) dz[0] = dz[1] = 0.f;
+  if (!r.hit) {
+    out[0] = out[1] = out[2] = O.bg;
+    return;
+  }
+  out[0] = out[1] = out[2] = 0.f;
+  float light = 1.0f;
+  float t = r.tmin;
+  if (!(t < r.tmax)) {
+    out[0] = out[1] = out[2] = O.bg;  // light = 1
+    return;
+  }
+  Marcher<G> m;
+  m.init();
+  float delta_t;
+  unsigned idx = m.locate(T, r, O.step, t, l, mask, delta_t);
+  for (int it = 0; it < MAX_MARCH_STEPS; ++it) {
+    typename LeafFetch<Tree, G, KPL>::type fetch;
+    float c0[KPL], c1[KPL], c2[KPL];  // lane l owns basis functions l, l+G, ...
+    const float sigma = fetch.issue(T, idx, l, c0, c1, c2);
     const float t_next = t + delta_t;
     const bool more = t_next < r.tmax;
     float delta_n = 0.f;
     unsigned idx_n = 0;
     if (more) idx_n = m.locate(T, r, O.step, t_next, l, mask, delta_n);
+    fetch.finish(T, l, sigma > O.sigma_thresh, c0, c1, c2);
     ++visits;
     if (sigma > O.sigma_thresh) {
       ++hits;
@@ -511,9 +588,10 @@ __device__ __forceinline__ void lane_basis(const TreeDev& T, const Ray& r, int l
   }
 }
 
-// DEPTH = true also stores depth [n] (times fetch_ray's zscale) and acc [n] (trace_forward<DEPTH>)
-template <int G, int KPL, bool DEPTH = false>
-__global__ void __launch_bounds__(256) octree_render_kernel(TreeDev T, Opts O, RaySrc S, float* __restrict__ out_rgb,
+// DEPTH = true also stores depth [n] (times fetch_ray's zscale) and acc [n] (trace_forward<DEPTH>); Tree = QuantTreeDev
+// renders a compressed tree
+template <int G, int KPL, bool DEPTH = false, class Tree = TreeDev>
+__global__ void __launch_bounds__(256) octree_render_kernel(Tree T, Opts O, RaySrc S, float* __restrict__ out_rgb,
                                                             unsigned long long* __restrict__ counters,
                                                             float* __restrict__ out_depth, float* __restrict__ out_acc) {
   Ray r;
@@ -526,7 +604,7 @@ __global__ void __launch_bounds__(256) octree_render_kernel(TreeDev T, Opts O, R
   lane_basis<G, KPL>(T, r, l, bl);
   float out[3], dz[2];
   unsigned visits = 0, hits = 0;
-  trace_forward<G, KPL, DEPTH>(T, O, r, bl, l, mask, out, visits, hits, dz);
+  trace_forward<G, KPL, DEPTH, Tree>(T, O, r, bl, l, mask, out, visits, hits, dz);
   if (l < 3) out_rgb[3 * oi + l] = l == 0 ? out[0] : l == 1 ? out[1] : out[2];
   if constexpr (DEPTH) {
     if (l == 0) {
@@ -826,6 +904,47 @@ int tree_dev(const char* where, const pob_octree* t, TreeDev& T) {
   return 0;
 }
 
+int quant_tree_dev(const char* where, const pob_octree_quant* t, QuantTreeDev& T) {
+  if (!t) return pob_fail(where, "tree is NULL");
+  if (!t->child_dev || !t->sigma_dev) return pob_fail(where, "tree child/sigma pointer is NULL");
+  if (t->N < 2 || t->N > 8) return pob_fail(where, "tree branch factor N must be in [2, 8]");
+  if (t->n_nodes < 1) return pob_fail(where, "tree has no nodes");
+  const double leaves = double(t->n_nodes) * t->N * t->N * t->N;
+  if (leaves >= 4294967296.0) return pob_fail(where, "tree too large (leaf index must fit 32 bits)");
+  const int K = t->basis_dim;
+  if (t->format == POB_OCTREE_RGBA) {
+    if (K != 1) return pob_fail(where, "RGBA trees have basis_dim 1");
+  } else if (t->format == POB_OCTREE_SH) {
+    if (!(K == 1 || K == 4 || K == 9 || K == 16 || K == 25)) return pob_fail(where, "SH basis_dim must be 1,4,9,16,25");
+  } else {
+    return pob_fail(where, "unsupported data format (RGBA and SH only; SG is out of scope)");
+  }
+  if (t->bits < 1 || t->bits > 16) return pob_fail(where, "bits must be in [1, 16] (palette indices are uint16)");
+  if (t->retain < 0 || t->retain > K) return pob_fail(where, "retain must be in [0, basis_dim]");
+  if (t->retain > 0 && !t->retained_dev) return pob_fail(where, "retained pointer is NULL with retain > 0");
+  if (t->retain < K && (!t->map_dev || !t->palette_dev))
+    return pob_fail(where, "map/palette pointer is NULL with retain < basis_dim");
+  T.data = nullptr;
+  T.child = t->child_dev;
+  T.N = t->N;
+  T.D = 0;
+  T.K = K;
+  T.rgba = t->format == POB_OCTREE_RGBA;
+  for (int a = 0; a < 3; ++a) {
+    T.off[a] = t->offset[a];
+    T.inv[a] = t->invradius[a];
+  }
+  T.sigma = t->sigma_dev;
+  T.map = t->map_dev;
+  T.palette = reinterpret_cast<const __half*>(t->palette_dev);
+  T.retained = reinterpret_cast<const __half*>(t->retained_dev);
+  T.retain = t->retain;
+  T.ncolors = 1 << t->bits;
+  T.leaves = (unsigned long long)leaves;
+  if (pob_sm_count_cached() <= 0) return pob_fail(where, "no sm_90 CUDA device (there is no CPU fallback)");
+  return 0;
+}
+
 int opts_dev(const char* where, const pob_octree_opts* o, Opts& O) {
   if (!o) return pob_fail(where, "options are NULL");
   // every march iteration advances by at least step_size (unit cube): below sqrt(3) / MAX_MARCH_STEPS a diagonal ray
@@ -908,9 +1027,55 @@ int ray_src(const char* where, const float* o, const float* d, const float* v, l
   return 0;
 }
 
+// pob_octree_render_quant / pob_octree_render_depth_quant (depth outputs null for the former)
+int render_quant(const char* W, const pob_octree_quant* tree, const pob_octree_opts* opts, const float* origins_dev,
+                 const float* dirs_dev, const float* vdirs_dev, int64_t n_rays, const pob_camera* cam, int row0,
+                 int nrows, float* out_rgb_dev, float* out_depth_dev, float* out_acc_dev,
+                 unsigned long long* counters_dev, void* stream, bool depth) {
+  QuantTreeDev T;
+  Opts O;
+  RaySrc S;
+  unsigned blocks = 0;
+  if (int rc = quant_tree_dev(W, tree, T)) return rc;
+  if (int rc = opts_dev(W, opts, O)) return rc;
+  const int G = group_width(T.K);
+  if (int rc = ray_src(W, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0, nrows, S, blocks, G)) return rc;
+  if (!out_rgb_dev || (depth && (!out_depth_dev || !out_acc_dev))) return pob_fail(W, "output pointer is NULL");
+  if (blocks == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  pob_count_launch();
+  octree_dispatch(G, T.K, [&](auto g_, auto kpl_) {
+    constexpr int g = decltype(g_)::value, kpl = decltype(kpl_)::value;
+    if (depth)
+      octree_render_kernel<g, kpl, true, QuantTreeDev><<<blocks, 256, 0, st>>>(T, O, S, out_rgb_dev, counters_dev,
+                                                                               out_depth_dev, out_acc_dev);
+    else
+      octree_render_kernel<g, kpl, false, QuantTreeDev><<<blocks, 256, 0, st>>>(T, O, S, out_rgb_dev, counters_dev,
+                                                                                nullptr, nullptr);
+  });
+  POB_CUDA(W, cudaGetLastError());
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
+
+int pob_octree_render_quant(const pob_octree_quant* tree, const pob_octree_opts* opts, const float* origins_dev,
+                            const float* dirs_dev, const float* vdirs_dev, int64_t n_rays, const pob_camera* cam,
+                            int row0, int nrows, float* out_rgb_dev, unsigned long long* counters_dev, void* stream) {
+  return render_quant("pob_octree_render_quant", tree, opts, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0,
+                      nrows, out_rgb_dev, nullptr, nullptr, counters_dev, stream, false);
+}
+
+int pob_octree_render_depth_quant(const pob_octree_quant* tree, const pob_octree_opts* opts, const float* origins_dev,
+                                  const float* dirs_dev, const float* vdirs_dev, int64_t n_rays,
+                                  const pob_camera* cam, int row0, int nrows, float* out_rgb_dev,
+                                  float* out_depth_dev, float* out_acc_dev, unsigned long long* counters_dev,
+                                  void* stream) {
+  return render_quant("pob_octree_render_depth_quant", tree, opts, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0,
+                      nrows, out_rgb_dev, out_depth_dev, out_acc_dev, counters_dev, stream, true);
+}
 
 int pob_octree_render(const pob_octree* tree, const pob_octree_opts* opts, const float* origins_dev,
                       const float* dirs_dev, const float* vdirs_dev, int64_t n_rays, const pob_camera* cam,

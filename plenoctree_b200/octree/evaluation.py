@@ -1,14 +1,15 @@
 """`python -m plenoctree_b200.octree.evaluation` and `eval_octree` (octree/evaluation.py:75-123,
 octree/nerf/utils.py:448-498): render every test view of a PlenOctree, PSNR / SSIM against the ground truth
 LPIPS is added when its downloaded weights can be found (nerf/lpips.py), else reported as nan.  `--write_disp DIR`
-writes each view's disparity map as `disp_{i:04d}.png`, as nerf_sh.eval does for the NeRF."""
+writes each view's disparity map as `disp_{i:04d}.png`, as nerf_sh.eval does for the NeRF.  `--input` may also be a
+compressed tree written by octree.compression (quantised or --noquant), rendered as stored."""
 import os
 
 import numpy as np
 import torch
 
 from ..nerf.utils import compute_psnr, compute_ssim, save_img, write_video
-from .n3tree import N3Tree
+from .n3tree import load_tree
 from .renderer import VolumeRenderer, disparity
 
 
@@ -65,7 +66,7 @@ def main(unused_argv):
     F.update_flags(FLAGS)
     dev = torch.device("cuda")
     dataset = datasets.get_dataset("test", FLAGS, device=dev)
-    t = N3Tree.load(FLAGS.input, map_location=dev)
+    t = load_tree(FLAGS.input, map_location=dev)      # tree.npz, or a compressed one (octree.compression)
     from ..nerf.lpips import load_lpips
     extra = {}
     disp_fn = None

@@ -51,6 +51,8 @@ class DataFormat:
 
 
 class N3Tree:
+    read_only = False   # True for a tree loaded from a --noquant compressed file (load_tree)
+
     def __init__(self, N=2, data_dim=4, depth_limit=10, init_reserve=1, init_refine=0, geom_resize_fact=1.5,
                  radius=0.5, center=(0.5, 0.5, 0.5), data_format="RGBA", extra_data=None, map_location="cuda",
                  device=None):
@@ -166,6 +168,8 @@ class N3Tree:
 
     def parameters(self):
         """svox N3Tree is an nn.Module whose only parameter is `data` (octree/optimization.py:187)."""
+        if self.read_only:
+            raise ValueError("a compressed PlenOctree is read-only: it has no trainable parameters")
         self.data.requires_grad_(True)
         return [self.data]
 
@@ -296,6 +300,9 @@ class N3Tree:
     @classmethod
     def load(cls, path, map_location="cuda", device=None):
         z = np.load(path)
+        if compressed_layout(z) is not None:
+            raise ValueError(f"{path} is a compressed PlenOctree (octree.compression output), a read-only final format: "
+                             "it can be rendered and evaluated (octree.n3tree.load_tree) but not optimised or refined")
         dev = torch.device(device if device is not None else map_location)
         t = cls.__new__(cls)
         t.device = dev
@@ -324,6 +331,202 @@ class N3Tree:
     def __repr__(self):
         return (f"plenoctree_b200.N3Tree(N={self.N}, data_dim={self.data_dim}, depth_limit={self.depth_limit}, "
                 f"capacity:{self.n_internal - self.n_free}/{self.capacity}, data_format={self.data_format!r})")
+
+
+# ---- compressed trees (octree.compression output) ----------------------------------------------------------
+BOOKKEEPING = ("parent_depth", "geom_resize_fact", "n_free", "n_internal", "depth_limit")
+
+
+def _files(z):
+    return set(z.files) if hasattr(z, "files") else set(z.keys())
+
+
+def compressed_layout(z):
+    """'quant' for a quantised octree.compression file (it has quant_map), 'noquant' for a --noquant one (data, but
+    none of the refine bookkeeping keys), None for an ordinary tree.npz."""
+    files = _files(z)
+    if "quant_map" in files:
+        return "quant"
+    if "data" in files and not files & set(BOOKKEEPING):
+        return "noquant"
+    return None
+
+
+class QuantTree:
+    """A compressed PlenOctree on the device, as octree.compression writes it: per leaf an fp32 sigma and, per basis
+    function k, fp16 RGB coefficients (k < retain) or a uint16 index into that function's fp16 palette.  Read-only:
+    VolumeRenderer.forward / render_persp draw it (pob_octree_render_quant); nothing trains or refines it."""
+    read_only = True
+
+    def __init__(self, child, sigma, qmap, palette, retained, offset, invradius, data_format, device):
+        self.device = device
+        self.data_format = data_format
+        self.N = int(child.shape[-1])
+        self.n_internal = int(child.shape[0])
+        self.retain = 0 if retained is None else int(retained.shape[0])
+        self.bits = int(palette.shape[1]).bit_length() - 1
+        up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(device)   # noqa: E731
+        self.child = up(child.astype(np.int32))
+        self.sigma = up(sigma.astype(np.float32))
+        self.map = up(qmap.astype(np.uint16).view(np.int16))           # uint16 bits (torch has no uint16 arithmetic)
+        self.palette = up(palette.astype(np.float16))
+        self.retained = None if retained is None else up(retained.astype(np.float16))
+        self.offset = up(offset.astype(np.float32))
+        self.invradius = up(invradius.astype(np.float32))
+
+    def device_bytes(self):
+        return sum(t.numel() * t.element_size() for t in (self.child, self.sigma, self.map, self.palette, self.retained)
+                   if t is not None)
+
+    def parameters(self):
+        raise ValueError("a compressed PlenOctree is read-only: it has no trainable parameters")
+
+    def c_struct(self):
+        t = _lib.OctreeQuant()
+        t.child_dev = self.child.data_ptr()
+        t.n_nodes = self.n_internal
+        t.N = self.N
+        t.basis_dim = self.data_format.basis_dim
+        t.format = self.data_format.format
+        t.retain = self.retain
+        t.bits = self.bits
+        t.sigma_dev = self.sigma.data_ptr()
+        t.map_dev = self.map.data_ptr() if self.map.numel() else None
+        t.palette_dev = self.palette.data_ptr() if self.palette.numel() else None
+        t.retained_dev = None if self.retained is None else self.retained.data_ptr()
+        off = self.offset.cpu().numpy()
+        inv = self.invradius.cpu().numpy()
+        for a in range(3):
+            t.offset[a] = float(off[a])
+            t.invradius[a] = float(inv[a])
+        return t
+
+    def __repr__(self):
+        return (f"plenoctree_b200.QuantTree(N={self.N}, nodes={self.n_internal}, data_format={self.data_format!r}, "
+                f"bits={self.bits}, retain={self.retain})")
+
+
+def _key(z, files, key):
+    if key not in files:
+        raise ValueError(f"compressed tree: missing key {key!r}")
+    return np.asarray(z[key])
+
+
+def _shape(arr, want, key):
+    if tuple(arr.shape) != tuple(want):
+        raise ValueError(f"compressed tree: {key!r} has shape {tuple(arr.shape)}, expected {tuple(want)}")
+
+
+def _geometry(z, files):
+    """-> child, offset, invradius, DataFormat of a compressed file, checked: child [n, N, N, N] with 2 <= N <= 8, fewer
+    than 2^32 leaves, and every internal cell pointing at a node inside the array."""
+    child = _key(z, files, "child")
+    N = child.shape[-1] if child.ndim == 4 else 0
+    if child.ndim != 4 or child.shape[1:] != (N, N, N) or not 2 <= N <= 8 or child.shape[0] < 1 \
+            or not np.issubdtype(child.dtype, np.integer):
+        raise ValueError(f"compressed tree: 'child' must be an integer array [n_nodes, N, N, N] with N in [2, 8], "
+                         f"got {child.dtype} {tuple(child.shape)}")
+    n = child.shape[0]
+    if n * N ** 3 >= 2 ** 32:
+        raise ValueError("compressed tree: 'child' has 2^32 or more leaves")
+    c = child.reshape(n, -1).astype(np.int64)
+    target = np.arange(n, dtype=np.int64)[:, None] + c
+    if ((c != 0) & ((target <= 0) | (target >= n))).any():
+        raise ValueError("compressed tree: 'child' points outside the node array")
+    inv = (_key(z, files, "invradius3") if "invradius3" in files
+           else np.full(3, float(_key(z, files, "invradius")), dtype=np.float32))
+    off = _key(z, files, "offset")
+    _shape(inv, (3,), "invradius3")
+    _shape(off, (3,), "offset")
+    fmt = DataFormat(str(z["data_format"]) if "data_format" in files else None)
+    if "data_dim" in files and int(z["data_dim"]) != fmt.data_dim():
+        raise ValueError(f"compressed tree: 'data_dim' {int(z['data_dim'])} does not match data format {fmt!r}")
+    return child, off, inv, fmt
+
+
+def read_compressed(z):
+    """The host arrays of a compressed file (an npz or dict), checked -> dict(layout, child, offset, invradius,
+    data_format) plus data (--noquant) or sigma, quant_map, quant_colors, data_retained (None when absent).  These
+    arrays come from outside the program and index device memory, so a bad one raises ValueError naming the key:
+    shapes against `child`, palette sizes against the data format, and every palette index inside its palette."""
+    layout = compressed_layout(z)
+    if layout is None:
+        raise ValueError("not a compressed PlenOctree: no 'quant_map', and 'data' comes with the refine bookkeeping")
+    files = _files(z)
+    if "extra_data" in files:
+        raise NotImplementedError("extra_data (SG/ASG formats) is outside the scope of this path")
+    child, off, inv, fmt = _geometry(z, files)
+    leaf_shape = child.shape
+    out = dict(layout=layout, child=child, offset=off, invradius=inv, data_format=fmt)
+    if layout == "noquant":
+        data = _key(z, files, "data")
+        _shape(data, leaf_shape + (fmt.data_dim(),), "data")
+        out["data"] = data
+        return out
+    sigma = _key(z, files, "sigma")
+    _shape(sigma, leaf_shape, "sigma")
+    qmap = _key(z, files, "quant_map")
+    colors = _key(z, files, "quant_colors")
+    if qmap.ndim != 5 or not np.issubdtype(qmap.dtype, np.integer):
+        raise ValueError(f"compressed tree: 'quant_map' must be an integer array [Kq, n_nodes, N, N, N], got "
+                         f"{qmap.dtype} {tuple(qmap.shape)}")
+    Kq = qmap.shape[0]
+    _shape(qmap, (Kq,) + leaf_shape, "quant_map")
+    C = colors.shape[1] if colors.ndim == 3 else 0
+    if colors.ndim != 3 or C < 2 or C > 65536 or C & (C - 1):
+        raise ValueError(f"compressed tree: 'quant_colors' must be [Kq, 2^bits, 3] with 1 <= bits <= 16, got "
+                         f"{tuple(colors.shape)}")
+    _shape(colors, (Kq, C, 3), "quant_colors")
+    retained = None
+    if "data_retained" in files:
+        retained = np.asarray(z["data_retained"])
+        _shape(retained, (retained.shape[0] if retained.ndim else 0,) + leaf_shape + (3,), "data_retained")
+    retain = 0 if retained is None else retained.shape[0]
+    if retain + Kq != fmt.basis_dim:
+        raise ValueError(f"compressed tree: 'quant_colors' ({Kq}) and 'data_retained' ({retain}) basis functions do "
+                         f"not add up to the {fmt.basis_dim} of data format {fmt!r}")
+    for j in range(Kq):
+        lo, hi = int(qmap[j].min()), int(qmap[j].max())
+        if lo < 0 or hi >= C:
+            raise ValueError(f"compressed tree: 'quant_map'[{j}] holds index {hi if hi >= C else lo}, outside the "
+                             f"{C} entries of 'quant_colors'[{j}]")
+    out.update(sigma=sigma, quant_map=qmap, quant_colors=colors, data_retained=retained)
+    return out
+
+
+def load_tree(src, map_location="cuda", device=None):
+    """Any PlenOctree file (path, or an already loaded npz / dict): an ordinary tree.npz through N3Tree.load, a
+    quantised octree.compression file as a QuantTree, a --noquant one as a read-only fp32 N3Tree without the refine
+    bookkeeping.  Compressed files are checked by read_compressed first."""
+    z = np.load(src) if isinstance(src, (str, bytes)) or hasattr(src, "__fspath__") else src
+    if compressed_layout(z) is None:
+        return N3Tree.load(src, map_location=map_location, device=device)
+    c = read_compressed(z)
+    dev = torch.device(device if device is not None else map_location)
+    if dev.type != "cuda":
+        raise RuntimeError("plenoctree_b200 trees live on a CUDA device (there is no CPU path)")
+    child, fmt = c["child"], c["data_format"]
+    if c["layout"] == "quant":
+        return QuantTree(child, c["sigma"], c["quant_map"], c["quant_colors"], c["data_retained"], c["offset"],
+                         c["invradius"], fmt, dev)
+    t = N3Tree.__new__(N3Tree)
+    t.device = dev
+    t.N = int(child.shape[-1])
+    t.data_format = fmt
+    t.data_dim = fmt.data_dim()
+    t.data = torch.from_numpy(c["data"].astype(np.float32)).to(dev)
+    t.child = torch.from_numpy(child.astype(np.int32)).to(dev)
+    t.parent_depth = None
+    t.n_internal = int(child.shape[0])
+    t.n_free = 0
+    t.depth_limit = None
+    t.geom_resize_fact = None
+    t.invradius = torch.from_numpy(c["invradius"].astype(np.float32)).to(dev)
+    t.offset = torch.from_numpy(c["offset"].astype(np.float32)).to(dev)
+    t.grad = None
+    t._leaves = None
+    t.read_only = True
+    return t
 
 
 class N3TreeView:

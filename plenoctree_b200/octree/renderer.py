@@ -9,6 +9,8 @@
     (no svox counterpart)                                            forward / render_persp(..., return_depth=True)
                                                                      -> (rgb, depth, acc) like nerf/utils.py's
                                                                      render_image; disparity(depth, acc) -> disp
+    (no svox counterpart)                                            the same forward on a compressed tree
+                                                                     (n3tree.load_tree -> QuantTree): no gradients
     mse.backward(); optimizer.step()  optimization.py:205-208        train_persp + N3Tree.sgd_step: one launch for
                                                                      render + clamp-MSE gradient + scatter
 
@@ -140,6 +142,7 @@ class VolumeRenderer:
         of the same shape with 1 channel"""
         tree = self.tree
         t = tree.c_struct()
+        quant = isinstance(t, _lib.OctreeQuant)      # a compressed tree (n3tree.QuantTree)
         if cam is None:
             ro, rd, rv = rays
             shape = (ro.shape[0],)
@@ -149,13 +152,13 @@ class VolumeRenderer:
             src = (None, None, None, 0, ctypes.byref(cam), row0, nrows)
         out = torch.empty(shape + (3,), dtype=torch.float32, device=tree.device)
         if not return_depth:
-            check(lib.pob_octree_render(ctypes.byref(t), ctypes.byref(opts), *src, ptr(out), ptr(counters),
-                                        stream_ptr()))
+            fn = lib.pob_octree_render_quant if quant else lib.pob_octree_render
+            check(fn(ctypes.byref(t), ctypes.byref(opts), *src, ptr(out), ptr(counters), stream_ptr()))
             return out
         depth = torch.empty(shape + (1,), dtype=torch.float32, device=tree.device)
         acc = torch.empty(shape + (1,), dtype=torch.float32, device=tree.device)
-        check(lib.pob_octree_render_depth(ctypes.byref(t), ctypes.byref(opts), *src, ptr(out), ptr(depth), ptr(acc),
-                                          ptr(counters), stream_ptr()))
+        fn = lib.pob_octree_render_depth_quant if quant else lib.pob_octree_render_depth
+        check(fn(ctypes.byref(t), ctypes.byref(opts), *src, ptr(out), ptr(depth), ptr(acc), ptr(counters), stream_ptr()))
         return out, depth, acc
 
     @staticmethod
@@ -164,9 +167,15 @@ class VolumeRenderer:
             t = torch.from_numpy(t)
         return t.to(device=dev, dtype=torch.float32).reshape(-1, 3).contiguous()
 
+    def _check_trainable(self, what):
+        if getattr(self.tree, "read_only", False):
+            raise ValueError(f"{what} needs gradients, and a compressed PlenOctree is read-only (it renders forward "
+                             "only)")
+
     def _render(self, rays, cam, row0, nrows, opts, counters, return_depth):
-        data = self.tree.data
-        if torch.is_grad_enabled() and data.requires_grad:
+        data = getattr(self.tree, "data", None)      # a QuantTree has none
+        if torch.is_grad_enabled() and data is not None and data.requires_grad:
+            self._check_trainable("rendering with tree.data.requires_grad")
             fn = _RenderDepthFn if return_depth else _RenderFn
             return fn.apply(data, self, rays, cam, row0, nrows, opts)
         return self._render_raw(rays, cam, row0, nrows, opts, counters, return_depth)
@@ -195,6 +204,7 @@ class VolumeRenderer:
         """One training image of octree.optimization (octree/optimization.py:201-207) in ONE kernel: render the slab,
         mse = mean((clamp(im,0,1) - gt)^2), scatter d mse / d data into tree.grad_buffer().  gt: [H,W,3] (or the
         slab's rows).  Returns (sum of squared errors as a 1-element float64 device tensor, image or None)."""
+        self._check_trainable("train_persp")
         tree = self.tree
         cam = make_camera(c2w, width, height, fx, fy)
         H, W = int(height), int(width)
