@@ -63,7 +63,12 @@ typedef struct pob_posenc {
  * ------------------------------------------------------------------------------------------- */
 int pob_abi_version(void);
 const char* pob_last_error(void);
-/* number of SMs of the current CUDA device (persistent-grid size); <0 on error */
+/* number of SMs the kernels split their work for (persistent-grid size): the current CUDA device's, or the
+ * environment variable POB_SM_COUNT when it is set (read on every call; for tests and diagnosis: it selects the work
+ * split of a smaller H100, such as the 114-SM PCIe card or a MIG slice, and changes no code path).  POB_SM_COUNT must
+ * be an integer from 16 to the device's SM count; any other value makes every entry point that reads the count (the
+ * MLP evaluations, pob_render_rays, the pob_loss_and_grad family, pob_draw_uniforms and the octree entry points) fail
+ * with a message naming it, before anything is launched, and this function return -3.  <0 on error */
 int pob_sm_count(void);
 
 /* Instrumentation used by bench.py: number of kernels this library has launched so far, and

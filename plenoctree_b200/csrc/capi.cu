@@ -1,5 +1,7 @@
 // capi.cu — extern "C" entry points declared in include/plenoctree_b200.h.
+#include <cerrno>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <string>
 
@@ -65,18 +67,35 @@ int K_of(int sh_deg) { return sh_deg < 0 ? 1 : (sh_deg + 1) * (sh_deg + 1); }
 
 bool valid_deg(int sh_deg) { return sh_deg >= -1 && sh_deg <= 4; }
 
-int g_sm_count = -1;
+// The weight gradient has 16 units of work (optim.cu: wgrad_assign_roles), each needing a CTA of its own; from 16
+// SMs up the data gradient keeps at least one CTA, and its CTAs plus the weight gradient's fit on the device.
+constexpr int MIN_SPLIT_SMS = 16;
+int g_device_sms = -1;
+thread_local std::string g_sm_count_env;   // the refused POB_SM_COUNT value, for the message
+
+// SM count the kernels split their work for: the device's, or POB_SM_COUNT when set (read on every call).
+// -1: no CUDA device, -2: not compute capability 9.0, -3: POB_SM_COUNT is not an integer in [16, device SMs].
 int sm_count() {
-  if (g_sm_count > 0) return g_sm_count;
-  int dev = 0, n = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return -1;
-  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return -1;
-  int major = 0, minor = 0;
-  cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-  cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
-  if (major != 9 || minor != 0) return -2;  // sm_90a only (wgmma)
-  g_sm_count = n;
-  return n;
+  if (g_device_sms <= 0) {
+    int dev = 0, n = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) return -1;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return -1;
+    int major = 0, minor = 0;
+    cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
+    cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
+    if (major != 9 || minor != 0) return -2;  // sm_90a only (wgmma)
+    g_device_sms = n;
+  }
+  const char* e = getenv("POB_SM_COUNT");
+  if (!e) return g_device_sms;
+  char* end = nullptr;
+  errno = 0;
+  const long v = strtol(e, &end, 10);
+  if (end == e || *end != '\0' || errno != 0 || v < MIN_SPLIT_SMS || v > g_device_sms) {
+    g_sm_count_env = e;
+    return -3;
+  }
+  return int(v);
 }
 
 // packed blob layout of one MLP
@@ -108,10 +127,7 @@ int check_common(const char* where, const void* packed, int sh_deg, int precisio
   if (!packed) return fail(where, "packed weights pointer is NULL");
   if (precision != POB_PREC_FP16 && precision != POB_PREC_FP16X3)
     return fail(where, "precision must be POB_PREC_FP16 or POB_PREC_FP16X3");
-  int n = sm_count();
-  if (n == -2) return fail(where, "device is not compute capability 9.0 (sm_90a build)");
-  if (n <= 0) return fail(where, "no CUDA device");
-  return 0;
+  return pob_sms_or_fail(where) > 0 ? 0 : 1;
 }
 
 pob::FwdParams base_params(const void* packed, int sh_deg, pob::NetDesc net) {
@@ -128,7 +144,19 @@ pob::FwdParams base_params(const void* packed, int sh_deg, pob::NetDesc net) {
 
 }  // namespace
 
-int pob_sm_count_cached() { return sm_count(); }
+int pob_sms_or_fail(const char* where) {
+  const int n = sm_count();
+  if (n > 0) return n;
+  if (n == -3)
+    pob_fail(where, ("POB_SM_COUNT=\"" + g_sm_count_env + "\" is not an integer from " +
+                     std::to_string(MIN_SPLIT_SMS) + " to the device's " + std::to_string(g_device_sms) + " SMs")
+                        .c_str());
+  else if (n == -2)
+    pob_fail(where, "device is not compute capability 9.0 (sm_90a build)");
+  else
+    pob_fail(where, "no sm_90 CUDA device (there is no CPU fallback)");
+  return 0;
+}
 int pob_check_common(const char* where, const void* packed, int sh_deg, int precision) {
   return check_common(where, packed, sh_deg, precision);
 }
@@ -407,7 +435,7 @@ int pob_draw_uniforms(uint64_t seed, float step, const float* step_dev, float* t
   if (n_t < 0 || n_u < 0 || n_sp < 0) return fail("pob_draw_uniforms", "negative size");
   if ((n_t && !t_rand_dev) || (n_u && !u_dev) || (n_sp && !sp_points_dev))
     return fail("pob_draw_uniforms", "NULL pointer");
-  if (sm_count() <= 0) return fail("pob_draw_uniforms", "no sm_90 CUDA device (there is no CPU fallback)");
+  if (!pob_sms_or_fail("pob_draw_uniforms")) return 1;
   pob_count_launch();
   POB_CUDA("pob_draw_uniforms", pob::launch_draw_uniforms(seed, step, step_dev, t_rand_dev, n_t, u_dev, n_u,
                                                           sp_points_dev, n_sp, sp_radius, (cudaStream_t)stream));

@@ -6,7 +6,8 @@
 
 int pob_fail(const char* where, const char* what);
 int pob_cuda_fail(const char* where, cudaError_t e);
-int pob_sm_count_cached();
+// the SM count the kernels split their work for (capi.cu: sm_count), or 0 with the reason recorded under `where`
+int pob_sms_or_fail(const char* where);
 int pob_check_common(const char* where, const void* packed, int sh_deg, int precision);
 // POB_SIGMA_RELU or POB_SIGMA_SOFTPLUS, else pob_fail
 int pob_check_sigma_activation(const char* where, int sigma_activation);

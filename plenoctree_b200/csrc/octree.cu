@@ -900,7 +900,7 @@ int tree_dev(const char* where, const pob_octree* t, TreeDev& T) {
     T.off[a] = t->offset[a];
     T.inv[a] = t->invradius[a];
   }
-  if (pob_sm_count_cached() <= 0) return pob_fail(where, "no sm_90 CUDA device (there is no CPU fallback)");
+  if (!pob_sms_or_fail(where)) return 1;
   return 0;
 }
 
@@ -941,7 +941,7 @@ int quant_tree_dev(const char* where, const pob_octree_quant* t, QuantTreeDev& T
   T.retain = t->retain;
   T.ncolors = 1 << t->bits;
   T.leaves = (unsigned long long)leaves;
-  if (pob_sm_count_cached() <= 0) return pob_fail(where, "no sm_90 CUDA device (there is no CPU fallback)");
+  if (!pob_sms_or_fail(where)) return 1;
   return 0;
 }
 
@@ -1199,8 +1199,8 @@ int pob_octree_sgd_step(float* data_dev, float* grad_dev, int64_t n, float lr, v
   const char* W = "pob_octree_sgd_step";
   if (!data_dev || !grad_dev) return pob_fail(W, "NULL pointer");
   if (n < 0) return pob_fail(W, "negative size");
-  const int sms = pob_sm_count_cached();
-  if (sms <= 0) return pob_fail(W, "no sm_90 CUDA device (there is no CPU fallback)");
+  const int sms = pob_sms_or_fail(W);
+  if (!sms) return 1;
   if ((reinterpret_cast<uintptr_t>(data_dev) | reinterpret_cast<uintptr_t>(grad_dev)) & 15)
     return pob_fail(W, "data / grad must be 16-byte aligned");
   if (n == 0) return 0;
@@ -1216,8 +1216,8 @@ int pob_octree_sgd_momentum_step(float* data_dev, float* grad_dev, float* buf_de
   if (!data_dev || !grad_dev || !buf_dev) return pob_fail(W, "NULL pointer");
   if (n < 0) return pob_fail(W, "negative size");
   if (!(momentum >= 0.f) || !isfinite(momentum)) return pob_fail(W, "momentum must be finite and >= 0");
-  const int sms = pob_sm_count_cached();
-  if (sms <= 0) return pob_fail(W, "no sm_90 CUDA device (there is no CPU fallback)");
+  const int sms = pob_sms_or_fail(W);
+  if (!sms) return 1;
   if ((reinterpret_cast<uintptr_t>(data_dev) | reinterpret_cast<uintptr_t>(grad_dev) |
        reinterpret_cast<uintptr_t>(buf_dev)) & 15)
     return pob_fail(W, "data / grad / buf must be 16-byte aligned");
@@ -1234,7 +1234,7 @@ int pob_octree_adam_step(float* data_dev, float* grad_dev, float* m_dev, float* 
   const char* W = "pob_octree_adam_step";
   if (!data_dev || !grad_dev || !m_dev || !v_dev) return pob_fail(W, "NULL pointer");
   if (n < 0) return pob_fail(W, "negative size");
-  if (pob_sm_count_cached() <= 0) return pob_fail(W, "no sm_90 CUDA device (there is no CPU fallback)");
+  if (!pob_sms_or_fail(W)) return 1;
   if (n == 0) return 0;
   pob_count_launch();
   POB_CUDA(W, pob::launch_adam(data_dev, grad_dev, m_dev, v_dev, n, lr, step, nullptr, 0.9f, 0.999f, eps, 1.0f,
@@ -1267,7 +1267,7 @@ int pob_grid_weight_render(const float* sigma_grid_dev, int reso, const pob_came
   if (reso < 1 || reso > 2048) return pob_fail(W, "reso must be in [1, 2048]");
   if (n_cams < 0 || n_cams > 65535) return pob_fail(W, "n_cams must be in [0, 65535] per call");
   if (max_width < 1 || max_height < 1) return pob_fail(W, "bad image size");
-  if (pob_sm_count_cached() <= 0) return pob_fail(W, "no sm_90 CUDA device (there is no CPU fallback)");
+  if (!pob_sms_or_fail(W)) return 1;
   if (n_cams == 0) return 0;
   dim3 grid(unsigned(((max_width + 15) / 16) * ((max_height + 15) / 16)), unsigned(n_cams));
   pob_count_launch();

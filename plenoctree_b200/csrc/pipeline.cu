@@ -162,7 +162,8 @@ int forward_levels(const char* where, const pob_render_config& c, Workspace& w, 
                    const float* z_base, const float* t_rand, const float* u, int u_per_ray,
                    const float* z_fine, int precision, bool save, cudaStream_t st,
                    const float* sp_points = nullptr, long long sp_n = 0) {
-  const int sms = pob_sm_count_cached();
+  const int sms = pob_sms_or_fail(where);
+  if (!sms) return 1;
   const int Nc = c.num_coarse_samples, Nf = c.num_fine_samples;
   const NetDesc net = cfg_net(c);
   Level& C = w.lv[0];
@@ -318,7 +319,8 @@ int pob_loss_and_grad_flags(const pob_render_config* cfg, const pob_train_hparam
   if (sparsity && !sp_points_dev) return pob_fail(where, "sparsity term needs sp_points");
   if (!(hp->loss_scale > 0.f)) return pob_fail(where, "loss_scale must be positive");
   cudaStream_t st = (cudaStream_t)stream;
-  const int sms = pob_sm_count_cached();
+  const int sms = pob_sms_or_fail(where);
+  if (!sms) return 1;
   const int K = cfg->sh_deg < 0 ? 1 : (cfg->sh_deg + 1) * (cfg->sh_deg + 1);
   const NetDesc net = cfg_net(*cfg);
   const int W = posenc_width(net.pe);
