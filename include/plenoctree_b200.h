@@ -345,6 +345,25 @@ typedef struct pob_camera {
   float width, height;
 } pob_camera;
 
+/* NDC description of a forward-facing (LLFF) scene, svox NDCConfig(width, height, focal): the training images' size
+ * and focal in pixels (octree/optimization.py:170-174, octree/nerf/utils.py:451-457, octree/extraction.py:187-193).
+ * All three must be finite and > 0. */
+typedef struct pob_ndc {
+  float width, height, focal;
+} pob_ndc;
+
+/* The rays the octree march takes for a forward-facing scene: explicit world rays (origins/dirs/vdirs [n_rays,3],
+ * cam NULL) or the pixel-row slab [row0, row0+nrows) of a perspective camera (cam != NULL, ray pointers ignored; the
+ * pixel rays of pob_octree_render, row-major), turned into NDC as the reference's convert_to_ndc
+ * (nerf_sh/nerf/datasets.py:40-60, near = 1): origin moved onto the plane z = -1, then projected.  out_origins_dev /
+ * out_dirs_dev [n,3] receive the NDC origins and the NDC directions normalised to unit length; out_vdirs_dev [n,3] the
+ * view directions, unchanged (explicit rays) or the pixel's unit world direction (camera), so that SH colours stay a
+ * function of the world direction as in NeRF-SH training.  The outputs feed the explicit-ray entry points below
+ * (render, backward, depth, compressed trees) unchanged. */
+int pob_ndc_rays(const pob_ndc* ndc, const float* origins_dev, const float* dirs_dev, const float* vdirs_dev,
+                 int64_t n_rays, const pob_camera* cam, int row0, int nrows, float* out_origins_dev,
+                 float* out_dirs_dev, float* out_vdirs_dev, void* stream);
+
 /* VolumeRenderer.forward(rays) / render_persp(c2w, width, height, fx): composite the tree along rays.
  * Either explicit rays (origins/dirs/vdirs [n_rays,3], cam NULL) or a pixel-row slab [row0, row0+nrows) of a
  * perspective camera (cam != NULL, ray pointers ignored; out is [nrows*width, 3] row-major).
@@ -428,6 +447,11 @@ int pob_octree_train_persp(const pob_octree* tree, const pob_octree_opts* opts, 
                            int nrows, const float* gt_rgb_dev, float grad_scale, float* grad_data_dev,
                            double* sq_err_sum_dev, float* out_rgb_dev, void* stream);
 
+/* pob_octree_train_persp of a forward-facing scene: each pixel's ray is marched in NDC, as pob_ndc_rays makes it. */
+int pob_octree_train_persp_ndc(const pob_octree* tree, const pob_octree_opts* opts, const pob_camera* cam,
+                               const pob_ndc* ndc, int row0, int nrows, const float* gt_rgb_dev, float grad_scale,
+                               float* grad_data_dev, double* sq_err_sum_dev, float* out_rgb_dev, void* stream);
+
 /* torch.optim.SGD(lr, momentum 0).step() fused with zero_grad (octree/optimization.py:187-189,205-208):
  * data -= lr * grad; grad = 0, touching only entries whose gradient is non-zero. */
 int pob_octree_sgd_step(float* data_dev, float* grad_dev, int64_t n, float lr, void* stream);
@@ -456,6 +480,13 @@ int pob_octree_query(const pob_octree* tree, const float* points_dev, int64_t n,
 int pob_grid_weight_render(const float* sigma_grid_dev, int reso, const pob_camera* cams_dev, int n_cams,
                            int max_width, int max_height, const float offset[3], const float invradius[3],
                            const pob_octree_opts* opts, float* max_weight_dev, uint8_t* hit_dev, void* stream);
+
+/* pob_grid_weight_render of a forward-facing scene (octree/extraction.py:187-193): every pixel's ray is marched
+ * through the grid in NDC, as pob_ndc_rays makes it; offset / invradius map NDC coordinates into the grid. */
+int pob_grid_weight_render_ndc(const float* sigma_grid_dev, int reso, const pob_camera* cams_dev, int n_cams,
+                               int max_width, int max_height, const float offset[3], const float invradius[3],
+                               const pob_octree_opts* opts, const pob_ndc* ndc, float* max_weight_dev,
+                               uint8_t* hit_dev, void* stream);
 
 #ifdef __cplusplus
 }

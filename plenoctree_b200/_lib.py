@@ -76,12 +76,16 @@ SIGNATURES = {
     "pob_octree_render_quant": (_i, [_vp, _vp, _fp, _fp, _fp, _i64, _vp, _i, _i, _fp, _vp, _vp]),
     "pob_octree_render_depth_quant": (_i, [_vp, _vp, _fp, _fp, _fp, _i64, _vp, _i, _i, _fp, _fp, _fp, _vp, _vp]),
     "pob_octree_train_persp": (_i, [_vp, _vp, _vp, _i, _i, _fp, _c.c_float, _fp, _vp, _fp, _vp]),
+    "pob_octree_train_persp_ndc": (_i, [_vp, _vp, _vp, _vp, _i, _i, _fp, _c.c_float, _fp, _vp, _fp, _vp]),
+    "pob_ndc_rays": (_i, [_vp, _fp, _fp, _fp, _i64, _vp, _i, _i, _fp, _fp, _fp, _vp]),
     "pob_octree_sgd_step": (_i, [_fp, _fp, _i64, _c.c_float, _vp]),
     "pob_octree_sgd_momentum_step": (_i, [_fp, _fp, _fp, _i64, _c.c_float, _c.c_float, _i, _vp]),
     "pob_octree_adam_step": (_i, [_fp, _fp, _fp, _fp, _i64, _c.c_float, _c.c_float, _c.c_float, _vp]),
     "pob_octree_query": (_i, [_vp, _fp, _i64, _vp, _vp]),
     "pob_grid_weight_render": (_i, [_fp, _i, _vp, _i, _i, _i, _c.POINTER(_c.c_float), _c.POINTER(_c.c_float),
                                     _vp, _fp, _vp, _vp]),
+    "pob_grid_weight_render_ndc": (_i, [_fp, _i, _vp, _i, _i, _i, _c.POINTER(_c.c_float), _c.POINTER(_c.c_float),
+                                        _vp, _vp, _fp, _vp, _vp]),
 }
 
 
@@ -139,6 +143,11 @@ class OctreeQuant(_c.Structure):
 class OctreeOpts(_c.Structure):
     _fields_ = [("step_size", _c.c_float), ("background_brightness", _c.c_float), ("sigma_thresh", _c.c_float),
                 ("stop_thresh", _c.c_float)]
+
+
+class Ndc(_c.Structure):
+    """pob_ndc: svox NDCConfig(width, height, focal) of a forward-facing scene."""
+    _fields_ = [("width", _c.c_float), ("height", _c.c_float), ("focal", _c.c_float)]
 
 
 class Camera(_c.Structure):

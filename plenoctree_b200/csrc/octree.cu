@@ -109,6 +109,32 @@ __device__ __forceinline__ float cam_ray(const Cam& c, int ix, int iy, float* o,
   return nrm;
 }
 
+// NDC description of a forward-facing (LLFF) scene: the training images' width, height and focal (svox NDCConfig)
+struct Ndc {
+  float width, height, focal;
+};
+
+// svox world2ndc as the reference's convert_to_ndc (nerf_sh/nerf/datasets.py:40-60, near = 1) in its operation order:
+// the origin moves onto the plane z = -1, then the projection; the NDC direction is then normalised for the march.
+// The ray's view direction is not touched: SH colours stay a function of the world direction, as in NeRF-SH training.
+__device__ __forceinline__ void world_to_ndc(const Ndc& n, float* o, float* d) {
+  const float t = -__fadd_rn(1.0f, o[2]) / d[2];
+  float c[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) c[a] = __fadd_rn(o[a], __fmul_rn(t, d[a]));
+  const float sx = -(__fmul_rn(2.0f, n.focal) / n.width), sy = -(__fmul_rn(2.0f, n.focal) / n.height);
+  const float cx = c[0] / c[2], cy = c[1] / c[2];
+  d[0] = __fmul_rn(sx, __fsub_rn(d[0] / d[2], cx));
+  d[1] = __fmul_rn(sy, __fsub_rn(d[1] / d[2], cy));
+  d[2] = -2.0f / c[2];
+  o[0] = __fmul_rn(sx, cx);
+  o[1] = __fmul_rn(sy, cy);
+  o[2] = __fadd_rn(1.0f, 2.0f / c[2]);
+  const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(d[0], d[0]), __fmul_rn(d[1], d[1])), __fmul_rn(d[2], d[2])));
+#pragma unroll
+  for (int a = 0; a < 3; ++a) d[a] = d[a] / nrm;
+}
+
 // transform_coord + _get_delta_scale + unit-cube intersection (svox trace_ray prologue)
 __device__ __forceinline__ void setup_ray(const float* off, const float* inv, const float* ow, const float* dw,
                                           const float* vw, Ray& r) {
@@ -532,10 +558,11 @@ __device__ __forceinline__ void trace_backward(const TreeDev& T, const Opts& O, 
 
 // ---- ray fetch: lane group -> ray index (pixel tiles for the perspective camera) --------------------------
 // zscale (optional) receives the factor from a distance along the ray's direction vector to the reported depth:
-// 1 for explicit rays, the camera-axis factor 1 / |(x, y, -1)| for a perspective pixel.
-template <int G>
+// 1 for explicit rays, the camera-axis factor 1 / |(x, y, -1)| for a perspective pixel.  NDC = true turns a
+// perspective pixel's ray into NDC (world_to_ndc) before the march; its view direction stays the world one.
+template <int G, bool NDC = false>
 __device__ __forceinline__ bool fetch_ray(const RaySrc& S, const TreeDev& T, Ray& r, long long& out_index,
-                                          float* zscale = nullptr) {
+                                          float* zscale = nullptr, const Ndc& ndc = Ndc{}) {
   constexpr int RPB = 256 / G;  // rays per CTA
   const int grp = threadIdx.x / G;
   float o[3], d[3];
@@ -561,7 +588,13 @@ __device__ __forceinline__ bool fetch_ray(const RaySrc& S, const TreeDev& T, Ray
   const int iyl = ty * TH + grp / TW;  // row inside the slab
   if (ix >= W || iyl >= S.nrows) return false;
   const float nrm = cam_ray(S.cam, ix, S.row0 + iyl, o, d);
-  setup_ray(T.off, T.inv, o, d, d, r);
+  if constexpr (NDC) {
+    const float v[3] = {d[0], d[1], d[2]};
+    world_to_ndc(ndc, o, d);
+    setup_ray(T.off, T.inv, o, d, v, r);
+  } else {
+    setup_ray(T.off, T.inv, o, d, d, r);
+  }
   out_index = (long long)iyl * W + ix;
   if (zscale) *zscale = 1.0f / nrm;
   return true;
@@ -661,14 +694,15 @@ __global__ void __launch_bounds__(256) octree_backward_kernel(TreeDev T, Opts O,
 // One training pass over a camera slab (octree/optimization.py:201-207 minus the optimiser):
 //   im = render_persp(c2w); mse = mean((clamp(im,0,1) - gt)^2); mse.backward()
 // g = grad_scale * 2 * (clamp(im) - gt) inside the clamp range, 0 outside (torch.clamp's gradient).
-template <int G, int KPL>
+// NDC = true marches the slab's rays in NDC (fetch_ray<NDC>, svox VolumeRenderer(ndc=...)); ndc is unused otherwise.
+template <int G, int KPL, bool NDC = false>
 __global__ void __launch_bounds__(256) octree_train_kernel(TreeDev T, Opts O, RaySrc S, const float* __restrict__ gt,
                                                            float grad_scale, float* __restrict__ grad_data,
                                                            double* __restrict__ sq_err_sum,
-                                                           float* __restrict__ out_rgb) {
+                                                           float* __restrict__ out_rgb, Ndc ndc) {
   Ray r;
   long long oi;
-  const bool have = fetch_ray<G>(S, T, r, oi);
+  const bool have = fetch_ray<G, NDC>(S, T, r, oi, nullptr, ndc);
   float err = 0.f;
   if (have) {
     const int l = threadIdx.x % G;
@@ -817,10 +851,12 @@ __global__ void octree_query_kernel(TreeDev T, const float* __restrict__ pts, lo
 // svox grid_trace_ray for every pixel of every camera in ONE launch; weights are max-reduced straight into the
 // output grid (the reference keeps a per-camera grid and runs torch.max over 2^27 voxels per camera,
 // octree/extraction.py:199-212).  Weights are >= 0, so the float max is an integer atomicMax on the bit pattern.
+// NDC = true marches every pixel's ray in NDC (octree/extraction.py:187-193, opts.ndc_*); ndc is unused otherwise.
+template <bool NDC = false>
 __global__ void __launch_bounds__(256) grid_weight_kernel(const float* __restrict__ sigma, int reso, const Cam* __restrict__ cams,
                                                           float off0, float off1, float off2, float inv0, float inv1,
                                                           float inv2, Opts O, float* __restrict__ wmax,
-                                                          uint8_t* __restrict__ hit) {
+                                                          uint8_t* __restrict__ hit, Ndc ndc) {
   const Cam c = cams[blockIdx.y];
   const int W = int(c.width), H = int(c.height);
   const int tiles_x = (W + 15) / 16;
@@ -829,6 +865,7 @@ __global__ void __launch_bounds__(256) grid_weight_kernel(const float* __restric
   if (ix >= W || iy >= H) return;
   float o[3], d[3];
   cam_ray(c, ix, iy, o, d);
+  if constexpr (NDC) world_to_ndc(ndc, o, d);
   const float off[3] = {off0, off1, off2}, inv[3] = {inv0, inv1, inv2};
   Ray r;
   setup_ray(off, inv, o, d, d, r);
@@ -862,6 +899,37 @@ __global__ void __launch_bounds__(256) grid_weight_kernel(const float* __restric
       if (light <= O.stop_thresh) return;
     }
     t += delta_t;
+  }
+}
+
+// The NDC rays of explicit world rays (S.o != null: origins / dirs / vdirs) or of a perspective camera's pixel-row
+// slab (row-major, the pixel order of fetch_ray), one thread per ray: origins and unit directions in NDC
+// (world_to_ndc), view directions copied (explicit) or the pixel's unit world direction.  The explicit-ray entry
+// points march them unchanged.
+__global__ void __launch_bounds__(256) ndc_rays_kernel(RaySrc S, Ndc ndc, float* __restrict__ out_o,
+                                                       float* __restrict__ out_d, float* __restrict__ out_v) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= S.n) return;
+  float o[3], d[3], v[3];
+  if (S.o != nullptr) {
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      o[a] = __ldg(S.o + 3 * i + a);
+      d[a] = __ldg(S.d + 3 * i + a);
+      v[a] = __ldg(S.v + 3 * i + a);
+    }
+  } else {
+    const int W = int(S.cam.width);
+    cam_ray(S.cam, int(i % W), S.row0 + int(i / W), o, d);
+#pragma unroll
+    for (int a = 0; a < 3; ++a) v[a] = d[a];
+  }
+  world_to_ndc(ndc, o, d);
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    out_o[3 * i + a] = o[a];
+    out_d[3 * i + a] = d[a];
+    out_v[3 * i + a] = v[a];
   }
 }
 
@@ -955,6 +1023,17 @@ int opts_dev(const char* where, const pob_octree_opts* o, Opts& O) {
   O.bg = o->background_brightness;
   O.sigma_thresh = o->sigma_thresh;
   O.stop_thresh = o->stop_thresh;
+  return 0;
+}
+
+int ndc_dev(const char* where, const pob_ndc* n, Ndc& N) {
+  if (!n) return pob_fail(where, "NDC description is NULL");
+  if (!(n->width > 0.f && n->height > 0.f && n->focal > 0.f) || !isfinite(n->width) || !isfinite(n->height) ||
+      !isfinite(n->focal))
+    return pob_fail(where, "NDC width, height and focal must be finite and > 0");
+  N.width = n->width;
+  N.height = n->height;
+  N.focal = n->focal;
   return 0;
 }
 
@@ -1057,9 +1136,94 @@ int render_quant(const char* W, const pob_octree_quant* tree, const pob_octree_o
   return 0;
 }
 
+// pob_octree_train_persp (ndc NULL) / pob_octree_train_persp_ndc
+int train_persp(const char* W, const pob_octree* tree, const pob_octree_opts* opts, const pob_camera* cam,
+                const pob_ndc* ndc, int row0, int nrows, const float* gt_rgb_dev, float grad_scale,
+                float* grad_data_dev, double* sq_err_sum_dev, float* out_rgb_dev, void* stream) {
+  TreeDev T;
+  Opts O;
+  RaySrc S;
+  Ndc N{};
+  unsigned blocks = 0;
+  if (int rc = tree_dev(W, tree, T)) return rc;
+  if (int rc = opts_dev(W, opts, O)) return rc;
+  if (ndc != nullptr)
+    if (int rc = ndc_dev(W, ndc, N)) return rc;
+  if (!cam) return pob_fail(W, "camera is NULL");
+  if (O.sigma_thresh != 0.f || O.stop_thresh != 0.f)
+    return pob_fail(W, "training renders with sigma_thresh = stop_thresh = 0 (svox fast=False)");
+  const int G = group_width(T.K);
+  if (int rc = ray_src(W, nullptr, nullptr, nullptr, 0, cam, row0, nrows, S, blocks, G)) return rc;
+  if (!gt_rgb_dev || !grad_data_dev) return pob_fail(W, "gt / gradient pointer is NULL");
+  if (blocks == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  pob_count_launch();
+  if (ndc == nullptr) {
+    POB_OCTREE_DISPATCH(octree_train_kernel, G, T.K, T, O, S, gt_rgb_dev, grad_scale, grad_data_dev, sq_err_sum_dev,
+                        out_rgb_dev, N);
+  } else {
+    octree_dispatch(G, T.K, [&](auto g_, auto kpl_) {
+      octree_train_kernel<decltype(g_)::value, decltype(kpl_)::value, true><<<blocks, 256, 0, st>>>(
+          T, O, S, gt_rgb_dev, grad_scale, grad_data_dev, sq_err_sum_dev, out_rgb_dev, N);
+    });
+  }
+  POB_CUDA(W, cudaGetLastError());
+  return 0;
+}
+
+// pob_grid_weight_render (ndc NULL) / pob_grid_weight_render_ndc
+int grid_weights(const char* W, const float* sigma_grid_dev, int reso, const pob_camera* cams_dev, int n_cams,
+                 int max_width, int max_height, const float offset[3], const float invradius[3],
+                 const pob_octree_opts* opts, const pob_ndc* ndc, float* max_weight_dev, uint8_t* hit_dev,
+                 void* stream) {
+  Opts O;
+  Ndc N{};
+  if (int rc = opts_dev(W, opts, O)) return rc;
+  if (ndc != nullptr)
+    if (int rc = ndc_dev(W, ndc, N)) return rc;
+  if (!sigma_grid_dev || !cams_dev || !max_weight_dev) return pob_fail(W, "NULL pointer");
+  if (reso < 1 || reso > 2048) return pob_fail(W, "reso must be in [1, 2048]");
+  if (n_cams < 0 || n_cams > 65535) return pob_fail(W, "n_cams must be in [0, 65535] per call");
+  if (max_width < 1 || max_height < 1) return pob_fail(W, "bad image size");
+  if (!pob_sms_or_fail(W)) return 1;
+  if (n_cams == 0) return 0;
+  dim3 grid(unsigned(((max_width + 15) / 16) * ((max_height + 15) / 16)), unsigned(n_cams));
+  pob_count_launch();
+  const Cam* cams = reinterpret_cast<const Cam*>(cams_dev);
+  if (ndc == nullptr)
+    grid_weight_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(
+        sigma_grid_dev, reso, cams, offset[0], offset[1], offset[2], invradius[0], invradius[1], invradius[2], O,
+        max_weight_dev, hit_dev, N);
+  else
+    grid_weight_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(
+        sigma_grid_dev, reso, cams, offset[0], offset[1], offset[2], invradius[0], invradius[1], invradius[2], O,
+        max_weight_dev, hit_dev, N);
+  POB_CUDA(W, cudaGetLastError());
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
+
+int pob_ndc_rays(const pob_ndc* ndc, const float* origins_dev, const float* dirs_dev, const float* vdirs_dev,
+                 int64_t n_rays, const pob_camera* cam, int row0, int nrows, float* out_origins_dev,
+                 float* out_dirs_dev, float* out_vdirs_dev, void* stream) {
+  const char* W = "pob_ndc_rays";
+  Ndc N;
+  RaySrc S;
+  unsigned tiles = 0;
+  if (int rc = ndc_dev(W, ndc, N)) return rc;
+  if (int rc = ray_src(W, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0, nrows, S, tiles, 4)) return rc;
+  if (!out_origins_dev || !out_dirs_dev || !out_vdirs_dev) return pob_fail(W, "output pointer is NULL");
+  if (!pob_sms_or_fail(W)) return 1;
+  if (S.n == 0) return 0;
+  pob_count_launch();
+  ndc_rays_kernel<<<unsigned((S.n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(S, N, out_origins_dev, out_dirs_dev,
+                                                                                 out_vdirs_dev);
+  POB_CUDA(W, cudaGetLastError());
+  return 0;
+}
 
 int pob_octree_render_quant(const pob_octree_quant* tree, const pob_octree_opts* opts, const float* origins_dev,
                             const float* dirs_dev, const float* vdirs_dev, int64_t n_rays, const pob_camera* cam,
@@ -1173,26 +1337,16 @@ int pob_octree_render_depth_backward(const pob_octree* tree, const pob_octree_op
 int pob_octree_train_persp(const pob_octree* tree, const pob_octree_opts* opts, const pob_camera* cam, int row0,
                            int nrows, const float* gt_rgb_dev, float grad_scale, float* grad_data_dev,
                            double* sq_err_sum_dev, float* out_rgb_dev, void* stream) {
-  const char* W = "pob_octree_train_persp";
-  TreeDev T;
-  Opts O;
-  RaySrc S;
-  unsigned blocks = 0;
-  if (int rc = tree_dev(W, tree, T)) return rc;
-  if (int rc = opts_dev(W, opts, O)) return rc;
-  if (!cam) return pob_fail(W, "camera is NULL");
-  if (O.sigma_thresh != 0.f || O.stop_thresh != 0.f)
-    return pob_fail(W, "training renders with sigma_thresh = stop_thresh = 0 (svox fast=False)");
-  const int G = group_width(T.K);
-  if (int rc = ray_src(W, nullptr, nullptr, nullptr, 0, cam, row0, nrows, S, blocks, G)) return rc;
-  if (!gt_rgb_dev || !grad_data_dev) return pob_fail(W, "gt / gradient pointer is NULL");
-  if (blocks == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  pob_count_launch();
-  POB_OCTREE_DISPATCH(octree_train_kernel, G, T.K, T, O, S, gt_rgb_dev, grad_scale, grad_data_dev, sq_err_sum_dev,
-                      out_rgb_dev);
-  POB_CUDA(W, cudaGetLastError());
-  return 0;
+  return train_persp("pob_octree_train_persp", tree, opts, cam, nullptr, row0, nrows, gt_rgb_dev, grad_scale,
+                     grad_data_dev, sq_err_sum_dev, out_rgb_dev, stream);
+}
+
+int pob_octree_train_persp_ndc(const pob_octree* tree, const pob_octree_opts* opts, const pob_camera* cam,
+                               const pob_ndc* ndc, int row0, int nrows, const float* gt_rgb_dev, float grad_scale,
+                               float* grad_data_dev, double* sq_err_sum_dev, float* out_rgb_dev, void* stream) {
+  if (!ndc) return pob_fail("pob_octree_train_persp_ndc", "NDC description is NULL");
+  return train_persp("pob_octree_train_persp_ndc", tree, opts, cam, ndc, row0, nrows, gt_rgb_dev, grad_scale,
+                     grad_data_dev, sq_err_sum_dev, out_rgb_dev, stream);
 }
 
 int pob_octree_sgd_step(float* data_dev, float* grad_dev, int64_t n, float lr, void* stream) {
@@ -1260,22 +1414,17 @@ int pob_octree_query(const pob_octree* tree, const float* points_dev, int64_t n,
 int pob_grid_weight_render(const float* sigma_grid_dev, int reso, const pob_camera* cams_dev, int n_cams,
                            int max_width, int max_height, const float offset[3], const float invradius[3],
                            const pob_octree_opts* opts, float* max_weight_dev, uint8_t* hit_dev, void* stream) {
-  const char* W = "pob_grid_weight_render";
-  Opts O;
-  if (int rc = opts_dev(W, opts, O)) return rc;
-  if (!sigma_grid_dev || !cams_dev || !max_weight_dev) return pob_fail(W, "NULL pointer");
-  if (reso < 1 || reso > 2048) return pob_fail(W, "reso must be in [1, 2048]");
-  if (n_cams < 0 || n_cams > 65535) return pob_fail(W, "n_cams must be in [0, 65535] per call");
-  if (max_width < 1 || max_height < 1) return pob_fail(W, "bad image size");
-  if (!pob_sms_or_fail(W)) return 1;
-  if (n_cams == 0) return 0;
-  dim3 grid(unsigned(((max_width + 15) / 16) * ((max_height + 15) / 16)), unsigned(n_cams));
-  pob_count_launch();
-  grid_weight_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(
-      sigma_grid_dev, reso, reinterpret_cast<const Cam*>(cams_dev), offset[0], offset[1], offset[2], invradius[0],
-      invradius[1], invradius[2], O, max_weight_dev, hit_dev);
-  POB_CUDA(W, cudaGetLastError());
-  return 0;
+  return grid_weights("pob_grid_weight_render", sigma_grid_dev, reso, cams_dev, n_cams, max_width, max_height, offset,
+                      invradius, opts, nullptr, max_weight_dev, hit_dev, stream);
+}
+
+int pob_grid_weight_render_ndc(const float* sigma_grid_dev, int reso, const pob_camera* cams_dev, int n_cams,
+                               int max_width, int max_height, const float offset[3], const float invradius[3],
+                               const pob_octree_opts* opts, const pob_ndc* ndc, float* max_weight_dev,
+                               uint8_t* hit_dev, void* stream) {
+  if (!ndc) return pob_fail("pob_grid_weight_render_ndc", "NDC description is NULL");
+  return grid_weights("pob_grid_weight_render_ndc", sigma_grid_dev, reso, cams_dev, n_cams, max_width, max_height,
+                      offset, invradius, opts, ndc, max_weight_dev, hit_dev, stream);
 }
 
 }  // extern "C"

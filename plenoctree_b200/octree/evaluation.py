@@ -2,7 +2,11 @@
 octree/nerf/utils.py:448-498): render every test view of a PlenOctree, PSNR / SSIM against the ground truth
 LPIPS is added when its downloaded weights can be found (nerf/lpips.py), else reported as nan.  `--write_disp DIR`
 writes each view's disparity map as `disp_{i:04d}.png`, as nerf_sh.eval does for the NeRF.  `--input` may also be a
-compressed tree written by octree.compression (quantised or --noquant), rendered as stored."""
+compressed tree written by octree.compression (quantised or --noquant), rendered as stored.  Forward-facing scenes
+('llff' in --config, not --spherify) are rendered in NDC (renderer.scene_ndc).  There `--write_disp` writes acc / depth
+with depth a distance along the unit NDC direction, so its maps differ from nerf_sh.eval's for the same model, whose
+depth is the parameter t along the un-normalised NDC direction: by that direction's length per pixel, about 2 near the
+image centre."""
 import os
 
 import numpy as np
@@ -10,7 +14,7 @@ import torch
 
 from ..nerf.utils import compute_psnr, compute_ssim, save_img, write_video
 from .n3tree import load_tree
-from .renderer import VolumeRenderer, disparity
+from .renderer import VolumeRenderer, disparity, scene_ndc
 
 
 def eval_octree(t, dataset, args, want_frames=False, lpips_fn=None, metrics=None, disp_fn=None):
@@ -18,7 +22,8 @@ def eval_octree(t, dataset, args, want_frames=False, lpips_fn=None, metrics=None
     (nerf/lpips.py::load_lpips) the mean LPIPS(gt, render) is left in `metrics["lpips"]`.  With `disp_fn`, each view's
     disparity [H,W,1] (renderer.disparity of the same render's depth and acc) is passed to disp_fn(idx, disp)."""
     w, h, focal = dataset.w, dataset.h, dataset.focal
-    r = VolumeRenderer(t, step_size=args.renderer_step_size)
+    ndc = scene_ndc(args, w, h, focal)
+    r = VolumeRenderer(t, step_size=args.renderer_step_size, **({} if ndc is None else {"ndc": ndc}))
     avg_psnr = avg_ssim = avg_lpips = 0.0
     frames = []
     with torch.no_grad():

@@ -9,8 +9,16 @@
 
 `args` carries the reference's flag names (extraction.py:66-176, octree/nerf/utils.py:60-253); `default_args()`
 returns the reference defaults.  `nerf` is plenoctree_b200.nerf.models.NerfModel; `dataset` needs .w .h .focal
-.camtoworlds [n,4,4] (and .size), like octree/nerf/datasets.py.  Vanilla-NeRF SH projection, SG and NDC/LLFF are
-outside the scope of this path and raise NotImplementedError.
+.camtoworlds [n,4,4] (and .size), like octree/nerf/datasets.py.  Vanilla-NeRF SH projection and SG are outside the
+scope of this path and raise NotImplementedError.
+
+Forward-facing (LLFF) scenes: the tree lives in NDC, where the model was trained, and the weight mask marches the
+training cameras' rays in NDC when renderer.scene_ndc says so ('llff' in --config and not --spherify).  --z_min /
+--z_max drop the grid's z slices outside [z_min, z_max] as the reference does (extraction.py:257-260,298-301).  The
+reference's weight mask cannot take a cropped grid (its reshape to reso^3 fails); here the dropped slices are empty
+space to the weight render: they neither occlude the rest of the grid nor enter the tree.  NDC x and y go past +-1
+wherever a camera sees beyond the frustum of the reference pose, so the box (--radius / --center) must reach that far
+in x and y or the tree leaves that content out (DESIGN.md §8).
 """
 import ctypes
 import os
@@ -22,7 +30,7 @@ import torch
 from .. import _lib, ops
 from .._lib import check, lib, ptr, stream_ptr
 from .n3tree import N3Tree
-from .renderer import camera_array
+from .renderer import camera_array, scene_ndc
 
 
 def default_args(**kw):
@@ -68,10 +76,10 @@ def _grid_sigmas(nerf, reso, offset, scale):
     return torch.cat(parts)
 
 
-def calculate_grid_weights(dataset, sigmas, reso, invradius, offset, step_size=1e-4, cam_chunk=4096):
+def calculate_grid_weights(dataset, sigmas, reso, invradius, offset, step_size=1e-4, cam_chunk=4096, ndc=None):
     """extraction.py:181-214.  One launch marches the rays of every training camera through the grid and keeps the
     per-voxel maximum weight directly (atomic max); the reference renders one weight grid per camera and reduces
-    with torch.max."""
+    with torch.max.  ndc (renderer.NDCConfig): the rays are marched in NDC (extraction.py:187-193)."""
     dev = sigmas.device
     grid = sigmas.reshape(reso, reso, reso).contiguous().float()
     wmax = torch.zeros_like(grid)
@@ -86,10 +94,12 @@ def calculate_grid_weights(dataset, sigmas, reso, invradius, offset, step_size=1
     o.stop_thresh = 0.0
     off = (ctypes.c_float * 3)(*[float(v) for v in offset.detach().cpu().numpy().reshape(3)])
     inv = (ctypes.c_float * 3)(*[float(v) for v in invradius.detach().cpu().numpy().reshape(3)])
+    ndc_args = () if ndc is None else (ctypes.byref(_lib.Ndc(*map(float, ndc))),)
+    fn = lib.pob_grid_weight_render if ndc is None else lib.pob_grid_weight_render_ndc
     for c0 in range(0, cams.shape[0], cam_chunk):
         sub = cams[c0:c0 + cam_chunk].contiguous()
-        check(lib.pob_grid_weight_render(ptr(grid), reso, ptr(sub), sub.shape[0], int(dataset.w), int(dataset.h), off,
-                                         inv, ctypes.byref(o), ptr(wmax), None, stream_ptr()))
+        check(fn(ptr(grid), reso, ptr(sub), sub.shape[0], int(dataset.w), int(dataset.h), off, inv, ctypes.byref(o),
+                 *ndc_args, ptr(wmax), None, stream_ptr()))
     if world > 1:
         import torch.distributed as dist
         dist.all_reduce(wmax, op=dist.ReduceOp.MAX)
@@ -101,26 +111,42 @@ def _axes(reso, offset, scale, dev):
     return [(arr - offset[a]) / scale[a] for a in range(3)]
 
 
+def z_keep(args, zz):
+    """the z slices the grid keeps: zz >= z_min and zz <= z_max, the reference's zz[zz >= args.z_min] / zz[zz <=
+    args.z_max] (extraction.py:257-260,298-301) as a mask over zz [reso]; None when neither flag is set"""
+    z_min, z_max = getattr(args, "z_min", None), getattr(args, "z_max", None)
+    if z_min is None and z_max is None:
+        return None
+    keep = torch.ones_like(zz, dtype=torch.bool)
+    if z_min is not None:
+        keep &= zz >= z_min
+    if z_max is not None:
+        keep &= zz <= z_max
+    return keep
+
+
 def auto_scale(args, center, radius, nerf):
-    """extraction.py:244-286: bounding box of the voxels whose sigma passes scale_alpha_thresh."""
-    if args.z_min is not None or args.z_max is not None:
-        raise NotImplementedError("z_min / z_max (NDC scenes) are outside the scope of this path")
+    """extraction.py:244-286: bounding box of the voxels whose sigma passes scale_alpha_thresh (inside the z crop)."""
     reso = 2 ** args.init_grid_depth
     radius = torch.tensor(radius, dtype=torch.float32)
     center = torch.tensor(center, dtype=torch.float32)
     scale = 0.5 / radius
     offset = 0.5 * (1.0 - center / radius)
     sigmas = _grid_sigmas(nerf, reso, offset.tolist(), scale.tolist())
-    return _bbox_of_dense(sigmas, args.scale_alpha_thresh, reso, offset, scale)
+    keep = z_keep(args, _axes(reso, offset, scale, sigmas.device)[2])
+    return _bbox_of_dense(sigmas, args.scale_alpha_thresh, reso, offset, scale, keep)
 
 
-def _bbox_of_dense(sigmas, alpha_thresh, reso, offset, scale):
+def _bbox_of_dense(sigmas, alpha_thresh, reso, offset, scale, keep=None):
     """centre and half-extent of the box around the voxel centres whose sigma reaches the alpha threshold, grown by
     half a grid step (extraction.py:276-286: the margin is 0.5 / reso in WORLD units, as in the reference).
-    sigmas: [reso^3] x-major; offset / scale: the grid's world -> [0,1]^3 transform (torch float32 [3])."""
+    sigmas: [reso^3] x-major; offset / scale: the grid's world -> [0,1]^3 transform (torch float32 [3]); keep: the z
+    slices of the crop (z_keep) or None."""
     approx_delta = 2.0 / reso
     sigma_thresh = -np.log(1.0 - alpha_thresh) / approx_delta
     mask = (sigmas >= sigma_thresh).reshape(reso, reso, reso)
+    if keep is not None:
+        mask = mask & keep
     xx, yy, zz = _axes(reso, offset.to(sigmas.device), scale.to(sigmas.device), sigmas.device)
     lc, uc = [], []
     for a, ax in enumerate((xx, yy, zz)):
@@ -134,27 +160,28 @@ def _bbox_of_dense(sigmas, alpha_thresh, reso, offset, scale):
 
 def step1(args, tree, nerf, dataset, refine_chunk=2000000):
     """extraction.py:288-353: dense sigma grid -> mask (sigma or weight) -> level-by-level refinement."""
-    if args.z_min is not None or args.z_max is not None:
-        raise NotImplementedError("z_min / z_max (NDC scenes) are outside the scope of this path")
     reso = 2 ** (args.init_grid_depth + 1)
     offset, scale = tree.offset, tree.invradius
     approx_delta = 2.0 / reso
     sigma_thresh = -np.log(1.0 - args.alpha_thresh) / approx_delta
     sigmas = _grid_sigmas(nerf, reso, offset.tolist(), scale.tolist())
+    xx, yy, zz = _axes(reso, offset, scale, tree.device)
+    keep = z_keep(args, zz)
     if args.masking_mode == "sigma":
         mask = sigmas >= sigma_thresh
     elif args.masking_mode == "weight":
+        if keep is not None:            # the cropped slices are not part of the grid: empty space to the rays
+            sigmas = sigmas.reshape(reso, reso, reso).masked_fill(~keep, 0.0).reshape(-1)
         grid_weights = calculate_grid_weights(dataset, sigmas, reso, tree.invradius, tree.offset,
-                                              step_size=args.renderer_step_size)
+                                              step_size=args.renderer_step_size,
+                                              ndc=scene_ndc(args, dataset.w, dataset.h, dataset.focal))
         mask = grid_weights.reshape(-1) >= args.weight_thresh
         del grid_weights
     else:
         raise ValueError
     del sigmas
-    idx = torch.nonzero(mask.reshape(reso, reso, reso))  # x-major order == grid[mask] of the reference
+    grid = grid_points(mask.reshape(reso, reso, reso), keep, xx, yy, zz)
     del mask
-    xx, yy, zz = _axes(reso, offset, scale, tree.device)
-    grid = torch.stack([xx[idx[:, 0]], yy[idx[:, 1]], zz[idx[:, 2]]], dim=1).contiguous()
     for _ in range(args.init_grid_depth - 1):
         tree[grid].refine()
     if grid.shape[0] <= refine_chunk:
@@ -164,6 +191,15 @@ def step1(args, tree, nerf, dataset, refine_chunk=2000000):
             tree[grid[j:j + refine_chunk]].refine()
     assert tree.max_depth == args.init_grid_depth
     return grid
+
+
+def grid_points(mask, keep, xx, yy, zz):
+    """the voxel centres of mask [reso]^3 inside the z crop (keep, or None), in x-major order: grid[mask] of the
+    reference's (cropped) meshgrid"""
+    if keep is not None:
+        mask = mask & keep
+    idx = torch.nonzero(mask)
+    return torch.stack([xx[idx[:, 0]], yy[idx[:, 1]], zz[idx[:, 2]]], dim=1).contiguous()
 
 
 def step2(args, tree, nerf, cells_per_launch=None):

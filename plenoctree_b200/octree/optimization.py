@@ -11,6 +11,7 @@
 Multi-GPU (SURVEY §8e, C5): every image's pixel rows are split over the ranks, each rank scatters into its own
 dense gradient buffer, and the touched rows are exchanged (exchange_gradients: compacted indices + values, all-gathered)
 before the replicated SGD update.  Both optimiser branches of the reference are fused with zero_grad: SGD (`--sgd`, all shipped configs) and Adam (`--nosgd`).
+Forward-facing scenes train in NDC under renderer.scene_ndc's condition, the one extraction and evaluation use.
 """
 import math
 import os
@@ -20,7 +21,7 @@ import numpy as np
 import torch
 
 from .n3tree import N3Tree
-from .renderer import VolumeRenderer
+from .renderer import VolumeRenderer, scene_ndc
 
 
 def default_args(**kw):
@@ -156,7 +157,7 @@ def optimize(args, tree, train_c2w, train_gt, test_c2w, test_gt, focal, log=prin
     if K > 0 and rank == 0:
         vis_dir = render_dir(args.input)
         os.makedirs(vis_dir, exist_ok=True)
-    r = VolumeRenderer(tree, step_size=args.renderer_step_size)
+    r = VolumeRenderer(tree, step_size=args.renderer_step_size, ndc=scene_ndc(args, W, H, focal))
     best_validation_psnr = run_test_step(r, test_c2w, test_gt, H, W, focal, vis_dir, 0, K)
     log(f"** initial val psnr {best_validation_psnr}")
     best_t = None

@@ -3,6 +3,8 @@
     reference call                                                   here
     svox.VolumeRenderer(t, step_size=..., ndc=None)                  VolumeRenderer(tree, step_size, ...)
       octree/optimization.py:174, octree/nerf/utils.py:456
+    svox.VolumeRenderer(t, ..., ndc=svox.NDCConfig(w, h, focal))     VolumeRenderer(tree, ..., ndc=NDCConfig(w, h,
+      forward-facing (LLFF) scenes, octree/optimization.py:170-174    focal)): every call below marches NDC rays
     r.render_persp(c2w, height=H, width=W, fx=focal, fast=False)     render_persp (autograd-aware: the image
       octree/optimization.py:178,202, octree/nerf/utils.py:471        carries a grad_fn that fills tree.data.grad)
     r.forward(rays)  (svox.Rays(origins, dirs, viewdirs))            forward / __call__
@@ -15,7 +17,13 @@
                                                                      render + clamp-MSE gradient + scatter
 
 All arithmetic is in the CUDA library (csrc/octree.cu) behind include/plenoctree_b200.h; torch carries device
-memory, streams and the autograd edge only.  NDC rays (LLFF) are outside the scope of this path.
+memory, streams and the autograd edge only.
+
+NDC (forward-facing scenes): each world ray is turned into NDC as the reference's convert_to_ndc does (near = 1) and
+its direction normalised for the march, while the SH view direction stays the world direction, as the LLFF NeRF-SH
+model was trained.  render_persp and forward build these rays with pob_ndc_rays and march them through the
+explicit-ray entry points (so gradients, depth and compressed trees work as for world rays); train_persp marches them
+inside its fused launch (pob_octree_train_persp_ndc).  Depth is then a distance along the unit NDC direction.
 """
 import collections
 import ctypes
@@ -27,6 +35,19 @@ from .. import _lib
 from .._lib import check, lib, ptr, stream_ptr
 
 Rays = collections.namedtuple("Rays", ("origins", "dirs", "viewdirs"))
+NDCConfig = collections.namedtuple("NDCConfig", ("width", "height", "focal"))     # svox.NDCConfig
+
+
+def scene_ndc(args, width, height, focal):
+    """The NDCConfig the octree CLIs (extraction, optimization, evaluation) march a scene in, or None: a forward-facing
+    LLFF scene, i.e. 'llff' in --config and not --spherify, the condition of the reference's extraction and evaluation
+    (octree/extraction.py:187, octree/nerf/utils.py:451), under which its datasets hand NeRF-SH NDC rays.  The
+    reference's optimization.py:170 tests 'llff' alone, so with --spherify it would optimise in NDC a tree that
+    extraction built and evaluation renders in world space; every CLI here uses the one condition instead.  The
+    background brightness stays svox's default 1.0 in NDC too, as the reference leaves it."""
+    if "llff" in (getattr(args, "config", None) or "") and not getattr(args, "spherify", False):
+        return NDCConfig(int(width), int(height), float(focal))
+    return None
 
 
 def make_camera(c2w, width, height, fx, fy=None):
@@ -123,11 +144,27 @@ def disparity(depth, acc):
 
 class VolumeRenderer:
     def __init__(self, tree, step_size=1e-3, background_brightness=1.0, ndc=None):
-        if ndc is not None:
-            raise NotImplementedError("NDC rays (LLFF) are outside the scope of this path")
         self.tree = tree
         self.step_size = float(step_size)
         self.background_brightness = float(background_brightness)
+        self.ndc = None
+        if ndc is not None:
+            ndc = NDCConfig(*ndc)
+            self.ndc = _lib.Ndc(float(ndc.width), float(ndc.height), float(ndc.focal))
+
+    def _ndc_rays(self, rays, cam, row0, nrows):
+        """pob_ndc_rays: the NDC rays of explicit world rays (cam None) or of a camera's pixel-row slab"""
+        dev = self.tree.device
+        if cam is None:
+            ro, rd, rv = rays
+            n = ro.shape[0]
+            src = (ptr(ro), ptr(rd), ptr(rv), n, None, 0, 0)
+        else:
+            n = nrows * int(cam.width)
+            src = (None, None, None, 0, ctypes.byref(cam), row0, nrows)
+        out = [torch.empty((n, 3), dtype=torch.float32, device=dev) for _ in range(3)]
+        check(lib.pob_ndc_rays(ctypes.byref(self.ndc), *src, *map(ptr, out), stream_ptr()))
+        return tuple(out)
 
     def _opts(self, fast):
         o = _lib.OctreeOpts()
@@ -186,6 +223,8 @@ class VolumeRenderer:
         the segment midpoints z, as the parameter of origin + z * dirs (csrc/octree.cu, trace_forward)."""
         dev = self.tree.device
         r3 = (self._f32(rays.origins, dev), self._f32(rays.dirs, dev), self._f32(rays.viewdirs, dev))
+        if self.ndc is not None:
+            r3 = self._ndc_rays(r3, None, 0, 0)
         return self._render(r3, None, 0, 0, self._opts(fast), counters, return_depth)
 
     __call__ = forward
@@ -198,7 +237,12 @@ class VolumeRenderer:
         1 / |(x, y, -1)|), the quantity disparity() turns into nerf_sh.eval's disparity maps."""
         cam = make_camera(c2w, width, height, fx, fy)
         row0, nrows = (0, int(height)) if rows is None else rows
-        return self._render(None, cam, row0, nrows, self._opts(fast), counters, return_depth)
+        if self.ndc is None:
+            return self._render(None, cam, row0, nrows, self._opts(fast), counters, return_depth)
+        out = self._render(self._ndc_rays(None, cam, row0, nrows), None, 0, 0, self._opts(fast), counters,
+                           return_depth)
+        shape = (nrows, int(width), -1)
+        return tuple(x.reshape(shape) for x in out) if return_depth else out.reshape(shape)
 
     def train_persp(self, c2w, gt, width, height, fx, fy=None, rows=None, want_image=False, sq_err=None):
         """One training image of octree.optimization (octree/optimization.py:201-207) in ONE kernel: render the slab,
@@ -221,6 +265,8 @@ class VolumeRenderer:
         out = torch.empty((nrows, W, 3), dtype=torch.float32, device=tree.device) if want_image else None
         t = tree.c_struct()
         o = self._opts(False)
-        check(lib.pob_octree_train_persp(ctypes.byref(t), ctypes.byref(o), ctypes.byref(cam), row0, nrows, ptr(gt),
-                                         1.0 / float(H * W * 3), ptr(g), ptr(sq_err), ptr(out), stream_ptr()))
+        src = (ctypes.byref(cam),) if self.ndc is None else (ctypes.byref(cam), ctypes.byref(self.ndc))
+        fn = lib.pob_octree_train_persp if self.ndc is None else lib.pob_octree_train_persp_ndc
+        check(fn(ctypes.byref(t), ctypes.byref(o), *src, row0, nrows, ptr(gt), 1.0 / float(H * W * 3), ptr(g),
+                 ptr(sq_err), ptr(out), stream_ptr()))
         return sq_err, out
