@@ -81,13 +81,19 @@ def _tail_ok(buf, n):
     return bool((buf[n:] == CANARY).all())
 
 
-def _raw(blob, sh, pts, prec, want_rgb=True):
-    """pob_eval_points_raw -> (raw_rgb [m, 3K] reference channel-major | None, raw_sigma [m])"""
-    from plenoctree_b200._lib import check, lib, ptr, stream_ptr
+def _raw(blob, sh, pts, prec, want_rgb=True, pe=None, act=0):
+    """pob_eval_points_raw -> (raw_rgb [m, 3K] reference channel-major | None, raw_sigma [m]); pe (encoder) or act
+    (trunk activation, _lib.NET_*) away from the default: pob_eval_points_raw_pe with that descriptor"""
+    from plenoctree_b200._lib import check, lib, posenc_ref, posenc_struct, ptr, stream_ptr
     m, C3 = pts.shape[0], 3 * L.K_of(sh)
     rb = _canary(m * C3) if want_rgb else None
     sb = _canary(m)
-    check(lib.pob_eval_points_raw(ptr(blob), sh, ptr(pts), m, ptr(rb), ptr(sb), prec, stream_ptr()))
+    d = posenc_struct(pe, act)
+    if d is None:
+        check(lib.pob_eval_points_raw(ptr(blob), sh, ptr(pts), m, ptr(rb), ptr(sb), prec, stream_ptr()))
+    else:
+        check(lib.pob_eval_points_raw_pe(ptr(blob), sh, posenc_ref(d), ptr(pts), m, ptr(rb), ptr(sb), prec,
+                                         stream_ptr()))
     torch.cuda.synchronize()
     assert _tail_ok(sb, m) and (rb is None or _tail_ok(rb, m * C3)), ("write past the output", m)
     return (rb[:m * C3].view(torch.float32).view(m, C3) if want_rgb else None), sb[:m].view(torch.float32)
@@ -117,11 +123,16 @@ def _grid(blob, sh, reso, off, sc, x0, nx, ny, nz, prec, want_rgb):
     return (rb[:m * C3].view(torch.float32).view(m, C3) if want_rgb else None), sb[:m].view(torch.float32)
 
 
-def _cells(blob, sh, pts, n_cells, S, prec):
-    from plenoctree_b200._lib import check, lib, ptr, stream_ptr
+def _cells(blob, sh, pts, n_cells, S, prec, pe=None, act=0):
+    from plenoctree_b200._lib import check, lib, posenc_ref, posenc_struct, ptr, stream_ptr
     W = 3 * L.K_of(sh) + 1
     ob = _canary(n_cells * W)
-    check(lib.pob_eval_cells_mean(ptr(blob), sh, ptr(pts), n_cells, S, ptr(ob), prec, stream_ptr()))
+    d = posenc_struct(pe, act)
+    if d is None:
+        check(lib.pob_eval_cells_mean(ptr(blob), sh, ptr(pts), n_cells, S, ptr(ob), prec, stream_ptr()))
+    else:
+        check(lib.pob_eval_cells_mean_pe(ptr(blob), sh, posenc_ref(d), ptr(pts), n_cells, S, ptr(ob), prec,
+                                         stream_ptr()))
     torch.cuda.synchronize()
     assert _tail_ok(ob, n_cells * W), ("write past the output", n_cells, S)
     return ob[:n_cells * W].view(torch.float32).view(n_cells, W)
@@ -135,9 +146,9 @@ def _blob(flat, sh):
 # =====================================================================================================================
 # fp64 references
 # =====================================================================================================================
-def _heads_params(flat, K, dev):
+def _heads_params(flat, K, dev, enc_width=L.ENC_DIM):
     """packed heads weight [256, NH] and bias [NH] (fp32) on dev, and the channel-major index of the 3K rgb columns"""
-    Wh, bh = L.heads_matrix(np.asarray(flat, np.float32), K)
+    Wh, bh = L.heads_matrix(np.asarray(flat, np.float32), K, enc_width)
     cols9 = torch.tensor([L.heads_column(K, o) for o in range(3 * K)], device=dev)
     return torch.from_numpy(Wh).to(dev), torch.from_numpy(bh).to(dev), cols9
 
@@ -168,12 +179,18 @@ def _hilo(w):
 
 class X3Ref:
     """fp64 evaluation of one MLP with the operands the fp16x3 forward represents: weights and biases hi + lo,
-    posenc from the fp32 arguments (x * 2^j exact, + fp32(pi/2) as an fp32 add, fp64 sine), exact ReLU."""
+    posenc of encoder pe from the fp32 arguments (x * 2^j exact, + fp32(pi/2) as an fp32 add, fp64 sine), the trunk
+    activation act in fp64 (relu exact)."""
 
-    def __init__(self, flat, sh, dev):
+    def __init__(self, flat, sh, dev, pe=None, act="relu"):
+        from oracle import posenc_oracle as PO
+        from oracle import net_activation_oracle as NA
+        self.pe = PO.DEFAULT if pe is None else tuple(pe)
+        self.act = NA.activation(act)
+        W = PO.width(self.pe)
         K = self.K = L.K_of(sh)
-        w_off, b_off, _ = L.flat_offsets(K)
-        dims = L.layer_dims(K)
+        w_off, b_off, _ = L.flat_offsets(K, W)
+        dims = L.layer_dims(K, W)
         fl = torch.as_tensor(np.asarray(flat, np.float32)).to(dev)
         self.Whi, self.W, self.B = [], [], []
         for l in range(8):
@@ -182,7 +199,7 @@ class X3Ref:
             self.W.append(hi + lo)
             bhi, blo = _hilo(fl[b_off[l]:b_off[l] + 256])
             self.B.append(bhi + blo)
-        Wh, bh, self.cols9 = _heads_params(flat, K, dev)
+        Wh, bh, self.cols9 = _heads_params(flat, K, dev, W)
         hi, lo = _hilo(Wh)
         self.Wh_hi, self.Wh = hi, hi + lo
         hi, lo = _hilo(bh)
@@ -191,10 +208,8 @@ class X3Ref:
     def __call__(self, x, pert=None):
         """x fp32 [n, 3] -> (packed heads [n, NH], sum |h_7 w| + |b| [n, NH]) in fp64.  pert: one term of the error
         compensation left out (sensitivity guard)."""
-        j = torch.arange(10, device=x.device, dtype=torch.float32)
-        xb = (x[:, None, :] * torch.exp2(j)[None, :, None]).reshape(-1, 30)
-        arg = torch.cat([xb, xb + torch.tensor(np.float32(np.pi / 2), device=x.device)], 1)
-        e = torch.cat([x.double(), torch.sin(arg.double())], 1)
+        from tests.test_posenc import _ref_features
+        e = torch.cat([x.double(), _ref_features(x, self.pe)], 1)
         if pert == "posenc_unit_lo_dropped":        # one 8-column unit of the posenc tile, hi part only
             e = e.clone()
             e[:, 16:24] = e[:, 16:24].half().double()
@@ -209,7 +224,7 @@ class X3Ref:
             if pert == "trunk_slot_hi_hi" and l == 3:          # K-slot 5 of layer 3 evaluated hi * hi only
                 s = slice(160, 192)
                 pre = pre - a[:, s] @ W[s] + a[:, s].half().double() @ self.Whi[3][s]
-            h = pre.clamp_min(0)
+            h = self.act(pre)
             if l == 4:
                 h4 = h
         if pert == "heads_single_pass":

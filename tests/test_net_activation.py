@@ -19,6 +19,7 @@ import torch
 
 from plenoctree_b200 import layouts as L
 from oracle import net_activation_oracle as NA
+from oracle import posenc_oracle as PO
 from tests.test_train import OUT
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -35,6 +36,12 @@ WG_EPS_W_PRODUCTION = 1e-3
 # fp16x3 whole gradient of a softplus trunk against fp64, relative L2 (test_gradient_vs_fp64_oracle): [1.0e-4, against
 # the fp32 oracle's 6.1e-6 and the fp16 step's 5.9e-3]
 SOFTPLUS_X3_REL = 3e-4
+# fp16x3 posenc tile: sines (hi + lo) against fp64 of the kernel's fp32 arguments, beyond lo's representation error, in
+# units of 2^-24; dO's rgb columns (the fp32 product G.rgb * Y_k with the fp32 SH basis, stored in fp16 or hi + lo)
+# beyond the rounding of the stored value, in units of 2^-24 * |G.rgb|.  Measured on an H100 80 GB HBM3 at a 700 W
+# power limit over this file's cases and test_flag_matrix.py's rows, the largest value in brackets.
+SIN_X3_ALLOW = 3.0          # [1.41]
+DO_ALLOW = 6.0              # [2.84 fp16x3, 1.74 fp16]
 
 
 def _record(name, payload):
@@ -302,34 +309,34 @@ def _grad_of_output(act, h):
 
 
 def _act64(act, z):
-    from oracle import nerf_sh_oracle as O
-    return NA.NET_ACTIVATIONS[act](z)
+    return NA.activation(act)(z)
 
 
-def _make_model(case, act, precision=1):
+def _make_model(case, act, precision=1, pe=PO.DEFAULT, sigma_act="relu"):
     from plenoctree_b200.nerf.models import NerfModel
-    from tests.test_train_stages import _params
+    from tests.test_posenc import _gpu_params
     m = NerfModel(sh_deg=case.sh, num_coarse_samples=case.nc, num_fine_samples=case.nf, max_rays=case.R,
-                  sparsity_npoints=case.nsp, net_activation=act)
-    fc, ff = _params(case.sh, case.seed)
+                  sparsity_npoints=case.nsp, net_activation=act, sigma_activation=sigma_act,
+                  white_bkgd=getattr(case, "white", True), min_deg_point=pe[0], max_deg_point=pe[1],
+                  legacy_posenc_order=pe[2])
+    fc, ff = _gpu_params(pe, case.sh, case.seed)
     for f in (fc, ff):
-        _centre_sigma(f, case.sh, act)
+        _centre_sigma(f, case.sh, act, pe)
     m.set_params(np.concatenate([fc, ff]) if case.nf else fc)
     return m
 
 
-def _centre_sigma(flat, sh, act):
+def _centre_sigma(flat, sh, act, pe=PO.DEFAULT):
     """centre every trunk layer's pre-activations and raw sigma over the scene box (each bias minus the mean, raw
     sigma's minus the median), the state a trained network sits in.  With the relu trunk's initial parameters a
     softplus trunk's pre-activations drift up layer by layer (softplus >= 0 adds a common positive part) until raw
     sigma is negative everywhere: an empty scene, a zero gradient."""
-    from oracle import nerf_sh_oracle as O
-    _, b_off, _ = L.flat_offsets(L.K_of(sh))
+    _, b_off, _ = L.flat_offsets(L.K_of(sh), PO.width(pe))
     box = torch.from_numpy(np.random.RandomState(5).uniform(-1.5, 1.5, (4000, 3)).astype(np.float32))
-    f = NA.NET_ACTIVATIONS[act]
+    f = NA.activation(act)
     with torch.no_grad():
-        params = O.unflatten(flat, sh)
-        enc = O.posenc(box)
+        params = PO.unflatten(flat, sh, pe)
+        enc = PO.encode(box, pe)
         h = enc
         for i in range(8):
             z = h @ params[i][0] + params[i][1]
@@ -338,34 +345,71 @@ def _centre_sigma(flat, sh, act):
             h = f(z - torch.from_numpy(shift))
             if i == 4:
                 h = torch.cat([h, enc], -1)
-        _, sig = NA.eval_points_raw(O.unflatten(flat, sh), box, act)
+        _, sig = NA.mlp(PO.unflatten(flat, sh, pe), enc, act)
     flat[b_off[8]] -= np.float32(np.median(sig.numpy()))
 
 
-def _check_level(ws, lv, flat, grad, case, scale, st, act, x3):
-    """saving forward, data gradient and weight gradient of one level, fp16 (x3 False) or fp16x3"""
-    from tests.test_train_stages import _gemm_excess, _ulp16
-    from tests.test_train_x3 import _repr_err, _weights_hilo
+def _sin_excess(e_hi, e_lo, ref, x3):
+    """sine columns against fp64 of the kernel's fp32 arguments.  fp16: beyond one fp16 ulp, in units of SIN_ABS
+    (test_train_stages.py); fp16x3: hi + lo beyond lo's representation error, in units of 2^-24 (|sin| <= 1)"""
+    from tests.test_train_stages import SIN_ABS, _ulp16
+    from tests.test_train_x3 import _repr_err
+    if x3:
+        err = (e_hi.double() + e_lo.double() - ref).abs() - _repr_err(e_lo)
+        return float((err.clamp_min(0) / U24).max())
+    err = (e_hi.double() - ref.half().double()).abs()
+    return float(((err - _ulp16(ref)).clamp_min(0) / SIN_ABS).max())
+
+
+def _sigma_want(sig, onray, sigma_act):
+    """the rgbs epilogue's density from fp64 raw sigma (+ noise): the model's activation on ray rows, relu on the
+    free sparsity rows; and the extra allowance of softplus (test_sigma_activation.py: SP_BAR, SP_FLOOR)"""
+    from tests.test_sigma_activation import SP_BAR, SP_FLOOR, softplus64
+    if sigma_act == "softplus":
+        sp = softplus64(sig)
+        return (torch.where(onray, sp, sig.clamp_min(0)),
+                torch.where(onray, SP_BAR * U24 * sp + SP_FLOOR, torch.zeros_like(sig)))
+    return sig.clamp_min(0), torch.zeros_like(sig)
+
+
+def _check_level(ws, lv, flat, grad, sh, scale, st, act, x3, pe=PO.DEFAULT, sigma_act="relu", call=None, alt=None):
+    """saving forward (posenc tile, trunk, rgbs epilogue), data gradient (dO, dZ) and weight gradient of one level,
+    fp16 (x3 False) or fp16x3, for any encoder pe, trunk activation act and density sigma_act.  call: the rays, free
+    points, noise and ray count of the training call (the posenc tile, rgbs and dO checks need them).  alt: a flag
+    replaced ({"pe", "act", "sigma_act"}): the same stages against the reference of the wrong flag, under guard_*."""
+    from tests.test_train_stages import FWD_ALLOW as FWD16, _sh_basis, _ulp16
+    from tests.test_train_x3 import FWD_ALLOW as FWD3, _repr_err, _split_ok, _weights_hilo
+    from tests.test_posenc import _ref_features
+    alt = alt or {}
     dev = ws.device
-    K = L.K_of(case.sh)
+    K = L.K_of(sh)
     NH = L.heads_width(K)
     C3 = 3 * K
-    w_off, b_off, P = L.flat_offsets(K)
-    dims = L.layer_dims(K)
+    EW = PO.width(pe)
+    relu = act == "relu"
+    fwd_allow = FWD3 if x3 else FWD16
+    w_off, b_off, P = L.flat_offsets(K, EW)
+    dims = L.layer_dims(K, EW)
     if x3:
-        W, B, Wh, bh = _weights_hilo(flat, K, dev)
+        W, B, Wh, bh = _weights_hilo(flat, K, dev, EW)
     else:
         fl = torch.from_numpy(flat).to(dev)
         W = [fl[w_off[l]:w_off[l] + dims[l][0] * 256].view(dims[l][0], 256).half().double() for l in range(8)]
         B = [fl[b_off[l]:b_off[l] + 256].half().double() for l in range(8)]
-        Wh_np, bh_np = L.heads_matrix(flat, K)
+        Wh_np, bh_np = L.heads_matrix(flat, K, EW)
         Wh, bh = (torch.from_numpy(a).to(dev).half().double() for a in (Wh_np, bh_np))
     cols9 = torch.tensor([L.heads_column(K, o) for o in range(C3)], device=dev)
-    M, tiles = lv["M"], lv["tiles"]
+    N, M, Mr, tiles = lv["N"], lv["M"], lv["M_rays"], lv["tiles"]
     view = lambda k: L.workspace_view(ws, lv, k)
-    H, E, DZ, DO = (view(k) for k in ("H", "E", "DZ", "DO"))
+    H, E, DZ, DO, MASK = (view(k) for k in ("H", "E", "DZ", "DO", "mask"))
     if x3:
         Hl, El, DZl, DOl = (view(k) for k in ("H_lo", "E_lo", "DZ_lo", "DO_lo"))
+    if call is not None:
+        o, d, v = (torch.from_numpy(a).to(dev) for a in call["rays"])
+        z = view("z").reshape(-1)
+        rgbs, G = view("rgbs"), view("G")
+        sp = torch.from_numpy(call["sp"]).to(dev) if call["sp"] is not None and M > Mr else None
+        noise = torch.from_numpy(call["noise"]).to(dev).reshape(-1) if call["noise"] is not None else None
     shapes = {**{f"w{l}": (dims[l][0], 256) for l in range(8)}, **{f"b{l}": (256,) for l in range(8)},
               "wh": (256, NH), "bh": (NH,)}
     acc = {k: torch.zeros(s, dtype=torch.float64, device=dev) for k, s in shapes.items()}
@@ -391,11 +435,15 @@ def _check_level(ws, lv, flat, grad, case, scale, st, act, x3):
         err = (got - ref).abs() - rnd - extra
         return float((err.clamp_min(0) / (U24 * amag).clamp_min(1e-300)).max())
 
+    def bits(t):
+        return t.view(torch.int16)
+
     CH = 128
     for t0 in range(0, tiles, CH):
         t1 = min(tiles, t0 + CH)
         r0, r1 = t0 * L.TILE_M, t1 * L.TILE_M
-        real = torch.arange(r0, r1, device=dev) < M
+        s = torch.arange(r0, r1, device=dev)
+        real = s < M
         h_hi = [L.decode_h(H[t0:t1], l) for l in range(8)]
         dz_hi = [L.decode_dz(DZ[t0:t1], l) for l in range(8)]
         nd = 64 * ((NH + 63) // 64)
@@ -406,29 +454,112 @@ def _check_level(ws, lv, flat, grad, case, scale, st, act, x3):
             dz_lo = [L.decode_dz(DZl[t0:t1], l) for l in range(8)]
             do_lo = L.decode_do(DOl[t0:t1])[:, :nd]
             e_lo = L.decode_e(El[t0:t1])
+            st.add("split_violations_e", _split_ok(e_hi, e_lo))
         else:
             h_lo = [torch.zeros_like(x) for x in h_hi]
             dz_lo = [torch.zeros_like(x) for x in dz_hi]
             do_lo, e_lo = torch.zeros_like(do_hi), torch.zeros_like(e_hi)
-        e63 = (e_hi.double() + e_lo.double())[:, :63]
+        eW = (e_hi.double() + e_lo.double())[:, :EW]
         hd = [a.double() + b.double() for a, b in zip(h_hi, h_lo)]
+        # ---- posenc tile: xyz bit-exact, sines against fp64 of the fp32 arguments, pad columns [W, 63) zero, col 63
+        # the constant one (lo 0)
+        st.add("posenc_pad_nonzero_bits", int(((bits(e_hi[:, EW:63]) != 0) | (bits(e_lo[:, EW:63]) != 0)).sum()))
+        st.add("posenc_col63_not_one", int(((e_hi[:, 63] != 1) | (e_lo[:, 63] != 0)).sum()))
+        if call is not None:
+            sc = s.clamp_max(M - 1)                  # load_point clamps the row: padded rows repeat row M-1
+            ray = (sc // N).clamp_max(call["n"] - 1)
+            x = o[ray] + z[sc.clamp_max(Mr - 1)][:, None] * d[ray]
+            if sp is not None:
+                x = torch.where((sc >= Mr)[:, None], sp[(sc - Mr).clamp_min(0)], x)
+            xh = x.half()
+            st.add("posenc_xyz_bit_mismatches", int((bits(e_hi[:, :3]) != bits(xh)).sum()))
+            if x3:
+                st.add("posenc_xyz_bit_mismatches", int((bits(e_lo[:, :3]) != bits((x - xh.float()).half())).sum()))
+            if EW > 3:
+                st.max("posenc_sin_excess", _sin_excess(e_hi[:, 3:EW], e_lo[:, 3:EW], _ref_features(x, pe), x3))
+                if "pe" in alt:
+                    st.max("guard_posenc_sin", _sin_excess(e_hi[:, 3:EW], e_lo[:, 3:EW],
+                                                           _ref_features(x, alt["pe"]), x3))
         # ---- forward: h_l = f(pre) within the rounding of the stored value + f's fp32 bound + the GEMM allowance
+        mask = [L.decode_mask(MASK[l, r0:r1]) for l in range(8)] if relu else None
         for l in range(8):
-            a = e63 if l == 0 else (torch.cat([hd[4], e63], 1) if l == 5 else hd[l - 1])
+            a = eW if l == 0 else (torch.cat([hd[4], eW], 1) if l == 5 else hd[l - 1])
             pre = a @ W[l] + B[l]
             amag = a.abs() @ W[l].abs() + B[l].abs()
             ref = _act64(act, pre)
-            st.max("fwd_excess", excess(l, h_hi[l], h_lo[l], ref, amag, ACT_BOUND * U24 * ref.abs()))
+            st.max("fwd_excess", excess(l, h_hi[l], h_lo[l], ref, amag, 0.0 if relu else ACT_BOUND * U24 * ref.abs()))
+            if "act" in alt:
+                alt_ref = _act64(alt["act"], pre)
+                st.max(f"guard_fwd_l{l}", excess(l, h_hi[l], h_lo[l], alt_ref, amag,
+                                                 0.0 if alt["act"] == "relu" else ACT_BOUND * U24 * alt_ref.abs()))
             st.add("h_nonfinite", int((~torch.isfinite(hd[l])).sum()))
             st.max("pre_min", float(pre[real].min()))
             st.max("pre_max_neg", -float(pre[real].max()))
-        # ---- data gradient: dZ_l = dH_l * f'(h_l) with f' from the kernel's own saved h_l
+            if relu and x3:
+                pos = hd[l] > 0
+                st.add("mask_clear_but_positive", int((pos & ~mask[l]).sum()))
+                st.add("mask_set_value_zero_not_tiny", int((mask[l] & ~pos & (pre > 2.0 ** -20)).sum()))
+            elif relu:
+                st.add("mask_mismatches", int((mask[l] != (h_hi[l] != 0)).sum()))
+        # ---- rgbs epilogue: density activation (+ noise) on ray rows, relu on sparsity rows, sigmoid of the SH sum
+        if call is not None:
+            heads = hd[7] @ Wh + bh
+            hmag = hd[7].abs() @ Wh.abs() + bh.abs()
+            rr = s[real]
+            onray = rr < Mr
+            got = rgbs[r0:r0 + rr.numel()].double()
+            sig = heads[real, 0]
+            sig_tol = fwd_allow * U24 * hmag[real, 0]
+            if noise is not None:
+                sig = sig + torch.where(onray, noise[rr.clamp_max(Mr - 1)].double(), torch.zeros_like(sig))
+                sig_tol = sig_tol + U24 * sig.abs()
+            want, extra = _sigma_want(sig, onray, sigma_act)
+            st.max("rgbs_sigma_excess", ((got[:, 3] - want).abs() / (sig_tol + extra).clamp_min(1e-300)).max())
+            if "sigma_act" in alt:
+                want, extra = _sigma_want(sig, onray, alt["sigma_act"])
+                st.max("guard_rgbs_sigma", ((got[:, 3] - want).abs() / (sig_tol + extra).clamp_min(1e-300)).max())
+            if onray.any():
+                Y = _sh_basis(sh, v[rr[onray] // N].double()) if sh >= 0 else \
+                    torch.ones(int(onray.sum()), 1, dtype=torch.float64, device=dev)
+                hr = heads[real][onray][:, 1:1 + C3].view(-1, K, 3)
+                hm = hmag[real][onray][:, 1:1 + C3].view(-1, K, 3)
+                prer = (Y[:, :, None] * hr).sum(1)
+                tol = 0.25 * ((Y.abs()[:, :, None] * (fwd_allow * U24 * hm + 4 * U24 * hr.abs())).sum(1)) + 2 ** -21
+                st.max("rgbs_rgb_excess", ((got[onray, :3] - torch.sigmoid(prer)).abs() / tol).max())
+            # ---- dO: G.w in column 0, G.rgb x SH basis in the heads columns, zero on free / padded rows and pads
+            g = torch.zeros(r1 - r0, 4, dtype=torch.float32, device=dev)
+            g[:int(real.sum())] = G[r0:r0 + int(real.sum())]
+            gh = g[:, 3].half()
+            st.add("dO_sigma_bit_mismatches", int((bits(do_hi[:, 0]) != bits(gh)).sum()))
+            if x3:
+                st.add("dO_sigma_bit_mismatches", int((bits(do_lo[:, 0]) != bits((g[:, 3] - gh.float()).half())).sum()))
+            ray_rows = s < Mr
+            Yall = torch.zeros(r1 - r0, K, dtype=torch.float64, device=dev)
+            if ray_rows.any():
+                Yall[ray_rows] = (_sh_basis(sh, v[s[ray_rows] // N].double()) if sh >= 0 else 1.0)
+            ref_do = (g[:, None, :3].double() * Yall[:, :, None]).reshape(-1, C3)
+            got_do = do_hi[:, 1:1 + C3].double() + do_lo[:, 1:1 + C3].double()
+            # beyond the rounding of the stored value, in units of 2^-24 * |G.rgb|: the fp32 SH basis cancels (e.g.
+            # 2zz - xx - yy), so its error is absolute, on the scale of |G.rgb|, not relative to G.rgb * Y_k
+            if x3:
+                rnd = _repr_err(do_lo[:, 1:1 + C3])
+            else:
+                big = torch.maximum(ref_do.abs(), got_do.abs())
+                rnd = torch.where(big < 2.0 ** -14, U24, 0.5 * _ulp16(big))
+            gmag = g[:, None, :3].double().abs().expand(-1, K, 3).reshape(-1, C3)
+            err = (got_do - ref_do).abs() - rnd
+            st.max("dO_rgb_excess", (err.clamp_min(0) / (U24 * gmag).clamp_min(1e-300)).max())
+            nzr = (do_hi != 0) | (do_lo != 0)
+            st.add("dO_free_or_padded_rgb_nonzero", int(nzr[~ray_rows, 1:1 + C3].sum()))
+            st.add("dO_padded_sigma_nonzero", int(nzr[~real, 0].sum()))
+            st.add("dO_pad_columns_nonzero", int(nzr[:, 1 + C3:nd].sum()))
+        # ---- data gradient: dZ_l = dH_l * f'(h_l) with f' from the kernel's own saved h_l (relu: its mask words)
         dod = (do_hi.double() + do_lo.double())[:, :NH]
         dzd = [a.double() + b.double() for a, b in zip(dz_hi, dz_lo)]
         for l in range(7, -1, -1):
             a, Wt = (dod, Wh.T) if l == 7 else (dzd[l + 1], W[l + 1][:256].T)
             dh = a @ Wt
-            gp = _grad_of_output(act, hd[l])
+            gp = mask[l].double() if relu else _grad_of_output(act, hd[l])
             ref = dh * gp
             amag = (a.abs() @ Wt.abs()) * gp.abs()
             if x3:
@@ -436,18 +567,23 @@ def _check_level(ws, lv, flat, grad, case, scale, st, act, x3):
                 normal = ~sub_row.expand_as(ref)
                 ref_n = torch.where(normal, ref, dzd[l])
             else:
-                ref_n = ref
+                normal, ref_n = None, ref
             st.max("bwd_excess", excess(l, dz_hi[l], dz_lo[l], ref_n, amag, 0.0))
-            # mutation: the relu mask of h_l in place of f'(h_l)
-            mut = dh * (hd[l] > 0).double()
-            st.min("bwd_excess_relu_mask_mutation", excess(l, dz_hi[l], dz_lo[l], mut, amag, 0.0))
+            if "act" in alt:
+                gpa = _grad_of_output(alt["act"], hd[l])
+                mut = dh * gpa
+                st.max(f"guard_bwd_l{l}", excess(l, dz_hi[l], dz_lo[l], mut, (a.abs() @ Wt.abs()) * gpa.abs(), 0.0))
+            if not relu:
+                # mutation: the relu mask of h_l in place of f'(h_l)
+                mut = dh * (hd[l] > 0).double()
+                st.min("bwd_excess_relu_mask_mutation", excess(l, dz_hi[l], dz_lo[l], mut, amag, 0.0))
             st.add("dz_nonfinite", int((~torch.isfinite(dzd[l])).sum()))
-            st.add("dz_padded_nonzero", int((dz_hi[l][~real] != 0).sum()))
+            st.add("dz_padded_nonzero", int(((dz_hi[l][~real] != 0) | (dz_lo[l][~real] != 0)).sum()))
             st.max("dz_headroom", float(dz_hi[l].abs().max()) / 65504.0)
         # ---- weight-gradient sums
         for l in range(1, 8):
-            wsum(f"w{l}", hd[l - 1] if l != 5 else torch.cat([hd[4], e63], 1), dzd[l])
-        wsum("w0", e63, dzd[0])
+            wsum(f"w{l}", hd[l - 1] if l != 5 else torch.cat([hd[4], eW], 1), dzd[l])
+        wsum("w0", eW, dzd[0])
         for l in range(8):
             wsum(f"b{l}", dzd[l], None)
         wsum("wh", hd[7], dod)
@@ -491,38 +627,64 @@ class _Stats:
         self.d[key] = self.d.get(key, 0) + int(val)
 
 
-def _stage_case(case, act, precision, wg_w_bar=None):
+def _check_call(model, state, ctx, precision, act, pe=PO.DEFAULT, sigma_act="relu", alt=None):
+    """_check_level on every level of the training call in the model's workspace -> {MLP_i: stages}"""
     from plenoctree_b200.nerf.train import default_loss_scale
-    from tests import test_train_stages as TS, test_train_x3 as TX
-    x3 = precision == X3
-    model = _make_model(case, act)
-    state, ctx = TX._run(case, model, precision, fill=0xFF)
     ws = model.workspace(True, precision)
-    views = L.train_workspace_views(model.cfg, ctx["n"], case.nsp > 0, precision=precision)
+    views = L.train_workspace_views(model.cfg, ctx["n"], ctx["sp"] is not None, precision=precision)
     assert views["total"] == ws.numel()
-    scale = default_loss_scale(ctx["n"], X3) if x3 else default_loss_scale(ctx["n"])
+    scale = default_loss_scale(ctx["n"], precision)
     params = model.params.cpu().numpy()
+    P = model.P
+    noise = ctx.get("noise")
     res = {}
     for i, lv in enumerate(views["levels"]):
         s = _Stats()
-        P = model.P
-        _check_level(ws, lv, params[i * P:(i + 1) * P], state.grads[i * P:(i + 1) * P], case, scale, s, act, x3)
+        last = i == len(views["levels"]) - 1
+        call = dict(rays=ctx["rays"], n=ctx["n"], sp=ctx["sp"] if last else None,
+                    noise=noise[i] if noise is not None else None)
+        _check_level(ws, lv, params[i * P:(i + 1) * P], state.grads[i * P:(i + 1) * P], model.sh_deg, scale, s, act,
+                     precision == X3, pe, sigma_act, call, alt)
         res[f"MLP_{i}"] = dict(stages=s.d, M=lv["M"], tiles=lv["tiles"])
-    _record(f"stages_{act}_{'fp16x3' if x3 else 'fp16'}_{case.name}", res)
+    return res
+
+
+def _assert_call(res, precision, act, wg_w_bar=None):
+    from tests import test_train_stages as TS, test_train_x3 as TX
+    x3 = precision == X3
     fwd_allow, bwd_allow = (TX.FWD_ALLOW, TX.BWD_ALLOW) if x3 else (TS.FWD_ALLOW, TS.BWD_ALLOW)
     wg_w, wg_b = (TX.WG_EPS_W, TX.WG_EPS_B) if x3 else (TS.WG_EPS_W, TS.WG_EPS_B)
     wg_w = wg_w_bar or wg_w
+    zero = ["h_nonfinite", "dz_nonfinite", "dz_padded_nonzero", "posenc_xyz_bit_mismatches", "posenc_pad_nonzero_bits",
+            "posenc_col63_not_one", "dO_sigma_bit_mismatches", "dO_free_or_padded_rgb_nonzero",
+            "dO_padded_sigma_nonzero", "dO_pad_columns_nonzero"]
+    if x3:
+        zero.append("split_violations_e")
+    if act == "relu":
+        zero += ["mask_clear_but_positive", "mask_set_value_zero_not_tiny"] if x3 else ["mask_mismatches"]
     for mlp, r in res.items():
         s = r["stages"]
-        for k in ("h_nonfinite", "dz_nonfinite", "dz_padded_nonzero"):
-            assert s[k] == 0, (mlp, k, s[k])
+        for k in zero:
+            assert s[k] == 0, (act, mlp, k, s[k])
+        assert s.get("posenc_sin_excess", 0.0) <= (SIN_X3_ALLOW if x3 else 1.0), (act, mlp, s)
         assert s["fwd_excess"] <= fwd_allow, (act, mlp, s)
+        assert s["rgbs_sigma_excess"] <= 1.0 and s.get("rgbs_rgb_excess", 0.0) <= 1.0, (act, mlp, s)
+        assert s["dO_rgb_excess"] <= DO_ALLOW, (act, mlp, s)
         assert s["bwd_excess"] <= bwd_allow, (act, mlp, s)
         assert s["dz_headroom"] < 1.0, (mlp, s)
         assert s["wgrad_w_max_err_over_abs_sum"] <= wg_w, (act, mlp, s)
         assert s["wgrad_b_max_err_over_abs_sum"] <= wg_b, (act, mlp, s)
         if not x3:
             assert s["wgrad_w_rel_l2"] <= TS.WG_EPS2_W and s["wgrad_b_rel_l2"] <= TS.WG_EPS2_B, (act, mlp, s)
+
+
+def _stage_case(case, act, precision, wg_w_bar=None):
+    from tests import test_train_x3 as TX
+    model = _make_model(case, act)
+    state, ctx = TX._run(case, model, precision, fill=0xFF)
+    res = _check_call(model, state, ctx, precision, act)
+    _record(f"stages_{act}_{'fp16x3' if precision == X3 else 'fp16'}_{case.name}", res)
+    _assert_call(res, precision, act, wg_w_bar)
     return res
 
 

@@ -813,7 +813,16 @@ def _check_levels(model, views, ws, rays, z_base, t_rand, u, upr, st, px=None, g
         r = check_composite(f, comp, disp, acc, w)
         if px is not None:
             G = L.workspace_view(ws, lv, "G")[:Mr].view(n, N, 4)
-            b = composite_bwd_ref(f, comp, torch.from_numpy(px).to(dev), gscale)
+            if model.sigma_activation == "softplus":
+                # d sigma / d raw sigma = sigmoid(raw) = -expm1(-sigma) in G.w (test_sigma_activation.py: GW_SP_EXTRA)
+                from tests.test_sigma_activation import GW_SP_EXTRA
+                fac = f["delta"] * f["a"] * (-torch.expm1(-rgbs[..., 3].double()))
+                b = composite_bwd_ref(f, comp, torch.from_numpy(px).to(dev), gscale, factor=fac)
+                b["mag_gw"] = b["mag_gw"] + GW_SP_EXTRA * b["Gw"].abs()
+                b_relu = composite_bwd_ref(f, comp, torch.from_numpy(px).to(dev), gscale)
+                r["relu_factor_guard"] = float(_norm((b_relu["Gw"] - b["Gw"]).abs(), b["mag_gw"]).max())
+            else:
+                b = composite_bwd_ref(f, comp, torch.from_numpy(px).to(dev), gscale)
             r.update(check_composite_bwd(b, G))
             r["sq64"] = float(b["sq"])
         res[f"level{i}"] = r
@@ -821,12 +830,17 @@ def _check_levels(model, views, ws, rays, z_base, t_rand, u, upr, st, px=None, g
 
 
 def _in_call(case):
-    from plenoctree_b200 import layouts as L
-    from plenoctree_b200.nerf.train import default_loss_scale
     from tests.test_train_x3 import _run
     model = case.model()
     n = case.n_call or case.R
-    state, ctx = _run(case, model, case.precision, n=n, fill=0xFF)
+    state, _ = _run(case, model, case.precision, n=n, fill=0xFF)
+    return _in_call_checks(case, model, state, n)
+
+
+def _in_call_checks(case, model, state, n):
+    """the ray-stage checks of a training call over n rays of `case` already in the model's workspace"""
+    from plenoctree_b200 import layouts as L
+    from plenoctree_b200.nerf.train import default_loss_scale
     (o, d, v, px), t_rand, u, sp, _ = case.inputs(n)
     ws = model.workspace(True, case.precision)
     views = L.train_workspace_views(model.cfg, n, case.nsp > 0, precision=case.precision)

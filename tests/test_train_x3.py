@@ -186,15 +186,15 @@ def _split_ok(hi, lo):
     return int(((lo.double().abs() > 0.5 * _ulp16(hi.double()) * (hi != 0)) | ((hi == 0) & (lo != 0))).sum())
 
 
-def _weights_hilo(flat, K, dev):
+def _weights_hilo(flat, K, dev, enc_width=L.ENC_DIM):
     """fp64 hi + lo of every operand pack_weights / pack_wt_lo make: W[l] [in, 256], B[l], Wh [256, NH], bh [NH]"""
-    w_off, b_off, _ = L.flat_offsets(K)
-    dims = L.layer_dims(K)
+    w_off, b_off, _ = L.flat_offsets(K, enc_width)
+    dims = L.layer_dims(K, enc_width)
     fl = torch.from_numpy(flat).to(dev)
     hl = lambda x: x.half().double() + (x - x.half().float()).half().double()
     W = [hl(fl[w_off[l]:w_off[l] + dims[l][0] * 256].view(dims[l][0], 256)) for l in range(8)]
     B = [hl(fl[b_off[l]:b_off[l] + 256]) for l in range(8)]
-    Wh_np, bh_np = L.heads_matrix(flat, K)
+    Wh_np, bh_np = L.heads_matrix(flat, K, enc_width)
     return W, B, hl(torch.from_numpy(Wh_np).to(dev)), hl(torch.from_numpy(bh_np).to(dev))
 
 
