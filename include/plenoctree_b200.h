@@ -488,6 +488,47 @@ int pob_grid_weight_render_ndc(const float* sigma_grid_dev, int reso, const pob_
                                const pob_octree_opts* opts, const pob_ndc* ndc, float* max_weight_dev,
                                uint8_t* hit_dev, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * SH projection of a vanilla NeRF (use_viewdirs) in octree.extraction step2 (octree/extraction.py:217-241,362-394,
+ * octree/nerf/sh_proj.py:273-306): coeff[p, c, k] = 4 pi / D * sum_d raw_rgb[p, d, c] Y_k(d) over D directions drawn
+ * uniformly on the sphere, Y_k the SH basis of the octree march (sh_basis), the leaf value the mean over its samples.
+ * The view branch raw_rgb = W11 relu(W10 [W9 h7 + b9; posenc(d)] + b10) + b11 is split as
+ *   a_p = W10_b (W9 h7 + b9) + b10   (per sample point, 128 values; W10_b = Dense_10 kernel rows [0, 256))
+ *   t_d = W10_e posenc(d, 0, deg_view, legacy_order)   (per direction; W10_e = rows [256, 256 + 3 + 6 deg_view))
+ * so that raw_rgb[p, d] = W11 relu(a_p + t_d) + b11.  All arithmetic is fp32.
+ * ------------------------------------------------------------------------------------------- */
+/* The point stage in one trunk pass: raw sigma and a_p of m points.  packed_dev is the plain-RGB (sh_deg -1) blob of
+ * the vanilla trunk and Dense_8 (rgb columns zero) packed with `posenc` (NULL = default; net_activation must be relu);
+ * the fp16 forward evaluates it once, writes raw sigma_dev [m] (the value pob_eval_points_raw gives for that blob) and
+ * keeps h7, the trunk's last activation, as fp16 in the workspace; then a_dev [m, 128] = h7 head_w + head_b in fp32
+ * with head_w_dev [256, 128] = W9 W10_b and head_b_dev [128] = b9 W10_b + b10 (Dense_9 has no activation).
+ * workspace_dev: pob_sh_proj_points_workspace_bytes(m) bytes (-1 for m < 0). */
+int64_t pob_sh_proj_points_workspace_bytes(int64_t m);
+int pob_sh_proj_points(const void* packed_dev, const pob_posenc* posenc, const float* points_dev, int64_t m,
+                       const float* head_w_dev, const float* head_b_dev, void* workspace_dev, float* a_dev,
+                       float* sigma_dev, void* stream);
+/* The direction sets of table blocks block0 .. block0 + n_blocks - 1, n_dirs directions each: direction d of block b
+ * is theta = acos(2u - 1), phi = 2 pi v, (sin theta cos phi, sin theta sin phi, cos theta) with (u, v) uniform in
+ * [0, 1) from Philox4x32-10 keyed by `seed`, counter (d, b, stream 0x5348).  A block's set depends on (seed, b) only.
+ *   w10e_dev  [3 + 6 deg_view, 128] fp32, W10_e as stored (kernel [in, out]);
+ *   dirs_dev  [n_blocks, n_dirs, 3] (may be NULL);  t_dev [n_blocks, 128, n_dirs] = W10_e posenc(d) (stored
+ *   direction-minor);  basis_dev [n_blocks, n_dirs, (sh_deg + 1)^2] = Y_k(d).
+ * 0 <= n_blocks <= 65535, 0 <= deg_view <= 32, legacy_order 0 / 1 (the posenc feature order of pob_posenc),
+ * 0 <= sh_deg <= 4. */
+int pob_sh_proj_directions(uint64_t seed, int64_t block0, int n_blocks, int n_dirs, int deg_view, int legacy_order,
+                           int sh_deg, const float* w10e_dev, float* dirs_dev, float* t_dev, float* basis_dev,
+                           void* stream);
+/* Leaf rows of a projected tree.  Cell i (of n_cells) owns sample points [i S, (i + 1) S) (S = samples_per_cell) and
+ * uses direction set i / cells_per_block of the tables (pob_sh_proj_directions with the same n_dirs and sh_deg, at
+ * least ceil(n_cells / cells_per_block) blocks).
+ *   a_dev [n_cells * S, 128] = a_p;  sigma_dev [n_cells * S] raw sigma;  w11_dev [128, 3] (Dense_11 kernel), b11_dev [3]
+ *   out_dev [n_cells, 3K + 1], K = (sh_deg + 1)^2: mean over the cell's points of [coeff (channel-major c K + k),
+ *   raw sigma] (octree/extraction.py:391-393).
+ * Every sum runs in a fixed order: a cell's row depends only on its points and its direction set. */
+int pob_sh_proj_cells(int64_t n_cells, int samples_per_cell, int cells_per_block, const float* a_dev,
+                      const float* sigma_dev, int n_dirs, int sh_deg, const float* t_dev, const float* basis_dev,
+                      const float* w11_dev, const float* b11_dev, float* out_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -86,6 +86,10 @@ SIGNATURES = {
                                     _vp, _fp, _vp, _vp]),
     "pob_grid_weight_render_ndc": (_i, [_fp, _i, _vp, _i, _i, _i, _c.POINTER(_c.c_float), _c.POINTER(_c.c_float),
                                         _vp, _vp, _fp, _vp, _vp]),
+    "pob_sh_proj_points_workspace_bytes": (_i64, [_i64]),
+    "pob_sh_proj_points": (_i, [_vp, _vp, _fp, _i64, _fp, _fp, _vp, _fp, _fp, _vp]),
+    "pob_sh_proj_directions": (_i, [_c.c_uint64, _i64, _i, _i, _i, _i, _i, _fp, _fp, _fp, _fp, _vp]),
+    "pob_sh_proj_cells": (_i, [_i64, _i, _i, _fp, _fp, _i, _i, _fp, _fp, _fp, _fp, _fp, _vp]),
 }
 
 

@@ -492,4 +492,20 @@ __device__ __forceinline__ void sh_basis(int deg, float x, float y, float z, flo
   }
 }
 
+// Philox4x32-10 (Salmon et al., SC'11): the counter-based generator of pob_draw_uniforms and of the SH projection's
+// direction draws.
+__device__ __forceinline__ uint4 philox4x32_10(uint4 ctr, uint2 key) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const uint32_t hi0 = __umulhi(0xD2511F53u, ctr.x), lo0 = 0xD2511F53u * ctr.x;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, ctr.z), lo1 = 0xCD9E8D57u * ctr.z;
+    ctr = make_uint4(hi1 ^ ctr.y ^ key.x, lo1, hi0 ^ ctr.w ^ key.y, lo0);
+    key.x += 0x9E3779B9u;
+    key.y += 0xBB67AE85u;
+  }
+  return ctr;
+}
+// 24 random bits -> [0, 1): never 1, like random.uniform
+__device__ __forceinline__ float u01(uint32_t x) { return float(x >> 8) * (1.0f / 16777216.0f); }
+
 }  // namespace pob

@@ -458,20 +458,6 @@ __global__ void sparsity_grad_kernel(const float4* __restrict__ rgbs, int n, flo
 // Philox4x32-10 (Salmon et al., SC'11), counter = (element / 4, stream id, step), key = seed: one launch replaces
 // the seven ATen launches (3 x rand + scale / shift) of a step.  The reference draws from jax.random's threefry
 // streams, which cannot be reproduced without JAX; parity tests inject their draws instead (SURVEY.md 7.2 RNG).
-__device__ __forceinline__ uint4 philox4x32_10(uint4 ctr, uint2 key) {
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    const uint32_t hi0 = __umulhi(0xD2511F53u, ctr.x), lo0 = 0xD2511F53u * ctr.x;
-    const uint32_t hi1 = __umulhi(0xCD9E8D57u, ctr.z), lo1 = 0xCD9E8D57u * ctr.z;
-    ctr = make_uint4(hi1 ^ ctr.y ^ key.x, lo1, hi0 ^ ctr.w ^ key.y, lo0);
-    key.x += 0x9E3779B9u;
-    key.y += 0xBB67AE85u;
-  }
-  return ctr;
-}
-// 24 random bits -> [0, 1): never 1, like random.uniform
-__device__ __forceinline__ float u01(uint32_t x) { return float(x >> 8) * (1.0f / 16777216.0f); }
-
 __global__ void draw_uniforms_kernel(unsigned long long seed, float step_host, const float* __restrict__ step_dev,
                                      float* __restrict__ t_rand, long long n_t, float* __restrict__ u, long long n_u,
                                      float* __restrict__ sp, long long n_sp, float sp_radius) {

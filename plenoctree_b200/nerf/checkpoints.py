@@ -276,3 +276,97 @@ def restore_model_state_from_jaxnerf(train_dir, model):
         return None
     model.set_params(flax_params_to_flat(sd["optimizer"]["target"]["params"], model.sh_deg, _posenc_of(model)))
     return True
+
+
+# ---- vanilla NeRF (use_viewdirs) parameters: octree.extraction's SH projection input -------------------------------
+# Dense_0..7 trunk (point posenc width W), Dense_8 raw sigma [256, 1], Dense_9 bottleneck [256, 256] (no activation),
+# Dense_10 condition layer [256 + 3 + 6 deg_view, 128] (rows [bottleneck | posenc(viewdir, 0, deg_view)]), Dense_11 rgb
+# [128, 3] (octree/nerf/model_utils.py:112-158; the rgb layer is 3 wide whatever sh_deg is, models.py:296-305).  A
+# vanilla parameter set is {"MLP_0": [(kernel [in, out], bias [out]) x 12], "MLP_1": ...} of fp32 numpy arrays.
+_VANILLA_TORCH_NAMES = ([f"input_layers.{i}" for i in range(8)]
+                        + ["sigma_layer", "bottleneck_layer", "condition_layers.0", "rgb_layer"])
+
+
+def vanilla_layer_dims(posenc=None, deg_view=4):
+    """(in, out) of Dense_0..Dense_11 of a vanilla NeRF MLP (net_depth_condition 1, net_width_condition 128)."""
+    return (layer_dims(1, posenc_width(posenc))[:8]
+            + [(256, 1), (256, 256), (256 + 3 + 6 * int(deg_view), 128), (128, 3)])
+
+
+def _vanilla_check(mlps, posenc, deg_view):
+    dims = vanilla_layer_dims(posenc, deg_view)
+    if "MLP_0" not in mlps:
+        raise ValueError("no MLP_0 in the parameter tree")
+    for mname, layers in mlps.items():
+        for i, ((k, b), (cin, cout)) in enumerate(zip(layers, dims)):
+            if k.shape != (cin, cout) or b.shape != (cout,):
+                hint = ("wrong min_deg_point / max_deg_point? Dense_0 has 3 + 6 (max_deg_point - min_deg_point) rows"
+                        if i in (0, 5) else
+                        "wrong deg_view? Dense_10 has 256 + 3 + 6 deg_view rows" if i == 10 else
+                        "not a vanilla NeRF (net_depth_condition 1, net_width_condition 128, 3 rgb channels)?")
+                raise ValueError(f"{mname}/Dense_{i}: expected kernel {(cin, cout)} and bias ({cout},), got "
+                                 f"{k.shape} and {b.shape} ({hint})")
+    return mlps
+
+
+def vanilla_from_flax_params(params, posenc=None, deg_view=4):
+    """["optimizer"]["target"]["params"] of a jaxnerf checkpoint -> vanilla parameter set (Dense_0..11 in order, as
+    restore_model_state_from_jaxnerf maps them: octree/nerf/models.py:66-113)."""
+    mlps = {}
+    m = 0
+    while f"MLP_{m}" in params:
+        src = params[f"MLP_{m}"]
+        layers = []
+        for i in range(12):
+            if f"Dense_{i}" not in src:
+                raise ValueError(f"MLP_{m}/Dense_{i} is missing (a vanilla NeRF has Dense_0..Dense_11)")
+            d = src[f"Dense_{i}"]
+            layers.append((np.asarray(d["kernel"], dtype=np.float32), np.asarray(d["bias"], dtype=np.float32)))
+        if "Dense_12" in src:
+            raise ValueError(f"MLP_{m}/Dense_12: net_depth_condition 1 expected (Dense_0..Dense_11)")
+        mlps[f"MLP_{m}"] = layers
+        m += 1
+    return _vanilla_check(mlps, posenc, deg_view)
+
+
+def vanilla_to_flax_params(mlps):
+    return {mname: {f"Dense_{i}": {"kernel": k, "bias": b} for i, (k, b) in enumerate(layers)}
+            for mname, layers in mlps.items()}
+
+
+def vanilla_from_torch_state_dict(sd, posenc=None, deg_view=4):
+    """state_dict of the reference's torch NerfModel(use_viewdirs=True) (octree/nerf/models.py:52-63) -> vanilla
+    parameter set; nn.Linear weight = kernel.T."""
+    mlps = {}
+    m = 0
+    while f"MLP_{m}.input_layers.0.weight" in sd:
+        layers = []
+        for tname in _VANILLA_TORCH_NAMES:
+            key = f"MLP_{m}.{tname}.weight"
+            if key not in sd:
+                raise ValueError(f"{key} is missing (a vanilla NeRF state_dict has {', '.join(_VANILLA_TORCH_NAMES)})")
+            layers.append((np.asarray(sd[key], dtype=np.float32).T.copy(),
+                           np.asarray(sd[f"MLP_{m}.{tname}.bias"], dtype=np.float32)))
+        mlps[f"MLP_{m}"] = layers
+        m += 1
+    return _vanilla_check(mlps, posenc, deg_view)
+
+
+def vanilla_to_torch_state_dict(mlps):
+    return {f"{mname}.{tname}.{w}": (np.ascontiguousarray(k.T) if w == "weight" else b)
+            for mname, layers in mlps.items() for tname, (k, b) in zip(_VANILLA_TORCH_NAMES, layers)
+            for w in ("weight", "bias")}
+
+
+def restore_vanilla(train_dir, is_jaxnerf_ckpt, posenc=None, deg_view=4):
+    """the vanilla parameter set of train_dir: the newest flax checkpoint_<step> (is_jaxnerf_ckpt) or *.ckpt, as
+    restore_model_state_from_jaxnerf / restore_model_state read them; None when there is none."""
+    if is_jaxnerf_ckpt:
+        sd = restore_flax_state_dict(train_dir)
+        return None if sd is None else vanilla_from_flax_params(sd["optimizer"]["target"]["params"], posenc, deg_view)
+    import torch
+    paths = sorted(glob.glob(os.path.join(train_dir, "*.ckpt")))
+    if not paths:
+        return None
+    ckpt = torch.load(paths[-1], map_location="cpu")
+    return vanilla_from_torch_state_dict({k: v.numpy() for k, v in ckpt["model"].items()}, posenc, deg_view)

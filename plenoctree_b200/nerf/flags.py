@@ -229,3 +229,38 @@ def check_model_scope(args):
     has it."""
     net_activation_code(args.net_activation)
     check_scope(_Trunk(args, "relu"))
+
+
+class _Override:
+    """`args` with some flags replaced (absl FlagValues cannot be copied field by field)"""
+
+    def __init__(self, args, **values):
+        self._args, self._values = args, values
+
+    def __getattr__(self, name):
+        return self._values[name] if name in self._values else getattr(self._args, name)
+
+
+MAX_DEG_VIEW = 32
+
+
+def check_projection_scope(args):
+    """octree.extraction of a vanilla NeRF (use_viewdirs): the SH projection of its view branch
+    (octree/extraction.py:217-241,362-394).  Accepts sh_deg 1-4, the reference's condition branch
+    (net_depth_condition 1, net_width_condition 128), a relu trunk and condition layer, 0 <= deg_view <= 32, and every
+    point-posenc, sample, dataset and density flag check_scope accepts.  Training, rendering and evaluating a vanilla
+    NeRF stay refused by check_scope."""
+    sh_deg = int(args.sh_deg)
+    if not 1 <= sh_deg <= 4:
+        raise NotImplementedError(
+            f"sh_deg={sh_deg}: projecting a vanilla NeRF needs an SH tree, 1 <= sh_deg <= 4 (with sh_deg 0 or less the "
+            "reference writes projected coefficients into an RGBA tree, and sh_deg -1 fails its order >= 0 assert)")
+    if (int(args.net_depth_condition), int(args.net_width_condition)) != (1, 128):
+        raise NotImplementedError(
+            f"net_depth_condition={args.net_depth_condition}, net_width_condition={args.net_width_condition}: the "
+            "projection kernel is built for one 128-wide condition layer (1, 128)")
+    if not 0 <= int(args.deg_view) <= MAX_DEG_VIEW:
+        raise NotImplementedError(
+            f"deg_view={args.deg_view}: 0 <= deg_view <= {MAX_DEG_VIEW} expected (scales above 2^31 of a unit "
+            "direction are below the resolution of an fp32 sine's argument)")
+    check_scope(_Override(args, use_viewdirs=False))

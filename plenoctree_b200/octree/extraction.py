@@ -9,8 +9,9 @@
 
 `args` carries the reference's flag names (extraction.py:66-176, octree/nerf/utils.py:60-253); `default_args()`
 returns the reference defaults.  `nerf` is plenoctree_b200.nerf.models.NerfModel; `dataset` needs .w .h .focal
-.camtoworlds [n,4,4] (and .size), like octree/nerf/datasets.py.  Vanilla-NeRF SH projection and SG are outside the
-scope of this path and raise NotImplementedError.
+.camtoworlds [n,4,4] (and .size), like octree/nerf/datasets.py.  A vanilla NeRF (use_viewdirs) is projected to SH
+in step2 (projection.py: projection_samples directions per block of leaves); SG is outside the scope of this path
+and raises NotImplementedError.
 
 Forward-facing (LLFF) scenes: the tree lives in NDC, where the model was trained, and the weight mask marches the
 training cameras' rays in NDC when renderer.scene_ndc says so ('llff' in --config and not --spherify).  --z_min /
@@ -205,14 +206,24 @@ def grid_points(mask, keep, xx, yy, zz):
 def step2(args, tree, nerf, cells_per_launch=None):
     """extraction.py:355-394 (SH data formats): S uniform samples per finest leaf, mean of [raw_rgb, raw_sigma].
     The per-cell mean is taken in the MLP kernel's epilogue (pob_eval_cells_mean); launches cover
-    `cells_per_launch` leaves (default: 2^22 points) instead of chunk // S = 320."""
-    if args.use_viewdirs:
-        raise NotImplementedError("vanilla-NeRF SH projection (use_viewdirs) is outside the scope of this path")
+    `cells_per_launch` leaves (default: 2^22 points) instead of chunk // S = 320.
+    A vanilla NeRF (args.use_viewdirs, nerf a projection.VanillaNerf) is projected to SH instead: each block of
+    projection.CELLS_PER_BLOCK leaves takes its own set of projection_samples directions (extraction.py:217-241), and
+    `cells_per_launch` (default: projection.blocks_per_launch) must be a multiple of the block."""
     rgba_tree = tree.data_format.format == 0
     import torch.distributed as dist
     S = int(args.samples_per_cell)
     leaf_ind = torch.where(tree.depths == tree.max_depth)[0]
-    if cells_per_launch is None:
+    if args.use_viewdirs:
+        from . import projection as P
+        if rgba_tree:
+            raise NotImplementedError("a vanilla NeRF is projected to an SH tree: sh_deg 1-4 expected")
+        D = int(args.projection_samples)
+        if cells_per_launch is None:
+            cells_per_launch = P.blocks_per_launch(S, D, args.sh_deg) * P.CELLS_PER_BLOCK
+        if cells_per_launch % P.CELLS_PER_BLOCK:
+            raise ValueError(f"cells_per_launch must be a multiple of {P.CELLS_PER_BLOCK} (one direction set each)")
+    elif cells_per_launch is None:
         cells_per_launch = max(1, (1 << 22) // S)
     rank, world = _rank_world()
     n = int(leaf_ind.shape[0])
@@ -229,7 +240,9 @@ def step2(args, tree, nerf, cells_per_launch=None):
         gen.manual_seed(20200823 + cid)
         u = torch.rand((chunk_inds.shape[0], S, 3), device=tree.device, generator=gen)
         points = tree[chunk_inds].sample(S, uniforms=u)
-        if not rgba_tree:
+        if args.use_viewdirs:
+            out[i:i + cells_per_launch] = P.project_leaves(nerf, args.sh_deg, D, points, S, i // P.CELLS_PER_BLOCK)
+        elif not rgba_tree:
             out[i:i + cells_per_launch] = ops.eval_cells_mean(nerf._blob(False), nerf.sh_deg, points.contiguous(), S,
                                                               precision=nerf.precision, posenc=nerf.posenc,
                                                               net_activation=nerf.net_act_code)
@@ -324,8 +337,16 @@ def _define_cli_flags():
 
 def load_nerf(FLAGS, device):
     """models.get_model_state(FLAGS, restore=True) of the octree side (octree/nerf/models.py:38-49): torch *.ckpt, or
-    a flax-format checkpoint_<step> with --is_jaxnerf_ckpt."""
+    a flax-format checkpoint_<step> with --is_jaxnerf_ckpt.  With --use_viewdirs the vanilla model of the SH
+    projection (projection.VanillaNerf)."""
     from ..nerf import checkpoints, models
+    if FLAGS.use_viewdirs:
+        from .projection import VanillaNerf
+        posenc = (FLAGS.min_deg_point, FLAGS.max_deg_point, bool(FLAGS.legacy_posenc_order))
+        mlps = checkpoints.restore_vanilla(FLAGS.train_dir, FLAGS.is_jaxnerf_ckpt, posenc, FLAGS.deg_view)
+        if mlps is None:
+            raise ValueError(f"no checkpoint found in {FLAGS.train_dir}")
+        return VanillaNerf(mlps, posenc, FLAGS.deg_view, FLAGS.num_fine_samples, device=device)
     margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, sigma_activation=FLAGS.sigma_activation,
                                net_activation=FLAGS.net_activation,
                                min_deg_point=FLAGS.min_deg_point, max_deg_point=FLAGS.max_deg_point,
@@ -347,7 +368,10 @@ def main(unused_argv):
     F = _define_cli_flags()
     FLAGS = F.FLAGS
     F.update_flags(FLAGS)
-    F.check_model_scope(FLAGS)
+    if FLAGS.use_viewdirs:
+        F.check_projection_scope(FLAGS)
+    else:
+        F.check_model_scope(FLAGS)
     torch.manual_seed(20200823)
     from .._dist import dist_finish, dist_init
     rank, _, dev = dist_init()       # under torchrun: NCCL group, this rank's GPU (x-slabs / leaf blocks / cameras)

@@ -1,7 +1,7 @@
 """Built-in stand-ins for the reference's shipped configuration files, so that the README command lines
 (`--config nerf_sh/config/blender`, `python -m octree.task_manager octree/config/syn_sh16.json ...`) work in a
 checkout that does not carry those files: when the named file does not exist, its base name selects a preset.
-A file on disk always wins.  Values: nerf_sh/config/{blender,tt}.yaml, octree/config/{syn_sh16,tt_sh25}.json.
+A file on disk always wins.  Values: nerf_sh/config/{blender,tt,misc/proj}.yaml, octree/config/{syn_sh16,tt_sh25}.json.
 """
 import os
 
@@ -13,6 +13,8 @@ NERF_SH = {
     "blender": dict(_NERF_SH_COMMON, dataset="blender", sh_deg=3),
     # Tanks and Temples (NSVF layout), SH25, wider sparsity prior
     "tt": dict(_NERF_SH_COMMON, dataset="nsvf", sh_deg=4, near=0.0, far=4.0, sparsity_radius=5.0, sparsity_length=0.2),
+    # misc/proj: a vanilla NeRF (use_viewdirs) projected to an SH25 tree by octree.extraction
+    "proj": dict(_NERF_SH_COMMON, dataset="blender", use_viewdirs=True, sh_deg=4),
 }
 
 
