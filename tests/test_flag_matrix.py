@@ -93,8 +93,11 @@ ENTRY_FWD = {
 }
 ENTRY_DGRAD = {"train"}
 ROW_ENTRIES = tuple(ENTRY_FWD)                 # every row calls every entry point at its precision
-# compiled, launched by no entry point: the saving OUT_SIGMA forward (launch_mlp_fwd accepts it; nothing passes it)
-UNREACHABLE_FWD = {(1, "OUT_SIGMA", True)}
+# the saving OUT_SIGMA forward is launched by pob_sh_proj_points alone (projection.cu), which refuses every trunk but
+# relu: its relu instantiation runs there (checked stage by stage in test_projection_stages.py,
+# test_point_stage_from_saved_tiles); the elu, softplus and tanh ones are compiled and launched by no entry point
+PROJ_FWD = {(1, "OUT_SIGMA", True, "relu")}
+UNREACHABLE_FWD = {(1, "OUT_SIGMA", True, a) for a in TRUNKS[1:]}
 
 
 def _tag(row):
@@ -143,8 +146,8 @@ def _compiled_fwd():
 
 def test_every_instantiation_is_reached():
     """the forward <NSPLIT, OUTM, SAVE, ACT> and data-gradient <NSPLIT, ACT> instantiations compiled in mlp_fwd.cu /
-    mlp_bwd.cu, against the entry table above: every one but the recorded unreachable one is launched by the rows of
-    this file; the table matches the sources' out_mode choices"""
+    mlp_bwd.cu, against the entry table above: every one but the recorded unreachable ones is launched by the rows of
+    this file or by the projection's point stage; the table matches the sources' out_mode choices"""
     fwd = _compiled_fwd()
     assert len(fwd) == 11, sorted(fwd)
     bwd_src = open(os.path.join(ROOT, "plenoctree_b200", "csrc", "mlp_bwd.cu")).read()
@@ -156,6 +159,12 @@ def test_every_instantiation_is_reached():
     assert "p.out_mode = pob::OUT_RGBS;" in capi and "p.out_mode = pob::OUT_CELL_MEAN;" in capi
     pipe = open(os.path.join(ROOT, "plenoctree_b200", "csrc", "pipeline.cu")).read()
     assert "p.out_mode = OUT_RGBS;" in pipe and "p.save_h = C.H;" in pipe
+    proj = open(os.path.join(ROOT, "plenoctree_b200", "csrc", "projection.cu")).read()
+    body = proj[proj.index("int pob_sh_proj_points("):proj.index("int pob_sh_proj_directions(")]
+    assert "if (net.net_act != pob::NET_RELU) return pob_fail(" in body
+    assert "p.out_mode = pob::OUT_SIGMA;" in body and "p.save_h = base + ws.h;" in body
+    assert "pob::launch_mlp_fwd(p, 1, sms," in body
+    assert "launch_mlp_fwd" not in proj.replace(body, "")
     acts = {(0 if r[0] == "fp16" else 1, r[1]) for r in MATRIX}
     reached_fwd, reached_bwd = set(), set()
     for prec_i, act in acts:
@@ -164,9 +173,10 @@ def test_every_instantiation_is_reached():
             reached_fwd.add(ENTRY_FWD[e](n) + (act,))
             if e in ENTRY_DGRAD:
                 reached_bwd.add((n, act))
-    want_fwd = {f + (a,) for f in fwd - UNREACHABLE_FWD for a in TRUNKS}
+    reached_fwd |= PROJ_FWD
+    want_fwd = {f + (a,) for f in fwd for a in TRUNKS} - UNREACHABLE_FWD
     assert reached_fwd == want_fwd, (want_fwd - reached_fwd, reached_fwd - want_fwd)
-    assert UNREACHABLE_FWD <= fwd
+    assert {f[:3] for f in UNREACHABLE_FWD | PROJ_FWD} <= fwd
     assert reached_bwd == {(n, a) for n in (1, X3) for a in TRUNKS}
 
 

@@ -387,6 +387,31 @@ def test_inference_forwards_do_not_depend_on_the_split(sh, monkeypatch):
         assert r["cell_err_over_bound"] <= 1.0, (sms, r["cell_err_over_bound"])
 
 
+@pytest.mark.gpu
+def test_projection_point_stage_does_not_depend_on_the_split(monkeypatch):
+    """pob_sh_proj_points (the saving relu forward on SRC_POINTS, then a_p): a_p, raw sigma and the whole workspace
+    (h_0..h_7, posenc and mask images) bit-identical at every count, at 9 tiles per CTA of 16 SMs"""
+    from plenoctree_b200.octree.projection import VanillaNerf
+    from oracle import projection_oracle as PJ
+    from tests.test_projection_stages import _points, _run_points
+    nerf = VanillaNerf({"MLP_0": PJ.init_params(45)}, (0, 10, False), 4, num_fine_samples=0)
+    M = 9 * MIN_SMS * L.TILE_M + 77
+    pts = _points(M, 9)
+    base, rep = None, {}
+    for c in ["device"] + [c for c in _counts() if c != "device"]:
+        sms = _set_sms(monkeypatch, c)
+        ws, a, s, ab, sb = _run_points(nerf, pts)
+        out = (a.contiguous().view(torch.int32), s.view(torch.int32), ws, ab, sb)
+        base = base or out
+        rep[str(sms)] = dict(a=int((out[0] != base[0]).sum()), sigma=int((out[1] != base[1]).sum()),
+                             workspace=int((out[2] != base[2]).sum()), tails=int((out[3] != base[3]).sum()) +
+                             int((out[4] != base[4]).sum()))
+    _record("projection_points", dict(counts=rep, M=M))
+    assert bool(torch.isfinite(base[0].view(torch.float32)).all()) and bool(torch.isfinite(base[1].view(torch.float32)).all())
+    for sms, r in rep.items():
+        assert all(v == 0 for v in r.values()), (sms, r)
+
+
 # =====================================================================================================================
 # H: octree optimiser steps
 # =====================================================================================================================
@@ -458,6 +483,13 @@ def test_out_of_range_counts_are_refused(monkeypatch):
     (o, d, v, px), t_rand, u, sp, _ = case.inputs(case.R)
     state = T.TrainState(model)
     nq = 4096 + 3
+    from oracle import projection_oracle as PJ
+    from plenoctree_b200.octree.projection import VanillaNerf
+    vn = VanillaNerf({"MLP_0": PJ.init_params(46)}, (0, 10, False), 4, num_fine_samples=0)
+    nd, ncell, S, psh = 40, 10, 2, 4
+    K = (psh + 1) ** 2
+    a_in, s_in = torch.zeros(ncell * S, 128, device=dev), torch.zeros(ncell * S, device=dev)
+    t_in, y_in = torch.zeros(128 * nd, device=dev), torch.zeros(nd * K, device=dev)
 
     def canary(k):
         return ES._canary(k, tail=0)
@@ -466,6 +498,10 @@ def test_out_of_range_counts_are_refused(monkeypatch):
         """name -> (call returning rc or raising PobError, buffers that must keep the canary)"""
         rb, sb, ob, gb, cb, tb = canary(m * C3), canary(m), canary(4 * m), canary(m * C3), canary(10 * (C3 + 1)), canary(64)
         q = [canary(nq) for _ in range(4)]
+        pw = canary(int(lib.pob_sh_proj_points_workspace_bytes(m)) // 4)
+        pa, ps = canary(m * 128), canary(m)
+        pd, pt, pb = canary(2 * nd * 3), canary(2 * 128 * nd), canary(2 * nd * K)
+        pc = canary(ncell * (3 * K + 1))
         f3 = ctypes.c_float * 3
         return {
             "pob_eval_points_raw": (lambda: lib.pob_eval_points_raw(ptr(blob), sh, ptr(x), m, ptr(rb), ptr(sb), 1,
@@ -484,6 +520,15 @@ def test_out_of_range_counts_are_refused(monkeypatch):
                 ptr(q[0]), ptr(q[1]), ptr(q[2]), nq, 0.5, 0.9, 1, stream_ptr()), q[:3]),
             "pob_octree_adam_step": (lambda: lib.pob_octree_adam_step(ptr(q[0]), ptr(q[1]), ptr(q[2]), ptr(q[3]), nq,
                                                                       0.5, 1.0, 1e-8, stream_ptr()), q),
+            "pob_sh_proj_points": (lambda: lib.pob_sh_proj_points(ptr(vn.sigma_blob), None, ptr(x), m, ptr(vn.head_w),
+                                                                  ptr(vn.head_b), ptr(pw), ptr(pa), ptr(ps),
+                                                                  stream_ptr()), [pw, pa, ps]),
+            "pob_sh_proj_directions": (lambda: lib.pob_sh_proj_directions(5, 0, 2, nd, 4, 0, psh, ptr(vn.w10e),
+                                                                          ptr(pd), ptr(pt), ptr(pb), stream_ptr()),
+                                       [pd, pt, pb]),
+            "pob_sh_proj_cells": (lambda: lib.pob_sh_proj_cells(ncell, S, 4, ptr(a_in), ptr(s_in), nd, psh, ptr(t_in),
+                                                                ptr(y_in), ptr(vn.w11), ptr(vn.b11), ptr(pc),
+                                                                stream_ptr()), [pc]),
         }
 
     def raises(fn):
