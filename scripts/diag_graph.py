@@ -6,7 +6,8 @@ import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
-from tests.test_train import _setup
+
+from tests.support.mlp_stages import _setup
 from plenoctree_b200.nerf.models import NerfModel, Rays
 from plenoctree_b200.nerf import train as T
 

@@ -92,7 +92,7 @@ def _octree_worker(rank, world, port, q):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
         import numpy as np
-        from tests.test_octree import look_at_pose, make_tree, to_device_tree
+        from tests.support.octree_scenes import look_at_pose, make_tree, to_device_tree
         from plenoctree_b200.octree import VolumeRenderer, optimization as OPT
         torch.cuda.set_device(0)
         otree = make_tree(61, 3, "SH16")
@@ -112,7 +112,7 @@ def test_octree_epoch_two_ranks_equals_one_rank():
     """C5 ray-parallel (SURVEY §8e): pixel-row slabs per rank + one all-reduce of the dense gradient per image must
     reproduce the single-process epoch (same SGD sequence) up to fp32 summation order."""
     import numpy as np
-    from tests.test_octree import look_at_pose, make_tree, to_device_tree
+    from tests.support.octree_scenes import look_at_pose, make_tree, to_device_tree
     from plenoctree_b200.octree import VolumeRenderer, optimization as OPT
     otree = make_tree(61, 3, "SH16")
     tree = to_device_tree(otree)

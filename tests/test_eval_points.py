@@ -1,17 +1,18 @@
 """GPU parity of the fused point evaluator (csrc/mlp_fwd.cu) through the C ABI:
 against the committed golden vectors of the reference's torch twin, against the CPU oracle on
 seeded inputs, ragged sizes, and the extraction grid sweep."""
-import json
+import functools
 import os
 
 import numpy as np
 import pytest
 import torch
 
+from tests.support.eval_stages import TOL_FP16_ANY
+from tests.support.records import record
+
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-OUT = os.path.join(ROOT, "gpurun_out")
 
 # Tolerances (relative to the largest reference magnitude of the compared tensor).
 #   FP16X3: error-compensated operands, fp32-class accuracy -> 1e-4 (north-star bar is 1e-3)
@@ -22,20 +23,9 @@ OUT = os.path.join(ROOT, "gpurun_out")
 #           error of the 10-layer fp16 chain reaches ~2e-3: those tests use TOL_FP16_ANY.
 TOL_X3 = 1e-4
 TOL_FP16 = 1e-3
-TOL_FP16_ANY = 3e-3
 
 
-def _record(name, payload):
-    os.makedirs(OUT, exist_ok=True)
-    path = os.path.join(OUT, "parity_eval_points.json")
-    data = {}
-    if os.path.exists(path):
-        try:
-            data = json.load(open(path))
-        except Exception:
-            data = {}
-    data[name] = payload
-    json.dump(data, open(path, "w"), indent=1)
+_record = functools.partial(record, "parity_eval_points.json")
 
 
 def _relmax(got, want):

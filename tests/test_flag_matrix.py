@@ -14,7 +14,7 @@ saved tiles (test_net_activation._check_level) and the per-ray stages (test_ray_
 the reference of a wrong flag (mutation guards), and the inference forwards of the fine MLP with the same flags.
 Once: a CUDA-graph replay of a row with every flag away from its default.
 """
-import json
+import functools
 import os
 import re
 from itertools import combinations
@@ -26,10 +26,10 @@ import torch
 from oracle import net_activation_oracle as NA
 from oracle import posenc_oracle as PO
 from plenoctree_b200 import layouts as L
-from tests.test_ray_stages import RayCase
-from tests.test_train import OUT
+from tests.support.model_flags import _alt_pe
+from tests.support.ray_stages import RayCase
+from tests.support.records import ROOT, record
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 X3 = 3
 GUARD = 10.0        # a check must miss its bar by at least this factor against the reference of a wrong flag
 CELL_S = 32         # cells of 32 samples: the cell-mean epilogue's per-32-row branch (S = 1 takes the other)
@@ -106,12 +106,7 @@ def _tag(row):
             + ("_noise" if noise else "") + ("" if white else "_black"))
 
 
-def _record(name, payload):
-    os.makedirs(OUT, exist_ok=True)
-    path = os.path.join(OUT, "parity_flag_matrix.json")
-    data = json.load(open(path)) if os.path.exists(path) else {}
-    data[name] = payload
-    json.dump(data, open(path, "w"), indent=1, default=float)
+_record = functools.partial(record, "parity_flag_matrix.json")
 
 
 # =====================================================================================================================
@@ -216,15 +211,6 @@ def test_reference_anchor_trunk(act):
 # =====================================================================================================================
 # GPU
 # =====================================================================================================================
-def _alt_pe(pe):
-    """an encoder of the same width that differs from pe: the other feature order, or (one degree) shifted degrees
-    where both orders coincide; None for W = 3 (no sines)"""
-    mn, mx, legacy = pe
-    if mn == mx:
-        return None
-    if mx - mn == 1:
-        return (mn - 1, mx - 1, legacy) if mn > 0 else (mn + 1, mx + 1, legacy)
-    return (mn, mx, not legacy)
 
 
 def _row_case(row):
@@ -233,7 +219,7 @@ def _row_case(row):
 
 
 def _row_model(row):
-    from tests.test_net_activation import _make_model
+    from tests.support.model_flags import _make_model
     prec, act, pe, dens = row[:4]
     return _make_model(_row_case(row), act, pe=pe, sigma_act=dens)
 
@@ -241,10 +227,10 @@ def _row_model(row):
 def _check_row(row):
     from plenoctree_b200 import ops
     from plenoctree_b200.nerf.models import Rays
-    from tests import test_net_activation as NT
-    from tests import test_ray_stages as RS
-    from tests.test_eval_stages import X3Ref, _cell_bound, _level_rows, _nbits, _x3_errors
-    from tests.test_train_x3 import _run
+    from tests.support import model_flags as NT
+    from tests.support import ray_stages as RS
+    from tests.support.eval_stages import X3Ref, _cell_bound, _level_rows, _nbits, _x3_errors
+    from tests.support.mlp_x3 import _run
     prec, act, pe, dens, sh = row[:5]
     case = _row_case(row)
     x3 = case.precision == X3
@@ -323,7 +309,7 @@ def _check_row(row):
     inf["grid_vs_points_bit_mismatches"] = _nbits(g_rgb, p_rgb) + _nbits(g_sig, p_sig[:, 0])
     inf["grid_sigma_only_bit_mismatches"] = _nbits(g_sig_only, p_sig[:, 0])
     if x3:
-        from tests.test_eval_stages import Stats
+        from tests.support.mlp_stages import Stats
         st = Stats()
         ref = X3Ref(model.params[i * model.P:(i + 1) * model.P].cpu().numpy(), sh, dev, pe, act)
         _x3_errors(ref, x, raw_rgb, raw_sig, st, "points")
@@ -336,12 +322,12 @@ def _check_row(row):
 
 
 def _assert_row(row, out):
-    from tests import test_ray_stages as RS
-    from tests import test_train_stages as TS
-    from tests import test_train_x3 as TX
-    from tests.test_eval_stages import X3_ALLOW
-    from tests.test_net_activation import SIN_X3_ALLOW, _assert_call
-    from tests.test_sigma_activation import GW_BAR
+    from tests.support import ray_stages as RS
+    from tests.support import mlp_stages as TS
+    from tests.support import mlp_x3 as TX
+    from tests.support.eval_stages import X3_ALLOW
+    from tests.support.model_flags import SIN_X3_ALLOW, _assert_call
+    from tests.support.ray_stages import GW_BAR
     prec, act, pe, dens = row[:4]
     x3 = prec == "fp16x3"
     _assert_call(out["stages"], X3 if x3 else 1, act)
@@ -385,8 +371,8 @@ def test_graph_replay_with_every_flag_non_default():
     from plenoctree_b200.nerf import train as T
     from plenoctree_b200.nerf.models import NerfModel, Rays
     from plenoctree_b200.nerf.rays import random_rays_np
-    from tests.test_net_activation import _centre_sigma
-    from tests.test_posenc import _gpu_params
+    from tests.support.model_flags import _centre_sigma
+    from tests.support.model_flags import _gpu_params
     pe, sh, R = (2, 8, True), 2, 256
     fc, ff = _gpu_params(pe, sh, 33)
     for f in (fc, ff):

@@ -3,15 +3,11 @@
 The flag only states that the caller will not read those tiles: every result the call returns, and every other byte
 of the workspace, must be what the call leaves without it.  train_step (and GraphedTrainStep) always set it;
 loss_and_grad keeps the tiles unless asked (keep_saved_tiles)."""
-import numpy as np
 import pytest
 import torch
 
 from plenoctree_b200 import _lib
-from plenoctree_b200 import layouts as L
-
-RAYS, NC, NF, NSP = 4096, 64, 128, 10000     # the production SH16 step (bench.py)
-FILL = 0x5A
+from tests.support.model_flags import FILL, NF, NSP, RAYS, _batch, _call, _equal_outside, _model, _saved_grad_ranges
 
 
 def test_unknown_flag_bit_refused():
@@ -20,52 +16,6 @@ def test_unknown_flag_bit_refused():
     rc = _lib.lib.pob_loss_and_grad_flags(*args, 2, None)
     assert rc != 0
     assert b"flags" in _lib.lib.pob_last_error()
-
-
-def _model(sh_deg, nf, nsp, near=2.0, far=6.0, R=RAYS):
-    from plenoctree_b200.nerf.models import NerfModel
-    model = NerfModel(sh_deg=sh_deg, num_coarse_samples=NC, num_fine_samples=nf, near=near, far=far,
-                      white_bkgd=True, max_rays=R, sparsity_npoints=nsp)
-    model.init_params(20200823)
-    return model
-
-
-def _batch(R, seed):
-    from plenoctree_b200.nerf.models import Rays
-    from plenoctree_b200.nerf.utils import random_rays_np
-    o, d, v, px = random_rays_np(R, seed)
-    b = torch.from_numpy(np.concatenate([o, d, v, px], axis=1)).cuda()
-    return {"rays": Rays(b[:, 0:3], b[:, 3:6], b[:, 6:9]), "pixels": b[:, 9:12]}, b
-
-
-def _call(model, state, batch, keep, precision=_lib.PREC_FP16, **kw):
-    """loss_and_grad from a workspace filled with FILL; returns (grads, stats_raw, workspace bytes)"""
-    from plenoctree_b200.nerf import train as T
-    ws = model.workspace(True, precision)
-    ws.fill_(FILL)
-    T.loss_and_grad(model, state, batch, precision=precision, keep_saved_tiles=keep, **kw)
-    torch.cuda.synchronize()
-    return state.grads.clone(), state.stats_raw.clone(), ws.clone()
-
-
-def _saved_grad_ranges(model, R, sparsity_on):
-    """[start, end) byte ranges of the DZ and DO images the call writes"""
-    views = L.train_workspace_views(model.cfg, R, sparsity_on)
-    out = []
-    for v in views["levels"]:
-        for name in ("DZ", "DO"):
-            off, shape = v[name]
-            out.append((off, off + int(np.prod(shape))))
-    return out
-
-
-def _equal_outside(w0, w1, ranges):
-    start = 0
-    for a, b in sorted(ranges) + [(w0.numel(), w0.numel())]:
-        if not torch.equal(w0[start:a], w1[start:a]):
-            return False
-        start = b
-    return True
 
 
 CASES = {   # sh_deg, nf, nsp, near, far, loss_and_grad keywords

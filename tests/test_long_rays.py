@@ -4,30 +4,35 @@
 against test_ray_stages.py's fp64 bars, and on the GPU the wide per-ray kernels (one 128-thread block per ray for
 256 < N <= 1024), the training and render calls, graph replay and the CLI.
 
-The fp64 references, the order-independent bars and the GPU wrappers are test_ray_stages.py's, used unchanged.
+The fp64 references, the order-independent bars and the GPU wrappers are those of tests/support/ray_stages.py, used
+unchanged.
 """
+import functools
 import os
 
 import numpy as np
 import pytest
 import torch
 
-import tests.test_ray_stages as RS
-from tests.test_ray_stages import (ACC_BAR, GUARD, GW_BAR, RayCase, _norm, _t, assert_composite, assert_pdf,
-                                   check_composite, check_composite_bwd, check_pdf, composite_bwd_ref, composite_ref,
-                                   emu_delta, pdf_families, ray_families)
+from tests.support import ray_stages as RS
+from tests.support.ray_stages import (ACC_BAR, GUARD, GW_BAR, RayCase, _norm, _t, assert_composite, assert_pdf,
+                                      check_composite, check_composite_bwd, check_pdf, composite_bwd_ref, composite_ref,
+                                      emu_delta, pdf_families, ray_families)
+from tests.support.records import record
 
 ACCEPT = [(3, 0), (1024, 0), (128, 384), (256, 768), (64, 960)]
 REFUSE = [(2, 0), (512, 513), (1025, 0)]
 LONG_N = [257, 288, 289, 384, 640, 1000, 1024]
 LONG_PDF = [(3, 1021), (128, 384), (256, 768), (1000, 24), (1023, 1)]
 
+_record = functools.partial(record, "parity_ray_stages.json")
+
 
 # =====================================================================================================================
 # CPU: the bound
 # =====================================================================================================================
 def _scope(nc, nf):
-    from tests.test_posenc import _scope_args
+    from tests.support.model_flags import _scope_args
     a = _scope_args()
     a.num_coarse_samples, a.num_fine_samples = nc, nf
     return a
@@ -278,7 +283,7 @@ def test_emulated_wide_pdf_within_bars(Nc, Nf):
 def test_wide_composite_kernels_vs_fp64(N):
     """pob_composite / pob_composite_bwd at W = 4 (S = 3..8 per thread, and both ends of S = 3 at 257 and 384) per
     element against fp64: both backgrounds, every ray family, R = 1 and R not a multiple of the block"""
-    RS.test_composite_kernels_vs_fp64(N)
+    RS.composite_kernels_vs_fp64(N)
 
 
 @pytest.mark.gpu
@@ -286,13 +291,13 @@ def test_wide_composite_kernels_vs_fp64(N):
 def test_wide_sample_pdf_kernel_vs_fp64(Nc, Nf):
     """pob_sample_pdf with the 1024-key sort: the u table, per-ray u and k/64 ties; sorted, coarse depths bit for
     bit, the fp64 bracket and bars"""
-    RS.test_sample_pdf_kernel_vs_fp64(Nc, Nf)
+    RS.sample_pdf_kernel_vs_fp64(Nc, Nf)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("lindisp", [False, True])
 def test_sample_coarse_bit_exact_1024(lindisp):
-    RS.test_sample_coarse_bit_exact(1024, lindisp)
+    RS.sample_coarse_bit_exact(1024, lindisp)
 
 
 @pytest.mark.gpu
@@ -328,21 +333,21 @@ def test_ray_stages_in_training_call_long(precision):
     """test_ray_stages.py's ray-stage checks inside pob_loss_and_grad at (128, 384), fp16 and fp16x3"""
     case = RayCase(3, 40, 128, 384, 200, precision=precision)
     res = RS._in_call(case)
-    RS._record(f"long_{case.name}", res)
+    _record(f"long_{case.name}", res)
     RS._assert_in_call(res)
 
 
 @pytest.mark.gpu
 def test_mlp_stages_in_training_call_long():
     """test_train_stages.py's stage checks of the saving forward, data and weight gradients at (128, 384)"""
-    from tests.test_train_stages import Case, _stage_case
+    from tests.support.mlp_stages import Case, _stage_case
     _stage_case(Case(3, 40, 128, 384, 200))
 
 
 @pytest.mark.gpu
 def test_mlp_stages_in_training_call_long_x3():
-    from tests.test_train_stages import Case
-    from tests.test_train_x3 import _stage_case_x3
+    from tests.support.mlp_stages import Case
+    from tests.support.mlp_x3 import _stage_case_x3
     _stage_case_x3(Case(3, 40, 128, 384, 200))
 
 
@@ -372,7 +377,7 @@ def test_ray_stages_render_call_long(randomized):
                           L.workspace_view(ws, lv, "acc")[:, None]], 1)
         st[f"out_bit_mismatches_{i}"] = int((got.view(torch.int32) != want.view(torch.int32)).sum())
     res["stage"] = st
-    RS._record(f"long_render_rand{int(randomized)}", res)
+    _record(f"long_render_rand{int(randomized)}", res)
     RS._assert_in_call(res)
 
 
@@ -413,7 +418,7 @@ def test_render_matches_executed_reference_long_rays(golden_dir, nc, nf):
                     assert e["rgb"] < 1e-3 and e["acc"] < 1e-3, (tag, pname, name, e)
                 else:
                     assert e["rel_rms"] < 1e-3 and e["psnr"] > 60 and e["rgb"] < 2e-2, (tag, pname, name, e)
-    RS._record(f"long_render_vs_reference_{tag_n}", rec)
+    _record(f"long_render_vs_reference_{tag_n}", rec)
 
 
 # =====================================================================================================================
@@ -425,7 +430,7 @@ def test_graphed_train_step_matches_eager_long():
     from plenoctree_b200.nerf import train as T
     from plenoctree_b200.nerf.models import NerfModel, Rays
     from plenoctree_b200.nerf.rays import random_rays_np
-    from tests.test_train_stages import _params
+    from tests.support.mlp_stages import _params
     R = 256
     fc, ff = _params(3, 33)
     o, d, v, px = random_rays_np(R, 33)
@@ -511,5 +516,5 @@ def test_cli_train_eval_long_rays(tmp_path):
     finally:
         for k, v in old.items():
             setattr(FLAGS, k, v)
-    RS._record("long_cli", dict(psnr_init=p_init, psnr_128_384=float(psnr), psnr_eval_256_768=float(psnr_long)))
+    _record("long_cli", dict(psnr_init=p_init, psnr_128_384=float(psnr), psnr_eval_256_768=float(psnr_long)))
     assert np.isfinite(psnr_long) and psnr > p_init + 5.0, (p_init, psnr, psnr_long)

@@ -6,51 +6,23 @@ svox is absent from the reference tree (parity unpinned, see oracle/octree_oracl
   * the CUDA kernels equal the oracle (tree topology and leaf lookup bit-exact; colours / gradients within the
     float32 tolerances written below).
 """
-import json
+import functools
 import os
 
 import numpy as np
 import pytest
 
 from oracle import octree_oracle as OO
+from tests.support.octree_scenes import assert_device_tree_build_matches, look_at_pose, make_tree, to_device_tree
+from tests.support.records import record
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-OUT = os.path.join(ROOT, "gpurun_out")
 
 # float32 march, identical operation order, differing only in expf ulps and the order of the K-term dot products
 TOL_RGB = 2e-5        # absolute, colours in [0,1]
 TOL_GRAD_REL = 2e-4   # relative to the largest gradient entry
 
 
-def _record(name, payload):
-    os.makedirs(OUT, exist_ok=True)
-    path = os.path.join(OUT, "parity_octree.json")
-    data = {}
-    if os.path.exists(path):
-        try:
-            data = json.load(open(path))
-        except Exception:
-            data = {}
-    data[name] = payload
-    json.dump(data, open(path, "w"), indent=1)
-
-
-def make_tree(seed, depth, data_format, density=0.35, radius=1.3, center=(0.1, -0.05, 0.0), sigma_scale=6.0):
-    """random sparse tree: refine `depth` levels at random occupied voxels, random coefficients, sigma >= 0 with
-    about half of the finest leaves empty (sigma = 0), coarse leaves empty."""
-    rs = np.random.RandomState(seed)
-    K = 1 if data_format == "RGBA" else int(data_format[2:])
-    D = 4 if data_format == "RGBA" else 3 * K + 1
-    reso = 2 ** (depth + 1)
-    mask = rs.rand(reso, reso, reso) < density
-    tree, _ = OO.build_tree_from_grid(mask, depth, radius, center, D, data_format)
-    n = tree.n_internal
-    tree.data[:n] = rs.normal(0, 1.0, size=tree.data[:n].shape).astype(np.float32)
-    sig = rs.uniform(0, sigma_scale, size=tree.data[:n, ..., -1].shape).astype(np.float32)
-    sig[rs.rand(*sig.shape) < 0.5] = 0.0
-    deep = (tree.parent_depth[:n, 1] == depth)[:, None, None, None]
-    tree.data[:n, ..., -1] = np.where(deep, sig, 0.0)
-    return tree
+_record = functools.partial(record, "parity_octree.json")
 
 
 def random_rays(seed, n, radius=1.3):
@@ -62,20 +34,6 @@ def random_rays(seed, n, radius=1.3):
     d = (d / np.linalg.norm(d, axis=1, keepdims=True)).astype(np.float32)
     d[: n // 8] *= -1.0  # some rays miss the volume
     return o, d, d.copy()
-
-
-def look_at_pose(seed, dist=3.5):
-    rs = np.random.RandomState(seed)
-    eye = rs.normal(size=3)
-    eye = eye / np.linalg.norm(eye) * dist
-    fwd = -eye / np.linalg.norm(eye)
-    up = np.array([0.0, 0.0, 1.0])
-    right = np.cross(fwd, up)
-    right /= np.linalg.norm(right)
-    up = np.cross(right, fwd)
-    c2w = np.eye(4, dtype=np.float32)
-    c2w[:3, 0], c2w[:3, 1], c2w[:3, 2], c2w[:3, 3] = right, up, -fwd, eye
-    return c2w
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -202,22 +160,6 @@ def test_oracle_forward_agrees_with_reference_compositing_quadrature():
 # ---------------------------------------------------------------------------------------------------------
 # GPU parity
 # ---------------------------------------------------------------------------------------------------------
-def to_device_tree(otree):
-    import torch
-    from plenoctree_b200.octree import N3Tree
-    fmt = otree.data_format
-    t = N3Tree(N=otree.N, data_dim=otree.data_dim, depth_limit=otree.depth_limit, init_reserve=otree.n_internal,
-               radius=0.5 / otree.invradius, center=(1 - 2 * otree.offset) * (0.5 / otree.invradius),
-               data_format=fmt)
-    n = otree.n_internal
-    t.invradius = torch.from_numpy(otree.invradius).cuda()
-    t.offset = torch.from_numpy(otree.offset).cuda()
-    t.data[:n] = torch.from_numpy(otree.data[:n]).cuda()
-    t.child[:n] = torch.from_numpy(otree.child[:n]).cuda()
-    t.parent_depth[:n] = torch.from_numpy(otree.parent_depth[:n]).cuda()
-    t.n_internal = n
-    t._leaves = None
-    return t
 
 
 def test_extraction_sequence_matches_executed_reference(golden_dir):
@@ -317,39 +259,6 @@ def test_optimization_loop_matches_executed_reference(golden_dir):
             best, best_data = v, tree.data.copy()
     assert z["train_psnr"][-1] > z["train_psnr"][0] + 0.5 and best_data is not None          # it did learn
     assert np.abs(best_data - z["data_best"]).max() < 2e-5 * np.abs(z["data_best"]).max()
-
-
-def assert_device_tree_build_matches(otree, refines, radius, center, rs, query_box=2.0):
-    """A device N3Tree refined by the same sequence of `tree[points].refine()` calls as the oracle tree `otree`
-    (refines: float32 [n,3] world-point arrays, one call each) has the oracle's topology bit for bit; query_packed is
-    bit-exact on points of [-query_box, query_box]^3 around the box centre, leaves / depths are identical and sample
-    agrees."""
-    import torch
-    from plenoctree_b200.octree import N3Tree
-    L = otree.depth_limit
-    tree = N3Tree(N=otree.N, data_dim=otree.data_dim, depth_limit=L, init_reserve=16, geom_resize_fact=1.0,
-                  radius=radius, center=center, data_format=otree.data_format)
-    for pts in refines:
-        tree[torch.from_numpy(pts).cuda()].refine()
-    n = otree.n_internal
-    assert tree.n_internal == n and tree.max_depth == otree.max_depth == L
-    assert (tree.child[:n].cpu().numpy() == otree.child[:n]).all()
-    assert (tree.parent_depth[:n].cpu().numpy() == otree.parent_depth[:n]).all()
-    pts = (np.asarray(center, dtype=np.float32) + rs.uniform(-query_box, query_box, size=(5000, 3))).astype(np.float32)
-    node, ijk, _, _ = otree.query(pts)
-    want = otree.pack_index(node, ijk)
-    got = tree.query_packed(torch.from_numpy(pts).cuda()).cpu().numpy()
-    assert (got == want).all()
-    # leaves / depths / sample agree with the oracle
-    lv = otree.leaves()
-    assert (tree._all_leaves().cpu().numpy() == lv).all()
-    assert (tree.depths.cpu().numpy() == otree.leaf_depths(lv)).all()
-    sel = np.nonzero(otree.leaf_depths(lv) == L)[0][:300]
-    u = rs.rand(sel.size, 5, 3).astype(np.float32)
-    got = tree[torch.from_numpy(sel).cuda()].sample(5, torch.from_numpy(u).cuda()).cpu().numpy()
-    want = otree.sample(lv[sel], 5, u)
-    np.testing.assert_allclose(got, want, rtol=0, atol=1e-6)
-    return tree
 
 
 @pytest.mark.gpu

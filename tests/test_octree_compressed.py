@@ -12,7 +12,6 @@ load_tree, QuantTree, pob_octree_render_quant / pob_octree_render_depth_quant (c
   same images; octree.optimization refuses a compressed input.
 """
 import ctypes
-import functools
 import os
 import re
 
@@ -23,26 +22,18 @@ from oracle import octree_oracle as OO
 from plenoctree_b200 import _lib
 from plenoctree_b200.octree import compression as C
 from plenoctree_b200.octree.n3tree import N3Tree, compressed_layout, read_compressed
+from tests.support.octree_scenes import CASES, _pair, _state, _tree, f32
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-f32 = np.float32
 
 
 # ---------------------------------------------------------------------------------------------------------
 # files
 # ---------------------------------------------------------------------------------------------------------
-def _state(otree):
-    """the keys N3Tree.save writes (data in fp16, like svox) for an oracle tree"""
-    n = otree.n_internal
-    return {"data_dim": np.int64(otree.data_dim), "child": otree.child[:n].copy(),
-            "parent_depth": otree.parent_depth[:n].copy(), "n_internal": np.int64(n), "n_free": np.int64(0),
-            "invradius3": otree.invradius.astype(f32), "offset": otree.offset.astype(f32),
-            "depth_limit": np.int64(otree.depth_limit), "geom_resize_fact": np.float64(1.5),
-            "data": otree.data[:n].astype(np.float16), "data_format": str(otree.data_format)}
 
 
 def _small_tree(N, fmt, seed):
-    from tests.test_octree_march import _fill, _to_world
+    from tests.support.octree_scenes import _fill, _to_world
     rs = np.random.RandomState(seed)
     K = 1 if fmt == "RGBA" else int(fmt[2:])
     otree = OO.N3Tree(N=N, data_dim=4 if fmt == "RGBA" else 3 * K + 1, depth_limit=3, radius=(1.2, 0.9, 1.0),
@@ -205,39 +196,7 @@ def test_c_entry_points_validate_the_descriptor(change, msg):
 # ---------------------------------------------------------------------------------------------------------
 # GPU
 # ---------------------------------------------------------------------------------------------------------
-SH25_SPEC = (2, 7, "SH25", (1.0, 1.2, 0.9), (0.1, -0.05, 0.2), (-1, 1, -1))
-# tree -> (bits, retain, weighted) compressions
-CASES = {
-    "n2_d8_sh16": [(16, 0, False), (5, 2, True)],
-    "n3_d4_sh16": [(5, 0, False), (16, 2, False)],
-    "n2_d7_sh25": [(5, 2, False), (16, 0, True)],
-    "chain_d26_rgba": [(16, 0, False), (5, 0, True)],
-}
 CASE_IDS = [(name, i) for name in CASES for i in range(len(CASES[name]))]
-
-
-@functools.lru_cache(maxsize=None)
-def _tree(name):
-    """-> oracle tree, world points of its occupied cells (test_octree_march's trees; SH25 built the same way)"""
-    from tests.test_octree_march import _build, _fill, _shell_voxels, _to_world
-    if name != "n2_d7_sh25":
-        otree, _, pts = _build(name)
-        return otree, pts
-    N, L, fmt, radius, center, region = SH25_SPEC
-    rs = np.random.RandomState(sum(map(ord, name)))
-    otree = OO.N3Tree(N=N, data_dim=76, depth_limit=L, init_reserve=1024, geom_resize_fact=1.5, radius=radius,
-                      center=center, data_format=fmt)
-    pts = _to_world(otree, _shell_voxels(N, L, region, rs))
-    for _ in range(L):
-        otree.refine_at(pts)
-    _fill(otree, rs)
-    return otree, pts
-
-
-@functools.lru_cache(maxsize=None)
-def _compressed(name, i):
-    bits, retain, weighted = CASES[name][i]
-    return C.compress_tree(_state(_tree(name)[0]), bits=bits, sigma_thresh=2.0, retain=retain, weighted=weighted)
 
 
 def _rays(otree, pts, n=512, seed=0):
@@ -256,20 +215,6 @@ def _rays(otree, pts, n=512, seed=0):
     return np.concatenate([o, inside]).astype(f32), np.concatenate([d, di]).astype(f32)
 
 
-def _pair(name, i):
-    """(compressed renderer, fp32 renderer of decompress_data of the same file)"""
-    import torch
-    from tests.test_octree import to_device_tree
-    from plenoctree_b200.octree import VolumeRenderer, load_tree
-    otree, _ = _tree(name)
-    c = _compressed(name, i)
-    q = load_tree(c, map_location="cuda")
-    ref = to_device_tree(otree)
-    n = otree.n_internal
-    ref.data[:n] = torch.from_numpy(C.decompress_data(c)).cuda()
-    return q, ref
-
-
 def _forward(r, o, d, fast, return_depth):
     import torch
     from plenoctree_b200.octree import Rays
@@ -284,7 +229,7 @@ def _forward(r, o, d, fast, return_depth):
 @pytest.mark.parametrize("name,i", CASE_IDS)
 def test_renders_bit_identical_to_the_decompressed_tree(name, i):
     import torch
-    from tests.test_octree_march import CAM_F, CAM_H, CAM_W, _cameras
+    from tests.support.octree_scenes import CAM_F, CAM_H, CAM_W, _cameras
     from plenoctree_b200.octree import QuantTree, VolumeRenderer
     q, ref = _pair(name, i)
     assert isinstance(q, QuantTree) and q.retain == CASES[name][i][1] and q.bits == CASES[name][i][0]
@@ -332,7 +277,7 @@ def test_device_bytes_and_refusals():
         r.train_persp(np.eye(4, dtype=f32), torch.zeros(8, 8, 3), 8, 8, 10.0)
     # a --noquant file: an fp32 tree that renders like the original, and refuses gradients
     from plenoctree_b200.octree import load_tree
-    from tests.test_octree import to_device_tree
+    from tests.support.octree_scenes import to_device_tree
     otree, pts = _tree("n3_d4_sh16")
     z = _state(otree)
     nq = load_tree(C.compress_tree(dict(z), quantize=False))
@@ -371,7 +316,7 @@ def test_cli_evaluation_of_compressed_files(tmp_path):
     octree.optimization refuses a compressed input"""
     import subprocess
     import sys
-    from tests.test_octree_momentum import _cli, _scene
+    from tests.support.octree_scenes import _cli, _scene
     common = _scene(tmp_path)
     z = dict(np.load(str(tmp_path / "tree.npz")))
     c = C.compress_tree(dict(z), bits=6, sigma_thresh=2.0, retain=1)

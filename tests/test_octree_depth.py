@@ -23,9 +23,10 @@ import numpy as np
 import pytest
 
 from oracle import octree_depth_oracle as DO, octree_oracle as OO
-from tests.test_octree_march import (CAM_F, CAM_H, CAM_W, NAMES, SENSITIVITY, STOP, U24, _cameras, _fill, _first,
-                                     _record as _record_march, _rows, _safe_fast_rays, _to_world, _unit_rand,
-                                     device_tree, fwd64, world)
+from tests.support.octree_refs import SENSITIVITY, U24, _first, _rows, _safe_fast_rays, fwd64
+from tests.support.octree_scenes import (CAM_F, CAM_H, CAM_W, NAMES, STOP, _cameras, _fill, _to_world, _unit_rand,
+                                         device_tree, world)
+from tests.support.records import record
 
 f32, f64 = np.float32, np.float64
 
@@ -42,7 +43,7 @@ N_SEQ = 24                  # rays launched one at a time for the bit-identity o
 
 
 def _record(name, payload):
-    _record_march(f"depth_{name}", payload)
+    record("parity_octree_march.json", f"depth_{name}", payload)
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -459,7 +460,7 @@ def test_cli_evaluation_write_disp(tmp_path):
     import json
     import torch
     from PIL import Image
-    from tests.test_octree_momentum import _cli, _scene
+    from tests.support.octree_scenes import _cli, _scene
     from plenoctree_b200.octree import N3Tree, VolumeRenderer, disparity
     common = _scene(tmp_path)
     out = tmp_path / "disp"

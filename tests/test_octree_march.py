@@ -19,313 +19,23 @@ axis-aligned c2w sits on cell-face planes (zero direction components, positions 
   dropped) each move a checked value by more than SENSITIVITY x its bar.
 """
 import functools
-import json
-import os
-import time
 
 import numpy as np
 import pytest
 
 from oracle import octree_oracle as OO
-from tests.test_octree import OUT, assert_device_tree_build_matches, to_device_tree
+from tests.support.octree_refs import (GRAD_ALLOW, RGB_ALLOW, SENSITIVITY, SQ_ALLOW, TRAIN_ALLOW, U24, _check_grad,
+                                       _first, _layout, _rows, _safe_fast_rays, bwd64, fwd64)
+from tests.support.octree_scenes import (CAM_F, CAM_H, CAM_W, NAMES, SPECS, STOP, _cameras, _fill, _to_world,
+                                         _unit_rand, assert_device_tree_build_matches, device_tree, f32, f64, world)
+from tests.support.records import record
 
-f32, f64 = np.float32, np.float64
-U24 = 2.0 ** -24
-
-# ---- bars (measured on an H100 80 GB HBM3 at a 400 W power limit; the largest value over all trees in brackets)
-# render: |rgb - fp64| per ray and channel in units of 2^-24 * (1 + n_hits + sum_j tau_j + sum_j w_j sum_k (|b_k| + 1) |c_jk|)
-# (the 1 is the background composite; a basis value's rounding is absolute, not relative, since its polynomial cancels)
-RGB_ALLOW = 1.6             # [0.80]
-# backward: per element, in units of 2^-24 * sum over the contributing visits reaching it of |term| x its rounding depth
-# (see bwd64); the fp32 oracle's own backward measures [0.65] in this unit on the CPU
-GRAD_ALLOW = 1.4            # [0.70]
-# training pass: the same unit, the upstream gradient carrying the forward's error (RGB_ALLOW x its unit), which
-# dominates the unit: the kernel's own image sets the clamp mask and g, so its rgb error does not reach the gradient
-TRAIN_ALLOW = 0.13          # [0.065]
-# sum of squared errors (float per thread and CTA, double across CTAs): 2^-24 * sum (2 |diff| U + 16 diff^2)
-SQ_ALLOW = 0.06             # [0.031]
 # SGD: data - lr * g is one fused, correctly rounded operation, within 2^-24 * (|data| + |lr g|) of fp64  [0.998]
-STOP_MARGIN = 1e-4          # relative distance of the fp64 transmittance from stop_thresh for exact early-stop paths
-SENSITIVITY = 10.0
-STOP = 1e-2                 # svox fast=True: sigma_thresh = stop_thresh = 1e-2
+
 N_SINGLE = 32               # single-ray launches per ray set
 
 
-def _record(name, payload):
-    os.makedirs(OUT, exist_ok=True)
-    path = os.path.join(OUT, "parity_octree_march.json")
-    data = json.load(open(path)) if os.path.exists(path) else {}
-    data[name] = payload
-    json.dump(data, open(path, "w"), indent=1)
-
-
-# ---------------------------------------------------------------------------------------------------------
-# trees
-# ---------------------------------------------------------------------------------------------------------
-def _sh64(K, d):
-    """the SH basis of OO.sh_basis in fp64"""
-    x, y, z = (np.asarray(d, dtype=f64)[:, a] for a in range(3))
-    xx, yy, zz, xy, yz, xz = x * x, y * y, z * z, x * y, y * z, x * z
-    C1, C2, C3, C4 = OO.SH_C1, OO.SH_C2, OO.SH_C3, OO.SH_C4
-    b = [np.full_like(x, OO.SH_C0), -C1 * y, C1 * z, -C1 * x,
-         C2[0] * xy, C2[1] * yz, C2[2] * (2.0 * zz - xx - yy), C2[3] * xz, C2[4] * (xx - yy),
-         C3[0] * y * (3 * xx - yy), C3[1] * xy * z, C3[2] * y * (4 * zz - xx - yy), C3[3] * z * (2 * zz - 3 * xx - 3 * yy),
-         C3[4] * x * (4 * zz - xx - yy), C3[5] * z * (xx - yy), C3[6] * x * (xx - 3 * yy),
-         C4[0] * xy * (xx - yy), C4[1] * yz * (3 * xx - yy), C4[2] * xy * (7 * zz - 1), C4[3] * yz * (7 * zz - 3),
-         C4[4] * (zz * (35 * zz - 30) + 3), C4[5] * xz * (7 * zz - 3), C4[6] * (xx - yy) * (7 * zz - 1),
-         C4[7] * xz * (xx - 3 * yy), C4[8] * (xx * (xx - 3 * yy) - yy * (3 * xx - yy))]
-    return np.stack(b[:K], axis=1)
-
-
-def _shell_voxels(N, L, region, rs, R=0.32):
-    """voxel centres (unit cube) of the level-L cells that a sphere of radius R about the box centre passes through,
-    restricted to the directions in `region` (octant signs; 0 = both)"""
-    reso = N ** (L + 1)
-    n = int(8 * 4 * np.pi * R * R * reso * reso / 2 ** sum(1 for s in region if s))
-    v = rs.normal(size=(n, 3))
-    v /= np.linalg.norm(v, axis=1, keepdims=True)
-    for a, s in enumerate(region):
-        if s:
-            v[:, a] = s * np.abs(v[:, a])
-    idx = np.unique(np.floor((0.5 + R * v) * reso).astype(np.int64), axis=0)
-    return (idx + 0.5) / reso
-
-
-def _to_world(otree, unit):
-    return ((np.asarray(unit, dtype=f64) - otree.offset) / otree.invradius).astype(f32)
-
-
-def _fill(otree, rs, tau_cell=0.6, cap_level=12):
-    """every cell of every node: coefficients N(0,1); sigma sized to an optical depth of up to tau_cell across the
-    cell (capped at level cap_level), 20 % of it negated"""
-    n, N = otree.n_internal, otree.N
-    otree.data[:n] = rs.normal(0, 1, size=otree.data[:n].shape).astype(f32)
-    lvl = np.minimum(otree.parent_depth[:n, 1], cap_level).astype(f64)
-    cell = (N ** -(lvl + 1.0)) / otree.invradius.astype(f64).mean()          # world cell size
-    sig = rs.uniform(0, tau_cell, size=otree.data[:n, ..., -1].shape) / cell[:, None, None, None]
-    sig[rs.rand(*sig.shape) < 0.2] *= -1.0
-    otree.data[:n, ..., -1] = sig.astype(f32)
-
-
-SPECS = {
-    # name: N, depth, format, radius, center, shell region (None = chain tree)
-    "n2_d8_sh16": (2, 8, "SH16", (1.1, 0.8, 1.4), (0.15, -0.1, 0.05), (1, 1, 0)),
-    "n2_d9_sh4": (2, 9, "SH4", (0.9, 1.3, 1.05), (-0.2, 0.1, 0.3), (1, -1, 1)),
-    "n3_d4_sh16": (3, 4, "SH16", (1.2, 1.0, 0.85), (0.05, 0.2, -0.1), (-1, 1, 1)),
-    "n4_d3_sh9": (4, 3, "SH9", (0.8, 1.25, 1.0), (0.1, 0.0, 0.25), (1, 1, -1)),
-    "chain_d26_rgba": (2, 26, "RGBA", (1.3, 0.95, 1.15), (-0.05, 0.12, 0.0), None),
-}
-CHAIN = ((0.3712345, 0.6184021, 0.4421377, 12), (0.6931472, 0.2718282, 0.5772157, 16),
-         (0.0137035, 0.0291172, 0.0083145, 26))
-
-
-def _build(name):
-    """-> oracle tree, list of refine() point sets (world), world points of occupied cells"""
-    N, L, fmt, radius, center, region = SPECS[name]
-    K = 1 if fmt == "RGBA" else int(fmt[2:])
-    D = 4 if fmt == "RGBA" else 3 * K + 1
-    rs = np.random.RandomState(sum(map(ord, name)))
-    otree = OO.N3Tree(N=N, data_dim=D, depth_limit=L, init_reserve=1024, geom_resize_fact=1.5, radius=radius,
-                      center=center, data_format=fmt)
-    refines = []
-    if region is None:
-        for *p, depth in CHAIN:
-            w = _to_world(otree, [p])
-            while True:
-                node, _, _, _ = otree.query(w)
-                if otree.parent_depth[node[0], 1] >= depth:
-                    break
-                otree.refine_at(w)
-                refines.append(w)
-        pts = _to_world(otree, [p[:3] for p in CHAIN])
-    else:
-        pts = _to_world(otree, _shell_voxels(N, L, region, rs))
-        for _ in range(L):
-            otree.refine_at(pts)
-            refines.append(pts)
-        if name.startswith("n3") and otree.n_internal % 2 == 0:
-            # an odd node count makes the SGD length n_internal * 27 * 49 odd: the kernel's scalar tail runs
-            extra = _to_world(otree, [[0.5 - 0.4 * s if s else 0.02 for s in region]])
-            assert otree.refine_at(extra)
-            refines.append(extra)
-    _fill(otree, rs)
-    return otree, refines, pts
-
-
-def _unit_rand(rs, n):
-    v = rs.normal(size=(n, 3))
-    return (v / np.linalg.norm(v, axis=1, keepdims=True)).astype(f32)
-
-
-def _face_world(otree, a, target):
-    """a world coordinate whose tree coordinate (offset + invradius * x, rounded like the kernel) is exactly target"""
-    off, inv = otree.offset[a], otree.invradius[a]
-    x = f32((f64(target) - off) / inv)
-    for _ in range(4096):
-        t = f32(off + f32(inv * x))
-        if t == target:
-            return x
-        x = np.nextafter(x, f32(np.inf) if t < target else f32(-np.inf))
-    raise AssertionError("no world coordinate maps onto the face plane")
-
-
-def _cameras(otree):
-    """two axis-aligned cameras whose origins lie on cell-face planes in the two axes across the view direction:
-    one outside the box looking down -z, one inside looking down -x"""
-    N = otree.N
-    faces = (f32(0.5), f32(0.25)) if N != 3 else (f32(1.0 / 3.0), f32(2.0 / 3.0))
-    out = []
-    for rot, axes, along in ((np.eye(3), (0, 1), (2, 1.35)), (np.array([[0, 0, 1], [1, 0, 0], [0, 1, 0]]), (1, 2), (0, 0.7))):
-        c2w = np.eye(4, dtype=f32)
-        c2w[:3, :3] = rot
-        for a, t in zip(axes, faces):
-            c2w[a, 3] = _face_world(otree, a, t)
-        c2w[along[0], 3] = _to_world(otree, [[along[1]] * 3])[0, along[0]]
-        out.append(c2w)
-    return out
-
-
-CAM_W, CAM_H, CAM_F = 24, 24, 16.0
-
-
-def _ray_sets(name, otree, pts):
-    """-> list of (set name, origins, dirs, step_size, background)"""
-    rs = np.random.RandomState(7 + sum(map(ord, name)))
-    rad = 0.5 / otree.invradius.astype(f64)
-    cen = (0.5 - otree.offset.astype(f64)) / otree.invradius.astype(f64)
-    cams = [OO.persp_rays(c, CAM_W, CAM_H, CAM_F) for c in _cameras(otree)]
-    if SPECS[name][5] is None:
-        o = np.repeat(pts, 96, axis=0)
-        return [("chain_points", o, _unit_rand(rs, o.shape[0]), 2e-6, 0.25),
-                ("camera_out", cams[0][0], cams[0][1], 2e-6, 1.0),
-                ("camera_in", cams[1][0], cams[1][1], 2e-6, 0.25)]
-    n = 384
-    o = (cen + 3.0 * rad.max() * _unit_rand(rs, n)).astype(f32)
-    tgt = pts[rs.randint(0, pts.shape[0], n)] + (rs.uniform(-0.02, 0.02, (n, 3)) * rad).astype(f32)
-    d = (tgt - o) / np.linalg.norm(tgt - o, axis=1, keepdims=True)
-    d[: n // 8] *= -1.0                                                   # some miss the box
-    inside = np.concatenate([pts[rs.randint(0, pts.shape[0], n // 2)],      # in occupied cells
-                             (cen + rad * rs.uniform(-0.95, 0.95, (n - n // 2, 3)))]).astype(f32)
-    return [("orbit", o, d.astype(f32), 1e-5, 1.0),
-            ("inside", inside, _unit_rand(rs, n), 1e-3, 0.25),
-            ("camera_out", cams[0][0], cams[0][1], 1e-5, 0.25),
-            ("camera_in", cams[1][0], cams[1][1], 1e-3, 1.0)]
-
-
-@functools.lru_cache(maxsize=None)
-def world(name):
-    t0 = time.time()
-    otree, refines, pts = _build(name)
-    sets = []
-    for sname, o, d, step, bg in _ray_sets(name, otree, pts):
-        v = d.copy()
-        vis = OO.march_visits(otree, o, d, v, step, bg)
-        visf = OO.march_visits(otree, o, d, v, step, bg, STOP, STOP)
-        sets.append(dict(name=sname, o=o, d=d, v=v, step=step, bg=bg, vis=vis, visf=visf))
-    return dict(otree=otree, refines=refines, pts=pts, sets=sets, build_s=time.time() - t0)
-
-
-@functools.lru_cache(maxsize=None)
-def device_tree(name):
-    return to_device_tree(world(name)["otree"])
-
-
-# ---------------------------------------------------------------------------------------------------------
-# references shaded from a visit list
-# ---------------------------------------------------------------------------------------------------------
-def _layout(otree):
-    rgba = str(otree.data_format).upper().startswith("RGBA")
-    return rgba, (1 if rgba else (otree.data_dim - 1) // 3)
-
-
-def _rows(otree, leaf):
-    return otree.data.reshape(-1, otree.data_dim)[leaf]
-
-
-def _first(ray, R):
-    return np.searchsorted(ray, np.arange(R))
-
-
-def _excl(x, ray, first):
-    """exclusive prefix sum of x within each ray's (contiguous) segment"""
-    c = np.cumsum(x) - x
-    return c - c[first[ray]] if x.size else c
-
-
-def fwd64(otree, vis, v, bg, sigma_thresh=0.0, rows=None, delta_t=None):
-    """fp64 forward of the march in `vis` on the fp32 tree data -> dict (rgb [R,3], U [R,3] the bar unit / 2^-24, and
-    the per-visit quantities the backward needs)"""
-    rgba, K = _layout(otree)
-    ray, R = vis["ray"], vis["miss"].shape[0]
-    rows = (_rows(otree, vis["leaf"]) if rows is None else rows).astype(f64)
-    dt = (vis["delta_t"] if delta_t is None else delta_t).astype(f64)
-    ds = vis["delta_scale"].astype(f64)[ray]
-    basis = np.ones((R, 1)) if rgba else _sh64(K, v)
-    b = basis[ray]
-    babs = np.abs(basis) + (0.0 if rgba else 1.0)   # a basis value's rounding is absolute (its polynomial cancels)
-    sig = rows[:, -1]
-    hit = sig > sigma_thresh
-    tau = np.where(hit, dt * ds * sig, 0.0)
-    first = _first(ray, R)
-    S = _excl(tau, ray, first)
-    T = np.exp(-S)
-    w = np.where(hit, T * -np.expm1(-tau), 0.0)
-    coef = rows[:, :3 * K].reshape(-1, 3, K)
-    pre = np.einsum("vk,vck->vc", b, coef)
-    apre = np.einsum("vk,vck->vc", babs[ray], np.abs(coef))
-    col = 1.0 / (1.0 + np.exp(-pre))
-    out = np.stack([np.bincount(ray, w * col[:, c], minlength=R) for c in range(3)], axis=1)
-    tend = np.exp(-np.bincount(ray, tau, minlength=R))
-    stopped = vis["stopped"] if sigma_thresh > 0 else np.zeros(R, dtype=bool)
-    scale = 1.0 / np.where(stopped, 1.0 - tend, 1.0)[:, None]          # early termination renormalises
-    out = np.where(stopped[:, None], out * scale, out + tend[:, None] * bg)
-    nh = np.bincount(ray, hit, minlength=R)
-    U = (1.0 + nh + np.bincount(ray, tau, minlength=R))[:, None] + np.stack(
-        [np.bincount(ray, w * apre[:, c], minlength=R) for c in range(3)], axis=1)
-    U = U * scale
-    return dict(rgb=out, U=U, hit=hit, tau=tau, S=S, T=T, w=w, col=col, apre=apre, basis=basis, babs=babs, tend=tend,
-                dt=dt, ds=ds,
-                nh_before=_excl(hit.astype(f64), ray, first), first=first)
-
-
-def bwd64(otree, vis, f, g, gerr, bg):
-    """fp64 backward (both svox passes) from the forward `f` of the same visit list and the upstream gradient g [R,3].
-    -> (touched packed leaves [U], gradient [U, D], bar unit / 2^-24 [U, D]); gerr [R,3] bounds the error of g in the
-    forward's unit."""
-    rgba, K = _layout(otree)
-    D = otree.data_dim
-    ray, R = vis["ray"], vis["miss"].shape[0]
-    h = np.nonzero(f["hit"])[0]
-    r = ray[h]
-    s, w, T, tau, S = f["col"][h], f["w"][h], f["T"][h], f["tau"][h], f["S"][h]
-    gh, gabs = g[r], (np.abs(g) + gerr)[r]
-    b = f["basis"][r]
-    tnext = T * np.exp(-tau)
-    # pass 1: colour
-    coef = w[:, None] * s * (1.0 - s) * gh                                       # [H,3]
-    dcol = (coef[:, :, None] * b[:, None, :]).reshape(-1, 3 * K)
-    depth = 1.0 + f["nh_before"][h] + S
-    # the weight carries T_j's rounding (1 - att cancels when tau is small), s (1 - s) the absolute rounding of 1 - s
-    ds1 = s * (1.0 - s)
-    acol = ((gabs * (ds1 * T[:, None] + w[:, None] * (ds1 * (depth[:, None] + f["apre"][h]) + 1.0)))[:, :, None]
-            * f["babs"][r][:, None, :]).reshape(-1, 3 * K)
-    # pass 2: density, accum_j = sum_{i > j} w_i total_i + T_end * bg * sum(g)
-    total = (s * gh).sum(axis=1)
-    wt = np.zeros(ray.shape[0])
-    wt[h] = f["w"][h] * total
-    after = np.bincount(ray, wt, minlength=R)[ray] - (_excl(wt, ray, f["first"]) + wt)
-    accum = after[h] + f["tend"][r] * bg * g[r].sum(axis=1)
-    dsig = f["dt"][h] * f["ds"][h] * (total * tnext - accum)
-    asig = f["dt"][h] * f["ds"][h] * ((s * gabs).sum(axis=1) * tnext * (depth + tau) + (gabs * f["U"][r]).sum(axis=1))
-    uniq, inv = np.unique(vis["leaf"][h], return_inverse=True)
-    grad = np.zeros((uniq.size, D))
-    unit = np.zeros((uniq.size, D))
-    for c in range(3 * K):
-        grad[:, c] = np.bincount(inv, dcol[:, c], minlength=uniq.size)
-        unit[:, c] = np.bincount(inv, acol[:, c], minlength=uniq.size)
-    grad[:, D - 1] = np.bincount(inv, dsig, minlength=uniq.size)
-    unit[:, D - 1] = np.bincount(inv, asig, minlength=uniq.size)
-    return uniq, grad, unit
+_record = functools.partial(record, "parity_octree_march.json")
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -399,7 +109,6 @@ def test_visit_list_reproduces_volume_render(N, fmt):
 # ---------------------------------------------------------------------------------------------------------
 # GPU
 # ---------------------------------------------------------------------------------------------------------
-NAMES = list(SPECS)
 
 
 def _renderer(name, step, bg):
@@ -413,13 +122,6 @@ def _forward(r, o, d, v, fast, counters=None):
     with torch.no_grad():
         return r.forward(Rays(torch.from_numpy(o), torch.from_numpy(d), torch.from_numpy(v)), fast=fast,
                          counters=counters)
-
-
-def _safe_fast_rays(f, vis):
-    """rays whose fp64 transmittance after every contributing visit stays STOP_MARGIN (relative) away from STOP"""
-    after = f["T"] * np.exp(-f["tau"])
-    near = f["hit"] & (np.abs(after - STOP) <= STOP_MARGIN * STOP)
-    return np.bincount(vis["ray"], near, minlength=vis["miss"].shape[0]) == 0
 
 
 def _guards(otree, vis, v, step, bg, f, unit):
@@ -523,19 +225,6 @@ def test_render_persp_bit_identities(name):
             device_tree(name).grad = None
             assert np.array_equal(img.cpu().numpy().view(np.int32), ref.view(np.int32))
         assert (d == 0).sum() >= 2 * CAM_W          # a pixel row and a pixel column run along cell-face planes
-
-
-def _check_grad(name, otree, got, uniq, grad, unit, allow, tag):
-    """kernel gradient got [n*N^3, D] against the fp64 one: exact 0 off the touched leaves, per-element bar on them"""
-    rest = np.ones(got.shape[0], dtype=bool)
-    rest[uniq] = False
-    n_nonzero_rest = int((got[rest] != 0).sum())
-    assert n_nonzero_rest == 0, (name, tag, n_nonzero_rest)
-    e = np.abs(got[uniq].astype(f64) - grad) / (U24 * np.maximum(unit, 1e-300))
-    e[(unit == 0) & (got[uniq] == 0)] = 0.0
-    worst = float(e.max())
-    assert worst <= allow, (name, tag, worst, np.unravel_index(np.argmax(e), e.shape))
-    return worst
 
 
 @pytest.mark.gpu

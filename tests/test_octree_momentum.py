@@ -9,19 +9,17 @@ renders (`--render_interval`) and octree.evaluation's `--write_vid`.
   on the golden scene against the executed reference; the two CLIs end to end.
 """
 import functools
-import json
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
 from oracle import octree_oracle as OO
+from tests.support.octree_scenes import _cli, _scene
+from tests.support.records import record
 
 f32, f64 = np.float32, np.float64
 U24 = 2.0 ** -24
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 RUNS = {"momentum": False, "nesterov": True}           # golden run name -> nesterov
 
 
@@ -49,14 +47,7 @@ def _golden_tree(z):
     return tree
 
 
-def _record(name, payload):
-    """measured errors, kept beside tests/test_octree.py's records"""
-    from tests.test_octree import OUT
-    os.makedirs(OUT, exist_ok=True)
-    path = os.path.join(OUT, "parity_octree_momentum.json")
-    data = json.load(open(path)) if os.path.exists(path) else {}
-    data[name] = payload
-    json.dump(data, open(path, "w"), indent=1)
+_record = functools.partial(record, "parity_octree_momentum.json")
 
 
 def _psnr(mse):
@@ -181,7 +172,7 @@ def test_render_interval_images_match_the_reference_writes(golden_dir, run):
 # ---------------------------------------------------------------------------------------------------------
 @functools.lru_cache(maxsize=None)
 def _production_tree(name):
-    from tests.test_octree_march import _build
+    from tests.support.octree_scenes import _build
     return _build(name)[0]
 
 
@@ -264,7 +255,7 @@ def test_sgd_step_momentum_zero_is_the_plain_kernel_and_buffer_lifetime():
     starts at zero, persists across steps, and clone() / shrink_to_fit() drop it."""
     import torch
     from plenoctree_b200._lib import check, lib, ptr, stream_ptr
-    from tests.test_octree import to_device_tree
+    from tests.support.octree_scenes import to_device_tree
     otree = _production_tree("n3_d4_sh16")
     tree = to_device_tree(otree)
     n = otree.n_internal * otree.N ** 3 * otree.data_dim
@@ -305,7 +296,7 @@ def test_optimize_matches_executed_reference(golden_dir, tmp_path, run):
     --render_interval PNGs (names exact, bytes within the one-LSB truncation of a render equal up to float rounding)."""
     import torch
     from PIL import Image
-    from tests.test_octree import to_device_tree
+    from tests.support.octree_scenes import to_device_tree
     from plenoctree_b200.octree import optimization as OPT
     zs, zm = _golden(golden_dir)
     H, W, focal, step = int(zs["H"]), int(zs["W"]), float(zs["focal"]), float(zs["step_size"])
@@ -342,38 +333,6 @@ def test_optimize_matches_executed_reference(golden_dir, tmp_path, run):
     OPT.optimize(args, to_device_tree(_golden_tree(zs)), list(zs["train_c2w"]), to(zs["train_gt"]),
                  list(zs["val_c2w"]), to(zs["val_gt"]), focal, log=lambda *a: None)
     assert not (tmp_path / "quiet").exists()
-
-
-def _scene(tmp_path):
-    """a Blender-layout scene (the writer tests/test_pipeline.py uses) of 32x32 views of a random SH16 tree, and a
-    perturbed copy of the tree as tree.npz"""
-    import torch
-    from tests.test_octree import look_at_pose, make_tree, to_device_tree
-    from plenoctree_b200.nerf import datasets as D
-    from plenoctree_b200.octree import VolumeRenderer
-    otree = make_tree(61, 3, "SH16")
-    teacher = to_device_tree(otree)
-    W, cam_x = 32, 0.6911112070083618
-    focal = 0.5 * W / np.tan(0.5 * cam_x)
-    poses = {"train": [look_at_pose(s) for s in range(4)], "val": [look_at_pose(s) for s in range(10, 13)],
-             "test": [look_at_pose(s) for s in range(20, 22)]}
-    r = VolumeRenderer(teacher, step_size=1e-3)
-    with torch.no_grad():
-        images = {k: [r.render_persp(p, W, W, focal).clamp_(0, 1).cpu().numpy() for p in ps] for k, ps in poses.items()}
-    D.write_blender_scene(str(tmp_path / "scene"), images, poses, cam_x)
-    student = to_device_tree(otree)
-    torch.manual_seed(2)
-    with torch.no_grad():
-        student.data[..., :-1] += 0.5 * torch.randn_like(student.data[..., :-1])
-    student.save(str(tmp_path / "tree.npz"), compress=False)
-    (tmp_path / "cfg.yaml").write_text("dataset: blender\nfactor: 0\nwhite_bkgd: true\n")
-    return ["--config", str(tmp_path / "cfg"), "--data_dir", str(tmp_path / "scene"), "--renderer_step_size", "1e-3"]
-
-
-def _cli(module, argv):
-    r = subprocess.run([sys.executable, "-m", module] + argv, capture_output=True, text=True, cwd=ROOT, timeout=900)
-    assert r.returncode == 0, (r.stdout[-2000:], r.stderr[-3000:])
-    return r.stdout
 
 
 @pytest.mark.gpu

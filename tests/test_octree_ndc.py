@@ -11,7 +11,6 @@ trees, the fused training pass and extraction's grid-weight mask, and the CLIs t
   directions in place of world ones, and no NDC transform at all, must each miss that bound.
 """
 import functools
-import json
 import os
 import types
 
@@ -20,7 +19,7 @@ import pytest
 
 from oracle import octree_ndc_oracle as ON
 from oracle import octree_oracle as OO
-from tests.test_octree import OUT
+from tests.support.records import record
 
 f32, f64 = np.float32, np.float64
 U24 = 2.0 ** -24
@@ -30,13 +29,7 @@ NDC_RAY_ULPS = 0        # kernel NDC rays against the float32 oracle: same opera
 PSNR_BOUND = 18.0
 
 
-def _record(name, payload):
-    os.makedirs(OUT, exist_ok=True)
-    path = os.path.join(OUT, "parity_octree_ndc.json")
-    data = json.load(open(path)) if os.path.exists(path) else {}
-    data[name] = payload
-    json.dump(data, open(path, "w"), indent=1)
-    print(name, json.dumps(payload))
+_record = functools.partial(record, "parity_octree_ndc.json", echo=True)
 
 
 def _ulps(a, b):
@@ -191,8 +184,8 @@ def ndc_cameras():
 @functools.lru_cache(maxsize=None)
 def device_tree(name):
     """a device copy of test_octree_march's tree `name` of this module's own (that module's SGD test steps its copy)"""
-    from tests.test_octree import to_device_tree
-    from tests.test_octree_march import world
+    from tests.support.octree_scenes import to_device_tree
+    from tests.support.octree_scenes import world
     return to_device_tree(world(name)["otree"])
 
 
@@ -232,7 +225,7 @@ def test_ndc_ray_kernel_matches_oracle():
 
 
 def _march_names():
-    from tests.test_octree_march import NAMES
+    from tests.support.octree_scenes import NAMES
     return NAMES
 
 
@@ -243,7 +236,8 @@ def test_render_backward_depth_on_ndc_rays(name):
     test_octree_march.py's fp64 bars; depth and acc bit-identical to the explicit-ray entry point on the NDC rays"""
     import torch
     from plenoctree_b200.octree import Rays
-    from tests.test_octree_march import GRAD_ALLOW, RGB_ALLOW, _check_grad, bwd64, fwd64, world
+    from tests.support.octree_refs import GRAD_ALLOW, RGB_ALLOW, _check_grad, bwd64, fwd64
+    from tests.support.octree_scenes import world
     otree = world(name)["otree"]
     tree = device_tree(name)
     step, bg = 1e-3, 1.0
@@ -289,7 +283,7 @@ def test_render_backward_depth_on_ndc_rays(name):
 def test_compressed_tree_renders_ndc_bit_identical_to_decompressed(name, i):
     import torch
     from plenoctree_b200.octree import Rays
-    from tests.test_octree_compressed import _pair
+    from tests.support.octree_scenes import _pair
     q, ref = _pair(name, i)
     rq, rf = _renderer(q, 1e-3, 1.0), _renderer(ref, 1e-3, 1.0)
     contributing = 0
@@ -314,7 +308,8 @@ def test_train_pass_ndc_matches_fp64(name):
     """the fused NDC training pass: its image equals render_persp in NDC bit for bit; its gradient is exactly 0 off
     the oracle's leaf path and within test_octree_march.py's training bar on it; the squared error within its bar"""
     import torch
-    from tests.test_octree_march import RGB_ALLOW, SQ_ALLOW, TRAIN_ALLOW, _check_grad, bwd64, fwd64, world
+    from tests.support.octree_refs import RGB_ALLOW, SQ_ALLOW, TRAIN_ALLOW, _check_grad, bwd64, fwd64
+    from tests.support.octree_scenes import world
     otree = world(name)["otree"]
     tree = device_tree(name)
     step = 1e-3
@@ -349,7 +344,7 @@ def test_train_pass_ndc_matches_fp64(name):
 
 def _grid_ndc_march(reso, cams):
     """test_grid_weights.march with the cameras' NDC rays"""
-    from tests.test_grid_weights import STEP, geometry, merge, per_voxel, shade64, sigma_host
+    from tests.support.grid_weights import STEP, geometry, merge, per_voxel, shade64, sigma_host
     off, inv = geometry()
     parts, visits = [], 0
     for c2w in cams:
@@ -370,8 +365,8 @@ def test_grid_weights_ndc_exact_path_and_values(reso):
     import torch
     from plenoctree_b200.octree.extraction import calculate_grid_weights
     from plenoctree_b200.octree.renderer import NDCConfig
-    from tests.test_grid_weights import STEP, WEIGHT_ALLOW, check_launch, device_sigma, geometry, take
-    from tests.test_grid_weights import cam_rows
+    from tests.support.grid_weights import STEP, WEIGHT_ALLOW, check_launch, device_sigma, geometry, take
+    from tests.support.grid_weights import cam_rows
     from plenoctree_b200 import _lib
     from plenoctree_b200._lib import check, lib, ptr, stream_ptr
     import ctypes

@@ -5,6 +5,7 @@ mains with the reference's flag names and a YAML config:
     -> tree.npz -> octree.optimization -> tree_opt.npz -> octree.evaluation
 
 CPU part: flags / YAML / dataset loader / SSIM golden.  GPU part: the whole chain on 48x48 images."""
+import functools
 import json
 import os
 
@@ -12,29 +13,11 @@ import numpy as np
 import pytest
 import torch
 
-
-def _set_flags(**kw):
-    from plenoctree_b200.nerf import flags as F
-    F.define_flags()
-    if not F.FLAGS.is_parsed():
-        F.FLAGS.mark_as_parsed()
-    for k, v in kw.items():
-        setattr(F.FLAGS, k, v)
-    return F.FLAGS
+from tests.support.model_flags import _set_flags
+from tests.support.records import record
 
 
-def _record_pipeline(name, payload):
-    out = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out")
-    os.makedirs(out, exist_ok=True)
-    path = os.path.join(out, "pipeline.json")
-    data = {}
-    if os.path.exists(path):
-        try:
-            data = json.load(open(path))
-        except Exception:   # noqa: BLE001
-            data = {}
-    data[name] = payload
-    json.dump(data, open(path, "w"), indent=1)
+_record_pipeline = functools.partial(record, "pipeline.json")
 
 
 def test_flags_yaml_and_scope(tmp_path):

@@ -9,8 +9,8 @@ GPU: the training stages of each encoder against fp64 built from the kernels' ow
 (test_net_activation._check_level), the evaluators against the training forward, legacy against standard order, the default
 encoder against the parent's entry points, and the CLI chain with a non-default encoder."""
 import ctypes
+import functools
 import os
-import types
 
 import numpy as np
 import pytest
@@ -19,6 +19,8 @@ import torch
 from oracle import nerf_sh_oracle as O
 from oracle import posenc_oracle as PO
 from plenoctree_b200 import layouts as L
+from tests.support.model_flags import _gpu_params, _scope_args
+from tests.support.records import record
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLDEN = os.path.join(HERE, "golden", "ref_posenc.npz")
@@ -35,14 +37,6 @@ def _tag(pe):
 
 def _g():
     return np.load(GOLDEN)
-
-
-def _scope_args(**kw):
-    base = dict(use_viewdirs=False, sg_dim=-1, dataset="blender", net_depth=8, net_width=256, skip_layer=4,
-                min_deg_point=0, max_deg_point=10, net_activation="relu", rgb_activation="sigmoid",
-                sigma_activation="relu", legacy_posenc_order=False, render_path=False, spherify=False)
-    base.update(kw)
-    return types.SimpleNamespace(**base)
 
 
 # =====================================================================================================================
@@ -249,15 +243,6 @@ def test_no_gpu_descriptor_calls_fail_loudly():
 # =====================================================================================================================
 # GPU
 # =====================================================================================================================
-def _gpu_params(pe, sh, seed):
-    """two MLPs of the oracle's initialisation for encoder pe, Dense_8 scaled by 30 (as test_train_stages._params)"""
-    out = []
-    w_off = L.flat_offsets(L.K_of(sh), PO.width(pe))[0]
-    for s in (seed, seed + 1):
-        f = PO.init_flat_params(sh, s, bias_scale=0.05, pe=pe)
-        f[w_off[8]:w_off[8] + 256] *= 30.0
-        out.append(f)
-    return out
 
 
 def _model(pe, sh=3, R=24, nc=32, nf=64, nsp=64, seed=17):
@@ -306,25 +291,7 @@ def _oracle_grad(m, ctx, pe, sh, precision=1):
     return np.concatenate([gc, gf])
 
 
-def _ref_features(x, pe):
-    """fp64 sines of the kernel's fp32 arguments: [M, W - 3] in the encoder's column order"""
-    cols = []
-    half_pi = torch.tensor(np.float32(np.pi / 2), device=x.device)
-    for kind, j, c in PO.feature_index(pe)[3:]:
-        xb = x[:, c] * float(2 ** j)                                 # exact fp32 product
-        cols.append(torch.sin((xb if kind == "sin" else xb + half_pi).double()))
-    return torch.stack(cols, 1) if cols else torch.zeros(x.shape[0], 0, dtype=torch.float64, device=x.device)
-
-
-def _record(name, payload):
-    """measured errors go beside the other parity records (tests/test_train.py: OUT)"""
-    import json
-    from tests.test_train import OUT
-    os.makedirs(OUT, exist_ok=True)
-    path = os.path.join(OUT, "posenc.json")
-    data = json.load(open(path)) if os.path.exists(path) else {}
-    data[name] = payload
-    json.dump(data, open(path, "w"), indent=1, default=float)
+_record = functools.partial(record, "posenc.json")
 
 
 @pytest.mark.gpu
@@ -332,7 +299,7 @@ def _record(name, payload):
 def test_train_stages_posenc(pe):
     """stages of every level against fp64 built from the kernels' own saved tiles (test_net_activation._check_level
     with the encoder), then the compact flat gradient against the fp64 oracle of the encoder (test_train.py's gate)"""
-    from tests import test_net_activation as NT
+    from tests.support import model_flags as NT
     sh, R = 3, 24
     m = _model(pe, sh, R)
     state, ctx = _train_call(m, R)
@@ -518,7 +485,7 @@ def test_x3_training_with_posenc():
 def test_cli_chain_with_posenc_flags(tmp_path):
     """nerf_sh.train with max_deg_point 8 and legacy_posenc_order learns a synthetic scene and its checkpoint reloads;
     nerf_sh.eval, octree.extraction, octree.optimization and octree.evaluation run on that model"""
-    from tests.test_pipeline import _set_flags
+    from tests.support.model_flags import _set_flags
     from plenoctree_b200.nerf import checkpoints as C, datasets as D
     from plenoctree_b200.nerf.models import NerfModel, Rays
     from plenoctree_b200.nerf.utils import generate_rays, pose_spherical, render_image

@@ -173,7 +173,7 @@ def test_point_stage_sigma_and_a(pe):
     """One trunk pass (the saving fp16 forward) gives raw sigma bit-identical to the sigma sweeps' forward on the
     same blob, and a_p = h7 W + b within the fp16 point-evaluation bound of tests/test_eval_points.py."""
     from plenoctree_b200 import ops
-    from tests.test_eval_points import TOL_FP16_ANY
+    from tests.support.eval_stages import TOL_FP16_ANY
     layers, nerf = _model(12, pe)
     pts = _points(3000)                                     # not a multiple of the 128-row tile
     a, sig = nerf.point_stage(pts)

@@ -18,7 +18,7 @@ Every workspace and output starts as 0xFF or a NaN canary.  Each check that comp
 against the reference of a plausible mistake (guard_*), which must miss its bar by GUARD.  The measured maxima go to
 parity_projection_stages.json beside the other parity records (tests/test_train.py: OUT).
 """
-import json
+import functools
 import math
 import os
 import time
@@ -31,10 +31,11 @@ from oracle import nerf_sh_oracle as O
 from oracle import posenc_oracle as PO
 from oracle import projection_oracle as PJ
 from plenoctree_b200 import layouts as L
-from tests.test_train import OUT
+from tests.support.mlp_stages import Stats
+from tests.support.model_flags import CANARY, _canary, _points, _run_points
+from tests.support.records import record
 
 U = 2.0 ** -24
-CANARY = 0x7FBADBAD         # a NaN bit pattern behind every output
 GUARD = 10.0
 ENCODERS = ((0, 10, False), (0, 10, True), (2, 8, True), (0, 0, False), (9, 10, True))   # test_flag_matrix.ENCODERS
 
@@ -54,12 +55,7 @@ ROWS_ALLOW = 1.0            # [0.25 on the kernel's own inputs; 0.18 against the
 GOLDEN_REL = 1e-5
 
 
-def _record(name, payload):
-    os.makedirs(OUT, exist_ok=True)
-    path = os.path.join(OUT, "parity_projection_stages.json")
-    data = json.load(open(path)) if os.path.exists(path) else {}
-    data[name] = payload
-    json.dump(data, open(path, "w"), indent=1, default=float)
+_record = functools.partial(record, "parity_projection_stages.json")
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -69,20 +65,6 @@ def _file_wall_time():
     yield
     if torch.cuda.is_available():
         _record("wall_s", time.time() - t0)
-
-
-class _Stats:
-    def __init__(self):
-        self.d = {}
-
-    def max(self, key, val):
-        self.d[key] = max(self.d.get(key, float("-inf")), float(val))
-
-    def min(self, key, val):
-        self.d[key] = min(self.d.get(key, float("inf")), float(val))
-
-    def add(self, key, val):
-        self.d[key] = self.d.get(key, 0) + int(val)
 
 
 def _ulp32(x):
@@ -290,11 +272,6 @@ def test_cells_matrix_covers_every_pair():
 # =====================================================================================================================
 # GPU helpers
 # =====================================================================================================================
-def _canary(shape, tail=1024):
-    """(int32 buffer of the canary, float32 view of its first prod(shape) words)"""
-    n = int(np.prod(shape))
-    buf = torch.full((n + tail,), CANARY, dtype=torch.int32, device="cuda")
-    return buf, buf[:n].view(torch.float32).view(shape)
 
 
 def _tail_ok(buf, shape):
@@ -305,28 +282,10 @@ def _mlps(seed, pe, deg_view):
     return {"MLP_0": PJ.init_params(seed, pe, deg_view), "MLP_1": PJ.init_params(seed + 1, pe, deg_view)}
 
 
-def _points(n, seed):
-    rs = np.random.RandomState(seed)
-    return torch.from_numpy(rs.uniform(-1.2, 1.2, size=(n, 3)).astype(np.float32)).cuda()
-
-
 def _sigma_flat(layers):
     """the plain-RGB (sh_deg -1) flat parameters of VanillaNerf's sigma blob: the trunk, Dense_8, zero rgb columns"""
     return np.concatenate([np.asarray(a, np.float32).reshape(-1) for k, b in layers[:9] for a in (k, b)] +
                           [np.zeros(256 * 3 + 3, np.float32)])
-
-
-def _run_points(nerf, pts):
-    """pob_sh_proj_points on a 0xFF workspace and canary outputs -> (ws, a, sigma, a_buf, sigma_buf)"""
-    from plenoctree_b200._lib import check, lib, posenc_ref, ptr, stream_ptr
-    m = pts.shape[0]
-    ws = torch.full((int(lib.pob_sh_proj_points_workspace_bytes(m)),), 0xFF, dtype=torch.uint8, device="cuda")
-    ab, a = _canary((m, 128))
-    sb, s = _canary((m,))
-    check(lib.pob_sh_proj_points(ptr(nerf.sigma_blob), posenc_ref(nerf._pe), ptr(pts), m, ptr(nerf.head_w),
-                                 ptr(nerf.head_b), ptr(ws), ptr(a), ptr(s), stream_ptr()))
-    torch.cuda.synchronize()
-    return ws, a, s, ab, sb
 
 
 def _ws_views(ws, m):
@@ -338,15 +297,15 @@ def _ws_views(ws, m):
 
 
 def _alt_pe(pe):
-    from tests.test_flag_matrix import _alt_pe as alt
+    from tests.support.model_flags import _alt_pe as alt
     return alt(pe)
 
 
 def _check_points(nerf, layers, pe, pts, ws, a, sig, st):
     """A: every stage of one pob_sh_proj_points call against fp64 of the kernel's own previous stage"""
-    from tests.test_net_activation import _sin_excess
-    from tests.test_posenc import _ref_features
-    from tests.test_train_stages import FWD_ALLOW, _gemm_excess
+    from tests.support.model_flags import _sin_excess
+    from tests.support.model_flags import _ref_features
+    from tests.support.mlp_stages import FWD_ALLOW, _gemm_excess
     dev = pts.device
     m = pts.shape[0]
     EW = PO.width(pe)
@@ -432,12 +391,12 @@ def test_point_stage_from_saved_tiles(pe, monkeypatch):
     """posenc tile, h_0..h_7, mask words, raw sigma and a_p of pob_sh_proj_points against fp64 of the kernel's own
     previous stage, at ragged and tile-edge sizes; the last size at 16 SMs (9 tiles per CTA: every ring phase)"""
     from plenoctree_b200.octree.projection import VanillaNerf
-    from tests.test_sm_splits import _set_sms
-    from tests.test_train_stages import FWD_ALLOW
+    from tests.support.model_flags import _set_sms
+    from tests.support.mlp_stages import FWD_ALLOW
     t0 = time.time()
     layers = PJ.init_params(41, pe, 4)
     nerf = VanillaNerf({"MLP_0": layers}, pe, 4, num_fine_samples=0)
-    st = _Stats()
+    st = Stats()
     st.max("head_err_over_half_ulp", _head_half_ulp(nerf, layers))
     for i, m in enumerate(A_SIZES):
         if m == A_SIZES[-1]:
@@ -527,7 +486,7 @@ def test_direction_tables_at_fp32_arguments(deg_view, legacy):
     """directions against the host Philox and fp64 at the kernel's fp32 arguments, t_d against fp64 sines of the
     fp32 posenc arguments the reference forms, the SH basis (sh_deg 0..4) against fp64 of the kernel's directions"""
     nerf = _dir_model(deg_view, legacy)
-    st = _Stats()
+    st = Stats()
     for sh in range(5):
         tables, ok = _tables(nerf, sh, 300, 3 + sh, 2, seed=5 + sh)
         st.add("tails_written", int(not ok))
@@ -541,7 +500,7 @@ def test_direction_table_edges():
     """n_dirs at the 32-direction CTA edges and 10 000, 65 535 blocks of one direction, block indices across the
     counter's high word; a block's directions do not depend on the call it is drawn in; uniform on the sphere"""
     nerf = _dir_model(4, False)
-    st = _Stats()
+    st = Stats()
     for D in (1, 31, 32, 33, 10000):
         tables, ok = _tables(nerf, 4, D, 11, 2, seed=21)
         st.add("tails_written", int(not ok))
@@ -660,7 +619,7 @@ def test_leaf_rows_against_fp64(row):
     tables, ok = _tables(nerf, sh, D, 9, n_blk, seed=77)
     a, sig = nerf.point_stage(pts)
     out, tail = _cells(nerf, a, sig, S, sh, tables, cpb, n_cells)
-    st = _Stats()
+    st = Stats()
     st.add("tails_written", int(not ok) + int(not tail))
     leaves = _leaf_sample(n_cells, cpb, max(1, 64 // S), S, D, np.random.RandomState(S + D))
     _check_rows(out, nerf, a, sig, S, sh, tables, cpb, leaves, st)
@@ -686,7 +645,7 @@ def test_production_launch():
     b0 = 5
     out = P.project_leaves(nerf, sh, D, pts, S, b0)
     torch.cuda.synchronize()
-    st = _Stats()
+    st = Stats()
     st.add("rows_nonfinite", int((~torch.isfinite(out)).sum()))
     a, sig = nerf.point_stage(pts.reshape(-1, 3))
     tables, ok = _tables(nerf, sh, D, b0, nb, seed=P.PROJ_SEED)
@@ -752,7 +711,7 @@ def test_chain_against_the_executed_reference(golden_dir):
     directions, pob_sh_proj_cells at S = 1: the executed reference's coefficients and sigma for sh_deg 1..4 within
     its fp32 rounding + the point stage's measured error carried forward + the rows' rounding bound"""
     from plenoctree_b200.octree.projection import VanillaNerf
-    from tests.test_eval_points import TOL_FP16_ANY
+    from tests.support.eval_stages import TOL_FP16_ANY
     z = np.load(os.path.join(golden_dir, "ref_projection.npz"))
     mlps = {"MLP_0": PJ.init_params(int(z["seeds"][0])), "MLP_1": PJ.init_params(int(z["seeds"][1]))}
     nerf = VanillaNerf(mlps, (0, 10, False), 4, num_fine_samples=128)
@@ -768,7 +727,7 @@ def test_chain_against_the_executed_reference(golden_dir):
     enc = PO.posenc(torch.from_numpy(d32).double(), 0, 4).to(dev)
     t64 = (enc @ torch.from_numpy(mlps["MLP_1"][10][0][256:]).double().to(dev)).T.contiguous()      # [128, D]
     t32 = t64.float()
-    st = _Stats()
+    st = Stats()
     for sh in range(1, 5):
         K = (sh + 1) ** 2
         Y64 = O.sh_basis(sh, torch.from_numpy(d32).double().to(dev))
@@ -810,7 +769,7 @@ def test_chain_against_the_oracle_across_flags(pe, deg_view, nfs):
     posenc order, b10 left out of the composed head bias."""
     from plenoctree_b200.octree import projection as P
     from plenoctree_b200.octree.projection import VanillaNerf
-    from tests.test_eval_points import TOL_FP16_ANY
+    from tests.support.eval_stages import TOL_FP16_ANY
     dev = torch.device("cuda")
     mlps = _mlps(61, pe, deg_view)
     nerf = VanillaNerf(mlps, pe, deg_view, num_fine_samples=nfs)
@@ -836,7 +795,7 @@ def test_chain_against_the_oracle_across_flags(pe, deg_view, nfs):
         ref = PJ.leaf_rows(l64(layers), p64.reshape(n, S, 3), d64, sh, pe, deg_view).to(dev)
         return float(((out[:, :-1].double() - ref[:, :-1]).abs() / bnd.clamp_min(1e-300)).max()), ref
 
-    st = _Stats()
+    st = Stats()
     st.add("tails_written", int(not ok) + int(not tail))
     r, ref = ratio(used)
     st.max("oracle_excess", r / ROWS_ALLOW)

@@ -1,40 +1,18 @@
 """GPU parity of the per-ray stages and of NerfModel.__call__ against the CPU oracle
 (BASELINE config 1: 1024 rays x 64 samples, SH16, plus the full 64+128 hierarchical path)."""
-import json
-import os
+import functools
 
 import numpy as np
 import pytest
 import torch
 
+from tests.support.mlp_stages import _rays
+from tests.support.records import record
+
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-OUT = os.path.join(ROOT, "gpurun_out")
 
-
-def _record(name, payload):
-    os.makedirs(OUT, exist_ok=True)
-    path = os.path.join(OUT, "parity_render.json")
-    data = json.load(open(path)) if os.path.exists(path) else {}
-    data[name] = payload
-    json.dump(data, open(path, "w"), indent=1)
-
-
-def _rays(n, seed, radius=4.0):
-    """rays of random spherical poses through random pixels of an 800x800 / focal 1111 camera."""
-    from oracle import nerf_sh_oracle as O
-    rs = np.random.RandomState(seed)
-    o = np.zeros((n, 3), np.float32)
-    d = np.zeros((n, 3), np.float32)
-    for i in range(n):
-        c2w = O.pose_spherical(rs.uniform(-180, 180), rs.uniform(-90, 0), radius)
-        x, y = rs.randint(0, 800), rs.randint(0, 800)
-        cam = np.array([(x - 400) / 1111.1, -(y - 400) / 1111.1, -1.0], np.float32)
-        d[i] = c2w[:3, :3] @ cam
-        o[i] = c2w[:3, 3]
-    v = d / np.linalg.norm(d, axis=-1, keepdims=True)
-    return o, d, v.astype(np.float32)
+_record = functools.partial(record, "parity_render.json")
 
 
 def _lib():

@@ -13,34 +13,20 @@ Bounds (u = 2^-24):
 - G.w = dalpha * delta * exp(-sigma delta) * (-expm1f(-sigma)): test_ray_stages.py's magnitude of the relu factor's
   G.w, plus expm1f's 1 ulp (2 u relative) and the one more product (u / 2): GW_SP_EXTRA = 2.5 u |G.w|.
 """
-import json
+import functools
 import os
-import types
 
 import numpy as np
 import pytest
 import torch
 
-from tests.test_ray_stages import GUARD, GW_BAR, U24, RayCase, _norm, composite_bwd_ref, composite_ref
-from tests.test_train import OUT
-from tests.test_train_stages import CASES
-
-SP_BAR = 4.0            # softplus in the heads epilogue, in units of u * softplus64(x)
-SP_FLOOR = 2.0 ** -148  # absolute: expf's denormal outputs below x = -87
-GW_SP_EXTRA = 2.5       # G.w's extra relative magnitude of the softplus factor, in units of u * |G.w|
+from tests.support.mlp_stages import CASES
+from tests.support.model_flags import SP_BAR, SP_FLOOR, _scope_args, softplus64
+from tests.support.ray_stages import GUARD, GW_BAR, GW_SP_EXTRA, RayCase, U24, _norm, composite_bwd_ref, composite_ref
+from tests.support.records import record
 
 
-def _record(name, payload):
-    os.makedirs(OUT, exist_ok=True)
-    path = os.path.join(OUT, "parity_sigma_activation.json")
-    data = json.load(open(path)) if os.path.exists(path) else {}
-    data[name] = payload
-    json.dump(data, open(path, "w"), indent=1)
-
-
-def softplus64(x):
-    x = torch.as_tensor(x).double()
-    return x.clamp_min(0) + torch.log1p(torch.exp(-x.abs()))
+_record = functools.partial(record, "parity_sigma_activation.json")
 
 
 def _sp_excess(sigma, x):
@@ -140,7 +126,7 @@ def loss_and_grads_act(flat_c, flat_f, sh_deg, rays, pixels, cfg, t_rand, u, sp_
 def test_restated_oracle_with_relu_equals_the_oracle():
     """with relu the restatement above computes what oracle/nerf_sh_oracle.py computes, bit for bit"""
     from oracle import nerf_sh_oracle as O
-    from tests.test_train import _setup
+    from tests.support.mlp_stages import _setup
     fc, ff, rays, px, t_rand, u, sp = _setup(3, 6, 16, 20, 5)
     cfg = dict(num_coarse_samples=64, num_fine_samples=16, near=2.0, far=6.0, white_bkgd=True, sparsity_weight=1e-3,
                sparsity_length=0.05, weight_decay_mult=0.1)
@@ -218,14 +204,6 @@ def test_oracle_loss_matches_executed_reference_softplus(golden_dir):
         _, s_raw = O.eval_points_raw(pf, _t(sp))
         alt = float(g["sparsity_weight"]) * (1.0 - torch.exp(-float(g["sparsity_length"]) * softplus64(s_raw)).mean())
     assert abs(float(alt) - float(g["loss_sp"])) > 100 * 1e-4 * abs(float(g["loss_sp"]))
-
-
-def _scope_args(**kw):
-    a = dict(use_viewdirs=False, sg_dim=-1, dataset="blender", net_depth=8, net_width=256, skip_layer=4, min_deg_point=0,
-             max_deg_point=10, net_activation="relu", rgb_activation="sigmoid", sigma_activation="relu",
-             legacy_posenc_order=False, render_path=False, spherify=False)
-    a.update(kw)
-    return types.SimpleNamespace(**a)
 
 
 def test_check_scope_sigma_activation():
@@ -312,7 +290,7 @@ class SoftplusCase(RayCase):
 
     def model(self, max_rays=None):
         from plenoctree_b200.nerf.models import NerfModel
-        from tests.test_train_stages import _params
+        from tests.support.mlp_stages import _params
         m = NerfModel(sh_deg=self.sh, num_coarse_samples=self.nc, num_fine_samples=self.nf, white_bkgd=self.white,
                       lindisp=self.lindisp, max_rays=max_rays or self.R, sparsity_npoints=self.nsp,
                       sigma_activation="softplus")
@@ -326,7 +304,7 @@ class SoftplusCase(RayCase):
 
 
 def _level_points(ctx, lv, z, sp, dev):
-    from tests.test_eval_stages import _level_rows
+    from tests.support.eval_stages import _level_rows
     return _level_rows(ctx, lv, z, sp, dev)
 
 
@@ -338,7 +316,7 @@ def _softplus_call(case):
     from plenoctree_b200 import layouts as L, ops
     from plenoctree_b200.nerf.models import Rays
     from plenoctree_b200.nerf.train import default_loss_scale
-    from tests.test_train_x3 import _run
+    from tests.support.mlp_x3 import _run
     dev = torch.device("cuda")
     model = case.model()
     n = case.R
@@ -440,7 +418,7 @@ def test_softplus_gradient_vs_fp64_oracle():
     GRAD_GAIN times closer to the fp32 oracle than the fp16 step; the fp16 step within test_train.py's gates"""
     from plenoctree_b200.nerf import train as T
     from plenoctree_b200.nerf.models import NerfModel, Rays
-    from tests.test_train_x3 import FLOOR_SLACK, GRAD_GAIN, LOSS_REL, X3, _oracle_inputs
+    from tests.support.mlp_x3 import FLOOR_SLACK, GRAD_GAIN, LOSS_REL, X3, _oracle_inputs
     R, nf, nsp = 96, 128, 300
     fc, ff, rays, px, t_rand, u, sp = _oracle_inputs(77, 3, R, nf, nsp)
     cfg = dict(num_coarse_samples=64, num_fine_samples=nf, near=2.0, far=6.0, white_bkgd=True,

@@ -24,6 +24,7 @@ and 114 (SH25), the fp16x3 passes at 17 and 61.
 Weight-gradient bar: WG_EPS_W was measured with up to ~1 200 tiles summed per CTA.  At 16 SMs every wgrad CTA sums
 every tile of its level (its role has one CTA per row half), so the cases below keep a level at <= 392 tiles.
 """
+import functools
 import json
 import os
 import re
@@ -34,20 +35,15 @@ import pytest
 import torch
 
 from plenoctree_b200 import layouts as L
-from tests.test_train import OUT
-from tests.test_train_stages import Case
+from tests.support.mlp_stages import Case
+from tests.support.model_flags import _device_sms, _set_sms
+from tests.support.records import ROOT, record
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 COUNTS = (16, 17, 32, 60, 61, 64, 114, "device")
 MIN_SMS = 16
 
 
-def _record(name, payload):
-    os.makedirs(OUT, exist_ok=True)
-    path = os.path.join(OUT, "parity_sm_splits.json")
-    data = json.load(open(path)) if os.path.exists(path) else {}
-    data[name] = payload
-    json.dump(data, open(path, "w"), indent=1, default=float)
+_record = functools.partial(record, "parity_sm_splits.json")
 
 
 # =====================================================================================================================
@@ -115,23 +111,6 @@ def test_split_tables_differ_between_counts():
 # =====================================================================================================================
 # GPU: the count in effect
 # =====================================================================================================================
-def _device_sms():
-    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
-
-
-def _set_sms(monkeypatch, n):
-    """make the library split its work for n SMs ("device": POB_SM_COUNT unset) until the test ends"""
-    from plenoctree_b200._lib import lib
-    dev = _device_sms()
-    if n == "device":
-        monkeypatch.delenv("POB_SM_COUNT", raising=False)
-        n = dev
-    else:
-        if n > dev:
-            pytest.skip(f"{n} SMs: the device has {dev}")
-        monkeypatch.setenv("POB_SM_COUNT", str(n))
-    assert lib.pob_sm_count() == n
-    return n
 
 
 def _counts():
@@ -163,7 +142,7 @@ STAGE_CASES = [
 def test_fp16_stages_at_split(sms, case, monkeypatch):
     """test_train_stages' checks unchanged (0xFF-filled workspace, sensitivity guard on) at this count: forward and
     data gradient against fp64 from their own inputs, weight gradient + reduce against fp64 sums at WG_EPS_W"""
-    from tests import test_train_stages as TS
+    from tests.support import mlp_stages as TS
     table = split_table(sms, L.heads_width(L.K_of(case.sh)))
     monkeypatch.setattr(TS, "_record", lambda name, res: _record(f"fp16_stages/{sms}/{name}", {**res, "split": table}))
     TS._stage_case(case)
@@ -173,7 +152,7 @@ def test_fp16_stages_at_split(sms, case, monkeypatch):
 @pytest.mark.parametrize("case", [Case(3, 96, 64, 128, 300), Case(4, 40, 64, 128, 64)], ids=lambda c: c.name)
 def test_fp16x3_stages_at_split(sms, case, monkeypatch):
     """test_train_x3's checks unchanged: the x3 data gradient and all three wgrad passes run on all `sms` SMs"""
-    from tests import test_train_x3 as TX
+    from tests.support import mlp_x3 as TX
     table = split_table(sms, L.heads_width(L.K_of(case.sh)))
     monkeypatch.setattr(TX, "_record", lambda name, res: _record(f"fp16x3_stages/{sms}/{name}", {**res, "split": table}))
     TX._stage_case_x3(case)
@@ -183,7 +162,7 @@ def test_fp16x3_stages_at_split(sms, case, monkeypatch):
 @pytest.mark.parametrize("case", [Case(3, 96, 64, 128, 300), Case(4, 40, 64, 128, 64)], ids=lambda c: c.name)
 def test_elu_trunk_stages_at_split(sms, case, monkeypatch):
     """test_net_activation's fp16 checks with an elu trunk: its data gradient reads h, not the masks"""
-    from tests import test_net_activation as NA
+    from tests.support import model_flags as NA
     table = split_table(sms, L.heads_width(L.K_of(case.sh)))
     monkeypatch.setattr(NA, "_record", lambda name, res: _record(f"elu_stages/{sms}/{name}", {**res, "split": table}))
     NA._stage_case(case, "elu", 1)
@@ -269,7 +248,7 @@ def test_l2_discard_at_split(sms, sh_deg):
     discards, each dZ / dO tile depends on the split.  Gradient bit-identical, the loss sums (float atomics over rays)
     within test_l2_discard's bar, every workspace byte outside DZ / DO identical."""
     from plenoctree_b200.nerf import train as T
-    from tests import test_l2_discard as LD
+    from tests.support import model_flags as LD
     R = 512
     model = LD._model(sh_deg, LD.NF, 1000, R=R)
     state = T.TrainState(model)
@@ -288,7 +267,7 @@ def test_l2_discard_at_split(sms, sh_deg):
 def test_graph_replay_at_split(sms):
     """a GraphedTrainStep captured at 60 SMs replays the eager train_step at 60 bit for bit (params, Adam moments)"""
     from plenoctree_b200.nerf import train as T
-    from tests import test_l2_discard as LD
+    from tests.support import model_flags as LD
     R = 512
     batch, b12 = LD._batch(R, 13)
     outs = []
@@ -320,7 +299,7 @@ def test_inference_forwards_do_not_depend_on_the_split(sh, monkeypatch):
     from oracle import nerf_sh_oracle as O
     from plenoctree_b200 import ops
     from plenoctree_b200.nerf.models import Rays
-    from tests import test_eval_stages as ES
+    from tests.support import eval_stages as ES
     t0 = time.time()
     dev = torch.device("cuda")
     blob = ES._blob(O.init_flat_params(sh, 43, bias_scale=0.05), sh)
@@ -393,7 +372,7 @@ def test_projection_point_stage_does_not_depend_on_the_split(monkeypatch):
     (h_0..h_7, posenc and mask images) bit-identical at every count, at 9 tiles per CTA of 16 SMs"""
     from plenoctree_b200.octree.projection import VanillaNerf
     from oracle import projection_oracle as PJ
-    from tests.test_projection_stages import _points, _run_points
+    from tests.support.model_flags import _points, _run_points
     nerf = VanillaNerf({"MLP_0": PJ.init_params(45)}, (0, 10, False), 4, num_fine_samples=0)
     M = 9 * MIN_SMS * L.TILE_M + 77
     pts = _points(M, 9)
@@ -471,7 +450,7 @@ def test_out_of_range_counts_are_refused(monkeypatch):
     from plenoctree_b200._lib import PobError, lib, ptr, stream_ptr
     from plenoctree_b200.nerf import train as T
     from plenoctree_b200.nerf.models import Rays
-    from tests import test_eval_stages as ES
+    from tests.support import eval_stages as ES
     dev = torch.device("cuda")
     sh = 3
     blob = ES._blob(O.init_flat_params(sh, 47, bias_scale=0.05), sh)

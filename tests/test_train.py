@@ -1,41 +1,17 @@
 """GPU parity of value_and_grad(loss_fn) + Adam against the CPU oracle's autograd."""
-import json
-import os
+import functools
 
 import numpy as np
 import pytest
 import torch
 
+from tests.support.mlp_stages import _setup
+from tests.support.records import record
+
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-OUT = os.path.join(ROOT, "gpurun_out")
 
-
-def _record(name, payload):
-    os.makedirs(OUT, exist_ok=True)
-    path = os.path.join(OUT, "parity_train.json")
-    data = json.load(open(path)) if os.path.exists(path) else {}
-    data[name] = payload
-    json.dump(data, open(path, "w"), indent=1)
-
-
-def _setup(sh_deg, R, nf, nsp, seed):
-    from oracle import nerf_sh_oracle as O
-    from tests.test_render import _rays
-    fc = O.init_flat_params(sh_deg, seed, bias_scale=0.05)
-    ff = O.init_flat_params(sh_deg, seed + 1, bias_scale=0.05)
-    K = (sh_deg + 1) ** 2
-    for f in (fc, ff):
-        off = O.param_count(sh_deg) - 3 * K - 1 - 256 * 3 * K - 256
-        f[off:off + 256] *= 30.0
-    o, d, v = _rays(R, seed)
-    rs = np.random.RandomState(seed)
-    px = rs.uniform(0, 1, size=(R, 3)).astype(np.float32)
-    t_rand = rs.uniform(0, 1, size=(R, 64)).astype(np.float32)
-    u = rs.uniform(0, 1, size=(R, nf)).astype(np.float32) if nf else None
-    sp = rs.uniform(-1.5, 1.5, size=(nsp, 3)).astype(np.float32) if nsp else None
-    return fc, ff, (o, d, v), px, t_rand, u, sp
+_record = functools.partial(record, "parity_train.json")
 
 
 def _layer_report(g, ref, sh_deg):
@@ -166,7 +142,7 @@ def test_training_reduces_loss():
     """a few hundred steps on a fixed synthetic batch: the loss must go down (teacher = constant colour)."""
     from plenoctree_b200.nerf.models import NerfModel, Rays
     from plenoctree_b200.nerf import train as T
-    from tests.test_render import _rays
+    from tests.support.mlp_stages import _rays
     R = 512
     o, d, v = _rays(R, 4)
     px = np.tile(np.array([[0.8, 0.3, 0.1]], np.float32), (R, 1))
