@@ -93,16 +93,10 @@ SIGNATURES = {
 }
 
 
-class Posenc(_c.Structure):
-    """The point-encoder fields of pob_posenc: posenc(x, min_deg, max_deg, legacy_order); a NULL pointer is
-    (0, 10, 0).  The library also reads the trailing net_activation (NetDesc); ctypes keeps a structure of up to
-    16 bytes in a zero-filled inline buffer, so a bare Posenc reads as a relu trunk."""
-    _fields_ = [("min_deg", _i), ("max_deg", _i), ("legacy_order", _i)]
-
-
-class NetDesc(Posenc):
-    """the whole pob_posenc: Posenc's fields, then net_activation (NET_*; 0 = relu)."""
-    _fields_ = [("net_activation", _i)]
+class NetDesc(_c.Structure):
+    """pob_posenc, the network beyond sh_deg: the point encoder posenc(x, min_deg, max_deg, legacy_order) and the
+    trunk activation net_activation (NET_*).  A NULL pointer is (0, 10, 0, NET_RELU)."""
+    _fields_ = [("min_deg", _i), ("max_deg", _i), ("legacy_order", _i), ("net_activation", _i)]
 
 
 POSENC_DEFAULT = (0, 10, False)   # flags min_deg_point, max_deg_point, legacy_posenc_order of the reference
@@ -118,7 +112,7 @@ def posenc_struct(posenc, net_activation=NET_RELU):
 
 
 def posenc_ref(struct):
-    """pointer argument of a Posenc (None -> NULL)."""
+    """pointer argument of a NetDesc (None -> NULL)."""
     return None if struct is None else _c.addressof(struct)
 
 

@@ -3,7 +3,7 @@ the same names and defaults, and `update_flags` (utils.py:233-244): a YAML file 
 reference's own config files (nerf_sh/config/blender.yaml, tt.yaml) drive this package unchanged.
 
 Flags that select features outside the scope of this path are accepted (so existing command lines keep parsing) and
-rejected by `check_model_scope` (every CLI's check) when set to an unsupported value."""
+rejected by `check_scope` (every CLI's check) when set to an unsupported value."""
 import os
 
 import yaml
@@ -194,8 +194,9 @@ def check_samples(num_coarse_samples, num_fine_samples):
 
 
 def check_scope(args):
-    """features of the reference the relu-trunk path does not cover: fail loudly instead of training something else.
-    A model with another trunk activation is checked by check_model_scope, which every CLI calls."""
+    """features of the reference the NeRF-SH path does not cover (every CLI's check): fail loudly instead of training
+    something else.  The trunk activation is any the kernels build (net_activation_code, which says why it refuses
+    the others)."""
     if args.use_viewdirs:
         raise NotImplementedError("use_viewdirs (vanilla NeRF colour head) is outside the NeRF-SH path")
     if args.sg_dim > 0:
@@ -206,29 +207,12 @@ def check_scope(args):
         raise NotImplementedError("the fused kernel is built for the 8x256 trunk with the skip after layer 4")
     check_posenc(args.min_deg_point, args.max_deg_point)
     check_samples(getattr(args, "num_coarse_samples", 64), getattr(args, "num_fine_samples", 128))
-    if (str(args.net_activation).lower(), str(args.rgb_activation).lower()) != ("relu", "sigmoid"):
-        raise NotImplementedError("activations other than relu (trunk) / sigmoid (rgb)")
+    net_activation_code(args.net_activation)
+    if str(args.rgb_activation).lower() != "sigmoid":
+        raise NotImplementedError(f"rgb_activation {args.rgb_activation!r}: sigmoid expected")
     sigma_activation_code(args.sigma_activation)
     if (args.render_path or args.spherify) and args.dataset != "llff":
         raise ValueError("render_path / spherify apply to the llff dataset only")        # datasets.py:194-195,496-497
-
-
-class _Trunk:
-    """`args` with its net_activation replaced (absl FlagValues cannot be copied field by field)"""
-
-    def __init__(self, args, net_activation):
-        self._args, self.net_activation = args, net_activation
-
-    def __getattr__(self, name):
-        return getattr(self._args, name)
-
-
-def check_model_scope(args):
-    """check_scope for a model with any trunk activation the kernels build: net_activation relu, elu, softplus or
-    tanh in any case (net_activation_code, which refuses the others and says why), every other flag as check_scope
-    has it."""
-    net_activation_code(args.net_activation)
-    check_scope(_Trunk(args, "relu"))
 
 
 class _Override:
@@ -250,6 +234,10 @@ def check_projection_scope(args):
     (net_depth_condition 1, net_width_condition 128), a relu trunk and condition layer, 0 <= deg_view <= 32, and every
     point-posenc, sample, dataset and density flag check_scope accepts.  Training, rendering and evaluating a vanilla
     NeRF stay refused by check_scope."""
+    if str(args.net_activation).lower() != "relu":
+        raise NotImplementedError(
+            f"net_activation {args.net_activation!r}: the projection kernel is built for a relu trunk and condition "
+            "layer")
     sh_deg = int(args.sh_deg)
     if not 1 <= sh_deg <= 4:
         raise NotImplementedError(

@@ -108,6 +108,18 @@ class NerfModel:
         else:
             self.u_table = None
 
+    @classmethod
+    def from_flags(cls, args, *, max_rays, sparsity_npoints=0, device="cuda"):
+        """the model the flags of `args` describe (sh_deg, the sample counts, near / far, white_bkgd, lindisp, the
+        point encoder and both activations).  The caller picks the workspace: max_rays rays per call and the
+        sparsity points of a training step."""
+        return cls(sh_deg=args.sh_deg, num_coarse_samples=args.num_coarse_samples,
+                   num_fine_samples=args.num_fine_samples, near=args.near, far=args.far, white_bkgd=args.white_bkgd,
+                   lindisp=args.lindisp, max_rays=max_rays, sparsity_npoints=sparsity_npoints, device=device,
+                   sigma_activation=args.sigma_activation, min_deg_point=args.min_deg_point,
+                   max_deg_point=args.max_deg_point, legacy_posenc_order=args.legacy_posenc_order,
+                   net_activation=args.net_activation)
+
     # ---- parameters --------------------------------------------------------------------------
     def init_params(self, seed=20200823):
         g = torch.Generator().manual_seed(seed)
@@ -229,23 +241,16 @@ def ctypes_ref(struct):
     return ctypes.addressof(struct)
 
 
-def get_model_state(args, device="cuda", seed=20200823, restore=True):
-    """models.get_model_state (nerf_sh/nerf/models.py:38-49): builds the model from a flags-like object,
-    initialises parameters + Adam moments and, when `restore` and args.train_dir holds a flax-format
-    `checkpoint_<step>`, restores parameters / moments / step from the newest one (checkpoints.py)."""
+def get_model_state(args, device="cuda", seed=20200823, restore=True, *, max_rays, sparsity_npoints=0):
+    """models.get_model_state (nerf_sh/nerf/models.py:38-49): builds the model of the flags `args`
+    (NerfModel.from_flags, with the caller's workspace), initialises parameters + Adam moments and, when `restore`
+    and args.train_dir holds a flax-format `checkpoint_<step>`, restores parameters / moments / step from the newest
+    one (checkpoints.py)."""
     from .train import TrainState
-    model = NerfModel(sh_deg=args.sh_deg, num_coarse_samples=args.num_coarse_samples,
-                      num_fine_samples=args.num_fine_samples, near=args.near, far=args.far,
-                      white_bkgd=args.white_bkgd, lindisp=getattr(args, "lindisp", False),
-                      max_rays=getattr(args, "batch_size", 4096),
-                      sparsity_npoints=getattr(args, "sparsity_npoints", 0), device=device,
-                      sigma_activation=getattr(args, "sigma_activation", "relu"),
-                      min_deg_point=getattr(args, "min_deg_point", 0), max_deg_point=getattr(args, "max_deg_point", 10),
-                      legacy_posenc_order=getattr(args, "legacy_posenc_order", False),
-                      net_activation=getattr(args, "net_activation", "relu"))
+    model = NerfModel.from_flags(args, max_rays=max_rays, sparsity_npoints=sparsity_npoints, device=device)
     model.init_params(seed)
     state = TrainState(model)
-    if restore and getattr(args, "train_dir", None):
+    if restore and args.train_dir:
         from . import checkpoints
         checkpoints.restore_checkpoint(args.train_dir, model, state)
     return model, state

@@ -17,19 +17,11 @@ F.define_flags()
 def main(unused_argv):
     F.update_flags(FLAGS)
     F.check_flags(FLAGS)
-    F.check_model_scope(FLAGS)
+    F.check_scope(FLAGS)
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
     torch.cuda.set_device(dev)
     dataset = datasets.get_dataset("test", FLAGS, device=dev)
-    margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, sigma_activation=FLAGS.sigma_activation,
-                               net_activation=FLAGS.net_activation,
-                               min_deg_point=FLAGS.min_deg_point, max_deg_point=FLAGS.max_deg_point,
-                               legacy_posenc_order=FLAGS.legacy_posenc_order,
-                               num_coarse_samples=FLAGS.num_coarse_samples,
-                               num_fine_samples=FLAGS.num_fine_samples, near=FLAGS.near, far=FLAGS.far,
-                               white_bkgd=FLAGS.white_bkgd, lindisp=FLAGS.lindisp, batch_size=min(FLAGS.chunk, 8192),
-                               sparsity_npoints=0, train_dir=None))
-    model, state = models.get_model_state(margs, device=dev, restore=False)
+    model, state = models.get_model_state(FLAGS, device=dev, restore=False, max_rays=min(FLAGS.chunk, 8192))
     step = checkpoints.restore_checkpoint(FLAGS.train_dir, model, state)
     if step is None:
         raise ValueError(f"no checkpoint_* in {FLAGS.train_dir}")

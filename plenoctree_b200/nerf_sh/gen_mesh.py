@@ -63,18 +63,10 @@ def marching_cubes(model, c1, c2, reso, isosurface, chunk, coarse=False):
 def main(unused_argv):
     F.update_flags(FLAGS)
     F.check_flags(FLAGS, require_data=False)
-    F.check_model_scope(FLAGS)
+    F.check_scope(FLAGS)
     reso, c1, c2 = _triple(FLAGS.reso, int), _triple(FLAGS.c1, float), _triple(FLAGS.c2, float)
     rank, world, dev = _dist.dist_init()
-    margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, sigma_activation=FLAGS.sigma_activation,
-                               net_activation=FLAGS.net_activation,
-                               min_deg_point=FLAGS.min_deg_point, max_deg_point=FLAGS.max_deg_point,
-                               legacy_posenc_order=FLAGS.legacy_posenc_order,
-                               num_coarse_samples=FLAGS.num_coarse_samples,
-                               num_fine_samples=FLAGS.num_fine_samples, near=FLAGS.near, far=FLAGS.far,
-                               white_bkgd=FLAGS.white_bkgd, lindisp=FLAGS.lindisp, batch_size=1024,
-                               sparsity_npoints=0, train_dir=None))
-    model, state = models.get_model_state(margs, device=dev, restore=False)
+    model, state = models.get_model_state(FLAGS, device=dev, restore=False, max_rays=1024)
     if checkpoints.restore_checkpoint(FLAGS.train_dir, model, state) is None:
         raise ValueError(f"no checkpoint_* in {FLAGS.train_dir}")
     mesh_path = os.path.join(FLAGS.train_dir, "mesh.obj")

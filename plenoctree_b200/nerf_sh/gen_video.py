@@ -42,7 +42,7 @@ def orbit_poses(num_views, elevation, radius, up_axis):
 def main(unused_argv):
     F.update_flags(FLAGS)
     F.check_flags(FLAGS, require_data=False)
-    F.check_model_scope(FLAGS)
+    F.check_scope(FLAGS)
     rank, world, dev = _dist.dist_init()
     render_poses = orbit_poses(FLAGS.num_views, FLAGS.elevation, float(FLAGS.radius), FLAGS.up_axis)
     if FLAGS.write_poses and rank == 0:
@@ -52,15 +52,7 @@ def main(unused_argv):
     if FLAGS.intrin is not None:
         K = np.loadtxt(FLAGS.intrin)
         focal = (K[0, 0] + K[1, 1]) * 0.5
-    margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, sigma_activation=FLAGS.sigma_activation,
-                               net_activation=FLAGS.net_activation,
-                               min_deg_point=FLAGS.min_deg_point, max_deg_point=FLAGS.max_deg_point,
-                               legacy_posenc_order=FLAGS.legacy_posenc_order,
-                               num_coarse_samples=FLAGS.num_coarse_samples,
-                               num_fine_samples=FLAGS.num_fine_samples, near=FLAGS.near, far=FLAGS.far,
-                               white_bkgd=FLAGS.white_bkgd, lindisp=FLAGS.lindisp, batch_size=min(FLAGS.chunk, 8192),
-                               sparsity_npoints=0, train_dir=None))
-    model, state = models.get_model_state(margs, device=dev, restore=False)
+    model, state = models.get_model_state(FLAGS, device=dev, restore=False, max_rays=min(FLAGS.chunk, 8192))
     if checkpoints.restore_checkpoint(FLAGS.train_dir, model, state) is None:
         raise ValueError(f"no checkpoint_* in {FLAGS.train_dir}")
     video_dir = os.path.join(FLAGS.train_dir, "video", "e{:03}".format(int(-FLAGS.elevation * 10)))

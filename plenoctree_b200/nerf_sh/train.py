@@ -31,7 +31,7 @@ def main(unused_argv):
     rank, world, dev = _dist_init()
     F.update_flags(FLAGS)
     F.check_flags(FLAGS, world=world)
-    F.check_model_scope(FLAGS)
+    F.check_scope(FLAGS)
     torch.manual_seed(20200823 + rank)
     os.makedirs(FLAGS.train_dir, exist_ok=True)
     render_dir = os.path.join(FLAGS.train_dir, "render")
@@ -44,17 +44,9 @@ def main(unused_argv):
     test_dataset = datasets.get_dataset("test", FLAGS, device=dev)
     h0print("* Load model")
     per_rank = FLAGS.batch_size // world
-    margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, sigma_activation=FLAGS.sigma_activation,
-                               net_activation=FLAGS.net_activation,
-                               min_deg_point=FLAGS.min_deg_point, max_deg_point=FLAGS.max_deg_point,
-                               legacy_posenc_order=FLAGS.legacy_posenc_order,
-                               num_coarse_samples=FLAGS.num_coarse_samples,
-                               num_fine_samples=FLAGS.num_fine_samples, near=FLAGS.near, far=FLAGS.far,
-                               white_bkgd=FLAGS.white_bkgd, lindisp=FLAGS.lindisp,
-                               batch_size=per_rank,   # workspace capacity; test renders chunk by it
-                               sparsity_npoints=FLAGS.sparsity_npoints if FLAGS.sparsity_weight > 0 else 0,
-                               train_dir=FLAGS.train_dir))
-    model, state = models.get_model_state(margs, device=dev, restore=True)
+    model, state = models.get_model_state(
+        FLAGS, device=dev, restore=True, max_rays=per_rank,   # workspace capacity; test renders chunk by it
+        sparsity_npoints=FLAGS.sparsity_npoints if FLAGS.sparsity_weight > 0 else 0)
     model.noise_std = FLAGS.noise_std
     learning_rate_fn = functools.partial(T.learning_rate_decay, lr_init=FLAGS.lr_init, lr_final=FLAGS.lr_final,
                                          max_steps=FLAGS.max_steps, lr_delay_steps=FLAGS.lr_delay_steps,

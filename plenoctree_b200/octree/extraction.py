@@ -347,15 +347,7 @@ def load_nerf(FLAGS, device):
         if mlps is None:
             raise ValueError(f"no checkpoint found in {FLAGS.train_dir}")
         return VanillaNerf(mlps, posenc, FLAGS.deg_view, FLAGS.num_fine_samples, device=device)
-    margs = type("A", (), dict(sh_deg=FLAGS.sh_deg, sigma_activation=FLAGS.sigma_activation,
-                               net_activation=FLAGS.net_activation,
-                               min_deg_point=FLAGS.min_deg_point, max_deg_point=FLAGS.max_deg_point,
-                               legacy_posenc_order=FLAGS.legacy_posenc_order,
-                               num_coarse_samples=FLAGS.num_coarse_samples,
-                               num_fine_samples=FLAGS.num_fine_samples, near=FLAGS.near, far=FLAGS.far,
-                               white_bkgd=FLAGS.white_bkgd, lindisp=FLAGS.lindisp, batch_size=min(FLAGS.chunk, 8192),
-                               sparsity_npoints=0, train_dir=None))
-    nerf, _ = models.get_model_state(margs, device=device, restore=False)
+    nerf, _ = models.get_model_state(FLAGS, device=device, restore=False, max_rays=min(FLAGS.chunk, 8192))
     ok = (checkpoints.restore_model_state_from_jaxnerf(FLAGS.train_dir, nerf) if FLAGS.is_jaxnerf_ckpt
           else checkpoints.restore_model_state(FLAGS.train_dir, nerf))
     if not ok:
@@ -371,7 +363,7 @@ def main(unused_argv):
     if FLAGS.use_viewdirs:
         F.check_projection_scope(FLAGS)
     else:
-        F.check_model_scope(FLAGS)
+        F.check_scope(FLAGS)
     torch.manual_seed(20200823)
     from .._dist import dist_finish, dist_init
     rank, _, dev = dist_init()       # under torchrun: NCCL group, this rank's GPU (x-slabs / leaf blocks / cameras)

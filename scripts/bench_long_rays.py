@@ -21,7 +21,7 @@ from plenoctree_b200.nerf import train as T  # noqa: E402
 from plenoctree_b200.nerf.models import NerfModel, Rays, ctypes_ref  # noqa: E402
 from plenoctree_b200.nerf.rays import random_rays_np  # noqa: E402
 from plenoctree_b200.nerf.utils import generate_rays, pose_spherical, render_image  # noqa: E402
-from scripts.bench_sigma_activation import card, timed  # noqa: E402
+from scripts.bench_model_flags import card, timed  # noqa: E402
 
 CONFIGS = ((64, 128), (128, 256), (128, 384), (256, 768))
 BATCHES = (1024, 4096)

@@ -42,16 +42,16 @@ def _scope(nc, nf):
 def test_sample_counts_accepted(nc, nf):
     from plenoctree_b200.nerf import flags as F
     F.check_samples(nc, nf)
-    F.check_model_scope(_scope(nc, nf))
+    F.check_scope(_scope(nc, nf))
 
 
 @pytest.mark.parametrize("nc,nf", REFUSE)
 def test_sample_counts_refused_with_the_bound(nc, nf):
-    """flags.check_samples, check_model_scope (before any data is loaded) and NerfModel (before any device memory)
+    """flags.check_samples, check_scope (before any data is loaded) and NerfModel (before any device memory)
     refuse the same counts and name the bound"""
     from plenoctree_b200.nerf import flags as F
     from plenoctree_b200.nerf.models import NerfModel
-    for call in (lambda: F.check_samples(nc, nf), lambda: F.check_model_scope(_scope(nc, nf)),
+    for call in (lambda: F.check_samples(nc, nf), lambda: F.check_scope(_scope(nc, nf)),
                  lambda: NerfModel(num_coarse_samples=nc, num_fine_samples=nf, max_rays=8)):
         with pytest.raises((ValueError, NotImplementedError)) as e:
             call()

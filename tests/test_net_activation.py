@@ -179,59 +179,55 @@ def test_reference_loader_reproduced():
         np.testing.assert_array_equal(g[f"{act}_ckpt_raw_rgb_fine"], g[f"{act}_twin_raw_rgb_fine"])
 
 
-def test_check_model_scope_net_activation():
-    """check_model_scope (every CLI's check) accepts the built trunk activations under both namings in any case, and
-    refuses gelu / swish / silu with the pre-activation reason and other names as not built; check_scope keeps the
-    relu-trunk scope"""
+def test_check_scope_net_activation():
+    """check_scope (every CLI's check) accepts the built trunk activations under both namings in any case, and
+    refuses gelu / swish / silu with the pre-activation reason and other names as not built"""
     from plenoctree_b200.nerf import flags as F
     for names, code in ((("relu", "ReLU", "RELU"), 0), (("elu", "ELU", "Elu"), 1), (("softplus", "Softplus"), 2),
                         (("tanh", "Tanh", "TANH"), 3)):
         for name in names:
-            F.check_model_scope(_scope_args(net_activation=name))
-            F.check_model_scope(_scope_args(net_activation=name, sigma_activation="Softplus", rgb_activation="Sigmoid"))
+            F.check_scope(_scope_args(net_activation=name))
+            F.check_scope(_scope_args(net_activation=name, sigma_activation="Softplus", rgb_activation="Sigmoid"))
             assert F.net_activation_code(name) == code
-            if code:
-                with pytest.raises(NotImplementedError, match="relu"):
-                    F.check_scope(_scope_args(net_activation=name))
     for bad in ("gelu", "GELU", "swish", "silu", "SiLU"):
         with pytest.raises(NotImplementedError, match="pre-activation"):
-            F.check_model_scope(_scope_args(net_activation=bad))
+            F.check_scope(_scope_args(net_activation=bad))
     for bad in ("sigmoid", "leaky_relu", "softmax", "relu6", "LeakyReLU"):
         with pytest.raises(NotImplementedError, match="not built"):
-            F.check_model_scope(_scope_args(net_activation=bad))
+            F.check_scope(_scope_args(net_activation=bad))
 
 
-def test_check_model_scope_refuses_what_check_scope_refuses():
-    """every other flag is checked as check_scope checks it, whatever the trunk activation"""
+def test_check_scope_other_flags_whatever_the_trunk():
+    """every other flag is checked the same way whatever the trunk activation"""
     from plenoctree_b200.nerf import flags as F
     for net in ("relu", "elu", "Tanh"):
         for mn in range(11):
             for mx in range(mn, 11):
-                F.check_model_scope(_scope_args(net_activation=net, min_deg_point=mn, max_deg_point=mx))
+                F.check_scope(_scope_args(net_activation=net, min_deg_point=mn, max_deg_point=mx))
         for mn, mx in ((0, 11), (-1, 10), (5, 4), (0, 16), (11, 11)):
             with pytest.raises(NotImplementedError, match="min_deg_point"):
-                F.check_model_scope(_scope_args(net_activation=net, min_deg_point=mn, max_deg_point=mx))
+                F.check_scope(_scope_args(net_activation=net, min_deg_point=mn, max_deg_point=mx))
         for kw in (dict(net_depth=6), dict(net_width=128), dict(skip_layer=3), dict(use_viewdirs=True),
                    dict(sg_dim=4), dict(rgb_activation="relu"), dict(sigma_activation="elu"),
                    dict(sigma_activation="tanh")):
             with pytest.raises(NotImplementedError):
-                F.check_model_scope(_scope_args(net_activation=net, **kw))
+                F.check_scope(_scope_args(net_activation=net, **kw))
         with pytest.raises(ValueError, match="llff"):
-            F.check_model_scope(_scope_args(net_activation=net, render_path=True))
+            F.check_scope(_scope_args(net_activation=net, render_path=True))
     args = _scope_args(net_activation="ELU")
-    F.check_model_scope(args)
+    F.check_scope(args)
     assert args.net_activation == "ELU"                    # the caller's flags are left as they are
 
 
 def test_abi_net_descriptor():
     """the ctypes NetDesc is pob_posenc of the header, field for field; codes match; out-of-range codes are refused
-    at the boundary; a bare Posenc (the encoder fields only) reads as a relu trunk"""
+    at the boundary"""
     import re
     from plenoctree_b200 import _lib
     hdr = open(os.path.join(ROOT, "include", "plenoctree_b200.h")).read()
     body = re.search(r"typedef struct pob_posenc \{(.*?)\} pob_posenc;", hdr, re.S).group(1)
     fields = re.findall(r"int (\w+);", body)
-    assert fields == [f[0] for f in _lib.Posenc._fields_ + _lib.NetDesc._fields_]
+    assert fields == [f[0] for f in _lib.NetDesc._fields_]
     assert ctypes.sizeof(_lib.NetDesc) == 4 * len(fields) == 16
     for name in ("RELU", "ELU", "SOFTPLUS", "TANH"):
         m = re.search(rf"#define POB_NET_{name} (\d+)", hdr)
@@ -247,8 +243,6 @@ def test_abi_net_descriptor():
         d = _lib.NetDesc(0, 10, 0, bad)
         assert lib.pob_param_count_pe(3, ctypes.addressof(d)) == -1
         assert b"net_activation" in lib.pob_last_error()
-    bare = _lib.Posenc(2, 8, 1)
-    assert bytes((ctypes.c_char * 16).from_address(ctypes.addressof(bare)))[12:] == b"\0" * 4
     assert _lib.posenc_struct(None) is None and _lib.posenc_struct((0, 10, False), 0) is None
     s = _lib.posenc_struct(None, _lib.NET_TANH)
     assert (s.min_deg, s.max_deg, s.legacy_order, s.net_activation) == (0, 10, 0, 3)

@@ -46,6 +46,62 @@ def test_flags_yaml_and_scope(tmp_path):
     FLAGS.use_viewdirs = False
 
 
+# each CLI's workspace: (max_rays, sparsity_npoints) from its flags, world = 2 ranks for training
+_CLI_WORKSPACE = {
+    "train": lambda a: (a.batch_size // 2, a.sparsity_npoints if a.sparsity_weight > 0 else 0),
+    "eval": lambda a: (min(a.chunk, 8192), 0),
+    "gen_video": lambda a: (min(a.chunk, 8192), 0),
+    "gen_mesh": lambda a: (1024, 0),
+    "extraction": lambda a: (min(a.chunk, 8192), 0),
+}
+
+
+@pytest.mark.parametrize("cli", sorted(_CLI_WORKSPACE))
+def test_model_from_flags_matches_hand_copied_arguments(cli):
+    """NerfModel.from_flags builds the model that each CLI built from its own copy of the model flags"""
+    import types
+    from plenoctree_b200.nerf import flags as F
+    from plenoctree_b200.nerf.models import NerfModel
+    defaults = {name: default for name, (_, default, _) in F._COMMON.items()}
+    if cli == "extraction":
+        defaults.update(F._OCTREE_DEFAULTS)
+    variants = [dict(), dict(min_deg_point=2, max_deg_point=8, legacy_posenc_order=True), dict(net_activation="elu"),
+                dict(net_activation="Tanh", sigma_activation="Softplus"), dict(sigma_activation="softplus"),
+                dict(num_coarse_samples=256, num_fine_samples=768), dict(sparsity_weight=0.0, batch_size=4096),
+                dict(sh_deg=4, near=0.5, far=3.0, white_bkgd=False, lindisp=True, num_fine_samples=0, chunk=2048,
+                     min_deg_point=1, max_deg_point=9, net_activation="softplus", sigma_activation="softplus")]
+    for kw in variants:
+        args = types.SimpleNamespace(**{**defaults, "sh_deg": 3, **kw})
+        max_rays, nsp = _CLI_WORKSPACE[cli](args)
+        # the hand-built copy the CLIs passed, read back as get_model_state read it
+        margs = type("A", (), dict(sh_deg=args.sh_deg, sigma_activation=args.sigma_activation,
+                                   net_activation=args.net_activation, min_deg_point=args.min_deg_point,
+                                   max_deg_point=args.max_deg_point, legacy_posenc_order=args.legacy_posenc_order,
+                                   num_coarse_samples=args.num_coarse_samples,
+                                   num_fine_samples=args.num_fine_samples, near=args.near, far=args.far,
+                                   white_bkgd=args.white_bkgd, lindisp=args.lindisp, batch_size=max_rays,
+                                   sparsity_npoints=nsp))
+        old = NerfModel(sh_deg=margs.sh_deg, num_coarse_samples=margs.num_coarse_samples,
+                        num_fine_samples=margs.num_fine_samples, near=margs.near, far=margs.far,
+                        white_bkgd=margs.white_bkgd, lindisp=margs.lindisp, max_rays=margs.batch_size,
+                        sparsity_npoints=margs.sparsity_npoints, device="cpu", sigma_activation=margs.sigma_activation,
+                        min_deg_point=margs.min_deg_point, max_deg_point=margs.max_deg_point,
+                        legacy_posenc_order=margs.legacy_posenc_order, net_activation=margs.net_activation)
+        new = NerfModel.from_flags(args, max_rays=max_rays, sparsity_npoints=nsp, device="cpu")
+
+        def fields(m):
+            cfg = {k: getattr(m.cfg, k) for k, _ in m.cfg._fields_ if k != "posenc"}
+            desc = None if m._posenc_struct is None else tuple(getattr(m._posenc_struct, k)
+                                                               for k, _ in m._posenc_struct._fields_)
+            return dict(sh_deg=m.sh_deg, nc=m.num_coarse_samples, nf=m.num_fine_samples, near=m.near, far=m.far,
+                        white_bkgd=m.white_bkgd, lindisp=m.lindisp, max_rays=m.max_rays,
+                        sparsity_npoints=m.sparsity_npoints, posenc=m.posenc, net_act_code=m.net_act_code,
+                        sigma_act_code=m.sigma_act_code, P=m.P, cfg=cfg, desc=desc,
+                        cfg_posenc_set=m.cfg.posenc is not None)
+        assert fields(new) == fields(old), kw
+        assert torch.equal(new.z_base, old.z_base), kw
+
+
 def test_ssim_matches_reference_torch_twin(golden_dir):
     from plenoctree_b200.nerf.utils import compute_ssim
     z = np.load(os.path.join(golden_dir, "ssim.npz"))

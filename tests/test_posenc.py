@@ -159,7 +159,7 @@ def test_check_scope_table():
         with pytest.raises(NotImplementedError, match="min_deg_point"):
             F.check_scope(_scope_args(min_deg_point=mn, max_deg_point=mx))
     for kw in (dict(net_depth=6), dict(net_width=128), dict(skip_layer=3), dict(use_viewdirs=True), dict(sg_dim=4),
-               dict(net_activation="elu"), dict(rgb_activation="relu"), dict(sigma_activation="elu")):
+               dict(net_activation="gelu"), dict(rgb_activation="relu"), dict(sigma_activation="elu")):
         with pytest.raises(NotImplementedError):
             F.check_scope(_scope_args(**kw))
 
@@ -215,18 +215,18 @@ def test_abi_posenc_descriptor():
     lib = _lib.lib
     hdr = open(os.path.join(os.path.dirname(HERE), "include", "plenoctree_b200.h")).read()
     assert "typedef struct pob_posenc {" in hdr and "const pob_posenc* posenc;" in hdr
-    assert [f[0] for f in _lib.Posenc._fields_] == ["min_deg", "max_deg", "legacy_order"]
+    assert [f[0] for f in _lib.NetDesc._fields_] == ["min_deg", "max_deg", "legacy_order", "net_activation"]
     assert _lib.RenderConfig._fields_[-1] == ("posenc", ctypes.c_void_p)
     assert _lib.RenderConfig(3, 64, 128, 1, 4096, 10000).posenc is None        # an unset descriptor is NULL
     for sh in (-1, 3, 4):
         assert lib.pob_param_count_pe(sh, None) == lib.pob_param_count(sh)
-        d = _lib.Posenc(0, 10, 0)
+        d = _lib.NetDesc(0, 10, 0, 0)
         assert lib.pob_param_count_pe(sh, ctypes.addressof(d)) == lib.pob_param_count(sh)
         for pe in ((2, 8, 1), (0, 0, 0), (3, 10, 0), (10, 10, 1)):
-            d = _lib.Posenc(*pe)
+            d = _lib.NetDesc(*pe, 0)
             assert lib.pob_param_count_pe(sh, ctypes.addressof(d)) == PO.param_count(sh, pe)
     for bad in ((0, 11, 0), (-1, 5, 0), (6, 5, 0), (0, 10, 2)):
-        d = _lib.Posenc(*bad)
+        d = _lib.NetDesc(*bad, 0)
         assert lib.pob_param_count_pe(3, ctypes.addressof(d)) == -1
     assert _lib.posenc_struct((0, 10, False)) is None and _lib.posenc_struct(None) is None
 
@@ -235,7 +235,7 @@ def test_no_gpu_descriptor_calls_fail_loudly():
     if torch.cuda.is_available():
         return
     from plenoctree_b200 import _lib
-    d = _lib.Posenc(2, 8, 1)
+    d = _lib.NetDesc(2, 8, 1, 0)
     rc = _lib.lib.pob_eval_points_raw_pe(1, 3, ctypes.addressof(d), 1, 16, None, 1, 1, None)
     assert rc != 0 and len(_lib.lib.pob_last_error()) > 0
 
@@ -411,7 +411,7 @@ def test_explicit_default_descriptor_is_the_null_descriptor():
     from plenoctree_b200 import _lib
     from plenoctree_b200._lib import check, lib, ptr, stream_ptr
     sh, R = 3, 24
-    d = _lib.Posenc(0, 10, 0)
+    d = _lib.NetDesc(0, 10, 0, 0)
     dp = ctypes.addressof(d)
     flat = torch.from_numpy(np.concatenate(_gpu_params((0, 10, False), sh, 3))).cuda()
     P = flat.numel() // 2
@@ -462,7 +462,7 @@ def test_explicit_default_descriptor_is_the_null_descriptor():
     for a, b in zip(*grads):
         assert torch.equal(a, b)
     # a refused descriptor fails loudly at the boundary
-    bad = _lib.Posenc(0, 11, 0)
+    bad = _lib.NetDesc(0, 11, 0, 0)
     assert lib.pob_eval_points_raw_pe(ptr(b0), sh, ctypes.addressof(bad), ptr(pts), 16, None, ptr(g1), 1,
                                       stream_ptr()) != 0
     assert b"max_deg" in lib.pob_last_error()

@@ -51,8 +51,10 @@ def test_check_scope_still_refuses_use_viewdirs():
     from plenoctree_b200.nerf import flags as F
     with pytest.raises(NotImplementedError, match="use_viewdirs"):
         F.check_scope(_args())
-    with pytest.raises(NotImplementedError, match="use_viewdirs"):
-        F.check_model_scope(_args())
+    # check_scope builds an elu trunk for NeRF-SH; the projection refuses it itself
+    F.check_scope(_args(use_viewdirs=False, net_activation="elu"))
+    with pytest.raises(NotImplementedError, match="projection kernel is built for a relu trunk"):
+        F.check_projection_scope(_args(net_activation="elu"))
 
 
 def test_proj_preset_and_file_on_disk_wins(tmp_path):

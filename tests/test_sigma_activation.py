@@ -215,7 +215,7 @@ def test_check_scope_sigma_activation():
     for bad in ("sigmoid", "elu", "softmax", "Sigmoid", "shifted_softplus"):
         with pytest.raises(NotImplementedError):
             F.check_scope(_scope_args(sigma_activation=bad))
-    for kw in (dict(net_activation="elu"), dict(net_activation="softplus", sigma_activation="softplus"),
+    for kw in (dict(net_activation="gelu"), dict(net_activation="swish", sigma_activation="softplus"),
                dict(rgb_activation="relu", sigma_activation="softplus")):
         with pytest.raises(NotImplementedError):
             F.check_scope(_scope_args(**kw))
