@@ -10,14 +10,12 @@
 // products, exp, sigmoid, compositing sums) may contract to FMA and uses the fast exp / reciprocal — the march is
 // instruction-issue bound (ncu: sm__throughput 73-79 %, DRAM 5 %), so instruction count is what matters.
 //
-// Thread mapping (GPU-first, not svox's thread-per-ray): a *group* of G lanes owns one ray (G = 4 by default,
-// see group_width(); 8 / 16 / 32 selectable for profiling).  All lanes of a group walk the tree together
-// (same-address loads broadcast), lane l owns basis functions l, l+G, ...: the 3K coefficient gather of a
-// contributing leaf is three coalesced segments per group instead of 3K strided scalar loads per thread, the dot
-// products finish with log2(G) shuffles, and the backward scatter issues coalesced RED.ADD.F32.  Pixels are tiled
-// per CTA so that neighbouring rays share L1 lines.
+// Thread mapping (GPU-first, not svox's thread-per-ray): a *group* of G = 4 lanes owns one ray.  All lanes of a
+// group walk the tree together (same-address loads broadcast), lane l owns basis functions l, l+G, ...: the 3K
+// coefficient gather of a contributing leaf is three coalesced segments per group instead of 3K strided scalar loads
+// per thread, the dot products finish with log2(G) shuffles, and the backward scatter issues coalesced RED.ADD.F32.
+// Pixels are tiled per CTA so that neighbouring rays share L1 lines.
 #include <cstdint>
-#include <cstdlib>
 #include <type_traits>
 
 #include "../../include/plenoctree_b200.h"
@@ -33,6 +31,13 @@ namespace {
 // (renderer_step_size 1e-5, octree/config/syn_sh16.json:16,22,24), since every iteration advances by >= step_size.
 constexpr int MAX_MARCH_STEPS = 1 << 20;
 constexpr int MAX_TREE_DEPTH = 40;
+
+// Lanes per ray.  The march is instruction-issue bound and every lane of a group repeats the walk, so fewer lanes per
+// ray = fewer instructions per ray.  Measured 800x800 / depth-8 SH16: 16 lanes 4.1 ms, 8 lanes 2.25 ms, 4 lanes
+// 1.65 ms (2 lanes: 1.52 ms render but 4.7 ms training pass — not kept).
+constexpr int G = 4;
+// Rays per 256-thread CTA; a perspective camera's CTA renders a TILE_W x TILE_H pixel tile.
+constexpr int RPB = 256 / G, TILE_W = 8, TILE_H = RPB / TILE_W;
 
 struct TreeDev {
   const float* data;
@@ -182,14 +187,11 @@ __device__ __forceinline__ long long query_leaf(const int32_t* __restrict__ chil
   return idx;
 }
 
-template <int G>
 __device__ __forceinline__ unsigned group_mask() {
-  if (G == 32) return 0xffffffffu;
   const unsigned lane = threadIdx.x & 31;
   return ((1u << G) - 1u) << (lane / G * G);
 }
 
-template <int G>
 __device__ __forceinline__ float group_sum(float v, unsigned mask) {
 #pragma unroll
   for (int s = G / 2; s > 0; s >>= 1) v += __shfl_xor_sync(mask, v, s, G);
@@ -206,10 +208,9 @@ __device__ __forceinline__ float sigmoidf(float x) { return __fdividef(1.0f, 1.0
 // idle lanes are the stack), the shared depth is a count-leading-zeros of the XOR of the integer coordinates, and
 // the position inside the leaf is frac(x * 2^(depth+1)) — bit-identical to the iterated form.  Other branch
 // factors, and levels deeper than 22, use the plain walk.
-template <int G>
 struct Marcher {
   unsigned pq0, pq1, pq2;
-  static constexpr int PW = G >= 8 ? 1 : 8 / G;   // path registers per lane: levels l, l+G, ... are cached
+  static constexpr int PW = 8 / G;   // path registers per lane: levels l, l+G, ... are cached
   static constexpr int CACHED = G * PW;
   int pdepth;     // depth of the previous leaf, -1 = no previous sample
   int path[PW];   // lane l, register j: node entered at level l + j*G (level 0: root)
@@ -321,7 +322,7 @@ struct Marcher {
 // trees load sigma, the retained coefficients and the palette indices in issue() and the palette entries in finish()
 // (a dependent gather, so it waits for the indices while locate() runs).  Both produce fp32 coefficients that the
 // shading arithmetic consumes unchanged: lane l owns basis functions l, l+G, ...
-template <int G, int KPL>
+template <int KPL>
 struct DenseFetch {
   __device__ __forceinline__ float issue(const TreeDev& T, unsigned idx, int l, float* c0, float* c1, float* c2) {
     const int K = T.K, D = T.D;
@@ -342,7 +343,7 @@ struct DenseFetch {
   __device__ __forceinline__ void finish(const TreeDev&, int, bool, float*, float*, float*) {}
 };
 
-template <int G, int KPL>
+template <int KPL>
 struct QuantFetch {
   unsigned m[KPL];   // palette index of basis function l + j*G (palette-coded functions only)
 
@@ -380,14 +381,30 @@ struct QuantFetch {
   }
 };
 
-template <class Tree, int G, int KPL>
+template <class Tree, int KPL>
 struct LeafFetch {
-  using type = DenseFetch<G, KPL>;
+  using type = DenseFetch<KPL>;
 };
-template <int G, int KPL>
-struct LeafFetch<QuantTreeDev, G, KPL> {
-  using type = QuantFetch<G, KPL>;
+template <int KPL>
+struct LeafFetch<QuantTreeDev, KPL> {
+  using type = QuantFetch<KPL>;
 };
+
+// the three colour channels' SH dot products basis . c of one leaf, summed over the lane group
+template <int KPL>
+__device__ __forceinline__ void sh_dot(const float* basis_l, const float* c0, const float* c1, const float* c2,
+                                       unsigned mask, float& p0, float& p1, float& p2) {
+  p0 = p1 = p2 = 0.f;
+#pragma unroll
+  for (int j = 0; j < KPL; ++j) {
+    p0 += basis_l[j] * c0[j];
+    p1 += basis_l[j] * c1[j];
+    p2 += basis_l[j] * c2[j];
+  }
+  p0 = group_sum(p0, mask);
+  p1 = group_sum(p1, mask);
+  p2 = group_sum(p2, mask);
+}
 
 // ---- forward march of one ray by one lane group -------------------------------------------------------
 // Software-pipelined: the loads of the current leaf (sigma and this lane's three coefficients, issued
@@ -402,7 +419,7 @@ struct LeafFetch<QuantTreeDev, G, KPL> {
 // Early termination rescales both by 1 / (1 - light) like the colour, so a stopped ray has acc = 1.  A ray that
 // misses the box has depth = acc = 0.  The colour, the march and the counters are those of DEPTH = false.
 // Tree = QuantTreeDev marches a compressed tree: only the leaf fetch differs (LeafFetch).
-template <int G, int KPL, bool DEPTH = false, class Tree = TreeDev>
+template <int KPL, bool DEPTH = false, class Tree = TreeDev>
 __device__ __forceinline__ void trace_forward(const Tree& T, const Opts& O, const Ray& r, const float* basis_l, int l,
                                               unsigned mask, float* out, unsigned& visits, unsigned& hits,
                                               float* dz = nullptr) {
@@ -418,12 +435,12 @@ __device__ __forceinline__ void trace_forward(const Tree& T, const Opts& O, cons
     out[0] = out[1] = out[2] = O.bg;  // light = 1
     return;
   }
-  Marcher<G> m;
+  Marcher m;
   m.init();
   float delta_t;
   unsigned idx = m.locate(T, r, O.step, t, l, mask, delta_t);
   for (int it = 0; it < MAX_MARCH_STEPS; ++it) {
-    typename LeafFetch<Tree, G, KPL>::type fetch;
+    typename LeafFetch<Tree, KPL>::type fetch;
     float c0[KPL], c1[KPL], c2[KPL];  // lane l owns basis functions l, l+G, ...
     const float sigma = fetch.issue(T, idx, l, c0, c1, c2);
     const float t_next = t + delta_t;
@@ -437,16 +454,8 @@ __device__ __forceinline__ void trace_forward(const Tree& T, const Opts& O, cons
       ++hits;
       const float att = __expf(-delta_t * r.delta_scale * sigma);
       const float weight = light * (1.0f - att);
-      float p0 = 0.f, p1 = 0.f, p2 = 0.f;
-#pragma unroll
-      for (int j = 0; j < KPL; ++j) {
-        p0 += basis_l[j] * c0[j];
-        p1 += basis_l[j] * c1[j];
-        p2 += basis_l[j] * c2[j];
-      }
-      p0 = group_sum<G>(p0, mask);
-      p1 = group_sum<G>(p1, mask);
-      p2 = group_sum<G>(p2, mask);
+      float p0, p1, p2;
+      sh_dot<KPL>(basis_l, c0, c1, c2, mask, p0, p1, p2);
       out[0] += weight * sigmoidf(p0);
       out[1] += weight * sigmoidf(p1);
       out[2] += weight * sigmoidf(p2);
@@ -483,7 +492,7 @@ __device__ __forceinline__ void trace_forward(const Tree& T, const Opts& O, cons
 // DEPTH = true adds the upstream gradients gz = d loss / d depth and ga = d loss / d acc of trace_forward<DEPTH>: each
 // visit's `total` gains z_i gz + ga (the value it composites into g . out + gz depth + ga acc, which the caller passes
 // as accum) and only the sigma gradient changes, since depth and acc do not depend on the colour coefficients.
-template <int G, int KPL, bool DEPTH = false>
+template <int KPL, bool DEPTH = false>
 __device__ __forceinline__ void trace_backward(const TreeDev& T, const Opts& O, const Ray& r, const float* basis_l, int l,
                                                unsigned mask, const float* g, float accum,
                                                float* __restrict__ grad, float gz = 0.f, float ga = 0.f) {
@@ -492,11 +501,13 @@ __device__ __forceinline__ void trace_backward(const TreeDev& T, const Opts& O, 
   float t = r.tmin;
   const int K = T.K, D = T.D;
   if (!(t < r.tmax)) return;
-  Marcher<G> m;
+  Marcher m;
   m.init();
   float delta_t;
   unsigned idx = m.locate(T, r, O.step, t, l, mask, delta_t);
   for (int it = 0; it < MAX_MARCH_STEPS; ++it) {
+    // DenseFetch::issue's loads, written out with K and D hoisted: calling DenseFetch here changes the generated code
+    // of the KPL = 4 and 7 backward and training kernels
     const float* __restrict__ val = T.data + size_t(idx) * unsigned(D);
     const float sigma = __ldg(val + D - 1);
     float c0[KPL], c1[KPL], c2[KPL];  // lane l owns basis functions l, l+G, ...
@@ -518,16 +529,8 @@ __device__ __forceinline__ void trace_backward(const TreeDev& T, const Opts& O, 
     if (sigma > 0.0f) {
       const float att = __expf(-delta_t * r.delta_scale * sigma);
       const float weight = light * (1.0f - att);
-      float p0 = 0.f, p1 = 0.f, p2 = 0.f;
-#pragma unroll
-      for (int j = 0; j < KPL; ++j) {
-        p0 += basis_l[j] * c0[j];
-        p1 += basis_l[j] * c1[j];
-        p2 += basis_l[j] * c2[j];
-      }
-      p0 = group_sum<G>(p0, mask);
-      p1 = group_sum<G>(p1, mask);
-      p2 = group_sum<G>(p2, mask);
+      float p0, p1, p2;
+      sh_dot<KPL>(basis_l, c0, c1, c2, mask, p0, p1, p2);
       const float s0 = sigmoidf(p0), s1 = sigmoidf(p1), s2 = sigmoidf(p2);
       float* gv = grad + size_t(idx) * unsigned(D);
       const float t0 = weight * s0 * (1.0f - s0) * g[0];
@@ -560,10 +563,9 @@ __device__ __forceinline__ void trace_backward(const TreeDev& T, const Opts& O, 
 // zscale (optional) receives the factor from a distance along the ray's direction vector to the reported depth:
 // 1 for explicit rays, the camera-axis factor 1 / |(x, y, -1)| for a perspective pixel.  NDC = true turns a
 // perspective pixel's ray into NDC (world_to_ndc) before the march; its view direction stays the world one.
-template <int G, bool NDC = false>
+template <bool NDC = false>
 __device__ __forceinline__ bool fetch_ray(const RaySrc& S, const TreeDev& T, Ray& r, long long& out_index,
                                           float* zscale = nullptr, const Ndc& ndc = Ndc{}) {
-  constexpr int RPB = 256 / G;  // rays per CTA
   const int grp = threadIdx.x / G;
   float o[3], d[3];
   if (S.o != nullptr) {
@@ -580,12 +582,11 @@ __device__ __forceinline__ bool fetch_ray(const RaySrc& S, const TreeDev& T, Ray
     if (zscale) *zscale = 1.0f;
     return true;
   }
-  constexpr int TW = RPB >= 64 ? 8 : 4, TH = RPB / TW;
   const int W = int(S.cam.width);
-  const int tiles_x = (W + TW - 1) / TW;
+  const int tiles_x = (W + TILE_W - 1) / TILE_W;
   const int tx = blockIdx.x % tiles_x, ty = blockIdx.x / tiles_x;
-  const int ix = tx * TW + grp % TW;
-  const int iyl = ty * TH + grp / TW;  // row inside the slab
+  const int ix = tx * TILE_W + grp % TILE_W;
+  const int iyl = ty * TILE_H + grp / TILE_W;  // row inside the slab
   if (ix >= W || iyl >= S.nrows) return false;
   const float nrm = cam_ray(S.cam, ix, S.row0 + iyl, o, d);
   if constexpr (NDC) {
@@ -600,7 +601,7 @@ __device__ __forceinline__ bool fetch_ray(const RaySrc& S, const TreeDev& T, Ray
   return true;
 }
 
-template <int G, int KPL>
+template <int KPL>
 __device__ __forceinline__ void lane_basis(const TreeDev& T, const Ray& r, int l, float* bl) {
   if (T.rgba) {
 #pragma unroll
@@ -623,21 +624,21 @@ __device__ __forceinline__ void lane_basis(const TreeDev& T, const Ray& r, int l
 
 // DEPTH = true also stores depth [n] (times fetch_ray's zscale) and acc [n] (trace_forward<DEPTH>); Tree = QuantTreeDev
 // renders a compressed tree
-template <int G, int KPL, bool DEPTH = false, class Tree = TreeDev>
+template <int KPL, bool DEPTH = false, class Tree = TreeDev>
 __global__ void __launch_bounds__(256) octree_render_kernel(Tree T, Opts O, RaySrc S, float* __restrict__ out_rgb,
                                                             unsigned long long* __restrict__ counters,
                                                             float* __restrict__ out_depth, float* __restrict__ out_acc) {
   Ray r;
   long long oi;
   float zscale;
-  if (!fetch_ray<G>(S, T, r, oi, DEPTH ? &zscale : nullptr)) return;
+  if (!fetch_ray(S, T, r, oi, DEPTH ? &zscale : nullptr)) return;
   const int l = threadIdx.x % G;
-  const unsigned mask = group_mask<G>();
+  const unsigned mask = group_mask();
   float bl[KPL];
-  lane_basis<G, KPL>(T, r, l, bl);
+  lane_basis<KPL>(T, r, l, bl);
   float out[3], dz[2];
   unsigned visits = 0, hits = 0;
-  trace_forward<G, KPL, DEPTH, Tree>(T, O, r, bl, l, mask, out, visits, hits, dz);
+  trace_forward<KPL, DEPTH, Tree>(T, O, r, bl, l, mask, out, visits, hits, dz);
   if (l < 3) out_rgb[3 * oi + l] = l == 0 ? out[0] : l == 1 ? out[1] : out[2];
   if constexpr (DEPTH) {
     if (l == 0) {
@@ -654,7 +655,7 @@ __global__ void __launch_bounds__(256) octree_render_kernel(Tree T, Opts O, RayS
 // VolumeRenderer backward for an upstream gradient d loss / d rgb  (svox trace_ray_backward).  DEPTH = true adds
 // d loss / d depth and d loss / d acc of octree_render_kernel<DEPTH>; each of the three gradient arrays may be null
 // (zero).
-template <int G, int KPL, bool DEPTH = false>
+template <int KPL, bool DEPTH = false>
 __global__ void __launch_bounds__(256) octree_backward_kernel(TreeDev T, Opts O, RaySrc S,
                                                               const float* __restrict__ grad_out,
                                                               float* __restrict__ grad_data,
@@ -663,21 +664,21 @@ __global__ void __launch_bounds__(256) octree_backward_kernel(TreeDev T, Opts O,
   Ray r;
   long long oi;
   float zscale;
-  if (!fetch_ray<G>(S, T, r, oi, DEPTH ? &zscale : nullptr)) return;
+  if (!fetch_ray(S, T, r, oi, DEPTH ? &zscale : nullptr)) return;
   const int l = threadIdx.x % G;
-  const unsigned mask = group_mask<G>();
+  const unsigned mask = group_mask();
   float bl[KPL];
-  lane_basis<G, KPL>(T, r, l, bl);
+  lane_basis<KPL>(T, r, l, bl);
   float out[3], dz[2];
   unsigned visits = 0, hits = 0;
   Opts Of = O;
   Of.sigma_thresh = 0.f;
   Of.stop_thresh = 0.f;
-  trace_forward<G, KPL, DEPTH>(T, Of, r, bl, l, mask, out, visits, hits, dz);
+  trace_forward<KPL, DEPTH>(T, Of, r, bl, l, mask, out, visits, hits, dz);
   if constexpr (!DEPTH) {
     float g[3] = {__ldg(grad_out + 3 * oi), __ldg(grad_out + 3 * oi + 1), __ldg(grad_out + 3 * oi + 2)};
     const float accum = g[0] * out[0] + g[1] * out[1] + g[2] * out[2];
-    trace_backward<G, KPL>(T, Of, r, bl, l, mask, g, accum, grad_data);
+    trace_backward<KPL>(T, Of, r, bl, l, mask, g, accum, grad_data);
   } else {
     float g[3] = {0.f, 0.f, 0.f};
     if (grad_out != nullptr)
@@ -687,7 +688,7 @@ __global__ void __launch_bounds__(256) octree_backward_kernel(TreeDev T, Opts O,
     const float ga = grad_acc != nullptr ? __ldg(grad_acc + oi) : 0.f;
     float accum = g[0] * out[0] + g[1] * out[1] + g[2] * out[2];
     accum = __fadd_rn(accum, __fmaf_rn(gz, dz[0], ga * dz[1]));
-    trace_backward<G, KPL, true>(T, Of, r, bl, l, mask, g, accum, grad_data, gz, ga);
+    trace_backward<KPL, true>(T, Of, r, bl, l, mask, g, accum, grad_data, gz, ga);
   }
 }
 
@@ -695,23 +696,23 @@ __global__ void __launch_bounds__(256) octree_backward_kernel(TreeDev T, Opts O,
 //   im = render_persp(c2w); mse = mean((clamp(im,0,1) - gt)^2); mse.backward()
 // g = grad_scale * 2 * (clamp(im) - gt) inside the clamp range, 0 outside (torch.clamp's gradient).
 // NDC = true marches the slab's rays in NDC (fetch_ray<NDC>, svox VolumeRenderer(ndc=...)); ndc is unused otherwise.
-template <int G, int KPL, bool NDC = false>
+template <int KPL, bool NDC = false>
 __global__ void __launch_bounds__(256) octree_train_kernel(TreeDev T, Opts O, RaySrc S, const float* __restrict__ gt,
                                                            float grad_scale, float* __restrict__ grad_data,
                                                            double* __restrict__ sq_err_sum,
                                                            float* __restrict__ out_rgb, Ndc ndc) {
   Ray r;
   long long oi;
-  const bool have = fetch_ray<G, NDC>(S, T, r, oi, nullptr, ndc);
+  const bool have = fetch_ray<NDC>(S, T, r, oi, nullptr, ndc);
   float err = 0.f;
   if (have) {
     const int l = threadIdx.x % G;
-    const unsigned mask = group_mask<G>();
+    const unsigned mask = group_mask();
     float bl[KPL];
-    lane_basis<G, KPL>(T, r, l, bl);
+    lane_basis<KPL>(T, r, l, bl);
     float out[3];
     unsigned visits = 0, hits = 0;
-    trace_forward<G, KPL>(T, O, r, bl, l, mask, out, visits, hits);
+    trace_forward<KPL>(T, O, r, bl, l, mask, out, visits, hits);
     float g[3];
     float accum = 0.f;
 #pragma unroll
@@ -723,7 +724,7 @@ __global__ void __launch_bounds__(256) octree_train_kernel(TreeDev T, Opts O, Ra
       accum += g[c] * out[c];
     }
     if (out_rgb != nullptr && l < 3) out_rgb[3 * oi + l] = l == 0 ? out[0] : l == 1 ? out[1] : out[2];
-    if (g[0] != 0.f || g[1] != 0.f || g[2] != 0.f) trace_backward<G, KPL>(T, O, r, bl, l, mask, g, accum, grad_data);
+    if (g[0] != 0.f || g[1] != 0.f || g[2] != 0.f) trace_backward<KPL>(T, O, r, bl, l, mask, g, accum, grad_data);
     if (l != 0) err = 0.f;
   }
   // CTA reduction of the squared error (one double atomic per CTA)
@@ -943,72 +944,62 @@ namespace {
 
 using namespace pob;
 
-int tree_dev(const char* where, const pob_octree* t, TreeDev& T) {
-  if (!t) return pob_fail(where, "tree is NULL");
-  if (!t->data_dev || !t->child_dev) return pob_fail(where, "tree data/child pointer is NULL");
+// The geometry both tree formats share: branch factor, node count, the 32-bit leaf index, basis_dim per format,
+// offset and invradius.  rgba_msg is the format's message for an RGBA tree whose basis_dim is not 1.
+template <class Desc>
+int tree_geometry(const char* where, const Desc* t, const char* rgba_msg, TreeDev& T) {
   if (t->N < 2 || t->N > 8) return pob_fail(where, "tree branch factor N must be in [2, 8]");
   if (t->n_nodes < 1) return pob_fail(where, "tree has no nodes");
   if (double(t->n_nodes) * t->N * t->N * t->N >= 4294967296.0) return pob_fail(where, "tree too large (leaf index must fit 32 bits)");
   const int K = t->basis_dim;
   if (t->format == POB_OCTREE_RGBA) {
-    if (K != 1 || t->data_dim != 4) return pob_fail(where, "RGBA trees have data_dim 4");
+    if (K != 1) return pob_fail(where, rgba_msg);
   } else if (t->format == POB_OCTREE_SH) {
     if (!(K == 1 || K == 4 || K == 9 || K == 16 || K == 25)) return pob_fail(where, "SH basis_dim must be 1,4,9,16,25");
-    if (t->data_dim != 3 * K + 1) return pob_fail(where, "data_dim must be 3*basis_dim + 1 (sigma last)");
   } else {
     return pob_fail(where, "unsupported data format (RGBA and SH only; SG is out of scope)");
   }
-  T.data = t->data_dev;
   T.child = t->child_dev;
   T.N = t->N;
-  T.D = t->data_dim;
   T.K = K;
   T.rgba = t->format == POB_OCTREE_RGBA;
   for (int a = 0; a < 3; ++a) {
     T.off[a] = t->offset[a];
     T.inv[a] = t->invradius[a];
   }
+  return 0;
+}
+
+int tree_dev(const char* where, const pob_octree* t, TreeDev& T) {
+  if (!t) return pob_fail(where, "tree is NULL");
+  if (!t->data_dev || !t->child_dev) return pob_fail(where, "tree data/child pointer is NULL");
+  if (int rc = tree_geometry(where, t, "RGBA trees have data_dim 4", T)) return rc;
+  if (T.rgba && t->data_dim != 4) return pob_fail(where, "RGBA trees have data_dim 4");
+  if (!T.rgba && t->data_dim != 3 * T.K + 1) return pob_fail(where, "data_dim must be 3*basis_dim + 1 (sigma last)");
+  T.data = t->data_dev;
+  T.D = t->data_dim;
   if (!pob_sms_or_fail(where)) return 1;
   return 0;
 }
 
-int quant_tree_dev(const char* where, const pob_octree_quant* t, QuantTreeDev& T) {
+int tree_dev(const char* where, const pob_octree_quant* t, QuantTreeDev& T) {
   if (!t) return pob_fail(where, "tree is NULL");
   if (!t->child_dev || !t->sigma_dev) return pob_fail(where, "tree child/sigma pointer is NULL");
-  if (t->N < 2 || t->N > 8) return pob_fail(where, "tree branch factor N must be in [2, 8]");
-  if (t->n_nodes < 1) return pob_fail(where, "tree has no nodes");
-  const double leaves = double(t->n_nodes) * t->N * t->N * t->N;
-  if (leaves >= 4294967296.0) return pob_fail(where, "tree too large (leaf index must fit 32 bits)");
-  const int K = t->basis_dim;
-  if (t->format == POB_OCTREE_RGBA) {
-    if (K != 1) return pob_fail(where, "RGBA trees have basis_dim 1");
-  } else if (t->format == POB_OCTREE_SH) {
-    if (!(K == 1 || K == 4 || K == 9 || K == 16 || K == 25)) return pob_fail(where, "SH basis_dim must be 1,4,9,16,25");
-  } else {
-    return pob_fail(where, "unsupported data format (RGBA and SH only; SG is out of scope)");
-  }
+  if (int rc = tree_geometry(where, t, "RGBA trees have basis_dim 1", T)) return rc;
   if (t->bits < 1 || t->bits > 16) return pob_fail(where, "bits must be in [1, 16] (palette indices are uint16)");
-  if (t->retain < 0 || t->retain > K) return pob_fail(where, "retain must be in [0, basis_dim]");
+  if (t->retain < 0 || t->retain > T.K) return pob_fail(where, "retain must be in [0, basis_dim]");
   if (t->retain > 0 && !t->retained_dev) return pob_fail(where, "retained pointer is NULL with retain > 0");
-  if (t->retain < K && (!t->map_dev || !t->palette_dev))
+  if (t->retain < T.K && (!t->map_dev || !t->palette_dev))
     return pob_fail(where, "map/palette pointer is NULL with retain < basis_dim");
   T.data = nullptr;
-  T.child = t->child_dev;
-  T.N = t->N;
   T.D = 0;
-  T.K = K;
-  T.rgba = t->format == POB_OCTREE_RGBA;
-  for (int a = 0; a < 3; ++a) {
-    T.off[a] = t->offset[a];
-    T.inv[a] = t->invradius[a];
-  }
   T.sigma = t->sigma_dev;
   T.map = t->map_dev;
   T.palette = reinterpret_cast<const __half*>(t->palette_dev);
   T.retained = reinterpret_cast<const __half*>(t->retained_dev);
   T.retain = t->retain;
   T.ncolors = 1 << t->bits;
-  T.leaves = (unsigned long long)leaves;
+  T.leaves = (unsigned long long)t->n_nodes * t->N * t->N * t->N;
   if (!pob_sms_or_fail(where)) return 1;
   return 0;
 }
@@ -1037,46 +1028,10 @@ int ndc_dev(const char* where, const pob_ndc* n, Ndc& N) {
   return 0;
 }
 
-// Group width / coefficients per lane.  Default: 4 lanes per ray (the march is instruction-issue bound and every
-// lane of a group repeats the walk, so fewer lanes per ray = fewer instructions per ray; lane l owns basis functions
-// l, l+4, ...).  Measured 800x800 / depth-8 SH16: 16 lanes 4.1 ms, 8 lanes 2.25 ms, 4 lanes 1.65 ms.
-// (2 lanes: 1.52 ms render but 4.7 ms training pass — not kept.)  POB_OCTREE_G=8|16|32 selects the other
-// mappings (profiling).
-int group_width(int K) {
-  static int env = -1;
-  if (env < 0) {
-    const char* e = getenv("POB_OCTREE_G");
-    env = e ? atoi(e) : 0;
-  }
-  if (env == 32) return 32;
-  if (env == 16) return K > 16 ? 32 : 16;
-  if (env == 8) return 8;
-  return 4;
-}
-
-// (G, K) -> the <G, KPL> instantiation: f(integral_constant G, integral_constant KPL) launches it
-template <class F>
-void octree_dispatch(int G, int K, F&& f) {
-  using std::integral_constant;
-  if (G == 32) f(integral_constant<int, 32>(), integral_constant<int, 1>());
-  else if (G == 16) f(integral_constant<int, 16>(), integral_constant<int, 1>());
-  else if (G == 4 && K <= 4) f(integral_constant<int, 4>(), integral_constant<int, 1>());
-  else if (G == 4 && K <= 12) f(integral_constant<int, 4>(), integral_constant<int, 3>());
-  else if (G == 4 && K <= 16) f(integral_constant<int, 4>(), integral_constant<int, 4>());
-  else if (G == 4) f(integral_constant<int, 4>(), integral_constant<int, 7>());
-  else if (K <= 8) f(integral_constant<int, 8>(), integral_constant<int, 1>());
-  else if (K <= 16) f(integral_constant<int, 8>(), integral_constant<int, 2>());
-  else f(integral_constant<int, 8>(), integral_constant<int, 4>());
-}
-
-#define POB_OCTREE_DISPATCH(KERNEL, G, K, ...)                                                               \
-  octree_dispatch((G), (K), [&](auto g_, auto kpl_) {                                                        \
-    KERNEL<decltype(g_)::value, decltype(kpl_)::value><<<blocks, 256, 0, st>>>(__VA_ARGS__);                 \
-  })
-
+// explicit rays (cam NULL) or a camera's pixel-row slab; blocks = the march grid (fetch_ray's RPB rays or
+// TILE_W x TILE_H pixels per CTA)
 int ray_src(const char* where, const float* o, const float* d, const float* v, long long n, const pob_camera* cam,
-            int row0, int nrows, RaySrc& S, unsigned& blocks, int G) {
-  const int rpb = 256 / G;
+            int row0, int nrows, RaySrc& S, unsigned& blocks) {
   S.o = o;
   S.d = d;
   S.v = v;
@@ -1086,7 +1041,7 @@ int ray_src(const char* where, const float* o, const float* d, const float* v, l
   if (cam == nullptr) {
     if (!o || !d || !v) return pob_fail(where, "ray pointers are NULL");
     if (n < 0) return pob_fail(where, "negative ray count");
-    blocks = unsigned((n + rpb - 1) / rpb);
+    blocks = unsigned((n + RPB - 1) / RPB);
     return 0;
   }
   S.o = S.d = S.v = nullptr;
@@ -1101,37 +1056,50 @@ int ray_src(const char* where, const float* o, const float* d, const float* v, l
   S.row0 = row0;
   S.nrows = nrows;
   S.n = (long long)nrows * W;
-  const int tw = rpb >= 64 ? 8 : 4, th = rpb / tw;
-  blocks = unsigned(((W + tw - 1) / tw) * ((nrows + th - 1) / th));
+  blocks = unsigned(((W + TILE_W - 1) / TILE_W) * ((nrows + TILE_H - 1) / TILE_H));
   return 0;
 }
 
-// pob_octree_render_quant / pob_octree_render_depth_quant (depth outputs null for the former)
-int render_quant(const char* W, const pob_octree_quant* tree, const pob_octree_opts* opts, const float* origins_dev,
-                 const float* dirs_dev, const float* vdirs_dev, int64_t n_rays, const pob_camera* cam, int row0,
-                 int nrows, float* out_rgb_dev, float* out_depth_dev, float* out_acc_dev,
-                 unsigned long long* counters_dev, void* stream, bool depth) {
-  QuantTreeDev T;
+// What a march launch needs: the tree (TreeDev or QuantTreeDev), the options, the rays, the grid and the stream
+template <class Tree>
+struct March {
+  Tree T;
   Opts O;
   RaySrc S;
   unsigned blocks = 0;
-  if (int rc = quant_tree_dev(W, tree, T)) return rc;
-  if (int rc = opts_dev(W, opts, O)) return rc;
-  const int G = group_width(T.K);
-  if (int rc = ray_src(W, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0, nrows, S, blocks, G)) return rc;
-  if (!out_rgb_dev || (depth && (!out_depth_dev || !out_acc_dev))) return pob_fail(W, "output pointer is NULL");
-  if (blocks == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
+  cudaStream_t st;
+};
+
+struct NoChecks {
+  int operator()() const { return 0; }
+};
+
+// Validates the tree, the options, the caller's own `checks` (which may read M.T and M.O) and the ray source, and
+// reports the first failure in that order.
+template <class Desc, class Tree, class Checks = NoChecks>
+int march_setup(const char* W, const Desc* tree, const pob_octree_opts* opts, const float* origins_dev,
+                const float* dirs_dev, const float* vdirs_dev, long long n_rays, const pob_camera* cam, int row0,
+                int nrows, void* stream, March<Tree>& M, Checks checks = {}) {
+  if (int rc = tree_dev(W, tree, M.T)) return rc;
+  if (int rc = opts_dev(W, opts, M.O)) return rc;
+  if (int rc = checks()) return rc;
+  if (int rc = ray_src(W, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0, nrows, M.S, M.blocks)) return rc;
+  M.st = (cudaStream_t)stream;
+  return 0;
+}
+
+// launch(integral_constant KPL) launches the march kernel for the tree's basis functions per lane (K = basis_dim,
+// lane l owns l, l+G, ...); an empty grid launches nothing
+template <class Tree, class F>
+int march_launch(const char* W, const March<Tree>& M, F&& launch) {
+  using std::integral_constant;
+  if (M.blocks == 0) return 0;
   pob_count_launch();
-  octree_dispatch(G, T.K, [&](auto g_, auto kpl_) {
-    constexpr int g = decltype(g_)::value, kpl = decltype(kpl_)::value;
-    if (depth)
-      octree_render_kernel<g, kpl, true, QuantTreeDev><<<blocks, 256, 0, st>>>(T, O, S, out_rgb_dev, counters_dev,
-                                                                               out_depth_dev, out_acc_dev);
-    else
-      octree_render_kernel<g, kpl, false, QuantTreeDev><<<blocks, 256, 0, st>>>(T, O, S, out_rgb_dev, counters_dev,
-                                                                                nullptr, nullptr);
-  });
+  const int K = M.T.K;
+  if (K <= 4) launch(integral_constant<int, 1>());
+  else if (K <= 12) launch(integral_constant<int, 3>());
+  else if (K <= 16) launch(integral_constant<int, 4>());
+  else launch(integral_constant<int, 7>());
   POB_CUDA(W, cudaGetLastError());
   return 0;
 }
@@ -1140,35 +1108,26 @@ int render_quant(const char* W, const pob_octree_quant* tree, const pob_octree_o
 int train_persp(const char* W, const pob_octree* tree, const pob_octree_opts* opts, const pob_camera* cam,
                 const pob_ndc* ndc, int row0, int nrows, const float* gt_rgb_dev, float grad_scale,
                 float* grad_data_dev, double* sq_err_sum_dev, float* out_rgb_dev, void* stream) {
-  TreeDev T;
-  Opts O;
-  RaySrc S;
+  March<TreeDev> M;
   Ndc N{};
-  unsigned blocks = 0;
-  if (int rc = tree_dev(W, tree, T)) return rc;
-  if (int rc = opts_dev(W, opts, O)) return rc;
-  if (ndc != nullptr)
-    if (int rc = ndc_dev(W, ndc, N)) return rc;
-  if (!cam) return pob_fail(W, "camera is NULL");
-  if (O.sigma_thresh != 0.f || O.stop_thresh != 0.f)
-    return pob_fail(W, "training renders with sigma_thresh = stop_thresh = 0 (svox fast=False)");
-  const int G = group_width(T.K);
-  if (int rc = ray_src(W, nullptr, nullptr, nullptr, 0, cam, row0, nrows, S, blocks, G)) return rc;
+  const auto checks = [&] {
+    if (ndc != nullptr)
+      if (int rc = ndc_dev(W, ndc, N)) return rc;
+    if (!cam) return pob_fail(W, "camera is NULL");
+    if (M.O.sigma_thresh != 0.f || M.O.stop_thresh != 0.f)
+      return pob_fail(W, "training renders with sigma_thresh = stop_thresh = 0 (svox fast=False)");
+    return 0;
+  };
+  if (int rc = march_setup(W, tree, opts, nullptr, nullptr, nullptr, 0, cam, row0, nrows, stream, M, checks)) return rc;
   if (!gt_rgb_dev || !grad_data_dev) return pob_fail(W, "gt / gradient pointer is NULL");
-  if (blocks == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  pob_count_launch();
-  if (ndc == nullptr) {
-    POB_OCTREE_DISPATCH(octree_train_kernel, G, T.K, T, O, S, gt_rgb_dev, grad_scale, grad_data_dev, sq_err_sum_dev,
-                        out_rgb_dev, N);
-  } else {
-    octree_dispatch(G, T.K, [&](auto g_, auto kpl_) {
-      octree_train_kernel<decltype(g_)::value, decltype(kpl_)::value, true><<<blocks, 256, 0, st>>>(
-          T, O, S, gt_rgb_dev, grad_scale, grad_data_dev, sq_err_sum_dev, out_rgb_dev, N);
-    });
-  }
-  POB_CUDA(W, cudaGetLastError());
-  return 0;
+  return march_launch(W, M, [&](auto kpl) {
+    if (ndc == nullptr)
+      octree_train_kernel<decltype(kpl)::value, false><<<M.blocks, 256, 0, M.st>>>(
+          M.T, M.O, M.S, gt_rgb_dev, grad_scale, grad_data_dev, sq_err_sum_dev, out_rgb_dev, N);
+    else
+      octree_train_kernel<decltype(kpl)::value, true><<<M.blocks, 256, 0, M.st>>>(
+          M.T, M.O, M.S, gt_rgb_dev, grad_scale, grad_data_dev, sq_err_sum_dev, out_rgb_dev, N);
+  });
 }
 
 // pob_grid_weight_render (ndc NULL) / pob_grid_weight_render_ndc
@@ -1214,7 +1173,7 @@ int pob_ndc_rays(const pob_ndc* ndc, const float* origins_dev, const float* dirs
   RaySrc S;
   unsigned tiles = 0;
   if (int rc = ndc_dev(W, ndc, N)) return rc;
-  if (int rc = ray_src(W, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0, nrows, S, tiles, 4)) return rc;
+  if (int rc = ray_src(W, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0, nrows, S, tiles)) return rc;
   if (!out_origins_dev || !out_dirs_dev || !out_vdirs_dev) return pob_fail(W, "output pointer is NULL");
   if (!pob_sms_or_fail(W)) return 1;
   if (S.n == 0) return 0;
@@ -1228,8 +1187,15 @@ int pob_ndc_rays(const pob_ndc* ndc, const float* origins_dev, const float* dirs
 int pob_octree_render_quant(const pob_octree_quant* tree, const pob_octree_opts* opts, const float* origins_dev,
                             const float* dirs_dev, const float* vdirs_dev, int64_t n_rays, const pob_camera* cam,
                             int row0, int nrows, float* out_rgb_dev, unsigned long long* counters_dev, void* stream) {
-  return render_quant("pob_octree_render_quant", tree, opts, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0,
-                      nrows, out_rgb_dev, nullptr, nullptr, counters_dev, stream, false);
+  const char* W = "pob_octree_render_quant";
+  March<QuantTreeDev> M;
+  if (int rc = march_setup(W, tree, opts, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0, nrows, stream, M))
+    return rc;
+  if (!out_rgb_dev) return pob_fail(W, "output pointer is NULL");
+  return march_launch(W, M, [&](auto kpl) {
+    octree_render_kernel<decltype(kpl)::value, false, QuantTreeDev><<<M.blocks, 256, 0, M.st>>>(
+        M.T, M.O, M.S, out_rgb_dev, counters_dev, nullptr, nullptr);
+  });
 }
 
 int pob_octree_render_depth_quant(const pob_octree_quant* tree, const pob_octree_opts* opts, const float* origins_dev,
@@ -1237,29 +1203,29 @@ int pob_octree_render_depth_quant(const pob_octree_quant* tree, const pob_octree
                                   const pob_camera* cam, int row0, int nrows, float* out_rgb_dev,
                                   float* out_depth_dev, float* out_acc_dev, unsigned long long* counters_dev,
                                   void* stream) {
-  return render_quant("pob_octree_render_depth_quant", tree, opts, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0,
-                      nrows, out_rgb_dev, out_depth_dev, out_acc_dev, counters_dev, stream, true);
+  const char* W = "pob_octree_render_depth_quant";
+  March<QuantTreeDev> M;
+  if (int rc = march_setup(W, tree, opts, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0, nrows, stream, M))
+    return rc;
+  if (!out_rgb_dev || !out_depth_dev || !out_acc_dev) return pob_fail(W, "output pointer is NULL");
+  return march_launch(W, M, [&](auto kpl) {
+    octree_render_kernel<decltype(kpl)::value, true, QuantTreeDev><<<M.blocks, 256, 0, M.st>>>(
+        M.T, M.O, M.S, out_rgb_dev, counters_dev, out_depth_dev, out_acc_dev);
+  });
 }
 
 int pob_octree_render(const pob_octree* tree, const pob_octree_opts* opts, const float* origins_dev,
                       const float* dirs_dev, const float* vdirs_dev, int64_t n_rays, const pob_camera* cam,
                       int row0, int nrows, float* out_rgb_dev, unsigned long long* counters_dev, void* stream) {
   const char* W = "pob_octree_render";
-  TreeDev T;
-  Opts O;
-  RaySrc S;
-  unsigned blocks = 0;
-  if (int rc = tree_dev(W, tree, T)) return rc;
-  if (int rc = opts_dev(W, opts, O)) return rc;
-  const int G = group_width(T.K);
-  if (int rc = ray_src(W, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0, nrows, S, blocks, G)) return rc;
+  March<TreeDev> M;
+  if (int rc = march_setup(W, tree, opts, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0, nrows, stream, M))
+    return rc;
   if (!out_rgb_dev) return pob_fail(W, "output pointer is NULL");
-  if (blocks == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  pob_count_launch();
-  POB_OCTREE_DISPATCH(octree_render_kernel, G, T.K, T, O, S, out_rgb_dev, counters_dev, nullptr, nullptr);
-  POB_CUDA(W, cudaGetLastError());
-  return 0;
+  return march_launch(W, M, [&](auto kpl) {
+    octree_render_kernel<decltype(kpl)::value><<<M.blocks, 256, 0, M.st>>>(M.T, M.O, M.S, out_rgb_dev, counters_dev,
+                                                                           nullptr, nullptr);
+  });
 }
 
 int pob_octree_render_depth(const pob_octree* tree, const pob_octree_opts* opts, const float* origins_dev,
@@ -1267,45 +1233,29 @@ int pob_octree_render_depth(const pob_octree* tree, const pob_octree_opts* opts,
                             int row0, int nrows, float* out_rgb_dev, float* out_depth_dev, float* out_acc_dev,
                             unsigned long long* counters_dev, void* stream) {
   const char* W = "pob_octree_render_depth";
-  TreeDev T;
-  Opts O;
-  RaySrc S;
-  unsigned blocks = 0;
-  if (int rc = tree_dev(W, tree, T)) return rc;
-  if (int rc = opts_dev(W, opts, O)) return rc;
-  const int G = group_width(T.K);
-  if (int rc = ray_src(W, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0, nrows, S, blocks, G)) return rc;
+  March<TreeDev> M;
+  if (int rc = march_setup(W, tree, opts, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0, nrows, stream, M))
+    return rc;
   if (!out_rgb_dev || !out_depth_dev || !out_acc_dev) return pob_fail(W, "output pointer is NULL");
-  if (blocks == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  pob_count_launch();
-  octree_dispatch(G, T.K, [&](auto g_, auto kpl_) {
-    octree_render_kernel<decltype(g_)::value, decltype(kpl_)::value, true><<<blocks, 256, 0, st>>>(
-        T, O, S, out_rgb_dev, counters_dev, out_depth_dev, out_acc_dev);
+  return march_launch(W, M, [&](auto kpl) {
+    octree_render_kernel<decltype(kpl)::value, true><<<M.blocks, 256, 0, M.st>>>(M.T, M.O, M.S, out_rgb_dev,
+                                                                                 counters_dev, out_depth_dev,
+                                                                                 out_acc_dev);
   });
-  POB_CUDA(W, cudaGetLastError());
-  return 0;
 }
 
 int pob_octree_render_backward(const pob_octree* tree, const pob_octree_opts* opts, const float* origins_dev,
                                const float* dirs_dev, const float* vdirs_dev, int64_t n_rays, const pob_camera* cam,
                                int row0, int nrows, const float* grad_out_dev, float* grad_data_dev, void* stream) {
   const char* W = "pob_octree_render_backward";
-  TreeDev T;
-  Opts O;
-  RaySrc S;
-  unsigned blocks = 0;
-  if (int rc = tree_dev(W, tree, T)) return rc;
-  if (int rc = opts_dev(W, opts, O)) return rc;
-  const int G = group_width(T.K);
-  if (int rc = ray_src(W, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0, nrows, S, blocks, G)) return rc;
+  March<TreeDev> M;
+  if (int rc = march_setup(W, tree, opts, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0, nrows, stream, M))
+    return rc;
   if (!grad_out_dev || !grad_data_dev) return pob_fail(W, "gradient pointer is NULL");
-  if (blocks == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  pob_count_launch();
-  POB_OCTREE_DISPATCH(octree_backward_kernel, G, T.K, T, O, S, grad_out_dev, grad_data_dev, nullptr, nullptr);
-  POB_CUDA(W, cudaGetLastError());
-  return 0;
+  return march_launch(W, M, [&](auto kpl) {
+    octree_backward_kernel<decltype(kpl)::value><<<M.blocks, 256, 0, M.st>>>(M.T, M.O, M.S, grad_out_dev,
+                                                                             grad_data_dev, nullptr, nullptr);
+  });
 }
 
 int pob_octree_render_depth_backward(const pob_octree* tree, const pob_octree_opts* opts, const float* origins_dev,
@@ -1314,24 +1264,14 @@ int pob_octree_render_depth_backward(const pob_octree* tree, const pob_octree_op
                                      const float* grad_depth_dev, const float* grad_acc_dev, float* grad_data_dev,
                                      void* stream) {
   const char* W = "pob_octree_render_depth_backward";
-  TreeDev T;
-  Opts O;
-  RaySrc S;
-  unsigned blocks = 0;
-  if (int rc = tree_dev(W, tree, T)) return rc;
-  if (int rc = opts_dev(W, opts, O)) return rc;
-  const int G = group_width(T.K);
-  if (int rc = ray_src(W, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0, nrows, S, blocks, G)) return rc;
+  March<TreeDev> M;
+  if (int rc = march_setup(W, tree, opts, origins_dev, dirs_dev, vdirs_dev, n_rays, cam, row0, nrows, stream, M))
+    return rc;
   if (!grad_data_dev) return pob_fail(W, "gradient pointer is NULL");
-  if (blocks == 0) return 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  pob_count_launch();
-  octree_dispatch(G, T.K, [&](auto g_, auto kpl_) {
-    octree_backward_kernel<decltype(g_)::value, decltype(kpl_)::value, true><<<blocks, 256, 0, st>>>(
-        T, O, S, grad_rgb_dev, grad_data_dev, grad_depth_dev, grad_acc_dev);
+  return march_launch(W, M, [&](auto kpl) {
+    octree_backward_kernel<decltype(kpl)::value, true><<<M.blocks, 256, 0, M.st>>>(
+        M.T, M.O, M.S, grad_rgb_dev, grad_data_dev, grad_depth_dev, grad_acc_dev);
   });
-  POB_CUDA(W, cudaGetLastError());
-  return 0;
 }
 
 int pob_octree_train_persp(const pob_octree* tree, const pob_octree_opts* opts, const pob_camera* cam, int row0,

@@ -27,6 +27,7 @@ inside its fused launch (pob_octree_train_persp_ndc).  Depth is then a distance 
 """
 import collections
 import ctypes
+import math
 
 import numpy as np
 import torch
@@ -79,60 +80,42 @@ def camera_array(c2ws, width, height, fx, fy=None, device="cuda"):
     return torch.from_numpy(out).to(device)
 
 
+def _ray_src(rays, cam, row0, nrows):
+    """-> (the origins, dirs, vdirs, n_rays, cam, row0, nrows arguments of the octree entry points, the leading shape of
+    their outputs): explicit rays (cam None) give [n], a camera's pixel-row slab [nrows, W]"""
+    if cam is None:
+        ro, rd, rv = rays
+        return (ptr(ro), ptr(rd), ptr(rv), ro.shape[0], None, 0, 0), (ro.shape[0],)
+    return (None, None, None, 0, ctypes.byref(cam), row0, nrows), (nrows, int(cam.width))
+
+
 class _RenderFn(torch.autograd.Function):
-    """autograd edge: d loss / d tree.data through pob_octree_render_backward."""
+    """autograd edge: d loss / d tree.data through pob_octree_render_backward, or with return_depth, of (rgb, depth,
+    acc) through pob_octree_render_depth_backward (an output whose gradient autograd leaves undefined is passed as
+    NULL, i.e. zero)."""
 
     @staticmethod
-    def forward(ctx, data, renderer, rays, cam, row0, nrows, opts):
-        ctx.renderer, ctx.rays, ctx.cam, ctx.row0, ctx.nrows = renderer, rays, cam, row0, nrows
-        return renderer._render_raw(rays, cam, row0, nrows, opts)
+    def forward(ctx, data, renderer, rays, cam, row0, nrows, opts, return_depth):
+        ctx.set_materialize_grads(not return_depth)
+        ctx.renderer, ctx.src, ctx.return_depth = renderer, (rays, cam, row0, nrows), return_depth
+        return renderer._render_raw(rays, cam, row0, nrows, opts, return_depth=return_depth)
 
     @staticmethod
-    def backward(ctx, grad_out):
-        r = ctx.renderer
-        tree = r.tree
+    def backward(ctx, *grads):
+        tree = ctx.renderer.tree
         g = torch.zeros_like(tree.data)
         t = tree.c_struct()
-        o = r._opts(False)
-        go = grad_out.reshape(-1, 3).contiguous().float()
-        if ctx.cam is None:
-            ro, rd, rv = ctx.rays
-            check(lib.pob_octree_render_backward(ctypes.byref(t), ctypes.byref(o), ptr(ro), ptr(rd), ptr(rv),
-                                                 ro.shape[0], None, 0, 0, ptr(go), ptr(g), stream_ptr()))
-        else:
-            check(lib.pob_octree_render_backward(ctypes.byref(t), ctypes.byref(o), None, None, None, 0,
-                                                 ctypes.byref(ctx.cam), ctx.row0, ctx.nrows, ptr(go), ptr(g),
-                                                 stream_ptr()))
-        return g, None, None, None, None, None, None
-
-
-class _RenderDepthFn(torch.autograd.Function):
-    """autograd edge of (rgb, depth, acc): d loss / d tree.data through pob_octree_render_depth_backward (an output
-    whose gradient autograd leaves undefined is passed as NULL, i.e. zero)."""
-
-    @staticmethod
-    def forward(ctx, data, renderer, rays, cam, row0, nrows, opts):
-        ctx.set_materialize_grads(False)
-        ctx.renderer, ctx.rays, ctx.cam, ctx.row0, ctx.nrows = renderer, rays, cam, row0, nrows
-        return renderer._render_raw(rays, cam, row0, nrows, opts, return_depth=True)
-
-    @staticmethod
-    def backward(ctx, g_rgb, g_depth, g_acc):
-        r = ctx.renderer
-        tree = r.tree
-        g = torch.zeros_like(tree.data)
-        t = tree.c_struct()
-        o = r._opts(False)
+        o = ctx.renderer._opts(False)
+        src, _ = _ray_src(*ctx.src)
         flat = lambda x, c: None if x is None else x.reshape(-1, c).contiguous().float()   # noqa: E731
-        gr, gd, ga = flat(g_rgb, 3), flat(g_depth, 1), flat(g_acc, 1)
-        if ctx.cam is None:
-            ro, rd, rv = ctx.rays
-            src = (ptr(ro), ptr(rd), ptr(rv), ro.shape[0], None, 0, 0)
+        if ctx.return_depth:
+            gr, gd, ga = flat(grads[0], 3), flat(grads[1], 1), flat(grads[2], 1)
+            check(lib.pob_octree_render_depth_backward(ctypes.byref(t), ctypes.byref(o), *src, ptr(gr), ptr(gd),
+                                                       ptr(ga), ptr(g), stream_ptr()))
         else:
-            src = (None, None, None, 0, ctypes.byref(ctx.cam), ctx.row0, ctx.nrows)
-        check(lib.pob_octree_render_depth_backward(ctypes.byref(t), ctypes.byref(o), *src, ptr(gr), ptr(gd), ptr(ga),
-                                                   ptr(g), stream_ptr()))
-        return g, None, None, None, None, None, None
+            check(lib.pob_octree_render_backward(ctypes.byref(t), ctypes.byref(o), *src, ptr(flat(grads[0], 3)),
+                                                 ptr(g), stream_ptr()))
+        return g, None, None, None, None, None, None, None
 
 
 def disparity(depth, acc):
@@ -154,15 +137,8 @@ class VolumeRenderer:
 
     def _ndc_rays(self, rays, cam, row0, nrows):
         """pob_ndc_rays: the NDC rays of explicit world rays (cam None) or of a camera's pixel-row slab"""
-        dev = self.tree.device
-        if cam is None:
-            ro, rd, rv = rays
-            n = ro.shape[0]
-            src = (ptr(ro), ptr(rd), ptr(rv), n, None, 0, 0)
-        else:
-            n = nrows * int(cam.width)
-            src = (None, None, None, 0, ctypes.byref(cam), row0, nrows)
-        out = [torch.empty((n, 3), dtype=torch.float32, device=dev) for _ in range(3)]
+        src, shape = _ray_src(rays, cam, row0, nrows)
+        out = [torch.empty((math.prod(shape), 3), dtype=torch.float32, device=self.tree.device) for _ in range(3)]
         check(lib.pob_ndc_rays(ctypes.byref(self.ndc), *src, *map(ptr, out), stream_ptr()))
         return tuple(out)
 
@@ -180,13 +156,7 @@ class VolumeRenderer:
         tree = self.tree
         t = tree.c_struct()
         quant = isinstance(t, _lib.OctreeQuant)      # a compressed tree (n3tree.QuantTree)
-        if cam is None:
-            ro, rd, rv = rays
-            shape = (ro.shape[0],)
-            src = (ptr(ro), ptr(rd), ptr(rv), ro.shape[0], None, 0, 0)
-        else:
-            shape = (nrows, int(cam.width))
-            src = (None, None, None, 0, ctypes.byref(cam), row0, nrows)
+        src, shape = _ray_src(rays, cam, row0, nrows)
         out = torch.empty(shape + (3,), dtype=torch.float32, device=tree.device)
         if not return_depth:
             fn = lib.pob_octree_render_quant if quant else lib.pob_octree_render
@@ -213,8 +183,7 @@ class VolumeRenderer:
         data = getattr(self.tree, "data", None)      # a QuantTree has none
         if torch.is_grad_enabled() and data is not None and data.requires_grad:
             self._check_trainable("rendering with tree.data.requires_grad")
-            fn = _RenderDepthFn if return_depth else _RenderFn
-            return fn.apply(data, self, rays, cam, row0, nrows, opts)
+            return _RenderFn.apply(data, self, rays, cam, row0, nrows, opts, return_depth)
         return self._render_raw(rays, cam, row0, nrows, opts, counters, return_depth)
 
     def forward(self, rays, fast=False, counters=None, return_depth=False):

@@ -113,7 +113,7 @@ def main():
             for p in poses:
                 r.render_persp(p, W, H, focal, fast=fast, counters=counters)
         visits, hits = [int(v) / len(poses) for v in counters.cpu().tolist()]
-        # algorithmic bytes: per leaf visit the child entries along the descent are L1/L2-resident (shared by the 16
+        # algorithmic bytes: per leaf visit the child entries along the descent are L1/L2-resident (shared by the 4
         # lanes and by neighbouring rays); the compulsory part is sigma (4 B) per visit + 3K coefficients per hit
         alg = visits * 4 + hits * 3 * K * 4
         out[f"render_persp_fast{int(fast)}"] = {
