@@ -1,4 +1,4 @@
-// capi_util.h — helpers shared by the extern "C" translation units (capi.cu, pipeline.cu).
+// capi_util.h — helpers shared by the extern "C" translation units (capi.cu, pipeline.cu, projection.cu).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -8,6 +8,8 @@ int pob_fail(const char* where, const char* what);
 int pob_cuda_fail(const char* where, cudaError_t e);
 // the SM count the kernels split their work for (capi.cu: sm_count), or 0 with the reason recorded under `where`
 int pob_sms_or_fail(const char* where);
+// sh_deg, the packed weights pointer and precision of an MLP call, then the device: its SM count, or 0 after a
+// refusal recorded under `where`
 int pob_check_common(const char* where, const void* packed, int sh_deg, int precision);
 // POB_SIGMA_RELU or POB_SIGMA_SOFTPLUS, else pob_fail
 int pob_check_sigma_activation(const char* where, int sigma_activation);
@@ -15,7 +17,20 @@ int pob_check_sigma_activation(const char* where, int sigma_activation);
 // 0 / 1 and net_activation a POB_NET_* code, otherwise pob_fail
 struct pob_posenc;
 int pob_check_posenc(const char* where, const pob_posenc* posenc, pob::NetDesc& out);
+// the FwdParams of one MLP (weights, sh_deg and network; no source or output)
 pob::FwdParams pob_base_params(const void* packed, int sh_deg, pob::NetDesc net);
+// the first checks of every point evaluator, pob_check_common then pob_check_posenc: the SM count and, in p, the
+// base params of the network, or 0 after a refusal recorded under `where`.  Internal to each translation unit, so the
+// library exports no symbol for it.
+static inline int pob_eval_setup(const char* where, const void* packed, int sh_deg, const pob_posenc* posenc,
+                                 int precision, pob::FwdParams& p) {
+  const int sms = pob_check_common(where, packed, sh_deg, precision);
+  if (!sms) return 0;
+  pob::NetDesc net;
+  if (pob_check_posenc(where, posenc, net)) return 0;
+  p = pob_base_params(packed, sh_deg, net);
+  return sms;
+}
 
 #define POB_CUDA(where, call)                               \
   do {                                                      \
@@ -33,3 +48,11 @@ struct PobPhaseTimer {
   int slot;
   cudaStream_t st;
 };
+
+// one kernel launch on stream `st`: counted, timed under `phase` and its error returned from the caller
+#define POB_LAUNCH(where, phase, st, call) \
+  do {                                     \
+    pob_count_launch();                    \
+    PobPhaseTimer _t(phase, st);           \
+    POB_CUDA(where, call);                 \
+  } while (0)

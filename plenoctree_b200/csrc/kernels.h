@@ -118,6 +118,9 @@ struct FwdParams {
   int net_act;                 // NetAct of Dense_0..Dense_7
 };
 
+// sh_deg -1 (3 raw rgb channels) to 4, and the coefficients per channel of a degree: K = 1 for -1, else (sh_deg+1)^2
+inline bool valid_deg(int sh_deg) { return sh_deg >= -1 && sh_deg <= 4; }
+inline int K_of(int sh_deg) { return sh_deg < 0 ? 1 : (sh_deg + 1) * (sh_deg + 1); }
 // padded heads width for K spherical-harmonic coefficients per channel
 inline int heads_width(int K) { return ((1 + 3 * K) + 15) / 16 * 16; }
 // bytes of one forward weight image (hi or lo): the trunk slots, then the heads slots of NH rows

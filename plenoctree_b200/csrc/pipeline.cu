@@ -19,6 +19,8 @@ using namespace pob;
 
 struct Level {
   // sizes
+  int N;              // samples per ray (0: no fine level)
+  bool last;          // the last level: in training its arrays also carry the sparsity points behind its rays
   long long M;        // samples
   long long tiles;    // 128-row tiles of padded_rows(M)
   // buffers
@@ -35,7 +37,8 @@ struct Level {
 };
 
 struct Workspace {
-  Level lv[2];        // coarse, fine; in training the LAST level also carries the sparsity points behind its rays
+  Level lv[2];        // coarse, fine
+  int levels;         // 1 or 2
   float* partials[2]; // wgrad partials of the two MLPs' launches
   uint32_t* progress; // per tile of level 0, then of level 1: mlp_bwd -> mlp_wgrad progress counters (wgrad_body.cuh)
   size_t progress_bytes;
@@ -73,12 +76,13 @@ Workspace carve(const pob_render_config& c, int training, uint8_t* base, bool x3
     return p;
   };
   const long long R = c.max_rays;
-  const int Ns[2] = {c.num_coarse_samples, c.num_fine_samples > 0 ? c.num_coarse_samples + c.num_fine_samples : 0};
-  const int last = c.num_fine_samples > 0 ? 1 : 0;
+  w.levels = c.num_fine_samples > 0 ? 2 : 1;
   for (int l = 0; l < 2; ++l) {
     Level& L = w.lv[l];
-    const long long Mr = R * Ns[l];                                    // ray samples
-    L.M = Mr + ((training && l == last) ? c.sparsity_npoints : 0);     // + sparsity points (train.py:77-83)
+    L.N = l == 0 ? c.num_coarse_samples : (w.levels == 2 ? c.num_coarse_samples + c.num_fine_samples : 0);
+    L.last = l == w.levels - 1;
+    const long long Mr = R * L.N;                                      // ray samples
+    L.M = Mr + ((training && L.last) ? c.sparsity_npoints : 0);        // + sparsity points (train.py:77-83)
     L.tiles = tiles_for(L.M);
     if (Mr == 0) continue;
     L.z = (float*)take(sizeof(float) * Mr);
@@ -104,7 +108,7 @@ Workspace carve(const pob_render_config& c, int training, uint8_t* base, bool x3
   if (training && x3) {
     for (int l = 0; l < 2; ++l) {
       Level& L = w.lv[l];
-      if (R * Ns[l] == 0) continue;
+      if (L.N == 0) continue;
       L.H_lo = take(size_t(L.tiles) * NUM_TRUNK * A_TILE_BYTES);
       L.E_lo = take(size_t(L.tiles) * E_TILE_BYTES);
       L.DZ_lo = take(size_t(L.tiles) * NUM_TRUNK * A_TILE_BYTES);
@@ -112,104 +116,70 @@ Workspace carve(const pob_render_config& c, int training, uint8_t* base, bool x3
     }
     for (int i = 0; i < 2; ++i)
       for (int q = 0; q < 2; ++q) w.partials_x3[i][q] = (float*)take(sizeof(float) * WG_MAX_CTAS * WG_PARTIAL_FLOATS);
-    const int K = c.sh_deg < 0 ? 1 : (c.sh_deg + 1) * (c.sh_deg + 1);
-    for (int i = 0; i < 2; ++i) w.wt_lo[i] = take(bwd_image_bytes(heads_width(K)));
+    for (int i = 0; i < 2; ++i) w.wt_lo[i] = take(bwd_image_bytes(heads_width(K_of(c.sh_deg))));
   }
   w.total = off;
   return w;
 }
 
-int check_cfg(const char* where, const pob_render_config* c) {
+// the config's checks; `net` is then its point encoder and trunk activation
+int check_cfg(const char* where, const pob_render_config* c, NetDesc& net) {
   if (!c) return pob_fail(where, "config is NULL");
-  if (c->sh_deg < -1 || c->sh_deg > 4) return pob_fail(where, "sh_deg must be in [-1, 4]");
+  if (!valid_deg(c->sh_deg)) return pob_fail(where, "sh_deg must be in [-1, 4]");
   if (c->num_coarse_samples < 3 || c->num_coarse_samples > MAX_RAY_SAMPLES)
     return pob_fail(where, "num_coarse_samples must be in [3, 1024]");
   if (c->num_fine_samples < 0 || c->num_coarse_samples + c->num_fine_samples > MAX_RAY_SAMPLES)
     return pob_fail(where, "num_coarse_samples + num_fine_samples must be <= 1024");
   if (c->max_rays <= 0) return pob_fail(where, "max_rays must be positive");
   if (c->sparsity_npoints < 0) return pob_fail(where, "sparsity_npoints must be >= 0");
-  NetDesc net;
   if (int e = pob_check_posenc(where, c->posenc, net)) return e;
   return pob_check_sigma_activation(where, c->sigma_activation);
 }
 
-// the point encoder and trunk activation of a config that check_cfg accepted
-NetDesc cfg_net(const pob_render_config& c) {
-  NetDesc net;
-  pob_check_posenc("", c.posenc, net);
-  return net;
-}
-
-FwdParams ray_fwd_params(const void* packed, int sh_deg, NetDesc net, const float* o, const float* d,
-                         const float* v, const float* z, int R, int N, float4* out) {
-  FwdParams p = pob_base_params(packed, sh_deg, net);
-  p.src_mode = SRC_RAYS;
-  p.M = (long long)R * N;
-  p.M_rays = p.M;
-  p.origins = o;
-  p.directions = d;
-  p.viewdirs = v;
-  p.zvals = z;
-  p.n_per_ray = N;
-  p.out_mode = OUT_RGBS;
-  p.out_rgbs = out;
-  return p;
-}
-
-// forward of both levels; fills comp/disp/acc (and rgbs, weights, z) of the workspace levels
-int forward_levels(const char* where, const pob_render_config& c, Workspace& w, const void* pk_c,
-                   const void* pk_f, const float* o, const float* d, const float* v, int R,
-                   const float* z_base, const float* t_rand, const float* u, int u_per_ray,
-                   const float* z_fine, int precision, bool save, cudaStream_t st,
-                   const float* sp_points = nullptr, long long sp_n = 0) {
-  const int sms = pob_sms_or_fail(where);
-  if (!sms) return 1;
-  const int Nc = c.num_coarse_samples, Nf = c.num_fine_samples;
-  const NetDesc net = cfg_net(c);
-  Level& C = w.lv[0];
-  { pob_count_launch(1); PobPhaseTimer _t(POB_PH_RENDER, st); POB_CUDA(where, launch_sample_coarse(z_base, t_rand, R, Nc, C.z, st)); }
-  {
-    FwdParams p = ray_fwd_params(pk_c, c.sh_deg, net, o, d, v, C.z, R, Nc, C.rgbs);
-    p.sigma_noise = c.sigma_noise_coarse_dev;
-    p.sigma_act = c.sigma_activation;
-    if (Nf == 0 && sp_n > 0) {     // single-level model: the sparsity points ride on this launch
-      p.M += sp_n;
-      p.extra_points = sp_points;
-    }
-    if (save) {
-      p.save_h = C.H;
-      p.save_e = C.E;
-      p.save_mask = C.mask;
-      p.save_h_lo = C.H_lo;   // x3 only (null otherwise)
-      p.save_e_lo = C.E_lo;
-    }
-    { pob_count_launch(1); PobPhaseTimer _t(POB_PH_FWD, st); POB_CUDA(where, launch_mlp_fwd(p, precision, sms, st)); }
-  }
-  { pob_count_launch(1); PobPhaseTimer _t(POB_PH_RENDER, st); POB_CUDA(where, launch_composite_fwd(C.rgbs, C.z, d, R, Nc, c.white_bkgd, C.comp, C.disp, C.acc, C.weights, st)); }
-  if (Nf > 0) {
-    Level& F = w.lv[1];
-    if (z_fine)
-      POB_CUDA(where, cudaMemcpyAsync(F.z, z_fine, sizeof(float) * size_t(R) * (Nc + Nf),
-                                      cudaMemcpyDeviceToDevice, st));
+// forward of every level; fills comp/disp/acc (and rgbs, weights, z) of the workspace levels.  The depths of a level
+// are the coarse draw, the caller's z_fine or the resampling of the coarse weights.
+int forward_levels(const char* where, const pob_render_config& c, NetDesc net, int sms, Workspace& w,
+                   const void* const packed[2], const float* o, const float* d, const float* v, int R,
+                   const float* z_base, const float* t_rand, const float* u, int u_per_ray, const float* z_fine,
+                   int precision, bool save, cudaStream_t st, const float* sp_points = nullptr, long long sp_n = 0) {
+  const float* const noise[2] = {c.sigma_noise_coarse_dev, c.sigma_noise_fine_dev};
+  for (int l = 0; l < w.levels; ++l) {
+    Level& L = w.lv[l];
+    if (l == 0)
+      POB_LAUNCH(where, POB_PH_RENDER, st, launch_sample_coarse(z_base, t_rand, R, L.N, L.z, st));
+    else if (z_fine)
+      POB_CUDA(where, cudaMemcpyAsync(L.z, z_fine, sizeof(float) * size_t(R) * L.N, cudaMemcpyDeviceToDevice, st));
     else
-      { pob_count_launch(1); PobPhaseTimer _t(POB_PH_RENDER, st); POB_CUDA(where, launch_sample_pdf(C.z, C.weights, u, u_per_ray, R, Nc, Nf, F.z, st)); }
-    FwdParams p = ray_fwd_params(pk_f, c.sh_deg, net, o, d, v, F.z, R, Nc + Nf, F.rgbs);
-    p.sigma_noise = c.sigma_noise_fine_dev;
+      POB_LAUNCH(where, POB_PH_RENDER, st,
+                 launch_sample_pdf(w.lv[0].z, w.lv[0].weights, u, u_per_ray, R, c.num_coarse_samples,
+                                   c.num_fine_samples, L.z, st));
+    FwdParams p = pob_base_params(packed[l], c.sh_deg, net);
+    p.src_mode = SRC_RAYS;
+    p.M = (long long)R * L.N;
+    p.M_rays = p.M;
+    p.origins = o;
+    p.directions = d;
+    p.viewdirs = v;
+    p.zvals = L.z;
+    p.n_per_ray = L.N;
+    p.out_mode = OUT_RGBS;
+    p.out_rgbs = L.rgbs;
+    p.sigma_noise = noise[l];
     p.sigma_act = c.sigma_activation;
-    if (sp_n > 0) {                // the sparsity points ride behind the fine level's ray samples (same MLP)
+    if (L.last && sp_n > 0) {     // the sparsity points ride behind the last level's ray samples (same MLP)
       p.M += sp_n;
       p.extra_points = sp_points;
     }
     if (save) {
-      p.save_h = F.H;
-      p.save_e = F.E;
-      p.save_mask = F.mask;
-      p.save_h_lo = F.H_lo;   // x3 only (null otherwise)
-      p.save_e_lo = F.E_lo;
+      p.save_h = L.H;
+      p.save_e = L.E;
+      p.save_mask = L.mask;
+      p.save_h_lo = L.H_lo;   // x3 only (null otherwise)
+      p.save_e_lo = L.E_lo;
     }
-    { pob_count_launch(1); PobPhaseTimer _t(POB_PH_FWD, st); POB_CUDA(where, launch_mlp_fwd(p, precision, sms, st)); }
-    { pob_count_launch(1); PobPhaseTimer _t(POB_PH_RENDER, st); POB_CUDA(where, launch_composite_fwd(F.rgbs, F.z, d, R, Nc + Nf, c.white_bkgd, F.comp, F.disp, F.acc,
-                                         F.weights, st)); }
+    POB_LAUNCH(where, POB_PH_FWD, st, launch_mlp_fwd(p, precision, sms, st));
+    POB_LAUNCH(where, POB_PH_RENDER, st,
+               launch_composite_fwd(L.rgbs, L.z, d, R, L.N, c.white_bkgd, L.comp, L.disp, L.acc, L.weights, st));
   }
   return 0;
 }
@@ -253,12 +223,14 @@ int check_workspace_extent(const char* where, const void* ws, size_t bytes) {
 extern "C" {
 
 int64_t pob_workspace_bytes(const pob_render_config* cfg, int training) {
-  if (check_cfg("pob_workspace_bytes", cfg)) return -1;
+  NetDesc net;
+  if (check_cfg("pob_workspace_bytes", cfg, net)) return -1;
   return (int64_t)carve(*cfg, training, nullptr).total;
 }
 
 int64_t pob_train_workspace_bytes(const pob_render_config* cfg, int precision) {
-  if (check_cfg("pob_train_workspace_bytes", cfg)) return -1;
+  NetDesc net;
+  if (check_cfg("pob_train_workspace_bytes", cfg, net)) return -1;
   if (precision != POB_PREC_FP16 && precision != POB_PREC_FP16X3) {
     pob_fail("pob_train_workspace_bytes", "precision must be POB_PREC_FP16 or POB_PREC_FP16X3");
     return -1;
@@ -272,8 +244,10 @@ int pob_render_rays(const pob_render_config* cfg, const void* packed_coarse_dev,
                     int u_per_ray, const float* z_fine_dev, float* out_coarse_dev, float* out_fine_dev,
                     void* workspace_dev, int precision, void* stream) {
   const char* where = "pob_render_rays";
-  if (int e = check_cfg(where, cfg)) return e;
-  if (int e = pob_check_common(where, packed_coarse_dev, cfg->sh_deg, precision)) return e;
+  NetDesc net;
+  if (int e = check_cfg(where, cfg, net)) return e;
+  const int sms = pob_check_common(where, packed_coarse_dev, cfg->sh_deg, precision);
+  if (!sms) return 1;
   if (n_rays < 0 || n_rays > cfg->max_rays) return pob_fail(where, "n_rays exceeds cfg->max_rays");
   if (n_rays == 0) return 0;
   if (!origins_dev || !directions_dev || !viewdirs_dev || !z_base_dev || !workspace_dev || !out_coarse_dev)
@@ -282,14 +256,14 @@ int pob_render_rays(const pob_render_config* cfg, const void* packed_coarse_dev,
     return pob_fail(where, "fine level needs packed_fine, u (or z_fine) and out_fine");
   cudaStream_t st = (cudaStream_t)stream;
   Workspace w = carve(*cfg, 0, (uint8_t*)workspace_dev);
-  if (int e = forward_levels(where, *cfg, w, packed_coarse_dev, packed_fine_dev, origins_dev, directions_dev,
-                             viewdirs_dev, n_rays, z_base_dev, t_rand_dev, u_dev, u_per_ray, z_fine_dev,
-                             precision, false, st))
+  const void* const packed[2] = {packed_coarse_dev, packed_fine_dev};
+  if (int e = forward_levels(where, *cfg, net, sms, w, packed, origins_dev, directions_dev, viewdirs_dev, n_rays,
+                             z_base_dev, t_rand_dev, u_dev, u_per_ray, z_fine_dev, precision, false, st))
     return e;
   const unsigned grid = (n_rays + 255) / 256;
-  pob_count_launch(cfg->num_fine_samples > 0 ? 2 : 1);
+  pob_count_launch(w.levels);
   pack_outputs_kernel<<<grid, 256, 0, st>>>(w.lv[0].comp, w.lv[0].disp, w.lv[0].acc, n_rays, out_coarse_dev);
-  if (cfg->num_fine_samples > 0)
+  if (w.levels == 2)
     pack_outputs_kernel<<<grid, 256, 0, st>>>(w.lv[1].comp, w.lv[1].disp, w.lv[1].acc, n_rays, out_fine_dev);
   POB_CUDA(where, cudaGetLastError());
   return 0;
@@ -303,26 +277,24 @@ int pob_loss_and_grad_flags(const pob_render_config* cfg, const pob_train_hparam
                             void* mlp0_done_event, const float* params_dev, int precision, int flags, void* stream) {
   const char* where = "pob_loss_and_grad";
   if (flags & ~POB_TRAIN_DISCARD_SAVED_GRADS) return pob_fail(where, "unknown bits in flags");
-  if (int e = check_cfg(where, cfg)) return e;
+  NetDesc net;
+  if (int e = check_cfg(where, cfg, net)) return e;
   if (!hp) return pob_fail(where, "hparams is NULL");
-  if (int e = pob_check_common(where, packed_coarse_dev, cfg->sh_deg, precision)) return e;
+  const int sms = pob_check_common(where, packed_coarse_dev, cfg->sh_deg, precision);
+  if (!sms) return 1;
   const bool x3 = precision == POB_PREC_FP16X3;
   if (n_rays <= 0 || n_rays > cfg->max_rays) return pob_fail(where, "n_rays out of range");
   if (!origins_dev || !directions_dev || !viewdirs_dev || !pixels_dev || !z_base_dev || !workspace_dev ||
       !grad_flat_dev || !stats_dev)
     return pob_fail(where, "NULL pointer");
   if (x3 && !params_dev) return pob_fail(where, "POB_PREC_FP16X3 needs params_dev (the flat fp32 parameters)");
-  const int Nc = cfg->num_coarse_samples, Nf = cfg->num_fine_samples;
-  if (Nf > 0 && (!packed_fine_dev || (!u_dev && !z_fine_dev)))
+  if (cfg->num_fine_samples > 0 && (!packed_fine_dev || (!u_dev && !z_fine_dev)))
     return pob_fail(where, "fine level needs packed_fine and u (or z_fine)");
   const bool sparsity = hp->sparsity_weight > 0.f && cfg->sparsity_npoints > 0;
   if (sparsity && !sp_points_dev) return pob_fail(where, "sparsity term needs sp_points");
   if (!(hp->loss_scale > 0.f)) return pob_fail(where, "loss_scale must be positive");
   cudaStream_t st = (cudaStream_t)stream;
-  const int sms = pob_sms_or_fail(where);
-  if (!sms) return 1;
-  const int K = cfg->sh_deg < 0 ? 1 : (cfg->sh_deg + 1) * (cfg->sh_deg + 1);
-  const NetDesc net = cfg_net(*cfg);
+  const int K = K_of(cfg->sh_deg);
   const int W = posenc_width(net.pe);
   const int P = flat_layout(K, W).total;
   Workspace w = carve(*cfg, 1, (uint8_t*)workspace_dev, x3);
@@ -332,31 +304,31 @@ int pob_loss_and_grad_flags(const pob_render_config* cfg, const pob_train_hparam
   POB_CUDA(where, cudaMemsetAsync(w.progress, 0, w.progress_bytes, st));
   if (x3) {
     // residual of the transposed weights (the packed blob holds only their hi part)
-    for (int mlp = 0; mlp < (Nf > 0 ? 2 : 1); ++mlp)
-      { pob_count_launch(1); PobPhaseTimer _t(POB_PH_OPTIM, st); POB_CUDA(where, launch_pack_wt_lo(params_dev + size_t(mlp) * P, K, W, w.wt_lo[mlp], st)); }
+    for (int mlp = 0; mlp < w.levels; ++mlp)
+      POB_LAUNCH(where, POB_PH_OPTIM, st, launch_pack_wt_lo(params_dev + size_t(mlp) * P, K, W, w.wt_lo[mlp], st));
   }
   // The sparsity points (train.py:77-83: eval_points_raw of the fine MLP on uniform points) ride behind the ray
   // samples of the last level: same MLP, same launches, rows [n_rays * N, n_rays * N + sp_n) of its arrays.
   const long long sp_n = sparsity ? cfg->sparsity_npoints : 0;
-  if (int e = forward_levels(where, *cfg, w, packed_coarse_dev, packed_fine_dev, origins_dev, directions_dev,
-                             viewdirs_dev, n_rays, z_base_dev, t_rand_dev, u_dev, u_per_ray, z_fine_dev,
-                             precision, true, st, sp_points_dev, sp_n))
+  const void* const packed[2] = {packed_coarse_dev, packed_fine_dev};
+  if (int e = forward_levels(where, *cfg, net, sms, w, packed, origins_dev, directions_dev, viewdirs_dev, n_rays,
+                             z_base_dev, t_rand_dev, u_dev, u_per_ray, z_fine_dev, precision, true, st, sp_points_dev,
+                             sp_n))
     return e;
   const float gscale = hp->loss_scale * 2.0f / (3.0f * float(n_rays));
-  Level& C = w.lv[0];
-  Level& F = w.lv[1];
-  Level& LAST = Nf > 0 ? F : C;
-  const long long Mr_last = (long long)n_rays * (Nf > 0 ? Nc + Nf : Nc);
-  // ---- upstream gradients ----
-  { pob_count_launch(1); PobPhaseTimer _t(POB_PH_RENDER, st); POB_CUDA(where, launch_composite_bwd(C.rgbs, C.z, directions_dev, C.comp, pixels_dev, n_rays, Nc,
-                                       cfg->white_bkgd, gscale, cfg->sigma_activation, C.G, stats_dev + (Nf > 0 ? 1 : 0), st)); }
-  if (Nf > 0)
-    { pob_count_launch(1); PobPhaseTimer _t(POB_PH_RENDER, st); POB_CUDA(where, launch_composite_bwd(F.rgbs, F.z, directions_dev, F.comp, pixels_dev, n_rays, Nc + Nf,
-                                         cfg->white_bkgd, gscale, cfg->sigma_activation, F.G, stats_dev + 0, st)); }
+  // ---- upstream gradients: stats slot 0 takes the last level's loss, slot 1 the coarse one's of two levels ----
+  for (int l = 0; l < w.levels; ++l) {
+    Level& L = w.lv[l];
+    POB_LAUNCH(where, POB_PH_RENDER, st,
+               launch_composite_bwd(L.rgbs, L.z, directions_dev, L.comp, pixels_dev, n_rays, L.N, cfg->white_bkgd,
+                                    gscale, cfg->sigma_activation, L.G, stats_dev + (L.last ? 0 : 1), st));
+  }
   if (sparsity) {
+    Level& L = w.lv[w.levels - 1];
+    const long long Mr = (long long)n_rays * L.N;
     const float coef = hp->loss_scale * hp->sparsity_weight * hp->sparsity_length / float(sp_n);
-    { pob_count_launch(1); PobPhaseTimer _t(POB_PH_RENDER, st); POB_CUDA(where, launch_sparsity_grad(LAST.rgbs + Mr_last, int(sp_n), hp->sparsity_length, coef,
-                                                                                                    LAST.G + Mr_last, stats_dev + 2, st)); }
+    POB_LAUNCH(where, POB_PH_RENDER, st,
+               launch_sparsity_grad(L.rgbs + Mr, int(sp_n), hp->sparsity_length, coef, L.G + Mr, stats_dev + 2, st));
   }
   // ---- backward: per MLP one dgrad launch, then ONE wgrad launch over its saved dZ / h tiles ----
   // MLP_0 (coarse level only) is finished first: its branch of the graph is independent of MLP_1's
@@ -368,19 +340,18 @@ int pob_loss_and_grad_flags(const pob_render_config* cfg, const pob_train_hparam
   // 400 W power limit: 29.1-29.6 ms against 31.8-32.1 ms with the fp16 split (pass 0 beside the data gradient).
   const int NH = heads_width(K);
   const int dgrad_ctas = sms * (NH <= 64 ? DGRAD_SMS_OF_132 : DGRAD_SMS_OF_132_NH80) / 132;
-  for (int mlp = 0; mlp < (Nf > 0 ? 2 : 1); ++mlp) {
-    Level& L = mlp == 0 ? C : F;
-    const long long Mr = (long long)n_rays * (mlp == 0 ? Nc : Nc + Nf);
-    const long long Mm = Mr + (&L == &LAST ? sp_n : 0);
-    const void* pk = mlp == 0 ? packed_coarse_dev : packed_fine_dev;
+  for (int mlp = 0; mlp < w.levels; ++mlp) {
+    Level& L = w.lv[mlp];
+    const long long Mr = (long long)n_rays * L.N;
+    const long long Mm = Mr + (L.last ? sp_n : 0);
     BwdParams b;
     memset(&b, 0, sizeof(b));
     b.M = Mm;
     b.M_rays = Mr;
     b.G = L.G;
     b.viewdirs = viewdirs_dev;
-    b.n_per_ray = mlp == 0 ? Nc : Nc + Nf;
-    FwdParams base = pob_base_params(pk, cfg->sh_deg, net);
+    b.n_per_ray = L.N;
+    FwdParams base = pob_base_params(packed[mlp], cfg->sh_deg, net);
     b.w = base.w;
     b.sh_deg = cfg->sh_deg;
     b.K = base.K;
@@ -391,11 +362,11 @@ int pob_loss_and_grad_flags(const pob_render_config* cfg, const pob_train_hparam
     b.h_lo = L.H_lo;
     b.save_dz = L.DZ;
     b.save_do = L.DO;
-    b.progress = w.progress + (mlp == 0 ? 0 : C.tiles);
+    b.progress = w.progress + (mlp == 0 ? 0 : w.lv[0].tiles);
     b.wt_lo = w.wt_lo[mlp];
     b.save_dz_lo = L.DZ_lo;
     b.save_do_lo = L.DO_lo;
-    { pob_count_launch(); PobPhaseTimer _t(POB_PH_BWD, st); POB_CUDA(where, launch_mlp_bwd(b, precision, x3 ? sms : dgrad_ctas, st)); }
+    POB_LAUNCH(where, POB_PH_BWD, st, launch_mlp_bwd(b, precision, x3 ? sms : dgrad_ctas, st));
     const WgradSegment segs[X3_WGRAD_PASSES] = {{L.H, L.DZ, L.E, L.DO},
                                                 {L.H, L.DZ_lo, L.E, L.DO_lo},
                                                 {L.H_lo, L.DZ, L.E_lo, L.DO}};
@@ -415,11 +386,12 @@ int pob_loss_and_grad_flags(const pob_render_config* cfg, const pob_train_hparam
       passes[q].partials = partials[q];
       const int nctas = wgrad_assign_roles(g, (q == 0 && !x3) ? sms - dgrad_ctas : sms, passes[q].role_start,
                                            passes[q].role_count);
-      { pob_count_launch(); PobPhaseTimer _t(POB_PH_WGRAD, st); POB_CUDA(where, launch_mlp_wgrad(g, nctas, st)); }
+      POB_LAUNCH(where, POB_PH_WGRAD, st, launch_mlp_wgrad(g, nctas, st));
     }
-    { pob_count_launch(); PobPhaseTimer _t(POB_PH_OPTIM, st); POB_CUDA(where, launch_reduce_grads(passes, npass, K, W, 1.0f / hp->loss_scale,
-                                        grad_flat_dev + size_t(mlp) * P, st)); }
-    if (mlp == 0 && Nf > 0 && mlp0_done_event) POB_CUDA(where, cudaEventRecord((cudaEvent_t)mlp0_done_event, st));
+    POB_LAUNCH(where, POB_PH_OPTIM, st,
+               launch_reduce_grads(passes, npass, K, W, 1.0f / hp->loss_scale, grad_flat_dev + size_t(mlp) * P, st));
+    if (mlp == 0 && w.levels == 2 && mlp0_done_event)
+      POB_CUDA(where, cudaEventRecord((cudaEvent_t)mlp0_done_event, st));
   }
   return 0;
 }
@@ -452,17 +424,17 @@ int pob_adam_update_pe(int sh_deg, const pob_posenc* posenc, int num_mlps, float
                        float* m_dev, float* v_dev, float lr, float step, const float* lr_step_dev, float grad_mult,
                        float weight_decay_coef, void* packed_coarse_dev, void* packed_fine_dev, void* stream) {
   const char* where = "pob_adam_update";
-  if (sh_deg < -1 || sh_deg > 4) return pob_fail(where, "sh_deg must be in [-1, 4]");
+  if (!valid_deg(sh_deg)) return pob_fail(where, "sh_deg must be in [-1, 4]");
   NetDesc net;
   if (int e = pob_check_posenc(where, posenc, net)) return e;
   if (num_mlps < 1 || num_mlps > 2) return pob_fail(where, "num_mlps must be 1 or 2");
   if (!params_dev || !grads_dev || !m_dev || !v_dev || !packed_coarse_dev || (num_mlps == 2 && !packed_fine_dev))
     return pob_fail(where, "NULL pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  const int K = sh_deg < 0 ? 1 : (sh_deg + 1) * (sh_deg + 1);
-  const long long P = flat_layout(K, posenc_width(net.pe)).total;
-  { pob_count_launch(1); PobPhaseTimer _t(POB_PH_OPTIM, st); POB_CUDA(where, launch_adam(params_dev, grads_dev, m_dev, v_dev, P * num_mlps, lr, step, lr_step_dev, 0.9f, 0.999f, 1e-8f,
-                              grad_mult, weight_decay_coef, st)); }
+  const long long P = flat_layout(K_of(sh_deg), posenc_width(net.pe)).total;
+  POB_LAUNCH(where, POB_PH_OPTIM, st,
+             launch_adam(params_dev, grads_dev, m_dev, v_dev, P * num_mlps, lr, step, lr_step_dev, 0.9f, 0.999f, 1e-8f,
+                         grad_mult, weight_decay_coef, st));
   if (int e = pob_pack_weights_pe(params_dev, sh_deg, posenc, packed_coarse_dev, stream)) return e;
   if (num_mlps == 2)
     if (int e = pob_pack_weights_pe(params_dev + P, sh_deg, posenc, packed_fine_dev, stream)) return e;

@@ -330,19 +330,16 @@ int pob_sh_proj_points(const void* packed_dev, const pob_posenc* posenc, const f
                        const float* head_w_dev, const float* head_b_dev, void* workspace_dev, float* a_dev,
                        float* sigma_dev, void* stream) {
   const char* W = "pob_sh_proj_points";
-  if (int e = pob_check_common(W, packed_dev, -1, POB_PREC_FP16)) return e;
-  pob::NetDesc net;
-  if (int e = pob_check_posenc(W, posenc, net)) return e;
-  if (net.net_act != pob::NET_RELU) return pob_fail(W, "the vanilla trunk of the projection is relu");
+  pob::FwdParams p;
+  const int sms = pob_eval_setup(W, packed_dev, -1, posenc, POB_PREC_FP16, p);
+  if (!sms) return 1;
+  if (p.net_act != pob::NET_RELU) return pob_fail(W, "the vanilla trunk of the projection is relu");
   if (m < 0) return pob_fail(W, "negative point count");
   if (m == 0) return 0;
   if (!points_dev || !head_w_dev || !head_b_dev || !workspace_dev || !a_dev || !sigma_dev)
     return pob_fail(W, "NULL pointer");
-  const int sms = pob_sms_or_fail(W);
-  if (!sms) return 1;
   const pob::PointWs ws = pob::point_ws(m);
   uint8_t* base = static_cast<uint8_t*>(workspace_dev);
-  pob::FwdParams p = pob_base_params(packed_dev, -1, net);
   p.src_mode = pob::SRC_POINTS;
   p.M = m;
   p.points = points_dev;
@@ -351,16 +348,13 @@ int pob_sh_proj_points(const void* packed_dev, const pob_posenc* posenc, const f
   p.save_h = base + ws.h;
   p.save_e = base + ws.e;
   p.save_mask = reinterpret_cast<uint32_t*>(base + ws.mask);
-  pob_count_launch(2);
-  {
-    PobPhaseTimer _t(POB_PH_FWD, (cudaStream_t)stream);
-    POB_CUDA(W, pob::launch_mlp_fwd(p, 1, sms, (cudaStream_t)stream));
-  }
+  cudaStream_t st = (cudaStream_t)stream;
+  POB_LAUNCH(W, POB_PH_FWD, st, pob::launch_mlp_fwd(p, POB_PREC_FP16, sms, st));
   const size_t smem = pob::A_TILE_BYTES + size_t(pob::A_KC) * pob::PROJ_H * sizeof(float);
   POB_CUDA(W, cudaFuncSetAttribute(pob::proj_point_a_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
   const long long tiles = (m + pob::TILE_M - 1) / pob::TILE_M;
-  pob::proj_point_a_kernel<<<unsigned(tiles), 256, smem, (cudaStream_t)stream>>>(base + ws.h, m, head_w_dev,
-                                                                                  head_b_dev, a_dev);
+  pob_count_launch();
+  pob::proj_point_a_kernel<<<unsigned(tiles), 256, smem, st>>>(base + ws.h, m, head_w_dev, head_b_dev, a_dev);
   POB_CUDA(W, cudaGetLastError());
   return 0;
 }
@@ -378,7 +372,7 @@ int pob_sh_proj_directions(uint64_t seed, int64_t block0, int n_blocks, int n_di
   if (!w10e_dev || !t_dev || !basis_dev) return pob_fail(W, "NULL pointer");
   if (!pob_sms_or_fail(W)) return 1;
   if (n_blocks == 0) return 0;
-  const int K = (sh_deg + 1) * (sh_deg + 1);
+  const int K = pob::K_of(sh_deg);
   const size_t smem = size_t(pob::DIRS_PER_CTA) * (3 + 6 * deg_view) * sizeof(float);
   POB_CUDA(W, cudaFuncSetAttribute(pob::proj_directions_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                    int(smem)));
@@ -401,7 +395,7 @@ int pob_sh_proj_cells(int64_t n_cells, int samples_per_cell, int cells_per_block
     return pob_fail(W, "NULL pointer");
   if (!pob_sms_or_fail(W)) return 1;
   if (n_cells == 0) return 0;
-  const int K = (sh_deg + 1) * (sh_deg + 1);
+  const int K = pob::K_of(sh_deg);
   const int G = samples_per_cell >= pob::PT ? 1 : pob::PT / samples_per_cell;
   const long long n_blk = (n_cells + cells_per_block - 1) / cells_per_block;
   const long long ctas = n_blk * ((cells_per_block + G - 1) / G);

@@ -139,10 +139,11 @@ def _compiled_fwd():
     return {(int(n), o, s == "true") for n, o, s in found}
 
 
-def test_every_instantiation_is_reached():
+def test_every_instantiation_is_reached_by_an_entry_point():
     """the forward <NSPLIT, OUTM, SAVE, ACT> and data-gradient <NSPLIT, ACT> instantiations compiled in mlp_fwd.cu /
     mlp_bwd.cu, against the entry table above: every one but the recorded unreachable ones is launched by the rows of
-    this file or by the projection's point stage; the table matches the sources' out_mode choices"""
+    this file or by the projection's point stage; the table matches the sources' out_mode choices (the training
+    forward is the one saving launch of forward_levels, the projection's the only other one and relu only)"""
     fwd = _compiled_fwd()
     assert len(fwd) == 11, sorted(fwd)
     bwd_src = open(os.path.join(ROOT, "plenoctree_b200", "csrc", "mlp_bwd.cu")).read()
@@ -153,12 +154,15 @@ def test_every_instantiation_is_reached():
     assert capi.count("p.out_mode = raw_rgb_dev ? pob::OUT_RAW : pob::OUT_SIGMA;") == 2     # points_raw, grid
     assert "p.out_mode = pob::OUT_RGBS;" in capi and "p.out_mode = pob::OUT_CELL_MEAN;" in capi
     pipe = open(os.path.join(ROOT, "plenoctree_b200", "csrc", "pipeline.cu")).read()
-    assert "p.out_mode = OUT_RGBS;" in pipe and "p.save_h = C.H;" in pipe
+    fwd_levels = pipe[pipe.index("int forward_levels("):pipe.index("__global__ void pack_outputs_kernel")]
+    assert "p.out_mode = OUT_RGBS;" in fwd_levels and "p.save_h = L.H;" in fwd_levels
+    assert fwd_levels.count("launch_mlp_fwd(") == 1 and pipe.count("launch_mlp_fwd(") == 1
     proj = open(os.path.join(ROOT, "plenoctree_b200", "csrc", "projection.cu")).read()
     body = proj[proj.index("int pob_sh_proj_points("):proj.index("int pob_sh_proj_directions(")]
-    assert "if (net.net_act != pob::NET_RELU) return pob_fail(" in body
+    assert "if (p.net_act != pob::NET_RELU) return pob_fail(" in body
     assert "p.out_mode = pob::OUT_SIGMA;" in body and "p.save_h = base + ws.h;" in body
-    assert "pob::launch_mlp_fwd(p, 1, sms," in body
+    assert "pob::launch_mlp_fwd(p, POB_PREC_FP16, sms," in body
+    assert "#define POB_PREC_FP16 1\n" in open(os.path.join(ROOT, "include", "plenoctree_b200.h")).read()
     assert "launch_mlp_fwd" not in proj.replace(body, "")
     acts = {(0 if r[0] == "fp16" else 1, r[1]) for r in MATRIX}
     reached_fwd, reached_bwd = set(), set()
