@@ -529,6 +529,55 @@ int pob_sh_proj_cells(int64_t n_cells, int samples_per_cell, int cells_per_block
                       const float* sigma_dev, int n_dirs, int sh_deg, const float* t_dev, const float* basis_dev,
                       const float* w11_dev, const float* b11_dev, float* out_dev, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Vanilla NeRF (use_viewdirs, sh_deg -1) inference: NerfModel.__call__ and eval_points_raw with the view branch
+ *   (nerf_sh/nerf/models.py:143-214,216-348, model_utils.py:30-94).  Per MLP the branch is split as in the SH
+ *   projection above: a_p = h7 (W9 W10_b) comes out of the tensor-core forward as heads columns 8..135 (column 0 is
+ *   raw sigma, 1..7 are zero), t_r = W10_e posenc(viewdir_r, 0, deg_view, legacy_order) + c per ray (or point) with
+ *   c = b9 W10_b + b10, and raw_rgb = W11 act(a_p + t_r) + b11, act = the trunk activation (pob_posenc
+ *   net_activation), all in fp32 inside the forward's epilogue.  fp16 only; training is not covered.
+ * ------------------------------------------------------------------------------------------- */
+/* Folded flat parameters of one MLP: Dense_0..Dense_8 in the order of pob_pack_weights_pe (kernel [in,out], bias),
+ * then the folded head W9 W10_b [256, 128] (no bias).  The forward rounds it to fp16: a caller that forms it in fp64
+ * and rounds it to fp16 itself passes values the packing keeps exactly. */
+int64_t pob_vanilla_param_count(const pob_posenc* posenc);
+int64_t pob_vanilla_packed_bytes(void);
+int pob_pack_vanilla(const float* flat_dev, const pob_posenc* posenc, void* packed_dev, void* stream);
+
+/* The view branch of both MLPs (index 0 coarse, 1 fine), device fp32 arrays: w10e [3 + 6 deg_view, 128] (Dense_10
+ * kernel rows [256, 256 + 3 + 6 deg_view)), c [128] = b9 W10_b + b10, w11 [128, 3], b11 [3].  The viewdir encoder
+ * takes legacy_order from the config's pob_posenc. */
+typedef struct pob_view_mlp {
+  const float* w10e_dev;
+  const float* c_dev;
+  const float* w11_dev;
+  const float* b11_dev;
+} pob_view_mlp;
+typedef struct pob_view_branch {
+  int deg_view; /* 0..32 */
+  pob_view_mlp mlp[2];
+} pob_view_branch;
+
+/* pob_workspace_bytes(cfg, 0) plus the two levels' per-ray tables; -1 on a refused config */
+int64_t pob_vanilla_workspace_bytes(const pob_render_config* cfg);
+/* pob_render_rays for vanilla blobs (pob_pack_vanilla): the same arguments and outputs; cfg->sh_deg must be -1,
+ * precision POB_PREC_FP16; workspace_dev holds pob_vanilla_workspace_bytes(cfg) bytes and is 8-byte aligned (the
+ * per-ray tables inside it are read in float2 pairs; cudaMalloc's 256-byte alignment satisfies both). */
+int pob_render_rays_vanilla(const pob_render_config* cfg, const pob_view_branch* view, const void* packed_coarse_dev,
+                            const void* packed_fine_dev, const float* origins_dev, const float* directions_dev,
+                            const float* viewdirs_dev, int n_rays, const float* z_base_dev, const float* t_rand_dev,
+                            const float* u_dev, int u_per_ray, const float* z_fine_dev, float* out_coarse_dev,
+                            float* out_fine_dev, void* workspace_dev, int precision, void* stream);
+/* MLP `mlp` (0 / 1 of view) on m points with one view direction each.  With out_rgbs_dev NULL, eval_points_raw:
+ * raw_rgb_dev [m, 3] and raw_sigma_dev [m]; otherwise eval_points: out_rgbs_dev [m, 4] = (sigmoid(raw_rgb),
+ * sigma_activation (POB_SIGMA_*) of raw sigma) and the raw pointers are ignored.  table_dev: m * 128 floats of scratch
+ * (the per-point t), 8-byte aligned (the forward's epilogue reads it in float2 pairs); 512 bytes per point, so a
+ * caller evaluates large point sets in chunks (VanillaNerfModel.eval_points_raw: 2^20 points per call). */
+int pob_eval_points_vanilla(const void* packed_dev, const pob_posenc* posenc, const pob_view_branch* view, int mlp,
+                            const float* points_dev, const float* viewdirs_dev, int64_t m, float* table_dev,
+                            float* raw_rgb_dev, float* raw_sigma_dev, float* out_rgbs_dev, int sigma_activation,
+                            void* stream);
+
 #ifdef __cplusplus
 }
 #endif

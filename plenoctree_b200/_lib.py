@@ -90,6 +90,13 @@ SIGNATURES = {
     "pob_sh_proj_points": (_i, [_vp, _vp, _fp, _i64, _fp, _fp, _vp, _fp, _fp, _vp]),
     "pob_sh_proj_directions": (_i, [_c.c_uint64, _i64, _i, _i, _i, _i, _i, _fp, _fp, _fp, _fp, _vp]),
     "pob_sh_proj_cells": (_i, [_i64, _i, _i, _fp, _fp, _i, _i, _fp, _fp, _fp, _fp, _fp, _vp]),
+    "pob_vanilla_param_count": (_i64, [_vp]),
+    "pob_vanilla_packed_bytes": (_i64, []),
+    "pob_pack_vanilla": (_i, [_fp, _vp, _vp, _vp]),
+    "pob_vanilla_workspace_bytes": (_i64, [_vp]),
+    "pob_render_rays_vanilla": (_i, [_vp, _vp, _vp, _vp, _fp, _fp, _fp, _i, _fp, _fp, _fp, _i, _fp, _fp, _fp, _vp, _i,
+                                     _vp]),
+    "pob_eval_points_vanilla": (_i, [_vp, _vp, _vp, _i, _fp, _fp, _i64, _fp, _fp, _fp, _fp, _i, _vp]),
 }
 
 
@@ -120,6 +127,16 @@ class RenderConfig(_c.Structure):
     _fields_ = [("sh_deg", _i), ("num_coarse_samples", _i), ("num_fine_samples", _i), ("white_bkgd", _i),
                 ("max_rays", _i), ("sparsity_npoints", _i), ("sigma_noise_coarse_dev", _vp),
                 ("sigma_noise_fine_dev", _vp), ("sigma_activation", _i), ("posenc", _vp)]
+
+
+class ViewMlp(_c.Structure):
+    """pob_view_mlp: the view branch of one vanilla MLP (device fp32 arrays)."""
+    _fields_ = [("w10e_dev", _vp), ("c_dev", _vp), ("w11_dev", _vp), ("b11_dev", _vp)]
+
+
+class ViewBranch(_c.Structure):
+    """pob_view_branch: deg_view and the view branch of MLP_0 (coarse) and MLP_1 (fine)."""
+    _fields_ = [("deg_view", _i), ("mlp", ViewMlp * 2)]
 
 
 class TrainHParams(_c.Structure):

@@ -115,7 +115,33 @@ pob::MlpPacked packed_view(const void* blob, int K) {
   return w;
 }
 
+// packed blob of one vanilla MLP: its forward image (fp16) only
+size_t vanilla_blob_bytes() { return (pob::fwd_image_bytes(pob::VANILLA_NH) + 1023) / 1024 * 1024; }
+
 }  // namespace
+
+int pob_check_view(const char* where, const pob_view_branch* view, int n_mlps) {
+  if (!view) return pob_fail(where, "view branch descriptor is NULL");
+  if (view->deg_view < 0 || view->deg_view > pob::MAX_DEG_VIEW)
+    return pob_fail(where, "deg_view must be in [0, 32] (the posenc scale 2^(deg_view - 1) of a unit direction)");
+  for (int i = 0; i < n_mlps; ++i) {
+    const pob_view_mlp& v = view->mlp[i];
+    if (!v.w10e_dev || !v.c_dev || !v.w11_dev || !v.b11_dev) return pob_fail(where, "NULL view branch array");
+  }
+  return 0;
+}
+pob::FwdParams pob_vanilla_params(const void* packed, pob::NetDesc net, const pob_view_branch& view, int mlp,
+                                  const float* t) {
+  pob::FwdParams p = pob_base_params(packed, -1, net);
+  p.NH = pob::VANILLA_NH;
+  p.w.w_lo = nullptr;    // the vanilla blob holds the fp16 forward image only
+  p.w.wt_hi = nullptr;
+  p.out_mode = pob::OUT_VANILLA;
+  p.view_t = t;
+  p.view_w11 = view.mlp[mlp].w11_dev;
+  p.view_b11 = view.mlp[mlp].b11_dev;
+  return p;
+}
 
 int pob_sms_or_fail(const char* where) {
   const int n = sm_count();
@@ -397,6 +423,58 @@ int pob_eval_points_raw_host(const void* packed_dev, int sh_deg, const float* po
                              int precision) {
   return pob_eval_points_raw_host_pe(packed_dev, sh_deg, nullptr, points_host, m, raw_rgb_host, raw_sigma_host,
                                      precision);
+}
+
+int64_t pob_vanilla_param_count(const pob_posenc* posenc) {
+  pob::NetDesc net;
+  if (pob_check_posenc("pob_vanilla_param_count", posenc, net)) return -1;
+  return pob::vanilla_flat_layout(pob::posenc_width(net.pe)).total;
+}
+int64_t pob_vanilla_packed_bytes(void) { return int64_t(vanilla_blob_bytes()); }
+
+int pob_pack_vanilla(const float* flat_dev, const pob_posenc* posenc, void* packed_dev, void* stream) {
+  const char* where = "pob_pack_vanilla";
+  pob::NetDesc net;
+  if (int e = pob_check_posenc(where, posenc, net)) return e;
+  if (!flat_dev || !packed_dev) return pob_fail(where, "NULL pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  POB_LAUNCH(where, POB_PH_OPTIM, st,
+             pob::launch_pack_vanilla(flat_dev, pob::posenc_width(net.pe), static_cast<uint8_t*>(packed_dev), st));
+  return 0;
+}
+
+int pob_eval_points_vanilla(const void* packed_dev, const pob_posenc* posenc, const pob_view_branch* view, int mlp,
+                            const float* points_dev, const float* viewdirs_dev, int64_t m, float* table_dev,
+                            float* raw_rgb_dev, float* raw_sigma_dev, float* out_rgbs_dev, int sigma_activation,
+                            void* stream) {
+  const char* where = "pob_eval_points_vanilla";
+  pob::NetDesc net;
+  if (!packed_dev) return pob_fail(where, "packed weights pointer is NULL");
+  if (int e = pob_check_posenc(where, posenc, net)) return e;
+  if (mlp != 0 && mlp != 1) return pob_fail(where, "mlp must be 0 or 1");
+  if (int e = pob_check_view(where, view, mlp + 1)) return e;
+  if (int e = pob_check_sigma_activation(where, sigma_activation)) return e;
+  if (m < 0) return pob_fail(where, "negative point count");
+  if (!points_dev || !viewdirs_dev || !table_dev || (!out_rgbs_dev && (!raw_rgb_dev || !raw_sigma_dev)))
+    return pob_fail(where, "NULL pointer");
+  if (reinterpret_cast<uintptr_t>(table_dev) & 7) return pob_fail(where, "table_dev must be 8-byte aligned");
+  const int sms = pob_sms_or_fail(where);
+  if (!sms) return 1;
+  if (m == 0) return 0;
+  pob::FwdParams p = pob_vanilla_params(packed_dev, net, *view, mlp, table_dev);
+  p.src_mode = pob::SRC_POINTS;
+  p.M = m;
+  p.points = points_dev;
+  p.out_rgbs = reinterpret_cast<float4*>(out_rgbs_dev);
+  p.out_rgb = raw_rgb_dev;
+  p.out_sigma = raw_sigma_dev;
+  p.sigma_act = sigma_activation;
+  cudaStream_t st = (cudaStream_t)stream;
+  POB_LAUNCH(where, POB_PH_FWD, st,
+             pob::launch_view_table(viewdirs_dev, m, view->deg_view, net.pe.legacy, view->mlp[mlp].w10e_dev,
+                                    view->mlp[mlp].c_dev, table_dev, st));
+  POB_LAUNCH(where, POB_PH_FWD, st, pob::launch_mlp_fwd_vanilla(p, sms, st));
+  return 0;
 }
 
 int pob_sample_coarse(const float* z_base_dev, const float* t_rand_dev, int n_rays, int n_samples,

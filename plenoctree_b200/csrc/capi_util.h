@@ -32,6 +32,13 @@ static inline int pob_eval_setup(const char* where, const void* packed, int sh_d
   return sms;
 }
 
+// vanilla NeRF (pob_view_branch): deg_view in [0, 32] and the four arrays of MLPs 0 .. n_mlps - 1, else pob_fail
+struct pob_view_branch;
+int pob_check_view(const char* where, const pob_view_branch* view, int n_mlps);
+// the FwdParams of one vanilla MLP (OUT_VANILLA, heads VANILLA_NH wide) with view-branch MLP `mlp` and table `t`
+pob::FwdParams pob_vanilla_params(const void* packed, pob::NetDesc net, const pob_view_branch& view, int mlp,
+                                  const float* t);
+
 #define POB_CUDA(where, call)                               \
   do {                                                      \
     cudaError_t _e = (call);                                \

@@ -16,7 +16,8 @@ struct MlpPacked {
 };
 
 enum SrcMode : int { SRC_POINTS = 0, SRC_RAYS = 1, SRC_GRID = 2 };
-enum OutMode : int { OUT_RAW = 0, OUT_SIGMA = 1, OUT_RGBS = 2, OUT_CELL_MEAN = 3 };
+// OUT_VANILLA: the vanilla NeRF view branch behind the VANILLA_NH-wide heads (fp16, inference only)
+enum OutMode : int { OUT_RAW = 0, OUT_SIGMA = 1, OUT_RGBS = 2, OUT_CELL_MEAN = 3, OUT_VANILLA = 4 };
 // density activation of OUT_RGBS (the values of POB_SIGMA_* in the C ABI)
 enum SigmaAct : int { SIGMA_RELU = 0, SIGMA_SOFTPLUS = 1 };
 
@@ -116,6 +117,12 @@ struct FwdParams {
   uint8_t* save_e_lo;          // [ntile][16 KB]
   // ---- model, continued ----
   int net_act;                 // NetAct of Dense_0..Dense_7
+  // ---- OUT_VANILLA: raw_rgb = W11 act(a_p + t_r) + b11 with a_p = heads columns VIEW_COL0.. (act = net_act) ----
+  const float* view_t;         // [rows][VIEW_H] fp32: row s / n_per_ray (SRC_RAYS) or s (SRC_POINTS)
+  const float* view_w11;       // [VIEW_H][3] (Dense_11 kernel)
+  const float* view_b11;       // [3]
+  // out_rgbs set: (sigmoid(raw_rgb), density activation of raw sigma (+ noise)); else out_rgb [M,3] and out_sigma [M]
+  // take raw_rgb and raw sigma
 };
 
 // sh_deg -1 (3 raw rgb channels) to 4, and the coefficients per channel of a degree: K = 1 for -1, else (sh_deg+1)^2
@@ -131,6 +138,18 @@ inline size_t bwd_image_bytes(int NH) { return size_t(bwd_slots(NH)) * WSLOT_BYT
 // precision: 1 = single fp16 pass (10-bit mantissa operands, fp32 accumulate, reduced SFU sine),
 //            3 = error-compensated 3-pass split (hi*hi + lo*hi + hi*lo, libdevice sinf)
 cudaError_t launch_mlp_fwd(const FwdParams& p, int nsplit, int num_sms, cudaStream_t stream);
+// the vanilla view-branch forward (out_mode OUT_VANILLA, FwdParams view_*): fp16 inference only
+cudaError_t launch_mlp_fwd_vanilla(const FwdParams& p, int num_sms, cudaStream_t stream);
+
+// forward weight image of a vanilla NeRF MLP (heads VANILLA_NH wide) from its folded flat parameters
+// (vanilla_flat_layout); only the fp16 "hi" image: the vanilla forward is fp16 inference
+cudaError_t launch_pack_vanilla(const float* flat, int W, uint8_t* w_hi, cudaStream_t stream);
+
+// t[r][j] = sum_e W10_e[e][j] posenc(viewdirs[r], 0, deg_view, legacy)[e] + c[j] of n view directions (projection.cu;
+// the same posenc and matvec as the SH projection's direction tables)
+cudaError_t launch_view_table(const float* viewdirs, long long n, int deg_view, int legacy, const float* w10e,
+                              const float* c, float* t, cudaStream_t stream);
+constexpr int MAX_DEG_VIEW = 32;
 
 // flat fp32 parameters of one MLP in reference order (Dense_0..Dense_9: kernel [in,out] then
 // bias; flat_layout(K, W), W = posenc_width) -> packed images.  The images do not depend on W: rows [W, 63) of the
@@ -310,6 +329,15 @@ inline FlatLayout flat_layout(int K, int W) {
     off += out;
   }
   L.total = off;
+  return L;
+}
+// folded flat parameters of a vanilla NeRF MLP: Dense_0..Dense_8 as flat_layout(1, W), then the folded head
+// W9 W10_b [256, VIEW_H] (no bias: b9 W10_b + b10 rides in the view table)
+inline FlatLayout vanilla_flat_layout(int W) {
+  FlatLayout L = flat_layout(1, W);
+  L.out_dim[9] = VIEW_H;
+  L.b_off[9] = L.w_off[9] + WIDTH * VIEW_H;
+  L.total = L.b_off[9];
   return L;
 }
 

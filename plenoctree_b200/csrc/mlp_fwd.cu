@@ -193,6 +193,7 @@ __device__ __forceinline__ float* stage_row(uint8_t* a_tile, int wg, int r) {
 template <int NSPLIT, int OUTM, bool SAVE, int ACT>
 __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_constant__ FwdParams p) {
   constexpr bool MASKS = SAVE && ACT == NET_RELU;
+  constexpr int HN = OUTM == OUT_VANILLA ? VANILLA_NH : HEADS_N;   // heads MMA width
   extern __shared__ __align__(1024) uint8_t smem[];
   constexpr bool PRECISE = (NSPLIT == 3);
   using SM = Smem<NSPLIT, SAVE>;
@@ -253,7 +254,7 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
   constexpr uint64_t W_DESC = make_sdesc_hi(16, 512, LAYOUT_SW64);
   RingPos pos;
   float acc[128];
-  float hacc[HEADS_N / 2];
+  float hacc[HN / 2];
   uint32_t afr[64];        // fp16: the previous layer's ReLU output as the register A operand (acc_to_afrag)
   long long it = blockIdx.x;
 
@@ -302,7 +303,8 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
           const uint32_t* a = afr + 8 * j + 4 * k;
           const uint64_t bd = sdesc(W_DESC, b + 32u * k);
           const uint32_t sd = (j != 0 || k != 0) ? 1u : 0u;
-          if constexpr (HEADS) wgmma_m64n80_rs(d, a[0], a[1], a[2], a[3], bd, sd);
+          if constexpr (HEADS && HN == VANILLA_NH) wgmma_m64n136_rs(d, a[0], a[1], a[2], a[3], bd, sd);
+          else if constexpr (HEADS) wgmma_m64n80_rs(d, a[0], a[1], a[2], a[3], bd, sd);
           else wgmma_m64n256_rs(d, a[0], a[1], a[2], a[3], bd, sd);
         }
       } else {
@@ -313,7 +315,8 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
         for (int k = 0; k < 2; ++k) {
           if (k == 0 && bias_slot) continue;
           const uint32_t ko = uint32_t(k) * 32u;
-          if constexpr (HEADS) wgmma_m64n80<0, 0>(d, sdesc(A_DESC, a + ko), sdesc(W_DESC, b + ko), 1u);
+          if constexpr (HEADS && HN == VANILLA_NH) wgmma_m64n136<0, 0>(d, sdesc(A_DESC, a + ko), sdesc(W_DESC, b + ko), 1u);
+          else if constexpr (HEADS) wgmma_m64n80<0, 0>(d, sdesc(A_DESC, a + ko), sdesc(W_DESC, b + ko), 1u);
           else wgmma_m64n256<0, 0>(d, sdesc(A_DESC, a + ko), sdesc(W_DESC, b + ko), 1u);
         }
       }
@@ -414,6 +417,71 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
     if (NSPLIT == 1) __syncwarp();
   };
 
+  // vanilla view branch, in registers: the quad of lanes holding rows fr and fr + 8 holds their 128 a_p columns, 32
+  // per lane (8-column groups j = 1..16).  Each lane forms its share of W11 act(a_p + t_r) in a fixed column order, the
+  // quad sums the shares with two butterfly shuffles (every lane ends with the same sums), and lane 0 of the quad writes
+  // row fr, lane 1 row fr + 8.  No staging, no a_p in memory.
+  auto vanilla_epilogue = [&]() {
+    const int q = int(lane & 3);
+    const long long row0 = it * TILE_M + 64 * wg + fr;
+    const float* tr[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      long long s = row0 + 8 * h;
+      if (s >= p.M) s = p.M - 1;
+      tr[h] = p.view_t + (p.src_mode == SRC_RAYS ? s / p.n_per_ray : s) * VIEW_H;
+    }
+    float pre[2][3];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {   // one row at a time: the softplus condition layer then fits without spilling
+      pre[h][0] = pre[h][1] = pre[h][2] = 0.f;
+#pragma unroll
+      for (int j = VIEW_COL0 / 8; j < HN / 8; ++j) {
+        const int col = 8 * j - VIEW_COL0 + fc;   // this lane's column pair of 8-column group j
+        const float2 t2 = __ldg(reinterpret_cast<const float2*>(tr[h] + col));
+        const float z0 = net_act_f32<ACT>(hacc[4 * j + 2 * h] + t2.x);
+        const float z1 = net_act_f32<ACT>(hacc[4 * j + 2 * h + 1] + t2.y);
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+          const float w0 = __ldg(p.view_w11 + col * 3 + c), w1 = __ldg(p.view_w11 + (col + 1) * 3 + c);
+          pre[h][c] = fmaf(w1, z1, fmaf(w0, z0, pre[h][c]));
+        }
+      }
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        pre[h][c] += __shfl_xor_sync(0xffffffffu, pre[h][c], 1);
+        pre[h][c] += __shfl_xor_sync(0xffffffffu, pre[h][c], 2);
+      }
+    }
+    // raw sigma of rows fr, fr + 8: column 0, held by lane 0 of the quad
+    const float sg0 = __shfl_sync(0xffffffffu, hacc[0], int(lane) & ~3);
+    const float sg1 = __shfl_sync(0xffffffffu, hacc[2], int(lane) & ~3);
+    if (q < 2) {
+      const long long s = row0 + 8 * q;
+      if (s < p.M) {
+        const float r0 = (q ? pre[1][0] : pre[0][0]) + __ldg(p.view_b11);
+        const float r1 = (q ? pre[1][1] : pre[0][1]) + __ldg(p.view_b11 + 1);
+        const float r2 = (q ? pre[1][2] : pre[0][2]) + __ldg(p.view_b11 + 2);
+        float sigma_raw = q ? sg1 : sg0;
+        if (p.out_rgbs) {
+          if (p.sigma_noise != nullptr) sigma_raw += __ldg(p.sigma_noise + s);   // add_gaussian_noise
+          float4 o;
+          o.x = 1.f / (1.f + expf(-r0));
+          o.y = 1.f / (1.f + expf(-r1));
+          o.z = 1.f / (1.f + expf(-r2));
+          o.w = p.sigma_act == SIGMA_SOFTPLUS ? softplus_f32(sigma_raw) : fmaxf(sigma_raw, 0.f);
+          p.out_rgbs[s] = o;
+        } else {
+          p.out_rgb[3 * s] = r0;
+          p.out_rgb[3 * s + 1] = r1;
+          p.out_rgb[3 * s + 2] = r2;
+          p.out_sigma[s] = sigma_raw;
+        }
+      }
+    }
+    __syncwarp();
+  };
+
   for (; it < num_tiles; it += gridDim.x) {
     // ---- positional encoding of the warpgroup's 64 rows (two threads per row, four 16-byte units each) ----
     {
@@ -464,7 +532,8 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
         act_to_afrag<ACT>(acc, afr);
       }
       chain_layer(hacc, NUM_TRUNK);
-      heads_epilogue();
+      if constexpr (OUTM == OUT_VANILLA) vanilla_epilogue();
+      else heads_epilogue();
     } else {
       // ---- x3: every operand from shared memory; the epilogue rewrites the warpgroup's rows of the A tiles ----
       for (int l = 0; l <= NUM_TRUNK; ++l) {
@@ -557,6 +626,30 @@ __global__ void __launch_bounds__(FWD_THREADS, 1) mlp_fwd_kernel(const __grid_co
         heads_epilogue();
       }
     }
+  }
+}
+
+// the vanilla view-branch forward (OUT_VANILLA): fp16, no training saves, no free points behind the ray samples
+cudaError_t launch_mlp_fwd_vanilla(const FwdParams& p, int num_sms, cudaStream_t stream) {
+  if (p.M <= 0) return cudaSuccess;
+  if (p.out_mode != OUT_VANILLA || p.NH != VANILLA_NH || p.save_h || !p.view_t || !p.view_w11 || !p.view_b11 ||
+      (!p.out_rgbs && (!p.out_rgb || !p.out_sigma)) || (p.src_mode == SRC_RAYS && p.M != p.M_rays) ||
+      (p.sigma_act != SIGMA_RELU && p.sigma_act != SIGMA_SOFTPLUS) || !posenc_valid(p.pe))
+    return cudaErrorInvalidValue;
+  const long long tiles = (p.M + TILE_M - 1) / TILE_M;
+  const int grid = int(tiles < num_sms ? tiles : num_sms);
+  auto launch = [&](auto kernel) -> cudaError_t {
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SM_TOTAL);
+    if (e != cudaSuccess) return e;
+    kernel<<<grid, FWD_THREADS, SM_TOTAL, stream>>>(p);
+    return cudaGetLastError();
+  };
+  switch (p.net_act) {
+    case NET_RELU: return launch(mlp_fwd_kernel<1, OUT_VANILLA, false, NET_RELU>);
+    case NET_ELU: return launch(mlp_fwd_kernel<1, OUT_VANILLA, false, NET_ELU>);
+    case NET_SOFTPLUS: return launch(mlp_fwd_kernel<1, OUT_VANILLA, false, NET_SOFTPLUS>);
+    case NET_TANH: return launch(mlp_fwd_kernel<1, OUT_VANILLA, false, NET_TANH>);
+    default: return cudaErrorInvalidValue;
   }
 }
 

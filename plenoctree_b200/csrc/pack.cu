@@ -47,12 +47,21 @@ __device__ __forceinline__ float heads_weight(const PackArgs& a, int i, int n) {
   return heads_param(a, a.L.w_off[8] + i, a.L.w_off[9] + i * (3 * a.K), n);
 }
 
+// vanilla heads (VANILLA = true, NH = VANILLA_NH): W[in=i -> packed column n] of sigma (column 0) and the folded head
+// (columns VIEW_COL0..; vanilla_flat_layout), zero in between; the folded head has no bias
+__device__ __forceinline__ float vanilla_heads_weight(const PackArgs& a, int i, int n) {
+  if (n == 0) return a.flat[a.L.w_off[8] + i];
+  return n < VIEW_COL0 ? 0.f : a.flat[a.L.w_off[9] + i * VIEW_H + (n - VIEW_COL0)];
+}
+
+// VANILLA: the forward image of a vanilla MLP only (no dgrad slots)
+template <bool VANILLA>
 __global__ void pack_weights_kernel(const __grid_constant__ PackArgs a) {
   const int NH = a.NH;
   const long long n_fwd_trunk = (long long)FWD_TRUNK_SLOTS * 256 * 32;
   const long long n_fwd_heads = (long long)FWD_HEAD_SLOTS * NH * 32;
   const int hs = bwd_head_slots(NH);
-  const long long n_bwd = (long long)bwd_slots(NH) * 256 * 32;
+  const long long n_bwd = VANILLA ? 0 : (long long)bwd_slots(NH) * 256 * 32;
   const long long total = n_fwd_trunk + n_fwd_heads + n_bwd;
   const long long first = a.dgrad_only ? n_fwd_trunk + n_fwd_heads : 0;
   for (long long t = first + blockIdx.x * (long long)blockDim.x + threadIdx.x; t < total;
@@ -84,8 +93,14 @@ __global__ void pack_weights_kernel(const __grid_constant__ PackArgs a) {
       const int j = int(u / (NH * 32));
       const int n = int(u / 32) % NH, kk = int(u % 32);
       float v = 0.f;
-      if (j < 8) v = heads_weight(a, 32 * j + kk, n);
-      else if (kk == 31) v = heads_param(a, a.L.b_off[8], a.L.b_off[9], n);   // bias slot
+      if (VANILLA) {
+        if (j < 8) v = vanilla_heads_weight(a, 32 * j + kk, n);
+        else if (kk == 31 && n == 0) v = a.flat[a.L.b_off[8]];                 // bias slot: sigma only
+      } else if (j < 8) {
+        v = heads_weight(a, 32 * j + kk, n);
+      } else if (kk == 31) {
+        v = heads_param(a, a.L.b_off[8], a.L.b_off[9], n);   // bias slot
+      }
       put_hilo(a.w_hi, a.w_lo, size_t(FWD_TRUNK_SLOTS) * WSLOT_BYTES + size_t(j) * NH * 64 + w_slot_offset(n, kk), v);
     } else {
       const long long u = t - n_fwd_trunk - n_fwd_heads;
@@ -118,7 +133,7 @@ cudaError_t launch_pack(const float* flat, int K, int W, uint8_t* w_hi, uint8_t*
   a.wt_hi = wt_hi;
   a.wt_lo = wt_lo;
   a.dgrad_only = dgrad_only;
-  pack_weights_kernel<<<592, 256, 0, stream>>>(a);
+  pack_weights_kernel<false><<<592, 256, 0, stream>>>(a);
   return cudaGetLastError();
 }
 
@@ -127,6 +142,18 @@ cudaError_t launch_pack(const float* flat, int K, int W, uint8_t* w_hi, uint8_t*
 cudaError_t launch_pack_weights(const float* flat, int K, int W, uint8_t* w_hi, uint8_t* w_lo,
                                 uint8_t* wt_hi, cudaStream_t stream) {
   return launch_pack(flat, K, W, w_hi, w_lo, wt_hi, nullptr, 0, stream);
+}
+
+cudaError_t launch_pack_vanilla(const float* flat, int W, uint8_t* w_hi, cudaStream_t stream) {
+  PackArgs a = {};
+  a.flat = flat;
+  a.L = vanilla_flat_layout(W);
+  a.K = 1;
+  a.W = W;
+  a.NH = VANILLA_NH;
+  a.w_hi = w_hi;
+  pack_weights_kernel<true><<<592, 256, 0, stream>>>(a);
+  return cudaGetLastError();
 }
 
 cudaError_t launch_pack_wt_lo(const float* flat, int K, int W, uint8_t* wt_lo, cudaStream_t stream) {

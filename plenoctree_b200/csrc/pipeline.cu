@@ -1,5 +1,6 @@
 // pipeline.cu — host-side sequencing of the kernels into the two reference-level operations:
 //   pob_render_rays    = NerfModel.__call__            (nerf_sh/nerf/models.py:216-348)
+//   pob_render_rays_vanilla: the same with use_viewdirs (the view branch in the forward's epilogue)
 //   pob_loss_and_grad  = value_and_grad(loss_fn)       (nerf_sh/train.py:66-116)
 //   pob_adam_update    = optimizer.apply_gradient      (nerf_sh/train.py:119) + operand re-pack
 // Everything is enqueued on the caller's stream; nothing synchronises with the host.
@@ -34,6 +35,7 @@ struct Level {
   uint8_t *H, *E, *DZ, *DO;
   uint32_t* mask;
   uint8_t *H_lo, *E_lo, *DZ_lo, *DO_lo;   // x3 training: residual images of H, E, DZ, DO
+  float* view_t;      // vanilla rendering: [R, VIEW_H] per-ray view table of the level's MLP
 };
 
 struct Workspace {
@@ -66,7 +68,8 @@ constexpr int DGRAD_SMS_OF_132 = 56;
 constexpr int DGRAD_SMS_OF_132_NH80 = 60;
 
 // deterministic carve of the caller-provided workspace (x3: the training workspace of the fp16x3 step)
-Workspace carve(const pob_render_config& c, int training, uint8_t* base, bool x3 = false) {
+// (vanilla: the render workspace plus the per-ray view tables, behind everything else)
+Workspace carve(const pob_render_config& c, int training, uint8_t* base, bool x3 = false, bool vanilla = false) {
   Workspace w;
   memset(&w, 0, sizeof(w));
   size_t off = 0;
@@ -118,6 +121,9 @@ Workspace carve(const pob_render_config& c, int training, uint8_t* base, bool x3
       for (int q = 0; q < 2; ++q) w.partials_x3[i][q] = (float*)take(sizeof(float) * WG_MAX_CTAS * WG_PARTIAL_FLOATS);
     for (int i = 0; i < 2; ++i) w.wt_lo[i] = take(bwd_image_bytes(heads_width(K_of(c.sh_deg))));
   }
+  if (vanilla)
+    for (int l = 0; l < 2; ++l)
+      if (w.lv[l].N > 0) w.lv[l].view_t = (float*)take(sizeof(float) * VIEW_H * size_t(R));
   w.total = off;
   return w;
 }
@@ -137,11 +143,13 @@ int check_cfg(const char* where, const pob_render_config* c, NetDesc& net) {
 }
 
 // forward of every level; fills comp/disp/acc (and rgbs, weights, z) of the workspace levels.  The depths of a level
-// are the coarse draw, the caller's z_fine or the resampling of the coarse weights.
+// are the coarse draw, the caller's z_fine or the resampling of the coarse weights.  With `view` the packed blobs are
+// vanilla MLPs: each level first tabulates its MLP's view branch for the rays, then runs the vanilla forward.
 int forward_levels(const char* where, const pob_render_config& c, NetDesc net, int sms, Workspace& w,
                    const void* const packed[2], const float* o, const float* d, const float* v, int R,
                    const float* z_base, const float* t_rand, const float* u, int u_per_ray, const float* z_fine,
-                   int precision, bool save, cudaStream_t st, const float* sp_points = nullptr, long long sp_n = 0) {
+                   int precision, bool save, cudaStream_t st, const float* sp_points = nullptr, long long sp_n = 0,
+                   const pob_view_branch* view = nullptr) {
   const float* const noise[2] = {c.sigma_noise_coarse_dev, c.sigma_noise_fine_dev};
   for (int l = 0; l < w.levels; ++l) {
     Level& L = w.lv[l];
@@ -153,7 +161,16 @@ int forward_levels(const char* where, const pob_render_config& c, NetDesc net, i
       POB_LAUNCH(where, POB_PH_RENDER, st,
                  launch_sample_pdf(w.lv[0].z, w.lv[0].weights, u, u_per_ray, R, c.num_coarse_samples,
                                    c.num_fine_samples, L.z, st));
-    FwdParams p = pob_base_params(packed[l], c.sh_deg, net);
+    FwdParams p;
+    if (view) {
+      POB_LAUNCH(where, POB_PH_FWD, st,
+                 launch_view_table(v, R, view->deg_view, net.pe.legacy, view->mlp[l].w10e_dev, view->mlp[l].c_dev,
+                                   L.view_t, st));
+      p = pob_vanilla_params(packed[l], net, *view, l, L.view_t);
+    } else {
+      p = pob_base_params(packed[l], c.sh_deg, net);
+      p.out_mode = OUT_RGBS;
+    }
     p.src_mode = SRC_RAYS;
     p.M = (long long)R * L.N;
     p.M_rays = p.M;
@@ -162,7 +179,6 @@ int forward_levels(const char* where, const pob_render_config& c, NetDesc net, i
     p.viewdirs = v;
     p.zvals = L.z;
     p.n_per_ray = L.N;
-    p.out_mode = OUT_RGBS;
     p.out_rgbs = L.rgbs;
     p.sigma_noise = noise[l];
     p.sigma_act = c.sigma_activation;
@@ -177,7 +193,8 @@ int forward_levels(const char* where, const pob_render_config& c, NetDesc net, i
       p.save_h_lo = L.H_lo;   // x3 only (null otherwise)
       p.save_e_lo = L.E_lo;
     }
-    POB_LAUNCH(where, POB_PH_FWD, st, launch_mlp_fwd(p, precision, sms, st));
+    POB_LAUNCH(where, POB_PH_FWD, st,
+               view ? launch_mlp_fwd_vanilla(p, sms, st) : launch_mlp_fwd(p, precision, sms, st));
     POB_LAUNCH(where, POB_PH_RENDER, st,
                launch_composite_fwd(L.rgbs, L.z, d, R, L.N, c.white_bkgd, L.comp, L.disp, L.acc, L.weights, st));
   }
@@ -218,6 +235,41 @@ int check_workspace_extent(const char* where, const void* ws, size_t bytes) {
   return 0;
 }
 
+// pob_render_rays and pob_render_rays_vanilla (view != NULL) past their own checks
+int render_rays(const char* where, const pob_render_config* cfg, const pob_view_branch* view, NetDesc net, int sms,
+                const void* packed_coarse_dev, const void* packed_fine_dev, const float* origins_dev,
+                const float* directions_dev, const float* viewdirs_dev, int n_rays, const float* z_base_dev,
+                const float* t_rand_dev, const float* u_dev, int u_per_ray, const float* z_fine_dev,
+                float* out_coarse_dev, float* out_fine_dev, void* workspace_dev, int precision, void* stream) {
+  if (n_rays < 0 || n_rays > cfg->max_rays) return pob_fail(where, "n_rays exceeds cfg->max_rays");
+  if (n_rays == 0) return 0;
+  if (!origins_dev || !directions_dev || !viewdirs_dev || !z_base_dev || !workspace_dev || !out_coarse_dev)
+    return pob_fail(where, "NULL pointer");
+  if (cfg->num_fine_samples > 0 && (!packed_fine_dev || (!u_dev && !z_fine_dev) || !out_fine_dev))
+    return pob_fail(where, "fine level needs packed_fine, u (or z_fine) and out_fine");
+  cudaStream_t st = (cudaStream_t)stream;
+  Workspace w = carve(*cfg, 0, (uint8_t*)workspace_dev, false, view != nullptr);
+  const void* const packed[2] = {packed_coarse_dev, packed_fine_dev};
+  if (int e = forward_levels(where, *cfg, net, sms, w, packed, origins_dev, directions_dev, viewdirs_dev, n_rays,
+                             z_base_dev, t_rand_dev, u_dev, u_per_ray, z_fine_dev, precision, false, st, nullptr, 0,
+                             view))
+    return e;
+  const unsigned grid = (n_rays + 255) / 256;
+  pob_count_launch(w.levels);
+  pack_outputs_kernel<<<grid, 256, 0, st>>>(w.lv[0].comp, w.lv[0].disp, w.lv[0].acc, n_rays, out_coarse_dev);
+  if (w.levels == 2)
+    pack_outputs_kernel<<<grid, 256, 0, st>>>(w.lv[1].comp, w.lv[1].disp, w.lv[1].acc, n_rays, out_fine_dev);
+  POB_CUDA(where, cudaGetLastError());
+  return 0;
+}
+
+// the config checks of the vanilla entry points: check_cfg, then sh_deg -1
+int check_vanilla_cfg(const char* where, const pob_render_config* cfg, NetDesc& net) {
+  if (int e = check_cfg(where, cfg, net)) return e;
+  if (cfg->sh_deg != -1) return pob_fail(where, "a vanilla NeRF has the plain-RGB head: cfg->sh_deg must be -1");
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -248,25 +300,34 @@ int pob_render_rays(const pob_render_config* cfg, const void* packed_coarse_dev,
   if (int e = check_cfg(where, cfg, net)) return e;
   const int sms = pob_check_common(where, packed_coarse_dev, cfg->sh_deg, precision);
   if (!sms) return 1;
-  if (n_rays < 0 || n_rays > cfg->max_rays) return pob_fail(where, "n_rays exceeds cfg->max_rays");
-  if (n_rays == 0) return 0;
-  if (!origins_dev || !directions_dev || !viewdirs_dev || !z_base_dev || !workspace_dev || !out_coarse_dev)
-    return pob_fail(where, "NULL pointer");
-  if (cfg->num_fine_samples > 0 && (!packed_fine_dev || (!u_dev && !z_fine_dev) || !out_fine_dev))
-    return pob_fail(where, "fine level needs packed_fine, u (or z_fine) and out_fine");
-  cudaStream_t st = (cudaStream_t)stream;
-  Workspace w = carve(*cfg, 0, (uint8_t*)workspace_dev);
-  const void* const packed[2] = {packed_coarse_dev, packed_fine_dev};
-  if (int e = forward_levels(where, *cfg, net, sms, w, packed, origins_dev, directions_dev, viewdirs_dev, n_rays,
-                             z_base_dev, t_rand_dev, u_dev, u_per_ray, z_fine_dev, precision, false, st))
-    return e;
-  const unsigned grid = (n_rays + 255) / 256;
-  pob_count_launch(w.levels);
-  pack_outputs_kernel<<<grid, 256, 0, st>>>(w.lv[0].comp, w.lv[0].disp, w.lv[0].acc, n_rays, out_coarse_dev);
-  if (w.levels == 2)
-    pack_outputs_kernel<<<grid, 256, 0, st>>>(w.lv[1].comp, w.lv[1].disp, w.lv[1].acc, n_rays, out_fine_dev);
-  POB_CUDA(where, cudaGetLastError());
-  return 0;
+  return render_rays(where, cfg, nullptr, net, sms, packed_coarse_dev, packed_fine_dev, origins_dev, directions_dev,
+                     viewdirs_dev, n_rays, z_base_dev, t_rand_dev, u_dev, u_per_ray, z_fine_dev, out_coarse_dev,
+                     out_fine_dev, workspace_dev, precision, stream);
+}
+
+int64_t pob_vanilla_workspace_bytes(const pob_render_config* cfg) {
+  NetDesc net;
+  if (check_vanilla_cfg("pob_vanilla_workspace_bytes", cfg, net)) return -1;
+  return (int64_t)carve(*cfg, 0, nullptr, false, true).total;
+}
+
+int pob_render_rays_vanilla(const pob_render_config* cfg, const pob_view_branch* view, const void* packed_coarse_dev,
+                            const void* packed_fine_dev, const float* origins_dev, const float* directions_dev,
+                            const float* viewdirs_dev, int n_rays, const float* z_base_dev, const float* t_rand_dev,
+                            const float* u_dev, int u_per_ray, const float* z_fine_dev, float* out_coarse_dev,
+                            float* out_fine_dev, void* workspace_dev, int precision, void* stream) {
+  const char* where = "pob_render_rays_vanilla";
+  NetDesc net;
+  if (int e = check_vanilla_cfg(where, cfg, net)) return e;
+  if (precision != POB_PREC_FP16) return pob_fail(where, "the vanilla forward is fp16: precision must be POB_PREC_FP16");
+  if (!packed_coarse_dev) return pob_fail(where, "packed weights pointer is NULL");
+  if (int e = pob_check_view(where, view, cfg->num_fine_samples > 0 ? 2 : 1)) return e;
+  if (reinterpret_cast<uintptr_t>(workspace_dev) & 7) return pob_fail(where, "workspace_dev must be 8-byte aligned");
+  const int sms = pob_sms_or_fail(where);
+  if (!sms) return 1;
+  return render_rays(where, cfg, view, net, sms, packed_coarse_dev, packed_fine_dev, origins_dev, directions_dev,
+                     viewdirs_dev, n_rays, z_base_dev, t_rand_dev, u_dev, u_per_ray, z_fine_dev, out_coarse_dev,
+                     out_fine_dev, workspace_dev, precision, stream);
 }
 
 int pob_loss_and_grad_flags(const pob_render_config* cfg, const pob_train_hparams* hp, const void* packed_coarse_dev,

@@ -28,15 +28,14 @@
 namespace pob {
 namespace {
 
-constexpr int PROJ_H = 128;        // width of the condition layer (net_width_condition)
+constexpr int PROJ_H = VIEW_H;     // width of the condition layer (net_width_condition)
 constexpr int PT = 64;             // points per tile
 constexpr int DT = 64;             // directions per tile
 constexpr int PROJ_THREADS = 256;  // 16 x 16 threads, 4 x 4 pairs each
 constexpr int MAX_K = 25;
 // leaf coefficients of one CTA: at most 64 leaves x 3K <= 4800, 19 per thread
 constexpr int ACC_PER_THREAD = (PT * 3 * MAX_K + PROJ_THREADS - 1) / PROJ_THREADS;
-constexpr int DIRS_PER_CTA = 32;   // direction-table kernel
-constexpr int MAX_DEG_VIEW = 32;
+constexpr int DIRS_PER_CTA = 32;   // direction-table kernels
 constexpr uint32_t PROJ_STREAM = 0x5348u;   // Philox counter word of the direction draws ("SH")
 
 // A direction of block `blk`: theta = acos(2u - 1), phi = 2 pi v (sh_proj.spherical_uniform_sampling), then
@@ -50,8 +49,43 @@ __device__ __forceinline__ float3 proj_direction(unsigned long long seed, long l
   return make_float3(__fmul_rn(s, cosf(phi)), __fmul_rn(s, sinf(phi)), cosf(theta));
 }
 
+// The posenc-and-matvec body of the direction tables, for one CTA of PROJ_H threads once dsm holds nd <= DIRS_PER_CTA
+// directions: enc = posenc(d, 0, deg_view, legacy) as nerf_sh/nerf/model_utils.py:145-173 (feature order in the
+// header), then thread j forms acc[dd] = sum_e W10_e[e][j] enc[dd][e] in order of e.
+__device__ __forceinline__ void view_matvec(const float3* dsm, int nd, int E, int deg_view, int legacy, int tid,
+                                            const float* __restrict__ w10e, float* enc,
+                                            float (&acc)[DIRS_PER_CTA]) {
+  const int L = deg_view;
+  for (int i = tid; i < nd * E; i += PROJ_H) {
+    const int dd = i / E, e = i - dd * E;
+    const float3 v = dsm[dd];
+    float f;
+    if (e < 3) {
+      f = e == 0 ? v.x : (e == 1 ? v.y : v.z);
+    } else {
+      int q = e - 3, l, c, cosine;
+      if (legacy) {
+        l = q / 6, cosine = (q % 6) >= 3, c = q % 3;
+      } else {
+        cosine = q >= 3 * L, q -= cosine ? 3 * L : 0, l = q / 3, c = q % 3;
+      }
+      const float x = (c == 0 ? v.x : (c == 1 ? v.y : v.z)) * exp2f(float(l));   // exact: a power of two
+      f = sinf(cosine ? __fadd_rn(x, 1.5707963705062866f) : x);
+    }
+    enc[dd * E + e] = f;
+  }
+  __syncthreads();
+#pragma unroll
+  for (int dd = 0; dd < DIRS_PER_CTA; ++dd) acc[dd] = 0.f;
+  for (int e = 0; e < E; ++e) {
+    const float w = __ldg(w10e + (long long)e * PROJ_H + tid);
+#pragma unroll
+    for (int dd = 0; dd < DIRS_PER_CTA; ++dd) acc[dd] = fmaf(w, enc[min(dd, nd - 1) * E + e], acc[dd]);
+  }
+}
+
 // grid (ceil(D / 32), n_blocks), 128 threads: thread j forms t_d[j] = sum_e W10_e[e][j] posenc(d)[e] of 32
-// directions.  posenc(d, 0, deg_view, legacy) as nerf_sh/nerf/model_utils.py:145-173 (feature order in the header).
+// directions (view_matvec).
 __global__ void __launch_bounds__(PROJ_H) proj_directions_kernel(unsigned long long seed, long long block0, int D,
                                                                  int deg_view, int legacy, int sh_deg, int K,
                                                                  const float* __restrict__ w10e,
@@ -80,38 +114,36 @@ __global__ void __launch_bounds__(PROJ_H) proj_directions_kernel(unsigned long l
       if (k < K) yo[k] = y[k];
   }
   __syncthreads();
-  const int L = deg_view;
-  for (int i = tid; i < nd * E; i += PROJ_H) {
-    const int dd = i / E, e = i - dd * E;
-    const float3 v = dsm[dd];
-    float f;
-    if (e < 3) {
-      f = e == 0 ? v.x : (e == 1 ? v.y : v.z);
-    } else {
-      int q = e - 3, l, c, cosine;
-      if (legacy) {
-        l = q / 6, cosine = (q % 6) >= 3, c = q % 3;
-      } else {
-        cosine = q >= 3 * L, q -= cosine ? 3 * L : 0, l = q / 3, c = q % 3;
-      }
-      const float x = (c == 0 ? v.x : (c == 1 ? v.y : v.z)) * exp2f(float(l));   // exact: a power of two
-      f = sinf(cosine ? __fadd_rn(x, 1.5707963705062866f) : x);
-    }
-    enc[dd * E + e] = f;
-  }
-  __syncthreads();
   float acc[DIRS_PER_CTA];
-#pragma unroll
-  for (int dd = 0; dd < DIRS_PER_CTA; ++dd) acc[dd] = 0.f;
-  for (int e = 0; e < E; ++e) {
-    const float w = __ldg(w10e + (long long)e * PROJ_H + tid);
-#pragma unroll
-    for (int dd = 0; dd < DIRS_PER_CTA; ++dd) acc[dd] = fmaf(w, enc[min(dd, nd - 1) * E + e], acc[dd]);
-  }
+  view_matvec(dsm, nd, E, deg_view, legacy, tid, w10e, enc, acc);
   float* row = tT + (b * PROJ_H + tid) * (long long)D + d0;
 #pragma unroll
   for (int dd = 0; dd < DIRS_PER_CTA; ++dd)
     if (dd < nd) row[dd] = acc[dd];
+}
+
+// grid ceil(n / 32), 128 threads: t[r][j] = sum_e W10_e[e][j] posenc(v_r)[e] + c[j] for the view directions v_r of 32
+// rays (or points): the per-ray table of the vanilla forward (mlp_fwd.cu, OUT_VANILLA)
+__global__ void __launch_bounds__(PROJ_H) view_table_kernel(const float* __restrict__ viewdirs, long long n,
+                                                            int deg_view, int legacy, const float* __restrict__ w10e,
+                                                            const float* __restrict__ c, float* __restrict__ t) {
+  extern __shared__ float enc[];   // [DIRS_PER_CTA][E]
+  __shared__ float3 dsm[DIRS_PER_CTA];
+  const int E = 3 + 6 * deg_view;
+  const long long r0 = (long long)blockIdx.x * DIRS_PER_CTA;
+  const int nd = int(min((long long)DIRS_PER_CTA, n - r0));
+  const int tid = threadIdx.x;
+  if (tid < nd) {
+    const float* v = viewdirs + (r0 + tid) * 3;
+    dsm[tid] = make_float3(v[0], v[1], v[2]);
+  }
+  __syncthreads();
+  float acc[DIRS_PER_CTA];
+  view_matvec(dsm, nd, E, deg_view, legacy, tid, w10e, enc, acc);
+  const float cj = c[tid];
+#pragma unroll
+  for (int dd = 0; dd < DIRS_PER_CTA; ++dd)
+    if (dd < nd) t[(r0 + dd) * PROJ_H + tid] = acc[dd] + cj;
 }
 
 struct ProjSmem {
@@ -320,6 +352,18 @@ PointWs point_ws(long long m) {
 }
 
 }  // namespace
+
+cudaError_t launch_view_table(const float* viewdirs, long long n, int deg_view, int legacy, const float* w10e,
+                              const float* c, float* t, cudaStream_t stream) {
+  if (n <= 0) return cudaSuccess;
+  const size_t smem = size_t(DIRS_PER_CTA) * (3 + 6 * deg_view) * sizeof(float);
+  cudaError_t e = cudaFuncSetAttribute(view_table_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+  if (e != cudaSuccess) return e;
+  view_table_kernel<<<unsigned((n + DIRS_PER_CTA - 1) / DIRS_PER_CTA), PROJ_H, smem, stream>>>(
+      viewdirs, n, deg_view, legacy, w10e, c, t);
+  return cudaGetLastError();
+}
+
 }  // namespace pob
 
 extern "C" {

@@ -252,3 +252,29 @@ def check_projection_scope(args):
             f"deg_view={args.deg_view}: 0 <= deg_view <= {MAX_DEG_VIEW} expected (scales above 2^31 of a unit "
             "direction are below the resolution of an fp32 sine's argument)")
     check_scope(_Override(args, use_viewdirs=False))
+
+
+def check_vanilla_scope(args):
+    """nerf_sh.eval / gen_video of a vanilla NeRF (use_viewdirs, the reference's nerf_sh/config/misc/og_nerf): the
+    fp16 forward with the view branch in its epilogue (nerf/vanilla.py).  Accepts use_viewdirs with sh_deg -1 and
+    sg_dim -1, the reference's condition branch (net_depth_condition 1, net_width_condition 128), 0 <= deg_view <= 32,
+    any trunk activation check_scope accepts (applied after the condition layer too, model_utils.py:90) and every
+    point-posenc, sample, dataset and density flag check_scope accepts.  Training a vanilla NeRF stays refused by
+    check_scope."""
+    if not args.use_viewdirs:
+        raise ValueError("check_vanilla_scope: use_viewdirs is not set (a NeRF-SH model goes through check_scope)")
+    if int(args.sh_deg) >= 0 or int(args.sg_dim) > 0:
+        # the reference's get_model asserts the same (nerf_sh/nerf/models.py:388-395)
+        raise NotImplementedError(
+            f"You can only use up to one of: SH, SG or use_viewdirs (sh_deg={args.sh_deg}, sg_dim={args.sg_dim}). "
+            "A vanilla NeRF is rendered with sh_deg -1: --config nerf_sh/config/misc/og_nerf; misc/proj (sh_deg 4) "
+            "is the config of octree.extraction's SH projection of that model")
+    if (int(args.net_depth_condition), int(args.net_width_condition)) != (1, 128):
+        raise NotImplementedError(
+            f"net_depth_condition={args.net_depth_condition}, net_width_condition={args.net_width_condition}: the "
+            "vanilla forward is built for one 128-wide condition layer (1, 128)")
+    if not 0 <= int(args.deg_view) <= MAX_DEG_VIEW:
+        raise NotImplementedError(
+            f"deg_view={args.deg_view}: 0 <= deg_view <= {MAX_DEG_VIEW} expected (scales above 2^31 of a unit "
+            "direction are below the resolution of an fp32 sine's argument)")
+    check_scope(_Override(args, use_viewdirs=False))

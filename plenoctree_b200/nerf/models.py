@@ -45,7 +45,67 @@ def glorot_uniform_flat(sh_deg, generator=None, posenc=None):
     return torch.cat(parts).float()
 
 
-class NerfModel:
+class RaySampler:
+    """The per-ray inputs of NerfModel.__call__ shared by the NeRF-SH and the vanilla model (nerf/vanilla.py): the
+    un-jittered depth table, the deterministic inverse-CDF uniforms, the jitter / uniforms of a randomized call and
+    the density noise.  Needs num_coarse_samples, num_fine_samples, num_mlps, near, far, lindisp, noise_std, device
+    and cfg (RenderConfig)."""
+
+    def _init_depths(self):
+        # un-jittered depth table, computed with the reference expression (model_utils.py:125-129)
+        t_vals = torch.linspace(0.0, 1.0, self.num_coarse_samples, dtype=torch.float32)
+        if self.lindisp:
+            zb = 1.0 / (1.0 / self.near * (1.0 - t_vals) + 1.0 / self.far * t_vals)
+        else:
+            zb = self.near * (1.0 - t_vals) + self.far * t_vals
+        self.z_base = zb.to(self.device)
+        # deterministic u of piecewise_constant_pdf (model_utils.py:259-262)
+        if self.num_fine_samples > 0:
+            self.u_table = torch.linspace(0.0, 1.0 - float(np.finfo(np.float32).eps), self.num_fine_samples,
+                                          dtype=torch.float32).to(self.device)
+        else:
+            self.u_table = None
+
+    def _set_sigma_noise(self, n, randomized, sigma_noise):
+        """add_gaussian_noise (nerf_sh/nerf/model_utils.py:317-332): when randomized and noise_std is set, raw sigma
+        of both levels gets normal(0, noise_std^2) noise.  sigma_noise = (coarse [n,Nc], fine [n,Nc+Nf]) passes the
+        already scaled draws explicitly (parity tests).  Returns the tensors (kept alive by the caller)."""
+        nc = nf = None
+        if sigma_noise is not None:
+            nc = _cuda_f32(sigma_noise[0], "sigma_noise[0]", self.num_coarse_samples)
+            if self.num_mlps == 2:
+                nf = _cuda_f32(sigma_noise[1], "sigma_noise[1]", self.num_coarse_samples + self.num_fine_samples)
+        elif randomized and self.noise_std is not None and self.noise_std > 0:
+            nc = torch.randn((n, self.num_coarse_samples), device=self.device) * float(self.noise_std)
+            if self.num_mlps == 2:
+                nf = torch.randn((n, self.num_coarse_samples + self.num_fine_samples),
+                                 device=self.device) * float(self.noise_std)
+        for t in (nc, nf):
+            if t is not None and t.shape[0] != n:
+                raise ValueError("sigma_noise must have one row per ray")
+        self.cfg.sigma_noise_coarse_dev = ptr(nc)
+        self.cfg.sigma_noise_fine_dev = ptr(nf)
+        return nc, nf
+
+    def _uniforms(self, n, randomized, t_rand, u):
+        if t_rand is not None:
+            t_rand = _cuda_f32(t_rand, "t_rand", self.num_coarse_samples)
+        elif randomized:
+            t_rand = torch.rand((n, self.num_coarse_samples), dtype=torch.float32, device=self.device)
+        upr = 0
+        if self.num_fine_samples > 0:
+            if u is not None:
+                u = _cuda_f32(u, "u", self.num_fine_samples)
+                upr = 1
+            elif randomized:
+                u = torch.rand((n, self.num_fine_samples), dtype=torch.float32, device=self.device)
+                upr = 1
+            else:
+                u = self.u_table
+        return t_rand, u, upr
+
+
+class NerfModel(RaySampler):
     """Nerf NN Model with both coarse and fine MLPs (nerf_sh/nerf/models.py:52-348), SH output head.
 
     Parameters live in one flat fp32 CUDA tensor `params` = [MLP_0 | MLP_1], each MLP in reference
@@ -94,19 +154,7 @@ class NerfModel:
         self.cfg.sigma_activation = self.sigma_act_code
         self.cfg.posenc = posenc_ref(self._posenc_struct)
         self._ws = {}
-        # un-jittered depth table, computed with the reference expression (model_utils.py:125-129)
-        t_vals = torch.linspace(0.0, 1.0, self.num_coarse_samples, dtype=torch.float32)
-        if self.lindisp:
-            zb = 1.0 / (1.0 / self.near * (1.0 - t_vals) + 1.0 / self.far * t_vals)
-        else:
-            zb = self.near * (1.0 - t_vals) + self.far * t_vals
-        self.z_base = zb.to(self.device)
-        # deterministic u of piecewise_constant_pdf (model_utils.py:259-262)
-        if self.num_fine_samples > 0:
-            self.u_table = torch.linspace(0.0, 1.0 - float(np.finfo(np.float32).eps), self.num_fine_samples,
-                                          dtype=torch.float32).to(self.device)
-        else:
-            self.u_table = None
+        self._init_depths()
 
     @classmethod
     def from_flags(cls, args, *, max_rays, sparsity_npoints=0, device="cuda"):
@@ -155,27 +203,6 @@ class NerfModel:
         return self.blobs[0] if (coarse or self.num_mlps == 1) else self.blobs[1]
 
     # ---- NerfModel.__call__ ------------------------------------------------------------------
-    def _set_sigma_noise(self, n, randomized, sigma_noise):
-        """add_gaussian_noise (nerf_sh/nerf/model_utils.py:317-332): when randomized and noise_std is set, raw sigma
-        of both levels gets normal(0, noise_std^2) noise.  sigma_noise = (coarse [n,Nc], fine [n,Nc+Nf]) passes the
-        already scaled draws explicitly (parity tests).  Returns the tensors (kept alive by the caller)."""
-        nc = nf = None
-        if sigma_noise is not None:
-            nc = _cuda_f32(sigma_noise[0], "sigma_noise[0]", self.num_coarse_samples)
-            if self.num_mlps == 2:
-                nf = _cuda_f32(sigma_noise[1], "sigma_noise[1]", self.num_coarse_samples + self.num_fine_samples)
-        elif randomized and self.noise_std is not None and self.noise_std > 0:
-            nc = torch.randn((n, self.num_coarse_samples), device=self.device) * float(self.noise_std)
-            if self.num_mlps == 2:
-                nf = torch.randn((n, self.num_coarse_samples + self.num_fine_samples),
-                                 device=self.device) * float(self.noise_std)
-        for t in (nc, nf):
-            if t is not None and t.shape[0] != n:
-                raise ValueError("sigma_noise must have one row per ray")
-        self.cfg.sigma_noise_coarse_dev = ptr(nc)
-        self.cfg.sigma_noise_fine_dev = ptr(nf)
-        return nc, nf
-
     def __call__(self, rays, randomized=False, t_rand=None, u=None, precision=None, z_fine=None, sigma_noise=None):
         """-> [(rgb_coarse, disp_coarse, acc_coarse), (rgb, disp, acc)] for up to max_rays rays.
 
@@ -202,23 +229,6 @@ class NerfModel:
         if out_f is not None:
             ret.append((out_f[:, :3], out_f[:, 3], out_f[:, 4]))
         return ret
-
-    def _uniforms(self, n, randomized, t_rand, u):
-        if t_rand is not None:
-            t_rand = _cuda_f32(t_rand, "t_rand", self.num_coarse_samples)
-        elif randomized:
-            t_rand = torch.rand((n, self.num_coarse_samples), dtype=torch.float32, device=self.device)
-        upr = 0
-        if self.num_fine_samples > 0:
-            if u is not None:
-                u = _cuda_f32(u, "u", self.num_fine_samples)
-                upr = 1
-            elif randomized:
-                u = torch.rand((n, self.num_fine_samples), dtype=torch.float32, device=self.device)
-                upr = 1
-            else:
-                u = self.u_table
-        return t_rand, u, upr
 
     # ---- point evaluation --------------------------------------------------------------------
     def eval_points_raw(self, points, viewdirs=None, coarse=False, want_rgb=True, precision=None):

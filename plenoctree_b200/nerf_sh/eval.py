@@ -1,14 +1,16 @@
 """`python -m plenoctree_b200.nerf_sh.eval` — the reference's `nerf_sh.eval` CLI (nerf_sh/eval.py:45-133): restore the
 newest checkpoint of train_dir, render every test image deterministically (randomized=False), write
 `test_preds/{idx:03d}.png`, `disp_{idx:03d}.png`, and the PSNR / SSIM summaries (psnr.txt, ssim.txt,
-psnrs_<step>.txt, ssims_<step>.txt — the block the reference keeps commented out at eval.py:99-127)."""
+psnrs_<step>.txt, ssims_<step>.txt — the block the reference keeps commented out at eval.py:99-127).  With
+use_viewdirs (nerf_sh/config/misc/og_nerf) the model is a vanilla NeRF (nerf/vanilla.py), restored from a flax
+checkpoint_<step> or a torch *.ckpt."""
 import os
 
 import numpy as np
 import torch
 from absl import app
 
-from ..nerf import checkpoints, datasets, flags as F, models, utils
+from ..nerf import checkpoints, datasets, flags as F, models, utils, vanilla
 
 FLAGS = F.FLAGS
 F.define_flags()
@@ -17,14 +19,21 @@ F.define_flags()
 def main(unused_argv):
     F.update_flags(FLAGS)
     F.check_flags(FLAGS)
-    F.check_scope(FLAGS)
+    if FLAGS.use_viewdirs:          # a vanilla NeRF (--config nerf_sh/config/misc/og_nerf)
+        F.check_vanilla_scope(FLAGS)
+    else:
+        F.check_scope(FLAGS)
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
     torch.cuda.set_device(dev)
     dataset = datasets.get_dataset("test", FLAGS, device=dev)
-    model, state = models.get_model_state(FLAGS, device=dev, restore=False, max_rays=min(FLAGS.chunk, 8192))
-    step = checkpoints.restore_checkpoint(FLAGS.train_dir, model, state)
-    if step is None:
-        raise ValueError(f"no checkpoint_* in {FLAGS.train_dir}")
+    if FLAGS.use_viewdirs:
+        model = vanilla.VanillaNerfModel.from_flags(FLAGS, max_rays=min(FLAGS.chunk, 8192), device=dev)
+        step = model.step
+    else:
+        model, state = models.get_model_state(FLAGS, device=dev, restore=False, max_rays=min(FLAGS.chunk, 8192))
+        step = checkpoints.restore_checkpoint(FLAGS.train_dir, model, state)
+        if step is None:
+            raise ValueError(f"no checkpoint_* in {FLAGS.train_dir}")
     out_dir = os.path.join(FLAGS.train_dir, "path_renders" if FLAGS.render_path else "test_preds")   # eval.py:63-65
     if FLAGS.save_output:
         os.makedirs(out_dir, exist_ok=True)

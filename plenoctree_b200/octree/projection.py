@@ -21,6 +21,7 @@ import torch
 
 from .._lib import NET_RELU, PREC_FP16, check, lib, posenc_ref, posenc_struct, ptr, stream_ptr
 from .. import ops
+from ..nerf.vanilla import fold_view_branch
 
 PROJ_SEED = 20200823
 CELLS_PER_BLOCK = 1024          # leaves sharing one direction set
@@ -46,12 +47,11 @@ class VanillaNerf:
                              "MLP of a model with a fine level)")
         layers = mlps["MLP_1"] if num_fine_samples > 0 else mlps["MLP_0"]
         trunk = [np.asarray(a, dtype=np.float32) for k, b in layers[:9] for a in (k, b)]
-        k9, b9 = (np.asarray(a, dtype=np.float64) for a in layers[9])
-        k10, b10 = (np.asarray(a, dtype=np.float64) for a in layers[10])
         k11, b11 = layers[11]
         dev = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).to(self.device)
-        self.head_w = dev(k9 @ k10[:256])                   # [256, 128]
-        self.head_b = dev(b9 @ k10[:256] + b10)             # [128]
+        head_w, head_b = fold_view_branch(layers)
+        self.head_w = dev(head_w)                           # [256, 128]
+        self.head_b = dev(head_b)                           # [128]
         flat = np.concatenate([a.reshape(-1) for a in trunk] + [np.zeros(256 * 3 + 3, np.float32)])
         self.sigma_blob = ops.pack_weights(torch.from_numpy(flat).to(self.device), -1, posenc=self.posenc)
         self.w10e = dev(np.asarray(layers[10][0], dtype=np.float32)[256:])   # [3 + 6 deg_view, 128]
