@@ -78,6 +78,9 @@ int pob_sm_count(void);
 long long pob_launch_count(void);
 void pob_timing_enable(int on);
 int pob_timing_read(double* ms_out, long long* launches_out);
+/* all kernel classes: the five of pob_timing_read, then the median cut (pob_quantize_median_cut).  Fills the first
+ * min(n, 6) entries of ms_out / launches_out (either may be NULL) and returns 6. */
+int pob_timing_read_phases(int n, double* ms_out, long long* launches_out);
 
 /* ---------------------------------------------------------------------------------------------
  * Parameters of one MLP (MLP_0 coarse / MLP_1 fine; nerf_sh/nerf/models.py:83-104).
@@ -576,6 +579,22 @@ int pob_render_rays_vanilla(const pob_render_config* cfg, const pob_view_branch*
 int pob_eval_points_vanilla(const void* packed_dev, const pob_posenc* posenc, const pob_view_branch* view, int mlp,
                             const float* points_dev, const float* viewdirs_dev, int64_t m, float* table_dev,
                             float* raw_rgb_dev, float* raw_sigma_dev, float* out_rgbs_dev, int sigma_activation,
+                            void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Palette quantisation of compressed trees (octree.compression: median_cut)
+ * ------------------------------------------------------------------------------------------- */
+/* Median cut of n_basis independent point sets of n points each, byte-identical to the numpy median_cut:
+ *   points_dev   [n_basis, n, 3] fp32
+ *   weights_dev  [n] fp64 shared by every set, or NULL for the unweighted cut
+ *   palette_dev  [n_basis, 2^bits, 3] fp32 out: the (weighted) mean of every box, zero for empty boxes
+ *   map_dev      [n_basis, n] uint16 out: the box of every point
+ * 0 <= bits <= 16, 0 <= n < 2^31, n_basis >= 1 with n_basis * n < 2^40.  workspace_dev holds
+ * pob_quantize_workspace_bytes(n_basis, n, weights != NULL) bytes, 256-byte aligned; the call is deterministic and
+ * independent of POB_SM_COUNT.  Every refusal returns before any launch. */
+int64_t pob_quantize_workspace_bytes(int64_t n_basis, int64_t n, int weighted);
+int pob_quantize_median_cut(const float* points_dev, const double* weights_dev, int64_t n_basis, int64_t n, int bits,
+                            float* palette_dev, uint16_t* map_dev, void* workspace_dev, int64_t workspace_bytes,
                             void* stream);
 
 #ifdef __cplusplus

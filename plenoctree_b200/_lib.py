@@ -33,6 +33,7 @@ SIGNATURES = {
     "pob_launch_count": (_c.c_longlong, []),
     "pob_timing_enable": (None, [_i]),
     "pob_timing_read": (_i, [_vp, _vp]),
+    "pob_timing_read_phases": (_i, [_i, _vp, _vp]),
     "pob_param_count": (_i64, [_i]),
     "pob_packed_bytes": (_i64, [_i]),
     "pob_pack_weights": (_i, [_fp, _i, _vp, _vp]),
@@ -97,6 +98,8 @@ SIGNATURES = {
     "pob_render_rays_vanilla": (_i, [_vp, _vp, _vp, _vp, _fp, _fp, _fp, _i, _fp, _fp, _fp, _i, _fp, _fp, _fp, _vp, _i,
                                      _vp]),
     "pob_eval_points_vanilla": (_i, [_vp, _vp, _vp, _i, _fp, _fp, _i64, _fp, _fp, _fp, _fp, _i, _vp]),
+    "pob_quantize_workspace_bytes": (_i64, [_i64, _i64, _i]),
+    "pob_quantize_median_cut": (_i, [_fp, _fp, _i64, _i64, _i, _fp, _fp, _vp, _i64, _vp]),
 }
 
 

@@ -29,8 +29,8 @@ struct TimedSlot {
   cudaEvent_t a, b;
 };
 static std::vector<TimedSlot> g_slots;
-static double g_phase_ms[POB_PH_COUNT] = {0, 0, 0, 0, 0};
-static long long g_phase_n[POB_PH_COUNT] = {0, 0, 0, 0, 0};
+static double g_phase_ms[POB_PH_COUNT] = {};
+static long long g_phase_n[POB_PH_COUNT] = {};
 PobPhaseTimer::PobPhaseTimer(int phase, cudaStream_t s) : slot(-1), st(s) {
   if (!g_timing) return;
   TimedSlot t;
@@ -215,13 +215,17 @@ void pob_timing_enable(int on) {
   }
 }
 
-int pob_timing_read(double* ms_out, long long* launches_out) {
+int pob_timing_read_phases(int n, double* ms_out, long long* launches_out) {
   drain_slots();
-  for (int i = 0; i < POB_PH_COUNT; ++i) {
+  for (int i = 0; i < n && i < POB_PH_COUNT; ++i) {
     if (ms_out) ms_out[i] = g_phase_ms[i];
     if (launches_out) launches_out[i] = g_phase_n[i];
   }
   return POB_PH_COUNT;
+}
+int pob_timing_read(double* ms_out, long long* launches_out) {
+  pob_timing_read_phases(POB_PH_LEGACY_COUNT, ms_out, launches_out);
+  return POB_PH_LEGACY_COUNT;
 }
 const char* pob_last_error(void) { return g_err.c_str(); }
 int pob_sm_count(void) { return sm_count(); }
@@ -539,5 +543,33 @@ int pob_sample_pdf(const float* z_coarse_dev, const float* weights_dev, const fl
   return 0;
 }
 
+
+int64_t pob_quantize_workspace_bytes(int64_t n_basis, int64_t n, int weighted) {
+  if (n_basis < 1 || n < 0 || n > INT32_MAX || n_basis * n >= (int64_t(1) << 40)) return -1;
+  return int64_t(pob::quant_layout(n_basis, n, weighted != 0).bytes);
+}
+
+int pob_quantize_median_cut(const float* points_dev, const double* weights_dev, int64_t n_basis, int64_t n, int bits,
+                            float* palette_dev, uint16_t* map_dev, void* workspace_dev, int64_t workspace_bytes,
+                            void* stream) {
+  const char* W = "pob_quantize_median_cut";
+  if (bits < 0 || bits > pob::QUANT_MAX_BITS) return pob_fail(W, "bits must be in [0, 16] (the map is uint16)");
+  if (n_basis < 1 || n < 0 || n > INT32_MAX || n_basis * n >= (int64_t(1) << 40))
+    return pob_fail(W, "need n_basis >= 1, 0 <= n < 2^31 (uint32 point indices) and n_basis * n < 2^40");
+  if (!palette_dev || (n > 0 && (!points_dev || !map_dev || !workspace_dev)))
+    return pob_fail(W, "NULL pointer");
+  if (reinterpret_cast<uintptr_t>(workspace_dev) % 256 != 0) return pob_fail(W, "workspace is not 256-byte aligned");
+  if (n > 0 && workspace_bytes < pob_quantize_workspace_bytes(n_basis, n, weights_dev != nullptr))
+    return pob_fail(W, "workspace is smaller than pob_quantize_workspace_bytes");
+  const int sms = pob_sms_or_fail(W);
+  if (!sms) return 1;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n == 0) {   // median_cut of no points: an all-zero palette, an empty map
+    POB_CUDA(W, cudaMemsetAsync(palette_dev, 0, size_t(n_basis) * (size_t(1) << bits) * 3 * sizeof(float), st));
+    return 0;
+  }
+  return pob::launch_quantize(points_dev, weights_dev, n, int(n_basis), bits, palette_dev, map_dev, workspace_dev,
+                              sms, st);
+}
 
 }  // extern "C"

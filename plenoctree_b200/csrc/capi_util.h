@@ -46,7 +46,9 @@ pob::FwdParams pob_vanilla_params(const void* packed, pob::NetDesc net, const po
   } while (0)
 
 // ---- instrumentation (bench.py): kernel launch counter and per-phase CUDA-event timing ---------
-enum PobPhase { POB_PH_FWD = 0, POB_PH_BWD, POB_PH_WGRAD, POB_PH_RENDER, POB_PH_OPTIM, POB_PH_COUNT };
+// pob_timing_read reports the first POB_PH_LEGACY_COUNT classes, pob_timing_read_phases all POB_PH_COUNT
+enum PobPhase { POB_PH_FWD = 0, POB_PH_BWD, POB_PH_WGRAD, POB_PH_RENDER, POB_PH_OPTIM, POB_PH_QUANT, POB_PH_COUNT };
+constexpr int POB_PH_LEGACY_COUNT = 5;
 void pob_count_launch(int n = 1);
 // records an event pair around [begin, end) of one kernel launch when timing is enabled
 struct PobPhaseTimer {

@@ -341,4 +341,19 @@ inline FlatLayout vanilla_flat_layout(int W) {
   return L;
 }
 
+// ---- quantize.cu ----------------------------------------------------------------------------
+// median cut of compressed-tree palettes (pob_quantize_median_cut): at most 2^16 colours, so at most 2^15 boxes split
+// in a round
+constexpr int QUANT_MAX_BITS = 16;
+constexpr int QUANT_MAX_COLORS = 1 << QUANT_MAX_BITS;
+// byte offsets of the workspace arrays of n_basis point sets of n points (256-byte aligned) and the total
+struct QuantLayout {
+  size_t idx[2], off[2], key[2], pos[2], up, split, wsorted, total, bytes;
+};
+QuantLayout quant_layout(int64_t n_basis, int64_t n, int weighted);
+// every launch of one quantisation, in order on `stream`, each counted and timed under POB_PH_QUANT; the caller has
+// checked the arguments.  0, or 1 after a launch error recorded for pob_last_error
+int launch_quantize(const float* points, const double* weights, int64_t n, int nb, int bits, float* palette,
+                            uint16_t* map, void* workspace, int sms, cudaStream_t stream);
+
 }  // namespace pob

@@ -9,7 +9,9 @@ The reference calls svox's C++ `quantize_median_cut` (third-party, not vendored,
 unpinned**).  The median cut below is the textbook one in its balanced form: `bits` rounds, every round splits
 every box at the (weighted) median of its longest axis, palette entry = (weighted) mean of the box; all boxes of a
 round are processed together with segment reductions, so a round is a few passes over the points.
-Host numpy: this is an offline, one-off step on a few million voxels.
+The numpy code below is the definition.  `compress_tree(..., device="cuda")` and the CLI's `--device` (default
+`auto`: the GPU when the CUDA library loads and a GPU is visible) run the same computation on the device
+(octree/quantize.py, csrc/quantize.cu), with byte-identical output; this module imports without the library.
 """
 import argparse
 import os
@@ -68,8 +70,14 @@ def median_cut(points, bits, weights=None):
     return palette.astype(np.float32), box
 
 
-def compress_tree(z, bits=16, sigma_thresh=2.0, retain=0, weighted=False, quantize=True):
-    """z: dict of a tree.npz -> dict of the compressed file (compression.py:80-139)."""
+def compress_tree(z, bits=16, sigma_thresh=2.0, retain=0, weighted=False, quantize=True, device=None):
+    """z: dict of a tree.npz -> dict of the compressed file (compression.py:80-139).  device None / "cpu": numpy;
+    "cuda": octree.quantize.compress_tree, which returns identical arrays."""
+    if device not in (None, "cpu"):
+        if device != "cuda":
+            raise ValueError(f"device must be None, 'cpu' or 'cuda', got {device!r}")
+        from . import quantize as Q
+        return Q.compress_tree(z, bits, sigma_thresh, retain, weighted, quantize)
     out = {k: v for k, v in z.items() if k not in ("parent_depth", "geom_resize_fact", "n_free", "n_internal", "depth_limit")}
     if not quantize:
         return out
@@ -116,6 +124,26 @@ def decompress_data(c):
     return np.concatenate([rgb.reshape(sigma.shape + (3 * basis_dim,)), sigma[..., None]], axis=-1)
 
 
+def resolve_device(device):
+    """--device auto | cpu | cuda -> "cpu" or "cuda".  auto: cuda when the CUDA library loads and a GPU it runs on is
+    visible, else cpu; cuda: an error when it cannot run."""
+    if device == "cpu":
+        return "cpu"
+    if device not in ("auto", "cuda"):
+        raise ValueError(f"--device must be auto, cpu or cuda, got {device!r}")
+    try:
+        from . import quantize as Q
+    except (ImportError, OSError) as e:
+        if device == "cuda":
+            raise RuntimeError(f"--device cuda: the CUDA library does not load ({e})") from e
+        return "cpu"
+    if Q.device_available():
+        return "cuda"
+    if device == "cuda":
+        raise RuntimeError("--device cuda: no CUDA GPU the library can run on (sm_90) is visible")
+    return "cpu"
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("input", type=str, nargs="+", help="Input npz(s)")
@@ -126,7 +154,10 @@ def main(argv=None):
     ap.add_argument("--weighted", action="store_true", help="Use weighted median cut")
     ap.add_argument("--sigma_thresh", type=float, default=2.0, help="Kill voxels under this sigma")
     ap.add_argument("--retain", type=int, default=0, help="Do not compress first x SH coeffs")
+    ap.add_argument("--device", choices=("auto", "cpu", "cuda"), default="auto",
+                    help="Where to quantise: auto uses the GPU when the CUDA library and a GPU are available")
     args = ap.parse_args(argv)
+    device = resolve_device(args.device)
     os.makedirs(args.out_dir, exist_ok=True)
     print("Quantization disabled, only applying deflate" if args.noquant else "Quantization enabled")
     for fname in args.input:
@@ -139,7 +170,8 @@ def main(argv=None):
         if not args.noquant and "quant_colors" in z:
             print(" > skip since source already compressed")
             continue
-        out = compress_tree(z, args.bits, args.sigma_thresh, args.retain, args.weighted, quantize=not args.noquant)
+        out = compress_tree(z, args.bits, args.sigma_thresh, args.retain, args.weighted, quantize=not args.noquant,
+                            device=device)
         np.savez_compressed(fname_c, **out)
         print(" > Size", os.path.getsize(fname) // (1024 * 1024), "MB ->", os.path.getsize(fname_c) // (1024 * 1024), "MB")
     return 0
