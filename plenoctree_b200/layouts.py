@@ -253,6 +253,7 @@ E_TILE_BYTES = A_CHUNK_BYTES              # [128 x 64] fp16
 DO_TILE_BYTES = 2 * A_CHUNK_BYTES         # [128 x 128] fp16
 WG_MAX_CTAS = 160
 WG_PARTIAL_FLOATS = 65536 + 256
+VIEW_H = 128                              # width of the vanilla condition layer (common.cuh: VIEW_H)
 
 
 def padded_rows(M):
@@ -265,7 +266,7 @@ def bwd_image_bytes(K):
     return blob_layout(K)["bwd_bytes"]
 
 
-def train_workspace_views(cfg, n_rays, sparsity_on, training=True, precision=1):
+def train_workspace_views(cfg, n_rays, sparsity_on, training=True, precision=1, vanilla=False):
     """Byte layout of the training workspace of `cfg` (a RenderConfig or anything with its fields) for a
     pob_loss_and_grad call over `n_rays` rays; `sparsity_on` = the call carries the sparsity points (weight > 0).
 
@@ -283,7 +284,13 @@ def train_workspace_views(cfg, n_rays, sparsity_on, training=True, precision=1):
     precision=3 (POB_PREC_FP16X3): the workspace of pob_loss_and_grad_prec at fp16x3
     (pob_train_workspace_bytes(cfg, 3)): the fp16 views, plus per level the residual images H_lo, E_lo, DZ_lo, DO_lo
     (shaped like H, E, DZ, DO), partials_x3 = [[mlp 0 pass 1, pass 2], [mlp 1 ...]] and wt_lo = [mlp 0, mlp 1]
-    (offset, bytes) of the residual dgrad weight images."""
+    (offset, bytes) of the residual dgrad weight images.
+
+    vanilla=True (with training=False): the workspace of pob_render_rays_vanilla (pob_vanilla_workspace_bytes(cfg)):
+    the render workspace, then one fp32 view table per level behind it, each level's view_t [n_rays, VIEW_H] (the
+    per-ray W10_e posenc(viewdir) + c of the level's MLP, carved for cfg.max_rays rays)."""
+    if vanilla and training:
+        raise ValueError("the vanilla workspace is a render workspace: vanilla=True needs training=False")
     R = int(cfg.max_rays)
     nc, nf, nsp = int(cfg.num_coarse_samples), int(cfg.num_fine_samples), int(cfg.sparsity_npoints)
     Ns = [nc, nc + nf if nf > 0 else 0]
@@ -327,6 +334,9 @@ def train_workspace_views(cfg, n_rays, sparsity_on, training=True, precision=1):
         v["mask"] = (take(NUM_TRUNK * tiles_cap * TILE_M * 8 * 4), (NUM_TRUNK, rows, 8))
         levels.append(v)
     if not training:
+        if vanilla:
+            for v in levels:
+                v["view_t"] = (take(4 * VIEW_H * R), (n_rays, VIEW_H))
         return dict(total=off, levels=levels, partials=[])
     partials = [take(4 * WG_MAX_CTAS * WG_PARTIAL_FLOATS) for _ in range(2)]
     progress = take(4 * sum(caps))   # mlp_bwd -> mlp_wgrad progress counters, level 0's tiles then level 1's
@@ -346,7 +356,7 @@ def train_workspace_views(cfg, n_rays, sparsity_on, training=True, precision=1):
 
 _VIEW_DTYPES = dict(z="float32", rgbs="float32", weights="float32", comp="float32", disp="float32", acc="float32",
                     G="float32", H="uint8", E="uint8", DZ="uint8", DO="uint8", mask="int32",
-                    progress="int32", H_lo="uint8", E_lo="uint8", DZ_lo="uint8", DO_lo="uint8")
+                    progress="int32", H_lo="uint8", E_lo="uint8", DZ_lo="uint8", DO_lo="uint8", view_t="float32")
 
 
 def workspace_view(ws, level, name):

@@ -17,7 +17,6 @@ Once: a CUDA-graph replay of a row with every flag away from its default.
 import functools
 import os
 import re
-from itertools import combinations
 
 import numpy as np
 import pytest
@@ -26,6 +25,7 @@ import torch
 from oracle import net_activation_oracle as NA
 from oracle import posenc_oracle as PO
 from plenoctree_b200 import layouts as L
+from tests.support.covering import assert_covers_every_pair
 from tests.support.model_flags import _alt_pe
 from tests.support.ray_stages import RayCase
 from tests.support.records import ROOT, record
@@ -114,14 +114,7 @@ _record = functools.partial(record, "parity_flag_matrix.json")
 # =====================================================================================================================
 def test_matrix_covers_every_pair():
     """every pair of values of any two dimensions appears in some row"""
-    for row in MATRIX:
-        for v, dim in zip(row, DIMS):
-            assert v in dim, (row, v)
-    missing = []
-    for i, j in combinations(range(len(DIMS)), 2):
-        seen = {(r[i], r[j]) for r in MATRIX}
-        missing += [(i, a, j, b) for a in DIMS[i] for b in DIMS[j] if (a, b) not in seen]
-    assert not missing, missing
+    assert_covers_every_pair(MATRIX, DIMS)
 
 
 def test_matrix_covers_both_encoder_branches_of_every_forward():

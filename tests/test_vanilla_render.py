@@ -18,10 +18,8 @@ import torch
 from oracle import posenc_oracle as PO
 from oracle import projection_oracle as PJ
 from tests.support import vanilla_ref as VR
+from tests.support.vanilla_ref import C_BRANCH, RGB_TOL, U, _h7_fp16, _mlps, _rays, _view_features
 
-U = 2.0 ** -24          # fp32 unit roundoff
-C_BRANCH = 512          # fp32 accumulation: 256 + 128 + 3 sums in sequence, activation ulps (kernels.h) included
-RGB_TOL = 1e-3          # test_render.test_nerf_forward_vs_oracle: fp16, same sample positions, max-abs
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -110,13 +108,6 @@ def test_og_nerf_preset_equals_the_reference_file_and_a_file_on_disk_wins(tmp_pa
     args = _args(**dict(more, config=str(tmp_path / "og_nerf")))
     F.update_flags(args)
     assert args.deg_view == 2 and args.factor == 4
-
-
-def _mlps(seed, pe=PO.DEFAULT, deg_view=4, sigma_scale=8.0):
-    mlps = {"MLP_0": PJ.init_params(seed, pe, deg_view), "MLP_1": PJ.init_params(seed + 1, pe, deg_view)}
-    for layers in mlps.values():                      # a dense blob around the origin: partially opaque rays
-        layers[8] = (layers[8][0] * sigma_scale, layers[8][1] + 2.0)
-    return mlps
 
 
 def test_fold_is_formed_in_fp64_and_rounded_once():
@@ -252,49 +243,10 @@ def test_paired_oracle_is_the_cross_broadcast_diagonal():
 
 
 # ---- GPU ----------------------------------------------------------------------------------------------------------
-def _rays(R, seed):
-    rs = np.random.RandomState(seed)
-    o = rs.normal(size=(R, 3))
-    o = (o / np.linalg.norm(o, axis=1, keepdims=True) * 4.0).astype(np.float32)
-    d = (rs.uniform(-0.6, 0.6, (R, 3)) - o).astype(np.float32)
-    d = (d / np.linalg.norm(d, axis=1, keepdims=True) * rs.uniform(0.8, 1.2, (R, 1))).astype(np.float32)
-    v = (d / np.linalg.norm(d, axis=1, keepdims=True)).astype(np.float32)
-    return o, d, v
-
-
 def _model(mlps, **kw):
     from plenoctree_b200.nerf.vanilla import VanillaNerfModel
     pe = kw.pop("pe", PO.DEFAULT)
     return VanillaNerfModel(mlps, min_deg_point=pe[0], max_deg_point=pe[1], legacy_posenc_order=pe[2], **kw)
-
-
-def _h7_fp16(mlps_layers, pts, pe, act_code):
-    """the fp16 h7 the kernel's heads MMA reads, probed through pob_eval_points_raw: Dense_9 of a plain-SH25 blob of
-    the same trunk set to unit columns, so raw rgb column j is h7[k] exactly (fp32 sums of one fp16 product)"""
-    from plenoctree_b200 import ops
-    K = 25
-    trunk = [np.asarray(a, np.float32).reshape(-1) for k, b in mlps_layers[:9] for a in (k, b)]
-    h = np.zeros((pts.shape[0], 256), np.float32)
-    for k0 in range(0, 256, 3 * K):
-        n = min(3 * K, 256 - k0)
-        w9 = np.zeros((256, 3 * K), np.float32)
-        w9[np.arange(k0, k0 + n), np.arange(n)] = 1.0
-        flat = np.concatenate(trunk + [w9.reshape(-1), np.zeros(3 * K, np.float32)])
-        blob = ops.pack_weights(torch.from_numpy(flat).cuda(), 4, posenc=pe)
-        rgb, _ = ops.eval_points_raw(blob, 4, pts, posenc=pe, net_activation=act_code)
-        h[:, k0:k0 + n] = rgb[:, :n].cpu().numpy()
-    return h.astype(np.float64)
-
-
-def _view_features(v32, deg_view, legacy):
-    """posenc(v, 0, deg_view, legacy) in fp64 of the fp32 sine arguments the direction tables form: x 2^l is exact,
-    the cosine's argument is the fp32 sum x 2^l + fp32(pi / 2)"""
-    m, L = v32.shape[0], deg_view
-    xb = (v32[:, None, :] * (2.0 ** np.arange(L, dtype=np.float32))[:, None]).astype(np.float32)     # [m, L, 3]
-    xc = (xb + np.float32(0.5 * np.pi)).astype(np.float32)
-    s, c = np.sin(xb.astype(np.float64)), np.sin(xc.astype(np.float64))
-    four = np.stack([s, c], 2).reshape(m, -1) if legacy else np.concatenate([s.reshape(m, -1), c.reshape(m, -1)], 1)
-    return np.concatenate([v32.astype(np.float64), four], 1)
 
 
 def _act64(name, z):
