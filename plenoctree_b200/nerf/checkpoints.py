@@ -43,45 +43,93 @@ def param_count(sh_deg, posenc=None):
     return sum(i * o + o for i, o in _dims(sh_deg, posenc))
 
 
-def flat_to_flax_params(flat, sh_deg, posenc=None):
-    """flat [num_mlps * P] -> {"MLP_0": {"Dense_i": {"kernel": [in,out], "bias": [out]}}, "MLP_1": ...}
-    (the pytree under ["optimizer"]["target"]["params"], nerf_sh/nerf/model_utils.py:60-93)."""
+# ---- one MLP stack per on-disk format ----------------------------------------------------------------------------
+# The format-neutral form of a checkpoint's parameters is {"MLP_0": [(kernel [in, out], bias [out]) per layer], ...}
+# of fp32 numpy arrays; each family (NeRF-SH here, vanilla NeRF below) is a layer count and shape list of it.
+def _mlp_names(present):
+    """MLP_0, MLP_1, ... for as long as present(name) holds"""
+    m = 0
+    while present(f"MLP_{m}"):
+        yield f"MLP_{m}"
+        m += 1
+
+
+def _from_flax(params, n_layers):
+    """{"MLP_m": {"Dense_i": {"kernel", "bias"}}} (Dense_0..Dense_{n_layers - 1}) -> the neutral form"""
+    return {mname: [(np.asarray(params[mname][f"Dense_{i}"]["kernel"], dtype=np.float32),
+                     np.asarray(params[mname][f"Dense_{i}"]["bias"], dtype=np.float32)) for i in range(n_layers)]
+            for mname in _mlp_names(params.__contains__)}
+
+
+def _to_flax(mlps):
+    return {mname: {f"Dense_{i}": {"kernel": k, "bias": b} for i, (k, b) in enumerate(layers)}
+            for mname, layers in mlps.items()}
+
+
+def _from_torch(sd, names):
+    """{"MLP_m.<name>.weight" [out, in], ".bias"} of the reference's torch twin -> the neutral form (kernel =
+    nn.Linear weight.T), one layer per entry of `names`"""
+    return {mname: [(np.asarray(sd[f"{mname}.{t}.weight"], dtype=np.float32).T.copy(),
+                     np.asarray(sd[f"{mname}.{t}.bias"], dtype=np.float32)) for t in names]
+            for mname in _mlp_names(lambda mname: f"{mname}.input_layers.0.weight" in sd)}
+
+
+def _to_torch(mlps, names):
+    return {f"{mname}.{t}.{w}": (np.ascontiguousarray(k.T) if w == "weight" else b)
+            for mname, layers in mlps.items() for t, (k, b) in zip(names, layers) for w in ("weight", "bias")}
+
+
+def _check_shapes(mlps, dims, refusal):
+    """refuses a parameter set without MLP_0 or with a layer that is not its (in, out) of `dims`;
+    refusal(mlp name, layer, (in, out), kernel, bias) is the family's message, naming the flag that sets the shape"""
+    if "MLP_0" not in mlps:
+        raise ValueError("no MLP_0 in the parameter tree")
+    for mname, layers in mlps.items():
+        for i, ((k, b), want) in enumerate(zip(layers, dims)):
+            if k.shape != want or b.shape != want[1:]:
+                raise ValueError(refusal(mname, i, want, k, b))
+    return mlps
+
+
+_POSENC_HINT = "wrong min_deg_point / max_deg_point? Dense_0 has 3 + 6 (max_deg_point - min_deg_point) rows"
+
+
+def _sh_refusal(mname, i, want, k, b):
+    hint = _POSENC_HINT if i in (0, 5) and k.shape[1:] == want[1:] else "wrong sh_deg?"
+    return f"{mname}/Dense_{i}: expected kernel {want}, got {k.shape} ({hint})"
+
+
+# ---- NeRF-SH: flat [MLP_0 | MLP_1] <-> the neutral form -----------------------------------------------------------
+def _split(flat, sh_deg, posenc):
     flat = np.asarray(flat, dtype=np.float32).reshape(-1)
     P = param_count(sh_deg, posenc)
     if flat.size % P != 0 or flat.size // P not in (1, 2):
         raise ValueError(f"expected {P} or {2 * P} parameters, got {flat.size}")
-    out = {}
+    mlps, off = {}, 0
     for m in range(flat.size // P):
-        off = m * P
-        mlp = {}
-        for i, (cin, cout) in enumerate(_dims(sh_deg, posenc)):
-            k = flat[off:off + cin * cout].reshape(cin, cout).copy()
-            off += cin * cout
-            b = flat[off:off + cout].copy()
-            off += cout
-            mlp[f"Dense_{i}"] = {"kernel": k, "bias": b}
-        out[f"MLP_{m}"] = mlp
-    return out
+        layers = []
+        for cin, cout in _dims(sh_deg, posenc):
+            layers.append((flat[off:off + cin * cout].reshape(cin, cout).copy(),
+                           flat[off + cin * cout:off + cin * cout + cout].copy()))
+            off += cin * cout + cout
+        mlps[f"MLP_{m}"] = layers
+    return mlps
+
+
+def _join(mlps, sh_deg, posenc):
+    mlps = _check_shapes(mlps, _dims(sh_deg, posenc), _sh_refusal)
+    return np.concatenate([a.reshape(-1) for layers in mlps.values() for k, b in layers for a in (k, b)]
+                          ).astype(np.float32)
+
+
+def flat_to_flax_params(flat, sh_deg, posenc=None):
+    """flat [num_mlps * P] -> {"MLP_0": {"Dense_i": {"kernel": [in,out], "bias": [out]}}, "MLP_1": ...}
+    (the pytree under ["optimizer"]["target"]["params"], nerf_sh/nerf/model_utils.py:60-93)."""
+    return _to_flax(_split(flat, sh_deg, posenc))
 
 
 def flax_params_to_flat(params, sh_deg, posenc=None):
-    parts = []
-    m = 0
-    while f"MLP_{m}" in params:
-        mlp = params[f"MLP_{m}"]
-        for i, (cin, cout) in enumerate(_dims(sh_deg, posenc)):
-            d = mlp[f"Dense_{i}"]
-            k = np.asarray(d["kernel"], dtype=np.float32)
-            b = np.asarray(d["bias"], dtype=np.float32)
-            if k.shape != (cin, cout) or b.shape != (cout,):
-                hint = ("wrong min_deg_point / max_deg_point? Dense_0 has 3 + 6 (max_deg_point - min_deg_point) rows"
-                        if i in (0, 5) and k.shape[1:] == (cout,) else "wrong sh_deg?")
-                raise ValueError(f"MLP_{m}/Dense_{i}: expected kernel {(cin, cout)}, got {k.shape} ({hint})")
-            parts += [k.reshape(-1), b]
-        m += 1
-    if m == 0:
-        raise ValueError("no MLP_0 in the parameter tree")
-    return np.concatenate(parts).astype(np.float32)
+    return _join(_from_flax(params, len(_TORCH_NAMES)), sh_deg, posenc)
 
 
 _TORCH_NAMES = [f"input_layers.{i}" for i in range(8)] + ["sigma_layer", "rgb_layer"]
@@ -90,25 +138,11 @@ _TORCH_NAMES = [f"input_layers.{i}" for i in range(8)] + ["sigma_layer", "rgb_la
 def flat_to_torch_state_dict(flat, sh_deg, posenc=None):
     """-> {"MLP_0.input_layers.0.weight": [out,in], ...} as numpy arrays: the state_dict of the reference's torch
     twin (octree/nerf/models.py:116-209, octree/nerf/model_utils.py:36-95), nn.Linear weight = kernel.T."""
-    out = {}
-    for mname, mlp in flat_to_flax_params(flat, sh_deg, posenc).items():
-        for i, tname in enumerate(_TORCH_NAMES):
-            out[f"{mname}.{tname}.weight"] = np.ascontiguousarray(mlp[f"Dense_{i}"]["kernel"].T)
-            out[f"{mname}.{tname}.bias"] = mlp[f"Dense_{i}"]["bias"]
-    return out
+    return _to_torch(_split(flat, sh_deg, posenc), _TORCH_NAMES)
 
 
 def torch_state_dict_to_flat(sd, sh_deg, posenc=None):
-    params = {}
-    m = 0
-    while f"MLP_{m}.input_layers.0.weight" in sd:
-        mlp = {}
-        for i, tname in enumerate(_TORCH_NAMES):
-            w = np.asarray(sd[f"MLP_{m}.{tname}.weight"], dtype=np.float32)
-            mlp[f"Dense_{i}"] = {"kernel": w.T, "bias": np.asarray(sd[f"MLP_{m}.{tname}.bias"], dtype=np.float32)}
-        params[f"MLP_{m}"] = mlp
-        m += 1
-    return flax_params_to_flat(params, sh_deg, posenc)
+    return _join(_from_torch(sd, _TORCH_NAMES), sh_deg, posenc)
 
 
 # ---- flax.serialization msgpack encoding -------------------------------------------------------------------------
@@ -257,16 +291,23 @@ def save_torch_ckpt(path, model):
     torch.save({"model": sd}, path)
 
 
-def restore_model_state(train_dir, model):
-    """models.restore_model_state (octree/nerf/models.py:52-63): newest *.ckpt of train_dir."""
+def _newest_torch_ckpt(train_dir):
+    """(the "model" state_dict as numpy arrays, path) of the newest *.ckpt of train_dir; (None, None) when none"""
     import torch
     paths = sorted(glob.glob(os.path.join(train_dir, "*.ckpt")))
     if not paths:
-        return None
+        return None, None
     ckpt = torch.load(paths[-1], map_location="cpu")
-    sd = {k: v.numpy() for k, v in ckpt["model"].items()}
+    return {k: v.numpy() for k, v in ckpt["model"].items()}, paths[-1]
+
+
+def restore_model_state(train_dir, model):
+    """models.restore_model_state (octree/nerf/models.py:52-63): newest *.ckpt of train_dir."""
+    sd, path = _newest_torch_ckpt(train_dir)
+    if sd is None:
+        return None
     model.set_params(torch_state_dict_to_flat(sd, model.sh_deg, _posenc_of(model)))
-    return paths[-1]
+    return path
 
 
 def restore_model_state_from_jaxnerf(train_dir, model):
@@ -282,7 +323,7 @@ def restore_model_state_from_jaxnerf(train_dir, model):
 # Dense_0..7 trunk (point posenc width W), Dense_8 raw sigma [256, 1], Dense_9 bottleneck [256, 256] (no activation),
 # Dense_10 condition layer [256 + 3 + 6 deg_view, 128] (rows [bottleneck | posenc(viewdir, 0, deg_view)]), Dense_11 rgb
 # [128, 3] (octree/nerf/model_utils.py:112-158; the rgb layer is 3 wide whatever sh_deg is, models.py:296-305).  A
-# vanilla parameter set is {"MLP_0": [(kernel [in, out], bias [out]) x 12], "MLP_1": ...} of fp32 numpy arrays.
+# vanilla parameter set is the neutral form itself, 12 layers an MLP.
 _VANILLA_TORCH_NAMES = ([f"input_layers.{i}" for i in range(8)]
                         + ["sigma_layer", "bottleneck_layer", "condition_layers.0", "rgb_layer"])
 
@@ -293,80 +334,59 @@ def vanilla_layer_dims(posenc=None, deg_view=4):
             + [(256, 1), (256, 256), (256 + 3 + 6 * int(deg_view), 128), (128, 3)])
 
 
-def _vanilla_check(mlps, posenc, deg_view):
-    dims = vanilla_layer_dims(posenc, deg_view)
-    if "MLP_0" not in mlps:
-        raise ValueError("no MLP_0 in the parameter tree")
-    for mname, layers in mlps.items():
-        for i, ((k, b), (cin, cout)) in enumerate(zip(layers, dims)):
-            if k.shape != (cin, cout) or b.shape != (cout,):
-                hint = ("wrong min_deg_point / max_deg_point? Dense_0 has 3 + 6 (max_deg_point - min_deg_point) rows"
-                        if i in (0, 5) else
-                        "wrong deg_view? Dense_10 has 256 + 3 + 6 deg_view rows" if i == 10 else
-                        "not a vanilla NeRF (net_depth_condition 1, net_width_condition 128, 3 rgb channels)?")
-                raise ValueError(f"{mname}/Dense_{i}: expected kernel {(cin, cout)} and bias ({cout},), got "
-                                 f"{k.shape} and {b.shape} ({hint})")
-    return mlps
+def _vanilla_refusal(mname, i, want, k, b):
+    hint = (_POSENC_HINT if i in (0, 5) else
+            "wrong deg_view? Dense_10 has 256 + 3 + 6 deg_view rows" if i == 10 else
+            "not a vanilla NeRF (net_depth_condition 1, net_width_condition 128, 3 rgb channels)?")
+    return (f"{mname}/Dense_{i}: expected kernel {want} and bias ({want[1]},), got {k.shape} and {b.shape} "
+            f"({hint})")
 
 
 def vanilla_from_flax_params(params, posenc=None, deg_view=4):
     """["optimizer"]["target"]["params"] of a jaxnerf checkpoint -> vanilla parameter set (Dense_0..11 in order, as
     restore_model_state_from_jaxnerf maps them: octree/nerf/models.py:66-113)."""
-    mlps = {}
-    m = 0
-    while f"MLP_{m}" in params:
-        src = params[f"MLP_{m}"]
-        layers = []
+    for mname in _mlp_names(params.__contains__):
         for i in range(12):
-            if f"Dense_{i}" not in src:
-                raise ValueError(f"MLP_{m}/Dense_{i} is missing (a vanilla NeRF has Dense_0..Dense_11)")
-            d = src[f"Dense_{i}"]
-            layers.append((np.asarray(d["kernel"], dtype=np.float32), np.asarray(d["bias"], dtype=np.float32)))
-        if "Dense_12" in src:
-            raise ValueError(f"MLP_{m}/Dense_12: net_depth_condition 1 expected (Dense_0..Dense_11)")
-        mlps[f"MLP_{m}"] = layers
-        m += 1
-    return _vanilla_check(mlps, posenc, deg_view)
+            if f"Dense_{i}" not in params[mname]:
+                raise ValueError(f"{mname}/Dense_{i} is missing (a vanilla NeRF has Dense_0..Dense_11)")
+        if "Dense_12" in params[mname]:
+            raise ValueError(f"{mname}/Dense_12: net_depth_condition 1 expected (Dense_0..Dense_11)")
+    return _check_shapes(_from_flax(params, 12), vanilla_layer_dims(posenc, deg_view), _vanilla_refusal)
 
 
-def vanilla_to_flax_params(mlps):
-    return {mname: {f"Dense_{i}": {"kernel": k, "bias": b} for i, (k, b) in enumerate(layers)}
-            for mname, layers in mlps.items()}
+vanilla_to_flax_params = _to_flax
 
 
 def vanilla_from_torch_state_dict(sd, posenc=None, deg_view=4):
     """state_dict of the reference's torch NerfModel(use_viewdirs=True) (octree/nerf/models.py:52-63) -> vanilla
     parameter set; nn.Linear weight = kernel.T."""
-    mlps = {}
-    m = 0
-    while f"MLP_{m}.input_layers.0.weight" in sd:
-        layers = []
+    for mname in _mlp_names(lambda mname: f"{mname}.input_layers.0.weight" in sd):
         for tname in _VANILLA_TORCH_NAMES:
-            key = f"MLP_{m}.{tname}.weight"
-            if key not in sd:
-                raise ValueError(f"{key} is missing (a vanilla NeRF state_dict has {', '.join(_VANILLA_TORCH_NAMES)})")
-            layers.append((np.asarray(sd[key], dtype=np.float32).T.copy(),
-                           np.asarray(sd[f"MLP_{m}.{tname}.bias"], dtype=np.float32)))
-        mlps[f"MLP_{m}"] = layers
-        m += 1
-    return _vanilla_check(mlps, posenc, deg_view)
+            if f"{mname}.{tname}.weight" not in sd:
+                raise ValueError(f"{mname}.{tname}.weight is missing (a vanilla NeRF state_dict has "
+                                 f"{', '.join(_VANILLA_TORCH_NAMES)})")
+    return _check_shapes(_from_torch(sd, _VANILLA_TORCH_NAMES), vanilla_layer_dims(posenc, deg_view),
+                         _vanilla_refusal)
 
 
 def vanilla_to_torch_state_dict(mlps):
-    return {f"{mname}.{tname}.{w}": (np.ascontiguousarray(k.T) if w == "weight" else b)
-            for mname, layers in mlps.items() for tname, (k, b) in zip(_VANILLA_TORCH_NAMES, layers)
-            for w in ("weight", "bias")}
+    return _to_torch(mlps, _VANILLA_TORCH_NAMES)
+
+
+def restore_vanilla_and_step(train_dir, is_jaxnerf_ckpt, posenc=None, deg_view=4):
+    """(the vanilla parameter set of train_dir, its step): the newest flax checkpoint_<step> (is_jaxnerf_ckpt) or
+    *.ckpt, as restore_model_state_from_jaxnerf / restore_model_state read them; the step is the flax file's (0 for
+    a torch file).  (None, None) when there is none."""
+    if is_jaxnerf_ckpt:
+        sd = restore_flax_state_dict(train_dir)
+        if sd is None:
+            return None, None
+        step = int((sd["optimizer"].get("state") or {}).get("step", 0))
+        return vanilla_from_flax_params(sd["optimizer"]["target"]["params"], posenc, deg_view), step
+    sd, _ = _newest_torch_ckpt(train_dir)
+    return (None, None) if sd is None else (vanilla_from_torch_state_dict(sd, posenc, deg_view), 0)
 
 
 def restore_vanilla(train_dir, is_jaxnerf_ckpt, posenc=None, deg_view=4):
-    """the vanilla parameter set of train_dir: the newest flax checkpoint_<step> (is_jaxnerf_ckpt) or *.ckpt, as
-    restore_model_state_from_jaxnerf / restore_model_state read them; None when there is none."""
-    if is_jaxnerf_ckpt:
-        sd = restore_flax_state_dict(train_dir)
-        return None if sd is None else vanilla_from_flax_params(sd["optimizer"]["target"]["params"], posenc, deg_view)
-    import torch
-    paths = sorted(glob.glob(os.path.join(train_dir, "*.ckpt")))
-    if not paths:
-        return None
-    ckpt = torch.load(paths[-1], map_location="cpu")
-    return vanilla_from_torch_state_dict({k: v.numpy() for k, v in ckpt["model"].items()}, posenc, deg_view)
+    """the vanilla parameter set of restore_vanilla_and_step; None when there is none."""
+    return restore_vanilla_and_step(train_dir, is_jaxnerf_ckpt, posenc, deg_view)[0]

@@ -228,6 +228,18 @@ class _Override:
 MAX_DEG_VIEW = 32
 
 
+def _check_view_branch(args, built):
+    """the view-branch flags the `built` code takes: the reference's condition branch and 0 <= deg_view <= 32"""
+    if (int(args.net_depth_condition), int(args.net_width_condition)) != (1, 128):
+        raise NotImplementedError(
+            f"net_depth_condition={args.net_depth_condition}, net_width_condition={args.net_width_condition}: the "
+            f"{built} is built for one 128-wide condition layer (1, 128)")
+    if not 0 <= int(args.deg_view) <= MAX_DEG_VIEW:
+        raise NotImplementedError(
+            f"deg_view={args.deg_view}: 0 <= deg_view <= {MAX_DEG_VIEW} expected (scales above 2^31 of a unit "
+            "direction are below the resolution of an fp32 sine's argument)")
+
+
 def check_projection_scope(args):
     """octree.extraction of a vanilla NeRF (use_viewdirs): the SH projection of its view branch
     (octree/extraction.py:217-241,362-394).  Accepts sh_deg 1-4, the reference's condition branch
@@ -243,14 +255,7 @@ def check_projection_scope(args):
         raise NotImplementedError(
             f"sh_deg={sh_deg}: projecting a vanilla NeRF needs an SH tree, 1 <= sh_deg <= 4 (with sh_deg 0 or less the "
             "reference writes projected coefficients into an RGBA tree, and sh_deg -1 fails its order >= 0 assert)")
-    if (int(args.net_depth_condition), int(args.net_width_condition)) != (1, 128):
-        raise NotImplementedError(
-            f"net_depth_condition={args.net_depth_condition}, net_width_condition={args.net_width_condition}: the "
-            "projection kernel is built for one 128-wide condition layer (1, 128)")
-    if not 0 <= int(args.deg_view) <= MAX_DEG_VIEW:
-        raise NotImplementedError(
-            f"deg_view={args.deg_view}: 0 <= deg_view <= {MAX_DEG_VIEW} expected (scales above 2^31 of a unit "
-            "direction are below the resolution of an fp32 sine's argument)")
+    _check_view_branch(args, "projection kernel")
     check_scope(_Override(args, use_viewdirs=False))
 
 
@@ -269,12 +274,5 @@ def check_vanilla_scope(args):
             f"You can only use up to one of: SH, SG or use_viewdirs (sh_deg={args.sh_deg}, sg_dim={args.sg_dim}). "
             "A vanilla NeRF is rendered with sh_deg -1: --config nerf_sh/config/misc/og_nerf; misc/proj (sh_deg 4) "
             "is the config of octree.extraction's SH projection of that model")
-    if (int(args.net_depth_condition), int(args.net_width_condition)) != (1, 128):
-        raise NotImplementedError(
-            f"net_depth_condition={args.net_depth_condition}, net_width_condition={args.net_width_condition}: the "
-            "vanilla forward is built for one 128-wide condition layer (1, 128)")
-    if not 0 <= int(args.deg_view) <= MAX_DEG_VIEW:
-        raise NotImplementedError(
-            f"deg_view={args.deg_view}: 0 <= deg_view <= {MAX_DEG_VIEW} expected (scales above 2^31 of a unit "
-            "direction are below the resolution of an fp32 sine's argument)")
+    _check_view_branch(args, "vanilla forward")
     check_scope(_Override(args, use_viewdirs=False))

@@ -13,7 +13,7 @@ tensor cores read.  Inference only: training a vanilla NeRF stays refused (flags
 import numpy as np
 import torch
 
-from .._lib import PREC_FP16, RenderConfig, ViewBranch, check, lib, posenc_ref, posenc_struct, ptr, stream_ptr
+from .._lib import PREC_FP16, ViewBranch, check, lib, posenc_ref, ptr, stream_ptr
 from .models import RaySampler, _cuda_f32, ctypes_ref
 
 POINTS_PER_CALL = 1 << 20        # points per pob_eval_points_vanilla call (a 512 MB view table)
@@ -35,6 +35,18 @@ def folded_flat(layers):
     return np.concatenate(parts)
 
 
+def view_branch(name, layers, deg_view, device):
+    """the view-branch arrays of one vanilla MLP on the device: (W10_e [3 + 6 deg_view, 128], c [128], W11 [128, 3],
+    b11 [3]), c = b9 W10_b + b10 (fold_view_branch).  A Dense_10 whose rows do not match deg_view is refused before
+    anything is uploaded: the kernels read 3 + 6 deg_view rows of W10_e."""
+    w10e = np.asarray(layers[10][0], dtype=np.float32)[256:]
+    if w10e.shape[0] != 3 + 6 * int(deg_view):
+        raise ValueError(f"{name}/Dense_10 has {256 + w10e.shape[0]} input rows, deg_view={deg_view} "
+                         f"needs {256 + 3 + 6 * int(deg_view)}")
+    dev = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).to(device)   # noqa: E731
+    return dev(w10e), dev(fold_view_branch(layers)[1]), dev(layers[11][0]), dev(layers[11][1])
+
+
 class VanillaNerfModel(RaySampler):
     """The reference's NerfModel with use_viewdirs (coarse MLP_0, fine MLP_1) on the device.  `mlps` is a vanilla
     parameter set {"MLP_0": [(kernel, bias) x 12], "MLP_1": ...} (checkpoints.vanilla_from_flax_params /
@@ -43,60 +55,36 @@ class VanillaNerfModel(RaySampler):
     def __init__(self, mlps, deg_view=4, num_coarse_samples=64, num_fine_samples=128, near=2.0, far=6.0,
                  white_bkgd=True, lindisp=False, max_rays=4096, device="cuda", noise_std=None, sigma_activation="relu",
                  min_deg_point=0, max_deg_point=10, legacy_posenc_order=False, net_activation="relu"):
-        from .flags import MAX_DEG_VIEW, check_posenc, check_samples, net_activation_code, sigma_activation_code
-        check_samples(num_coarse_samples, num_fine_samples)
+        from .flags import MAX_DEG_VIEW, check_posenc
         check_posenc(min_deg_point, max_deg_point)
         if not 0 <= int(deg_view) <= MAX_DEG_VIEW:
             raise ValueError(f"deg_view={deg_view}: 0 <= deg_view <= {MAX_DEG_VIEW} expected")
-        self.sh_deg = -1
+        super().__init__(-1, num_coarse_samples, num_fine_samples, near, far, white_bkgd, lindisp, max_rays, 0, device,
+                         noise_std, sigma_activation, min_deg_point, max_deg_point, legacy_posenc_order,
+                         net_activation)
         self.precision = PREC_FP16
-        self.posenc = (int(min_deg_point), int(max_deg_point), bool(legacy_posenc_order))
         self.deg_view = int(deg_view)
-        self.net_act_code = net_activation_code(net_activation)
-        self.sigma_act_code = sigma_activation_code(sigma_activation)
-        self._pe = posenc_struct(self.posenc, self.net_act_code)
-        self.num_coarse_samples = int(num_coarse_samples)
-        self.num_fine_samples = int(num_fine_samples)
-        self.num_mlps = 2 if self.num_fine_samples > 0 else 1
-        self.near, self.far = float(near), float(far)
-        self.white_bkgd = bool(white_bkgd)
-        self.lindisp = bool(lindisp)
-        self.max_rays = int(max_rays)
-        self.noise_std = noise_std
-        self.device = torch.device(device)
         self.step = None
         names = [f"MLP_{i}" for i in range(self.num_mlps)]
         missing = [n for n in names if n not in mlps]
         if missing:
             raise ValueError(f"the parameter set has no {missing[0]} (num_fine_samples={self.num_fine_samples} "
                              f"needs {' and '.join(names)})")
-        dev = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).to(self.device)   # noqa: E731
         nb = int(lib.pob_vanilla_packed_bytes())
         self.blobs, self._view_arrays = [], []
         self.view = ViewBranch()
         self.view.deg_view = self.deg_view
         for i, name in enumerate(names):
-            layers = mlps[name]
-            flat = dev(folded_flat(layers))
-            if flat.numel() != int(lib.pob_vanilla_param_count(posenc_ref(self._pe))):
+            flat = torch.from_numpy(folded_flat(mlps[name])).to(self.device)
+            if flat.numel() != int(lib.pob_vanilla_param_count(posenc_ref(self._posenc_struct))):
                 raise ValueError(f"{name}: Dense_0..Dense_8 do not match the point encoder {self.posenc}")
             blob = torch.zeros(nb, dtype=torch.uint8, device=self.device)
-            check(lib.pob_pack_vanilla(ptr(flat), posenc_ref(self._pe), ptr(blob), stream_ptr()))
-            _, c = fold_view_branch(layers)
-            arrays = (dev(layers[10][0][256:]), dev(c), dev(layers[11][0]), dev(layers[11][1]))
-            if arrays[0].shape[0] != 3 + 6 * self.deg_view:
-                raise ValueError(f"{name}/Dense_10 has {256 + arrays[0].shape[0]} input rows, deg_view={self.deg_view} "
-                                 f"needs {256 + 3 + 6 * self.deg_view}")
+            check(lib.pob_pack_vanilla(ptr(flat), posenc_ref(self._posenc_struct), ptr(blob), stream_ptr()))
+            arrays = view_branch(name, mlps[name], self.deg_view, self.device)
             m = self.view.mlp[i]
             m.w10e_dev, m.c_dev, m.w11_dev, m.b11_dev = (ptr(a) for a in arrays)
             self.blobs.append(blob)
             self._view_arrays.append(arrays)   # keeps the descriptor's arrays alive
-        self.cfg = RenderConfig(-1, self.num_coarse_samples, self.num_fine_samples, int(self.white_bkgd),
-                                self.max_rays, 0)
-        self.cfg.sigma_activation = self.sigma_act_code
-        self.cfg.posenc = posenc_ref(self._pe)
-        self._ws = None
-        self._init_depths()
 
     @classmethod
     def from_flags(cls, args, *, max_rays, device="cuda"):
@@ -105,56 +93,35 @@ class VanillaNerfModel(RaySampler):
         checkpoint's step (0 for a torch file)."""
         from . import checkpoints
         pe = (int(args.min_deg_point), int(args.max_deg_point), bool(args.legacy_posenc_order))
-        sd = checkpoints.restore_flax_state_dict(args.train_dir)
-        if sd is not None:
-            mlps = checkpoints.vanilla_from_flax_params(sd["optimizer"]["target"]["params"], pe, args.deg_view)
-            step = int((sd["optimizer"].get("state") or {}).get("step", 0))
+        for jaxnerf in (True, False):
+            mlps, step = checkpoints.restore_vanilla_and_step(args.train_dir, jaxnerf, pe, args.deg_view)
+            if mlps is not None:
+                break
         else:
-            mlps = checkpoints.restore_vanilla(args.train_dir, False, pe, args.deg_view)
-            step = 0
-        if mlps is None:
             raise ValueError(f"no checkpoint_* or *.ckpt in {args.train_dir}")
-        model = cls(mlps, deg_view=args.deg_view, num_coarse_samples=args.num_coarse_samples,
-                    num_fine_samples=args.num_fine_samples, near=args.near, far=args.far, white_bkgd=args.white_bkgd,
-                    lindisp=args.lindisp, max_rays=max_rays, device=device, noise_std=args.noise_std,
-                    sigma_activation=args.sigma_activation, min_deg_point=args.min_deg_point,
-                    max_deg_point=args.max_deg_point, legacy_posenc_order=args.legacy_posenc_order,
-                    net_activation=args.net_activation)
+        model = cls(mlps, deg_view=args.deg_view, max_rays=max_rays, device=device, noise_std=args.noise_std,
+                    **cls.flag_kwargs(args))
         model.step = step
         return model
 
-    def workspace(self):
-        if self._ws is None:
-            n = int(lib.pob_vanilla_workspace_bytes(ctypes_ref(self.cfg)))
-            if n < 0:
-                check(1)
-            self._ws = torch.empty(n, dtype=torch.uint8, device=self.device)
-        return self._ws
+    @property
+    def _pe(self):
+        """the encoder descriptor (RaySampler._posenc_struct), by the name the projection's VanillaNerf gives it"""
+        return self._posenc_struct
 
-    def __call__(self, rays, randomized=False, t_rand=None, u=None, z_fine=None, sigma_noise=None, precision=None):
-        """NerfModel.__call__ -> [(rgb_coarse, disp_coarse, acc_coarse), (rgb, disp, acc)] for up to max_rays rays
-        (the arguments of NerfModel.__call__; precision must be None or PREC_FP16)."""
+    def workspace(self):
+        return self._workspace(None, lambda: lib.pob_vanilla_workspace_bytes(ctypes_ref(self.cfg)))
+
+    def _precision(self, precision):
         if precision not in (None, PREC_FP16):
             raise ValueError("the vanilla forward is fp16 (PREC_FP16)")
-        o = _cuda_f32(rays.origins, "rays.origins", 3)
-        d = _cuda_f32(rays.directions, "rays.directions", 3)
-        v = _cuda_f32(rays.viewdirs, "rays.viewdirs", 3)
-        n = o.shape[0]
-        if n > self.max_rays:
-            raise ValueError(f"{n} rays exceed max_rays={self.max_rays}; chunk the call (utils.render_image)")
-        t_rand, u, upr = self._uniforms(n, randomized, t_rand, u)
-        z_fine = None if z_fine is None else _cuda_f32(z_fine, "z_fine")   # keep alive until the launch
-        noise = self._set_sigma_noise(n, randomized, sigma_noise)           # noqa: F841  (same)
-        out_c = torch.empty((n, 5), dtype=torch.float32, device=self.device)
-        out_f = torch.empty((n, 5), dtype=torch.float32, device=self.device) if self.num_mlps == 2 else None
+        return PREC_FP16
+
+    def _render(self, o, d, v, n, t_rand, u, upr, z_fine, out_c, out_f, precision):
         check(lib.pob_render_rays_vanilla(ctypes_ref(self.cfg), ctypes_ref(self.view), ptr(self.blobs[0]),
                                           ptr(self.blobs[1]) if self.num_mlps == 2 else None, ptr(o), ptr(d), ptr(v),
                                           n, ptr(self.z_base), ptr(t_rand), ptr(u), upr, ptr(z_fine), ptr(out_c),
-                                          ptr(out_f), ptr(self.workspace()), PREC_FP16, stream_ptr()))
-        ret = [(out_c[:, :3], out_c[:, 3], out_c[:, 4])]
-        if out_f is not None:
-            ret.append((out_f[:, :3], out_f[:, 3], out_f[:, 4]))
-        return ret
+                                          ptr(out_f), ptr(self.workspace()), precision, stream_ptr()))
 
     def _points(self, points, viewdirs, coarse, raw):
         p = _cuda_f32(points, "points", 3)
@@ -174,8 +141,8 @@ class VanillaNerfModel(RaySampler):
             rgb = sigma = None
         for i in range(0, m, POINTS_PER_CALL):
             j = min(m, i + POINTS_PER_CALL)
-            check(lib.pob_eval_points_vanilla(ptr(self.blobs[mlp]), posenc_ref(self._pe), ctypes_ref(self.view), mlp,
-                                              ptr(p[i:j]), ptr(v[i:j]), j - i, ptr(table),
+            check(lib.pob_eval_points_vanilla(ptr(self.blobs[mlp]), posenc_ref(self._posenc_struct),
+                                              ctypes_ref(self.view), mlp, ptr(p[i:j]), ptr(v[i:j]), j - i, ptr(table),
                                               ptr(rgb[i:j]) if raw else None, ptr(sigma[i:j]) if raw else None,
                                               None if raw else ptr(out[i:j]), self.sigma_act_code, stream_ptr()))
         return (rgb, sigma) if raw else (out[:, :3], out[:, 3:4])

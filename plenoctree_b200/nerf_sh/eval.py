@@ -10,7 +10,7 @@ import numpy as np
 import torch
 from absl import app
 
-from ..nerf import checkpoints, datasets, flags as F, models, utils, vanilla
+from ..nerf import datasets, flags as F, models, utils
 
 FLAGS = F.FLAGS
 F.define_flags()
@@ -19,21 +19,10 @@ F.define_flags()
 def main(unused_argv):
     F.update_flags(FLAGS)
     F.check_flags(FLAGS)
-    if FLAGS.use_viewdirs:          # a vanilla NeRF (--config nerf_sh/config/misc/og_nerf)
-        F.check_vanilla_scope(FLAGS)
-    else:
-        F.check_scope(FLAGS)
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
     torch.cuda.set_device(dev)
+    model, step = models.load_for_inference(FLAGS, dev, max_rays=min(FLAGS.chunk, 8192))
     dataset = datasets.get_dataset("test", FLAGS, device=dev)
-    if FLAGS.use_viewdirs:
-        model = vanilla.VanillaNerfModel.from_flags(FLAGS, max_rays=min(FLAGS.chunk, 8192), device=dev)
-        step = model.step
-    else:
-        model, state = models.get_model_state(FLAGS, device=dev, restore=False, max_rays=min(FLAGS.chunk, 8192))
-        step = checkpoints.restore_checkpoint(FLAGS.train_dir, model, state)
-        if step is None:
-            raise ValueError(f"no checkpoint_* in {FLAGS.train_dir}")
     out_dir = os.path.join(FLAGS.train_dir, "path_renders" if FLAGS.render_path else "test_preds")   # eval.py:63-65
     if FLAGS.save_output:
         os.makedirs(out_dir, exist_ok=True)

@@ -10,7 +10,7 @@ import numpy as np
 from absl import app, flags
 
 from .. import _dist
-from ..nerf import checkpoints, flags as F, models, utils, vanilla
+from ..nerf import flags as F, models, utils
 from ..nerf.models import Rays
 from ..nerf.rays import generate_rays, pose_spherical
 from ..nerf.utils import write_video
@@ -42,11 +42,8 @@ def orbit_poses(num_views, elevation, radius, up_axis):
 def main(unused_argv):
     F.update_flags(FLAGS)
     F.check_flags(FLAGS, require_data=False)
-    if FLAGS.use_viewdirs:          # a vanilla NeRF (--config nerf_sh/config/misc/og_nerf)
-        F.check_vanilla_scope(FLAGS)
-    else:
-        F.check_scope(FLAGS)
     rank, world, dev = _dist.dist_init()
+    model, _ = models.load_for_inference(FLAGS, dev, max_rays=min(FLAGS.chunk, 8192))
     render_poses = orbit_poses(FLAGS.num_views, FLAGS.elevation, float(FLAGS.radius), FLAGS.up_axis)
     if FLAGS.write_poses and rank == 0:
         np.savetxt(FLAGS.write_poses, render_poses.reshape(-1, 4))
@@ -55,12 +52,6 @@ def main(unused_argv):
     if FLAGS.intrin is not None:
         K = np.loadtxt(FLAGS.intrin)
         focal = (K[0, 0] + K[1, 1]) * 0.5
-    if FLAGS.use_viewdirs:
-        model = vanilla.VanillaNerfModel.from_flags(FLAGS, max_rays=min(FLAGS.chunk, 8192), device=dev)
-    else:
-        model, state = models.get_model_state(FLAGS, device=dev, restore=False, max_rays=min(FLAGS.chunk, 8192))
-        if checkpoints.restore_checkpoint(FLAGS.train_dir, model, state) is None:
-            raise ValueError(f"no checkpoint_* in {FLAGS.train_dir}")
     video_dir = os.path.join(FLAGS.train_dir, "video", "e{:03}".format(int(-FLAGS.elevation * 10)))
     frames_dir = os.path.join(video_dir, "frames")
     if rank == 0:

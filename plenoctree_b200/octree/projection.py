@@ -21,7 +21,7 @@ import torch
 
 from .._lib import NET_RELU, PREC_FP16, check, lib, posenc_ref, posenc_struct, ptr, stream_ptr
 from .. import ops
-from ..nerf.vanilla import fold_view_branch
+from ..nerf.vanilla import fold_view_branch, view_branch
 
 PROJ_SEED = 20200823
 CELLS_PER_BLOCK = 1024          # leaves sharing one direction set
@@ -45,17 +45,14 @@ class VanillaNerf:
         if num_fine_samples > 0 and "MLP_1" not in mlps:
             raise ValueError("num_fine_samples > 0 but the checkpoint has no MLP_1 (eval_points_raw evaluates the fine "
                              "MLP of a model with a fine level)")
-        layers = mlps["MLP_1"] if num_fine_samples > 0 else mlps["MLP_0"]
-        trunk = [np.asarray(a, dtype=np.float32) for k, b in layers[:9] for a in (k, b)]
-        k11, b11 = layers[11]
-        dev = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).to(self.device)
-        head_w, head_b = fold_view_branch(layers)
-        self.head_w = dev(head_w)                           # [256, 128]
-        self.head_b = dev(head_b)                           # [128]
-        flat = np.concatenate([a.reshape(-1) for a in trunk] + [np.zeros(256 * 3 + 3, np.float32)])
+        name = "MLP_1" if num_fine_samples > 0 else "MLP_0"
+        layers = mlps[name]
+        # head_b = c = b9 W10_b + b10: the bias a_p carries
+        self.w10e, self.head_b, self.w11, self.b11 = view_branch(name, layers, self.deg_view, self.device)
+        self.head_w = torch.from_numpy(fold_view_branch(layers)[0].astype(np.float32)).to(self.device)   # [256, 128]
+        flat = np.concatenate([np.asarray(a, dtype=np.float32).reshape(-1) for k, b in layers[:9] for a in (k, b)]
+                              + [np.zeros(256 * 3 + 3, np.float32)])
         self.sigma_blob = ops.pack_weights(torch.from_numpy(flat).to(self.device), -1, posenc=self.posenc)
-        self.w10e = dev(np.asarray(layers[10][0], dtype=np.float32)[256:])   # [3 + 6 deg_view, 128]
-        self.w11, self.b11 = dev(k11), dev(b11)
         self._ws = None
         self._pe = posenc_struct(self.posenc)
 

@@ -124,6 +124,21 @@ def test_missing_fine_mlp_and_too_many_blocks_are_refused():
     assert _lib.lib.pob_sh_proj_points_workspace_bytes(1) > _lib.lib.pob_sh_proj_points_workspace_bytes(0)
 
 
+def test_mismatched_deg_view_is_refused_before_upload(monkeypatch):
+    """VanillaNerf checks Dense_10's rows against deg_view (pob_sh_proj_directions reads 3 + 6 deg_view rows of
+    W10_e) before it uploads or packs anything"""
+    from plenoctree_b200.octree import projection as P
+    mlps = {"MLP_0": PJ.init_params(1), "MLP_1": PJ.init_params(2)}              # deg_view 4: 283 rows
+
+    def no_upload(*a, **k):
+        raise AssertionError("uploaded before the Dense_10 check")
+    monkeypatch.setattr(torch.Tensor, "to", no_upload)
+    monkeypatch.setattr(P.ops, "pack_weights", no_upload)
+    for nfs, name in ((0, "MLP_0"), (128, "MLP_1")):
+        with pytest.raises(ValueError, match=f"{name}/Dense_10 has 283 input rows, deg_view=5 needs 289"):
+            P.VanillaNerf(mlps, deg_view=5, num_fine_samples=nfs)
+
+
 def test_oracle_reproduces_the_executed_reference(golden_dir):
     z = np.load(os.path.join(golden_dir, "ref_projection.npz"))
     layers = PJ.init_params(int(z["seeds"][1]))                  # MLP_1: eval_points_raw's fine MLP
