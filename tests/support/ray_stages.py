@@ -2,7 +2,7 @@
 import numpy as np
 import torch
 
-from tests.support.mlp_stages import Case, _params
+from tests.support.mlp_stages import Case
 from tests.support.records import record
 
 
@@ -483,12 +483,12 @@ def sample_coarse_bit_exact(N, lindisp):
 
 
 class RayCase(Case):
-    """a training call of test_train_stages.py, plus background, lindisp, per-ray direction scale, a call over fewer
-    rays than max_rays and the precision"""
+    """a training call of test_train_stages.py, plus a per-ray direction scale and a call over fewer rays than
+    max_rays"""
 
-    def __init__(self, *a, white=True, lindisp=False, dir_scale=False, n_call=None, precision=1, **k):
+    def __init__(self, *a, dir_scale=False, n_call=None, **k):
         super().__init__(*a, **k)
-        self.white, self.lindisp, self.dir_scale, self.n_call, self.precision = white, lindisp, dir_scale, n_call, precision
+        self.dir_scale, self.n_call = dir_scale, n_call
 
     @property
     def name(self):
@@ -501,14 +501,6 @@ class RayCase(Case):
         if self.dir_scale:
             d = (d * np.random.RandomState(self.seed + 2).uniform(0.3, 3, (n, 1))).astype(np.float32)
         return (o, d, v, px), t_rand, u, sp, noise
-
-    def model(self, max_rays=None):
-        from plenoctree_b200.nerf.models import NerfModel
-        m = NerfModel(sh_deg=self.sh, num_coarse_samples=self.nc, num_fine_samples=self.nf, white_bkgd=self.white,
-                      lindisp=self.lindisp, max_rays=max_rays or self.R, sparsity_npoints=self.nsp)
-        fc, ff = _params(self.sh, self.seed)
-        m.set_params(np.concatenate([fc, ff]) if self.nf else fc)
-        return m
 
 
 def _check_levels(model, views, ws, rays, z_base, t_rand, u, upr, st, px=None, gscale=None):
@@ -557,10 +549,9 @@ def _check_levels(model, views, ws, rays, z_base, t_rand, u, upr, st, px=None, g
 
 
 def _in_call(case):
-    from tests.support.mlp_x3 import _run
     model = case.model()
     n = case.n_call or case.R
-    state, _ = _run(case, model, case.precision, n=n, fill=0xFF)
+    state, _ = case.run(model, n=n, fill=0xFF)
     return _in_call_checks(case, model, state, n)
 
 

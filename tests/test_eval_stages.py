@@ -24,8 +24,8 @@ import torch
 from plenoctree_b200 import layouts as L
 from tests.support.eval_stages import (CHUNK, M_RAGGED, X3Ref, X3_ALLOW, _blob, _cell_bound, _cells, _grid,
                                        _heads_params, _level_rows, _nbits, _raw, _raw_of_heads, _rgbs, _x3_errors)
-from tests.support.mlp_stages import (CASES, Case, FWD_ALLOW, SENSITIVITY, Stats, U24, _assert_stages, _check_all,
-                                      _sh_basis)
+from tests.support.mlp_stages import (CASES, FP16, FWD_ALLOW, SENSITIVITY, Case, Stats, U24, _sh_basis, assert_stages,
+                                      check_call)
 from tests.support.records import record
 
 # Sensitivity classes that cannot reach SENSITIVITY x X3_ALLOW; their ratios are recorded, and only that the perturbed
@@ -35,7 +35,7 @@ from tests.support.records import record
 # one weight slot's lo part [9.7 .. 13.7], one posenc unit's lo part [7.4 .. 13.8], the heads bias's lo part (a 2^-12
 # relative change of a bias of ~0.05) [1.6 .. 4.8].  The heads in a single fp16 pass reach [32 .. 48] and are asserted.
 X3_SENS_UNASSERTED = ("trunk_slot_hi_hi", "weight_slot_lo_dropped", "posenc_unit_lo_dropped", "heads_bias_hi_only")
-EPI_ABS = 2.0 ** -21        # rgb epilogue: expf + division, absolute (as in test_train_stages._check_level)
+EPI_ABS = 2.0 ** -21        # rgb epilogue: expf + division, absolute (as in mlp_stages.check_level)
 CELL_S = (1, 5, 32, 33, 96, 128, 256, 384)
 
 
@@ -60,7 +60,7 @@ def _m_many_tiles():
 
 def _rgb_check(rgb, raw_rgb, hm_rgb, vd, sh, allow):
     """the heads epilogue from the GPU's own OUT_RAW values: max of |rgb - sigmoid(sum_k Y_k raw_ck)| over its allowance
-    (test_train_stages._check_level: sigmoid slope 1/4 times the GEMM allowance plus 4 ulps of each coefficient, plus
+    (mlp_stages.check_level: sigmoid slope 1/4 times the GEMM allowance plus 4 ulps of each coefficient, plus
     EPI_ABS for expf and the division).  raw_rgb / hm_rgb channel-major [n, 3K] fp64."""
     n, K = raw_rgb.shape[0], L.K_of(sh)
     Y = _sh_basis(sh, vd.double()) if sh >= 0 else torch.ones(n, 1, dtype=torch.float64, device=vd.device)
@@ -93,7 +93,7 @@ def _fp16_vs_training(case, check_stages=False):
     state, ctx = case.run(model, fill=0xFF)
     res = {}
     if check_stages:
-        res = _check_all(case, model, state, ctx, case.nsp > 0)
+        res = check_call(model, state, ctx, FP16)
     n = ctx["n"]
     ws = model.workspace(True)
     tv = L.train_workspace_views(model.cfg, n, case.nsp > 0)
@@ -154,20 +154,20 @@ def _fp16_vs_training(case, check_stages=False):
             es = (raw_sig[r0:r1].double() - rs).abs() / (U24 * ms)
             st.max("raw_heads_excess", max(float(er.max()), float(es.max())))
             st.max("rgbs_from_raw_excess", _rgb_check(got[r0:r1, :3], raw_rgb[r0:r1].double(), mr, vd[r0:r1],
-                                                      case.sh, FWD_ALLOW))
+                                                      case.sh, FWD_ALLOW[FP16]))
         out[f"MLP_{i}"] = dict(fp16=st.d, M=M)
     res["wall_s"] = time.time() - t0
     _record(case.name, {k: v for k, v in res.items()})
     for k, r in out.items():
         _record(f"{case.name}:{k}", r)
     if check_stages:
-        _assert_stages({k: v for k, v in res.items() if k.startswith("MLP")})
+        assert_stages({k: v for k, v in res.items() if k.startswith("MLP")}, FP16, "relu")
     for k, r in out.items():
         s = r["fp16"]
         for key, val in s.items():
             if key.endswith("mismatches"):
                 assert val == 0, (case.name, k, key, val)
-        assert s["raw_heads_excess"] <= FWD_ALLOW, (case.name, k, s["raw_heads_excess"])
+        assert s["raw_heads_excess"] <= FWD_ALLOW[FP16], (case.name, k, s["raw_heads_excess"])
         assert s["rgbs_from_raw_excess"] <= 1.0, (case.name, k, s["rgbs_from_raw_excess"])
 
 
@@ -289,7 +289,7 @@ def test_point_forwards_shapes(sh, radius):
         st.max("fp16_raw_heads_excess", max(float(((raw16[a:b].double() - rr).abs() / (U24 * mr)).max()),
                                             float(((sig16[a:b].double() - rs_).abs() / (U24 * ms)).max())))
         st.max("fp16_rgbs_from_raw_excess", _rgb_check(got16[a:b, :3], raw16[a:b].double(), mr, vd0[a:b], sh,
-                                                       FWD_ALLOW))
+                                                       FWD_ALLOW[FP16]))
 
     # fp16x3 against fp64: OUT_RAW, OUT_SIGMA, OUT_RGBS at random view directions
     ref = X3Ref(model.params.cpu().numpy(), sh, dev)
@@ -330,7 +330,7 @@ def test_point_forwards_shapes(sh, radius):
     for key, val in s.items():
         if key.endswith("mismatches"):
             assert val == 0, (key, val)
-    assert s["fp16_raw_heads_excess"] <= FWD_ALLOW, s["fp16_raw_heads_excess"]
+    assert s["fp16_raw_heads_excess"] <= FWD_ALLOW[FP16], s["fp16_raw_heads_excess"]
     assert s["fp16_rgbs_from_raw_excess"] <= 1.0, s["fp16_rgbs_from_raw_excess"]
     assert s["x3_points_excess"] <= X3_ALLOW, s["x3_points_excess"]
     assert s["x3_rgbs_from_raw_excess"] <= 1.0, s["x3_rgbs_from_raw_excess"]

@@ -10,7 +10,7 @@ one-block-per-ray compositing backward (N > 256), a smooth trunk under the softp
 CPU: the matrix's covering properties, the forward / data-gradient instantiations each entry point reaches, and the
 anchor of the fp64 inference reference to the golden-anchored oracles.
 GPU, per row: one training call on a 0xFF-filled workspace, every level's stages against fp64 from the kernels' own
-saved tiles (test_net_activation._check_level) and the per-ray stages (test_ray_stages), each checked again against
+saved tiles (tests/support/mlp_stages.py: check_level) and the per-ray stages (test_ray_stages), each checked again against
 the reference of a wrong flag (mutation guards), and the inference forwards of the fine MLP with the same flags.
 Once: a CUDA-graph replay of a row with every flag away from its default.
 """
@@ -212,36 +212,30 @@ def test_reference_anchor_trunk(act):
 
 def _row_case(row):
     prec, act, pe, dens, sh, (R, nc, nf, nsp), noise, white = row
-    return RayCase(sh, R, nc, nf, nsp, noise=noise, white=white, precision=1 if prec == "fp16" else X3)
-
-
-def _row_model(row):
-    from tests.support.model_flags import _make_model
-    prec, act, pe, dens = row[:4]
-    return _make_model(_row_case(row), act, pe=pe, sigma_act=dens)
+    return RayCase(sh, R, nc, nf, nsp, noise=noise, white=white, precision=1 if prec == "fp16" else X3, act=act, pe=pe,
+                   sigma_act=dens, centre=True)
 
 
 def _check_row(row):
     from plenoctree_b200 import ops
     from plenoctree_b200.nerf.models import Rays
-    from tests.support import model_flags as NT
     from tests.support import ray_stages as RS
     from tests.support.eval_stages import X3Ref, _cell_bound, _level_rows, _nbits, _x3_errors
-    from tests.support.mlp_x3 import _run
+    from tests.support.mlp_stages import check_call
     prec, act, pe, dens, sh = row[:5]
     case = _row_case(row)
     x3 = case.precision == X3
     dev = torch.device("cuda")
-    model = _row_model(row)
+    model = case.model()
     n = case.R
-    state, ctx = _run(case, model, case.precision, fill=0xFF)
+    state, ctx = case.run(model, fill=0xFF)
     called = set()
 
     # ---- stage checks, and each again against the reference of a wrong flag
     alt = {"act": "softplus" if act == "relu" else "relu", "sigma_act": "softplus" if dens == "relu" else "relu"}
     if _alt_pe(pe) is not None:
         alt["pe"] = _alt_pe(pe)
-    res = NT._check_call(model, state, ctx, case.precision, act, pe, dens, alt)
+    res = check_call(model, state, ctx, case.precision, alt)
     called.add("train")
     rays = RS._in_call_checks(case, model, state, n)
     out = {"stages": res, "rays": rays, "alt": dict(alt), "guard_pe_skipped": "pe" not in alt}
@@ -320,17 +314,15 @@ def _check_row(row):
 
 def _assert_row(row, out):
     from tests.support import ray_stages as RS
-    from tests.support import mlp_stages as TS
-    from tests.support import mlp_x3 as TX
     from tests.support.eval_stages import X3_ALLOW
-    from tests.support.model_flags import SIN_X3_ALLOW, _assert_call
+    from tests.support.mlp_stages import BWD_ALLOW, FWD_ALLOW, SIN_ALLOW, assert_stages
     from tests.support.ray_stages import GW_BAR
     prec, act, pe, dens = row[:4]
     x3 = prec == "fp16x3"
-    _assert_call(out["stages"], X3 if x3 else 1, act)
+    precision = X3 if x3 else 1
+    assert_stages(out["stages"], precision, act, guard=False)
     RS._assert_in_call(out["rays"])
-    fwd_allow, bwd_allow = (TX.FWD_ALLOW, TX.BWD_ALLOW) if x3 else (TS.FWD_ALLOW, TS.BWD_ALLOW)
-    sin_bar = SIN_X3_ALLOW if x3 else 1.0
+    fwd_allow, bwd_allow, sin_bar = FWD_ALLOW[precision], BWD_ALLOW[precision], SIN_ALLOW[precision]
     for mlp, r in out["stages"].items():
         s = r["stages"]
         g_fwd = min(s[f"guard_fwd_l{l}"] for l in range(8))
@@ -368,10 +360,9 @@ def test_graph_replay_with_every_flag_non_default():
     from plenoctree_b200.nerf import train as T
     from plenoctree_b200.nerf.models import NerfModel, Rays
     from plenoctree_b200.nerf.rays import random_rays_np
-    from tests.support.model_flags import _centre_sigma
-    from tests.support.model_flags import _gpu_params
+    from tests.support.mlp_stages import _centre_sigma, params
     pe, sh, R = (2, 8, True), 2, 256
-    fc, ff = _gpu_params(pe, sh, 33)
+    fc, ff = params(sh, 33, pe)
     for f in (fc, ff):
         _centre_sigma(f, sh, "elu", pe)
     o, d, v, px = random_rays_np(R, 33)

@@ -340,15 +340,14 @@ def test_ray_stages_in_training_call_long(precision):
 @pytest.mark.gpu
 def test_mlp_stages_in_training_call_long():
     """test_train_stages.py's stage checks of the saving forward, data and weight gradients at (128, 384)"""
-    from tests.support.mlp_stages import Case, _stage_case
-    _stage_case(Case(3, 40, 128, 384, 200))
+    from tests.support.mlp_stages import Case, stage_case
+    stage_case(Case(3, 40, 128, 384, 200), functools.partial(record, "parity_train_stages.json"))
 
 
 @pytest.mark.gpu
 def test_mlp_stages_in_training_call_long_x3():
-    from tests.support.mlp_stages import Case
-    from tests.support.mlp_x3 import _stage_case_x3
-    _stage_case_x3(Case(3, 40, 128, 384, 200))
+    from tests.support.mlp_stages import X3, Case, stage_case
+    stage_case(Case(3, 40, 128, 384, 200, precision=X3), functools.partial(record, "parity_train_x3.json"), guard=False)
 
 
 @pytest.mark.gpu
@@ -430,9 +429,9 @@ def test_graphed_train_step_matches_eager_long():
     from plenoctree_b200.nerf import train as T
     from plenoctree_b200.nerf.models import NerfModel, Rays
     from plenoctree_b200.nerf.rays import random_rays_np
-    from tests.support.mlp_stages import _params
+    from tests.support.mlp_stages import params
     R = 256
-    fc, ff = _params(3, 33)
+    fc, ff = params(3, 33)
     o, d, v, px = random_rays_np(R, 33)
     b12 = torch.from_numpy(np.concatenate([o, d, v, px], axis=1)).cuda()
     lrs = [5e-4, 4e-4, 3e-4]

@@ -9,6 +9,7 @@ existing allowance: f is 1-Lipschitz, so the pre-activation's fp32 accumulation 
 The data gradient is held to fp64 dH_l * f'(h_l), with f' formed in fp64 from the kernel's saved h_l.
 """
 import ctypes
+import functools
 import os
 
 import numpy as np
@@ -17,7 +18,9 @@ import torch
 
 from plenoctree_b200 import layouts as L
 from oracle import net_activation_oracle as NA
-from tests.support.model_flags import X3, _act64, _centre_sigma, _make_model, _record, _scope_args, _stage_case
+from tests.support.mlp_stages import BWD_ALLOW, CASES, FP16, X3, Case, _centre_sigma, operands, stage_case
+from tests.support.model_flags import _act64, _scope_args
+from tests.support.records import record
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
@@ -30,6 +33,8 @@ WG_EPS_W_PRODUCTION = 1e-3
 # fp16x3 whole gradient of a softplus trunk against fp64, relative L2 (test_gradient_vs_fp64_oracle): [1.0e-4, against
 # the fp32 oracle's 6.1e-6 and the fp16 step's 5.9e-3]
 SOFTPLUS_X3_REL = 3e-4
+
+_record = functools.partial(record, "parity_net_activation.json")
 
 
 def _t(a):
@@ -265,15 +270,16 @@ def test_model_carries_the_activation_without_gpu_state():
 # =====================================================================================================================
 
 
-def _stage_cases():
-    from tests.support.mlp_stages import CASES
-    return CASES
+def _stage_case(case, act, precision, wg_w_bar=None):
+    tag = f"stages_{act}_{'fp16x3' if precision == X3 else 'fp16'}_"
+    return stage_case(case.replace(act=act, precision=precision, centre=True),
+                      lambda name, res: _record(tag + name, res), guard=False, wg_w_bar=wg_w_bar)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("precision", [1, X3], ids=["fp16", "fp16x3"])
 @pytest.mark.parametrize("act", ACTS)
-@pytest.mark.parametrize("case", _stage_cases(), ids=lambda c: c.name)
+@pytest.mark.parametrize("case", CASES, ids=lambda c: c.name)
 def test_net_activation_train_stages(case, act, precision):
     _stage_case(case, act, precision)
 
@@ -284,7 +290,6 @@ def test_net_activation_train_stages(case, act, precision):
 def test_net_activation_train_stages_production_step(act, precision):
     from plenoctree_b200._lib import RenderConfig, lib
     from plenoctree_b200.nerf.models import ctypes_ref
-    from tests.support.mlp_stages import Case
     need = int(lib.pob_train_workspace_bytes(ctypes_ref(RenderConfig(3, 64, 128, 1, 4096, 10000)), precision))
     free, _ = torch.cuda.mem_get_info()
     if free < need + (8 << 30):
@@ -296,12 +301,10 @@ def test_net_activation_train_stages_production_step(act, precision):
 @pytest.mark.parametrize("act", ACTS)
 def test_relu_mask_mutation_fails_the_data_gradient_bar(act):
     """applying the relu mask of h_l in place of f'(h_l) misses the data-gradient bar by far"""
-    from tests.support.mlp_stages import Case
-    from tests.support import mlp_stages as TS
-    res = _stage_case(Case(3, 96, 64, 128, 300), act, 1)
-    worst = min(r["stages"]["bwd_excess_relu_mask_mutation"] for r in res.values())
-    _record(f"relu_mask_mutation_{act}", dict(min_excess=worst, bar=TS.BWD_ALLOW))
-    assert worst > 10 * TS.BWD_ALLOW, worst
+    res = _stage_case(Case(3, 96, 64, 128, 300), act, FP16)
+    worst = min(r["stages"]["bwd_excess_relu_mask_mutation"] for k, r in res.items() if k.startswith("MLP"))
+    _record(f"relu_mask_mutation_{act}", dict(min_excess=worst, bar=BWD_ALLOW[FP16]))
+    assert worst > 10 * BWD_ALLOW[FP16], worst
 
 
 @pytest.mark.gpu
@@ -311,20 +314,18 @@ def test_relu_code_is_bit_identical_to_null(precision):
     gradient, render rows, points, grid and cell means"""
     from plenoctree_b200 import _lib, ops
     from plenoctree_b200.nerf.models import Rays
-    from tests.support.mlp_stages import Case
-    from tests.support.mlp_x3 import _run
-    case = Case(3, 64, 64, 128, 200)
+    case = Case(3, 64, 64, 128, 200, precision=precision, centre=True)
     outs = []
     null_struct = ops.posenc_struct
     for explicit in (False, True):
-        model = _make_model(case, "relu")
+        model = case.model()
         if explicit:
             model._posenc_struct = _lib.NetDesc(0, 10, 0, _lib.NET_RELU)
             model.cfg.posenc = ctypes.addressof(model._posenc_struct)
             # every ops call below passes an explicit {0, 10, 0, 0} descriptor instead of NULL
             ops.posenc_struct = lambda pe, net=0: _lib.NetDesc(0, 10, 0, int(net))
         try:
-            state, ctx = _run(case, model, precision, fill=0xFF)
+            state, ctx = case.run(model, fill=0xFF)
             ws = model.workspace(True, precision)
             views = L.train_workspace_views(model.cfg, ctx["n"], True, precision=precision)
             tiles = {f"{i}_{k}": L.workspace_view(ws, lv, k).clone() for i, lv in enumerate(views["levels"])
@@ -363,13 +364,11 @@ def test_inference_forwards_match_training_rows(act):
     training rows, and eval_points_raw within 1e-5 relative of an fp64 evaluation with the hi + lo operands."""
     from plenoctree_b200 import ops
     from plenoctree_b200.nerf.models import Rays
-    from tests.support.mlp_stages import Case
-    from tests.support.mlp_x3 import _run, _weights_hilo
-    case = Case(3, 64, 64, 128, 0)
+    case = Case(3, 64, 64, 128, 0, act=act, centre=True)
     rep = {}
     for precision in (1, X3):
-        model = _make_model(case, act)
-        state, ctx = _run(case, model, precision, fill=0xFF)
+        model = case.model()
+        state, ctx = case.replace(precision=precision).run(model, fill=0xFF)
         ws = model.workspace(True, precision)
         views = L.train_workspace_views(model.cfg, ctx["n"], False, precision=precision)
         o, d, v = ctx["rays"]
@@ -412,7 +411,7 @@ def test_inference_forwards_match_training_rows(act):
             assert torch.equal(g_sig, p_sig[:, 0]) and torch.equal(g_rgb, p_rgb), act
         else:
             flat = model.params[model.P:].cpu().numpy()
-            W, B, Wh, bh = _weights_hilo(flat, L.K_of(3), "cuda")
+            W, B, Wh, bh = operands(flat, L.K_of(3), "cuda", True)
             # posenc as the kernel forms it: exact fp32 x * 2^j, the cosine's argument added in fp32, sines in fp64
             j = torch.arange(10, device="cuda", dtype=torch.float32)
             xb = (x[:, None, :] * torch.exp2(j)[None, :, None]).reshape(-1, 30)
@@ -437,9 +436,9 @@ def test_gradient_vs_fp64_oracle(act):
     from oracle import nerf_sh_oracle as O
     from plenoctree_b200.nerf import train as T
     from plenoctree_b200.nerf.models import NerfModel, Rays
-    from tests.support.mlp_x3 import FLOOR_SLACK, GRAD_GAIN, LOSS_REL, _oracle_inputs
+    from tests.support.mlp_stages import FLOOR_SLACK, GRAD_GAIN, LOSS_REL, _setup
     R, nf, nsp = 96, 128, 300
-    fc, ff, rays, px, t_rand, u, sp = _oracle_inputs(77, 3, R, nf, nsp)
+    fc, ff, rays, px, t_rand, u, sp = _setup(3, R, nf, nsp, 77)
     for f in (fc, ff):
         _centre_sigma(f, 3, act)
     cfg = dict(num_coarse_samples=64, num_fine_samples=nf, near=2.0, far=6.0, white_bkgd=True,

@@ -6,7 +6,7 @@ descriptor, the host model, checkpoints and CLIs.
 CPU: the oracle (oracle/posenc_oracle.py) against the executed reference (tests/golden/ref_posenc.npz, written by
 tests/golden/make_golden_posenc.py), the checkpoint bridge, the flag scope, initialisation and the ABI tables.
 GPU: the training stages of each encoder against fp64 built from the kernels' own saved tiles
-(test_net_activation._check_level), the evaluators against the training forward, legacy against standard order, the default
+(tests/support/mlp_stages.py: check_level), the evaluators against the training forward, legacy against standard order, the default
 encoder against the parent's entry points, and the CLI chain with a non-default encoder."""
 import ctypes
 import functools
@@ -19,7 +19,8 @@ import torch
 from oracle import nerf_sh_oracle as O
 from oracle import posenc_oracle as PO
 from plenoctree_b200 import layouts as L
-from tests.support.model_flags import _gpu_params, _scope_args
+from tests.support.mlp_stages import FP16, assert_stages, check_call, params
+from tests.support.model_flags import _scope_args
 from tests.support.records import record
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -249,7 +250,7 @@ def _model(pe, sh=3, R=24, nc=32, nf=64, nsp=64, seed=17):
     from plenoctree_b200.nerf.models import NerfModel
     m = NerfModel(sh_deg=sh, num_coarse_samples=nc, num_fine_samples=nf, max_rays=R, sparsity_npoints=nsp,
                   min_deg_point=pe[0], max_deg_point=pe[1], legacy_posenc_order=pe[2])
-    fc, ff = _gpu_params(pe, sh, seed)
+    fc, ff = params(sh, seed, pe)
     m.set_params(np.concatenate([fc, ff]) if nf else fc)
     return m
 
@@ -297,19 +298,18 @@ _record = functools.partial(record, "posenc.json")
 @pytest.mark.gpu
 @pytest.mark.parametrize("pe", GPU_VARIANTS, ids=_tag)
 def test_train_stages_posenc(pe):
-    """stages of every level against fp64 built from the kernels' own saved tiles (test_net_activation._check_level
-    with the encoder), then the compact flat gradient against the fp64 oracle of the encoder (test_train.py's gate)"""
-    from tests.support import model_flags as NT
+    """stages of every level against fp64 built from the kernels' own saved tiles (mlp_stages.check_level with the
+    encoder), then the compact flat gradient against the fp64 oracle of the encoder (test_train.py's gate)"""
     sh, R = 3, 24
     m = _model(pe, sh, R)
     state, ctx = _train_call(m, R)
-    res = NT._check_call(m, state, ctx, 1, "relu", pe)
+    res = check_call(m, state, ctx, FP16)
     g = state.grads.double().cpu().numpy()
     ref = _oracle_grad(m, ctx, pe, sh)
     st = dict(stages=res, grad_rel_l2=float(np.linalg.norm(g - ref) / np.linalg.norm(ref)),
               grad_cosine=float(np.dot(g, ref) / (np.linalg.norm(g) * np.linalg.norm(ref))))
     _record(f"stages_{_tag(pe)}", st)
-    NT._assert_call(res, 1, "relu")
+    assert_stages(res, FP16, "relu", guard=False)
     assert st["grad_rel_l2"] < 2e-2 and st["grad_cosine"] > 0.9995, st
 
 
@@ -384,7 +384,7 @@ def test_legacy_matches_permuted_standard(degs):
     from plenoctree_b200.nerf.models import NerfModel
     sh = 3
     leg, std = degs + (True,), degs + (False,)
-    fl = np.concatenate(_gpu_params(leg, sh, 41))
+    fl = np.concatenate(params(sh, 41, leg))
     P = PO.param_count(sh, leg)
     fs = np.concatenate([PO.permute_rows(fl[:P], sh, leg, std), PO.permute_rows(fl[P:], sh, leg, std)])
     ml = NerfModel(sh_deg=sh, max_rays=64, min_deg_point=degs[0], max_deg_point=degs[1], legacy_posenc_order=True)
@@ -413,7 +413,7 @@ def test_explicit_default_descriptor_is_the_null_descriptor():
     sh, R = 3, 24
     d = _lib.NetDesc(0, 10, 0, 0)
     dp = ctypes.addressof(d)
-    flat = torch.from_numpy(np.concatenate(_gpu_params((0, 10, False), sh, 3))).cuda()
+    flat = torch.from_numpy(np.concatenate(params(sh, 3, (0, 10, False)))).cuda()
     P = flat.numel() // 2
     nb = int(lib.pob_packed_bytes(sh))
     b0, b1 = torch.zeros(nb, dtype=torch.uint8, device="cuda"), torch.full((nb,), 7, dtype=torch.uint8, device="cuda")

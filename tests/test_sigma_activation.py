@@ -288,15 +288,8 @@ def test_eval_points_act_vs_fp64(sh, prec):
 class SoftplusCase(RayCase):
     """a training call of test_ray_stages.py with the softplus density"""
 
-    def model(self, max_rays=None):
-        from plenoctree_b200.nerf.models import NerfModel
-        from tests.support.mlp_stages import _params
-        m = NerfModel(sh_deg=self.sh, num_coarse_samples=self.nc, num_fine_samples=self.nf, white_bkgd=self.white,
-                      lindisp=self.lindisp, max_rays=max_rays or self.R, sparsity_npoints=self.nsp,
-                      sigma_activation="softplus")
-        fc, ff = _params(self.sh, self.seed)
-        m.set_params(np.concatenate([fc, ff]) if self.nf else fc)
-        return m
+    def __init__(self, *a, **k):
+        super().__init__(*a, sigma_act="softplus", **k)
 
     @property
     def name(self):
@@ -316,11 +309,10 @@ def _softplus_call(case):
     from plenoctree_b200 import layouts as L, ops
     from plenoctree_b200.nerf.models import Rays
     from plenoctree_b200.nerf.train import default_loss_scale
-    from tests.support.mlp_x3 import _run
     dev = torch.device("cuda")
     model = case.model()
     n = case.R
-    _, ctx = _run(case, model, case.precision, n=n, fill=0xFF)
+    _, ctx = case.run(model, n=n, fill=0xFF)
     (o, d, v, px), t_rand, u, sp, noise = case.inputs(n)
     ws = model.workspace(True, case.precision)
     views = L.train_workspace_views(model.cfg, n, case.nsp > 0, precision=case.precision)
@@ -418,9 +410,9 @@ def test_softplus_gradient_vs_fp64_oracle():
     GRAD_GAIN times closer to the fp32 oracle than the fp16 step; the fp16 step within test_train.py's gates"""
     from plenoctree_b200.nerf import train as T
     from plenoctree_b200.nerf.models import NerfModel, Rays
-    from tests.support.mlp_x3 import FLOOR_SLACK, GRAD_GAIN, LOSS_REL, X3, _oracle_inputs
+    from tests.support.mlp_stages import FLOOR_SLACK, GRAD_GAIN, LOSS_REL, X3, _setup
     R, nf, nsp = 96, 128, 300
-    fc, ff, rays, px, t_rand, u, sp = _oracle_inputs(77, 3, R, nf, nsp)
+    fc, ff, rays, px, t_rand, u, sp = _setup(3, R, nf, nsp, 77)
     cfg = dict(num_coarse_samples=64, num_fine_samples=nf, near=2.0, far=6.0, white_bkgd=True,
                sparsity_weight=1e-3, sparsity_length=0.05)
     stats_o, ref = loss_and_grads_act(fc, ff, 3, rays, px, cfg, t_rand, u, sp, torch.float64, act="softplus")

@@ -35,7 +35,7 @@ import pytest
 import torch
 
 from plenoctree_b200 import layouts as L
-from tests.support.mlp_stages import Case
+from tests.support.mlp_stages import X3, Case, stage_case
 from tests.support.model_flags import _device_sms, _set_sms
 from tests.support.records import ROOT, record
 
@@ -139,33 +139,30 @@ STAGE_CASES = [
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", STAGE_CASES, ids=lambda c: c.name)
-def test_fp16_stages_at_split(sms, case, monkeypatch):
+def test_fp16_stages_at_split(sms, case):
     """test_train_stages' checks unchanged (0xFF-filled workspace, sensitivity guard on) at this count: forward and
     data gradient against fp64 from their own inputs, weight gradient + reduce against fp64 sums at WG_EPS_W"""
-    from tests.support import mlp_stages as TS
     table = split_table(sms, L.heads_width(L.K_of(case.sh)))
-    monkeypatch.setattr(TS, "_record", lambda name, res: _record(f"fp16_stages/{sms}/{name}", {**res, "split": table}))
-    TS._stage_case(case)
+    stage_case(case, lambda name, res: _record(f"fp16_stages/{sms}/{name}", {**res, "split": table}))
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", [Case(3, 96, 64, 128, 300), Case(4, 40, 64, 128, 64)], ids=lambda c: c.name)
-def test_fp16x3_stages_at_split(sms, case, monkeypatch):
+def test_fp16x3_stages_at_split(sms, case):
     """test_train_x3's checks unchanged: the x3 data gradient and all three wgrad passes run on all `sms` SMs"""
-    from tests.support import mlp_x3 as TX
     table = split_table(sms, L.heads_width(L.K_of(case.sh)))
-    monkeypatch.setattr(TX, "_record", lambda name, res: _record(f"fp16x3_stages/{sms}/{name}", {**res, "split": table}))
-    TX._stage_case_x3(case)
+    stage_case(case.replace(precision=X3),
+               lambda name, res: _record(f"fp16x3_stages/{sms}/{name}", {**res, "split": table}), guard=False)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", [Case(3, 96, 64, 128, 300), Case(4, 40, 64, 128, 64)], ids=lambda c: c.name)
-def test_elu_trunk_stages_at_split(sms, case, monkeypatch):
+def test_elu_trunk_stages_at_split(sms, case):
     """test_net_activation's fp16 checks with an elu trunk: its data gradient reads h, not the masks"""
-    from tests.support import model_flags as NA
     table = split_table(sms, L.heads_width(L.K_of(case.sh)))
-    monkeypatch.setattr(NA, "_record", lambda name, res: _record(f"elu_stages/{sms}/{name}", {**res, "split": table}))
-    NA._stage_case(case, "elu", 1)
+    stage_case(case.replace(act="elu", centre=True),
+               lambda name, res: _record(f"elu_stages/{sms}/stages_elu_fp16_{name}", {**res, "split": table}),
+               guard=False)
 
 
 # =====================================================================================================================

@@ -8,12 +8,17 @@ previous-stage tiles and masks, with the fp16 operands the kernels use: no mask 
 so the bars sit at the precision of the arithmetic (half an fp16 ulp for the rounding of the stored value plus an
 fp32 accumulation allowance of a stated multiple of 2^-24 * sum |a*w|).
 """
+import functools
+
 import numpy as np
 import pytest
 import torch
 
 from plenoctree_b200 import layouts as L
-from tests.support.mlp_stages import CASES, Case, _assert_stages, _check_all, _record, _stage_case
+from tests.support.mlp_stages import CASES, Case, FP16, assert_stages, check_call, stage_case
+from tests.support.records import record
+
+_record = functools.partial(record, "parity_train_stages.json")
 
 
 # =====================================================================================================================
@@ -124,7 +129,7 @@ def test_tile_decoders_roundtrip():
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", CASES, ids=lambda c: c.name)
 def test_train_stages(case):
-    _stage_case(case)
+    stage_case(case, _record)
 
 
 @pytest.mark.gpu
@@ -139,7 +144,7 @@ def test_train_stages_production_step():
     if free < need + (6 << 30):
         pytest.skip(f"the production step needs {need / 2**30:.1f} GB of workspace + ~6 GB for the reference; "
                     f"{free / 2**30:.1f} GB free on this (shared) device")
-    _stage_case(case, guard=False)
+    stage_case(case, _record, guard=False)
 
 
 @pytest.mark.gpu
@@ -162,6 +167,6 @@ def test_workspace_hygiene():
     fresh = small.model()
     state_f, _ = small.run(fresh, n=40, fill=0)
     assert torch.equal(state.grads, state_f.grads)
-    res = _check_all(small, model, state, ctx, True)
+    res = check_call(model, state, ctx, FP16)
     _record("stale_workspace_R96_then_R40", res)
-    _assert_stages(res)
+    assert_stages(res, FP16, "relu")

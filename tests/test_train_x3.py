@@ -6,6 +6,7 @@ compare each with an fp64 evaluation from the kernel's own previous-stage hi + l
 units test_train_stages.py uses: 2^-24 * sum |a*w| beyond the hi/lo representation error of the stored value.  End to
 end, the gradient is compared with the fp64 oracle, next to the fp16 step's on the same inputs.
 """
+import functools
 import os
 import re
 
@@ -14,13 +15,14 @@ import pytest
 import torch
 
 from plenoctree_b200 import layouts as L
-from tests.support.mlp_stages import CASES, Case
-from tests.support.mlp_x3 import (BWD_ALLOW, FLOOR_SLACK, FWD_ALLOW, GRAD_GAIN, LOSS_REL, X3, _oracle_inputs, _record,
-                                  _run, _stage_case_x3)
-from tests.support.records import ROOT
+from tests.support.mlp_stages import (BWD_ALLOW, CASES, FLOOR_SLACK, FWD_ALLOW, GRAD_GAIN, LOSS_REL, X3, Case, _setup,
+                                      stage_case)
+from tests.support.records import ROOT, record
+
+_record = functools.partial(record, "parity_train_x3.json")
 
 
-assert max(FWD_ALLOW, BWD_ALLOW) <= 2.0 ** 13 / 2 ** 7
+assert max(FWD_ALLOW[X3], BWD_ALLOW[X3]) <= 2.0 ** 13 / 2 ** 7
 
 
 # =====================================================================================================================
@@ -118,7 +120,7 @@ def test_x3_wgrad_passes_cover_every_product():
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", CASES, ids=lambda c: c.name)
 def test_x3_train_stages(case):
-    _stage_case_x3(case)
+    stage_case(case.replace(precision=X3), _record, guard=False)
 
 
 @pytest.mark.gpu
@@ -131,7 +133,7 @@ def test_x3_train_stages_production_step():
     free, _ = torch.cuda.mem_get_info()
     if free < need + (8 << 30):
         pytest.skip(f"needs {need / 2**30:.1f} GB of workspace + ~8 GB for the reference; {free / 2**30:.1f} GB free")
-    _stage_case_x3(Case(3, 4096, 64, 128, 10000))
+    stage_case(Case(3, 4096, 64, 128, 10000, precision=X3), _record, guard=False)
 
 
 def _fp64_mask_disagreements(model, ws, views, rays, sp):
@@ -180,7 +182,7 @@ def test_x3_gradient_vs_fp64_oracle():
     from plenoctree_b200.nerf.models import NerfModel, Rays
     from plenoctree_b200.nerf import train as T
     R, nf, nsp = 96, 128, 300
-    fc, ff, rays, px, t_rand, u, sp = _oracle_inputs(77, 3, R, nf, nsp)
+    fc, ff, rays, px, t_rand, u, sp = _setup(3, R, nf, nsp, 77)
     cfg = dict(num_coarse_samples=64, num_fine_samples=nf, near=2.0, far=6.0, white_bkgd=True,
                sparsity_weight=1e-3, sparsity_length=0.05)
     stats_o, ref = _oracle_grads(fc, ff, rays, px, cfg, t_rand, u, sp, torch.float64)
@@ -225,7 +227,7 @@ def test_x3_six_adam_steps_vs_fp64_oracle():
     from plenoctree_b200.nerf.models import NerfModel, Rays
     from plenoctree_b200.nerf import train as T
     R, nf, nsp, steps, lr = 48, 128, 64, 6, 5e-4
-    fc0, ff0, rays, px, _, _, _ = _oracle_inputs(91, 3, R, nf, nsp)
+    fc0, ff0, rays, px, _, _, _ = _setup(3, R, nf, nsp, 91)
     cfg = dict(num_coarse_samples=64, num_fine_samples=nf, near=2.0, far=6.0, white_bkgd=True,
                sparsity_weight=1e-3, sparsity_length=0.05)
     rs = np.random.RandomState(5)
@@ -276,7 +278,7 @@ def test_x3_graphed_matches_eager_and_repeats_bitwise():
     from plenoctree_b200.nerf.models import NerfModel, Rays
     from plenoctree_b200.nerf import train as T
     R = 256
-    fc, ff, rays, px, _, _, _ = _oracle_inputs(33, 3, R, 128, 0)
+    fc, ff, rays, px, _, _, _ = _setup(3, R, 128, 0, 33)
     b12 = torch.from_numpy(np.concatenate([rays[0], rays[1], rays[2], px], axis=1)).cuda()
     lrs = [5e-4, 4e-4, 3e-4]
     outs = []
@@ -296,10 +298,10 @@ def test_x3_graphed_matches_eager_and_repeats_bitwise():
         outs.append((model.params.clone(), state.m.clone(), state.v.clone()))
     for name, a, b in zip(("params", "m", "v"), *outs):
         assert torch.equal(a, b), name
-    case = Case(3, 96, 64, 128, 300)
+    case = Case(3, 96, 64, 128, 300, precision=X3)
     model = case.model()
-    g1 = _run(case, model, X3)[0].grads.clone()
-    g2 = _run(case, model, X3, fill=0xFF)[0].grads.clone()
+    g1 = case.run(model)[0].grads.clone()
+    g2 = case.run(model, fill=0xFF)[0].grads.clone()
     assert torch.isfinite(g1).all() and torch.equal(g1, g2)
 
 
@@ -308,9 +310,9 @@ def test_x3_call_leaves_fp16_results_alone():
     """An x3 call between two fp16 calls does not change the fp16 gradient (separate workspaces, same blobs)."""
     case = Case(3, 96, 64, 128, 300)
     model = case.model()
-    g_a = _run(case, model, 1)[0].grads.clone()
-    g_x3 = _run(case, model, X3)[0].grads.clone()
-    g_b = _run(case, model, 1)[0].grads.clone()
+    g_a = case.run(model)[0].grads.clone()
+    g_x3 = case.replace(precision=X3).run(model)[0].grads.clone()
+    g_b = case.run(model)[0].grads.clone()
     assert torch.equal(g_a, g_b)
     assert not torch.equal(g_a, g_x3)
 
